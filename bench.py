@@ -19,6 +19,8 @@ Legs (one JSON line on rank 0):
   cpu_baseline  the reference's own CPU path (oracle/_ref: unmodified reference sources driving cv2) on this
                 box's host cores, bounded sample (N=1, rank 0 only).
   --impl reference   only that CPU path, as its own JSON line.
+  --dump-outputs DIR  after the timed steps, the output planes of the last timed step as DIR/out_{y,u,v}.npy (float32; a
+                fixed seeded sample of rows, with DIR/out_{y,u,v}_rows.npy, when the frame exceeds 64 MB as float32).
 """
 from __future__ import annotations
 
@@ -58,7 +60,7 @@ def measured_hbm_peak():
             return float(json.loads(p.read_text())["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 class ClockSampler:
@@ -205,10 +207,31 @@ class DeviceFrames:
         self.out_args = [[(t.data_ptr(), t.stride(0)) for t in fr] for fr in self.d_out]
 
 
-def measure_config(name, cfg, ctx, spec, K, warmup, dev, rank, world, barrier, want_e2e, e2e_steps):
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(dump_dir, planes):
+    """Writes the output planes (uint8 arrays Y, U, V) as float32 .npy files.  A frame larger than DUMP_BYTES as float32
+    is cut to the same seeded sample of rows on every run; the row numbers go beside each plane."""
+    import numpy as np
+    d = Path(dump_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    total = 4 * sum(p.size for p in planes)
+    rng = np.random.default_rng(0)
+    for name, plane in zip(("out_y", "out_u", "out_v"), planes):
+        if total > DUMP_BYTES:
+            h = plane.shape[0]
+            rows = np.sort(rng.choice(h, max(1, int(h * 0.95 * DUMP_BYTES / total)), replace=False))
+            plane = plane[rows]
+            np.save(d / f"{name}_rows.npy", rows.astype(np.float64))
+        np.save(d / f"{name}.npy", plane.astype(np.float32))
+
+
+def measure_config(name, cfg, ctx, spec, K, warmup, dev, rank, world, barrier, want_e2e, e2e_steps, keep_outputs=False):
     """Device-resident leg, roofline leg (the frame gather kernel alone: isolated launches and a back-to-back stream) and,
     optionally, the end-to-end leg of one config.  Returns a dict of raw measurements (this rank's; times are reduced
-    with MAX over ranks by the caller where the contract asks for it)."""
+    with MAX over ranks by the caller where the contract asks for it); keep_outputs adds the host copies of the output
+    planes of the last timed step ("outputs")."""
     import torch
     import transform360_b200 as t360
     from transform360_b200 import synth
@@ -239,6 +262,8 @@ def measure_config(name, cfg, ctx, spec, K, warmup, dev, rank, world, barrier, w
     barrier()
     out = {"ms_total": e0.elapsed_time(e1), "launches": t360.kernel_launch_count() - launches0, "ring": ring,
            "plan_seconds": plan_seconds, "tiles": [list(ft.vft.plan_tile_counts(0)), list(ft.vft.plan_tile_counts(1))]}
+    if keep_outputs:  # step K - 1 wrote output buffer (K - 1) % 2; the legs below overwrite both
+        out["outputs"] = [fr.d_out[(K - 1) % 2][p][:, :spec.plane_dims(p)[2]].cpu().numpy() for p in range(3)]
 
     # ---- the dominant kernel alone: with the low-pass enabled a frame call also launches the blur kernels, so the gather
     # is timed through a second transform with the same geometry and the low-pass switched off (same jobs, same records)
@@ -367,7 +392,10 @@ def main():
     ap.add_argument("--skip-other-configs", action="store_true", help="do not add the short cfg3 / cfg4 legs (N=1 only)")
     ap.add_argument("--cpu-steps", type=int, default=12)
     ap.add_argument("--no-numa-bind", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the output planes of the last timed step to DIR (rank 0)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     cfg = CONFIGS[args.config]
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -378,7 +406,7 @@ def main():
         run_reference_arm(args, cfg, rank)
         return
 
-    # Page-locked frame buffers must live on the GPU's own NUMA node (20 vs 55 GB/s H2D on these 2-socket boxes): bind
+    # Page-locked frame buffers must live on the GPU's own NUMA node (H2D from the far socket of a 2-socket host is slower): bind
     # the rank to that node's CPUs before anything is allocated; the original affinity comes back for the CPU baseline.
     from transform360_b200.stream import bind_to_gpu_numa_node
     affinity0 = os.sched_getaffinity(0)
@@ -420,7 +448,9 @@ def main():
     K = args.steps
     sampler = ClockSampler(local_rank) if rank == 0 else None
     m = measure_config(args.config, cfg, ctx, spec, K, args.warmup, dev, rank, world, barrier, not args.skip_e2e,
-                       args.e2e_steps or min(K, 100))
+                       args.e2e_steps or min(K, 100), keep_outputs=bool(args.dump_outputs) and rank == 0)
+    if "outputs" in m:
+        dump_outputs(args.dump_outputs, m.pop("outputs"))
     (ms_total_max,) = max_over_ranks([m["ms_total"]])
     ms_per_step = ms_total_max / K
     value = in_px * K * world / (ms_total_max * 1e-3) / 1e6

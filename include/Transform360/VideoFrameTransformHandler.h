@@ -7,7 +7,7 @@
  * ever crosses the boundary, error text goes to stdout like the reference's printf.
  *
  * What differs is behind them: planning runs on the host, every per-frame pixel is produced by
- * hand-written sm_100a CUDA kernels (no OpenCV, no CPU fallback: without a usable CUDA device
+ * hand-written sm_90a CUDA kernels (no OpenCV, no CPU fallback: without a usable CUDA device
  * generateMapForPlane / transformFramePlane print the CUDA error and return 0).
  */
 #ifndef TRANSFORM360_B200_VIDEOFRAMETRANSFORMHANDLER_H

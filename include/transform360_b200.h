@@ -81,7 +81,9 @@ int T360B200_lowPassPlaneAsync(VideoFrameTransform* transform, const uint8_t* de
 void T360B200_setPinHostPlanes(VideoFrameTransform* transform, int enable);
 /* Tuning aid: when enabled, every whole-frame gather launch records a timeline of its consumer groups (per group and job:
  * wait start, data ready, done in ns of %globaltimer, job kind; 64 jobs per group, groups = SMs x groups per CTA);
- * T360B200_debugTraceRead copies it out after the stream has been synchronised and returns the number of 64-bit words. */
+ * T360B200_debugTraceRead copies it out after the stream has been synchronised and returns the number of 64-bit words;
+ * with out == NULL it copies nothing and returns the size of the trace buffer in 64-bit words (the largest trace any
+ * frame of this transform has needed so far; a smaller frame leaves the rows of its unused groups zero). */
 void T360B200_debugTrace(VideoFrameTransform* transform, int enable);
 unsigned long long T360B200_debugTraceRead(VideoFrameTransform* transform, unsigned long long* out, unsigned long long maxWords);
 /* Blocks until everything enqueued on the transform's own stream has finished; 1 = ok. */

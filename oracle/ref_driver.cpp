@@ -1,14 +1,14 @@
 // oracle/ref_driver.cpp -- TEST INFRASTRUCTURE, NOT PRODUCT CODE.
 //
 // Links against the reference's own, unmodified VideoFrameTransform.cpp and
-// VideoFrameTransformHandler.cpp (compiled from /root/reference where they
+// VideoFrameTransformHandler.cpp (compiled from the reference checkout where they
 // lie, see oracle/Makefile) and exposes, in addition to the reference C-ABI
 // those files export, read-only accessors for the plan the reference computed:
 //   warpMats_                 (reference VideoFrameTransform.h:150)
 //   filterKernelsX_/Y_        (reference VideoFrameTransform.h:155)
 //   segmentFilteringConfigs_  (reference VideoFrameTransform.h:159)
 // plus the setter for the OpenCV hooks declared in shim/opencv2/opencv.hpp.
-// The output .so lives in oracle/_ref/ (git-ignored, travels with gpurun).
+// The output .so lives in oracle/_ref/ (git-ignored, a build product).
 
 #include <map>
 #include <string>

@@ -227,7 +227,7 @@ def ref_lib():
         if _lib is not None:
             return _lib
         if not REF_SO.exists():
-            raise FileNotFoundError(f"{REF_SO} missing: run `make -C oracle ref` where /root/reference exists")
+            raise FileNotFoundError(f"{REF_SO} missing: run `make -C oracle ref` where the reference sources exist (REF=... FILTER=...)")
         lib = C.CDLL(str(REF_SO), mode=os.RTLD_LOCAL)
         vp = C.c_void_p
         lib.VideoFrameTransform_new.restype = vp

@@ -3,7 +3,7 @@
  * Scalar, single-threaded, written for legibility against the reference, not speed.
  * Compile with -ffp-contract=off and no -march/-ffast-math: every float expression below
  * must round exactly where the reference's C++ rounds (SURVEY.md Appendix C ledger).
- * "ref" = /root/reference/Transform360/Library/VideoFrameTransform.cpp.
+ * "ref" = the reference's Transform360/Library/VideoFrameTransform.cpp.
  */
 #define _GNU_SOURCE
 #include "t360_oracle.h"

@@ -4,7 +4,7 @@
  *   - the reference's geometry and low-pass plan (VideoFrameTransform.cpp), and
  *   - the OpenCV 4.x arithmetic the reference delegates pixels to (cv::remap with a
  *     CV_32FC2 map / cv::sepFilter2D u8->u8 with float kernels), which is a third-party
- *     dependency ABSENT from /root/reference (CMakeLists.txt:11 find_package(OpenCV),
+ *     dependency ABSENT from the reference (CMakeLists.txt:11 find_package(OpenCV),
  *     un-pinned; the build in this image is opencv-python-headless 4.13.0.92).
  *
  * PARITY PIN: the reference ships no tests, golden vectors or fixtures (SURVEY.md 4), so

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Prints the headline metrics of an .ncu-rep (run where ncu is installed; no GPU needed):
-    python profiles/ncu_metrics.py gpurun_out/prof.ncu-rep"""
+    python profiles/ncu_metrics.py prof.ncu-rep"""
 import csv
 import subprocess
 import sys

@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """Counts, per kernel of the shipped library, the SASS instructions that prove the path:
-    python profiles/sass_excerpt.py [lib.so] > profiles/r02_sass_excerpt.txt
+    python profiles/sass_excerpt.py [lib.so]
 UTMALDG (TMA box loads), UBLKCP (bulk copies), UTMAPF / UBLKPF (L2 prefetch), SYNCS (mbarriers), IDP.2A (two s16 x u8
-MACs), I2IP (saturate + pack), FFMA2 / FADD2 / FMUL2 (packed fp32 of the low-pass), I2F.U8 (byte-select conversion), ELECT."""
+MACs), I2IP (saturate + pack), I2F.U8 (byte-select conversion), ELECT."""
 import re
 import subprocess
 import sys
@@ -10,7 +10,7 @@ from collections import Counter
 
 lib = sys.argv[1] if len(sys.argv) > 1 else "transform360_b200/lib/libTransform360.so"
 sass = subprocess.run(["cuobjdump", "-sass", lib], capture_output=True, text=True, check=True).stdout
-want = re.compile(r"\b(UTMALDG[\w.]*|UBLKCP[\w.]*|UTMAPF[\w.]*|UBLKPF[\w.]*|SYNCS[\w.]*|IDP\.2A[\w.]*|I2IP[\w.]*|ELECT|FFMA2|FADD2|FMUL2|I2F\.U8)\b")
+want = re.compile(r"\b(UTMALDG[\w.]*|UBLKCP[\w.]*|UTMAPF[\w.]*|UBLKPF[\w.]*|SYNCS[\w.]*|IDP\.2A[\w.]*|I2IP[\w.]*|ELECT|I2F\.U8)\b")
 counts, fn = Counter(), None
 for line in sass.splitlines():
     m = re.search(r"Function : (\S+)", line)

@@ -6,10 +6,9 @@
 Decodes the share-job and tile-job records of a BASELINE config exactly like gather_frame.cu does (slot field = byte
 offset of a pixel's first weight vector in the shared-memory image), and counts per warp step the wavefronts of one weight
 load: a quarter-warp of 8 lanes per pass, a pass costs as many wavefronts as its fullest 16-byte bank group holds distinct
-addresses.  The same model on the previous dealing gave 4.46 / 4.98 (share / tile) where ncu's per-instruction view
-showed 4.49 / 5.05; with GroupMatcher::balance + PassDealer (csrc/gather_plan.cpp) it gives 4.42 / 4.49, and
-ncu 4.35 over all LDS.128 of the final cfg2 capture (record loads at 4.0 included).  Also prints the lower bound the
-chosen table copies allow (max(4, fullest bank group)), i.e. what is left to a better deal."""
+addresses.  With GroupMatcher::balance + PassDealer (csrc/gather_plan.cpp) the model gives 4.42 / 4.49 (share / tile)
+wavefronts per load at cfg2.  Also prints the lower bound the chosen table copies allow (max(4, fullest bank group)), i.e.
+what is left to a better deal."""
 import sys
 from pathlib import Path
 

@@ -1,11 +1,11 @@
 #!/usr/bin/env python
-"""Generates tests/golden/golden.json from THE REFERENCE ITSELF, run in this container:
-``oracle/_ref/libt360ref.so`` (unmodified /root/reference sources + oracle/shim) driving cv2 4.13.0.
+"""Generates tests/golden/golden.json from THE REFERENCE ITSELF:
+``oracle/_ref/libt360ref.so`` (unmodified reference sources + oracle/shim) driving cv2 4.13.0.
 
     python tests/golden/make_golden.py            # small cases (+ cfg1)
     python tests/golden/make_golden.py --full     # also cfg2/cfg3/cfg4 luma known answers
 
-Needs /root/reference (to build oracle/_ref) and cv2; the output is committed so that the tests do not.
+Needs the reference sources (to build oracle/_ref) and cv2; the output is committed so that the tests do not.
 Input planes are the integer-hash ``noise`` generator of SURVEY.md 8(d); plane p of a case uses
 noise(w, h, plane=p, frame=0).
 """

@@ -2,13 +2,17 @@
 against the libavfilter stand-in oracle/ffshim and driven by oracle/ff_driver.c, linked with
   * the reference library (oracle/_ref/libt360ref.so + cv2)            -> variant "ref"
   * the product          (transform360_b200/lib/libTransform360.so)    -> variant "b200".
-Same filter object code, same option strings; only libTransform360 differs.  Both .so files are prebuilt where
-/root/reference exists (make -C oracle ref) and travel to the GPU box."""
+Same filter object code, same option strings; only libTransform360 differs.  Both .so files are built where the
+reference sources are available (make -C oracle ref).  The product's own CUDA-frame filter is checked against the
+reference filter's frames, live where those objects are built, else against their recorded digests
+(tests/golden/live_reference.py)."""
 import numpy as np
 import pytest
 
 from oracle import c_oracle as co
 from oracle import ff_harness as ff
+from oracle import ref_harness as rh
+from tests.golden.live_reference import recorded
 
 needs_filters = pytest.mark.skipif(not (ff.available("ref") and ff.available("b200")), reason="oracle/_ref filter objects not built")
 
@@ -48,7 +52,7 @@ def test_option_table_and_config_output_through_the_product_headers():
 def test_unmodified_reference_filter_gives_identical_frames_with_either_library(args, dims):
     import torch
     if not torch.cuda.is_available():
-        pytest.fail("needs the B200 box")
+        pytest.fail("needs a CUDA device")
     w, h = dims
     planes = [co.noise_plane(w, h, 0, 3), co.noise_plane((w + 1) // 2, (h + 1) // 2, 1, 3), co.noise_plane((w + 1) // 2, (h + 1) // 2, 2, 3)]
     ref, b200 = ff.Filter("ref", args, w, h), ff.Filter("b200", args, w, h)
@@ -107,7 +111,6 @@ def test_cuda_filter_defaults_are_the_reference_filters():
     assert expected <= names and names - expected == {"sync"}
 
 
-@needs_filters
 @needs_cuda_filter
 @pytest.mark.gpu
 @pytest.mark.parametrize("args,dims,extra", [
@@ -122,15 +125,21 @@ def test_cuda_filter_defaults_are_the_reference_filters():
 def test_cuda_frame_filter_matches_the_reference_filter(args, dims, extra):
     """Device planes in, device planes out, whole frame per call on the device context's stream; the frames are those of
     the reference's software filter (reference object code + cv2) for the same option string."""
-    import torch
-    if not torch.cuda.is_available():
-        pytest.fail("needs the B200 box")
     w, h = dims
     planes = [co.noise_plane(w, h, 0, 3), co.noise_plane((w + 1) // 2, (h + 1) // 2, 1, 3), co.noise_plane((w + 1) // 2, (h + 1) // 2, 2, 3)]
-    ref = ff.Filter("ref", args, w, h)
+
+    def live():
+        ref = ff.Filter("ref", args, w, h)
+        frame = ref.filter(planes)
+        ref.close()
+        return {"size": [ref.out_w, ref.out_h], "planes": [rh.sha16(p) for p in frame]}
+    want = recorded(f"reference_filter/{args}/{w}x{h}", live, live=ff.available("ref"))
+    import torch
+    if not torch.cuda.is_available():
+        pytest.fail("needs a CUDA device")
     stream = torch.cuda.Stream()
     gpu = ff.CudaFilter(args + extra, w, h, stream=stream)
-    assert (ref.out_w, ref.out_h) == (gpu.out_w, gpu.out_h)
+    assert [gpu.out_w, gpu.out_h] == want["size"]
     # decoder surfaces are pitched: 256-byte rows with the plane in the first columns
     dev = []
     for p in planes:
@@ -139,33 +148,39 @@ def test_cuda_frame_filter_matches_the_reference_filter(args, dims, extra):
         store[:, :p.shape[1]] = torch.from_numpy(p).cuda()
         dev.append(store[:, :p.shape[1]])
     torch.cuda.synchronize()
-    want = ref.filter(planes)
     for frame in range(3):
         got = gpu.filter(dev, out_pitch_pad=48)
         stream.synchronize()
         for p in range(3):
-            assert np.array_equal(got[p].cpu().numpy(), want[p]), f"plane {p} of frame {frame} differs ({args})"
-            assert bool((gpu.last_store[p][:, want[p].shape[1]:] == 0xA5).all()), "wrote beyond the plane's width"
-    ref.close()
+            assert rh.sha16(got[p].cpu().numpy()) == want["planes"][p], f"plane {p} of frame {frame} differs ({args})"
+            assert bool((gpu.last_store[p][:, got[p].shape[1]:] == 0xA5).all()), "wrote beyond the plane's width"
     gpu.close()
 
 
 @needs_cuda_filter
 @pytest.mark.gpu
 def test_cuda_frame_filter_gray8_and_refusals():
-    import torch
-    if not torch.cuda.is_available():
-        pytest.fail("needs the B200 box")
-    from oracle import ref_harness as rh
     w, h = 512, 256
     y = co.noise_plane(w, h, 0, 5)
-    gpu = ff.CudaFilter("cube_edge_length=64:interpolation_alg=cubic:enable_low_pass_filter=0", w, h, sw_format=ff.AV_PIX_FMT_GRAY8)
+    args = "cube_edge_length=64:interpolation_alg=cubic:enable_low_pass_filter=0"
+    size = ff.CudaFilter(args, w, h, sw_format=ff.AV_PIX_FMT_GRAY8, device=False)
+    ow, oh = size.out_w, size.out_h
+    size.close()
+
+    def live():
+        t = rh.RefTransform(rh.default_context(interpolation_alg=2, enable_low_pass_filter=0))
+        assert t.generate_map(w, h, ow, oh, 0)
+        out = rh.sha16(t.transform_plane(y, ow, oh, 0))
+        t.close()
+        return out
+    want = recorded("reference_plane/gray8", live)
+    import torch
+    if not torch.cuda.is_available():
+        pytest.fail("needs a CUDA device")
+    gpu = ff.CudaFilter(args, w, h, sw_format=ff.AV_PIX_FMT_GRAY8)
     got = gpu.filter([torch.from_numpy(y).cuda()])
     torch.cuda.synchronize()
-    if rh.REF_SO.exists():
-        t = rh.RefTransform(rh.default_context(interpolation_alg=2, enable_low_pass_filter=0))
-        assert t.generate_map(w, h, gpu.out_w, gpu.out_h, 0)
-        assert np.array_equal(got[0].cpu().numpy(), t.transform_plane(y, gpu.out_w, gpu.out_h, 0))
+    assert rh.sha16(got[0].cpu().numpy()) == want
     # a frame pool that has nothing to hand out: ENOMEM surfaces, nothing crashes
     rc = gpu.L.t360f_filter_cuda(gpu.h, (ff.C.c_void_p * 1)(got[0].data_ptr()), (ff.C.c_int * 1)(w), (ff.C.c_void_p * 1)(None), (ff.C.c_int * 1)(0))
     assert rc == -12

@@ -5,7 +5,7 @@ Bars (task spec / BASELINE.json north_star):
   * segmented low-pass (cv::sepFilter2D replacement): float32 -> tolerance 1 LSB per north_star, but the
     kernel follows the oracle's operation order, so these tests also demand bit-exactness;
   * end to end vs the recorded outputs of the reference itself (tests/golden/golden.json).
-Nothing here reads /root/reference.
+Nothing here reads the reference sources.
 """
 import numpy as np
 import pytest
@@ -22,7 +22,7 @@ pytestmark = pytest.mark.gpu
 def torch_cuda():
     torch = pytest.importorskip("torch")
     if not torch.cuda.is_available():
-        pytest.fail("no CUDA device: the GPU tests must run on the B200 box (there is no CPU fallback to test)")
+        pytest.fail("no CUDA device: the GPU tests must run on an H100 (there is no CPU fallback to test)")
     assert t360.device_count() >= 1
     return torch
 
@@ -256,6 +256,31 @@ def _pitched(torch, arr, pitch):
     return base
 
 
+def test_debug_trace_has_a_row_per_consumer_group_of_the_device(torch_cuda):
+    """The frame gather's debug trace is sized by the library from the device's SM count (one CTA per SM, three consumer
+    groups per CTA for bicubic); the binding reads all of it, and the traced jobs have ordered timestamps."""
+    torch = torch_cuda
+    from transform360_b200.stream import FrameTransformer, StreamSpec
+    case = SMALL["cube_cubic"]
+    ctx, _ = _ctxs(case)
+    spec = StreamSpec(case["inp"][0], case["inp"][1], case["out"][0], case["out"][1])
+    ft = FrameTransformer(ctx, spec)
+    pitch = lambda w: (w + 255) // 256 * 256
+    d_in = [_pitched(torch, co.noise_plane(*spec.plane_dims(p)[:2], plane=p, frame=2), pitch(spec.plane_dims(p)[0])) for p in range(3)]
+    d_out = [torch.zeros((spec.plane_dims(p)[3], pitch(spec.plane_dims(p)[2])), dtype=torch.uint8, device="cuda") for p in range(3)]
+    torch.cuda.synchronize()
+    ft.vft.debug_trace(True)
+    ft.transform_frame_device([(t.data_ptr(), t.stride(0)) for t in d_in], [(t.data_ptr(), t.stride(0)) for t in d_out], 0)
+    torch.cuda.synchronize()
+    tr = ft.vft.read_trace().astype(np.int64)
+    ft.vft.debug_trace(False)
+    ft.close()
+    assert tr.shape == (torch.cuda.get_device_properties(0).multi_processor_count * 3, 64, 4)
+    used = tr[..., 2] > 0
+    assert used.any()
+    assert (tr[..., 1][used] >= tr[..., 0][used]).all() and (tr[..., 2][used] >= tr[..., 1][used]).all()
+
+
 @pytest.mark.parametrize("name,planes", [("cube_cubic", 3), ("cube_linear", 3), ("cube_lanczos", 3), ("cube_cubic", 2), ("cube_cubic", 1),
                                          ("rotated", 3), ("cube_to_equirect", 3), ("scaled_2x2", 3), ("scaled_fractional_lp", 3),
                                          ("barrel", 3), ("cube_nearest", 3), ("lr_stereo", 3)])
@@ -397,7 +422,7 @@ def test_frame_bytes_do_not_depend_on_the_gpu(torch_cuda):
     """SURVEY.md 4 item 4 / 8e: frame k gives identical planes whichever rank (GPU) processes it."""
     torch = torch_cuda
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (run with gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     import socket
     import torch.multiprocessing as mp
     with socket.socket() as s:

@@ -13,6 +13,7 @@ import transform360_b200 as t360
 from oracle import c_oracle as co
 from oracle import ref_harness as rh
 from tests.golden.cases import FULL, SMALL, plane_dims
+from tests.golden.live_reference import map_digest, plan_digest, recorded, segs_digest
 from transform360_b200 import build as t360_build
 
 ROOT = Path(__file__).resolve().parents[1]
@@ -43,7 +44,7 @@ def test_library_exports_declared_abi():
         assert getattr(lib, s)
 
 
-def test_context_layout_matches_reference_header():
+def test_context_layout_matches_reference_header(tmp_path):
     assert ctypes.sizeof(t360.FrameTransformContext) == 112
     assert t360.FrameTransformContext.interpolation_alg.offset == 28
     assert t360.FrameTransformContext.kernel_adjust_factor.offset == 108
@@ -57,7 +58,7 @@ def test_context_layout_matches_reference_header():
     prog = '#include "Transform360/VideoFrameTransformHandler.h"\n#include <stddef.h>\n#include <stdio.h>\n' \
            'int main(void){printf("%zu %zu %zu", sizeof(FrameTransformContext), offsetof(FrameTransformContext, interpolation_alg),' \
            ' offsetof(FrameTransformContext, kernel_adjust_factor));return 0;}'
-    exe = Path("/tmp/t360_abi_probe")
+    exe = tmp_path / "t360_abi_probe"
     subprocess.run(["gcc", "-std=c11", "-x", "c", "-", "-I", str(ROOT / "include"), "-o", str(exe)], input=prog, text=True, check=True)
     assert subprocess.run([str(exe)], capture_output=True, text=True).stdout == "112 28 108"
 
@@ -138,23 +139,27 @@ def test_full_size_plan_matches_golden(name, golden):
     hp.close()
 
 
-@pytest.mark.skipif(not rh.ref_available(), reason="oracle/_ref not built")
+def _reference_plan(rctx, dims):
+    """The compiled reference's plan for plane index 0 (live, or its record: tests/golden/live_reference.py)."""
+    def live():
+        ref = rh.RefTransform(rctx)
+        ok = bool(ref.generate_map(*dims, 0))
+        d = dict(plan_digest(ref, 0), ok=True) if ok else {"ok": False}
+        ref.close()
+        return d
+    return live
+
+
 def test_plan_matches_live_reference_with_odd_parameters():
     ov = dict(fixed_yaw=123.4, fixed_pitch=-67.8, fixed_roll=179.0, fixed_cube_offcenter_x=0.2, fixed_cube_offcenter_y=-0.15,
               fixed_cube_offcenter_z=-0.4, num_vertical_segments=12, num_horizontal_segments=7, expand_coef=1.05,
               kernel_height_scale_factor=1.7, kernel_adjust_factor=1.3, output_layout=t360.LAYOUT_EAC_32)
     ctx, rctx = t360.make_context(**ov), rh.default_context(**ov)
-    ref = rh.RefTransform(rctx)
-    assert ref.generate_map(700, 350, 300, 200, 0)
+    want = recorded("plan/odd_parameters", _reference_plan(rctx, (700, 350, 300, 200)))
+    assert want["ok"]
     hp = t360.HostPlan(ctx, 700, 350, 300, 200)
-    assert np.array_equal(hp.map.view(np.uint32), ref.map(0).view(np.uint32))
-    a, b = hp.segments(), ref.segments(0)
-    assert len(a) == len(b)
-    for s, r in zip(a, b):
-        assert s[:4] == r[:4]
-        assert np.array_equal(s[4].view(np.uint32), r[4].view(np.uint32))
-        assert np.array_equal(s[5].view(np.uint32), r[5].view(np.uint32))
-    ref.close()
+    assert map_digest(hp.map) == want["map"]
+    assert segs_digest(hp.segments()) == want["segs"]
     hp.close()
 
 
@@ -192,7 +197,6 @@ def _random_context(rng):
     return ov
 
 
-@pytest.mark.skipif(not rh.ref_available(), reason="oracle/_ref not built")
 @pytest.mark.parametrize("seed", [1, 2, 3])
 def test_random_parameter_sweep_against_the_compiled_reference(seed):
     """Random contexts over the whole option space (layouts both ways, stereo, rotation, off-centre, scale factors,
@@ -203,54 +207,56 @@ def test_random_parameter_sweep_against_the_compiled_reference(seed):
     out-of-range face index and the negative-sigma refusal fixed alongside this test.)"""
     rng = np.random.default_rng(seed)
     compared = 0
-    for _ in range(50):
+    for case in range(50):
         ov = _random_context(rng)
         iw, ih = int(rng.integers(64, 400)) * 2, int(rng.integers(32, 200)) * 2
         ow, oh = int(rng.integers(24, 160)) * 2, int(rng.integers(16, 120)) * 2
         ctx, rctx = t360.make_context(**ov), rh.default_context(**ov)
-        ref = rh.RefTransform(rctx)
-        ok_ref = bool(ref.generate_map(iw, ih, ow, oh, 0))
+        lr = ov["input_stereo_format"] != 2 and ov["output_stereo_format"] == 1
+
+        def live():
+            ref = rh.RefTransform(rctx)
+            d = {"ok": bool(ref.generate_map(iw, ih, ow, oh, 0))}
+            if d["ok"]:
+                d.update(plan_digest(ref, 0))
+                m = ref.map(0)
+                if lr and m.shape[1] % 2 == 1:
+                    d["map_without_centre"] = map_digest(np.delete(m.view(np.uint32), m.shape[1] // 2, axis=1))
+            ref.close()
+            return d
+        want = recorded(f"plan_sweep/{seed}/{case}", live)
         try:
             hp = t360.HostPlan(ctx, iw, ih, ow, oh)
         except ValueError:
             hp = None
-        assert ok_ref == (hp is not None), f"status differs for {ov} {(iw, ih, ow, oh)}"
+        assert want["ok"] == (hp is not None), f"status differs for {ov} {(iw, ih, ow, oh)}"
         if hp is None:
-            ref.close()
             continue
-        got, want = hp.map.view(np.uint32), ref.map(0).view(np.uint32)
-        assert got.shape == want.shape
-        differ = got != want
-        if differ.any():
+        got = hp.map.view(np.uint32)
+        assert list(got.shape) == want["shape"]
+        if map_digest(got) != want["map"]:
             mw = got.shape[1]
-            lr_centre = ov["input_stereo_format"] != 2 and ov["output_stereo_format"] == 1 and mw % 2 == 1
-            assert lr_centre and not np.delete(differ, mw // 2, axis=1).any(), f"map differs for {ov} {(iw, ih, ow, oh)}"
+            lr_centre = lr and mw % 2 == 1
+            assert lr_centre and map_digest(np.delete(got, mw // 2, axis=1)) == want["map_without_centre"], \
+                f"map differs for {ov} {(iw, ih, ow, oh)}"
             assert np.array_equal(got, co.generate_map(rctx, iw, ih, ow, oh).view(np.uint32)), "planner != C oracle on the centre column"
-        a, b = hp.segments(), ref.segments(0)
-        assert len(a) == len(b)
-        for s, r in zip(a, b):
-            assert s[:4] == r[:4]
-            assert np.array_equal(s[4].view(np.uint32), r[4].view(np.uint32)) and np.array_equal(s[5].view(np.uint32), r[5].view(np.uint32))
+        assert segs_digest(hp.segments()) == want["segs"]
         compared += 1
-        ref.close()
         hp.close()
     assert compared >= 40
 
 
-@pytest.mark.skipif(not rh.ref_available(), reason="oracle/_ref not built")
 @pytest.mark.parametrize("nh,adjust", [(0, 1), (-2, 1), (0, 0), (-3, 0)])
 def test_non_positive_horizontal_segment_counts_follow_the_reference(nh, adjust):
     """Not an error in the reference: with adjust_kernel its tile loop does not run (no tiles: the low-pass output stays
     zero), without adjust_kernel the value is ignored (cpp:224-235)."""
     ov = dict(interpolation_alg=2, enable_low_pass_filter=1, num_vertical_segments=5, num_horizontal_segments=nh, adjust_kernel=adjust)
     ctx, rctx = t360.make_context(**ov), rh.default_context(**ov)
-    ref = rh.RefTransform(rctx)
-    assert ref.generate_map(320, 160, 96, 64, 0)
+    want = recorded(f"plan/horizontal_segments/{nh}/{adjust}", _reference_plan(rctx, (320, 160, 96, 64)))
+    assert want["ok"]
     hp = t360.HostPlan(ctx, 320, 160, 96, 64)
-    a, b = hp.segments(), ref.segments(0)
-    assert len(a) == len(b) == (0 if adjust else 5)
-    for s, r in zip(a, b):
-        assert s[:4] == r[:4] and np.array_equal(s[4].view(np.uint32), r[4].view(np.uint32)) and np.array_equal(s[5].view(np.uint32), r[5].view(np.uint32))
-    assert np.array_equal(hp.map.view(np.uint32), ref.map(0).view(np.uint32))
-    ref.close()
+    a = hp.segments()
+    assert len(a) == (0 if adjust else 5)
+    assert segs_digest(a) == want["segs"]
+    assert map_digest(hp.map) == want["map"]
     hp.close()

@@ -1,6 +1,6 @@
-"""transform360_b200: B200-native implementation of Transform360's projection-remap hot path.
+"""transform360_b200: H100-native (sm_90a) implementation of Transform360's projection-remap hot path.
 
-The product is ``lib/libTransform360.so`` (C-ABI of the reference's VideoFrameTransformHandler.h, sm_100a
+The product is ``lib/libTransform360.so`` (C-ABI of the reference's VideoFrameTransformHandler.h, sm_90a
 CUDA kernels inside); this package is its Python binding plus the build script.  No CPU fallback exists.
 """
 from .handler import (CUBIC, LANCZOS4, LAYOUT_BARREL, LAYOUT_BARREL_SPLIT, LAYOUT_CUBEMAP_23_OFFCENTER,  # noqa: F401

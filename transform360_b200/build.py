@@ -1,9 +1,9 @@
-"""Builds transform360_b200/lib/libTransform360.so (the drop-in C-ABI library) in-tree with nvcc for sm_100a.
+"""Builds transform360_b200/lib/libTransform360.so (the drop-in C-ABI library) in-tree with nvcc for sm_90a (H100).
 
     python -m transform360_b200.build [--force] [--verbose]
 
 The artifact name follows the reference's CMake target (Transform360/CMakeLists.txt:9: libTransform360).
-The .so is git-ignored but travels to the GPU box with gpurun.
+The .so is a build product (git-ignored): build() makes it in the tree.
 """
 from __future__ import annotations
 
@@ -19,7 +19,7 @@ CSRC = PKG / "csrc"
 LIB_DIR = PKG / "lib"
 LIB = LIB_DIR / "libTransform360.so"
 SOURCES = ["geometry.cpp", "lowpass_plan.cpp", "sampling.cpp", "gather_plan.cpp", "kernels.cu", "gather_frame.cu", "video_frame_transform.cpp"]
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 
 
 def nvcc_path() -> str:

@@ -1,4 +1,4 @@
-// sm_100a kernels of the projection-remap hot path, part 2: the persistent frame gather.
+// sm_90a kernels of the projection-remap hot path, part 2: the persistent frame gather.
 //
 //   gatherFrameKernel<K, COPIES, GROUPS>   replaces cv::remap as the reference calls it (VideoFrameTransform.cpp:748-754)
 //   for all planes of a frame in ONE launch: per output pixel a K x K window of the 8-bit source is weighted with
@@ -404,7 +404,7 @@ gatherFrameKernel(const __grid_constant__ FrameGatherParams p, StagedParams jobs
     // from the global counter.  Lane i holds the header of job i of the batch.  The claim runs two batches ahead and the
     // header loads one, so neither the atomic nor the loads are waited for.  (Asking L2 for a job's records and source
     // box a job ahead with cp.async.bulk.prefetch paid while a job's box was the whole stage buffer; with the boxes cut
-    // to the rows a job needs the copies are not waited for either, and the prefetches cost 1.3 % of the frame.)
+    // to the rows a job needs the copies are not waited for either, and the prefetches only add producer work.)
     const int producer = blockIdx.x * GROUPS + g, dynamicBase = gridDim.x * GROUPS * 2 * kClaimBatch;
     auto loadBatch = [&](int base) {
       int4 h = make_int4(0, kJobExit << kJobKindShift, 0, 0);

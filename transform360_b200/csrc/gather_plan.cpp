@@ -211,7 +211,7 @@ void classifyTile(const HostPlan& h, int x0, int y0, bool seamPossible, TileClas
   }
   // The ring around a pole cap: the tile's windows span hundreds of columns, those of a 16 x 16 quadrant fit a class-0
   // box.  Also preferred to a class-1 job, whose box takes both stage buffers of a group and so cannot be loaded while
-  // the group computes (measured: 2.0 us of waiting per class-1 job against 0.15 us per class-0 job).
+  // the group computes (its group waits for every class-1 job's data; class-0 boxes arrive while the previous job runs).
   if (x1 - x0 == kGatherTileW && y1 - y0 == kFrameTileH) {
     bool all = true;
     for (int q = 0; q < 4 && all; ++q) {
@@ -459,9 +459,8 @@ void spreadGeneralJobs(std::vector<GatherJob>& jobs) {
   for (const GatherJob& j : jobs)
     (((j.outY >> kJobKindShift) & kJobKindMask) == kJobGeneral ? general : staged).push_back(j);
   if (general.empty() || staged.empty()) return;
-  // The first half of the staged jobs: none may land among the small jobs the launch ends with (a 5 us general job
-  // claimed there is the last thing to finish: 54.6 us per cfg2 frame with three quarters, 57.1 with nine tenths, 52.7 with
-  // anything from a twentieth to six tenths).
+  // The first half of the staged jobs: none may land among the small jobs the launch ends with (a general job, several
+  // times longer than a staged one, claimed there is the last thing to finish and stretches the frame).
   const size_t span = staged.size() / 2 + 1;
   jobs.clear();
   size_t g = 0;

@@ -1,4 +1,4 @@
-// sm_100a kernels of the projection-remap hot path, part 1: everything except the persistent frame gather
+// sm_90a kernels of the projection-remap hot path, part 1: everything except the persistent frame gather
 // (gather_frame.cu).
 //
 //   gatherKernel<K>        replace cv::remap as the reference calls it (VideoFrameTransform.cpp:748-754) for whole
@@ -127,48 +127,23 @@ __global__ void __launch_bounds__(256) blurTileKernel(BlurParams p) {
 // down the rows of the strip:
 //   horizontal: the 8 running sums advance together through the taps in chunks of 4; the source bytes they
 //     need form a sliding window kept as floats in a 12-register ring (3 groups of 4).  Each chunk issues
-//     the multiply-adds (sums 2j and 2j+1 advance as a register pair: packed FFMA2 for the even taps, whose two
-//     window floats are an aligned pair too, scalar FFMA for the odd ones), converts one new group of 4 bytes (I2F.U8
-//     with a byte selector: exact, one XU instruction each) fetched as one aligned 32-bit word and aligned with a
-//     funnel shift, and reads 4 taps as one 128-bit uniform load.
+//     the 32 scalar multiply-adds, converts one new group of 4 bytes (I2F.U8 with a byte selector: exact, one XU
+//     instruction each) fetched as one aligned 32-bit word and aligned with a funnel shift, and reads 4 taps as one
+//     128-bit uniform load.
 //     Tap arrays are zero-padded to a multiple of 4: fma(0, p, s) == s exactly, and starting the chain from
 //     +0 makes the first fma equal the reference's plain multiply, so the bits match the oracle's order.
 //   vertical: the last 2*HY+1 row results stay in a register ring; the symmetric-pair FMA chain of the oracle
-//     (packed: FMUL2 / FADD2 / FFMA2 on the same pairs) produces one output row per input row; rounding is the 1.5*2^23 magic add (round-half-even), and the low
+//     produces one output row per input row; rounding is the 1.5*2^23 magic add (round-half-even), and the low
 //     mantissa bytes of 8 results are packed into one 64-bit store.
+//   sm_90 has no packed single-precision FFMA2 / FADD2 / FMUL2: every operation is a scalar round-to-nearest
+//   instruction, in the oracle's order.
 // ---------------------------------------------------------------------------------------------------
-// Packed single precision (sm_100a: FFMA2 / FADD2 / FMUL2 work on an aligned register pair; each half is an independent
-// round-to-nearest operation, so the bits are those of two scalar instructions).
 #ifndef T360_BLUR_I2F
 #define T360_BLUR_I2F 1
 #endif
 #ifndef T360_BLUR_L2_AHEAD
 #define T360_BLUR_L2_AHEAD 2
 #endif
-#ifndef T360_BLUR_F32X2
-#define T360_BLUR_F32X2 1
-#endif
-__device__ __forceinline__ unsigned long long pack2(float lo, float hi) {
-  unsigned long long r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ void unpack2(unsigned long long v, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
-__device__ __forceinline__ void fma2(float k, float x0, float x1, float& s0, float& s1) {  // s = fma(k, x, s) on both halves
-  unsigned long long d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(pack2(k, k)), "l"(pack2(x0, x1)), "l"(pack2(s0, s1)));
-  unpack2(d, s0, s1);
-}
-__device__ __forceinline__ void mul2(float k, float x0, float x1, float& d0, float& d1) {
-  unsigned long long d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(pack2(k, k)), "l"(pack2(x0, x1)));
-  unpack2(d, d0, d1);
-}
-__device__ __forceinline__ void add2(float a0, float a1, float b0, float b1, float& d0, float& d1) {
-  unsigned long long d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(pack2(a0, a1)), "l"(pack2(b0, b1)));
-  unpack2(d, d0, d1);
-}
 
 __device__ __forceinline__ float byteToFloat(uint32_t word, int k) {
 #if T360_BLUR_I2F == 1
@@ -232,27 +207,10 @@ __device__ __forceinline__ void stripChunk(const StripRowReader<EDGE>& rd, const
   uint32_t grp = 0;
   if (!LAST) grp = rd.next(c + 3, prev);  // the group that replaces the 4 oldest window positions
   const float k[4] = {k4.x, k4.y, k4.z, k4.w};
-#if T360_BLUR_F32X2
-  // sums 2j and 2j + 1 advance as a pair; for even taps their two window floats are an aligned pair of the ring as well
-#pragma unroll
-  for (int t = 0; t < 4; ++t)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      constexpr int kRing = 12;
-      const int a = (4 * U + 2 * j + t) % kRing;
-      if ((t & 1) == 0) {
-        fma2(k[t], ring[a], ring[a + 1], s[2 * j], s[2 * j + 1]);
-      } else {
-        s[2 * j] = __fmaf_rn(k[t], ring[a], s[2 * j]);
-        s[2 * j + 1] = __fmaf_rn(k[t], ring[(a + 1) % kRing], s[2 * j + 1]);
-      }
-    }
-#else
 #pragma unroll
   for (int t = 0; t < 4; ++t)
 #pragma unroll
     for (int m = 0; m < 8; ++m) s[m] = __fmaf_rn(k[t], ring[(4 * U + m + t) % 12], s[m]);
-#endif
   if (!LAST) {
 #pragma unroll
     for (int b = 0; b < 4; ++b) ring[4 * U + b] = byteToFloat(grp, b);
@@ -339,21 +297,6 @@ __device__ __forceinline__ void stripBody(const StripParams& p, const StripJob& 
           // centre row is the one computed HY steps ago: ring slot (u - HY) mod L
           constexpr int kBig = 4 * L;
           float o[8];
-#if T360_BLUR_F32X2
-#pragma unroll
-          for (int m = 0; m < 8; m += 2) {
-            float a0, a1;
-            mul2(kv[0], R[(u - HY + kBig) % L][m], R[(u - HY + kBig) % L][m + 1], a0, a1);
-#pragma unroll
-            for (int i = 1; i <= HY; ++i) {
-              float p0, p1;
-              add2(R[(u - HY + i + kBig) % L][m], R[(u - HY + i + kBig) % L][m + 1], R[(u - HY - i + kBig) % L][m],
-                   R[(u - HY - i + kBig) % L][m + 1], p0, p1);
-              fma2(kv[i], p0, p1, a0, a1);
-            }
-            add2(a0, a1, 12582912.0f, 12582912.0f, o[m], o[m + 1]);  // low mantissa byte = rint(acc), half-even
-          }
-#else
 #pragma unroll
           for (int m = 0; m < 8; ++m) {
             float acc = __fmul_rn(kv[0], R[(u - HY + kBig) % L][m]);
@@ -362,7 +305,6 @@ __device__ __forceinline__ void stripBody(const StripParams& p, const StripJob& 
               acc = __fmaf_rn(kv[i], __fadd_rn(R[(u - HY + i + kBig) % L][m], R[(u - HY - i + kBig) % L][m]), acc);
             o[m] = __fadd_rn(acc, 12582912.0f);  // low mantissa byte = rint(acc), half-even
           }
-#endif
           const int y = job.y0 + j - 2 * HY;
           uint8_t* out = p.dst + (size_t)y * p.dstPitch + lx;
           const uint32_t lo = __byte_perm(__byte_perm(__float_as_uint(o[0]), __float_as_uint(o[1]), 0x0040),
@@ -387,7 +329,7 @@ template <int HY>
 #define T360_BLUR_PDL 0
 #endif
 #ifndef T360_BLUR_MINBLOCKS
-#define T360_BLUR_MINBLOCKS 6  // 85 registers: 130.3 us per cfg3 frame against 137.9 at 3 blocks (128 registers)
+#define T360_BLUR_MINBLOCKS 6  // H100 at 700 W: 80 registers (with spills), 142.4 us per cfg3 frame; 4 blocks 144.4 us, 3 blocks 157.2 us
 #endif
 __global__ void __launch_bounds__(128, T360_BLUR_MINBLOCKS) blurStripKernel(StripParams p) {
   const int job = blockIdx.x * 4 + (threadIdx.x >> 5);

@@ -1,4 +1,4 @@
-// Device-side interface of the remap hot path (sm_100a).  See kernels.cu.
+// Device-side interface of the remap hot path (sm_90a).  See kernels.cu.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -22,7 +22,8 @@ struct GatherParams {
 
 // ---- the persistent frame gather (gatherFrameKernel) -------------------------------------------------------------
 // One CTA per SM: gatherGroups(k) GROUPS of 8 consumer warps + 1 producer warp each, all sharing one copy of the weight
-// tables in shared memory.  A producer claims jobs from the frame's job list (an atomic counter, one job at a time: 55.8 us per cfg2 frame against 58.5 / 63.2 with batches of 2 / 4, whose last batches leave groups idle at the end),
+// tables in shared memory.  A producer claims jobs from the frame's job list (an atomic counter, one job at a time: batches of 2 / 4, T360_CLAIM_BATCH, left groups idle at the end of a frame on the B200, where this
+// was chosen; not re-measured on the H100),
 // and for every job fills one stage of its group's two-stage ring: the job header (st.shared), the job's
 // compact sampling records (cp.async.bulk) and its source window (ONE cp.async.bulk.tensor.2d box from the
 // pitch-linear plane), all signalled through the stage's "full" mbarrier.  The consumer warps wait for "full", compute,
@@ -38,8 +39,9 @@ struct GatherJob {
 // of decreasing height (boxVariantRows below), and a job names the lowest one that still holds the rows its windows span
 // (cfg2: the share jobs span 63 of the 72 rows their stage buffer holds, the 32 x 32 tiles 47 of 64, the quadrants 36 of
 // 64: 18 % fewer bytes from L2 into shared memory than with whole boxes).  Loading a box as a series of 8-row TMA boxes
-// instead -- one tensor map per class, any height -- saved 21 % of the bytes but cost 0.3 us of producer time per job
-// (6 - 9 TMA instructions + as many L2 prefetches): 67.3 us per cfg2 frame against 56.4.
+// instead -- one tensor map per class, any height -- saves 21 % of the bytes but costs the producer 6 - 9 TMA instructions
+// (+ as many L2 prefetches) per job, which made the frame slower than the bytes it saved (measured on the B200, where
+// this was decided; not re-measured on the H100).
 constexpr int kBoxVariants = 3;
 __host__ __device__ constexpr int jobBoxField(int boxX, int boxY, int variant) { return boxX | (boxY << 16) | variant; }
 __host__ __device__ constexpr int jobBoxX(int boxXY) { return boxXY & 0xfff0; }
@@ -91,8 +93,8 @@ __host__ __device__ constexpr int boxVariantFor(int k, int cls, int rows) {
   return v;
 }
 // Stages of a group's ring (a stage = one box + one record buffer).  Three fit beside the cubic tables if the boxes lose
-// a few rows, but measured slower (64.9 vs 58.1 us per cfg2 frame): they leave the SM only ~3 KB of L1 for the general
-// jobs and the job headers.
+// a few rows, but then leave the SM only ~3 KB of L1 for the general jobs and the job headers, which made the frame
+// slower (measured on the B200, where this was decided; not re-measured on the H100).
 __host__ __device__ constexpr int gatherStages(int /*k*/) { return 2; }
 // one stage buffer (TMA destinations need 128-byte alignment; the tail absorbs the over-read of a window's last word)
 __host__ __device__ constexpr int stageBytesOf(int k) {
@@ -110,8 +112,8 @@ __host__ __device__ constexpr int stageBytesOf(int k) {
 // model worse), and the host -- which already deals the pixels of a row segment to lanes -- picks the copy per pixel so
 // that the groups are evenly filled (an EMPTY group costs as much as an overfull one: a quarter-warp that finds no pixel
 // in one group must take two of another) and then deals the pixels to quarter-warps exactly (gather_plan.cpp:
-// GroupMatcher, PassDealer): 4.4 wavefronts per load in share jobs, 4.5 in tile jobs of the cfg2 plan in the bank model
-// (which reproduces ncu's per-instruction counts to 1 %); with the group taken from fracX >> 2 it is 4.3 / 4.75, with a
+// GroupMatcher, PassDealer): 4.4 wavefronts per load in share jobs, 4.5 in tile jobs of the cfg2 plan in the offline bank
+// model (profiles/weight_sim.py); with the group taken from fracX >> 2 it is 4.3 / 4.75, with a
 // group that depends on fracY a share job's column could not keep its lane.
 __host__ __device__ constexpr int weightSlotOf(int k, int phase) {
   (void)k;

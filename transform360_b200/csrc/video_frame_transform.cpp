@@ -387,7 +387,7 @@ class VideoFrameTransform {
     std::vector<std::vector<GatherJob>> byWave(chunks);
     // Which output rectangles are complete after which wave: 32-row bands of the full width by default (contiguous
     // copies: a band split into the three faces of a cube-map row finishes earlier per face, but strided rectangle
-    // copies ran at 11 GB/s where whole bands reach 16-45 GB/s; T360B200_PIPELINE_BLOCKS > 1 splits anyway).
+    // copies are much slower than whole contiguous bands; T360B200_PIPELINE_BLOCKS > 1 splits anyway).
     int blocks = 1;
     for (int nb : {4, 3, 2})
       if (plan.mapW % (nb * t360::kShareW) == 0 && nb <= pipelineBlocks_) { blocks = nb; break; }
@@ -747,6 +747,7 @@ class VideoFrameTransform {
   void enableTrace(bool on) { traceEnabled_ = on; }
   size_t readTrace(unsigned long long* out, size_t maxWords) {
     if (!trace_.ptr) return 0;
+    if (!out) return trace_.count;  // the caller asks how large a buffer the trace needs
     const size_t n = std::min(maxWords, trace_.count);
     if (cudaMemcpy(out, trace_.ptr, n * sizeof(unsigned long long), cudaMemcpyDeviceToHost) != cudaSuccess) return 0;
     return n;
@@ -1531,7 +1532,7 @@ T360_API int T360B200_lowPassPlaneAsync(VideoFrameTransform* t, const uint8_t* d
 T360_API void T360B200_setPinHostPlanes(VideoFrameTransform* t, int enable) { if (t) t->setPinHostPlanes(enable != 0); }
 T360_API void T360B200_debugTrace(VideoFrameTransform* t, int enable) { if (t) t->enableTrace(enable != 0); }
 T360_API unsigned long long T360B200_debugTraceRead(VideoFrameTransform* t, unsigned long long* out, unsigned long long maxWords) {
-  return t && out ? t->readTrace(out, maxWords) : 0;
+  return t ? t->readTrace(out, maxWords) : 0;
 }
 T360_API int T360B200_synchronize(VideoFrameTransform* t) { return t ? t->synchronize() : 0; }
 T360_API void* T360B200_stream(VideoFrameTransform* t) { return t ? t->stream() : nullptr; }
@@ -1548,4 +1549,4 @@ T360_API int T360B200_deviceCount(void) {
   }
   return n;
 }
-T360_API const char* T360B200_version(void) { return "transform360-b200 0.1 (sm_100a)"; }
+T360_API const char* T360B200_version(void) { return "transform360-b200 0.1 (sm_90a)"; }

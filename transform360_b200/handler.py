@@ -225,10 +225,11 @@ class VideoFrameTransform:
     def debug_trace(self, enable: bool) -> None:
         self._lib.T360B200_debugTrace(self._h, 1 if enable else 0)
 
-    def read_trace(self, max_groups: int = 148 * 3) -> np.ndarray:
-        """[groups][64 jobs][wait start, ready, done (ns), kind] of the last whole-frame gather (after a synchronize)."""
-        buf = np.zeros(max_groups * 64 * 4, np.uint64)
-        n = int(self._lib.T360B200_debugTraceRead(self._h, buf.ctypes.data, buf.size))
+    def read_trace(self) -> np.ndarray:
+        """[groups][64 jobs][wait start, ready, done (ns), kind] of the last whole-frame gather (after a synchronize); the
+        library sizes the trace from the device's SM count."""
+        buf = np.zeros(int(self._lib.T360B200_debugTraceRead(self._h, None, 0)), np.uint64)
+        n = int(self._lib.T360B200_debugTraceRead(self._h, buf.ctypes.data, buf.size)) if buf.size else 0
         return buf[:n].reshape(-1, 64, 4)
 
     def synchronize(self) -> bool:

@@ -51,8 +51,8 @@ class StreamSpec:
 
 def bind_to_gpu_numa_node(gpu_index: int):
     """Pins the calling process to the CPUs of the NUMA node the GPU hangs off (PCI sysfs), BEFORE it allocates the
-    page-locked frame buffers, so that they are first-touched on that node.  On the 2-socket B200 boxes a pinned host
-    plane on the far socket is DMA'd at 20 GB/s instead of 55 GB/s (H2D), and 8 ranks without affinity fight over the
+    page-locked frame buffers, so that they are first-touched on that node.  On a 2-socket host a pinned host
+    plane on the far socket is DMA'd more slowly than one on the GPU's node, and 8 ranks without affinity fight over the
     inter-socket link.  Returns (node, cpus bound) or None when the topology cannot be read."""
     import os
     import subprocess
