@@ -39,6 +39,14 @@ const int32_t* T360B200_hostPlanSamples(const T360HostPlan* plan);
  * T360B200_hostPlanDestroy. */
 int T360B200_hostPlanGather(T360HostPlan* plan, int info[10], const int32_t** jobs, const int32_t** records,
                             const uint32_t** compact);
+/* What the frame kernel runs for the general jobs of T360B200_hostPlanGather (the pole caps, whose windows fit no box as
+ * a 32 x 32 tile), and the whole launch list.  info = {pole-cap jobs, border jobs, words of *capRecords, launch jobs};
+ * *capJobs: (pole-cap + border jobs) x 4 ints in the job format, record offsets counting on after the compact records
+ * (the device buffer holds compact records, then *capRecords); *launchJobs: the job list the kernel claims from, in
+ * launch order (every job of T360B200_hostPlanGather but the general ones, and *capJobs).  Formats: csrc/kernels.cuh.
+ * Returns 1 on success; the pointers stay valid until T360B200_hostPlanDestroy. */
+int T360B200_hostPlanPoleCaps(T360HostPlan* plan, int info[4], const int32_t** capJobs, const uint32_t** capRecords,
+                              const int32_t** launchJobs);
 /* How the host deals the n <= 32 pixels of one warp step to lanes and copies of the weight table (csrc/gather_plan.h:
  * dealLanes): phases[i] = (fracY32 << 5) | fracX32 of pixel i; laneOf[i] / copyOf[i] receive its lane and table copy.
  * Returns the modelled shared-memory wavefronts of one 128-bit weight load of the warp (0 when n < 32: identity deal). */
@@ -96,7 +104,7 @@ void* T360B200_stream(VideoFrameTransform* transform);
 unsigned long long T360B200_kernelLaunchCount(void);
 /* Bytes of device memory held by the plan of one index (sampling plan + low-pass tables). */
 unsigned long long T360B200_planDeviceBytes(VideoFrameTransform* transform, int transformMatPlaneIndex);
-/* counts[0] = gather tiles staged through TMA into shared memory, counts[1] = tiles on the general (L1) path,
+/* counts[0] = gather jobs staged through TMA into shared memory, counts[1] = gather jobs reading through L1 (border jobs),
  * counts[2] = low-pass warp-jobs on the register-resident strip kernel, counts[3] = low-pass jobs on the general
  * (large vertical kernel) paths. */
 int T360B200_planTileCounts(VideoFrameTransform* transform, int transformMatPlaneIndex, int counts[4]);

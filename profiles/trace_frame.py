@@ -17,7 +17,7 @@ from bench import CONFIGS  # noqa: E402
 from transform360_b200 import synth  # noqa: E402
 from transform360_b200.stream import FrameTransformer, StreamSpec  # noqa: E402
 
-KINDS = {0: "class0", 1: "class1", 2: "general", 3: "share-stay", 4: "share", 5: "nop", 7: "seam"}
+KINDS = {0: "class0", 1: "class1", 3: "share-stay", 4: "share", 5: "nop", 7: "seam", 8: "pole-cap", 9: "border"}
 
 
 def main():

@@ -19,7 +19,10 @@
 //   * Share jobs (64 x 32 pixels, 3/5 of a cube map): a thread slides one K-row register window down its output column
 //     and fetches only the 1-2 new source rows per pixel, branch-free; 2.5 bytes of plan per pixel.
 //   * Tile jobs (32 x 32 or one 16 x 16 quadrant): a window per pixel, lanes cover 8 x 4 patches, 4 bytes of plan per
-//     pixel; seam jobs OR two boxes together; general jobs (pole caps) read their taps through L1 in the same launch.
+//     pixel; seam jobs OR two boxes together.
+//   * Pole-cap jobs (the pixels no tile's box holds, grouped by source position into class-0 boxes): a window per pixel,
+//     8 bytes of plan per pixel with its output position.  Only the few pixels whose window wraps around a plane border
+//     (border jobs) read their taps through L1.
 //   * Programmatic dependent launch lets the next frame's prologue run under this frame's tail; the job counter re-arms
 //     itself.
 #include "gather_common.cuh"
@@ -267,59 +270,36 @@ __device__ __forceinline__ void computeTileJob(const PlaneView& pv, uint32_t sta
   });
 }
 
-// ---- general job: taps through L1, any border case ------------------------------------------------------------------
-// Pole caps and whatever else fits no staging box: latency-bound.  So the four records of a thread are requested
-// together, then the windows of all (K = 8: two) pixels, and only then the arithmetic starts: two round trips to L2 /
-// DRAM per job instead of eight.  Windows that touch a plane border (rare) take the per-tap path of gatherPixel.
+// ---- pole-cap job: a class-0 box of pixels grouped by source position, each with its own output position -----------
+// Warp w takes steps w, w + 8, .. of the job's `steps` (kernels.cuh: "cap job").
+template <int K, int PITCH, int VS>
+__device__ __forceinline__ void computeCapJob(const PlaneView& pv, uint32_t stageAddr, uint32_t recAddr, int steps, uint32_t wAddr,
+                                              int warp, int lane) {
+  static_assert(PITCH % 4 == 0, "");
+  for (int s = warp; s < steps; s += kGroupWarps) {
+    const uint2 r = ldsVec2Imm<0>(recAddr + s * kCapStepBytes + lane * 8);
+    if (r.x & kRecordSkip) continue;
+    const uint32_t rowAddr = stageAddr + (r.x & 0x7ffcu);
+    const int sh = (int)(r.x << 3);
+    RowBytes<K> W[K];
+    staticFor<K>([&](auto R) { W[decltype(R)::value] = loadRow<K, decltype(R)::value * PITCH>(rowAddr, sh); });
+    const int acc = foldPixel<K, VS>(W, wAddr, (r.x >> 17) & kSlotFieldMask);
+    pv.dst[(size_t)(r.y >> 16) * pv.dstPitch + (r.y & 0xffffu)] = (uint8_t)biasedToByte(acc);
+  }
+}
+
+// ---- border job: pixels whose window leaves the plane (BORDER_WRAP), one tap at a time through L1 ------------------
 template <int K, int VS>
-__device__ __forceinline__ void computeGeneralJob(const PlaneView& pv, int outX, int outY, const unsigned char* wsmem, uint32_t wAddr,
-                                                  int lane, int warp) {
+__device__ __forceinline__ void computeBorderJob(const PlaneView& pv, uint32_t recAddr, int n, const unsigned char* wsmem, int warp, int lane) {
   SrcView sv;
   sv.bytes = pv.src;
   sv.misalign = (int)(reinterpret_cast<uintptr_t>(pv.src) & 3);
   sv.words = reinterpret_cast<const uint32_t*>(pv.src - sv.misalign);
   sv.w = pv.srcW; sv.h = pv.srcH; sv.pitch = pv.srcPitch;
-  const int y0 = outY + warp * kRowsPerThread;
-  if (outX + lane >= pv.dstW) return;
-  // full records, tile-major over tiles of 32 x gatherTileH(K) pixels
-  const int2* segment = pv.samples + ((size_t)(y0 / gatherTileH(K)) * pv.tilesPerRow + outX / kGatherTileW) * gatherTileH(K) * kGatherTileW +
-                        (y0 % gatherTileH(K)) * kGatherTileW + lane;
-  int2 full[kRowsPerThread];
-#pragma unroll
-  for (int j = 0; j < kRowsPerThread; ++j) full[j] = y0 + j < pv.dstH ? loadPlan(segment + j * kGatherTileW) : make_int2(0, 0);
-  constexpr int kBatch = K == 8 ? 2 : 4;  // windows in flight per thread (registers)
-#pragma unroll
-  for (int jb = 0; jb < kRowsPerThread; jb += kBatch) {
-    RowBytes<K> W[kBatch][K];
-    bool interior[kBatch];
-#pragma unroll
-    for (int b = 0; b < kBatch; ++b) {
-      const int col0 = recordCol0(full[jb + b].x), row0 = full[jb + b].y >> 10;
-      // no wrapping, and the aligned word reads stay inside the row even when the pitch equals the width
-      interior[b] = y0 + jb + b < pv.dstH && col0 >= 0 && row0 >= 0 && col0 + (K == 2 ? 8 : K + 4) <= sv.w && row0 + K <= sv.h;
-#pragma unroll
-      for (int r = 0; r < K; ++r) {
-        W[b][r].b[0] = 0;
-        if constexpr (K == 8) W[b][r].b[1] = 0;
-        if (interior[b]) {
-          const int off = (row0 + r) * sv.pitch + col0 + sv.misalign;
-          const uint32_t* q = sv.words + (off >> 2);
-          const int sh = (off & 3) * 8;
-          const uint32_t q0 = __ldg(q), q1 = __ldg(q + 1);
-          W[b][r].b[0] = __funnelshift_r(q0, q1, sh);
-          if constexpr (K == 8) W[b][r].b[1] = __funnelshift_r(q1, __ldg(q + 2), sh);
-        }
-      }
-    }
-#pragma unroll
-    for (int b = 0; b < kBatch; ++b) {
-      const int j = jb + b;
-      if (y0 + j >= pv.dstH) continue;
-      int v;
-      if (interior[b]) v = biasedToByte(foldPixel<K, VS>(W[b], wAddr, (uint32_t)weightSlotOf(K, full[j].y & 1023) << 4));
-      else v = gatherPixel<K, false, VS, weightDiagonal(K)>(sv, wsmem, recordCol0(full[j].x), full[j].y);
-      pv.dst[(size_t)(y0 + j) * pv.dstPitch + outX + recordColumn(full[j].x)] = (uint8_t)v;
-    }
+  for (int i = warp * 32 + lane; i < n; i += kGroupThreads) {
+    const uint4 r = ldsVecImm<0>(recAddr + i * kBorderPixelBytes);
+    const int v = gatherPixel<K, false, VS, weightDiagonal(K)>(sv, wsmem, (int)r.x, (int)r.y);
+    pv.dst[(size_t)(r.z >> 16) * pv.dstPitch + (r.z & 0xffffu)] = (uint8_t)v;
   }
 }
 
@@ -454,20 +434,23 @@ gatherFrameKernel(const __grid_constant__ FrameGatherParams p, StagedParams jobs
       if (lane == 0) {
         unsigned char* rec = groupBase + S * kStage + st * kRec;
         *reinterpret_cast<int4*>(rec) = h;
-        if (kind == kJobShare || kind == kJobShareStay || kind == kJobClass0 || kind == kJobClass1 || kind == kJobSeam) {
-          const int pl = h.y >> kJobPlaneShift;
-          const bool share = boxClassOf(kind) == 2;
-          // the source box: the lowest variant of its class that holds the rows the job's windows span (kernels.cuh)
-          const int cls = boxClassOf(kind), variant = jobBoxVariant(h.z), boxX = jobBoxX(h.z), boxY = jobBoxY(h.z);
-          const uint32_t boxBytes = (uint32_t)(stageBoxW(K, cls) * boxVariantRows(K, cls, variant));
-          const uint32_t recBytes = share ? shareJobRecordBytes(K) : tileJobRecordBytes(h.x);
-          mbarExpectTx(full + st, (kind == kJobSeam ? 2 : 1) * boxBytes + recBytes);
-          tmaLoadBox(groupBase + st * kStage, &maps.map[pl][cls][variant], boxX, boxY, full + st);
-          if (kind == kJobSeam)  // the part of the window beyond the right border, from the left of the plane
-            tmaLoadBox(groupBase + (st + 1) * kStage, &maps.map[pl][0][variant], boxX - planes[pl].srcW, boxY, full + st);
-          bulkCopyToShared(rec + 128, planes[pl].records + (unsigned)h.w, recBytes, full + st);
+        if (kind == kJobExit) {
+          mbarArrive(full + st);  // end of the list: the header is all there is
         } else {
-          mbarArrive(full + st);  // general job / end of list: the header is all there is
+          const int pl = h.y >> kJobPlaneShift;
+          const uint32_t recBytes = (uint32_t)jobRecordBytes(K, kind, h.x);
+          if (kind == kJobBorder) {  // records only: its taps are read through L1
+            mbarExpectTx(full + st, recBytes);
+          } else {
+            // the source box: the lowest variant of its class that holds the rows the job's windows span (kernels.cuh)
+            const int cls = boxClassOf(kind), variant = jobBoxVariant(h.z), boxX = jobBoxX(h.z), boxY = jobBoxY(h.z);
+            const uint32_t boxBytes = (uint32_t)(stageBoxW(K, cls) * boxVariantRows(K, cls, variant));
+            mbarExpectTx(full + st, (kind == kJobSeam ? 2 : 1) * boxBytes + recBytes);
+            tmaLoadBox(groupBase + st * kStage, &maps.map[pl][cls][variant], boxX, boxY, full + st);
+            if (kind == kJobSeam)  // the part of the window beyond the right border, from the left of the plane
+              tmaLoadBox(groupBase + (st + 1) * kStage, &maps.map[pl][0][variant], boxX - planes[pl].srcW, boxY, full + st);
+          }
+          bulkCopyToShared(rec + 128, planes[pl].records + (unsigned)h.w, recBytes, full + st);
         }
       }
       advance();
@@ -500,9 +483,11 @@ gatherFrameKernel(const __grid_constant__ FrameGatherParams p, StagedParams jobs
   unsigned long long* trace = jobs.trace && warp == 0 && lane == 0 ? jobs.trace + (size_t)(blockIdx.x * GROUPS + group) * kTraceJobsPerGroup * 4 : nullptr;
   uint32_t traced = 0;
   for (uint32_t st = 0, phase = 0;;) {
-    const unsigned long long t0 = trace ? now() : 0;
+    // (the timestamps go to the trace at once: two 64-bit values held over a job cost the K = 8 kernel a spill)
+    unsigned long long* const row = trace && traced < kTraceJobsPerGroup ? trace + traced * 4 : nullptr;
+    if (row) row[0] = now();
     mbarWait(full + st, phase);
-    const unsigned long long t1 = trace ? now() : 0;
+    if (row) row[1] = now();
     const uint32_t rec = recAddr + st * kRec;
     const uint4 h = ldsVec(rec);
     const int kind = ((int)h.y >> kJobKindShift) & kJobKindMask;
@@ -551,13 +536,15 @@ gatherFrameKernel(const __grid_constant__ FrameGatherParams p, StagedParams jobs
       }
       groupBarrier(group);
       computeTileJob<K, stageBoxW(K, 0), VS>(pv, boxAddr + st * kStage, outX, outY, ldsVec(rec + 128 + warp * 512 + lane * 16), wAddr, warp);
-    } else if (kind == kJobGeneral) {
-      computeGeneralJob<K, VS>(pv, outX, outY, wsmem, wAddr, lane, warp);
+    } else if (kind == kJobCap) {
+      computeCapJob<K, stageBoxW(K, 0), VS>(pv, boxAddr + st * kStage, rec + 128, (int)h.x, wAddr, warp, lane);
+    } else if (kind == kJobBorder) {
+      computeBorderJob<K, VS>(pv, rec + 128, (int)h.x, wsmem, warp, lane);
     }
     __syncwarp();
     if (lane == 0) mbarArrive(empty + st);  // this warp is done with the stage (its shared-memory reads are complete)
-    if (trace && traced < kTraceJobsPerGroup) {
-      trace[traced * 4 + 0] = t0; trace[traced * 4 + 1] = t1; trace[traced * 4 + 2] = now(); trace[traced * 4 + 3] = kind;
+    if (row) {
+      row[2] = now(); row[3] = kind;
       ++traced;
     }
     if (++st == S) { st = 0; phase ^= 1; }

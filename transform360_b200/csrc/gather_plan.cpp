@@ -5,7 +5,9 @@
 #include <climits>
 #include <cstdint>
 #include <cstring>
+#include <stdexcept>
 #include <thread>
+#include <utility>
 
 namespace t360 {
 namespace {
@@ -250,7 +252,7 @@ void classifyTile(const HostPlan& h, int x0, int y0, bool seamPossible, TileClas
       return;
     }
   }
-  out.kind = kJobGeneral;
+  out.kind = kJobGeneral;  // no box holds the tile: its pixels go to coverPoleCaps
   out.boxX = out.boxY = out.boxRows = 0;
 }
 
@@ -338,6 +340,132 @@ void writeTileRecords(const HostPlan& h, const GatherJob& job, uint32_t* out) {
                                            (slotField(k, sp.rowPhase & 1023, copyOf[i]) << 17);
       }
     }
+}
+
+// The output rectangle of a tile or share job (not clipped to the plane).
+JobRect tileRect(const GatherJob& job, int k) {
+  const int kind = (job.outY >> kJobKindShift) & kJobKindMask, quad = (job.outX & kJobQuadMask) - 1;
+  JobRect r;
+  r.x0 = job.outX & ~kJobQuadMask;
+  r.y0 = job.outY & kJobRowMask;
+  if (quad >= 0) { r.x0 += 16 * (quad & 1); r.y0 += 16 * (quad >> 1); }
+  const bool share = kind == kJobShare || kind == kJobShareStay;
+  r.x1 = r.x0 + (quad >= 0 ? 16 : (share ? kShareW : kGatherTileW));
+  r.y1 = r.y0 + (quad >= 0 ? 16 : (share ? shareH(k) : kFrameTileH));
+  return r;
+}
+
+// A pole-cap or border job with its records, before it has a place in the plan's record buffer.
+struct PixelJob {
+  GatherJob job;
+  std::vector<uint32_t> words;
+  JobRect rect;
+  int needRows;
+};
+
+struct CapPixel {
+  int x, y, col0, rowPhase;
+  int row() const { return rowPhase >> 10; }
+};
+
+PixelJob capJob(const HostPlan& h, const CapPixel* px, int n) {
+  const int k = h.kernelSize, copies = weightCopies(k), pitch = stageBoxW(k, 0);
+  PixelJob j;
+  int minC = INT32_MAX, minR = INT32_MAX, maxR = INT32_MIN;
+  j.rect = JobRect{INT32_MAX, INT32_MAX, INT32_MIN, INT32_MIN};
+  for (int i = 0; i < n; ++i) {
+    minC = std::min(minC, px[i].col0);
+    minR = std::min(minR, px[i].row());
+    maxR = std::max(maxR, px[i].row());
+    j.rect = JobRect{std::min(j.rect.x0, px[i].x), std::min(j.rect.y0, px[i].y), std::max(j.rect.x1, px[i].x + 1), std::max(j.rect.y1, px[i].y + 1)};
+  }
+  const int boxX = minC & ~15, boxY = minR, steps = (n + 31) / 32;
+  j.job = GatherJob{steps, kJobCap << kJobKindShift, jobBoxField(boxX, boxY, boxVariantFor(k, 0, maxR + k - minR)), 0};
+  j.needRows = maxR + k;
+  j.words.assign(static_cast<size_t>(steps) * kCapStepBytes / 4, 0u);
+  for (int s = 0; s < steps; ++s) {
+    const CapPixel* step = px + 32 * s;
+    const int m = std::min(32, n - 32 * s);
+    int slot[32], laneOf[32], copyOf[32];
+    for (int i = 0; i < m; ++i) slot[i] = weightSlotOf(k, step[i].rowPhase & 1023);
+    dealLanes(k, copies, m, slot, laneOf, copyOf);  // m < 32: identity order
+    uint32_t* words = &j.words[static_cast<size_t>(s) * kCapStepBytes / 4];
+    for (int lane = m; lane < 32; ++lane) words[2 * lane] = kRecordSkip;
+    for (int i = 0; i < m; ++i) {
+      const int off = (step[i].row() - boxY) * pitch + (step[i].col0 - boxX);
+      words[2 * laneOf[i]] = static_cast<uint32_t>(off) | (slotField(k, step[i].rowPhase & 1023, copyOf[i]) << 17);
+      words[2 * laneOf[i] + 1] = static_cast<uint32_t>(step[i].x) | (static_cast<uint32_t>(step[i].y) << 16);
+    }
+  }
+  return j;
+}
+
+PixelJob borderJob(const HostPlan& h, const CapPixel* px, int n) {
+  PixelJob j;
+  j.job = GatherJob{n, kJobBorder << kJobKindShift, 0, 0};
+  j.needRows = 0;  // (a window that wraps vertically reads the last rows)
+  j.rect = JobRect{INT32_MAX, INT32_MAX, INT32_MIN, INT32_MIN};
+  j.words.assign(static_cast<size_t>(n) * kBorderPixelBytes / 4, 0u);
+  for (int i = 0; i < n; ++i) {
+    j.words[4 * i] = static_cast<uint32_t>(px[i].col0);
+    j.words[4 * i + 1] = static_cast<uint32_t>(px[i].rowPhase);
+    j.words[4 * i + 2] = static_cast<uint32_t>(px[i].x) | (static_cast<uint32_t>(px[i].y) << 16);
+    j.needRows = std::max(j.needRows, px[i].row() >= 0 && px[i].row() + h.kernelSize <= h.inH ? px[i].row() + h.kernelSize : h.inH);
+    j.rect = JobRect{std::min(j.rect.x0, px[i].x), std::min(j.rect.y0, px[i].y), std::max(j.rect.x1, px[i].x + 1), std::max(j.rect.y1, px[i].y + 1)};
+  }
+  return j;
+}
+
+// The pixels of the tiles that no box holds (the pole caps: a tile's windows span hundreds of source columns there) are
+// grouped by SOURCE position instead: bands of source rows that fit a class-0 box, each cut greedily into runs of columns
+// that fit one (the fewest boxes for the band), each box into jobs of at most capJobMaxSteps(k) warp steps.  Inside a
+// job the pixels go in output order, so that a warp's byte stores land in as few output rows as the wedge allows.
+// Pixels whose window leaves the plane (BORDER_WRAP; NaN map entries) go to border jobs, per tile: a job's output
+// rectangle and source rows stay those of one tile (a plane streamed in row bands gets its output bands back early).
+void coverPoleCaps(const HostPlan& h, const std::vector<TileClass>& cls, int tilesX, int tilesY, std::vector<PixelJob>& out) {
+  const int k = h.kernelSize, boxW = stageBoxW(k, 0), boxH = stageBoxH(k, 0);
+  std::vector<CapPixel> cap, border;
+  std::vector<size_t> tileBorderStart;  // the border pixels of a tile are border[tileBorderStart[i] .. [i + 1])
+  for (int ty = 0; ty < tilesY; ++ty)
+    for (int tx = 0; tx < tilesX; ++tx) {
+      if (cls[static_cast<size_t>(ty) * tilesX + tx].kind != kJobGeneral) continue;
+      tileBorderStart.push_back(border.size());
+      for (int y = ty * kFrameTileH; y < std::min(h.mapH, (ty + 1) * kFrameTileH); ++y)
+        for (int x = tx * kGatherTileW; x < std::min(h.mapW, (tx + 1) * kGatherTileW); ++x) {
+          const SamplePoint& sp = h.samples[static_cast<size_t>(y) * h.mapW + x];
+          const CapPixel p{x, y, sp.col0, sp.rowPhase};
+          const bool inside = p.col0 >= 0 && p.row() >= 0 && p.col0 + k <= h.inW && p.row() + k <= h.inH;
+          (inside ? cap : border).push_back(p);
+        }
+    }
+  if (cap.empty() && border.empty()) return;
+  if (h.mapW > 65536 || h.mapH > 65536) throw std::invalid_argument("gather plan: pole-cap records hold 16-bit output positions");
+  auto outputOrder = [](const CapPixel& a, const CapPixel& b) { return a.y != b.y ? a.y < b.y : a.x < b.x; };
+  std::sort(cap.begin(), cap.end(), [](const CapPixel& a, const CapPixel& b) {
+    return a.row() != b.row() ? a.row() < b.row() : (a.y != b.y ? a.y < b.y : a.x < b.x);
+  });
+  for (size_t b0 = 0; b0 < cap.size();) {
+    size_t b1 = b0;
+    while (b1 < cap.size() && cap[b1].row() + k - cap[b0].row() <= boxH) ++b1;
+    std::sort(cap.begin() + b0, cap.begin() + b1, [](const CapPixel& a, const CapPixel& b) {
+      return a.col0 != b.col0 ? a.col0 < b.col0 : (a.y != b.y ? a.y < b.y : a.x < b.x);
+    });
+    for (size_t c0 = b0; c0 < b1;) {
+      const int boxX = cap[c0].col0 & ~15;
+      size_t c1 = c0;
+      while (c1 < b1 && cap[c1].col0 + k - boxX <= boxW) ++c1;
+      std::sort(cap.begin() + c0, cap.begin() + c1, outputOrder);
+      const int n = static_cast<int>(c1 - c0), jobs = ((n + 31) / 32 + capJobMaxSteps(k) - 1) / capJobMaxSteps(k);
+      const int per = ((n + jobs - 1) / jobs + 31) / 32 * 32;
+      for (int i = 0; i < n; i += per) out.push_back(capJob(h, &cap[c0 + i], std::min(per, n - i)));
+      c0 = c1;
+    }
+    b0 = b1;
+  }
+  tileBorderStart.push_back(border.size());
+  for (size_t t = 0; t + 1 < tileBorderStart.size(); ++t)  // (in output order already: a tile's pixels row by row)
+    for (size_t i = tileBorderStart[t]; i < tileBorderStart[t + 1]; i += borderJobMaxPixels(k))
+      out.push_back(borderJob(h, &border[i], static_cast<int>(std::min(tileBorderStart[t + 1] - i, static_cast<size_t>(borderJobMaxPixels(k))))));
 }
 
 }  // namespace
@@ -454,24 +582,6 @@ int dealLanes(int k, int copies, int n, const int* slot, int* laneOf, int* copyO
   return wavefronts;
 }
 
-void spreadGeneralJobs(std::vector<GatherJob>& jobs) {
-  std::vector<GatherJob> general, staged;
-  for (const GatherJob& j : jobs)
-    (((j.outY >> kJobKindShift) & kJobKindMask) == kJobGeneral ? general : staged).push_back(j);
-  if (general.empty() || staged.empty()) return;
-  // The first half of the staged jobs: none may land among the small jobs the launch ends with (a general job, several
-  // times longer than a staged one, claimed there is the last thing to finish and stretches the frame).
-  const size_t span = staged.size() / 2 + 1;
-  jobs.clear();
-  size_t g = 0;
-  for (size_t i = 0; i < staged.size(); ++i) {
-    // general job number g goes in front of staged job number g * span / general.size()
-    while (g < general.size() && g * span / general.size() <= i) jobs.push_back(general[g++]);
-    jobs.push_back(staged[i]);
-  }
-  while (g < general.size()) jobs.push_back(general[g++]);
-}
-
 std::vector<uint8_t> buildWeightImage(int k, const int16_t* table) {
   const int copies = weightCopies(k);
   std::vector<uint8_t> img(static_cast<size_t>(weightImageBytes(k, copies)), 0);
@@ -516,57 +626,82 @@ void buildGatherPlan(const HostPlan& h, bool stageTiles, GatherPlan& g) {
             classifyTile(h, t * 32, ty * kFrameTileH, seamPossible, cls[static_cast<size_t>(ty) * tilesX + t]);
       }
   });
-  // launch order: general tiles (latency-bound: they run while every group of the SM is busy), seam, class 1 (both
-  // need the two stage buffers), then the share jobs and finally the small class-0 tiles through the double-buffered
-  // TMA pipeline, which leaves a short, fine-grained tail
-  // (the cheapest jobs, the 16 x 16 quadrants, come last of all: every group has up to three jobs claimed ahead, so the
-  // launch ends within about three of its last jobs)
-  const int order[7] = {kJobGeneral, kJobSeam, kJobClass1, kJobShareStay, kJobShare, kJobClass0, kJobClass0};
-  size_t offset = 0;  // bytes
-  for (int step = 0; step < 7; ++step)
-    for (int ty = 0; ty < tilesY; ++ty)
-      for (int tx = 0; tx < tilesX; ++tx) {
-        const int kind = order[step];
-        const TileClass& c = cls[static_cast<size_t>(ty) * tilesX + tx];
-        if (c.kind != kind || (kind == kJobClass0 && c.quads != (step == 6))) continue;
-        for (int q = 0; q < (c.quads ? 4 : 1); ++q) {
-          GatherJob job{tx * 32, ty * kFrameTileH | (kind << kJobKindShift),
-                        kind == kJobGeneral ? 0 : jobBoxField(c.boxX, c.boxY, boxVariantFor(k, boxClassOf(kind), c.boxRows)), 0};
-          if (c.quads) {
-            job.outX |= q + 1;
-            job.boxXY = jobBoxField(c.quadBoxX[q], c.quadBoxY[q], boxVariantFor(k, 0, c.quadBoxRows[q]));
-          }
-          if (kind != kJobGeneral) {
-            job.recordOffset = static_cast<int>(offset / 16);
-            offset += boxClassOf(kind) == 2 ? shareJobRecordBytes(k) : tileJobRecordBytes(job.outX);
-          }
-          g.jobs.push_back(job);
+
+  // the tile list, sorted by rank: general tiles (no box, no records) first, then the staged kinds in launch order
+  for (int ty = 0; ty < tilesY; ++ty)
+    for (int tx = 0; tx < tilesX; ++tx) {
+      const TileClass& c = cls[static_cast<size_t>(ty) * tilesX + tx];
+      const int kind = c.kind;
+      if (kind < 0) continue;
+      for (int q = 0; q < (c.quads ? 4 : 1); ++q) {
+        GatherJob job{tx * 32, ty * kFrameTileH | (kind << kJobKindShift),
+                      kind == kJobGeneral ? 0 : jobBoxField(c.boxX, c.boxY, boxVariantFor(k, boxClassOf(kind), c.boxRows)), 0};
+        if (c.quads) {
+          job.outX |= q + 1;
+          job.boxXY = jobBoxField(c.quadBoxX[q], c.quadBoxY[q], boxVariantFor(k, 0, c.quadBoxRows[q]));
         }
-        switch (kind) {
-          case kJobGeneral: ++g.numGeneral; break;
-          case kJobSeam: ++g.numSeam; break;
-          case kJobShare: case kJobShareStay: ++g.numShare; break;
-          default: g.numStaged[kind] += c.quads ? 4 : 1; break;
-        }
+        g.jobs.push_back(job);
       }
+      switch (kind) {
+        case kJobGeneral: ++g.numGeneral; break;
+        case kJobSeam: ++g.numSeam; break;
+        case kJobShare: case kJobShareStay: ++g.numShare; break;
+        default: g.numStaged[kind] += c.quads ? 4 : 1; break;
+      }
+    }
+  std::stable_sort(g.jobs.begin(), g.jobs.end(), [](const GatherJob& a, const GatherJob& b) { return jobLaunchRank(a) < jobLaunchRank(b); });
+  size_t offset = 0;  // bytes
+  for (GatherJob& job : g.jobs) {
+    const int kind = (job.outY >> kJobKindShift) & kJobKindMask;
+    if (kind == kJobGeneral) continue;
+    job.recordOffset = static_cast<int>(offset / 16);
+    offset += jobRecordBytes(k, kind, job.outX);
+  }
   g.compact.assign(offset / 4, 0u);
-  g.jobNeedRows.assign(g.jobs.size(), h.inH);
+  std::vector<int> needRows(g.jobs.size(), h.inH);
+  std::vector<JobRect> rects(g.jobs.size());
   parallelRanges(static_cast<int>(g.jobs.size()), 2048, [&](int begin, int end) {
     for (int i = begin; i < end; ++i) {
       const GatherJob& job = g.jobs[i];
-      {  // the source rows the job reads: what a caller that streams the plane in must have delivered before it runs
-        int rect[4];
-        jobOutputRect(job, k, rect);
-        const Extent e = extentOf(h, rect[0], rect[1], std::min(rect[2], h.mapW), std::min(rect[3], h.mapH));
-        if (e.minR >= 0 && e.maxR + k <= h.inH) g.jobNeedRows[i] = e.maxR + k;
-      }
+      JobRect& r = rects[i];
+      r = tileRect(job, k);
+      r.x1 = std::min(r.x1, h.mapW);
+      r.y1 = std::min(r.y1, h.mapH);
       const int kind = (job.outY >> kJobKindShift) & kJobKindMask;
       if (kind == kJobGeneral) continue;
+      // the source rows the job reads: what a caller that streams the plane in must have delivered before it runs
+      const Extent e = extentOf(h, r.x0, r.y0, r.x1, r.y1);
+      if (e.minR >= 0 && e.maxR + k <= h.inH) needRows[i] = e.maxR + k;
       uint32_t* out = g.compact.data() + static_cast<size_t>(job.recordOffset) * 4;
       if (boxClassOf(kind) == 2) writeShareRecords(h, job, out);
       else writeTileRecords(h, job, out);
     }
   });
+
+  // the pixels of the general tiles: pole-cap and border jobs, their records after the tiles'
+  std::vector<PixelJob> pixelJobs;
+  coverPoleCaps(h, cls, tilesX, tilesY, pixelJobs);
+  for (PixelJob& pj : pixelJobs) {
+    const int kind = (pj.job.outY >> kJobKindShift) & kJobKindMask;
+    pj.job.recordOffset = static_cast<int>(offset / 16);
+    offset += jobRecordBytes(k, kind, pj.job.outX);
+    g.capJobs.push_back(pj.job);
+    g.capRecords.insert(g.capRecords.end(), pj.words.begin(), pj.words.end());
+    ++(kind == kJobCap ? g.numCap : g.numBorder);
+  }
+
+  // the launch list: index into `jobs`, or -1 - index into capJobs
+  std::vector<int> launch;
+  for (size_t i = 0; i < g.jobs.size(); ++i)
+    if (((g.jobs[i].outY >> kJobKindShift) & kJobKindMask) != kJobGeneral) launch.push_back(static_cast<int>(i));
+  for (size_t i = 0; i < g.capJobs.size(); ++i) launch.push_back(-1 - static_cast<int>(i));
+  auto jobOf = [&](int i) -> const GatherJob& { return i >= 0 ? g.jobs[i] : g.capJobs[-1 - i]; };
+  std::stable_sort(launch.begin(), launch.end(), [&](int a, int b) { return jobLaunchRank(jobOf(a)) < jobLaunchRank(jobOf(b)); });
+  for (int i : launch) {
+    g.launchJobs.push_back(jobOf(i));
+    g.launchNeedRows.push_back(i >= 0 ? needRows[i] : pixelJobs[-1 - i].needRows);
+    g.launchRects.push_back(i >= 0 ? rects[i] : pixelJobs[-1 - i].rect);
+  }
 }
 
 }  // namespace t360

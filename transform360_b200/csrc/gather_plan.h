@@ -11,35 +11,51 @@
 
 namespace t360 {
 
+struct JobRect {
+  int x0, y0, x1, y1;
+};
+
 struct GatherPlan {
   int tilesPerRow = 0, tileRows = 0, tileH = 0;  // grid of the FULL records: tiles of 32 x tileH pixels (general kernels)
   std::vector<int2> records;                     // full records: tile-major, lane-ordered (kernels.cuh)
-  std::vector<GatherJob> jobs;                   // general, seam, class 1, share, class 0 (empty: the plan is not staged)
-  std::vector<uint32_t> compact;                 // compact records of the staged jobs (GatherJob::recordOffset)
-  std::vector<int> jobNeedRows;                  // per job: source rows [0, n) it reads (inH if a window wraps vertically)
-  int numStaged[2] = {}, numSeam = 0, numGeneral = 0, numShare = 0;
-  int totalStaged() const { return numSeam + numShare + numStaged[0] + numStaged[1]; }
+  // The plane cut into share blocks and 32 x 32 tiles, sorted by jobLaunchRank (empty: the plan is not staged), and the
+  // compact records of its staged entries.  A general entry (a pole-cap tile) has no box and no records: its pixels are
+  // in capJobs.
+  std::vector<GatherJob> jobs;
+  std::vector<uint32_t> compact;
+  // The pixels of the general tiles as pole-cap and border jobs; their record offsets count on after `compact`, i.e. in
+  // the device's record buffer  compact ++ capRecords.
+  std::vector<GatherJob> capJobs;
+  std::vector<uint32_t> capRecords;
+  // What the frame kernel runs: `jobs` without the general tiles, and capJobs, in launch order; per job the source rows
+  // [0, n) it reads (inH if a window wraps vertically) and the bounding rectangle of the output pixels it writes.
+  std::vector<GatherJob> launchJobs;
+  std::vector<int> launchNeedRows;
+  std::vector<JobRect> launchRects;
+  int numStaged[2] = {}, numSeam = 0, numGeneral = 0, numShare = 0, numCap = 0, numBorder = 0;
+  int totalStaged() const { return numSeam + numShare + numStaged[0] + numStaged[1] + numCap; }
 };
 
 // stageTiles: cut the plane into jobs for the persistent kernel (kernel size >= 2 and BORDER_WRAP); otherwise only the
 // full records are produced (nearest neighbour, barrel layouts: whole-plane general kernels).
 void buildGatherPlan(const HostPlan& h, bool stageTiles, GatherPlan& g);
 
-// The output rectangle of a job {x0, y0, x1, y1} (clipped to the plane by the caller).
-inline void jobOutputRect(const GatherJob& job, int k, int rect[4]) {
-  const int kind = (job.outY >> kJobKindShift) & kJobKindMask, quad = (job.outX & kJobQuadMask) - 1;
-  rect[0] = job.outX & ~kJobQuadMask;
-  rect[1] = job.outY & kJobRowMask;
-  if (quad >= 0) { rect[0] += 16 * (quad & 1); rect[1] += 16 * (quad >> 1); }
-  const bool share = kind == kJobShare || kind == kJobShareStay;
-  rect[2] = rect[0] + (quad >= 0 ? 16 : (share ? kShareW : kGatherTileW));
-  rect[3] = rect[1] + (quad >= 0 ? 16 : (share ? shareH(k) : kFrameTileH));
+// Launch order of the jobs: border (latency-bound reads through L1, few; in the tile list: the general tiles), seam and class 1 (both need the two stage
+// buffers of a group), pole caps, share jobs, and finally the small class-0 tiles through the double-buffered TMA
+// pipeline, which leaves a short, fine-grained tail (the cheapest jobs, the 16 x 16 quadrants, come last of all: every
+// group has up to three jobs claimed ahead, so the launch ends within about three of its last jobs).  A list sorted by
+// this rank (stably: a frame's list keeps the planes in order inside a rank) is in launch order.
+inline int jobLaunchRank(const GatherJob& job) {
+  switch ((job.outY >> kJobKindShift) & kJobKindMask) {
+    case kJobBorder: case kJobGeneral: return 0;
+    case kJobSeam: return 1;
+    case kJobClass1: return 2;
+    case kJobCap: return 3;
+    case kJobShareStay: return 4;
+    case kJobShare: return 5;
+    default: return (job.outX & kJobQuadMask) ? 7 : 6;  // class 0: whole tiles, then quadrants
+  }
 }
-
-// Launch order of a job list that is sorted by kind (general, class 1, share, class 0): the general jobs -- latency-bound
-// reads through L1 that leave the shared-memory pipe idle -- are spread evenly over the first half of the staged jobs,
-// so that they run beside them instead of all at once at the start of the launch.
-void spreadGeneralJobs(std::vector<GatherJob>& jobs);
 
 
 // Deals n <= 32 pixels of one warp step to lanes (and table copies) so that the lanes one shared-memory pass serves

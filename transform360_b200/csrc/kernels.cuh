@@ -48,7 +48,11 @@ __host__ __device__ constexpr int jobBoxX(int boxXY) { return boxXY & 0xfff0; }
 __host__ __device__ constexpr int jobBoxY(int boxXY) { return (int)((unsigned)boxXY >> 16); }
 __host__ __device__ constexpr int jobBoxVariant(int boxXY) { return boxXY & 15; }
 using StagedTile = GatherJob;
-constexpr int kJobClass0 = 0, kJobClass1 = 1, kJobGeneral = 2, kJobShareStay = 3, kJobShare = 4, kJobNop = 5, kJobExit = 6, kJobSeam = 7;
+// kJobGeneral: a 32 x 32 tile whose windows fit no box (the pole caps).  It is an entry of the plan's tile list only;
+// the kernel runs its pixels as kJobCap jobs (grouped by source position into class-0 boxes) and, the few whose window
+// leaves the plane (wraps), as kJobBorder jobs (one tap at a time through L1).
+constexpr int kJobClass0 = 0, kJobClass1 = 1, kJobGeneral = 2, kJobShareStay = 3, kJobShare = 4, kJobNop = 5, kJobExit = 6, kJobSeam = 7,
+              kJobCap = 8, kJobBorder = 9;
 // A 32 x 32 job may cover one 16 x 16 quadrant of its tile only (a tile whose windows fit no box as a whole, but whose
 // quadrants do: the ring around a pole cap): outX carries 1 + the quadrant in its low bits (0: the whole tile), and the
 // records of the pixels outside the quadrant have kRecordSkip set.
@@ -93,8 +97,8 @@ __host__ __device__ constexpr int boxVariantFor(int k, int cls, int rows) {
   return v;
 }
 // Stages of a group's ring (a stage = one box + one record buffer).  Three fit beside the cubic tables if the boxes lose
-// a few rows, but then leave the SM only ~3 KB of L1 for the general jobs and the job headers, which made the frame
-// slower (measured on the B200, where this was decided; not re-measured on the H100).
+// a few rows (not measured since no job reads its windows through L1 any more; at the time the third stage left too
+// little L1 for those reads and made the frame slower, measured on the B200).
 __host__ __device__ constexpr int gatherStages(int /*k*/) { return 2; }
 // one stage buffer (TMA destinations need 128-byte alignment; the tail absorbs the over-read of a window's last word)
 __host__ __device__ constexpr int stageBytesOf(int k) {
@@ -156,7 +160,11 @@ __host__ __device__ constexpr int weightLanesPerPass(int k) { return k == 2 ? 16
 //                8 * j ..: off (15 bits) | position << 16 (5 bits: column in patch | row in patch << 3) | slotField << 17.
 //                4 bytes per pixel.  The pixels of a patch are dealt to lanes (and copies) per patch; pixels outside the
 //                plane carry a position that fails the bounds check.
-// General jobs read the full records below.
+//   cap job      GatherJob::outX = its warp steps S (outY: no row); step s (warp s % 8) = 32 x uint2 by lane at byte 256 s:
+//                {off (15 bits) | slotField << 17, or kRecordSkip;  outX | outY << 16 of the pixel in the plane}.
+//                8 bytes per pixel; the 32 pixels of a step are dealt to lanes (and copies) like a patch.
+//   border job   GatherJob::outX = its pixels n; pixel i = uint4 {col0, row0 << 10 | phase, outX | outY << 16, 0} at 16 i.
+// The whole-plane general kernels read the full records below.
 __host__ __device__ constexpr int shareWarpRecordBytes(int k) { return shareRows(k) / 8 * 32 * 16 + 32 * 4; }
 __host__ __device__ constexpr int shareJobRecordBytes(int k) { return kGroupWarps * shareWarpRecordBytes(k); }
 constexpr int kTileJobRecordBytes = kGroupWarps * 32 * 16;
@@ -168,6 +176,16 @@ __host__ __device__ constexpr int tileJobRecordBytes(int outXField) { return (ou
 __host__ __device__ constexpr int stageRecordBytes(int k) {
   return 128 + (shareJobRecordBytes(k) > kTileJobRecordBytes ? shareJobRecordBytes(k) : kTileJobRecordBytes);
 }
+constexpr int kCapStepBytes = 32 * 8, kBorderPixelBytes = 16;
+__host__ __device__ constexpr int capJobMaxSteps(int k) { return (stageRecordBytes(k) - 128) / kCapStepBytes; }
+__host__ __device__ constexpr int borderJobMaxPixels(int k) { return (stageRecordBytes(k) - 128) / kBorderPixelBytes; }
+// bytes of compact records of a job (outXField = GatherJob::outX)
+__host__ __device__ constexpr int jobRecordBytes(int k, int kind, int outXField) {
+  return kind == kJobShare || kind == kJobShareStay ? shareJobRecordBytes(k)
+         : kind == kJobCap                          ? outXField * kCapStepBytes
+         : kind == kJobBorder                       ? outXField * kBorderPixelBytes
+                                                    : tileJobRecordBytes(outXField);
+}
 constexpr int kRecordColumnShift = 27;
 
 // The persistent gather kernel takes the jobs of up to three image planes (Y, U, V of one frame) in ONE launch:
@@ -177,12 +195,9 @@ constexpr int kMaxFramePlanes = 3;
 struct PlaneView {
   const uint8_t* src;   // (blurred) input plane
   uint8_t* dst;
-  const int2* samples;  // full records (general jobs): lane-ordered, tile-major, see below
-  const uint4* records; // compact records (staged jobs)
+  const uint4* records; // compact records of the plane's jobs
   int srcW, srcH, srcPitch;
   int dstW, dstH, dstPitch;
-  int tilesPerRow;
-  int reserved;
 };
 struct FrameGatherParams {
   PlaneView plane[kMaxFramePlanes];
@@ -190,7 +205,7 @@ struct FrameGatherParams {
   int kernelSize, numPlanes;
 };
 
-// The general (whole plane, L1) kernels and the general jobs of the frame kernel use FULL records, 8 bytes per pixel:
+// The general (whole plane, L1) kernels use FULL records, 8 bytes per pixel:
 // {col0 | column << 27, row0 << 10 | phase}, tile-major over tiles of 32 x gatherTileH(k) pixels:
 //   records[((ty * tilesPerRow + tx) * gatherTileH(k) + rowInTile) * 32 + lane]
 // (tiles that stick out of the plane are padded with zero records).  Inside a 32-pixel row segment the records are in
@@ -286,8 +301,8 @@ constexpr int kBlurMaxSmem = 96 * 1024;
 // Launchers: enqueue on `stream`, return the CUDA status of the launch.  Each counts the kernels it launches.
 // General path for a whole plane: taps through L1, every border mode (BORDER_WRAP, BORDER_TRANSPARENT), nearest.
 cudaError_t launchGather(const GatherParams& p, int numSMs, cudaStream_t stream);
-// Whole planes in one persistent kernel: `jobs` lists the jobs of every plane, sorted by kind (general, seam, class 1,
-// share, class 0).  tensorMaps: per plane kNumBoxClasses CUtensorMap (128 bytes each) describing its source with the
+// Whole planes in one persistent kernel: `jobs` lists the jobs of every plane in launch order (gather_plan.h:
+// jobLaunchRank).  tensorMaps: per plane kNumBoxClasses CUtensorMap (128 bytes each) describing its source with the
 // staging boxes of p.kernelSize, i.e. [numPlanes][kNumBoxClasses].  BORDER_WRAP only.
 // programmatic: allow the launch to overlap the tail of the previous kernel on the stream (programmatic dependent launch).
 cudaError_t launchGatherFrame(const FrameGatherParams& p, const StagedParams& jobs, const void* tensorMaps, int numSMs,

@@ -78,15 +78,15 @@ struct DevicePlan {
   int inW = 0, inH = 0, outW = 0, outH = 0, mapW = 0, mapH = 0;
   int kernelSize = 0;
   bool transparent = false, lowPass = false;
-  DeviceBuffer<int2> samples;      // full records: tile-major, lane-ordered, 8 bytes per pixel (general kernels / jobs)
-  DeviceBuffer<uint32_t> records;  // compact records of the staged jobs (kernels.cuh): 2.5 - 4 bytes per pixel
+  DeviceBuffer<int2> samples;      // full records: tile-major, lane-ordered, 8 bytes per pixel (whole-plane general kernels)
+  DeviceBuffer<uint32_t> records;  // compact records of the frame kernel's jobs (kernels.cuh): 2.5 - 4 bytes per pixel (pole caps: 8)
   int tilesPerRow = 0;
-  // gather jobs: share blocks and tiles whose source windows fit a TMA staging box, and the rest
-  DeviceBuffer<GatherJob> gatherJobs;  // every job of the plane, sorted by kind (general, seam, class 1, share, class 0)
+  // gather jobs: share blocks and tiles whose source windows fit a TMA staging box, pole-cap and border jobs
+  DeviceBuffer<GatherJob> gatherJobs;  // every job of the plane, in launch order (gather_plan.h: jobLaunchRank)
   std::vector<GatherJob> hostJobs;     // the same list on the host: merged per frame by gatherFrame()
   std::vector<int> jobNeedRows;        // per host job: the source rows [0, n) it reads (streaming host planes in)
-  int numJobs = 0, numStaged[2] = {}, numSeam = 0, numShare = 0, numFallback = 0;
-  int totalStaged() const { return numSeam + numShare + numStaged[0] + numStaged[1]; }
+  std::vector<t360::JobRect> jobRects; // per host job: the output rectangle it writes into (streaming host planes out)
+  int numJobs = 0, numStaged = 0, numBorder = 0;  // staged: jobs with a TMA box; border: jobs reading through L1
   // low-pass: register-resident strip jobs grouped by vertical half-size 1..3, and the rest (large vertical kernels),
   // for one plane size
   struct BlurSet {
@@ -366,7 +366,7 @@ class VideoFrameTransform {
 
   // ---- streaming a large host plane through the device -------------------------------------------------------
   bool pipelineEligible(const DevicePlan& plan, int inW, int inH, int outW, int outH) const {
-    return plan.totalStaged() > 0 && !plan.transparent && !plan.lowPass && inW == plan.inW && inH == plan.inH &&
+    return plan.numJobs > 0 && !plan.transparent && !plan.lowPass && inW == plan.inW && inH == plan.inH &&
            outW == plan.mapW && outH == plan.mapH && static_cast<long long>(inW) * inH >= pipelineMinBytes_ && inH >= 64;
   }
 
@@ -396,17 +396,16 @@ class VideoFrameTransform {
     for (size_t i = 0; i < plan.hostJobs.size(); ++i) {
       const int c = waveOf(plan.jobNeedRows[i]);
       byWave[c].push_back(plan.hostJobs[i]);
-      int rect[4];
-      t360::jobOutputRect(plan.hostJobs[i], plan.kernelSize, rect);
-      for (int band = rect[1] / 32; band <= (std::min(rect[3], plan.mapH) - 1) / 32; ++band) {
-        int& slot = complete[static_cast<size_t>(band) * blocks + rect[0] / blockW];
-        slot = std::max(slot, c);
-      }
+      const t360::JobRect& r = plan.jobRects[i];  // (a pole-cap job's pixels may spread over several blocks)
+      for (int band = r.y0 / 32; band <= (r.y1 - 1) / 32; ++band)
+        for (int b = r.x0 / blockW; b <= (r.x1 - 1) / blockW; ++b) {
+          int& slot = complete[static_cast<size_t>(band) * blocks + b];
+          slot = std::max(slot, c);
+        }
     }
     std::vector<GatherJob> all;
     w.waveStart.assign(chunks + 1, 0);
     for (int c = 0; c < chunks; ++c) {
-      t360::spreadGeneralJobs(byWave[c]);
       w.waveStart[c] = static_cast<int>(all.size());
       all.insert(all.end(), byWave[c].begin(), byWave[c].end());
     }
@@ -765,7 +764,7 @@ class VideoFrameTransform {
     std::lock_guard<std::mutex> lock(mu_);
     auto it = plans_.find(planIndex);
     if (it == plans_.end()) return false;
-    counts[0] = it->second.totalStaged(); counts[1] = it->second.numFallback;
+    counts[0] = it->second.numStaged; counts[1] = it->second.numBorder;
     counts[2] = it->second.blur.numStripJobs[0] + it->second.blur.numStripJobs[1] + it->second.blur.numStripJobs[2];
     counts[3] = it->second.blur.numTileJobs + it->second.blur.numDirectJobs;
     return true;
@@ -894,23 +893,23 @@ class VideoFrameTransform {
       d.tilesPerRow = g.tilesPerRow;
       d.samples.reserve(g.records.size());
       CU(cudaMemcpy(d.samples.ptr, g.records.data(), g.records.size() * sizeof(int2), cudaMemcpyHostToDevice));
-      d.numFallback = g.numGeneral;
-      d.numSeam = g.numSeam;
-      d.numShare = g.numShare;
-      for (int c = 0; c < 2; ++c) d.numStaged[c] = g.numStaged[c];
-      d.numJobs = static_cast<int>(g.jobs.size());
-      if (!g.jobs.empty()) {
-        std::vector<GatherJob> launchOrder = g.jobs;  // (hostJobs stay sorted by kind: gatherFrame() merges the planes)
-        t360::spreadGeneralJobs(launchOrder);
-        d.gatherJobs.reserve(launchOrder.size());
-        CU(cudaMemcpy(d.gatherJobs.ptr, launchOrder.data(), launchOrder.size() * sizeof(GatherJob), cudaMemcpyHostToDevice));
+      d.numStaged = g.totalStaged();
+      d.numBorder = g.numBorder;
+      d.numJobs = static_cast<int>(g.launchJobs.size());
+      if (!g.launchJobs.empty()) {
+        d.gatherJobs.reserve(g.launchJobs.size());
+        CU(cudaMemcpy(d.gatherJobs.ptr, g.launchJobs.data(), g.launchJobs.size() * sizeof(GatherJob), cudaMemcpyHostToDevice));
       }
-      if (!g.compact.empty()) {
-        d.records.reserve(g.compact.size());
-        CU(cudaMemcpy(d.records.ptr, g.compact.data(), g.compact.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+      if (!g.compact.empty() || !g.capRecords.empty()) {  // one buffer: the tiles' records, then the pole caps'
+        d.records.reserve(g.compact.size() + g.capRecords.size());
+        if (!g.compact.empty())
+          CU(cudaMemcpy(d.records.ptr, g.compact.data(), g.compact.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+        if (!g.capRecords.empty())
+          CU(cudaMemcpy(d.records.ptr + g.compact.size(), g.capRecords.data(), g.capRecords.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
       }
-      d.hostJobs = std::move(g.jobs);
-      d.jobNeedRows = std::move(g.jobNeedRows);
+      d.hostJobs = std::move(g.launchJobs);
+      d.jobNeedRows = std::move(g.launchNeedRows);
+      d.jobRects = std::move(g.launchRects);
     }
     d.lowPass = ctx_.enable_low_pass_filter != 0;
     if (d.lowPass) {
@@ -1193,11 +1192,10 @@ class VideoFrameTransform {
       src = lane.blurred.ptr;
       srcPitch = bp;
     }
-    w.view = t360::PlaneView{src, dOut, plan.samples.ptr, reinterpret_cast<const uint4*>(plan.records.ptr), inW, inH, srcPitch,
-                             outW, outH, outPitch, plan.tilesPerRow, 0};
+    w.view = t360::PlaneView{src, dOut, reinterpret_cast<const uint4*>(plan.records.ptr), inW, inH, srcPitch, outW, outH, outPitch};
     // staged tiles need the plane the plan was made for (their windows were proven in-bounds for it) and a
     // TMA-describable layout (16-byte aligned base and pitch); otherwise every tile takes the general kernel
-    w.staged = plan.totalStaged() > 0 && !plan.transparent && inW == plan.inW && inH == plan.inH;
+    w.staged = plan.numJobs > 0 && !plan.transparent && inW == plan.inW && inH == plan.inH;
     if (w.staged) w.staged = planeMaps(lane, src, inW, inH, srcPitch, plan.kernelSize, w.maps);
     return true;
   }
@@ -1222,7 +1220,7 @@ class VideoFrameTransform {
       CU(t360::launchGatherFrame(fp, jobs, w.maps, numSMs_, s));
     } else {
       const t360::PlaneView& v = w.view;
-      t360::GatherParams gp{v.src, v.srcW, v.srcH, v.srcPitch, v.dst, v.dstW, v.dstH, v.dstPitch, v.samples, v.tilesPerRow,
+      t360::GatherParams gp{v.src, v.srcW, v.srcH, v.srcPitch, v.dst, v.dstW, v.dstH, v.dstPitch, plan.samples.ptr, plan.tilesPerRow,
                             weights_[plan.kernelSize].ptr, plan.kernelSize, plan.transparent ? 1 : 0};
       CU(t360::launchGather(gp, numSMs_, s));
     }
@@ -1296,17 +1294,13 @@ class VideoFrameTransform {
     std::unique_lock<std::mutex> listLock(frameJobsMu_);
     if (f.generation != planGeneration_ || f.numPlanes != numPlanes) {
       std::vector<GatherJob> merged;
-      const int order[7] = {t360::kJobGeneral, t360::kJobSeam, t360::kJobClass1, t360::kJobShareStay, t360::kJobShare, t360::kJobClass0, t360::kJobClass0};
-      for (int step = 0; step < 7; ++step)  // (quadrant jobs last, like in the per-plane lists)
-        for (int p = 0; p < numPlanes; ++p)
-          for (GatherJob t : work[p].plan->hostJobs) {
-            const int kind = order[step];
-            if (((t.outY >> t360::kJobKindShift) & t360::kJobKindMask) != kind) continue;
-            if (kind == t360::kJobClass0 && ((t.outX & t360::kJobQuadMask) != 0) != (step == 6)) continue;
-            t.outY |= p << t360::kJobPlaneShift;
-            merged.push_back(t);
-          }
-      t360::spreadGeneralJobs(merged);
+      for (int p = 0; p < numPlanes; ++p)
+        for (GatherJob t : work[p].plan->hostJobs) {
+          t.outY |= p << t360::kJobPlaneShift;
+          merged.push_back(t);
+        }
+      std::stable_sort(merged.begin(), merged.end(),
+                       [](const GatherJob& a, const GatherJob& b) { return t360::jobLaunchRank(a) < t360::jobLaunchRank(b); });
       CU(cudaDeviceSynchronize());  // a previous frame (on any stream) may still be reading the old list
       f.tiles.reserve(merged.size());
       CU(cudaMemcpy(f.tiles.ptr, merged.data(), merged.size() * sizeof(GatherJob), cudaMemcpyHostToDevice));
@@ -1471,6 +1465,18 @@ T360_API int T360B200_hostPlanGather(T360HostPlan* plan, int info[10], const int
   if (jobs) *jobs = g.jobs.empty() ? nullptr : reinterpret_cast<const int32_t*>(g.jobs.data());
   if (records) *records = reinterpret_cast<const int32_t*>(g.records.data());
   if (compact) *compact = g.compact.empty() ? nullptr : g.compact.data();
+  return 1;
+}
+T360_API int T360B200_hostPlanPoleCaps(T360HostPlan* plan, int info[4], const int32_t** capJobs, const uint32_t** capRecords,
+                                       const int32_t** launchJobs) {
+  int gatherInfo[10];
+  if (!plan || !info || !T360B200_hostPlanGather(plan, gatherInfo, nullptr, nullptr, nullptr)) return 0;
+  const t360::GatherPlan& g = plan->gather;
+  info[0] = g.numCap; info[1] = g.numBorder; info[2] = static_cast<int>(g.capRecords.size());
+  info[3] = static_cast<int>(g.launchJobs.size());
+  if (capJobs) *capJobs = g.capJobs.empty() ? nullptr : reinterpret_cast<const int32_t*>(g.capJobs.data());
+  if (capRecords) *capRecords = g.capRecords.empty() ? nullptr : g.capRecords.data();
+  if (launchJobs) *launchJobs = g.launchJobs.empty() ? nullptr : reinterpret_cast<const int32_t*>(g.launchJobs.data());
   return 1;
 }
 T360_API int T360B200_hostPlanSegment(const T360HostPlan* plan, int i, int rect[4], int numTaps[2], const float** kx,

@@ -98,6 +98,8 @@ def load(path: os.PathLike | None = None):
     L.T360B200_hostPlanSegment.argtypes = [vp, ci, C.POINTER(ci), C.POINTER(ci), C.POINTER(vp), C.POINTER(vp)]
     L.T360B200_hostPlanGather.restype = ci
     L.T360B200_hostPlanGather.argtypes = [vp, C.POINTER(ci), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]
+    L.T360B200_hostPlanPoleCaps.restype = ci
+    L.T360B200_hostPlanPoleCaps.argtypes = [vp, C.POINTER(ci), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]
     L.T360B200_weightImage.restype = ci
     L.T360B200_weightImage.argtypes = [ci, C.POINTER(vp)]
     L.T360B200_remapTable.restype = ci
@@ -134,7 +136,7 @@ EXPORTED_SYMBOLS = [
     "VideoFrameTransform_new", "VideoFrameTransform_delete", "VideoFrameTransform_generateMapForPlane",
     "VideoFrameTransform_transformFramePlane", "T360B200_hostPlanCreate", "T360B200_hostPlanDestroy",
     "T360B200_hostPlanInfo", "T360B200_hostPlanMap", "T360B200_hostPlanSamples", "T360B200_hostPlanSegment",
-    "T360B200_hostPlanGather", "T360B200_weightImage", "T360B200_dealLanes",
+    "T360B200_hostPlanGather", "T360B200_hostPlanPoleCaps", "T360B200_weightImage", "T360B200_dealLanes",
     "T360B200_remapTable", "T360B200_transformFramePlaneAsync", "T360B200_transformFrameAsync",
     "T360B200_lowPassPlaneAsync",
     "T360B200_setPinHostPlanes", "T360B200_debugTrace", "T360B200_debugTraceRead", "T360B200_synchronize", "T360B200_stream", "T360B200_kernelLaunchCount", "T360B200_planDeviceBytes",
@@ -300,6 +302,20 @@ class HostPlan:
             compact = np.frombuffer((C.c_uint32 * info[9]).from_address(comp.value), np.uint32).copy()
         return dict(tiles_per_row=tpr, tile_rows=trows, tile_h=th, jobs=j, records=records, compact=compact,
                     counts=dict(class0=info[4], class1=info[5], seam=info[6], general=info[7], share=info[8]))
+
+    def pole_caps(self):
+        """What the frame kernel runs for the general tiles of gather_plan(), and its launch list
+        (T360B200_hostPlanPoleCaps).  Returns a dict: counts {cap, border}, jobs int32[n][4] (pole-cap and border jobs,
+        record offsets counting on after gather_plan()'s compact records), records uint32[] (their records), launch
+        int32[m][4] (the job list the kernel claims from, in launch order)."""
+        info = (C.c_int * 4)()
+        jobs, recs, launch = C.c_void_p(), C.c_void_p(), C.c_void_p()
+        if not self._lib.T360B200_hostPlanPoleCaps(self._h, info, C.byref(jobs), C.byref(recs), C.byref(launch)):
+            raise ValueError("T360B200_hostPlanPoleCaps failed")
+        n, m = info[0] + info[1], info[3]
+        as_jobs = lambda p, k: np.frombuffer((C.c_int32 * (k * 4)).from_address(p.value), np.int32).reshape(k, 4).copy() if k and p.value else np.zeros((0, 4), np.int32)
+        records = np.frombuffer((C.c_uint32 * info[2]).from_address(recs.value), np.uint32).copy() if info[2] and recs.value else np.zeros(0, np.uint32)
+        return dict(counts=dict(cap=info[0], border=info[1]), jobs=as_jobs(jobs, n), records=records, launch=as_jobs(launch, m))
 
     def segments(self):
         out = []
