@@ -74,7 +74,7 @@ int T360B200_transformFramePlaneAsync(VideoFrameTransform* transform, const uint
  * planes run side by side (chroma on internal streams); one gather launch then takes the tiles of every plane;
  * `cudaStream` observes the completion of all of it.  Arrays have numPlanes (1..3) entries: device pointers, per-plane
  * widths / heights / pitches in bytes.  Scratch planes and schedulers are per stream (see above); generateMapForPlane
- * must not run concurrently with frames in flight. */
+ * must not run concurrently with frames in flight (T360B200_reconfigure may). */
 int T360B200_transformFrameAsync(VideoFrameTransform* transform, int numPlanes, const uint8_t* const* deviceInputs,
                                  uint8_t* const* deviceOutputs, const int* inputWidths, const int* inputHeights,
                                  const int* inputPitches, const int* outputWidths, const int* outputHeights,
@@ -83,6 +83,16 @@ int T360B200_transformFrameAsync(VideoFrameTransform* transform, int numPlanes, 
 int T360B200_lowPassPlaneAsync(VideoFrameTransform* transform, const uint8_t* deviceInput, uint8_t* deviceOutput,
                                int width, int height, int inputPitch, int outputPitch,
                                int transformMatPlaneIndex, void* cudaStream);
+/* Replaces the transform's FrameTransformContext. Every plan index generated so far is re-planned for the new
+ * context with the sizes it was generated with. Returns 1 on success. 0: message on stdout, old configuration
+ * still fully in effect.
+ * Frame-exact: work enqueued before the call (any entry point, any stream) completes with the old configuration, work
+ * enqueued after it returns uses the new one.  The call may overlap frames in flight and calls on other threads: host
+ * planning runs while they continue; the call then waits for the device's work enqueued so far, swaps the plans and
+ * releases the old ones.  Any field may change as long as the caller keeps the plane sizes it generated the maps for
+ * (layouts, stereo formats and scale factors included).  Before any generateMapForPlane only the context is replaced
+ * and no CUDA call is made. */
+int T360B200_reconfigure(VideoFrameTransform* transform, const FrameTransformContext* ctx);
 /* Opt-in (also: environment T360B200_PIN_HOST_PLANES=1): page-lock pageable caller planes in place the second time
  * the same buffer is seen (cudaHostRegister), so that recycled frame-pool buffers are DMA'd at full PCIe speed.  The
  * caller must keep such buffers alive until VideoFrameTransform_delete. */

@@ -17,7 +17,10 @@
 #include <memory>
 #include <mutex>
 #include <new>
+#include <shared_mutex>
 #include <stdexcept>
+#include <string>
+#include <thread>
 #include <vector>
 
 #include "host_plan.h"
@@ -78,6 +81,7 @@ struct DevicePlan {
   int inW = 0, inH = 0, outW = 0, outH = 0, mapW = 0, mapH = 0;
   int kernelSize = 0;
   bool transparent = false, lowPass = false;
+  int stereoFormat = STEREO_FORMAT_MONO;  // input_stereo_format of the context the plan was made with (low-pass passes)
   DeviceBuffer<int2> samples;      // full records: tile-major, lane-ordered, 8 bytes per pixel (whole-plane general kernels)
   DeviceBuffer<uint32_t> records;  // compact records of the frame kernel's jobs (kernels.cuh): 2.5 - 4 bytes per pixel (pole caps: 8)
   int tilesPerRow = 0;
@@ -118,6 +122,17 @@ struct DevicePlan {
            blur.tileJobs.bytes() + blur.directJobs.bytes() + blur.taps.bytes();
   }
 };
+
+// The host-side half of a plan index (no CUDA call): the planner's result and, for interpolating plans, the gather plan.
+struct HostIndexPlan {
+  HostPlan host;
+  t360::GatherPlan gather;
+};
+bool planOnHost(const FrameTransformContext& ctx, int inW, int inH, int outW, int outH, HostIndexPlan& p) {
+  if (!t360::buildHostPlan(ctx, inW, inH, outW, outH, p.host)) return false;
+  if (p.host.kernelSize > 0) t360::buildGatherPlan(p.host, p.host.kernelSize >= 2 && !p.host.transparentBorder, p.gather);
+  return true;
+}
 
 using EncodeTiledFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                    const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -285,11 +300,13 @@ class VideoFrameTransform {
   // reference generateMapForPlane (cpp:504-576): plan on the host, upload once.
   bool generateMapForPlane(int inW, int inH, int outW, int outH, int planIndex) {
     try {
-      HostPlan host;
-      if (!t360::buildHostPlan(ctx_, inW, inH, outW, outH, host)) return false;
+      std::lock_guard<std::mutex> planLock(planMu_);
+      HostIndexPlan host;
+      if (!planOnHost(ctx_, inW, inH, outW, outH, host)) return false;
       const DeviceRestore restoreDevice = ensureDevice();
+      DevicePlan plan = upload(host, ctx_);
       std::lock_guard<std::mutex> lock(mu_);
-      plans_[planIndex] = upload(host);
+      plans_[planIndex] = std::move(plan);
       ++planGeneration_;
       return true;
     } catch (const CudaFail& f) {
@@ -297,6 +314,66 @@ class VideoFrameTransform {
                   cudaGetErrorName(f.err), cudaGetErrorString(f.err), f.what);
     } catch (const std::exception& ex) {
       std::printf("Could not generate map for plane %d. Error: %s\n", planIndex, ex.what());
+    }
+    return false;
+  }
+
+  // Replaces the context of a running transform: every plan index is re-planned for `next` with the sizes it was
+  // generated with.  Host planning (all indices at once) runs while other threads keep enqueuing frames with the old
+  // plans; the entry points are held off only while the device waits for the work enqueued so far (it reads the old
+  // plans and lists) and the plans are swapped.  On any failure the old configuration stays in effect.
+  bool reconfigure(const FrameTransformContext& next) {
+    try {
+      std::lock_guard<std::mutex> planLock(planMu_);  // (one re-plan at a time, also against generateMapForPlane)
+      struct Sizes { int index, inW, inH, outW, outH; };
+      std::vector<Sizes> sizes;
+      {
+        std::lock_guard<std::mutex> lock(mu_);
+        for (const auto& kv : plans_) sizes.push_back({kv.first, kv.second.inW, kv.second.inH, kv.second.outW, kv.second.outH});
+      }
+      if (sizes.empty()) {  // nothing planned yet: the next generateMapForPlane uses the new context (no CUDA call here)
+        std::memcpy(&ctx_, &next, sizeof(ctx_));
+        return true;
+      }
+      std::vector<HostIndexPlan> host(sizes.size());
+      std::vector<int> planned(sizes.size(), 0);
+      std::vector<std::string> errors(sizes.size());
+      auto planOne = [&](size_t i) {
+        try {
+          planned[i] = planOnHost(next, sizes[i].inW, sizes[i].inH, sizes[i].outW, sizes[i].outH, host[i]);
+        } catch (const std::exception& ex) {
+          errors[i] = ex.what();
+        }
+      };
+      std::vector<std::thread> pool;  // luma and chroma side by side (each planner is multi-threaded over rows as well)
+      for (size_t i = 1; i < sizes.size(); ++i) pool.emplace_back(planOne, i);
+      planOne(0);
+      for (std::thread& t : pool) t.join();
+      for (size_t i = 0; i < sizes.size(); ++i)
+        if (!planned[i]) {
+          std::printf("Could not reconfigure the transform. Error: no plan for index %d%s%s\n", sizes[i].index, errors[i].empty() ? "" : ": ",
+                      errors[i].c_str());
+          return false;
+        }
+      const DeviceRestore restoreDevice = ensureDevice();
+      std::map<int, DevicePlan> plans;
+      for (size_t i = 0; i < sizes.size(); ++i) plans.emplace(sizes[i].index, upload(host[i], next));
+      {
+        std::unique_lock<std::shared_mutex> config(configMu_);  // no call of an entry point is in progress from here on
+        CU(cudaDeviceSynchronize());  // everything enqueued before this call has finished with the old plans
+        std::lock_guard<std::mutex> lock(mu_);
+        plans_.swap(plans);
+        std::memcpy(&ctx_, &next, sizeof(ctx_));
+        ++planGeneration_;  // the merged job and strip lists and the wave plans are rebuilt on first use
+        for (PlaneGraph& g : planeGraphs_) cudaGraphExecDestroy(g.exec);  // (they launch the old plans' jobs)
+        planeGraphs_.clear();
+      }
+      return true;  // (`plans` now holds the old plans: released here, nothing reads them any more)
+    } catch (const CudaFail& f) {
+      std::printf("Could not reconfigure the transform. Error: CUDA %s (%s) in %s\n", cudaGetErrorName(f.err), cudaGetErrorString(f.err), f.what);
+      cudaGetLastError();
+    } catch (const std::exception& ex) {
+      std::printf("Could not reconfigure the transform. Error: %s\n", ex.what());
     }
     return false;
   }
@@ -309,6 +386,7 @@ class VideoFrameTransform {
         std::printf("Could not transform the plane %d. Error: invalid plane description\n", imagePlaneIndex);
         return false;
       }
+      std::shared_lock<std::shared_mutex> config(configMu_);
       const DeviceRestore restoreDevice = ensureDevice();
       const DevicePlan* plan = findPlan(planIndex, imagePlaneIndex);
       if (!plan) return false;
@@ -635,6 +713,7 @@ class VideoFrameTransform {
   bool transformDevice(const uint8_t* dIn, uint8_t* dOut, int inW, int inH, int inPitch, int outW, int outH,
                        int outPitch, int planIndex, cudaStream_t stream) {
     try {
+      std::shared_lock<std::shared_mutex> config(configMu_);
       const DeviceRestore restoreDevice = ensureDevice();
       const DevicePlan* plan = findPlan(planIndex, planIndex);
       if (!plan) return false;
@@ -660,6 +739,7 @@ class VideoFrameTransform {
         std::printf("Could not transform the frame. Error: %d planes (1..%d supported)\n", numPlanes, kPlaneLanes);
         return false;
       }
+      std::shared_lock<std::shared_mutex> config(configMu_);
       const DeviceRestore restoreDevice = ensureDevice();
       cudaStream_t s = stream ? stream : stream_;
       StreamSlot& slot = slotFor(s);
@@ -725,6 +805,7 @@ class VideoFrameTransform {
   bool lowPassDevice(const uint8_t* dIn, uint8_t* dOut, int w, int h, int inPitch, int outPitch, int planIndex,
                      cudaStream_t stream) {
     try {
+      std::shared_lock<std::shared_mutex> config(configMu_);
       const DeviceRestore restoreDevice = ensureDevice();
       const DevicePlan* plan = findPlan(planIndex, planIndex);
       if (!plan) return false;
@@ -881,15 +962,17 @@ class VideoFrameTransform {
     return buf.ptr;
   }
 
-  DevicePlan upload(const HostPlan& h) {
+  // The device half of a plan index, for the context `ctx` it was planned with (moves the gather plan's job lists out).
+  DevicePlan upload(HostIndexPlan& p, const FrameTransformContext& ctx) {
+    const HostPlan& h = p.host;
     DevicePlan d;
     d.inW = h.inW; d.inH = h.inH; d.outW = h.outW; d.outH = h.outH; d.mapW = h.mapW; d.mapH = h.mapH;
     d.kernelSize = h.kernelSize;
     d.transparent = h.transparentBorder;
+    d.stereoFormat = ctx.input_stereo_format;
     if (d.kernelSize > 0) {
-      deviceWeights(ctx_.interpolation_alg);
-      t360::GatherPlan g;
-      t360::buildGatherPlan(h, d.kernelSize >= 2 && !d.transparent, g);
+      deviceWeights(ctx.interpolation_alg);
+      t360::GatherPlan& g = p.gather;
       d.tilesPerRow = g.tilesPerRow;
       d.samples.reserve(g.records.size());
       CU(cudaMemcpy(d.samples.ptr, g.records.data(), g.records.size() * sizeof(int2), cudaMemcpyHostToDevice));
@@ -911,11 +994,11 @@ class VideoFrameTransform {
       d.jobNeedRows = std::move(g.launchNeedRows);
       d.jobRects = std::move(g.launchRects);
     }
-    d.lowPass = ctx_.enable_low_pass_filter != 0;
+    d.lowPass = ctx.enable_low_pass_filter != 0;
     if (d.lowPass) {
       d.segments = h.segments;
       d.planTaps = h.taps;
-      buildBlurJobs(d.segments, d.planTaps, h.inW, h.inH, d.blur);
+      buildBlurJobs(d.segments, d.planTaps, h.inW, h.inH, d.stereoFormat, d.blur);
     }
     d.resizeNeeded = h.resize.needed;
     if (d.resizeNeeded) resizeFor(d, d.outW, d.outH);
@@ -968,14 +1051,14 @@ class VideoFrameTransform {
   // Tiles of the plan, applied once (mono) or to both halves of a stereo frame (reference cpp:630-691), cut
   // into CTA-sized jobs.  Segments that do not fit the plane are dropped, like the reference's caught cv::Exception.
   void buildBlurJobs(const std::vector<t360::LowPassSegment>& segments, const std::vector<float>& planTaps, int planeW, int planeH,
-                     DevicePlan::BlurSet& d) {
+                     int stereoFormat, DevicePlan::BlurSet& d) {
     struct { const std::vector<t360::LowPassSegment>& segments; const std::vector<float>& taps; int inW, inH; } h{segments, planTaps, planeW, planeH};
     std::vector<BlurJob> tiles, direct;
     std::vector<StripJob> strips[t360::kStripMaxHy];
     std::vector<float> taps = h.taps;  // original taps first (offsets of the plan stay valid), padded copies appended
     int offX[2] = {0, 0}, offY[2] = {0, 0}, passes = 1;
-    if (ctx_.input_stereo_format == STEREO_FORMAT_LR) { passes = 2; offX[1] = static_cast<int>(0.5 * h.inW); }
-    else if (ctx_.input_stereo_format == STEREO_FORMAT_TB) { passes = 2; offY[1] = static_cast<int>(0.5 * h.inH); }
+    if (stereoFormat == STEREO_FORMAT_LR) { passes = 2; offX[1] = static_cast<int>(0.5 * h.inW); }
+    else if (stereoFormat == STEREO_FORMAT_TB) { passes = 2; offY[1] = static_cast<int>(0.5 * h.inH); }
     std::vector<uint8_t> covered(static_cast<size_t>(h.inW) * h.inH, 0);
     int tileSmem = 0;
     // a warp-job covers 256 columns x `rows` rows; keep the grid at several thousand warps even for small planes
@@ -1099,7 +1182,7 @@ class VideoFrameTransform {
     auto it = plan.otherBlurs.find({w, h});
     if (it != plan.otherBlurs.end()) return it->second;
     DevicePlan::BlurSet& set = plan.otherBlurs[{w, h}];
-    buildBlurJobs(plan.segments, plan.planTaps, w, h, set);
+    buildBlurJobs(plan.segments, plan.planTaps, w, h, plan.stereoFormat, set);
     return set;
   }
 
@@ -1345,6 +1428,11 @@ class VideoFrameTransform {
   }
 
   FrameTransformContext ctx_;
+  // Every entry point that enqueues work holds configMu_ shared for as long as it uses a plan; reconfigure() swaps the
+  // plans under it exclusively.  planMu_ serialises planning (generateMapForPlane, reconfigure) and guards ctx_.  Lock
+  // order: planMu_, configMu_, hostCallMu_, then the others.
+  std::shared_mutex configMu_;
+  std::mutex planMu_;
   std::mutex mu_;
   std::mutex lazyMu_;  // per-size tables made on first use (resizeFor, blurFor)
   std::map<int, DevicePlan> plans_;
@@ -1534,6 +1622,10 @@ T360_API int T360B200_lowPassPlaneAsync(VideoFrameTransform* t, const uint8_t* d
     std::printf("Could not filter plane %d. Error: %s\n", planIndex, ex.what());
     return 0;
   }
+}
+T360_API int T360B200_reconfigure(VideoFrameTransform* t, const FrameTransformContext* ctx) {
+  if (!t || !ctx) return 0;
+  return t->reconfigure(*ctx);
 }
 T360_API void T360B200_setPinHostPlanes(VideoFrameTransform* t, int enable) { if (t) t->setPinHostPlanes(enable != 0); }
 T360_API void T360B200_debugTrace(VideoFrameTransform* t, int enable) { if (t) t->enableTrace(enable != 0); }

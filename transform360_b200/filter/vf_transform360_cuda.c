@@ -13,7 +13,8 @@
  * Options carry the names, defaults and ranges of the reference filter's table (vf:407-987) and the output size follows
  * its config_output (vf:167-304); they write straight into the FrameTransformContext handed to VideoFrameTransform_new.
  * Differences, on purpose: "size=WxH" is honoured (the reference accepts and then ignores it, vf:306-326); "sync=0" lets
- * the frame travel downstream without a stream synchronisation (consumers on the same stream need none).
+ * the frame travel downstream without a stream synchronisation (consumers on the same stream need none).  The view and
+ * quality options are also runtime commands (sendcmd, zmq; see t360_process_command).
  * To build inside an ffmpeg tree: copy to libavfilter/, add `extern const AVFilter ff_vf_transform360_cuda;` to
  * allfilters.c and `OBJS-$(CONFIG_TRANSFORM360_CUDA_FILTER) += vf_transform360_cuda.o` to the Makefile, link
  * -lTransform360 (INTEGRATION.md).
@@ -251,12 +252,57 @@ done:
   return ff_filter_frame(outlink, out);
 }
 
+/* Runtime commands (sendcmd, zmq): the view and quality options below are marked AV_OPT_FLAG_RUNTIME_PARAM.  Before the
+ * first frame a command only updates the parameters; after it the running transform is re-planned for them
+ * (T360B200_reconfigure: frames filtered before the command keep the old view, every later frame has the new one).
+ * Options that could change the output link's size or format (size, cube edge, layouts, stereo formats, scale factors)
+ * are refused with ENOSYS, invalid values with EINVAL; a refused command leaves every parameter as it was.
+ * This needs AV_OPT_FLAG_RUNTIME_PARAM and ff_filter_process_command (FFmpeg 4.2 and later).  A libavfilter without
+ * runtime options builds the filter without commands: the options are then fixed at init, as in the reference filter. */
+#ifdef AV_OPT_FLAG_RUNTIME_PARAM
+#define T360_COMMANDS 1
+#define VFR (AV_OPT_FLAG_VIDEO_PARAM | AV_OPT_FLAG_FILTERING_PARAM | AV_OPT_FLAG_RUNTIME_PARAM)
+#else
+#define T360_COMMANDS 0
+#define VFR (AV_OPT_FLAG_VIDEO_PARAM | AV_OPT_FLAG_FILTERING_PARAM)
+#endif
+
+#if T360_COMMANDS
+static int t360_process_command(AVFilterContext* ctx, const char* cmd, const char* arg, char* res, int res_len, int flags) {
+  T360CudaContext* s = ctx->priv;
+  const FrameTransformContext before = s->params;
+  int rc = ff_filter_process_command(ctx, cmd, arg, res, res_len, flags);
+  if (rc == AVERROR(ENOSYS)) return rc;
+  if (rc < 0) {
+    s->params = before;
+    av_log(ctx, AV_LOG_ERROR, "invalid value '%s' for %s\n", arg, cmd);
+    return AVERROR(EINVAL);
+  }
+  if (!s->maps_ready) return 0;
+  CudaFunctions* cu = s->cuda->internal->cuda_dl;
+  CUcontext popped;
+  if (cu->cuCtxPushCurrent(s->cuda->cuda_ctx)) {
+    s->params = before;
+    return AVERROR_EXTERNAL;
+  }
+  rc = T360B200_reconfigure(s->transform, &s->params) ? 0 : AVERROR(EINVAL);
+  cu->cuCtxPopCurrent(&popped);
+  if (rc) {
+    s->params = before;
+    av_log(ctx, AV_LOG_ERROR, "the transform refused %s=%s; the previous configuration stays in effect\n", cmd, arg);
+  }
+  return rc;
+}
+#endif
+
 #define FIELD(f) offsetof(T360CudaContext, f)
 #define PARAM(f) offsetof(T360CudaContext, params.f)
 #define VF (AV_OPT_FLAG_VIDEO_PARAM | AV_OPT_FLAG_FILTERING_PARAM)
 #define TEXT(name, help, off) {name, help, off, AV_OPT_TYPE_STRING, {.str = NULL}, 0, 0, VF, NULL}
 #define INT(name, help, off, def, lo, hi, unit) {name, help, off, AV_OPT_TYPE_INT, {.i64 = def}, lo, hi, VF, unit}
 #define REAL(name, help, off, def, lo, hi) {name, help, off, AV_OPT_TYPE_FLOAT, {.dbl = def}, lo, hi, VF, NULL}
+#define RUNTIME_INT(name, help, off, def, lo, hi, unit) {name, help, off, AV_OPT_TYPE_INT, {.i64 = def}, lo, hi, VFR, unit}
+#define RUNTIME_REAL(name, help, off, def, lo, hi) {name, help, off, AV_OPT_TYPE_FLOAT, {.dbl = def}, lo, hi, VFR, NULL}
 #define NAMED(name, value, unit) {name, NULL, 0, AV_OPT_TYPE_CONST, {.i64 = value}, 0, 0, VF, unit}
 #define NAMED2(upper, lower, value, unit) NAMED(upper, value, unit), NAMED(lower, value, unit)
 
@@ -281,32 +327,33 @@ static const AVOption transform360_cuda_options[] = {
     NAMED2("EQUIRECT", "equirect", LAYOUT_EQUIRECT, "layout"), NAMED2("FLAT_FIXED", "flat_fixed", LAYOUT_FLAT_FIXED, "layout"),
     NAMED2("BARREL", "barrel", LAYOUT_BARREL, "layout"), NAMED2("BARREL_SPLIT", "barrel_split", LAYOUT_BARREL_SPLIT, "layout"),
     NAMED2("EAC_32", "eac_32", LAYOUT_EAC_32, "layout"),
-    INT("vflip", "flip the second eye of a TB output", PARAM(vflip), 0, 0, 1, "flag"), NAMED("false", 0, "flag"), NAMED("true", 1, "flag"),
-    INT("is_horizontal_offset", "off-centre shift along the view axis only", PARAM(is_horizontal_offset), 0, 0, 1, NULL),
-    REAL("input_expand_coef", "face expansion of a cubemap input", PARAM(input_expand_coef), 1.01f, 0, 10),
-    REAL("expand_coef", "face expansion of the output", PARAM(expand_coef), 1.01f, 0, 10),
-    REAL("yaw", "degrees", PARAM(fixed_yaw), 0, -360, 360), REAL("pitch", "degrees", PARAM(fixed_pitch), 0, -180, 180),
-    REAL("roll", "degrees", PARAM(fixed_roll), 0, -180, 180),
-    REAL("hfov", "flat_fixed: horizontal field of view, degrees", PARAM(fixed_hfov), 120, -360, 360),
-    REAL("vfov", "flat_fixed: vertical field of view, degrees", PARAM(fixed_vfov), 110, -180, 180),
-    REAL("cube_offcenter_x", "off-centre projection", PARAM(fixed_cube_offcenter_x), 0, -1, 1),
-    REAL("cube_offcenter_y", "off-centre projection", PARAM(fixed_cube_offcenter_y), 0, -1, 1),
-    REAL("cube_offcenter_z", "off-centre projection", PARAM(fixed_cube_offcenter_z), 0, -1, 1),
-    /* sampling and the segmented low-pass (vf:721-986) */
-    INT("interpolation_alg", "nearest, linear, cubic or lanczos4", PARAM(interpolation_alg), CUBIC, 0, 4, "interp"),
+    /* the view: runtime commands too */
+    RUNTIME_INT("vflip", "flip the second eye of a TB output", PARAM(vflip), 0, 0, 1, "flag"), NAMED("false", 0, "flag"), NAMED("true", 1, "flag"),
+    RUNTIME_INT("is_horizontal_offset", "off-centre shift along the view axis only", PARAM(is_horizontal_offset), 0, 0, 1, NULL),
+    RUNTIME_REAL("input_expand_coef", "face expansion of a cubemap input", PARAM(input_expand_coef), 1.01f, 0, 10),
+    RUNTIME_REAL("expand_coef", "face expansion of the output", PARAM(expand_coef), 1.01f, 0, 10),
+    RUNTIME_REAL("yaw", "degrees", PARAM(fixed_yaw), 0, -360, 360), RUNTIME_REAL("pitch", "degrees", PARAM(fixed_pitch), 0, -180, 180),
+    RUNTIME_REAL("roll", "degrees", PARAM(fixed_roll), 0, -180, 180),
+    RUNTIME_REAL("hfov", "flat_fixed: horizontal field of view, degrees", PARAM(fixed_hfov), 120, -360, 360),
+    RUNTIME_REAL("vfov", "flat_fixed: vertical field of view, degrees", PARAM(fixed_vfov), 110, -180, 180),
+    RUNTIME_REAL("cube_offcenter_x", "off-centre projection", PARAM(fixed_cube_offcenter_x), 0, -1, 1),
+    RUNTIME_REAL("cube_offcenter_y", "off-centre projection", PARAM(fixed_cube_offcenter_y), 0, -1, 1),
+    RUNTIME_REAL("cube_offcenter_z", "off-centre projection", PARAM(fixed_cube_offcenter_z), 0, -1, 1),
+    /* sampling and the segmented low-pass (vf:721-986); runtime commands except the scale factors (they size the render) */
+    RUNTIME_INT("interpolation_alg", "nearest, linear, cubic or lanczos4", PARAM(interpolation_alg), CUBIC, 0, 4, "interp"),
     NAMED2("NEAREST", "nearest", NEAREST, "interp"), NAMED2("LINEAR", "linear", LINEAR, "interp"),
     NAMED2("CUBIC", "cubic", CUBIC, "interp"), NAMED2("LANCZOS4", "lanczos4", LANCZOS4, "interp"),
     REAL("width_scale_factor", "render at this multiple of the width, then area-resize", PARAM(width_scale_factor), 1, 0, 10),
     REAL("height_scale_factor", "render at this multiple of the height, then area-resize", PARAM(height_scale_factor), 1, 0, 10),
-    INT("enable_low_pass_filter", "anti-alias the input per segment", PARAM(enable_low_pass_filter), 1, 0, 1, NULL),
+    RUNTIME_INT("enable_low_pass_filter", "anti-alias the input per segment", PARAM(enable_low_pass_filter), 1, 0, 1, NULL),
     INT("enable_multi_threading", "accepted; the GPU takes all segments at once", PARAM(enable_multi_threading), 1, 0, 1, NULL),
-    INT("num_vertical_segments", "low-pass bands top to bottom", PARAM(num_vertical_segments), 5, 2, 500, NULL),
-    INT("num_horizontal_segments", "low-pass bands left to right", PARAM(num_horizontal_segments), 1, 1, 500, NULL),
-    REAL("kernel_height_scale_factor", "vertical kernel size factor", PARAM(kernel_height_scale_factor), 1, 0.1, 100),
-    REAL("min_kernel_half_height", "lower clamp of the vertical kernel", PARAM(min_kernel_half_height), 1, 0.5, 200),
-    REAL("max_kernel_half_height", "upper clamp of the vertical kernel", PARAM(max_kernel_half_height), 10000, 0.5, 100000),
-    INT("adjust_kernel", "scale the kernel with the off-centre magnification", PARAM(adjust_kernel), 1, 0, 1, NULL),
-    REAL("kernel_adjust_factor", "factor of that adjustment", PARAM(kernel_adjust_factor), 1, 0.1, 100),
+    RUNTIME_INT("num_vertical_segments", "low-pass bands top to bottom", PARAM(num_vertical_segments), 5, 2, 500, NULL),
+    RUNTIME_INT("num_horizontal_segments", "low-pass bands left to right", PARAM(num_horizontal_segments), 1, 1, 500, NULL),
+    RUNTIME_REAL("kernel_height_scale_factor", "vertical kernel size factor", PARAM(kernel_height_scale_factor), 1, 0.1, 100),
+    RUNTIME_REAL("min_kernel_half_height", "lower clamp of the vertical kernel", PARAM(min_kernel_half_height), 1, 0.5, 200),
+    RUNTIME_REAL("max_kernel_half_height", "upper clamp of the vertical kernel", PARAM(max_kernel_half_height), 10000, 0.5, 100000),
+    RUNTIME_INT("adjust_kernel", "scale the kernel with the off-centre magnification", PARAM(adjust_kernel), 1, 0, 1, NULL),
+    RUNTIME_REAL("kernel_adjust_factor", "factor of that adjustment", PARAM(kernel_adjust_factor), 1, 0.1, 100),
     /* this filter only */
     INT("sync", "drain the stream before the frame travels on", FIELD(sync), 1, 0, 1, NULL),
     {NULL}};
@@ -332,5 +379,8 @@ AVFilter ff_vf_transform360_cuda = {
     .priv_class = &transform360_cuda_class,
     .inputs = t360_cuda_inputs,
     .outputs = t360_cuda_outputs,
+#if T360_COMMANDS
+    .process_command = t360_process_command,
+#endif
     .flags_internal = FF_FILTER_FLAG_HWFRAME_AWARE,
 };

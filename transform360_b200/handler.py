@@ -110,6 +110,8 @@ def load(path: os.PathLike | None = None):
     L.T360B200_transformFrameAsync.argtypes = [vp, ci, vp, vp] + [vp] * 6 + [vp]
     L.T360B200_lowPassPlaneAsync.restype = ci
     L.T360B200_lowPassPlaneAsync.argtypes = [vp, vp, vp] + [ci] * 5 + [vp]
+    L.T360B200_reconfigure.restype = ci
+    L.T360B200_reconfigure.argtypes = [vp, C.POINTER(FrameTransformContext)]
     L.T360B200_setPinHostPlanes.restype = None
     L.T360B200_setPinHostPlanes.argtypes = [vp, ci]
     L.T360B200_debugTrace.restype = None
@@ -138,7 +140,7 @@ EXPORTED_SYMBOLS = [
     "T360B200_hostPlanInfo", "T360B200_hostPlanMap", "T360B200_hostPlanSamples", "T360B200_hostPlanSegment",
     "T360B200_hostPlanGather", "T360B200_hostPlanPoleCaps", "T360B200_weightImage", "T360B200_dealLanes",
     "T360B200_remapTable", "T360B200_transformFramePlaneAsync", "T360B200_transformFrameAsync",
-    "T360B200_lowPassPlaneAsync",
+    "T360B200_lowPassPlaneAsync", "T360B200_reconfigure",
     "T360B200_setPinHostPlanes", "T360B200_debugTrace", "T360B200_debugTraceRead", "T360B200_synchronize", "T360B200_stream", "T360B200_kernelLaunchCount", "T360B200_planDeviceBytes",
     "T360B200_planTileCounts", "T360B200_deviceCount", "T360B200_version",
 ]
@@ -220,6 +222,14 @@ class VideoFrameTransform:
     def low_pass_async(self, d_in: int, d_out: int, w, h, in_pitch, out_pitch, plan_index, stream: int = 0) -> bool:
         return bool(self._lib.T360B200_lowPassPlaneAsync(self._h, d_in, d_out, w, h, in_pitch, out_pitch, plan_index,
                                                          stream))
+
+    def reconfigure(self, ctx: FrameTransformContext) -> None:
+        """Replaces the context of the running transform (T360B200_reconfigure): frames enqueued before the call use the
+        old one, frames enqueued after it the new one; every generated plan index keeps its sizes.  Raises on refusal,
+        which leaves the old configuration in effect."""
+        if not self._lib.T360B200_reconfigure(self._h, C.byref(ctx)):
+            raise RuntimeError("T360B200_reconfigure returned 0 (message on stdout); the old configuration is still in effect")
+        self.ctx = ctx
 
     def set_pin_host_planes(self, enable: bool) -> None:
         self._lib.T360B200_setPinHostPlanes(self._h, 1 if enable else 0)
