@@ -93,6 +93,29 @@ int T360B200_lowPassPlaneAsync(VideoFrameTransform* transform, const uint8_t* de
  * (layouts, stereo formats and scale factors included).  Before any generateMapForPlane only the context is replaced
  * and no CUDA call is made. */
 int T360B200_reconfigure(VideoFrameTransform* transform, const FrameTransformContext* ctx);
+/* A FLAT_FIXED view, in degrees, as the context's fixed_yaw, fixed_pitch, fixed_hfov and fixed_vfov. */
+typedef struct T360View {
+  float yaw, pitch, hfov, vfov;
+} T360View;
+/* One frame of a FLAT_FIXED transform with its own view, without re-planning: the arguments and the asynchronous contract
+ * of T360B200_transformFrameAsync, plus `view`.  The frame equals, bit for bit, what a fresh transform would give for the
+ * transform's current context with fixed_yaw, fixed_pitch, fixed_hfov and fixed_vfov replaced by *view (low-pass and the
+ * INTER_AREA resize for scale factors != 1 included); the transform's context is not changed.  The gather computes the
+ * sampling positions from the view in one launch for all planes; a view-dependent low-pass is re-planned on the host and
+ * its lists are uploaded in stream order from page-locked memory (skipped when they equal the previous frame's on that
+ * stream).  The call never synchronises the device, so views may change every frame.  Like every entry point it is
+ * frame-exact against T360B200_reconfigure.  Returns 1 if everything was enqueued; 0 with a message on stdout for an
+ * output_layout other than FLAT_FIXED, a non-finite view, a plan index that was never generated, or an input plane of
+ * another size than its map was generated for. */
+int T360B200_transformFrameViewAsync(VideoFrameTransform* transform, const T360View* view, int numPlanes,
+                                     const uint8_t* const* deviceInputs, uint8_t* const* deviceOutputs, const int* inputWidths,
+                                     const int* inputHeights, const int* inputPitches, const int* outputWidths,
+                                     const int* outputHeights, const int* outputPitches, void* cudaStream);
+/* Host only, no CUDA: the sampling records the per-view kernel computes for one plane of a FLAT_FIXED context with the view
+ * substituted, int32 [mapHeight][mapWidth][2] (map = scaled output size) in the format of T360B200_hostPlanSamples.
+ * Returns 1 on success; 0 (message on stdout) for another layout, a non-finite view or invalid sizes. */
+int T360B200_viewSamples(const FrameTransformContext* ctx, const T360View* view, int inputWidth, int inputHeight,
+                         int outputWidth, int outputHeight, int32_t* samples);
 /* Opt-in (also: environment T360B200_PIN_HOST_PLANES=1): page-lock pageable caller planes in place the second time
  * the same buffer is seen (cudaHostRegister), so that recycled frame-pool buffers are DMA'd at full PCIe speed.  The
  * caller must keep such buffers alive until VideoFrameTransform_delete. */

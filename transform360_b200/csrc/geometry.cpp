@@ -20,6 +20,7 @@
 #include <thread>
 #include <vector>
 
+#include "flat_view.h"
 #include "host_plan.h"
 
 namespace t360 {
@@ -104,42 +105,25 @@ class Projector {
       return;
     }
     // second eye lives in the other half of a stacked / side-by-side input (cpp:1278-1300)
-    if (c_.input_stereo_format == STEREO_FORMAT_TB) {
-      *v = secondEye ? *v * 0.5f + 0.5f : *v * 0.5f;
-    } else if (c_.input_stereo_format == STEREO_FORMAT_LR) {
-      *u = secondEye ? *u * 0.5f + 0.5f : *u * 0.5f;
-    }
+    if (c_.input_stereo_format == STEREO_FORMAT_TB) *v = packEye(*v, secondEye);
+    else if (c_.input_stereo_format == STEREO_FORMAT_LR) *u = packEye(*u, secondEye);
   }
 
  private:
   // cpp:903-931: a stereo OUTPUT holds two complete projections; fold to one and remember which.
   bool splitOutputEyes(float& x, float& y) const {
     if (c_.input_stereo_format == STEREO_FORMAT_MONO) return false;
-    if (c_.output_stereo_format == STEREO_FORMAT_LR) {
-      if (x > 0.5f) { x = (x - 0.5f) / 0.5f; return true; }
-      x = x / 0.5f;
-    } else if (c_.output_stereo_format == STEREO_FORMAT_TB) {
-      if (y > 0.5f) {
-        y = (y - 0.5f) / 0.5f;
-        if (c_.vflip) y = 1.0f - y;
-        return true;
-      }
-      y = y / 0.5f;
-    }
+    if (c_.output_stereo_format == STEREO_FORMAT_LR) return splitEye(x, false);
+    if (c_.output_stereo_format == STEREO_FORMAT_TB) return splitEye(y, c_.vflip != 0);
     return false;
   }
 
-  // cpp:1265-1271
+  // cpp:1265-1271, folded over a pole / wrapped around the seam (cpp:101-123): flat_view.h, shared with the per-view kernel
   void flatWindow(float x, float y, float* u, float* v) const {
-    float lon = ((x - 0.5f) * c_.fixed_hfov + c_.fixed_yaw) / 360.0f + 0.5f;
-    float lat = ((y - 0.5f) * c_.fixed_vfov - c_.fixed_pitch) / 180.0f + 0.5f;
-    // reflect over a pole / wrap around the seam (cpp:101-123)
-    if (lat >= 1.0f) { lat = 2.0f - lat; lon += 0.5f; }
-    else if (lat < 0.0f) { lat = -lat; lon += 0.5f; }
-    if (lon >= 1.0f) lon -= static_cast<float>(static_cast<int>(lon));
-    else if (lon < 0.0f) lon += static_cast<float>(static_cast<int>(-lon) + 1);
-    *u = lon;
-    *v = lat;
+    const FlatView view{c_.fixed_yaw, c_.fixed_pitch, c_.fixed_hfov, c_.fixed_vfov};
+    bool fold;
+    *v = flatLat(view, y, &fold);
+    *u = flatLon(view, x, fold);
   }
 
   static Vec3 onSphere(float yaw, float pitch) {  // cpp:1095-1101 (float trig)
@@ -315,14 +299,14 @@ bool buildWarpMap(HostPlan& plan) {
   float* out = plan.map.data();
   auto rows = [&](int r0, int r1) {
     for (int i = r0; i < r1; ++i) {
-      const float y = (i + 0.5f) / H;  // cpp:537
+      const float y = pixelCentre(i, H);  // cpp:537
       float* row = out + static_cast<size_t>(i) * W * 2;
       for (int j = 0; j < W; ++j) {
-        const float x = (j + 0.5f) / W;  // cpp:538
+        const float x = pixelCentre(j, W);  // cpp:538
         float u, v;
         proj.project(x, y, &u, &v);
-        row[2 * j] = u * inW - 0.5f;  // pixel centres sit at integers for the sampler (cpp:544-545)
-        row[2 * j + 1] = v * inH - 0.5f;
+        row[2 * j] = toPixel(u, inW);  // pixel centres sit at integers for the sampler (cpp:544-545)
+        row[2 * j + 1] = toPixel(v, inH);
       }
     }
   };

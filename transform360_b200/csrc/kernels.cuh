@@ -5,6 +5,8 @@
 
 #include <cstdint>
 
+#include "flat_view.h"
+
 namespace t360 {
 
 // One gather launch: dst[y][x] = interpolate(src, samples[y][x]) for a whole plane.
@@ -315,6 +317,29 @@ cudaError_t launchBlur(const BlurParams& p, cudaStream_t stream);        // shar
 cudaError_t launchBlurDirect(const BlurParams& p, cudaStream_t stream);  // any kernel size, slow
 unsigned long long kernelLaunchCount();
 void countKernelLaunches(long long n);  // kernels launched through a replayed CUDA graph
+
+// ---- the per-view gather (view_gather.cu) ---------------------------------------------------------------------------
+// FLAT_FIXED frames whose view (yaw, pitch, hfov, vfov) is a launch parameter: the kernel computes every sampling record
+// itself (flat_view.h), so it needs no sampling plan.  One launch gathers every plane of the frame; BORDER_WRAP only.
+struct ViewPlane {
+  const uint8_t* src;  // (blurred) input plane, geometry.inW x geometry.inH
+  uint8_t* dst;        // render target, geometry.mapW x geometry.mapH
+  int srcPitch, dstPitch;
+  FlatGeometry geometry;
+  int tilesX, firstTile;  // filled by launchViewGather
+};
+struct ViewGatherParams {
+  ViewPlane plane[kMaxFramePlanes];
+  int numPlanes;
+  FlatView view;
+  const int16_t* weights;  // device copy of the [1024][k][k] table (nullptr for nearest)
+  int kernelSize;
+};
+// a CTA takes tiles of 32 output columns x viewTileRows(k) rows; a thread owns one column of a tile and walks down
+// kViewRowsPerThread of its rows
+constexpr int kViewRowsPerThread = 8;
+__host__ __device__ constexpr int viewTileRows(int k) { return gatherThreads(k) / 32 * kViewRowsPerThread; }
+cudaError_t launchViewGather(ViewGatherParams p, int numSMs, cudaStream_t stream);
 
 // bytes of dynamic shared memory a blur tile of (w x h) with the given tap counts needs
 inline int blurTileSmem(int w, int h, int nkx, int nky) {

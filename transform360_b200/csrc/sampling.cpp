@@ -17,6 +17,7 @@
 #include <thread>
 #include <vector>
 
+#include "flat_view.h"
 #include "host_plan.h"
 
 namespace t360 {
@@ -24,16 +25,7 @@ namespace {
 
 constexpr int kFracBits = 5, kPhases1D = 1 << kFracBits, kPhases2D = kPhases1D * kPhases1D;
 constexpr int kWeightOne = 1 << 15;
-
-// cvRound(float) as OpenCV computes it on x86 (cvtss2si, also in its SIMD paths): round half to even in the default FP
-// environment, and INT_MIN ("integer indefinite") for NaN and for values outside the int range.  It matters: an
-// off-centre projection with is_horizontal_offset divides by zero at the poles (reference cpp:1203-1206), the map
-// holds NaN there, and cv::remap samples column / row sat16(INT_MIN >> 5) = -32768 under BORDER_WRAP.
-inline int roundHalfEven(float v) {
-  if (!(v >= -2147483648.0f && v < 2147483648.0f)) return INT32_MIN;
-  return static_cast<int>(std::lrintf(v));
-}
-inline int clampToShort(int v) { return v < -32768 ? -32768 : (v > 32767 ? 32767 : v); }
+// (roundHalfEven, cvRound as OpenCV computes it on x86, and clampToShort: flat_view.h)
 
 // 1-D interpolation kernels at offset t in [0,1): taps for positions -(k/2-1) .. k/2
 void taps1D(int k, float t, float* w) {
@@ -132,18 +124,11 @@ void quantizeWarpMap(HostPlan& plan) {
   const size_t chunk = (n + nt - 1) / nt;
   auto range = [&plan, m, k](size_t begin, size_t end) {
   for (size_t i = begin; i < end; ++i) {
-    const float fx = m[2 * i], fy = m[2 * i + 1];
-    SamplePoint s;
-    if (k == 1) {
-      s.col0 = clampToShort(roundHalfEven(fx));
-      s.rowPhase = clampToShort(roundHalfEven(fy)) * 1024;
-    } else {
-      const int X = roundHalfEven(fx * kPhases1D), Y = roundHalfEven(fy * kPhases1D);
-      const int phase = (Y & (kPhases1D - 1)) * kPhases1D + (X & (kPhases1D - 1));
-      s.col0 = clampToShort(X >> kFracBits) - (k / 2 - 1);
-      s.rowPhase = (clampToShort(Y >> kFracBits) - (k / 2 - 1)) * 1024 + phase;
-    }
-    plan.samples[i] = s;
+    // per axis (flat_view.h, shared with the per-view kernel): sat16(round(f * 32) >> 5) - (k/2 - 1) and the 1/32 phase
+    int col0, fracX, row0, fracY;
+    quantizeAxis(m[2 * i], k, &col0, &fracX);
+    quantizeAxis(m[2 * i + 1], k, &row0, &fracY);
+    plan.samples[i] = SamplePoint{col0, row0 * 1024 + fracY * kPhases1D + fracX};
   }
   };
   std::vector<std::thread> pool;

@@ -10,6 +10,7 @@
 
 #include <algorithm>
 #include <climits>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -224,6 +225,45 @@ struct WavePlan {
   std::vector<std::vector<Rect>> rects;
 };
 
+// The low-pass job lists of one plane size on the host (VideoFrameTransform::buildBlurLists).
+struct BlurLists {
+  std::vector<StripJob> strips[t360::kStripMaxHy];
+  std::vector<BlurJob> tiles, direct;
+  std::vector<float> taps;
+  std::vector<int> tapSource;  // per entry of taps: 1 + the index of the plan's tap it copies, 0 for a padding zero
+  int tileSmem = 0;
+};
+
+// The per-view low-pass lists of a stream slot's previous frame and what they were made from.  The jobs (rectangles, tap
+// counts and offsets) depend on the view only through the segments' tap counts and on which neighbouring segments carry
+// identical taps; when those agree with the previous frame's, the jobs are reused and only the taps are refilled.
+struct ViewBlurCache {
+  std::vector<long long> key;
+  bool merged = false;
+  std::vector<uint8_t> jobs;
+  std::vector<int> tapCodes;  // per float of the tap image: plan index << 28 | (1 + plan tap), 0 for a zero
+  size_t stripAt[2][t360::kStripMaxHy] = {}, tileAt[2] = {}, directAt[2] = {}, tapAt[2] = {};
+  int numStrips[2][t360::kStripMaxHy] = {}, numTiles[2] = {}, numDirect[2] = {}, tileSmem[2] = {};
+};
+
+// Page-locked staging of lists that change from frame to frame (the per-view low-pass jobs and taps): a few entries, each
+// a page-locked host buffer and a device buffer, reused round robin.  An entry is refilled only after the frame that last
+// read it has finished on the device (its event), and a frame whose lists equal the previous frame's reuses that entry
+// without any copy.  Device memory stays bounded: kEntries buffers of the largest list seen.
+struct UploadRing {
+  static constexpr int kEntries = 3;
+  struct Entry {
+    uint8_t* host = nullptr;    // page-locked
+    uint8_t* device = nullptr;  // stream-ordered allocation on the slot's stream
+    size_t capacity = 0;
+    cudaEvent_t released = nullptr;  // recorded after the last frame that reads `device`
+    bool inFlight = false;
+  };
+  Entry entries[kEntries];
+  int last = -1;                    // the entry that holds lastContent
+  std::vector<uint8_t> lastContent;
+};
+
 // Everything asynchronous work on ONE caller stream shares: the lanes (scratch planes, side streams, job schedulers) and
 // the scheduler of the whole-frame launch.  Work on the same stream is ordered, so one set per stream is enough; callers
 // that enqueue on several streams at once get a set per stream instead of racing for one.
@@ -231,6 +271,8 @@ struct StreamSlot {
   PlaneLane lanes[kPlaneLanes];
   DeviceBuffer<int> frameClaim;
   cudaEvent_t fork = nullptr;
+  UploadRing viewJobs, viewTaps;  // the per-view low-pass lists (VideoFrameTransform::transformFrameView)
+  ViewBlurCache viewBlur;
 };
 
 // The strip jobs of all planes of a frame, by vertical half-size, with one merged tap buffer (rebuilt when a map is).
@@ -279,6 +321,13 @@ class VideoFrameTransform {
         }
         kv.second->frameClaim.release();
         if (kv.second->fork) cudaEventDestroy(kv.second->fork);
+        for (UploadRing* ring : {&kv.second->viewJobs, &kv.second->viewTaps})
+          for (UploadRing::Entry& e : ring->entries) {
+            if (e.released) cudaEventSynchronize(e.released);
+            if (e.device) cudaFree(e.device);
+            if (e.host) cudaFreeHost(e.host);
+            if (e.released) cudaEventDestroy(e.released);
+          }
       }
       frameJobs_.tiles.release();
       for (auto& b : frameBlur_.jobs) b.release();
@@ -332,6 +381,7 @@ class VideoFrameTransform {
         for (const auto& kv : plans_) sizes.push_back({kv.first, kv.second.inW, kv.second.inH, kv.second.outW, kv.second.outH});
       }
       if (sizes.empty()) {  // nothing planned yet: the next generateMapForPlane uses the new context (no CUDA call here)
+        std::unique_lock<std::shared_mutex> config(configMu_);  // (the per-view entry point reads the context under it)
         std::memcpy(&ctx_, &next, sizeof(ctx_));
         return true;
       }
@@ -823,6 +873,97 @@ class VideoFrameTransform {
     return false;
   }
 
+  // Whole frame with a per-frame FLAT_FIXED view, device to device, asynchronous on `stream`: the frame a fresh transform
+  // would give for the context with fixed_yaw / pitch / hfov / vfov replaced by `view`, with no re-plan.  The gather
+  // computes its sampling records from the view (view_gather.cu); the low-pass, which depends on the view, is re-planned
+  // on the host (the segment rectangles do not change, the taps do) and its lists go to the device through the slot's
+  // page-locked rings, in stream order.  Nothing here synchronises the device, and the plans' sampling data is not read.
+  bool transformFrameView(const t360::FlatView& view, int numPlanes, const uint8_t* const* dIn, uint8_t* const* dOut, const int* inW,
+                          const int* inH, const int* inPitch, const int* outW, const int* outH, const int* outPitch, cudaStream_t stream) {
+    try {
+      if (numPlanes < 1 || numPlanes > kPlaneLanes) {
+        std::printf("Could not transform the frame with a view. Error: %d planes (1..%d supported)\n", numPlanes, kPlaneLanes);
+        return false;
+      }
+      if (!std::isfinite(view.yaw) || !std::isfinite(view.pitch) || !std::isfinite(view.hfov) || !std::isfinite(view.vfov)) {
+        std::printf("Could not transform the frame with a view. Error: the view (yaw %g, pitch %g, hfov %g, vfov %g) is not finite\n",
+                    view.yaw, view.pitch, view.hfov, view.vfov);
+        return false;
+      }
+      std::shared_lock<std::shared_mutex> config(configMu_);
+      if (ctx_.output_layout != LAYOUT_FLAT_FIXED) {
+        std::printf("Could not transform the frame with a view. Error: per-frame views need output_layout FLAT_FIXED (%d), the transform has %d\n",
+                    static_cast<int>(LAYOUT_FLAT_FIXED), static_cast<int>(ctx_.output_layout));
+        return false;
+      }
+      FrameTransformContext ctx = ctx_;
+      ctx.fixed_yaw = view.yaw;
+      ctx.fixed_pitch = view.pitch;
+      ctx.fixed_hfov = view.hfov;
+      ctx.fixed_vfov = view.vfov;
+      const DevicePlan* plans[kPlaneLanes];
+      for (int p = 0; p < numPlanes; ++p) {
+        if (!(plans[p] = findPlan(p ? 1 : 0, p))) return false;
+        if (inW[p] != plans[p]->inW || inH[p] != plans[p]->inH) {
+          std::printf("Could not transform the frame with a view. Error: input plane %d is %dx%d, its map was generated for %dx%d\n", p, inW[p],
+                      inH[p], plans[p]->inW, plans[p]->inH);
+          return false;
+        }
+        if (plans[p]->kernelSize == 0) {
+          std::printf("Could not transform the frame with a view. Error: no interpolation algorithm %d\n", ctx.interpolation_alg);
+          return false;
+        }
+      }
+      const DeviceRestore restoreDevice = ensureDevice();
+      cudaStream_t s = stream ? stream : stream_;
+      StreamSlot& slot = slotFor(s);
+      const uint8_t* src[kPlaneLanes];
+      int srcPitch[kPlaneLanes];
+      for (int p = 0; p < numPlanes; ++p) { src[p] = dIn[p]; srcPitch[p] = inPitch[p]; }
+      if (plans[0]->lowPass && !viewLowPass(ctx, plans, numPlanes, dIn, inW, inH, inPitch, slot, s, src, srcPitch)) return false;
+
+      t360::ViewGatherParams vp{};
+      for (int p = 0; p < numPlanes; ++p) {
+        const DevicePlan& plan = *plans[p];
+        t360::ViewPlane& v = vp.plane[p];
+        v.src = src[p];
+        v.srcPitch = srcPitch[p];
+        v.dst = dOut[p];
+        v.dstPitch = outPitch[p];
+        if (outW[p] != plan.mapW || outH[p] != plan.mapH) {  // render at the map's size, then cv::resize(INTER_AREA) (cpp:755-777)
+          const int sp = alignedPitch(plan.mapW);
+          slot.lanes[p].scaled.reserve(static_cast<size_t>(sp) * plan.mapH + 64);
+          v.dst = slot.lanes[p].scaled.ptr;
+          v.dstPitch = sp;
+        }
+        const bool stereoIn = ctx.input_stereo_format != STEREO_FORMAT_MONO;
+        v.geometry = t360::FlatGeometry{plan.mapW, plan.mapH, plan.inW, plan.inH, plan.kernelSize,
+                                        stereoIn && ctx.output_stereo_format == STEREO_FORMAT_LR, stereoIn && ctx.output_stereo_format == STEREO_FORMAT_TB,
+                                        ctx.vflip != 0, ctx.input_stereo_format == STEREO_FORMAT_LR, ctx.input_stereo_format == STEREO_FORMAT_TB};
+      }
+      vp.numPlanes = numPlanes;
+      vp.view = view;
+      vp.kernelSize = plans[0]->kernelSize;
+      vp.weights = deviceWeights(ctx.interpolation_alg);
+      CU(t360::launchViewGather(vp, numSMs_, s));
+      for (int p = 0; p < numPlanes; ++p) {
+        if (vp.plane[p].dst == dOut[p]) continue;
+        const DevicePlan& plan = *plans[p];
+        const DevicePlan::Resize& r = resizeFor(plan, outW[p], outH[p]);
+        t360::AreaParams ap{vp.plane[p].dst, dOut[p], plan.mapW, plan.mapH, vp.plane[p].dstPitch, outW[p], outH[p], outPitch[p],
+                            r.cellW, r.cellH, r.xTaps.ptr, r.xFirst.ptr, r.yTaps.ptr, r.yFirst.ptr, r.xLinear.ptr, r.yLinear.ptr, r.xMax};
+        CU(t360::launchAreaResize(ap, s));
+      }
+      return true;
+    } catch (const CudaFail& f) {
+      std::printf("Could not transform the frame with a view. Error: CUDA %s (%s) in %s\n", cudaGetErrorName(f.err), cudaGetErrorString(f.err), f.what);
+      cudaGetLastError();
+    } catch (const std::exception& ex) {
+      std::printf("Could not transform the frame with a view. Error: %s\n", ex.what());
+    }
+    return false;
+  }
+
   // tuning aid: a timeline of the consumer groups of the last frame gather (see StagedParams::trace)
   void enableTrace(bool on) { traceEnabled_ = on; }
   size_t readTrace(unsigned long long* out, size_t maxWords) {
@@ -1050,16 +1191,26 @@ class VideoFrameTransform {
 
   // Tiles of the plan, applied once (mono) or to both halves of a stereo frame (reference cpp:630-691), cut
   // into CTA-sized jobs.  Segments that do not fit the plane are dropped, like the reference's caught cv::Exception.
-  void buildBlurJobs(const std::vector<t360::LowPassSegment>& segments, const std::vector<float>& planTaps, int planeW, int planeH,
-                     int stereoFormat, DevicePlan::BlurSet& d) {
+  // Host half: the job lists.  *needsClear (if asked for): whether some pixel of the plane lies under no segment -- it
+  // depends on the plane size and the segment rectangles only, not on the view.
+  static void buildBlurLists(const std::vector<t360::LowPassSegment>& segments, const std::vector<float>& planTaps, int planeW, int planeH,
+                             int stereoFormat, BlurLists& out, bool* needsClear) {
     struct { const std::vector<t360::LowPassSegment>& segments; const std::vector<float>& taps; int inW, inH; } h{segments, planTaps, planeW, planeH};
-    std::vector<BlurJob> tiles, direct;
-    std::vector<StripJob> strips[t360::kStripMaxHy];
-    std::vector<float> taps = h.taps;  // original taps first (offsets of the plan stay valid), padded copies appended
+    std::vector<BlurJob>& tiles = out.tiles;
+    std::vector<BlurJob>& direct = out.direct;
+    std::vector<StripJob>* strips = out.strips;
+    for (auto& v : out.strips) v.clear();
+    tiles.clear();
+    direct.clear();
+    std::vector<float>& taps = out.taps;
+    std::vector<int>& source = out.tapSource;
+    taps = h.taps;  // original taps first (offsets of the plan stay valid), padded copies appended
+    source.resize(taps.size());
+    for (size_t i = 0; i < source.size(); ++i) source[i] = static_cast<int>(i) + 1;
     int offX[2] = {0, 0}, offY[2] = {0, 0}, passes = 1;
     if (stereoFormat == STEREO_FORMAT_LR) { passes = 2; offX[1] = static_cast<int>(0.5 * h.inW); }
     else if (stereoFormat == STEREO_FORMAT_TB) { passes = 2; offY[1] = static_cast<int>(0.5 * h.inH); }
-    std::vector<uint8_t> covered(static_cast<size_t>(h.inW) * h.inH, 0);
+    std::vector<uint8_t> covered(needsClear ? static_cast<size_t>(h.inW) * h.inH : 0, 0);
     int tileSmem = 0;
     // a warp-job covers 256 columns x `rows` rows; keep the grid at several thousand warps even for small planes
     const long long stripsPerRow = (h.inW + t360::kStripW - 1) / t360::kStripW;
@@ -1075,9 +1226,12 @@ class VideoFrameTransform {
     auto padKx = [&](int off, int n) {
       auto it = paddedKx.find({off, n});
       if (it != paddedKx.end()) return it->second;
-      while (taps.size() % 4) taps.push_back(0.f);
+      while (taps.size() % 4) { taps.push_back(0.f); source.push_back(0); }
       const int at = static_cast<int>(taps.size()), chunks = (n + 3) / 4;
-      for (int i = 0; i < chunks * 4; ++i) taps.push_back(i < n ? h.taps[off + i] : 0.f);
+      for (int i = 0; i < chunks * 4; ++i) {
+        taps.push_back(i < n ? h.taps[off + i] : 0.f);
+        source.push_back(i < n ? off + i + 1 : 0);
+      }
       return paddedKx[{off, n}] = std::make_pair(at, chunks);
     };
     std::map<int, int> paddedKy1;  // a single vertical tap k becomes {0, k, 0}
@@ -1087,6 +1241,7 @@ class VideoFrameTransform {
       if (it != paddedKy1.end()) return it->second;
       const int at = static_cast<int>(taps.size());
       taps.push_back(0.f); taps.push_back(h.taps[off]); taps.push_back(0.f);
+      source.push_back(0); source.push_back(off + 1); source.push_back(0);
       return paddedKy1[off] = at;
     };
 
@@ -1114,7 +1269,8 @@ class VideoFrameTransform {
         }
         i = j;
         const int left = s.left + offX[pass], top = s.top + offY[pass];
-        for (int y = 0; y < s.height; ++y) std::memset(&covered[static_cast<size_t>(top + y) * h.inW + left], 1, s.width);
+        if (needsClear)
+          for (int y = 0; y < s.height; ++y) std::memset(&covered[static_cast<size_t>(top + y) * h.inW + left], 1, s.width);
         const int hy = s.kyCount / 2;
         if (hy <= t360::kStripMaxHy && (s.kyCount & 1) && (s.kxCount & 1)) {
           const auto kx = padKx(s.kxOffset, s.kxCount);
@@ -1145,12 +1301,26 @@ class VideoFrameTransform {
         }
       }
     }
-    d.needsClear = std::find(covered.begin(), covered.end(), 0) != covered.end();
-    for (int c = 0; c < t360::kStripMaxHy; ++c) {
+    if (needsClear) *needsClear = std::find(covered.begin(), covered.end(), 0) != covered.end();
+    for (int c = 0; c < t360::kStripMaxHy; ++c)
       // heaviest jobs first: the hardware block scheduler then balances the tail
       std::stable_sort(strips[c].begin(), strips[c].end(), [](const StripJob& a, const StripJob& b) {
         return static_cast<long long>(a.kxChunks + 2) * a.h * (1 + 3 * a.edge) > static_cast<long long>(b.kxChunks + 2) * b.h * (1 + 3 * b.edge);
       });
+    out.tileSmem = tileSmem;
+  }
+
+  // ... and the device half: the lists of one plane size uploaded once (plan generation, or the first use of a size)
+  void buildBlurJobs(const std::vector<t360::LowPassSegment>& segments, const std::vector<float>& planTaps, int planeW, int planeH,
+                     int stereoFormat, DevicePlan::BlurSet& d) {
+    BlurLists lists;
+    buildBlurLists(segments, planTaps, planeW, planeH, stereoFormat, lists, &d.needsClear);
+    const std::vector<StripJob>* strips = lists.strips;
+    const std::vector<BlurJob>& tiles = lists.tiles;
+    const std::vector<BlurJob>& direct = lists.direct;
+    const std::vector<float>& taps = lists.taps;
+    const int tileSmem = lists.tileSmem;
+    for (int c = 0; c < t360::kStripMaxHy; ++c) {
       d.numStripJobs[c] = static_cast<int>(strips[c].size());
       d.hostStrips[c] = strips[c];
       if (strips[c].empty()) continue;
@@ -1369,6 +1539,197 @@ class VideoFrameTransform {
       CU(t360::launchBlurFrameStrips(fp, c + 1, s));
     }
     return true;
+  }
+
+  // The low-pass of a per-view frame (transformFrameView): the segments and taps of every plan index for the view, the
+  // job lists cut from them, uploaded through the slot's rings, and the launches -- one per vertical kernel size for all
+  // planes when every plane takes the strip kernel only (as blurFrame), else per plane (as runLowPass).  src / srcPitch
+  // receive the blurred planes.
+  bool viewLowPass(const FrameTransformContext& ctx, const DevicePlan* const* plans, int numPlanes, const uint8_t* const* dIn, const int* inW,
+                   const int* inH, const int* inPitch, StreamSlot& slot, cudaStream_t s, const uint8_t** src, int* srcPitch) {
+    const int indices = numPlanes > 1 ? 2 : 1;
+    HostPlan h[2];
+    // what the job lists depend on: the plans (generation), the planes, and per segment its rectangle, tap counts and
+    // offsets and whether its taps equal its left neighbour's (buildBlurLists merges such segments)
+    std::vector<long long> key{static_cast<long long>(planGeneration_), numPlanes};
+    for (int idx = 0; idx < indices; ++idx) {
+      const DevicePlan& plan = *plans[idx];
+      h[idx].ctx = ctx;
+      h[idx].inW = plan.inW; h[idx].inH = plan.inH; h[idx].outW = plan.outW; h[idx].outH = plan.outH; h[idx].mapW = plan.mapW; h[idx].mapH = plan.mapH;
+      if (!t360::buildLowPassPlan(h[idx])) {
+        std::printf("Could not transform the frame with a view. Error: no low-pass plan for index %d\n", idx);
+        return false;
+      }
+      key.push_back(reinterpret_cast<intptr_t>(&plan));
+      key.push_back(static_cast<long long>(h[idx].taps.size()));
+      const std::vector<float>& taps = h[idx].taps;
+      const t360::LowPassSegment* prev = nullptr;
+      for (const t360::LowPassSegment& g : h[idx].segments) {
+        const bool same = prev && g.kxCount == prev->kxCount && g.kyCount == prev->kyCount &&
+                          std::memcmp(&taps[g.kxOffset], &taps[prev->kxOffset], sizeof(float) * g.kxCount) == 0 &&
+                          std::memcmp(&taps[g.kyOffset], &taps[prev->kyOffset], sizeof(float) * g.kyCount) == 0;
+        for (long long v : {g.left, g.top, g.width, g.height, g.kxOffset, g.kxCount, g.kyOffset, g.kyCount}) key.push_back(v);
+        key.push_back(same);
+        prev = &g;
+      }
+    }
+    ViewBlurCache& c = slot.viewBlur;
+    std::vector<uint8_t> taps;
+    if (c.key == key) {  // same jobs as the slot's previous frame: refill the taps only
+      taps.resize(c.tapCodes.size() * sizeof(float));
+      float* t = reinterpret_cast<float*>(taps.data());
+      for (size_t i = 0; i < c.tapCodes.size(); ++i) {
+        const int code = c.tapCodes[i];
+        t[i] = code ? h[code >> 28].taps[(code & ((1 << 28) - 1)) - 1] : 0.f;
+      }
+    } else {
+      c = ViewBlurCache{};
+      BlurLists lists[2];
+      for (int idx = 0; idx < indices; ++idx)  // (coverage: plan.blur.needsClear, computed once per plan)
+        buildBlurLists(h[idx].segments, h[idx].taps, plans[idx]->inW, plans[idx]->inH, plans[idx]->stereoFormat, lists[idx], nullptr);
+      c.merged = numPlanes > 1;
+      for (int p = 0; p < numPlanes && c.merged; ++p) {
+        const BlurLists& l = lists[p ? 1 : 0];
+        c.merged = l.tiles.empty() && l.direct.empty() && !plans[p]->blur.needsClear;
+      }
+      // one byte image of the jobs and one of the taps (with the provenance of every tap), 16-byte aligned arrays
+      std::vector<uint8_t> codes;
+      auto append = [](std::vector<uint8_t>& blob, const void* data, size_t bytes) {
+        blob.resize((blob.size() + 15) & ~size_t(15));
+        const size_t at = blob.size();
+        blob.insert(blob.end(), static_cast<const uint8_t*>(data), static_cast<const uint8_t*>(data) + bytes);
+        return at;
+      };
+      auto appendTaps = [&](const BlurLists& l, int idx) {
+        std::vector<int> code(l.tapSource.size());
+        for (size_t i = 0; i < code.size(); ++i) code[i] = l.tapSource[i] ? (idx << 28) | l.tapSource[i] : 0;
+        append(codes, code.data(), code.size() * sizeof(int));
+        return append(taps, l.taps.data(), l.taps.size() * sizeof(float));
+      };
+      if (c.merged) {  // (as blurFrame: the planes' strip jobs with the plane in `edge`, one tap buffer, heaviest jobs first)
+        std::vector<StripJob> all[t360::kStripMaxHy];
+        for (int p = 0; p < numPlanes; ++p) {
+          const BlurLists& l = lists[p ? 1 : 0];
+          const int base = static_cast<int>(appendTaps(l, p ? 1 : 0) / sizeof(float));
+          if (p == 0) c.tapAt[0] = 0;
+          for (int k = 0; k < t360::kStripMaxHy; ++k)
+            for (StripJob j : l.strips[k]) {
+              j.kxOffset += base;
+              j.kyOffset += base;
+              j.edge |= p << t360::kStripPlaneShift;
+              all[k].push_back(j);
+            }
+        }
+        for (int k = 0; k < t360::kStripMaxHy; ++k) {
+          std::stable_sort(all[k].begin(), all[k].end(), [](const StripJob& a, const StripJob& b) {
+            return static_cast<long long>(a.kxChunks + 2) * a.h * (1 + 3 * (a.edge & 1)) > static_cast<long long>(b.kxChunks + 2) * b.h * (1 + 3 * (b.edge & 1));
+          });
+          c.numStrips[0][k] = static_cast<int>(all[k].size());
+          c.stripAt[0][k] = append(c.jobs, all[k].data(), all[k].size() * sizeof(StripJob));
+        }
+      } else {
+        for (int idx = 0; idx < indices; ++idx) {
+          const BlurLists& l = lists[idx];
+          for (int k = 0; k < t360::kStripMaxHy; ++k) {
+            c.numStrips[idx][k] = static_cast<int>(l.strips[k].size());
+            c.stripAt[idx][k] = append(c.jobs, l.strips[k].data(), l.strips[k].size() * sizeof(StripJob));
+          }
+          c.numTiles[idx] = static_cast<int>(l.tiles.size());
+          c.tileAt[idx] = append(c.jobs, l.tiles.data(), l.tiles.size() * sizeof(BlurJob));
+          c.numDirect[idx] = static_cast<int>(l.direct.size());
+          c.directAt[idx] = append(c.jobs, l.direct.data(), l.direct.size() * sizeof(BlurJob));
+          c.tileSmem[idx] = l.tileSmem;
+          c.tapAt[idx] = appendTaps(l, idx);
+        }
+      }
+      codes.resize(taps.size());  // (trailing alignment)
+      c.tapCodes.assign(reinterpret_cast<const int*>(codes.data()), reinterpret_cast<const int*>(codes.data()) + codes.size() / sizeof(int));
+      c.key = std::move(key);
+    }
+    const std::vector<uint8_t>& jobs = c.jobs;
+    const bool merged = c.merged;
+    const auto& stripAt = c.stripAt;
+    const auto& numStrips = c.numStrips;
+    UploadRing::Entry* used[2];
+    const uint8_t* dJobs = stageUpload(slot.viewJobs, jobs, s, &used[0]);
+    const uint8_t* dTaps = stageUpload(slot.viewTaps, taps, s, &used[1]);
+    for (int p = 0; p < numPlanes; ++p) {
+      const int bp = alignedPitch(inW[p]);
+      slot.lanes[p].blurred.reserve(static_cast<size_t>(bp) * inH[p] + 64);
+      src[p] = slot.lanes[p].blurred.ptr;
+      srcPitch[p] = bp;
+    }
+    if (merged) {
+      t360::FrameStripParams fp{};
+      for (int p = 0; p < numPlanes; ++p) fp.plane[p] = {dIn[p], slot.lanes[p].blurred.ptr, inW[p], inH[p], inPitch[p], srcPitch[p]};
+      fp.taps = reinterpret_cast<const float*>(dTaps + c.tapAt[0]);
+      for (int c = 0; c < t360::kStripMaxHy; ++c) {
+        if (!numStrips[0][c]) continue;
+        fp.jobs = reinterpret_cast<const StripJob*>(dJobs + stripAt[0][c]);
+        fp.numJobs = numStrips[0][c];
+        CU(t360::launchBlurFrameStrips(fp, c + 1, s));
+      }
+    } else {
+      for (int p = 0; p < numPlanes; ++p) {
+        const int idx = p ? 1 : 0;
+        uint8_t* dst = slot.lanes[p].blurred.ptr;
+        const float* dt = reinterpret_cast<const float*>(dTaps + c.tapAt[idx]);
+        if (plans[p]->blur.needsClear) CU(cudaMemset2DAsync(dst, srcPitch[p], 0, inW[p], inH[p], s));  // reference cpp:625
+        for (int c = 0; c < t360::kStripMaxHy; ++c) {
+          if (!numStrips[idx][c]) continue;
+          t360::StripParams sp{dIn[p], dst, inW[p], inH[p], inPitch[p], srcPitch[p], reinterpret_cast<const StripJob*>(dJobs + stripAt[idx][c]),
+                               numStrips[idx][c], dt};
+          CU(t360::launchBlurStrips(sp, c + 1, s));
+        }
+        t360::BlurParams bp{dIn[p], dst, inW[p], inH[p], inPitch[p], srcPitch[p], reinterpret_cast<const BlurJob*>(dJobs + c.tileAt[idx]),
+                            c.numTiles[idx], dt, c.tileSmem[idx]};
+        if (bp.numJobs) CU(t360::launchBlur(bp, s));
+        if (c.numDirect[idx]) {
+          bp.jobs = reinterpret_cast<const BlurJob*>(dJobs + c.directAt[idx]);
+          bp.numJobs = c.numDirect[idx];
+          CU(t360::launchBlurDirect(bp, s));
+        }
+      }
+    }
+    for (UploadRing::Entry* e : used) {  // the entries may be refilled once these launches have finished
+      CU(cudaEventRecord(e->released, s));
+      e->inFlight = true;
+    }
+    return true;
+  }
+
+  // `bytes` on the device for work enqueued next on `s`: the ring entry that already holds them, or the next entry, refilled
+  // (page-locked copy, cudaMemcpyAsync on `s`) once the frame that last read it has finished.
+  static const uint8_t* stageUpload(UploadRing& ring, const std::vector<uint8_t>& bytes, cudaStream_t s, UploadRing::Entry** used) {
+    if (ring.last >= 0 && ring.lastContent == bytes) {
+      *used = &ring.entries[ring.last];
+      return ring.entries[ring.last].device;
+    }
+    const int i = (ring.last + 1) % UploadRing::kEntries;
+    UploadRing::Entry& e = ring.entries[i];
+    ring.last = -1;  // (until the entry holds the new bytes)
+    if (!e.released) CU(cudaEventCreateWithFlags(&e.released, cudaEventDisableTiming));
+    if (e.inFlight) CU(cudaEventSynchronize(e.released));
+    e.inFlight = false;
+    if (bytes.size() > e.capacity) {  // grows to the largest list seen (rarely: the list sizes depend on the tap counts)
+      const size_t cap = std::max<size_t>(bytes.size() + bytes.size() / 4, 4096);
+      if (e.host) CU(cudaFreeHost(e.host));
+      e.host = nullptr;
+      if (e.device) CU(cudaFreeAsync(e.device, s));
+      e.device = nullptr;
+      e.capacity = 0;
+      CU(cudaHostAlloc(reinterpret_cast<void**>(&e.host), cap, cudaHostAllocDefault));
+      CU(cudaMallocAsync(reinterpret_cast<void**>(&e.device), cap, s));
+      e.capacity = cap;
+    }
+    if (!bytes.empty()) {
+      std::memcpy(e.host, bytes.data(), bytes.size());
+      CU(cudaMemcpyAsync(e.device, e.host, bytes.size(), cudaMemcpyHostToDevice, s));
+    }
+    ring.last = i;
+    ring.lastContent = bytes;
+    *used = &e;
+    return e.device;
   }
 
   // The gathers of all planes of a frame as ONE launch (every plane staged).
@@ -1626,6 +1987,41 @@ T360_API int T360B200_lowPassPlaneAsync(VideoFrameTransform* t, const uint8_t* d
 T360_API int T360B200_reconfigure(VideoFrameTransform* t, const FrameTransformContext* ctx) {
   if (!t || !ctx) return 0;
   return t->reconfigure(*ctx);
+}
+T360_API int T360B200_transformFrameViewAsync(VideoFrameTransform* t, const T360View* view, int numPlanes, const uint8_t* const* dIn,
+                                              uint8_t* const* dOut, const int* inW, const int* inH, const int* inPitch, const int* outW,
+                                              const int* outH, const int* outPitch, void* stream) {
+  if (!t || !view || !dIn || !dOut || !inW || !inH || !inPitch || !outW || !outH || !outPitch) return 0;
+  const t360::FlatView v{view->yaw, view->pitch, view->hfov, view->vfov};
+  return t->transformFrameView(v, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, static_cast<cudaStream_t>(stream));
+}
+T360_API int T360B200_viewSamples(const FrameTransformContext* ctx, const T360View* view, int inW, int inH, int outW, int outH, int32_t* samples) {
+  if (!ctx || !view || !samples) return 0;
+  if (ctx->output_layout != LAYOUT_FLAT_FIXED) {
+    std::printf("Could not compute the view's samples. Error: output_layout %d is not FLAT_FIXED\n", static_cast<int>(ctx->output_layout));
+    return 0;
+  }
+  if (!std::isfinite(view->yaw) || !std::isfinite(view->pitch) || !std::isfinite(view->hfov) || !std::isfinite(view->vfov)) {
+    std::printf("Could not compute the view's samples. Error: the view is not finite\n");
+    return 0;
+  }
+  const int k = t360::kernelSizeOf(ctx->interpolation_alg);
+  const int mapW = static_cast<int>(ctx->width_scale_factor * outW + 0.5), mapH = static_cast<int>(ctx->height_scale_factor * outH + 0.5);
+  if (k == 0 || inW <= 0 || inH <= 0 || outW <= 0 || outH <= 0 || mapW <= 0 || mapH <= 0) {
+    std::printf("Could not compute the view's samples. Error: invalid interpolation or plane sizes\n");
+    return 0;
+  }
+  const bool stereoIn = ctx->input_stereo_format != STEREO_FORMAT_MONO;
+  const t360::FlatGeometry g{mapW, mapH, inW, inH, k, stereoIn && ctx->output_stereo_format == STEREO_FORMAT_LR,
+                             stereoIn && ctx->output_stereo_format == STEREO_FORMAT_TB, ctx->vflip != 0,
+                             ctx->input_stereo_format == STEREO_FORMAT_LR, ctx->input_stereo_format == STEREO_FORMAT_TB};
+  const t360::FlatView v{view->yaw, view->pitch, view->hfov, view->vfov};
+  for (int i = 0; i < mapH; ++i)
+    for (int j = 0; j < mapW; ++j) {
+      int32_t* out = samples + 2 * (static_cast<size_t>(i) * mapW + j);
+      t360::flatSample(v, g, i, j, out, out + 1);
+    }
+  return 1;
 }
 T360_API void T360B200_setPinHostPlanes(VideoFrameTransform* t, int enable) { if (t) t->setPinHostPlanes(enable != 0); }
 T360_API void T360B200_debugTrace(VideoFrameTransform* t, int enable) { if (t) t->enableTrace(enable != 0); }

@@ -46,6 +46,7 @@ typedef struct T360CudaContext {
 
   VideoFrameTransform* transform;
   int maps_ready;
+  int view_frames; /* a FLAT_FIXED view command arrived after the first frame: every frame passes its view */
   int sw_format, num_planes;
   AVBufferRef* out_frames;
   AVCUDADeviceContext* cuda;
@@ -233,10 +234,18 @@ static int t360_filter_frame(AVFilterLink* inlink, AVFrame* in) {
       in_pitch[p] = in->linesize[p];
       out_pitch[p] = out->linesize[p];
     }
-    rc = T360B200_transformFrameAsync(s->transform, s->num_planes, src, dst, in_w, in_h, in_pitch, out_w, out_h, out_pitch,
-                                      s->cuda->stream)
-             ? 0
-             : AVERROR_EXTERNAL;
+    if (s->view_frames) {
+      const T360View view = {s->params.fixed_yaw, s->params.fixed_pitch, s->params.fixed_hfov, s->params.fixed_vfov};
+      rc = T360B200_transformFrameViewAsync(s->transform, &view, s->num_planes, src, dst, in_w, in_h, in_pitch, out_w, out_h,
+                                            out_pitch, s->cuda->stream)
+               ? 0
+               : AVERROR_EXTERNAL;
+    } else {
+      rc = T360B200_transformFrameAsync(s->transform, s->num_planes, src, dst, in_w, in_h, in_pitch, out_w, out_h, out_pitch,
+                                        s->cuda->stream)
+               ? 0
+               : AVERROR_EXTERNAL;
+    }
     /* `in` is released below: its buffer goes back to the decoder's pool, which may hand it out again while the
      * gather still reads it unless the stream is drained first */
     if (!rc && s->sync && cu->cuStreamSynchronize(s->cuda->stream)) rc = AVERROR_EXTERNAL;
@@ -257,6 +266,9 @@ done:
  * (T360B200_reconfigure: frames filtered before the command keep the old view, every later frame has the new one).
  * Options that could change the output link's size or format (size, cube edge, layouts, stereo formats, scale factors)
  * are refused with ENOSYS, invalid values with EINVAL; a refused command leaves every parameter as it was.
+ * In a FLAT_FIXED filter the view commands (yaw, pitch, hfov, vfov) after the first frame re-plan nothing: they update the
+ * parameters, and from then on every frame goes through T360B200_transformFrameViewAsync with the current view, so a
+ * view can change every frame (head tracking, a camera path) at the cost of a frame, not of a re-plan.
  * This needs AV_OPT_FLAG_RUNTIME_PARAM and ff_filter_process_command (FFmpeg 4.2 and later).  A libavfilter without
  * runtime options builds the filter without commands: the options are then fixed at init, as in the reference filter. */
 #ifdef AV_OPT_FLAG_RUNTIME_PARAM
@@ -279,6 +291,11 @@ static int t360_process_command(AVFilterContext* ctx, const char* cmd, const cha
     return AVERROR(EINVAL);
   }
   if (!s->maps_ready) return 0;
+  if (s->params.output_layout == LAYOUT_FLAT_FIXED &&
+      (!strcmp(cmd, "yaw") || !strcmp(cmd, "pitch") || !strcmp(cmd, "hfov") || !strcmp(cmd, "vfov"))) {
+    s->view_frames = 1;
+    return 0;
+  }
   CudaFunctions* cu = s->cuda->internal->cuda_dl;
   CUcontext popped;
   if (cu->cuCtxPushCurrent(s->cuda->cuda_ctx)) {

@@ -53,6 +53,16 @@ FILTER_DEFAULTS = dict(  # the reference's AVOption defaults (vf_transform360.c:
     num_horizontal_segments=1, adjust_kernel=1, kernel_adjust_factor=1.0)
 
 
+class T360View(C.Structure):
+    """A FLAT_FIXED view in degrees (include/transform360_b200.h), as the context's fixed_yaw / pitch / hfov / vfov."""
+    _fields_ = [("yaw", C.c_float), ("pitch", C.c_float), ("hfov", C.c_float), ("vfov", C.c_float)]
+
+
+def as_view(view) -> T360View:
+    """A T360View from a T360View or a (yaw, pitch, hfov, vfov) sequence."""
+    return view if isinstance(view, T360View) else T360View(*[float(v) for v in view])
+
+
 def make_context(**overrides) -> FrameTransformContext:
     vals = dict(FILTER_DEFAULTS)
     for k in overrides:
@@ -112,6 +122,10 @@ def load(path: os.PathLike | None = None):
     L.T360B200_lowPassPlaneAsync.argtypes = [vp, vp, vp] + [ci] * 5 + [vp]
     L.T360B200_reconfigure.restype = ci
     L.T360B200_reconfigure.argtypes = [vp, C.POINTER(FrameTransformContext)]
+    L.T360B200_transformFrameViewAsync.restype = ci
+    L.T360B200_transformFrameViewAsync.argtypes = [vp, C.POINTER(T360View), ci, vp, vp] + [vp] * 6 + [vp]
+    L.T360B200_viewSamples.restype = ci
+    L.T360B200_viewSamples.argtypes = [C.POINTER(FrameTransformContext), C.POINTER(T360View)] + [ci] * 4 + [vp]
     L.T360B200_setPinHostPlanes.restype = None
     L.T360B200_setPinHostPlanes.argtypes = [vp, ci]
     L.T360B200_debugTrace.restype = None
@@ -140,7 +154,7 @@ EXPORTED_SYMBOLS = [
     "T360B200_hostPlanInfo", "T360B200_hostPlanMap", "T360B200_hostPlanSamples", "T360B200_hostPlanSegment",
     "T360B200_hostPlanGather", "T360B200_hostPlanPoleCaps", "T360B200_weightImage", "T360B200_dealLanes",
     "T360B200_remapTable", "T360B200_transformFramePlaneAsync", "T360B200_transformFrameAsync",
-    "T360B200_lowPassPlaneAsync", "T360B200_reconfigure",
+    "T360B200_lowPassPlaneAsync", "T360B200_reconfigure", "T360B200_transformFrameViewAsync", "T360B200_viewSamples",
     "T360B200_setPinHostPlanes", "T360B200_debugTrace", "T360B200_debugTraceRead", "T360B200_synchronize", "T360B200_stream", "T360B200_kernelLaunchCount", "T360B200_planDeviceBytes",
     "T360B200_planTileCounts", "T360B200_deviceCount", "T360B200_version",
 ]
@@ -217,6 +231,23 @@ class VideoFrameTransform:
 
         def call(stream: int = 0, _keep=(d_in, d_out, arrs)) -> bool:
             return bool(fn(h, n, pin, pout, *ptrs, stream))
+        return call
+
+    def make_view_frame_call(self, in_planes, out_planes, dims):
+        """Like make_frame_call, for T360B200_transformFrameViewAsync (FLAT_FIXED transforms): returns a callable
+        f(view, stream) -> bool that enqueues the whole frame with `view` (a T360View or (yaw, pitch, hfov, vfov))."""
+        n = len(in_planes)
+        VP, IA = C.c_void_p * n, C.c_int * n
+        d_in = VP(*[p[0] for p in in_planes])
+        d_out = VP(*[p[0] for p in out_planes])
+        arrs = [IA(*[d[0] for d in dims]), IA(*[d[1] for d in dims]), IA(*[p[1] for p in in_planes]),
+                IA(*[d[2] for d in dims]), IA(*[d[3] for d in dims]), IA(*[p[1] for p in out_planes])]
+        fn, h = self._lib.T360B200_transformFrameViewAsync, self._h
+        ptrs = [C.cast(a, C.c_void_p) for a in arrs]
+        pin, pout = C.cast(d_in, C.c_void_p), C.cast(d_out, C.c_void_p)
+
+        def call(view, stream: int = 0, _keep=(d_in, d_out, arrs)) -> bool:
+            return bool(fn(h, C.byref(as_view(view)), n, pin, pout, *ptrs, stream))
         return call
 
     def low_pass_async(self, d_in: int, d_out: int, w, h, in_pitch, out_pitch, plan_index, stream: int = 0) -> bool:
@@ -337,6 +368,17 @@ class HostPlan:
             b = np.frombuffer((C.c_float * nk[1]).from_address(ky.value), np.float32).copy()
             out.append((rect[0], rect[1], rect[2], rect[3], a, b))
         return out
+
+
+def view_samples(ctx: FrameTransformContext, view, in_w, in_h, out_w, out_h) -> np.ndarray:
+    """The sampling records the per-view kernel computes for one plane (T360B200_viewSamples, no CUDA):
+    int32 [map_h][map_w][2] like HostPlan.samples."""
+    scaled = lambda f, n: int(float(np.float32(f) * np.float32(n)) + 0.5)  # (float product, double sum: buildHostPlan)
+    map_w, map_h = scaled(ctx.width_scale_factor, out_w), scaled(ctx.height_scale_factor, out_h)
+    out = np.zeros((max(map_h, 0), max(map_w, 0), 2), np.int32)
+    if not load().T360B200_viewSamples(C.byref(ctx), C.byref(as_view(view)), in_w, in_h, out_w, out_h, out.ctypes.data):
+        raise ValueError("T360B200_viewSamples refused the arguments (message on stdout)")
+    return out
 
 
 def remap_table(interpolation_alg: int) -> np.ndarray | None:
