@@ -54,6 +54,15 @@ int T360B200_dealLanes(int interpolationAlg, int n, const int32_t* phases, int32
 /* The frame kernel's shared-memory image of the interpolation table (csrc/kernels.cuh: "Weight tables in shared
  * memory"); returns its size in bytes (0 if unsupported). */
 int T360B200_weightImage(int interpolationAlg, const uint8_t** image);
+/* The low-pass job lists of plans[0 .. numPlans) (no GPU needed) for planes of width x height (0: each plan's input size),
+ * as the device holds them: one plan's lists, or for 2-3 plans (the planes of a frame) their strip jobs merged into one
+ * list (the plane in each job's edge field).  *image: the packed lists (formats: csrc/kernels.cuh, csrc/lowpass_jobs.h),
+ * valid until the next call with the same plans[0] or its T360B200_hostPlanDestroy.  layout = {strip jobs by vertical
+ * half-size 1..3 (3 counts), tile jobs, direct jobs, taps, tile shared-memory bytes, needsClear (some pixel lies under no
+ * segment), byte offsets of the three strip arrays, of the tiles, the direct jobs and the taps, image bytes}.  Returns 1
+ * on success. */
+int T360B200_hostPlanBlurLists(T360HostPlan* const* plans, int numPlans, int width, int height, int layout[15],
+                               const uint8_t** image);
 /* low-pass segment i in the reference's order: rect = left, top, width, height; taps = kx then ky */
 int T360B200_hostPlanSegment(const T360HostPlan* plan, int i, int rect[4], int numTaps[2], const float** kx,
                              const float** ky);

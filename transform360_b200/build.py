@@ -18,7 +18,7 @@ ROOT = PKG.parent
 CSRC = PKG / "csrc"
 LIB_DIR = PKG / "lib"
 LIB = LIB_DIR / "libTransform360.so"
-SOURCES = ["geometry.cpp", "lowpass_plan.cpp", "sampling.cpp", "gather_plan.cpp", "kernels.cu", "gather_frame.cu", "view_gather.cu", "video_frame_transform.cpp"]
+SOURCES = ["geometry.cpp", "lowpass_plan.cpp", "lowpass_jobs.cpp", "sampling.cpp", "gather_plan.cpp", "kernels.cu", "gather_frame.cu", "view_gather.cu", "video_frame_transform.cpp"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 
 

@@ -4,9 +4,9 @@
 //   gatherKernel<K>        replace cv::remap as the reference calls it (VideoFrameTransform.cpp:748-754) for whole
 //   nearestKernel          planes the frame kernel cannot take (BORDER_TRANSPARENT plans, nearest neighbour, planes
 //                          TMA cannot describe): taps through L1, every border case.
-//   blurStripKernel<HY>    replace cv::sepFilter2D over the reference's tiles (cpp:173-204, 579-704):
-//   blurTileKernel         separable Gaussian, float32, fused multiply-add chain in the order cv2 4.13 uses
-//   blurDirectKernel       (see oracle/t360_oracle.c for the model and its pin), round-half-even, u8.
+//   blurFrameStripKernel<HY>  replace cv::sepFilter2D over the reference's tiles (cpp:173-204, 579-704) for 1-3 planes:
+//   blurTileKernel            separable Gaussian, float32, fused multiply-add chain in the order cv2 4.13 uses
+//   blurDirectKernel          (see oracle/t360_oracle.c for the model and its pin), round-half-even, u8.
 //   areaResizeKernel       replaces cv::resize(INTER_AREA) (cpp:770-776).
 #include "gather_common.cuh"
 
@@ -324,22 +324,15 @@ __device__ __forceinline__ void stripBody(const StripParams& p, const StripJob& 
   }
 }
 
-template <int HY>
 #ifndef T360_BLUR_PDL
 #define T360_BLUR_PDL 0
 #endif
 #ifndef T360_BLUR_MINBLOCKS
 #define T360_BLUR_MINBLOCKS 6  // H100 at 700 W: 80 registers (with spills), 142.4 us per cfg3 frame; 4 blocks 144.4 us, 3 blocks 157.2 us
 #endif
-__global__ void __launch_bounds__(128, T360_BLUR_MINBLOCKS) blurStripKernel(StripParams p) {
-  const int job = blockIdx.x * 4 + (threadIdx.x >> 5);
-  if (job >= p.numJobs) return;
-  const StripJob j = p.jobs[job];
-  if (j.edge) stripBody<HY, true>(p, j, threadIdx.x & 31);
-  else stripBody<HY, false>(p, j, threadIdx.x & 31);
-}
-
-template <int HY>
+// MULTI: the jobs name planes 0..2 in `edge`; otherwise every job is plane 0's (no per-job plane selection: as many
+// registers and spills as a kernel written for one plane)
+template <int HY, bool MULTI>
 __global__ void __launch_bounds__(128, T360_BLUR_MINBLOCKS) blurFrameStripKernel(const __grid_constant__ FrameStripParams fp) {
 #if T360_BLUR_PDL
   // the frame gather that follows on the stream may place its CTAs on SMs this grid has already left and run its
@@ -349,7 +342,7 @@ __global__ void __launch_bounds__(128, T360_BLUR_MINBLOCKS) blurFrameStripKernel
   const int job = blockIdx.x * 4 + (threadIdx.x >> 5);
   if (job >= fp.numJobs) return;
   const StripJob j = fp.jobs[job];
-  const int pl = j.edge >> kStripPlaneShift;
+  const int pl = MULTI ? j.edge >> kStripPlaneShift : 0;
   const FrameStripParams::Plane &a = fp.plane[0], &b = fp.plane[1], &c = fp.plane[2];
 #define T360_PICK(f) (pl == 0 ? a.f : (pl == 1 ? b.f : c.f))
   const StripParams p{T360_PICK(src), T360_PICK(dst), T360_PICK(width), T360_PICK(height), T360_PICK(srcPitch), T360_PICK(dstPitch),
@@ -492,26 +485,14 @@ cudaError_t launchAreaResize(const AreaParams& p, cudaStream_t stream) {
   return cudaGetLastError();
 }
 
-cudaError_t launchBlurStrips(const StripParams& p, int hy, cudaStream_t stream) {
-  if (p.numJobs <= 0) return cudaSuccess;
-  const int grid = (p.numJobs + 3) / 4;
-  switch (hy) {
-    case 0: case 1: blurStripKernel<1><<<grid, 128, 0, stream>>>(p); break;  // hy == 0: one tap, padded with two zeros
-    case 2: blurStripKernel<2><<<grid, 128, 0, stream>>>(p); break;
-    case 3: blurStripKernel<3><<<grid, 128, 0, stream>>>(p); break;
-    default: return cudaErrorInvalidValue;
-  }
-  gLaunches.fetch_add(1, std::memory_order_relaxed);
-  return cudaGetLastError();
-}
-
 cudaError_t launchBlurFrameStrips(const FrameStripParams& p, int hy, cudaStream_t stream) {
   if (p.numJobs <= 0) return cudaSuccess;
   const int grid = (p.numJobs + 3) / 4;
-  switch (hy) {
-    case 0: case 1: blurFrameStripKernel<1><<<grid, 128, 0, stream>>>(p); break;
-    case 2: blurFrameStripKernel<2><<<grid, 128, 0, stream>>>(p); break;
-    case 3: blurFrameStripKernel<3><<<grid, 128, 0, stream>>>(p); break;
+  const bool multi = p.numPlanes > 1;
+  switch (hy) {  // hy == 0: one tap, padded with two zeros
+    case 0: case 1: multi ? blurFrameStripKernel<1, true><<<grid, 128, 0, stream>>>(p) : blurFrameStripKernel<1, false><<<grid, 128, 0, stream>>>(p); break;
+    case 2: multi ? blurFrameStripKernel<2, true><<<grid, 128, 0, stream>>>(p) : blurFrameStripKernel<2, false><<<grid, 128, 0, stream>>>(p); break;
+    case 3: multi ? blurFrameStripKernel<3, true><<<grid, 128, 0, stream>>>(p) : blurFrameStripKernel<3, false><<<grid, 128, 0, stream>>>(p); break;
     default: return cudaErrorInvalidValue;
   }
   gLaunches.fetch_add(1, std::memory_order_relaxed);

@@ -280,14 +280,16 @@ struct AreaParams {
 };
 cudaError_t launchAreaResize(const AreaParams& p, cudaStream_t stream);
 
-// The strip jobs of all planes of a frame in ONE launch (StripJob::edge carries the plane in bits 8-9; kxOffset / kyOffset
-// index the merged tap buffer): one launch and one tail instead of three launches on three streams.
+// The register-resident low-pass (hy <= kStripMaxHy) of 1-3 planes in ONE launch (StripJob::edge carries the plane in
+// bits 8-9; kxOffset / kyOffset index the tap buffer, merged for several planes: lowpass_jobs.h): a frame takes one launch
+// and one tail instead of three launches on three streams; a single plane's list has plane 0 throughout.
 struct FrameStripParams {
   struct Plane {
     const uint8_t* src;
     uint8_t* dst;
     int width, height, srcPitch, dstPitch;
   } plane[kMaxFramePlanes];
+  int numPlanes;
   const StripJob* jobs;
   int numJobs;
   const float* taps;
@@ -312,7 +314,6 @@ cudaError_t launchGatherFrame(const FrameGatherParams& p, const StagedParams& jo
 // one-time set-up of the frame kernel for kernelSize on the current device (shared-memory opt-in, occupancy): call it
 // before capturing launchGatherFrame into a CUDA graph
 cudaError_t prepareGatherFrame(int kernelSize);
-cudaError_t launchBlurStrips(const StripParams& p, int hy, cudaStream_t stream);  // register-resident, hy <= kStripMaxHy
 cudaError_t launchBlur(const BlurParams& p, cudaStream_t stream);        // shared-memory tiles
 cudaError_t launchBlurDirect(const BlurParams& p, cudaStream_t stream);  // any kernel size, slow
 unsigned long long kernelLaunchCount();

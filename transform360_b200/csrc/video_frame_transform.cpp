@@ -27,6 +27,7 @@
 #include "host_plan.h"
 #include "gather_plan.h"
 #include "kernels.cuh"
+#include "lowpass_jobs.h"
 #include "transform360_b200.h"
 
 #define T360_API extern "C" __attribute__((visibility("default")))
@@ -92,17 +93,13 @@ struct DevicePlan {
   std::vector<int> jobNeedRows;        // per host job: the source rows [0, n) it reads (streaming host planes in)
   std::vector<t360::JobRect> jobRects; // per host job: the output rectangle it writes into (streaming host planes out)
   int numJobs = 0, numStaged = 0, numBorder = 0;  // staged: jobs with a TMA box; border: jobs reading through L1
-  // low-pass: register-resident strip jobs grouped by vertical half-size 1..3, and the rest (large vertical kernels),
-  // for one plane size
+  // low-pass: the job lists of one plane size, on the host (the whole-frame entry point merges the planes' lists) and
+  // packed into one device image
   struct BlurSet {
-    DeviceBuffer<StripJob> stripJobs[t360::kStripMaxHy];
-    int numStripJobs[t360::kStripMaxHy] = {};
-    DeviceBuffer<BlurJob> tileJobs, directJobs;
-    int numTileJobs = 0, numDirectJobs = 0, tileSmem = 0;
-    DeviceBuffer<float> taps;
+    t360::BlurLists lists;
+    t360::BlurLayout layout;
+    DeviceBuffer<uint8_t> image;
     bool needsClear = false;
-    std::vector<StripJob> hostStrips[t360::kStripMaxHy];  // (the whole-frame entry point merges the planes' strip jobs)
-    std::vector<float> hostTaps;
   };
   BlurSet blur;  // for the plane size the plan was generated for
   // (a caller may pass planes of another size: the reference then filters the segments that still fit, cpp:173-204)
@@ -119,10 +116,23 @@ struct DevicePlan {
   bool resizeNeeded = false;  // for the size the map was generated for
   mutable std::map<std::pair<int, int>, Resize> resizes;
   size_t deviceBytes() const {
-    return samples.bytes() + records.bytes() + gatherJobs.bytes() + blur.stripJobs[0].bytes() + blur.stripJobs[1].bytes() + blur.stripJobs[2].bytes() +
-           blur.tileJobs.bytes() + blur.directJobs.bytes() + blur.taps.bytes();
+    return samples.bytes() + records.bytes() + gatherJobs.bytes() + blur.image.bytes();
   }
 };
+
+// Whether the low-pass of a frame's planes runs as one strip launch per vertical half-size for all of them: every plane
+// has low-pass at the size it was planned for, the plan is not transparent, its segments cover the plane and its lists
+// (lists[p]) hold strip jobs only.
+bool mergeable(const DevicePlan* const* plans, const t360::BlurLists* const* lists, int numPlanes, const int* inW, const int* inH) {
+  if (numPlanes < 2) return false;
+  for (int p = 0; p < numPlanes; ++p) {
+    const DevicePlan& d = *plans[p];
+    if (!d.lowPass || d.transparent || inW[p] != d.inW || inH[p] != d.inH || d.blur.needsClear || !lists[p]->tiles.empty() ||
+        !lists[p]->direct.empty())
+      return false;
+  }
+  return true;
+}
 
 // The host-side half of a plan index (no CUDA call): the planner's result and, for interpolating plans, the gather plan.
 struct HostIndexPlan {
@@ -203,13 +213,21 @@ struct GatherWork {
   const void* resizeTables = nullptr;
 };
 
-// The tiles of all planes of a frame in one list (general, class 1, class 0; luma first inside each kind), rebuilt
-// when a map is regenerated.
-struct FrameJobList {
-  DeviceBuffer<GatherJob> tiles;
-  int numTiles = 0, numPlanes = 0;
+// The merged lists of a frame of 2 or 3 planes, built once per plan generation: the gather jobs of every plane in one
+// list (jobLaunchRank order, the plane in outY) and the planes' low-pass strip jobs in one image (mergeBlurLists).
+struct FrameLists {
   unsigned long long generation = ~0ull;
-  DeviceBuffer<int> claimCounter;
+  DeviceBuffer<GatherJob> gatherJobs;
+  int numGatherJobs = 0;
+  DeviceBuffer<uint8_t> blurImage;
+  t360::BlurLayout blurLayout;
+};
+// ... as one frame launches them (copied out under the lock)
+struct FrameListRefs {
+  const GatherJob* gatherJobs;
+  int numGatherJobs;
+  const uint8_t* blurImage;
+  t360::BlurLayout blurLayout;
 };
 
 // How the synchronous host-pointer call streams a large plane through the GPU: the input arrives in `chunks` row bands;
@@ -225,15 +243,6 @@ struct WavePlan {
   std::vector<std::vector<Rect>> rects;
 };
 
-// The low-pass job lists of one plane size on the host (VideoFrameTransform::buildBlurLists).
-struct BlurLists {
-  std::vector<StripJob> strips[t360::kStripMaxHy];
-  std::vector<BlurJob> tiles, direct;
-  std::vector<float> taps;
-  std::vector<int> tapSource;  // per entry of taps: 1 + the index of the plan's tap it copies, 0 for a padding zero
-  int tileSmem = 0;
-};
-
 // The per-view low-pass lists of a stream slot's previous frame and what they were made from.  The jobs (rectangles, tap
 // counts and offsets) depend on the view only through the segments' tap counts and on which neighbouring segments carry
 // identical taps; when those agree with the previous frame's, the jobs are reused and only the taps are refilled.
@@ -241,9 +250,8 @@ struct ViewBlurCache {
   std::vector<long long> key;
   bool merged = false;
   std::vector<uint8_t> jobs;
-  std::vector<int> tapCodes;  // per float of the tap image: plan index << 28 | (1 + plan tap), 0 for a zero
-  size_t stripAt[2][t360::kStripMaxHy] = {}, tileAt[2] = {}, directAt[2] = {}, tapAt[2] = {};
-  int numStrips[2][t360::kStripMaxHy] = {}, numTiles[2] = {}, numDirect[2] = {}, tileSmem[2] = {};
+  std::vector<int> tapCodes;  // per float of the tap image: plane << kTapPlaneShift | (1 + plan tap), 0 for a zero
+  t360::BlurLayout layout[2];  // merged: [0]; else per plan index
 };
 
 // Page-locked staging of lists that change from frame to frame (the per-view low-pass jobs and taps): a few entries, each
@@ -273,15 +281,6 @@ struct StreamSlot {
   cudaEvent_t fork = nullptr;
   UploadRing viewJobs, viewTaps;  // the per-view low-pass lists (VideoFrameTransform::transformFrameView)
   ViewBlurCache viewBlur;
-};
-
-// The strip jobs of all planes of a frame, by vertical half-size, with one merged tap buffer (rebuilt when a map is).
-struct FrameBlurList {
-  DeviceBuffer<StripJob> jobs[t360::kStripMaxHy];
-  int numJobs[t360::kStripMaxHy] = {};
-  DeviceBuffer<float> taps;
-  int numPlanes = 0;
-  unsigned long long generation = ~0ull;
 };
 
 constexpr int kPitchAlign = 256;
@@ -329,11 +328,11 @@ class VideoFrameTransform {
             if (e.released) cudaEventDestroy(e.released);
           }
       }
-      frameJobs_.tiles.release();
-      for (auto& b : frameBlur_.jobs) b.release();
-      frameBlur_.taps.release();
+      for (FrameLists& f : frameLists_) {
+        f.gatherJobs.release();
+        f.blurImage.release();
+      }
       trace_.release();
-      frameJobs_.claimCounter.release();
       for (cudaEvent_t e : chunkIn_) cudaEventDestroy(e);
       for (cudaEvent_t e : waveDone_) cudaEventDestroy(e);
       for (WavePlan& w : wavePlans_) w.jobs.release();
@@ -797,15 +796,18 @@ class VideoFrameTransform {
       cudaEvent_t frameFork_ = slot.fork;
       const DevicePlan* plans[kPlaneLanes];
       bool sideWork = false;  // does any chroma plane have work before its gather (low-pass, pre-fill)?
-      bool anyTransparent = false;
       for (int p = 0; p < numPlanes; ++p) {
         if (!(plans[p] = findPlan(p ? 1 : 0, p))) return false;
         if (p) sideWork = sideWork || plans[p]->lowPass || plans[p]->transparent;
-        anyTransparent = anyTransparent || plans[p]->transparent;
       }
       // Low-pass of all planes in one launch per vertical kernel size when every plane takes the strip kernel only
-      const bool mergedBlur = !anyTransparent && blurFrame(plans, numPlanes, dIn, inW, inH, inPitch, lanes_, s);
-      if (mergedBlur) sideWork = false;
+      const t360::BlurLists* lists[kPlaneLanes];
+      for (int p = 0; p < numPlanes; ++p) lists[p] = &plans[p]->blur.lists;
+      const bool mergedBlur = mergeable(plans, lists, numPlanes, inW, inH);
+      if (mergedBlur) {
+        blurFrame(plans, numPlanes, dIn, inW, inH, inPitch, lanes_, s);
+        sideWork = false;
+      }
       // Stage 1, planes side by side (chroma on its own lanes): everything before the gather.
       const bool fork = numPlanes > 1 && sideWork;
       if (fork) CU(cudaEventRecord(frameFork_, s));
@@ -987,8 +989,9 @@ class VideoFrameTransform {
     auto it = plans_.find(planIndex);
     if (it == plans_.end()) return false;
     counts[0] = it->second.numStaged; counts[1] = it->second.numBorder;
-    counts[2] = it->second.blur.numStripJobs[0] + it->second.blur.numStripJobs[1] + it->second.blur.numStripJobs[2];
-    counts[3] = it->second.blur.numTileJobs + it->second.blur.numDirectJobs;
+    const t360::BlurLayout& b = it->second.blur.layout;
+    counts[2] = b.numStrips[0] + b.numStrips[1] + b.numStrips[2];
+    counts[3] = b.numTiles + b.numDirect;
     return true;
   }
   size_t planBytes(int planIndex) {
@@ -1139,7 +1142,7 @@ class VideoFrameTransform {
     if (d.lowPass) {
       d.segments = h.segments;
       d.planTaps = h.taps;
-      buildBlurJobs(d.segments, d.planTaps, h.inW, h.inH, d.stereoFormat, d.blur);
+      buildBlurSet(d.segments, d.planTaps, h.inW, h.inH, d.stereoFormat, d.blur);
     }
     d.resizeNeeded = h.resize.needed;
     if (d.resizeNeeded) resizeFor(d, d.outW, d.outH);
@@ -1189,160 +1192,16 @@ class VideoFrameTransform {
     return d;
   }
 
-  // Tiles of the plan, applied once (mono) or to both halves of a stereo frame (reference cpp:630-691), cut
-  // into CTA-sized jobs.  Segments that do not fit the plane are dropped, like the reference's caught cv::Exception.
-  // Host half: the job lists.  *needsClear (if asked for): whether some pixel of the plane lies under no segment -- it
-  // depends on the plane size and the segment rectangles only, not on the view.
-  static void buildBlurLists(const std::vector<t360::LowPassSegment>& segments, const std::vector<float>& planTaps, int planeW, int planeH,
-                             int stereoFormat, BlurLists& out, bool* needsClear) {
-    struct { const std::vector<t360::LowPassSegment>& segments; const std::vector<float>& taps; int inW, inH; } h{segments, planTaps, planeW, planeH};
-    std::vector<BlurJob>& tiles = out.tiles;
-    std::vector<BlurJob>& direct = out.direct;
-    std::vector<StripJob>* strips = out.strips;
-    for (auto& v : out.strips) v.clear();
-    tiles.clear();
-    direct.clear();
-    std::vector<float>& taps = out.taps;
-    std::vector<int>& source = out.tapSource;
-    taps = h.taps;  // original taps first (offsets of the plan stay valid), padded copies appended
-    source.resize(taps.size());
-    for (size_t i = 0; i < source.size(); ++i) source[i] = static_cast<int>(i) + 1;
-    int offX[2] = {0, 0}, offY[2] = {0, 0}, passes = 1;
-    if (stereoFormat == STEREO_FORMAT_LR) { passes = 2; offX[1] = static_cast<int>(0.5 * h.inW); }
-    else if (stereoFormat == STEREO_FORMAT_TB) { passes = 2; offY[1] = static_cast<int>(0.5 * h.inH); }
-    std::vector<uint8_t> covered(needsClear ? static_cast<size_t>(h.inW) * h.inH : 0, 0);
-    int tileSmem = 0;
-    // a warp-job covers 256 columns x `rows` rows; keep the grid at several thousand warps even for small planes
-    const long long stripsPerRow = (h.inW + t360::kStripW - 1) / t360::kStripW;
-    // (each job recomputes 2*hy rows of horizontal sums at its top and bottom, so never fewer than 8 rows)
-    const long long wanted = static_cast<long long>(h.inH) * stripsPerRow / 5000;
-    const int rowsBudget = wanted >= 32 ? 32 : (wanted >= 16 ? 16 : 8);
-
-    auto sameTaps = [&](int offA, int nA, int offB, int nB) {
-      return nA == nB && (offA == offB || std::memcmp(&h.taps[offA], &h.taps[offB], sizeof(float) * nA) == 0);
-    };
-    // horizontal taps zero-padded to whole chunks of 4 at a 16-byte aligned offset (fma(0, p, s) == s exactly)
-    std::map<std::pair<int, int>, std::pair<int, int>> paddedKx;
-    auto padKx = [&](int off, int n) {
-      auto it = paddedKx.find({off, n});
-      if (it != paddedKx.end()) return it->second;
-      while (taps.size() % 4) { taps.push_back(0.f); source.push_back(0); }
-      const int at = static_cast<int>(taps.size()), chunks = (n + 3) / 4;
-      for (int i = 0; i < chunks * 4; ++i) {
-        taps.push_back(i < n ? h.taps[off + i] : 0.f);
-        source.push_back(i < n ? off + i + 1 : 0);
-      }
-      return paddedKx[{off, n}] = std::make_pair(at, chunks);
-    };
-    std::map<int, int> paddedKy1;  // a single vertical tap k becomes {0, k, 0}
-    auto padKy = [&](int off, int n) {
-      if (n != 1) return off;
-      auto it = paddedKy1.find(off);
-      if (it != paddedKy1.end()) return it->second;
-      const int at = static_cast<int>(taps.size());
-      taps.push_back(0.f); taps.push_back(h.taps[off]); taps.push_back(0.f);
-      source.push_back(0); source.push_back(off + 1); source.push_back(0);
-      return paddedKy1[off] = at;
-    };
-
-    for (int pass = 0; pass < passes; ++pass) {
-      // segments of one band that are horizontally adjacent and carry bit-identical kernels (always the case when
-      // the view-dependent scale is 1, e.g. no off-centre projection) are merged into one wide segment
-      // a segment that does not fit the plane is dropped, like the reference's caught cv::Exception (cpp:183-203) -- each
-      // one on its own, before any merging
-      auto fits = [&](const t360::LowPassSegment& g) {
-        const int l = g.left + offX[pass], t = g.top + offY[pass];
-        return l >= 0 && t >= 0 && g.width > 0 && g.height > 0 && l + g.width <= h.inW && t + g.height <= h.inH;
-      };
-      size_t i = 0;
-      while (i < h.segments.size()) {
-        t360::LowPassSegment s = h.segments[i];
-        size_t j = i + 1;
-        if (!fits(s)) { i = j; continue; }
-        while (j < h.segments.size()) {
-          const t360::LowPassSegment& n = h.segments[j];
-          if (n.top != s.top || n.height != s.height || n.left != s.left + s.width || !fits(n) ||
-              !sameTaps(n.kxOffset, n.kxCount, s.kxOffset, s.kxCount) || !sameTaps(n.kyOffset, n.kyCount, s.kyOffset, s.kyCount))
-            break;
-          s.width += n.width;
-          ++j;
-        }
-        i = j;
-        const int left = s.left + offX[pass], top = s.top + offY[pass];
-        if (needsClear)
-          for (int y = 0; y < s.height; ++y) std::memset(&covered[static_cast<size_t>(top + y) * h.inW + left], 1, s.width);
-        const int hy = s.kyCount / 2;
-        if (hy <= t360::kStripMaxHy && (s.kyCount & 1) && (s.kxCount & 1)) {
-          const auto kx = padKx(s.kxOffset, s.kxCount);
-          const int kyOff = padKy(s.kyOffset, s.kyCount), hx = s.kxCount / 2;
-          const int rows = std::min(rowsBudget, kx.second <= 3 ? 32 : (kx.second <= 8 ? 16 : 8));
-          for (int ty = 0; ty < s.height; ty += rows)
-            for (int tx = 0; tx < s.width; tx += t360::kStripW) {
-              StripJob j{left + tx, top + ty, std::min(t360::kStripW, s.width - tx), std::min(rows, s.height - ty),
-                         kx.first, kx.second, s.kxCount, kyOff, 0};
-              // interior strips read whole aligned words: first byte - 3 and the last prefetched group must stay in the row
-              const int firstByte = j.x0 - hx, lastByte = j.x0 + t360::kStripW - t360::kStripLanePx - hx + 4 * (kx.second + 3) + 7;
-              j.edge = (firstByte - 4 < 0 || lastByte >= h.inW) ? 1 : 0;
-              strips[std::max(hy, 1) - 1].push_back(j);
-            }
-        } else {
-          for (int ty = 0; ty < s.height; ty += t360::kBlurTileH)
-            for (int tx = 0; tx < s.width; tx += t360::kBlurTileW) {
-              BlurJob j{left + tx, top + ty, std::min(t360::kBlurTileW, s.width - tx), std::min(t360::kBlurTileH, s.height - ty),
-                        s.kxOffset, s.kxCount, s.kyOffset, s.kyCount};
-              const long long need = static_cast<long long>(t360::blurTileSmem(j.w, j.h, j.kxCount, j.kyCount));
-              if (need <= t360::kBlurMaxSmem) {
-                tiles.push_back(j);
-                tileSmem = std::max(tileSmem, static_cast<int>(need));
-              } else {
-                direct.push_back(j);
-              }
-            }
-        }
-      }
-    }
-    if (needsClear) *needsClear = std::find(covered.begin(), covered.end(), 0) != covered.end();
-    for (int c = 0; c < t360::kStripMaxHy; ++c)
-      // heaviest jobs first: the hardware block scheduler then balances the tail
-      std::stable_sort(strips[c].begin(), strips[c].end(), [](const StripJob& a, const StripJob& b) {
-        return static_cast<long long>(a.kxChunks + 2) * a.h * (1 + 3 * a.edge) > static_cast<long long>(b.kxChunks + 2) * b.h * (1 + 3 * b.edge);
-      });
-    out.tileSmem = tileSmem;
-  }
-
-  // ... and the device half: the lists of one plane size uploaded once (plan generation, or the first use of a size)
-  void buildBlurJobs(const std::vector<t360::LowPassSegment>& segments, const std::vector<float>& planTaps, int planeW, int planeH,
-                     int stereoFormat, DevicePlan::BlurSet& d) {
-    BlurLists lists;
-    buildBlurLists(segments, planTaps, planeW, planeH, stereoFormat, lists, &d.needsClear);
-    const std::vector<StripJob>* strips = lists.strips;
-    const std::vector<BlurJob>& tiles = lists.tiles;
-    const std::vector<BlurJob>& direct = lists.direct;
-    const std::vector<float>& taps = lists.taps;
-    const int tileSmem = lists.tileSmem;
-    for (int c = 0; c < t360::kStripMaxHy; ++c) {
-      d.numStripJobs[c] = static_cast<int>(strips[c].size());
-      d.hostStrips[c] = strips[c];
-      if (strips[c].empty()) continue;
-      d.stripJobs[c].reserve(strips[c].size());
-      CU(cudaMemcpy(d.stripJobs[c].ptr, strips[c].data(), strips[c].size() * sizeof(StripJob), cudaMemcpyHostToDevice));
-    }
-    d.numTileJobs = static_cast<int>(tiles.size());
-    d.numDirectJobs = static_cast<int>(direct.size());
-    d.tileSmem = tileSmem;
-    if (!tiles.empty()) {
-      d.tileJobs.reserve(tiles.size());
-      CU(cudaMemcpy(d.tileJobs.ptr, tiles.data(), tiles.size() * sizeof(BlurJob), cudaMemcpyHostToDevice));
-    }
-    if (!direct.empty()) {
-      d.directJobs.reserve(direct.size());
-      CU(cudaMemcpy(d.directJobs.ptr, direct.data(), direct.size() * sizeof(BlurJob), cudaMemcpyHostToDevice));
-    }
-    d.hostTaps = taps;
-    if (!taps.empty()) {
-      d.taps.reserve(taps.size());
-      CU(cudaMemcpy(d.taps.ptr, taps.data(), taps.size() * sizeof(float), cudaMemcpyHostToDevice));
-    }
+  // The low-pass lists of one plane size: cut on the host, packed into one image, uploaded once (plan generation, or the
+  // first use of a size)
+  void buildBlurSet(const std::vector<t360::LowPassSegment>& segments, const std::vector<float>& planTaps, int planeW, int planeH,
+                    int stereoFormat, DevicePlan::BlurSet& d) {
+    t360::buildBlurLists(segments, planTaps, planeW, planeH, stereoFormat, d.lists, &d.needsClear);
+    std::vector<uint8_t> image;
+    d.layout = t360::packBlurLists(d.lists, image, image);
+    if (image.empty()) return;
+    d.image.reserve(image.size());
+    CU(cudaMemcpy(d.image.ptr, image.data(), image.size(), cudaMemcpyHostToDevice));
   }
 
   // the low-pass jobs of a plan for planes of w x h (the planned size, or whatever the caller passes)
@@ -1352,26 +1211,43 @@ class VideoFrameTransform {
     auto it = plan.otherBlurs.find({w, h});
     if (it != plan.otherBlurs.end()) return it->second;
     DevicePlan::BlurSet& set = plan.otherBlurs[{w, h}];
-    buildBlurJobs(plan.segments, plan.planTaps, w, h, plan.stereoFormat, set);
+    buildBlurSet(plan.segments, plan.planTaps, w, h, plan.stereoFormat, set);
     return set;
+  }
+
+  // The low-pass of planes fp.plane[0 .. numPlanes) from one packed list (its arrays at `jobs` / `taps` + the layout's
+  // offsets): the strip jobs of every plane in one launch per vertical half-size (a job's plane is in its `edge`), then
+  // the tile and direct jobs, which only a single plane's list has.  clear: zero the planes first (reference cpp:625:
+  // Mat::zeros under dropped segments).
+  void launchLowPass(const t360::BlurLayout& l, bool clear, const uint8_t* jobs, const uint8_t* taps, t360::FrameStripParams fp, int numPlanes,
+                     cudaStream_t s) {
+    const t360::FrameStripParams::Plane& a = fp.plane[0];
+    if (clear)
+      for (int p = 0; p < numPlanes; ++p) CU(cudaMemset2DAsync(fp.plane[p].dst, fp.plane[p].dstPitch, 0, fp.plane[p].width, fp.plane[p].height, s));
+    fp.numPlanes = numPlanes;
+    fp.taps = reinterpret_cast<const float*>(taps + l.tapAt);
+    for (int c = 0; c < t360::kStripMaxHy; ++c) {
+      if (!l.numStrips[c]) continue;
+      fp.jobs = reinterpret_cast<const StripJob*>(jobs + l.stripAt[c]);
+      fp.numJobs = l.numStrips[c];
+      CU(t360::launchBlurFrameStrips(fp, c + 1, s));
+    }
+    t360::BlurParams bp{a.src, a.dst, a.width, a.height, a.srcPitch, a.dstPitch, reinterpret_cast<const BlurJob*>(jobs + l.tileAt), l.numTiles,
+                        fp.taps, l.tileSmem};
+    if (bp.numJobs) CU(t360::launchBlur(bp, s));
+    if (l.numDirect) {
+      bp.jobs = reinterpret_cast<const BlurJob*>(jobs + l.directAt);
+      bp.numJobs = l.numDirect;
+      CU(t360::launchBlurDirect(bp, s));
+    }
   }
 
   void runLowPass(const DevicePlan& plan, const uint8_t* dIn, uint8_t* dOut, int w, int h, int inPitch, int outPitch,
                   cudaStream_t s) {
     const DevicePlan::BlurSet& b = blurFor(plan, w, h);
-    if (b.needsClear) CU(cudaMemset2DAsync(dOut, outPitch, 0, w, h, s));  // reference cpp:625: Mat::zeros under dropped segments
-    for (int c = 0; c < t360::kStripMaxHy; ++c) {
-      if (!b.numStripJobs[c]) continue;
-      t360::StripParams sp{dIn, dOut, w, h, inPitch, outPitch, b.stripJobs[c].ptr, b.numStripJobs[c], b.taps.ptr};
-      CU(t360::launchBlurStrips(sp, c + 1, s));
-    }
-    t360::BlurParams bp{dIn, dOut, w, h, inPitch, outPitch, b.tileJobs.ptr, b.numTileJobs, b.taps.ptr, b.tileSmem};
-    if (b.numTileJobs) CU(t360::launchBlur(bp, s));
-    if (b.numDirectJobs) {
-      bp.jobs = b.directJobs.ptr;
-      bp.numJobs = b.numDirectJobs;
-      CU(t360::launchBlurDirect(bp, s));
-    }
+    t360::FrameStripParams fp{};
+    fp.plane[0] = {dIn, dOut, w, h, inPitch, outPitch};
+    launchLowPass(b.layout, b.needsClear, b.image.ptr, b.image.ptr, fp, 1, s);
   }
 
   // the tensor maps of a source plane, from the lane's cache or freshly encoded (false: not TMA-describable)
@@ -1479,66 +1355,17 @@ class VideoFrameTransform {
     }
   }
 
-  // The low-pass of all planes of a frame: one launch per vertical kernel half-size.  false: not applicable (a plane
-  // without low-pass, of another size than planned, or with segments the strip kernel cannot take) -- per-plane launches.
-  bool blurFrame(const DevicePlan* const* plans, int numPlanes, const uint8_t* const* dIn, const int* inW, const int* inH, const int* inPitch,
+  // The low-pass of all planes of a frame (mergeable): one launch per vertical kernel half-size.
+  void blurFrame(const DevicePlan* const* plans, int numPlanes, const uint8_t* const* dIn, const int* inW, const int* inH, const int* inPitch,
                  PlaneLane* lanes, cudaStream_t s) {
-    if (numPlanes < 2) return false;
-    for (int p = 0; p < numPlanes; ++p) {
-      const DevicePlan& plan = *plans[p];
-      if (!plan.lowPass || inW[p] != plan.inW || inH[p] != plan.inH || plan.blur.numTileJobs || plan.blur.numDirectJobs || plan.blur.needsClear)
-        return false;
-    }
-    FrameBlurList& f = frameBlur_;
-    {
-      std::lock_guard<std::mutex> lock(frameJobsMu_);
-      if (f.generation != planGeneration_ || f.numPlanes != numPlanes) {
-        std::vector<StripJob> merged[t360::kStripMaxHy];
-        std::vector<float> taps;
-        for (int p = 0; p < numPlanes; ++p) {
-          const DevicePlan::BlurSet& b = plans[p]->blur;
-          while (taps.size() % 4) taps.push_back(0.f);  // (the padded horizontal taps stay 16-byte aligned)
-          const int base = static_cast<int>(taps.size());
-          taps.insert(taps.end(), b.hostTaps.begin(), b.hostTaps.end());
-          for (int c = 0; c < t360::kStripMaxHy; ++c)
-            for (StripJob j : b.hostStrips[c]) {
-              j.kxOffset += base;
-              j.kyOffset += base;
-              j.edge |= p << t360::kStripPlaneShift;
-              merged[c].push_back(j);
-            }
-        }
-        CU(cudaDeviceSynchronize());  // a previous frame may still be reading the old lists
-        for (int c = 0; c < t360::kStripMaxHy; ++c) {
-          // heaviest jobs first: the hardware block scheduler then balances the tail
-          std::stable_sort(merged[c].begin(), merged[c].end(), [](const StripJob& a, const StripJob& b) {
-            return static_cast<long long>(a.kxChunks + 2) * a.h * (1 + 3 * (a.edge & 1)) > static_cast<long long>(b.kxChunks + 2) * b.h * (1 + 3 * (b.edge & 1));
-          });
-          f.numJobs[c] = static_cast<int>(merged[c].size());
-          if (merged[c].empty()) continue;
-          f.jobs[c].reserve(merged[c].size());
-          CU(cudaMemcpy(f.jobs[c].ptr, merged[c].data(), merged[c].size() * sizeof(StripJob), cudaMemcpyHostToDevice));
-        }
-        f.taps.reserve(std::max<size_t>(taps.size(), 4));
-        CU(cudaMemcpy(f.taps.ptr, taps.data(), taps.size() * sizeof(float), cudaMemcpyHostToDevice));
-        f.numPlanes = numPlanes;
-        f.generation = planGeneration_;
-      }
-    }
+    const FrameListRefs f = frameLists(plans, numPlanes);
     t360::FrameStripParams fp{};
     for (int p = 0; p < numPlanes; ++p) {
       const int bp = alignedPitch(inW[p]);
       lanes[p].blurred.reserve(static_cast<size_t>(bp) * inH[p] + 64);
       fp.plane[p] = {dIn[p], lanes[p].blurred.ptr, inW[p], inH[p], inPitch[p], bp};
     }
-    fp.taps = f.taps.ptr;
-    for (int c = 0; c < t360::kStripMaxHy; ++c) {
-      if (!f.numJobs[c]) continue;
-      fp.jobs = f.jobs[c].ptr;
-      fp.numJobs = f.numJobs[c];
-      CU(t360::launchBlurFrameStrips(fp, c + 1, s));
-    }
-    return true;
+    launchLowPass(f.blurLayout, false, f.blurImage, f.blurImage, fp, numPlanes, s);
   }
 
   // The low-pass of a per-view frame (transformFrameView): the segments and taps of every plan index for the view, the
@@ -1580,115 +1407,53 @@ class VideoFrameTransform {
       float* t = reinterpret_cast<float*>(taps.data());
       for (size_t i = 0; i < c.tapCodes.size(); ++i) {
         const int code = c.tapCodes[i];
-        t[i] = code ? h[code >> 28].taps[(code & ((1 << 28) - 1)) - 1] : 0.f;
+        t[i] = code ? h[(code >> t360::kTapPlaneShift) ? 1 : 0].taps[(code & ((1 << t360::kTapPlaneShift) - 1)) - 1] : 0.f;
       }
     } else {
       c = ViewBlurCache{};
-      BlurLists lists[2];
+      t360::BlurLists lists[2];
       for (int idx = 0; idx < indices; ++idx)  // (coverage: plan.blur.needsClear, computed once per plan)
-        buildBlurLists(h[idx].segments, h[idx].taps, plans[idx]->inW, plans[idx]->inH, plans[idx]->stereoFormat, lists[idx], nullptr);
-      c.merged = numPlanes > 1;
-      for (int p = 0; p < numPlanes && c.merged; ++p) {
-        const BlurLists& l = lists[p ? 1 : 0];
-        c.merged = l.tiles.empty() && l.direct.empty() && !plans[p]->blur.needsClear;
-      }
-      // one byte image of the jobs and one of the taps (with the provenance of every tap), 16-byte aligned arrays
-      std::vector<uint8_t> codes;
-      auto append = [](std::vector<uint8_t>& blob, const void* data, size_t bytes) {
-        blob.resize((blob.size() + 15) & ~size_t(15));
-        const size_t at = blob.size();
-        blob.insert(blob.end(), static_cast<const uint8_t*>(data), static_cast<const uint8_t*>(data) + bytes);
-        return at;
+        t360::buildBlurLists(h[idx].segments, h[idx].taps, plans[idx]->inW, plans[idx]->inH, plans[idx]->stereoFormat, lists[idx], nullptr);
+      const t360::BlurLists* perPlane[kPlaneLanes];
+      for (int p = 0; p < numPlanes; ++p) perPlane[p] = &lists[p ? 1 : 0];
+      c.merged = mergeable(plans, perPlane, numPlanes, inW, inH);
+      // one byte image of the jobs and one of the taps, with the provenance of every tap (tapSource; in a merged list it
+      // carries the plane already)
+      auto appendCodes = [&](const t360::BlurLists& l, const t360::BlurLayout& at, int plane) {
+        c.tapCodes.resize(taps.size() / sizeof(float), 0);
+        for (size_t i = 0; i < l.tapSource.size(); ++i)
+          c.tapCodes[at.tapAt / sizeof(float) + i] = l.tapSource[i] ? (plane << t360::kTapPlaneShift) | l.tapSource[i] : 0;
       };
-      auto appendTaps = [&](const BlurLists& l, int idx) {
-        std::vector<int> code(l.tapSource.size());
-        for (size_t i = 0; i < code.size(); ++i) code[i] = l.tapSource[i] ? (idx << 28) | l.tapSource[i] : 0;
-        append(codes, code.data(), code.size() * sizeof(int));
-        return append(taps, l.taps.data(), l.taps.size() * sizeof(float));
-      };
-      if (c.merged) {  // (as blurFrame: the planes' strip jobs with the plane in `edge`, one tap buffer, heaviest jobs first)
-        std::vector<StripJob> all[t360::kStripMaxHy];
-        for (int p = 0; p < numPlanes; ++p) {
-          const BlurLists& l = lists[p ? 1 : 0];
-          const int base = static_cast<int>(appendTaps(l, p ? 1 : 0) / sizeof(float));
-          if (p == 0) c.tapAt[0] = 0;
-          for (int k = 0; k < t360::kStripMaxHy; ++k)
-            for (StripJob j : l.strips[k]) {
-              j.kxOffset += base;
-              j.kyOffset += base;
-              j.edge |= p << t360::kStripPlaneShift;
-              all[k].push_back(j);
-            }
-        }
-        for (int k = 0; k < t360::kStripMaxHy; ++k) {
-          std::stable_sort(all[k].begin(), all[k].end(), [](const StripJob& a, const StripJob& b) {
-            return static_cast<long long>(a.kxChunks + 2) * a.h * (1 + 3 * (a.edge & 1)) > static_cast<long long>(b.kxChunks + 2) * b.h * (1 + 3 * (b.edge & 1));
-          });
-          c.numStrips[0][k] = static_cast<int>(all[k].size());
-          c.stripAt[0][k] = append(c.jobs, all[k].data(), all[k].size() * sizeof(StripJob));
-        }
+      if (c.merged) {
+        const t360::BlurLists all = t360::mergeBlurLists(perPlane, numPlanes);
+        c.layout[0] = t360::packBlurLists(all, c.jobs, taps);
+        appendCodes(all, c.layout[0], 0);
       } else {
         for (int idx = 0; idx < indices; ++idx) {
-          const BlurLists& l = lists[idx];
-          for (int k = 0; k < t360::kStripMaxHy; ++k) {
-            c.numStrips[idx][k] = static_cast<int>(l.strips[k].size());
-            c.stripAt[idx][k] = append(c.jobs, l.strips[k].data(), l.strips[k].size() * sizeof(StripJob));
-          }
-          c.numTiles[idx] = static_cast<int>(l.tiles.size());
-          c.tileAt[idx] = append(c.jobs, l.tiles.data(), l.tiles.size() * sizeof(BlurJob));
-          c.numDirect[idx] = static_cast<int>(l.direct.size());
-          c.directAt[idx] = append(c.jobs, l.direct.data(), l.direct.size() * sizeof(BlurJob));
-          c.tileSmem[idx] = l.tileSmem;
-          c.tapAt[idx] = appendTaps(l, idx);
+          c.layout[idx] = t360::packBlurLists(lists[idx], c.jobs, taps);
+          appendCodes(lists[idx], c.layout[idx], idx);
         }
       }
-      codes.resize(taps.size());  // (trailing alignment)
-      c.tapCodes.assign(reinterpret_cast<const int*>(codes.data()), reinterpret_cast<const int*>(codes.data()) + codes.size() / sizeof(int));
       c.key = std::move(key);
     }
-    const std::vector<uint8_t>& jobs = c.jobs;
-    const bool merged = c.merged;
-    const auto& stripAt = c.stripAt;
-    const auto& numStrips = c.numStrips;
     UploadRing::Entry* used[2];
-    const uint8_t* dJobs = stageUpload(slot.viewJobs, jobs, s, &used[0]);
+    const uint8_t* dJobs = stageUpload(slot.viewJobs, c.jobs, s, &used[0]);
     const uint8_t* dTaps = stageUpload(slot.viewTaps, taps, s, &used[1]);
+    t360::FrameStripParams fp{};
     for (int p = 0; p < numPlanes; ++p) {
       const int bp = alignedPitch(inW[p]);
       slot.lanes[p].blurred.reserve(static_cast<size_t>(bp) * inH[p] + 64);
       src[p] = slot.lanes[p].blurred.ptr;
       srcPitch[p] = bp;
+      fp.plane[p] = {dIn[p], slot.lanes[p].blurred.ptr, inW[p], inH[p], inPitch[p], bp};
     }
-    if (merged) {
-      t360::FrameStripParams fp{};
-      for (int p = 0; p < numPlanes; ++p) fp.plane[p] = {dIn[p], slot.lanes[p].blurred.ptr, inW[p], inH[p], inPitch[p], srcPitch[p]};
-      fp.taps = reinterpret_cast<const float*>(dTaps + c.tapAt[0]);
-      for (int c = 0; c < t360::kStripMaxHy; ++c) {
-        if (!numStrips[0][c]) continue;
-        fp.jobs = reinterpret_cast<const StripJob*>(dJobs + stripAt[0][c]);
-        fp.numJobs = numStrips[0][c];
-        CU(t360::launchBlurFrameStrips(fp, c + 1, s));
-      }
+    if (c.merged) {
+      launchLowPass(c.layout[0], false, dJobs, dTaps, fp, numPlanes, s);
     } else {
       for (int p = 0; p < numPlanes; ++p) {
-        const int idx = p ? 1 : 0;
-        uint8_t* dst = slot.lanes[p].blurred.ptr;
-        const float* dt = reinterpret_cast<const float*>(dTaps + c.tapAt[idx]);
-        if (plans[p]->blur.needsClear) CU(cudaMemset2DAsync(dst, srcPitch[p], 0, inW[p], inH[p], s));  // reference cpp:625
-        for (int c = 0; c < t360::kStripMaxHy; ++c) {
-          if (!numStrips[idx][c]) continue;
-          t360::StripParams sp{dIn[p], dst, inW[p], inH[p], inPitch[p], srcPitch[p], reinterpret_cast<const StripJob*>(dJobs + stripAt[idx][c]),
-                               numStrips[idx][c], dt};
-          CU(t360::launchBlurStrips(sp, c + 1, s));
-        }
-        t360::BlurParams bp{dIn[p], dst, inW[p], inH[p], inPitch[p], srcPitch[p], reinterpret_cast<const BlurJob*>(dJobs + c.tileAt[idx]),
-                            c.numTiles[idx], dt, c.tileSmem[idx]};
-        if (bp.numJobs) CU(t360::launchBlur(bp, s));
-        if (c.numDirect[idx]) {
-          bp.jobs = reinterpret_cast<const BlurJob*>(dJobs + c.directAt[idx]);
-          bp.numJobs = c.numDirect[idx];
-          CU(t360::launchBlurDirect(bp, s));
-        }
+        t360::FrameStripParams one{};
+        one.plane[0] = fp.plane[p];
+        launchLowPass(c.layout[p ? 1 : 0], plans[p]->blur.needsClear, dJobs, dTaps, one, 1, s);
       }
     }
     for (UploadRing::Entry* e : used) {  // the entries may be refilled once these launches have finished
@@ -1732,27 +1497,41 @@ class VideoFrameTransform {
     return e.device;
   }
 
-  // The gathers of all planes of a frame as ONE launch (every plane staged).
-  void gatherFrame(const GatherWork* work, int numPlanes, cudaStream_t s, StreamSlot& slot) {
-    FrameJobList& f = frameJobs_;
-    std::unique_lock<std::mutex> listLock(frameJobsMu_);
-    if (f.generation != planGeneration_ || f.numPlanes != numPlanes) {
-      std::vector<GatherJob> merged;
-      for (int p = 0; p < numPlanes; ++p)
-        for (GatherJob t : work[p].plan->hostJobs) {
+  // The merged lists of a frame of numPlanes (2 or 3) planes, built on first use in a plan generation.  A rebuild waits for
+  // the device: frames of the previous generation may still read the entry's buffers.
+  FrameListRefs frameLists(const DevicePlan* const* plans, int numPlanes) {
+    std::lock_guard<std::mutex> lock(frameListsMu_);
+    FrameLists& f = frameLists_[numPlanes - 2];
+    if (f.generation != planGeneration_) {
+      std::vector<GatherJob> jobs;
+      const t360::BlurLists* lists[kPlaneLanes];
+      for (int p = 0; p < numPlanes; ++p) {
+        for (GatherJob t : plans[p]->hostJobs) {
           t.outY |= p << t360::kJobPlaneShift;
-          merged.push_back(t);
+          jobs.push_back(t);
         }
-      std::stable_sort(merged.begin(), merged.end(),
-                       [](const GatherJob& a, const GatherJob& b) { return t360::jobLaunchRank(a) < t360::jobLaunchRank(b); });
-      CU(cudaDeviceSynchronize());  // a previous frame (on any stream) may still be reading the old list
-      f.tiles.reserve(merged.size());
-      CU(cudaMemcpy(f.tiles.ptr, merged.data(), merged.size() * sizeof(GatherJob), cudaMemcpyHostToDevice));
-      f.numTiles = static_cast<int>(merged.size());
-      f.numPlanes = numPlanes;
+        lists[p] = &plans[p]->blur.lists;
+      }
+      std::stable_sort(jobs.begin(), jobs.end(), [](const GatherJob& a, const GatherJob& b) { return t360::jobLaunchRank(a) < t360::jobLaunchRank(b); });
+      std::vector<uint8_t> image;
+      const t360::BlurLayout layout = t360::packBlurLists(t360::mergeBlurLists(lists, numPlanes), image, image);
+      if (f.generation != ~0ull) CU(cudaDeviceSynchronize());
+      f.gatherJobs.reserve(jobs.size());
+      if (!jobs.empty()) CU(cudaMemcpy(f.gatherJobs.ptr, jobs.data(), jobs.size() * sizeof(GatherJob), cudaMemcpyHostToDevice));
+      f.blurImage.reserve(image.size());
+      if (!image.empty()) CU(cudaMemcpy(f.blurImage.ptr, image.data(), image.size(), cudaMemcpyHostToDevice));
+      f.numGatherJobs = static_cast<int>(jobs.size());
+      f.blurLayout = layout;
       f.generation = planGeneration_;
     }
-    listLock.unlock();
+    return FrameListRefs{f.gatherJobs.ptr, f.numGatherJobs, f.blurImage.ptr, f.blurLayout};
+  }
+
+  // The gathers of all planes of a frame as ONE launch (every plane staged).
+  void gatherFrame(const GatherWork* work, int numPlanes, cudaStream_t s, StreamSlot& slot) {
+    const DevicePlan* plans[kPlaneLanes];
+    for (int p = 0; p < numPlanes; ++p) plans[p] = work[p].plan;
+    const FrameListRefs f = frameLists(plans, numPlanes);
     armScheduler(slot.frameClaim, s);
     t360::FrameGatherParams fp{};
     CUtensorMap maps[kPlaneLanes][t360::kNumBoxClasses][t360::kBoxVariants];
@@ -1767,7 +1546,7 @@ class VideoFrameTransform {
       trace_.reserve(static_cast<size_t>(numSMs_) * t360::gatherGroups(work[0].plan->kernelSize) * t360::kTraceJobsPerGroup * 4);
       CU(cudaMemsetAsync(trace_.ptr, 0, trace_.bytes(), s));
     }
-    t360::StagedParams jobs{f.tiles.ptr, f.numTiles, slot.frameClaim.ptr, traceEnabled_ ? trace_.ptr : nullptr};
+    t360::StagedParams jobs{f.gatherJobs, f.numGatherJobs, slot.frameClaim.ptr, traceEnabled_ ? trace_.ptr : nullptr};
     CU(t360::launchGatherFrame(fp, jobs, maps, numSMs_, s));
   }
 
@@ -1826,9 +1605,8 @@ class VideoFrameTransform {
   bool pinHostPlanes_ = false;
   std::mutex slotMu_;
   std::map<cudaStream_t, std::unique_ptr<StreamSlot>> slots_;
-  FrameJobList frameJobs_;
-  FrameBlurList frameBlur_;
-  std::mutex frameJobsMu_;
+  FrameLists frameLists_[kPlaneLanes - 1];  // frames of 2 and 3 planes
+  std::mutex frameListsMu_;
   DeviceBuffer<unsigned long long> trace_;
   bool traceEnabled_ = false;
   unsigned long long planGeneration_ = 0;
@@ -1867,6 +1645,7 @@ struct T360HostPlan {
   HostPlan plan;
   t360::GatherPlan gather;  // built on first use by T360B200_hostPlanGather
   bool gatherBuilt = false;
+  std::vector<uint8_t> blurImage;  // the last T360B200_hostPlanBlurLists image made with this plan first
 };
 
 T360_API T360HostPlan* T360B200_hostPlanCreate(const FrameTransformContext* ctx, int inW, int inH, int outW, int outH) {
@@ -1927,6 +1706,37 @@ T360_API int T360B200_hostPlanPoleCaps(T360HostPlan* plan, int info[4], const in
   if (capRecords) *capRecords = g.capRecords.empty() ? nullptr : g.capRecords.data();
   if (launchJobs) *launchJobs = g.launchJobs.empty() ? nullptr : reinterpret_cast<const int32_t*>(g.launchJobs.data());
   return 1;
+}
+T360_API int T360B200_hostPlanBlurLists(T360HostPlan* const* plans, int numPlans, int width, int height, int layout[15],
+                                        const uint8_t** image) {
+  if (!plans || numPlans < 1 || numPlans > t360::kMaxFramePlanes || !layout || !image) return 0;
+  for (int p = 0; p < numPlans; ++p)
+    if (!plans[p]) return 0;
+  try {
+    t360::BlurLists lists[t360::kMaxFramePlanes];
+    const t360::BlurLists* planes[t360::kMaxFramePlanes];
+    bool clear = false;
+    for (int p = 0; p < numPlans; ++p) {
+      const HostPlan& h = plans[p]->plan;
+      bool c = false;
+      t360::buildBlurLists(h.segments, h.taps, width > 0 ? width : h.inW, height > 0 ? height : h.inH, h.ctx.input_stereo_format, lists[p], &c);
+      clear = clear || c;
+      planes[p] = &lists[p];
+    }
+    std::vector<uint8_t>& img = plans[0]->blurImage;
+    img.clear();
+    const t360::BlurLayout l = t360::packBlurLists(numPlans > 1 ? t360::mergeBlurLists(planes, numPlans) : lists[0], img, img);
+    const long long v[15] = {l.numStrips[0], l.numStrips[1], l.numStrips[2], l.numTiles, l.numDirect, l.numTaps, l.tileSmem, clear,
+                             static_cast<long long>(l.stripAt[0]), static_cast<long long>(l.stripAt[1]), static_cast<long long>(l.stripAt[2]),
+                             static_cast<long long>(l.tileAt), static_cast<long long>(l.directAt), static_cast<long long>(l.tapAt),
+                             static_cast<long long>(img.size())};
+    for (int i = 0; i < 15; ++i) layout[i] = static_cast<int>(v[i]);
+    *image = img.data();
+    return 1;
+  } catch (const std::exception& ex) {
+    std::printf("Could not build the low-pass lists. Error: %s\n", ex.what());
+    return 0;
+  }
 }
 T360_API int T360B200_hostPlanSegment(const T360HostPlan* plan, int i, int rect[4], int numTaps[2], const float** kx,
                                       const float** ky) {

@@ -109,6 +109,8 @@ def load(path: os.PathLike | None = None):
     L.T360B200_hostPlanGather.restype = ci
     L.T360B200_hostPlanGather.argtypes = [vp, C.POINTER(ci), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]
     L.T360B200_hostPlanPoleCaps.restype = ci
+    L.T360B200_hostPlanBlurLists.restype = ci
+    L.T360B200_hostPlanBlurLists.argtypes = [vp, ci, ci, ci, C.POINTER(ci), C.POINTER(vp)]
     L.T360B200_hostPlanPoleCaps.argtypes = [vp, C.POINTER(ci), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]
     L.T360B200_weightImage.restype = ci
     L.T360B200_weightImage.argtypes = [ci, C.POINTER(vp)]
@@ -152,7 +154,7 @@ EXPORTED_SYMBOLS = [
     "VideoFrameTransform_new", "VideoFrameTransform_delete", "VideoFrameTransform_generateMapForPlane",
     "VideoFrameTransform_transformFramePlane", "T360B200_hostPlanCreate", "T360B200_hostPlanDestroy",
     "T360B200_hostPlanInfo", "T360B200_hostPlanMap", "T360B200_hostPlanSamples", "T360B200_hostPlanSegment",
-    "T360B200_hostPlanGather", "T360B200_hostPlanPoleCaps", "T360B200_weightImage", "T360B200_dealLanes",
+    "T360B200_hostPlanGather", "T360B200_hostPlanPoleCaps", "T360B200_hostPlanBlurLists", "T360B200_weightImage", "T360B200_dealLanes",
     "T360B200_remapTable", "T360B200_transformFramePlaneAsync", "T360B200_transformFrameAsync",
     "T360B200_lowPassPlaneAsync", "T360B200_reconfigure", "T360B200_transformFrameViewAsync", "T360B200_viewSamples",
     "T360B200_setPinHostPlanes", "T360B200_debugTrace", "T360B200_debugTraceRead", "T360B200_synchronize", "T360B200_stream", "T360B200_kernelLaunchCount", "T360B200_planDeviceBytes",
@@ -357,6 +359,22 @@ class HostPlan:
         as_jobs = lambda p, k: np.frombuffer((C.c_int32 * (k * 4)).from_address(p.value), np.int32).reshape(k, 4).copy() if k and p.value else np.zeros((0, 4), np.int32)
         records = np.frombuffer((C.c_uint32 * info[2]).from_address(recs.value), np.uint32).copy() if info[2] and recs.value else np.zeros(0, np.uint32)
         return dict(counts=dict(cap=info[0], border=info[1]), jobs=as_jobs(jobs, n), records=records, launch=as_jobs(launch, m))
+
+    def blur_lists(self, *others, width=0, height=0):
+        """The low-pass job lists of this plan -- merged with those of `others` (the other planes of a frame) when given --
+        for planes of width x height (0: the planned size), as the device holds them (T360B200_hostPlanBlurLists).  Returns
+        a dict: image (bytes), strips (3 arrays int32[n][9]: x0, y0, w, h, kxOffset, kxChunks, kxCount, kyOffset, edge),
+        tiles, direct (int32[n][8]: x0, y0, w, h, kxOffset, kxCount, kyOffset, kyCount), taps (float32), offsets (byte
+        offsets of strips 1..3, tiles, direct, taps), tile_smem, needs_clear."""
+        plans = (C.c_void_p * (1 + len(others)))(self._h, *[o._h for o in others])
+        lay, img = (C.c_int * 15)(), C.c_void_p()
+        if not self._lib.T360B200_hostPlanBlurLists(plans, len(plans), width, height, lay, C.byref(img)):
+            raise ValueError("T360B200_hostPlanBlurLists failed (message on stdout)")
+        image = C.string_at(img.value, lay[14]) if lay[14] else b""
+        arr = lambda at, n, cols, dt: np.frombuffer(image, dt, n * cols, at).reshape(n, cols).copy()
+        return dict(image=image, strips=[arr(lay[8 + c], lay[c], 9, np.int32) for c in range(3)], tiles=arr(lay[11], lay[3], 8, np.int32),
+                    direct=arr(lay[12], lay[4], 8, np.int32), taps=np.frombuffer(image, np.float32, lay[5], lay[13]).copy(),
+                    offsets=list(lay[8:14]), tile_smem=lay[6], needs_clear=bool(lay[7]))
 
     def segments(self):
         out = []
