@@ -125,6 +125,32 @@ int T360B200_transformFrameViewAsync(VideoFrameTransform* transform, const T360V
  * Returns 1 on success; 0 (message on stdout) for another layout, a non-finite view or invalid sizes. */
 int T360B200_viewSamples(const FrameTransformContext* ctx, const T360View* view, int inputWidth, int inputHeight,
                          int outputWidth, int outputHeight, int32_t* samples);
+/* An orientation, in degrees, as the context's fixed_yaw, fixed_pitch and fixed_roll. */
+typedef struct T360Orientation {
+  float yaw, pitch, roll;
+} T360Orientation;
+/* One frame of a CUBEMAP_32, CUBEMAP_23_OFFCENTER, EAC_32 or EQUIRECT transform (input EQUIRECT or CUBEMAP_32) with its own
+ * orientation, without re-planning: the arguments and the asynchronous contract of T360B200_transformFrameAsync, plus
+ * `orientation`.  The frame equals, bit for bit, what a fresh transform would give for the transform's current context
+ * with fixed_yaw, fixed_pitch and fixed_roll replaced by *orientation (low-pass and the INTER_AREA resize for scale factors
+ * != 1 included); the transform's context is not changed.  The gather computes every pixel's sampling position from the
+ * orientation in one launch for all planes; a low-pass is re-planned on the host for the orientation's yaw and pitch and
+ * its lists are uploaded in stream order from page-locked memory, as in T360B200_transformFrameViewAsync.  The call never
+ * synchronises the device, so the orientation may change every frame, and it is frame-exact against
+ * T360B200_reconfigure.  Returns 1 if everything was enqueued; 0 with a message on stdout for FLAT_FIXED (use
+ * T360B200_transformFrameViewAsync), BARREL or BARREL_SPLIT output, a non-finite orientation, a plan index that was never
+ * generated, or an input plane of another size than its map was generated for. */
+int T360B200_transformFrameOrientedAsync(VideoFrameTransform* transform, const T360Orientation* orientation, int numPlanes,
+                                         const uint8_t* const* deviceInputs, uint8_t* const* deviceOutputs,
+                                         const int* inputWidths, const int* inputHeights, const int* inputPitches,
+                                         const int* outputWidths, const int* outputHeights, const int* outputPitches,
+                                         void* cudaStream);
+/* Host only, no CUDA: the sampling records the per-frame orientation kernel computes for one plane of `ctx` with the
+ * orientation substituted, int32 [mapHeight][mapWidth][2] (map = scaled output size) in the format of
+ * T360B200_hostPlanSamples.  Returns 1 on success; 0 (message on stdout) for layouts without per-frame orientation, a
+ * non-finite orientation or invalid sizes. */
+int T360B200_orientedSamples(const FrameTransformContext* ctx, const T360Orientation* orientation, int inputWidth,
+                             int inputHeight, int outputWidth, int outputHeight, int32_t* samples);
 /* Opt-in (also: environment T360B200_PIN_HOST_PLANES=1): page-lock pageable caller planes in place the second time
  * the same buffer is seen (cudaHostRegister), so that recycled frame-pool buffers are DMA'd at full PCIe speed.  The
  * caller must keep such buffers alive until VideoFrameTransform_delete. */

@@ -22,6 +22,7 @@
 
 #include "flat_view.h"
 #include "host_plan.h"
+#include "oriented_view.h"
 
 namespace t360 {
 namespace {
@@ -55,17 +56,11 @@ constexpr FaceFrame kFrames23[6] = {
 class Projector {
  public:
   Projector(const FrameTransformContext& c, float inputPixelWidth) : c_(c), inPixW_(inputPixelWidth) {
-    // Euler angles are converted in double and stored as float (cpp:1233-1238).
-    const float s1 = static_cast<float>(std::sin(c.fixed_yaw * M_PI / 180.0f));
-    const float s2 = static_cast<float>(std::sin(c.fixed_pitch * M_PI / 180.0f));
-    const float s3 = static_cast<float>(std::sin(c.fixed_roll * M_PI / 180.0f));
-    const float c1 = static_cast<float>(std::cos(c.fixed_yaw * M_PI / 180.0f));
-    const float c2 = static_cast<float>(std::cos(c.fixed_pitch * M_PI / 180.0f));
-    const float c3 = static_cast<float>(std::cos(c.fixed_roll * M_PI / 180.0f));
-    // Coefficient groups exactly as parenthesised at cpp:1240-1244 (they are loop invariants there).
-    rxx_ = c1 * c3 + s1 * s2 * s3;  rxy_ = c3 * s1 * s2 - c1 * s3;  rxz_ = c2 * s1;
-    ryx_ = c2 * s3;                 ryy_ = c2 * c3;                 ryz_ = -s2;
-    rzx_ = c1 * s2 * s3 - c3 * s1;  rzy_ = c1 * c3 * s2 + s1 * s3;  rzz_ = c1 * c2;
+    // Euler angles -> rotation coefficients (cpp:1233-1244; oriented_view.h, shared with the per-frame orientation path)
+    const Rotation r = rotationFromAngles(c.fixed_yaw, c.fixed_pitch, c.fixed_roll);
+    rxx_ = r.xx; rxy_ = r.xy; rxz_ = r.xz;
+    ryx_ = r.yx; ryy_ = r.yy; ryz_ = r.yz;
+    rzx_ = r.zx; rzy_ = r.zy; rzz_ = r.zz;
     offCentre_ = std::abs(c.fixed_cube_offcenter_x) > kTiny || std::abs(c.fixed_cube_offcenter_y) > kTiny ||
                  std::abs(c.fixed_cube_offcenter_z) > kTiny;
     barrel_ = c.output_layout == LAYOUT_BARREL || c.output_layout == LAYOUT_BARREL_SPLIT;
@@ -139,10 +134,6 @@ class Projector {
                 f.origin.z + f.du.z * fx + f.dv.z * fy};  // cpp:1187-1189
   }
 
-  static float equiAngular(float t) {  // cpp:1074-1075: tan in double
-    return static_cast<float>(std::tan((t - 0.5f) * M_PI * 0.5f) * 0.5f + 0.5f);
-  }
-
   // Where the output pixel sits on the unit cube (or unit sphere); false = barrel dead zone.
   bool surfacePoint(float x, float y, Vec3& q) const {
     const float e = c_.expand_coef;
@@ -154,7 +145,7 @@ class Projector {
         // oracle/t360_oracle.c, such a pixel takes the last face's basis -- DESIGN.md 7.)
         const int row = static_cast<int>(y * 2), col = static_cast<int>(x * 3);
         float fx = x * 3.0f - col, fy = y * 2.0f - row;
-        if (c_.output_layout == LAYOUT_EAC_32) { fx = equiAngular(fx); fy = equiAngular(fy); }
+        if (c_.output_layout == LAYOUT_EAC_32) { fx = equiAngular(fx); fy = equiAngular(fy); }  // (tan in double: oriented_view.h)
         q = onCube(kFrames32, std::min(std::max(col + (1 - row) * 3, 0), 5), fx, fy);
         return true;
       }
@@ -164,7 +155,7 @@ class Projector {
         return true;
       }
       case LAYOUT_EQUIRECT:  // cpp:965-969
-        q = onSphere(static_cast<float>((2.0f * x - 1.0f) * M_PI), static_cast<float>((y - 0.5f) * M_PI));
+        q = onSphere(equirectYaw(x), equirectPitch(y));
         return true;
       case LAYOUT_BARREL: {  // cpp:970-982
         if (x <= 0.8f) {

@@ -6,6 +6,7 @@
 #include <cstdint>
 
 #include "flat_view.h"
+#include "oriented_view.h"
 
 namespace t360 {
 
@@ -341,6 +342,28 @@ struct ViewGatherParams {
 constexpr int kViewRowsPerThread = 8;
 __host__ __device__ constexpr int viewTileRows(int k) { return gatherThreads(k) / 32 * kViewRowsPerThread; }
 cudaError_t launchViewGather(ViewGatherParams p, int numSMs, cudaStream_t stream);
+
+// ---- the per-frame orientation gather (view_gather.cu) --------------------------------------------------------------
+// CUBEMAP_32, CUBEMAP_23_OFFCENTER, EAC_32 and EQUIRECT frames whose orientation (yaw, pitch, roll) is a launch parameter,
+// as its rotation coefficients: the kernel computes every pixel's sampling record (oriented_view.h), with the plan's
+// view-independent tables.  Same tiles, threads and taps as the per-view gather; BORDER_WRAP only.
+struct OrientedPlane {
+  const uint8_t* src;  // (blurred) input plane, geometry.inW x geometry.inH
+  uint8_t* dst;        // render target, geometry.mapW x geometry.mapH
+  int srcPitch, dstPitch;
+  SphereGeometry geometry;
+  const float* colTable;  // the plan's tables (buildSphereTables): column entries, then row entries (nullptr: none)
+  const float* rowTable;
+  int tilesX, firstTile;  // filled by launchOrientedGather
+};
+struct OrientedGatherParams {
+  OrientedPlane plane[kMaxFramePlanes];
+  int numPlanes;
+  Rotation rotation;
+  const int16_t* weights;  // device copy of the [1024][k][k] table (nullptr for nearest)
+  int kernelSize;
+};
+cudaError_t launchOrientedGather(OrientedGatherParams p, int numSMs, cudaStream_t stream);
 
 // bytes of dynamic shared memory a blur tile of (w x h) with the given tap counts needs
 inline int blurTileSmem(int w, int h, int nkx, int nky) {

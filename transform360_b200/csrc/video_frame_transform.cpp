@@ -115,6 +115,8 @@ struct DevicePlan {
   };
   bool resizeNeeded = false;  // for the size the map was generated for
   mutable std::map<std::pair<int, int>, Resize> resizes;
+  // the per-frame orientation path's view-independent tables (oriented_view.h: buildSphereTables), EAC_32 and EQUIRECT
+  DeviceBuffer<float> sphereTables;
   size_t deviceBytes() const {
     return samples.bytes() + records.bytes() + gatherJobs.bytes() + blur.image.bytes();
   }
@@ -966,6 +968,98 @@ class VideoFrameTransform {
     return false;
   }
 
+  // Whole frame of a CUBEMAP_32, CUBEMAP_23_OFFCENTER, EAC_32 or EQUIRECT transform with a per-frame orientation, device
+  // to device, asynchronous on `stream`: the frame a fresh transform would give for the context with fixed_yaw / pitch /
+  // roll replaced by `o`, with no re-plan.  The gather computes every sampling record from the rotation and the plan's
+  // tables (oriented_view.h); the low-pass, whose adjust_kernel taps depend on yaw and pitch, is re-planned on the host as
+  // in transformFrameView.  Nothing here synchronises the device, and the plans' sampling data is not read.
+  bool transformFrameOriented(const t360::Orientation& o, int numPlanes, const uint8_t* const* dIn, uint8_t* const* dOut, const int* inW,
+                              const int* inH, const int* inPitch, const int* outW, const int* outH, const int* outPitch, cudaStream_t stream) {
+    try {
+      if (numPlanes < 1 || numPlanes > kPlaneLanes) {
+        std::printf("Could not transform the frame with an orientation. Error: %d planes (1..%d supported)\n", numPlanes, kPlaneLanes);
+        return false;
+      }
+      if (!std::isfinite(o.yaw) || !std::isfinite(o.pitch) || !std::isfinite(o.roll)) {
+        std::printf("Could not transform the frame with an orientation. Error: the orientation (yaw %g, pitch %g, roll %g) is not finite\n",
+                    o.yaw, o.pitch, o.roll);
+        return false;
+      }
+      std::shared_lock<std::shared_mutex> config(configMu_);
+      if (!t360::orientedLayouts(ctx_)) {
+        std::printf("Could not transform the frame with an orientation. Error: per-frame orientations need output_layout CUBEMAP_32, "
+                    "CUBEMAP_23_OFFCENTER, EAC_32 or EQUIRECT and input_layout EQUIRECT or CUBEMAP_32, the transform has %d -> %d%s\n",
+                    static_cast<int>(ctx_.input_layout), static_cast<int>(ctx_.output_layout),
+                    ctx_.output_layout == LAYOUT_FLAT_FIXED ? " (FLAT_FIXED views: T360B200_transformFrameViewAsync)" : "");
+        return false;
+      }
+      FrameTransformContext ctx = ctx_;
+      ctx.fixed_yaw = o.yaw;
+      ctx.fixed_pitch = o.pitch;
+      ctx.fixed_roll = o.roll;
+      const DevicePlan* plans[kPlaneLanes];
+      for (int p = 0; p < numPlanes; ++p) {
+        if (!(plans[p] = findPlan(p ? 1 : 0, p))) return false;
+        if (inW[p] != plans[p]->inW || inH[p] != plans[p]->inH) {
+          std::printf("Could not transform the frame with an orientation. Error: input plane %d is %dx%d, its map was generated for %dx%d\n", p,
+                      inW[p], inH[p], plans[p]->inW, plans[p]->inH);
+          return false;
+        }
+        if (plans[p]->kernelSize == 0) {
+          std::printf("Could not transform the frame with an orientation. Error: no interpolation algorithm %d\n", ctx.interpolation_alg);
+          return false;
+        }
+      }
+      const DeviceRestore restoreDevice = ensureDevice();
+      cudaStream_t s = stream ? stream : stream_;
+      StreamSlot& slot = slotFor(s);
+      const uint8_t* src[kPlaneLanes];
+      int srcPitch[kPlaneLanes];
+      for (int p = 0; p < numPlanes; ++p) { src[p] = dIn[p]; srcPitch[p] = inPitch[p]; }
+      if (plans[0]->lowPass && !viewLowPass(ctx, plans, numPlanes, dIn, inW, inH, inPitch, slot, s, src, srcPitch)) return false;
+
+      t360::OrientedGatherParams op{};
+      for (int p = 0; p < numPlanes; ++p) {
+        const DevicePlan& plan = *plans[p];
+        t360::OrientedPlane& v = op.plane[p];
+        v.src = src[p];
+        v.srcPitch = srcPitch[p];
+        v.dst = dOut[p];
+        v.dstPitch = outPitch[p];
+        if (outW[p] != plan.mapW || outH[p] != plan.mapH) {  // render at the map's size, then cv::resize(INTER_AREA) (cpp:755-777)
+          const int sp = alignedPitch(plan.mapW);
+          slot.lanes[p].scaled.reserve(static_cast<size_t>(sp) * plan.mapH + 64);
+          v.dst = slot.lanes[p].scaled.ptr;
+          v.dstPitch = sp;
+        }
+        v.geometry = t360::sphereGeometry(ctx, plan.mapW, plan.mapH, plan.inW, plan.inH, plan.kernelSize);
+        v.colTable = plan.sphereTables.ptr;
+        v.rowTable = plan.sphereTables.ptr ? plan.sphereTables.ptr + t360::sphereTableRowOffset(v.geometry) : nullptr;
+      }
+      op.numPlanes = numPlanes;
+      op.rotation = t360::rotationFromAngles(o.yaw, o.pitch, o.roll);
+      op.kernelSize = plans[0]->kernelSize;
+      op.weights = deviceWeights(ctx.interpolation_alg);
+      CU(t360::launchOrientedGather(op, numSMs_, s));
+      for (int p = 0; p < numPlanes; ++p) {
+        if (op.plane[p].dst == dOut[p]) continue;
+        const DevicePlan& plan = *plans[p];
+        const DevicePlan::Resize& r = resizeFor(plan, outW[p], outH[p]);
+        t360::AreaParams ap{op.plane[p].dst, dOut[p], plan.mapW, plan.mapH, op.plane[p].dstPitch, outW[p], outH[p], outPitch[p],
+                            r.cellW, r.cellH, r.xTaps.ptr, r.xFirst.ptr, r.yTaps.ptr, r.yFirst.ptr, r.xLinear.ptr, r.yLinear.ptr, r.xMax};
+        CU(t360::launchAreaResize(ap, s));
+      }
+      return true;
+    } catch (const CudaFail& f) {
+      std::printf("Could not transform the frame with an orientation. Error: CUDA %s (%s) in %s\n", cudaGetErrorName(f.err),
+                  cudaGetErrorString(f.err), f.what);
+      cudaGetLastError();
+    } catch (const std::exception& ex) {
+      std::printf("Could not transform the frame with an orientation. Error: %s\n", ex.what());
+    }
+    return false;
+  }
+
   // tuning aid: a timeline of the consumer groups of the last frame gather (see StagedParams::trace)
   void enableTrace(bool on) { traceEnabled_ = on; }
   size_t readTrace(unsigned long long* out, size_t maxWords) {
@@ -1146,6 +1240,13 @@ class VideoFrameTransform {
     }
     d.resizeNeeded = h.resize.needed;
     if (d.resizeNeeded) resizeFor(d, d.outW, d.outH);
+    if (d.kernelSize > 0 && t360::orientedLayouts(ctx)) {
+      const std::vector<float> t = t360::buildSphereTables(t360::sphereGeometry(ctx, h.mapW, h.mapH, h.inW, h.inH, h.kernelSize));
+      if (!t.empty()) {
+        d.sphereTables.reserve(t.size());
+        CU(cudaMemcpy(d.sphereTables.ptr, t.data(), t.size() * sizeof(float), cudaMemcpyHostToDevice));
+      }
+    }
     return d;
   }
 
@@ -1830,6 +1931,43 @@ T360_API int T360B200_viewSamples(const FrameTransformContext* ctx, const T360Vi
     for (int j = 0; j < mapW; ++j) {
       int32_t* out = samples + 2 * (static_cast<size_t>(i) * mapW + j);
       t360::flatSample(v, g, i, j, out, out + 1);
+    }
+  return 1;
+}
+T360_API int T360B200_transformFrameOrientedAsync(VideoFrameTransform* t, const T360Orientation* orientation, int numPlanes,
+                                                  const uint8_t* const* dIn, uint8_t* const* dOut, const int* inW, const int* inH,
+                                                  const int* inPitch, const int* outW, const int* outH, const int* outPitch, void* stream) {
+  if (!t || !orientation || !dIn || !dOut || !inW || !inH || !inPitch || !outW || !outH || !outPitch) return 0;
+  const t360::Orientation o{orientation->yaw, orientation->pitch, orientation->roll};
+  return t->transformFrameOriented(o, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, static_cast<cudaStream_t>(stream));
+}
+T360_API int T360B200_orientedSamples(const FrameTransformContext* ctx, const T360Orientation* orientation, int inW, int inH, int outW,
+                                      int outH, int32_t* samples) {
+  if (!ctx || !orientation || !samples) return 0;
+  if (!t360::orientedLayouts(*ctx)) {
+    std::printf("Could not compute the orientation's samples. Error: layouts %d -> %d have no per-frame orientation\n",
+                static_cast<int>(ctx->input_layout), static_cast<int>(ctx->output_layout));
+    return 0;
+  }
+  if (!std::isfinite(orientation->yaw) || !std::isfinite(orientation->pitch) || !std::isfinite(orientation->roll)) {
+    std::printf("Could not compute the orientation's samples. Error: the orientation is not finite\n");
+    return 0;
+  }
+  const int k = t360::kernelSizeOf(ctx->interpolation_alg);
+  const int mapW = static_cast<int>(ctx->width_scale_factor * outW + 0.5), mapH = static_cast<int>(ctx->height_scale_factor * outH + 0.5);
+  if (k == 0 || inW <= 0 || inH <= 0 || outW <= 0 || outH <= 0 || mapW <= 0 || mapH <= 0) {
+    std::printf("Could not compute the orientation's samples. Error: invalid interpolation or plane sizes\n");
+    return 0;
+  }
+  const t360::SphereGeometry g = t360::sphereGeometry(*ctx, mapW, mapH, inW, inH, k);
+  const std::vector<float> tables = t360::buildSphereTables(g);
+  const float* colTab = tables.data();
+  const float* rowTab = tables.empty() ? nullptr : tables.data() + t360::sphereTableRowOffset(g);
+  const t360::Rotation r = t360::rotationFromAngles(orientation->yaw, orientation->pitch, orientation->roll);
+  for (int i = 0; i < mapH; ++i)
+    for (int j = 0; j < mapW; ++j) {
+      int32_t* out = samples + 2 * (static_cast<size_t>(i) * mapW + j);
+      t360::sphereSample(g, r, colTab, rowTab, i, j, out, out + 1);
     }
   return 1;
 }

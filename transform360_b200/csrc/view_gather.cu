@@ -1,14 +1,18 @@
-// sm_90a kernel of the per-view FLAT_FIXED path: every plane of a frame in one launch, with the view as a launch
-// parameter instead of a sampling plan.
+// sm_90a kernels of the per-frame paths: every plane of a frame in one launch, with the view (FLAT_FIXED) or the
+// orientation (cube maps, EAC, equirect) as a launch parameter instead of a sampling plan.
 //
-// In FLAT_FIXED the source column and its phase depend only on the output column (and on the pole fold and the eye),
-// the source row and its phase only on the output row (flat_view.h).  So a CTA computes, per tile of 32 columns x
-// viewTileRows(k) rows, a column table (32 columns x fold x eye) and a row table (rows x eye) in shared memory, with the
-// same host/device functions the planner uses -- bit-identical records -- and then a thread takes one column and walks
-// down kViewRowsPerThread rows of it.  The taps go through the read-only path with gatherPixel (gather_common.cuh):
-// whole aligned words for interior windows, per-tap wrapping (BORDER_WRAP, the only border mode FLAT_FIXED uses) for
-// windows that cross the seam or a plane edge.  The weight table is staged once per CTA (stageWeights); the grid is
-// persistent over the tiles of all planes.
+// Both share one persistent tile loop (gatherViewTiles): a CTA takes tiles of 32 columns x viewTileRows(k) rows over the
+// planes of the frame, a thread takes one column of a tile and walks down kViewRowsPerThread rows of it.  The taps go
+// through the read-only path with gatherPixel (gather_common.cuh): whole aligned words for interior windows, per-tap
+// wrapping (BORDER_WRAP, the only border mode of these layouts) for windows that cross the seam or a plane edge.  The
+// weight table is staged once per CTA (stageWeights).  Where the kernels differ is where a pixel's sampling record comes
+// from:
+//   - FLAT_FIXED (FlatPositions): the source column and its phase depend only on the output column (and on the pole fold
+//     and the eye), the source row and its phase only on the output row (flat_view.h).  So per tile the CTA computes a
+//     column table (32 columns x fold x eye) and a row table (rows x eye) in shared memory and each pixel combines them.
+//   - sphere outputs (SpherePositions): the rotation mixes both axes, so every pixel runs the whole chain
+//     (oriented_view.h: sphereSample), with the plan's per-column / per-row tables for the view-independent libm steps.
+// In both, the records come from the same host/device functions the planner (or its host twin) uses: bit-identical.
 #include "gather_common.cuh"
 
 #include <algorithm>
@@ -16,23 +20,57 @@
 namespace t360 {
 namespace {
 
-template <int K>
-__global__ void __launch_bounds__(gatherThreads(K), K == 8 ? 1 : 4) viewGatherKernel(const __grid_constant__ ViewGatherParams p, int numTiles) {
-  extern __shared__ __align__(16) unsigned char smem[];
+template <int K, class Params, class Positions>
+__device__ __forceinline__ void gatherViewTiles(const Params& p, int numTiles, unsigned char* smem, Positions& pos) {
   constexpr int kRows = viewTileRows(K);
-  constexpr int kWeightBytes = K >= 2 ? weightBytes<K>() : 0;
-  FlatColumn* colTab = reinterpret_cast<FlatColumn*>(smem + kWeightBytes);  // [eye][fold][32]
-  FlatRow* rowTab = reinterpret_cast<FlatRow*>(colTab + 4 * 32);             // [column eye][kRows]
-  bool* colEye = reinterpret_cast<bool*>(rowTab + 2 * kRows);                // [32]
-  if constexpr (K >= 2) stageWeights<K>(p.weights, smem);
-
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   for (int tile = blockIdx.x; tile < numTiles; tile += gridDim.x) {
     const int pl = (p.numPlanes > 2 && tile >= p.plane[2].firstTile) ? 2 : ((p.numPlanes > 1 && tile >= p.plane[1].firstTile) ? 1 : 0);
-    const ViewPlane& v = p.plane[pl];
-    const FlatGeometry& g = v.geometry;
+    const auto& v = p.plane[pl];
     const int t = tile - v.firstTile, ty = t / v.tilesX;
     const int x0 = (t - ty * v.tilesX) * 32, y0 = ty * kRows;
+    pos.beginTile(p, v, x0, y0);  // (synchronises the CTA where it builds tables)
+
+    const int j = x0 + lane;
+    if (j >= v.geometry.mapW) continue;
+    SrcView s;
+    s.bytes = v.src;
+    s.misalign = (int)(reinterpret_cast<uintptr_t>(v.src) & 3);
+    s.words = reinterpret_cast<const uint32_t*>(v.src - s.misalign);
+    s.w = v.geometry.inW; s.h = v.geometry.inH; s.pitch = v.srcPitch;
+    pos.beginColumn(lane);
+    const int r0 = warp * kViewRowsPerThread;
+#pragma unroll 1
+    for (int r = r0; r < r0 + kViewRowsPerThread; ++r) {
+      const int i = y0 + r;
+      if (i >= v.geometry.mapH) break;
+      int col0, rowPhase;
+      pos.record(p, v, lane, r, i, j, &col0, &rowPhase);
+      int value;
+      if constexpr (K == 1) {  // nearest: the rounded position, wrapped like cv::remap's BORDER_WRAP
+        value = __ldg(s.bytes + (size_t)wrapIndex(rowPhase >> 10, s.h) * s.pitch + wrapIndex(col0, s.w));
+      } else {
+        value = gatherPixel<K, false, 16384>(s, smem, col0, rowPhase);
+      }
+      v.dst[(size_t)i * v.dstPitch + j] = (uint8_t)value;
+    }
+  }
+}
+
+// FLAT_FIXED: per-tile column and row tables in shared memory, after the weights
+template <int K>
+struct FlatPositions {
+  static constexpr int kRows = viewTileRows(K);
+  static constexpr int kTableBytes = 4 * 32 * (int)sizeof(FlatColumn) + 2 * kRows * (int)sizeof(FlatRow) + 32;
+  FlatColumn* colTab;  // [eye][fold][32]
+  FlatRow* rowTab;     // [column eye][kRows]
+  bool* colEye;        // [32]
+  const FlatRow* rows;
+  __device__ explicit FlatPositions(unsigned char* tables)
+      : colTab(reinterpret_cast<FlatColumn*>(tables)), rowTab(reinterpret_cast<FlatRow*>(colTab + 4 * 32)),
+        colEye(reinterpret_cast<bool*>(rowTab + 2 * kRows)), rows(nullptr) {}
+  __device__ void beginTile(const ViewGatherParams& p, const ViewPlane& v, int x0, int y0) {
+    const FlatGeometry& g = v.geometry;
     __syncthreads();  // (the previous tile's tables have been read; the first time: the weights are staged)
     for (int e = threadIdx.x; e < 4 * 32 + 2 * kRows + 32; e += blockDim.x) {
       if (e < 4 * 32) {
@@ -47,38 +85,50 @@ __global__ void __launch_bounds__(gatherThreads(K), K == 8 ? 1 : 4) viewGatherKe
       }
     }
     __syncthreads();
-
-    const int j = x0 + lane;
-    if (j >= g.mapW) continue;
-    SrcView s;
-    s.bytes = v.src;
-    s.misalign = (int)(reinterpret_cast<uintptr_t>(v.src) & 3);
-    s.words = reinterpret_cast<const uint32_t*>(v.src - s.misalign);
-    s.w = g.inW; s.h = g.inH; s.pitch = v.srcPitch;
-    const FlatRow* rows = rowTab + (colEye[lane] ? kRows : 0);
-    const int r0 = warp * kViewRowsPerThread;
-#pragma unroll 1
-    for (int r = r0; r < r0 + kViewRowsPerThread; ++r) {
-      const int i = y0 + r;
-      if (i >= g.mapH) break;
-      const FlatRow row = rows[r];
-      const FlatColumn c = colTab[(row.eye ? 64 : 0) + (row.fold ? 32 : 0) + lane];
-      int value;
-      if constexpr (K == 1) {  // nearest: the rounded position, wrapped like cv::remap's BORDER_WRAP
-        value = __ldg(s.bytes + (size_t)wrapIndex(row.rowPart >> 10, s.h) * s.pitch + wrapIndex(c.col0, s.w));
-      } else {
-        value = gatherPixel<K, false, 16384>(s, smem, c.col0, row.rowPart + c.fracX);
-      }
-      v.dst[(size_t)i * v.dstPitch + j] = (uint8_t)value;
-    }
   }
+  __device__ void beginColumn(int lane) { rows = rowTab + (colEye[lane] ? kRows : 0); }
+  __device__ void record(const ViewGatherParams&, const ViewPlane&, int lane, int r, int, int, int* col0, int* rowPhase) const {
+    const FlatRow row = rows[r];
+    const FlatColumn c = colTab[(row.eye ? 64 : 0) + (row.fold ? 32 : 0) + lane];
+    *col0 = c.col0;
+    *rowPhase = row.rowPart + c.fracX;
+  }
+};
+
+// Sphere outputs: the whole chain per pixel, no shared tables
+struct SpherePositions {
+  __device__ void beginTile(const OrientedGatherParams&, const OrientedPlane&, int, int) {}
+  __device__ void beginColumn(int) {}
+  __device__ void record(const OrientedGatherParams& p, const OrientedPlane& v, int, int, int i, int j, int* col0, int* rowPhase) const {
+    sphereSample(v.geometry, p.rotation, v.colTable, v.rowTable, i, j, col0, rowPhase);
+  }
+};
+
+template <int K>
+__global__ void __launch_bounds__(gatherThreads(K), K == 8 ? 1 : 4) viewGatherKernel(const __grid_constant__ ViewGatherParams p, int numTiles) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  constexpr int kWeightBytes = K >= 2 ? weightBytes<K>() : 0;
+  FlatPositions<K> pos(smem + kWeightBytes);
+  if constexpr (K >= 2) stageWeights<K>(p.weights, smem);  // (the first tile's __syncthreads publishes them)
+  gatherViewTiles<K>(p, numTiles, smem, pos);
+}
+
+template <int K>
+__global__ void __launch_bounds__(gatherThreads(K), K == 8 ? 1 : 4) orientedGatherKernel(const __grid_constant__ OrientedGatherParams p, int numTiles) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  SpherePositions pos;
+  if constexpr (K >= 2) {
+    stageWeights<K>(p.weights, smem);
+    __syncthreads();  // (no tile synchronises after this)
+  }
+  gatherViewTiles<K>(p, numTiles, smem, pos);
 }
 
 template <int K>
 cudaError_t launchViewK(const ViewGatherParams& p, int numTiles, int numSMs, cudaStream_t stream) {
   static DeviceLaunchCfg cfgs;  // per kernel instantiation, one entry per device
   constexpr int threads = gatherThreads(K);
-  constexpr int smemBytes = (K >= 2 ? weightBytes<K>() : 0) + 4 * 32 * (int)sizeof(FlatColumn) + 2 * viewTileRows(K) * (int)sizeof(FlatRow) + 32;
+  constexpr int smemBytes = (K >= 2 ? weightBytes<K>() : 0) + FlatPositions<K>::kTableBytes;
   LaunchCfg cfg;
   cudaError_t err = prepare<viewGatherKernel<K>>(cfgs, threads, smemBytes, cfg);
   if (err != cudaSuccess) return err;
@@ -88,24 +138,58 @@ cudaError_t launchViewK(const ViewGatherParams& p, int numTiles, int numSMs, cud
   return cudaGetLastError();
 }
 
-}  // namespace
+template <int K>
+cudaError_t launchOrientedK(const OrientedGatherParams& p, int numTiles, int numSMs, cudaStream_t stream) {
+  static DeviceLaunchCfg cfgs;
+  constexpr int threads = gatherThreads(K);
+  constexpr int smemBytes = K >= 2 ? weightBytes<K>() : 0;
+  LaunchCfg cfg;
+  cudaError_t err = prepare<orientedGatherKernel<K>>(cfgs, threads, smemBytes, cfg);
+  if (err != cudaSuccess) return err;
+  const int grid = std::min(numSMs * cfg.perSM, numTiles);
+  orientedGatherKernel<K><<<grid, threads, smemBytes, stream>>>(p, numTiles);
+  gLaunches.fetch_add(1, std::memory_order_relaxed);
+  return cudaGetLastError();
+}
 
-cudaError_t launchViewGather(ViewGatherParams p, int numSMs, cudaStream_t stream) {
-  if (p.numPlanes < 1 || p.numPlanes > kMaxFramePlanes) return cudaErrorInvalidValue;
+// tiles of every plane, in plane order
+template <class Params>
+int assignTiles(Params& p) {
   const int rows = viewTileRows(p.kernelSize);
   int numTiles = 0;
   for (int i = 0; i < p.numPlanes; ++i) {
-    ViewPlane& v = p.plane[i];
+    auto& v = p.plane[i];
     v.tilesX = (v.geometry.mapW + 31) / 32;
     v.firstTile = numTiles;
     numTiles += v.tilesX * ((v.geometry.mapH + rows - 1) / rows);
   }
+  return numTiles;
+}
+
+}  // namespace
+
+cudaError_t launchViewGather(ViewGatherParams p, int numSMs, cudaStream_t stream) {
+  if (p.numPlanes < 1 || p.numPlanes > kMaxFramePlanes) return cudaErrorInvalidValue;
+  const int numTiles = assignTiles(p);
   if (numTiles <= 0) return cudaSuccess;
   switch (p.kernelSize) {
     case 1: return launchViewK<1>(p, numTiles, numSMs, stream);
     case 2: return launchViewK<2>(p, numTiles, numSMs, stream);
     case 4: return launchViewK<4>(p, numTiles, numSMs, stream);
     case 8: return launchViewK<8>(p, numTiles, numSMs, stream);
+    default: return cudaErrorInvalidValue;
+  }
+}
+
+cudaError_t launchOrientedGather(OrientedGatherParams p, int numSMs, cudaStream_t stream) {
+  if (p.numPlanes < 1 || p.numPlanes > kMaxFramePlanes) return cudaErrorInvalidValue;
+  const int numTiles = assignTiles(p);
+  if (numTiles <= 0) return cudaSuccess;
+  switch (p.kernelSize) {
+    case 1: return launchOrientedK<1>(p, numTiles, numSMs, stream);
+    case 2: return launchOrientedK<2>(p, numTiles, numSMs, stream);
+    case 4: return launchOrientedK<4>(p, numTiles, numSMs, stream);
+    case 8: return launchOrientedK<8>(p, numTiles, numSMs, stream);
     default: return cudaErrorInvalidValue;
   }
 }

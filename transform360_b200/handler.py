@@ -63,6 +63,18 @@ def as_view(view) -> T360View:
     return view if isinstance(view, T360View) else T360View(*[float(v) for v in view])
 
 
+class T360Orientation(C.Structure):
+    """An orientation in degrees (include/transform360_b200.h), as the context's fixed_yaw / pitch / roll."""
+    _fields_ = [("yaw", C.c_float), ("pitch", C.c_float), ("roll", C.c_float)]
+
+
+def as_orientation(orientation) -> T360Orientation:
+    """A T360Orientation from a T360Orientation or a (yaw, pitch, roll) sequence."""
+    if isinstance(orientation, T360Orientation):
+        return orientation
+    return T360Orientation(*[float(v) for v in orientation])
+
+
 def make_context(**overrides) -> FrameTransformContext:
     vals = dict(FILTER_DEFAULTS)
     for k in overrides:
@@ -128,6 +140,10 @@ def load(path: os.PathLike | None = None):
     L.T360B200_transformFrameViewAsync.argtypes = [vp, C.POINTER(T360View), ci, vp, vp] + [vp] * 6 + [vp]
     L.T360B200_viewSamples.restype = ci
     L.T360B200_viewSamples.argtypes = [C.POINTER(FrameTransformContext), C.POINTER(T360View)] + [ci] * 4 + [vp]
+    L.T360B200_transformFrameOrientedAsync.restype = ci
+    L.T360B200_transformFrameOrientedAsync.argtypes = [vp, C.POINTER(T360Orientation), ci, vp, vp] + [vp] * 6 + [vp]
+    L.T360B200_orientedSamples.restype = ci
+    L.T360B200_orientedSamples.argtypes = [C.POINTER(FrameTransformContext), C.POINTER(T360Orientation)] + [ci] * 4 + [vp]
     L.T360B200_setPinHostPlanes.restype = None
     L.T360B200_setPinHostPlanes.argtypes = [vp, ci]
     L.T360B200_debugTrace.restype = None
@@ -157,6 +173,7 @@ EXPORTED_SYMBOLS = [
     "T360B200_hostPlanGather", "T360B200_hostPlanPoleCaps", "T360B200_hostPlanBlurLists", "T360B200_weightImage", "T360B200_dealLanes",
     "T360B200_remapTable", "T360B200_transformFramePlaneAsync", "T360B200_transformFrameAsync",
     "T360B200_lowPassPlaneAsync", "T360B200_reconfigure", "T360B200_transformFrameViewAsync", "T360B200_viewSamples",
+    "T360B200_transformFrameOrientedAsync", "T360B200_orientedSamples",
     "T360B200_setPinHostPlanes", "T360B200_debugTrace", "T360B200_debugTraceRead", "T360B200_synchronize", "T360B200_stream", "T360B200_kernelLaunchCount", "T360B200_planDeviceBytes",
     "T360B200_planTileCounts", "T360B200_deviceCount", "T360B200_version",
 ]
@@ -250,6 +267,24 @@ class VideoFrameTransform:
 
         def call(view, stream: int = 0, _keep=(d_in, d_out, arrs)) -> bool:
             return bool(fn(h, C.byref(as_view(view)), n, pin, pout, *ptrs, stream))
+        return call
+
+    def make_oriented_frame_call(self, in_planes, out_planes, dims):
+        """Like make_frame_call, for T360B200_transformFrameOrientedAsync (cube-map, EAC and equirect outputs): returns a
+        callable f(orientation, stream) -> bool that enqueues the whole frame with `orientation` (a T360Orientation or
+        (yaw, pitch, roll))."""
+        n = len(in_planes)
+        VP, IA = C.c_void_p * n, C.c_int * n
+        d_in = VP(*[p[0] for p in in_planes])
+        d_out = VP(*[p[0] for p in out_planes])
+        arrs = [IA(*[d[0] for d in dims]), IA(*[d[1] for d in dims]), IA(*[p[1] for p in in_planes]),
+                IA(*[d[2] for d in dims]), IA(*[d[3] for d in dims]), IA(*[p[1] for p in out_planes])]
+        fn, h = self._lib.T360B200_transformFrameOrientedAsync, self._h
+        ptrs = [C.cast(a, C.c_void_p) for a in arrs]
+        pin, pout = C.cast(d_in, C.c_void_p), C.cast(d_out, C.c_void_p)
+
+        def call(orientation, stream: int = 0, _keep=(d_in, d_out, arrs)) -> bool:
+            return bool(fn(h, C.byref(as_orientation(orientation)), n, pin, pout, *ptrs, stream))
         return call
 
     def low_pass_async(self, d_in: int, d_out: int, w, h, in_pitch, out_pitch, plan_index, stream: int = 0) -> bool:
@@ -396,6 +431,18 @@ def view_samples(ctx: FrameTransformContext, view, in_w, in_h, out_w, out_h) -> 
     out = np.zeros((max(map_h, 0), max(map_w, 0), 2), np.int32)
     if not load().T360B200_viewSamples(C.byref(ctx), C.byref(as_view(view)), in_w, in_h, out_w, out_h, out.ctypes.data):
         raise ValueError("T360B200_viewSamples refused the arguments (message on stdout)")
+    return out
+
+
+def oriented_samples(ctx: FrameTransformContext, orientation, in_w, in_h, out_w, out_h) -> np.ndarray:
+    """The sampling records the per-frame orientation kernel computes for one plane (T360B200_orientedSamples, no CUDA):
+    int32 [map_h][map_w][2] like HostPlan.samples."""
+    scaled = lambda f, n: int(float(np.float32(f) * np.float32(n)) + 0.5)  # (float product, double sum: buildHostPlan)
+    map_w, map_h = scaled(ctx.width_scale_factor, out_w), scaled(ctx.height_scale_factor, out_h)
+    out = np.zeros((max(map_h, 0), max(map_w, 0), 2), np.int32)
+    if not load().T360B200_orientedSamples(C.byref(ctx), C.byref(as_orientation(orientation)), in_w, in_h, out_w, out_h,
+                                           out.ctypes.data):
+        raise ValueError("T360B200_orientedSamples refused the arguments (message on stdout)")
     return out
 
 

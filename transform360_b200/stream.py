@@ -129,6 +129,13 @@ class FrameTransformer:
         dims = [self.spec.plane_dims(p)[:4] for p in range(self.spec.num_planes)]
         return self.vft.make_view_frame_call(in_planes, out_planes, dims)
 
+    def oriented_frame_call(self, in_planes, out_planes):
+        """Prebuilt whole-frame call with a per-frame orientation (T360B200_transformFrameOrientedAsync: cube-map, EAC and
+        equirect outputs) for one (input, output) buffer pair.  Returns f(orientation, stream) -> bool; orientation:
+        T360Orientation or (yaw, pitch, roll)."""
+        dims = [self.spec.plane_dims(p)[:4] for p in range(self.spec.num_planes)]
+        return self.vft.make_oriented_frame_call(in_planes, out_planes, dims)
+
     def transform_frame_device(self, in_planes, out_planes, stream: int = 0):
         """in_planes / out_planes: per plane (device_address, pitch).  Asynchronous on `stream`; the planes of
         the frame run concurrently on the transform's internal lanes."""
