@@ -151,6 +151,31 @@ int T360B200_transformFrameOrientedAsync(VideoFrameTransform* transform, const T
  * non-finite orientation or invalid sizes. */
 int T360B200_orientedSamples(const FrameTransformContext* ctx, const T360Orientation* orientation, int inputWidth,
                              int inputHeight, int outputWidth, int outputHeight, int32_t* samples);
+/* A camera pose, in degrees, as the context's fixed_yaw, fixed_pitch, fixed_roll, fixed_hfov and fixed_vfov. */
+typedef struct T360Pose {
+  float yaw, pitch, roll, hfov, vfov;
+} T360Pose;
+/* One frame of any transform with its own pose, without re-planning: the arguments and the asynchronous contract of
+ * T360B200_transformFrameAsync, plus `pose`.  The frame equals, bit for bit, what a fresh transform would give for the
+ * transform's current context with its five view fields replaced by *pose (low-pass, the INTER_AREA resize for scale
+ * factors != 1 and the barrel layouts' transparent border included: chroma planes are pre-filled with 128, luma keeps the
+ * caller's bytes where no source pixel lands); the transform's context is not changed.  Every output layout is served, and
+ * for layouts other than FLAT_FIXED every input layout (any input but CUBEMAP_32 is read as equirect, as the planner
+ * does): FLAT_FIXED through the per-view kernel (roll plays no part in it), the others through the per-frame orientation
+ * kernel, so a caller can pass the current camera every frame without knowing which serves its layout.  Without low-pass
+ * a frame is one kernel launch.  The call never synchronises the device, and it is frame-exact against
+ * T360B200_reconfigure.  Returns 1 if everything was enqueued; 0 with a message on stdout, before any CUDA call, for a
+ * non-finite pose field, a transform without interpolation algorithm, a plan index that was never generated, an input
+ * plane of another size than its map was generated for, or 0 or more than 3 planes. */
+int T360B200_transformFramePoseAsync(VideoFrameTransform* transform, const T360Pose* pose, int numPlanes,
+                                     const uint8_t* const* deviceInputs, uint8_t* const* deviceOutputs, const int* inputWidths,
+                                     const int* inputHeights, const int* inputPitches, const int* outputWidths,
+                                     const int* outputHeights, const int* outputPitches, void* cudaStream);
+/* Host only, no CUDA: the sampling records the per-frame kernels compute for one plane of `ctx` with the pose substituted,
+ * int32 [mapHeight][mapWidth][2] (map = scaled output size) in the format of T360B200_hostPlanSamples.  Returns 1 on
+ * success; 0 (message on stdout) for an unknown output layout, a non-finite pose or invalid sizes. */
+int T360B200_poseSamples(const FrameTransformContext* ctx, const T360Pose* pose, int inputWidth, int inputHeight,
+                         int outputWidth, int outputHeight, int32_t* samples);
 /* Opt-in (also: environment T360B200_PIN_HOST_PLANES=1): page-lock pageable caller planes in place the second time
  * the same buffer is seen (cudaHostRegister), so that recycled frame-pool buffers are DMA'd at full PCIe speed.  The
  * caller must keep such buffers alive until VideoFrameTransform_delete. */

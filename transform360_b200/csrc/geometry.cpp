@@ -158,8 +158,8 @@ class Projector {
         q = onSphere(equirectYaw(x), equirectPitch(y));
         return true;
       case LAYOUT_BARREL: {  // cpp:970-982
-        if (x <= 0.8f) {
-          q = onSphere(static_cast<float>((2.5f * x - 1.0f) * e * M_PI), static_cast<float>((y * 0.5f - 0.25f) * e * M_PI));
+        if (x <= 0.8f) {  // (angles: oriented_view.h, shared with the per-frame pose path)
+          q = onSphere(barrelYaw(x, e), barrelPitch(y, e));
           return true;
         }
         const int half = static_cast<int>(y * 2);
@@ -168,8 +168,7 @@ class Projector {
       case LAYOUT_BARREL_SPLIT: {  // cpp:983-1068
         if (3.0f * x <= 2.0f) {
           const int half = static_cast<int>(y * 2);
-          q = onSphere(static_cast<float>(((3.0f / 2.0f * x - 0.5f) * e - half + 1.0f) * M_PI),
-                       static_cast<float>((y - 0.25f - 0.5f * half) * e * M_PI));
+          q = onSphere(barrelSplitYaw(x, half, e), barrelSplitPitch(y, half, e));
           return true;
         }
         const int quarter = static_cast<int>(y * 4);

@@ -344,9 +344,10 @@ __host__ __device__ constexpr int viewTileRows(int k) { return gatherThreads(k) 
 cudaError_t launchViewGather(ViewGatherParams p, int numSMs, cudaStream_t stream);
 
 // ---- the per-frame orientation gather (view_gather.cu) --------------------------------------------------------------
-// CUBEMAP_32, CUBEMAP_23_OFFCENTER, EAC_32 and EQUIRECT frames whose orientation (yaw, pitch, roll) is a launch parameter,
-// as its rotation coefficients: the kernel computes every pixel's sampling record (oriented_view.h), with the plan's
-// view-independent tables.  Same tiles, threads and taps as the per-view gather; BORDER_WRAP only.
+// Frames of every layout but FLAT_FIXED whose orientation (yaw, pitch, roll) is a launch parameter, as its rotation
+// coefficients: the kernel computes every pixel's sampling record (oriented_view.h), with the plan's view-independent
+// tables.  Same tiles, threads and taps as the per-view gather; BORDER_WRAP, or BORDER_TRANSPARENT for BARREL and
+// BARREL_SPLIT (chosen from the planes' output layout).
 struct OrientedPlane {
   const uint8_t* src;  // (blurred) input plane, geometry.inW x geometry.inH
   uint8_t* dst;        // render target, geometry.mapW x geometry.mapH

@@ -1,14 +1,17 @@
 // Sphere-output position chain with the orientation as a parameter: one definition for the host and the per-frame
-// orientation gather kernel (oriented_gather.cu).
+// orientation gather kernel (view_gather.cu).
 //
-// For output pixel (i, j) of a CUBEMAP_32, CUBEMAP_23_OFFCENTER, EAC_32 or EQUIRECT map, the planner (geometry.cpp,
-// Projector::project) computes: pixel centre -> output eye split -> point on the unit cube / sphere -> off-centre warp ->
-// rotation by yaw / pitch / roll -> input lookup (EQUIRECT: atan2f, asinf; CUBEMAP_32: gnomonic face coordinates) -> input
-// eye re-pack -> u * inW - 0.5f, v * inH - 0.5f -> cv::remap's 1/32-pixel quantisation.  Only the rotation depends on
-// the orientation.  What remains of libm is reproduced or tabulated so the device gets the planner's bits:
-//   - the EAC warp (double tan) depends on the column only for x and on the row only for y, and EQUIRECT's sin / cos of
-//     yaw / pitch (float sinf / cosf, FMA ifuncs on the host) on the column / the row: per-plan host tables
-//     (buildSphereTables, from the planner's own expressions: equiAngular, equirectYaw, equirectPitch below);
+// For output pixel (i, j) of a CUBEMAP_32, CUBEMAP_23_OFFCENTER, EAC_32, EQUIRECT, BARREL or BARREL_SPLIT map, the planner
+// (geometry.cpp, Projector::project) computes: pixel centre -> output eye split -> point on the unit cube / sphere (or the
+// barrel dead zone) -> off-centre warp -> rotation by yaw / pitch / roll -> input lookup (EQUIRECT: atan2f, asinf, and for
+// barrel outputs a clamp clear of the right edge; CUBEMAP_32: gnomonic face coordinates) -> input eye re-pack ->
+// u * inW - 0.5f, v * inH - 0.5f -> cv::remap's 1/32-pixel quantisation.  Only the rotation depends on the orientation.
+// What remains of libm is reproduced or tabulated so the device gets the planner's bits:
+//   - the EAC warp (double tan) depends on the column only for x and on the row only for y, and the sin / cos of yaw /
+//     pitch of EQUIRECT and of the barrel bands (float sinf / cosf, FMA ifuncs on the host) on the column (BARREL_SPLIT:
+//     and the row half) / the row: per-plan host tables (buildSphereTables, from the planner's own expressions:
+//     equiAngular, equirectYaw, equirectPitch, barrelYaw, barrelPitch, barrelSplitYaw, barrelSplitPitch below);
+//   - the barrel end caps are float + - * only (the face, BARREL_SPLIT's quarter turns, the disc test): on the device;
 //   - the rotation coefficients (double sin / cos of the angles, stored as float): computed on the host per frame by
 //     rotationFromAngles, which Projector's constructor calls too;
 //   - sqrtf, atan2f, asinf: __fsqrt_rn and the libm ports (libm_ports.h); the double steps of rayToSphere and of the
@@ -56,26 +59,43 @@ inline Rotation rotationFromAngles(float yaw, float pitch, float roll) {
 inline float equiAngular(float t) { return static_cast<float>(std::tan((t - 0.5f) * M_PI * 0.5f) * 0.5f + 0.5f); }  // cpp:1074-1075
 inline float equirectYaw(float x) { return static_cast<float>((2.0f * x - 1.0f) * M_PI); }                            // cpp:965-969
 inline float equirectPitch(float y) { return static_cast<float>((y - 0.5f) * M_PI); }
+inline float barrelYaw(float x, float e) { return static_cast<float>((2.5f * x - 1.0f) * e * M_PI); }      // cpp:970-982
+inline float barrelPitch(float y, float e) { return static_cast<float>((y * 0.5f - 0.25f) * e * M_PI); }
+inline float barrelSplitYaw(float x, int half, float e) {                                                  // cpp:983-1000
+  return static_cast<float>(((3.0f / 2.0f * x - 0.5f) * e - half + 1.0f) * M_PI);
+}
+inline float barrelSplitPitch(float y, int half, float e) { return static_cast<float>((y - 0.25f - 0.5f * half) * e * M_PI); }
 
 // Everything the chain needs besides the orientation and the tables.
 struct SphereGeometry {
   int mapW, mapH, inW, inH;
   int kernelSize;            // 1 (nearest), 2, 4, 8
-  int outputLayout;          // LAYOUT_CUBEMAP_32, LAYOUT_CUBEMAP_23_OFFCENTER, LAYOUT_EAC_32, LAYOUT_EQUIRECT
-  bool cubeInput;            // input_layout CUBEMAP_32 (else EQUIRECT)
+  int outputLayout;          // any but LAYOUT_FLAT_FIXED
+  bool cubeInput;            // input_layout CUBEMAP_32 (else treated as EQUIRECT, as the planner does)
   bool splitLR, splitTB;     // the output holds two eyes side by side / stacked (only when the input is stereo)
   bool vflip;
   bool packLR, packTB;       // the input holds two eyes side by side / stacked
   bool offCentre, horizontalOffset;
   float expand, inputExpand;  // expand_coef, input_expand_coef
   float ox, oy, oz;           // fixed_cube_offcenter_*
+  float inPixelWidth;         // 1.0f / inW, doubled for a side-by-side input: barrel outputs keep u half of it clear of 0 and 1
 };
 
-// Per-plan tables (buildSphereTables), [mapW] or [2 mapW] column entries followed by [mapH] or [2 mapH] row entries:
-// EAC_32: the warped face coordinate of the column / the row; EQUIRECT: sin, cos of the column's yaw / the row's pitch.
-// Other layouts need none.
+T360_HD bool barrelLayout(int layout) { return layout == LAYOUT_BARREL || layout == LAYOUT_BARREL_SPLIT; }
+
+// Per-plan tables (buildSphereTables), column entries followed by row entries:
+//   EAC_32: [mapW] / [mapH], the warped face coordinate of the column / the row;
+//   EQUIRECT, BARREL: [mapW][2] / [mapH][2], sin and cos of the column's yaw / the row's pitch;
+//   BARREL_SPLIT: [2][mapW][2] / [mapH][2], sin and cos of the yaw of the column in row half 0 and 1 / of the row's pitch.
+// (BARREL columns past the band, and BARREL_SPLIT columns past it, have entries nobody reads.)  Other layouts need none.
 inline size_t sphereTableRowOffset(const SphereGeometry& g) {
-  return g.outputLayout == LAYOUT_EQUIRECT ? 2 * static_cast<size_t>(g.mapW) : g.outputLayout == LAYOUT_EAC_32 ? g.mapW : 0;
+  const size_t w = static_cast<size_t>(g.mapW);
+  switch (g.outputLayout) {
+    case LAYOUT_EQUIRECT: case LAYOUT_BARREL: return 2 * w;
+    case LAYOUT_BARREL_SPLIT: return 4 * w;
+    case LAYOUT_EAC_32: return w;
+    default: return 0;
+  }
 }
 
 // The coordinate of column j / row i after the output eye split; the row already flipped upwards (cpp:936-938).
@@ -102,17 +122,27 @@ inline std::vector<float> buildSphereTables(const SphereGeometry& g) {
       const float y = sphereRowY(g, i);
       t[g.mapW + i] = equiAngular(y * 2.0f - static_cast<int>(y * 2));
     }
-  } else if (g.outputLayout == LAYOUT_EQUIRECT) {
-    t.resize(2 * (static_cast<size_t>(g.mapW) + g.mapH));
+  } else if (g.outputLayout == LAYOUT_EQUIRECT || barrelLayout(g.outputLayout)) {
+    const size_t rows = sphereTableRowOffset(g);
+    t.resize(rows + 2 * static_cast<size_t>(g.mapH));
+    auto sinCos = [&t](size_t at, float a) {
+      t[at] = std::sin(a);
+      t[at + 1] = std::cos(a);
+    };
+    const float e = g.expand;
     for (int j = 0; j < g.mapW; ++j) {
-      const float a = equirectYaw(sphereColumnX(g, j));
-      t[2 * j] = std::sin(a);
-      t[2 * j + 1] = std::cos(a);
+      const float x = sphereColumnX(g, j);
+      if (g.outputLayout == LAYOUT_EQUIRECT) sinCos(2 * j, equirectYaw(x));
+      else if (g.outputLayout == LAYOUT_BARREL) sinCos(2 * j, barrelYaw(x, e));
+      else
+        for (int half = 0; half < 2; ++half) sinCos(2 * (static_cast<size_t>(half) * g.mapW + j), barrelSplitYaw(x, half, e));
     }
     for (int i = 0; i < g.mapH; ++i) {
-      const float a = equirectPitch(sphereRowY(g, i));
-      t[2 * g.mapW + 2 * i] = std::sin(a);
-      t[2 * g.mapW + 2 * i + 1] = std::cos(a);
+      const float y = sphereRowY(g, i);
+      const float a = g.outputLayout == LAYOUT_EQUIRECT ? equirectPitch(y)
+                      : g.outputLayout == LAYOUT_BARREL ? barrelPitch(y, e)
+                                                        : barrelSplitPitch(y, static_cast<int>(y * 2), e);
+      sinCos(rows + 2 * static_cast<size_t>(i), a);
     }
   }
   return t;
@@ -215,8 +245,55 @@ T360_HD void cubeInputHD(const SphereGeometry& g, float tx, float ty, float tz, 
   *v = 0.0f;
 }
 
+// (sin yaw cos pitch, sin pitch, cos yaw cos pitch) from a column and a row entry of the tables (cpp:1095-1101)
+T360_HD SphereVec onSphereHD(const float* yawSinCos, const float* pitchSinCos) {
+  const float sy = yawSinCos[0], cy = yawSinCos[1], sp = pitchSinCos[0], cp = pitchSinCos[1];
+  return SphereVec{fMul(sy, cp), sp, fMul(cy, cp)};
+}
+
+// Where a BARREL / BARREL_SPLIT output pixel sits (cpp:970-1068, 1106-1113): the band on the unit sphere from the tables,
+// an end cap on the TOP / BOTTOM cube face.  false: outside the cap's disc (the dead zone).
+T360_HD bool barrelPoint(const SphereGeometry& g, const float* colTab, const float* rowTab, int i, int j, float x, float y, SphereVec& q) {
+  const float e = g.expand;
+  float fx, fy;
+  int face;
+  if (g.outputLayout == LAYOUT_BARREL) {
+    if (x <= 0.8f) {
+      q = onSphereHD(colTab + 2 * j, rowTab + 2 * i);
+      return true;
+    }
+    const int half = truncToInt(fMul(y, 2.0f));
+    face = half == 1 ? TOP : BOTTOM;
+    fx = fSub(fMul(x, 5.0f), 4.0f);
+    fy = fSub(fMul(y, 2.0f), static_cast<float>(half));
+  } else {
+    if (fMul(3.0f, x) <= 2.0f) {
+      const int half = truncToInt(fMul(y, 2.0f));  // (0 or 1: y = 1 - the row's centre after the eye split, in [0, 1))
+      q = onSphereHD(colTab + 2 * (static_cast<size_t>(half) * g.mapW + j), rowTab + 2 * i);
+      return true;
+    }
+    const int quarter = truncToInt(fMul(y, 4.0f));
+    fx = fSub(fMul(x, 3.0f), 2.0f);
+    fy = y;
+    switch (quarter) {  // the caps' four quarters, the first two turned by 180 degrees
+      case 0: fy = fMul(fy, 2.0f); fx = fSub(1.0f, fx); fy = fMul(fSub(0.5f, fy), e); break;
+      case 1: fy = fMul(fy, 2.0f); fx = fSub(1.0f, fx); fy = fSub(1.0f, fMul(e, fSub(fy, 0.5f))); break;
+      case 2: fy = fSub(fMul(fy, 2.0f), 0.5f); fy = fSub(1.0f, fMul(e, fSub(1.0f, fy))); break;
+      case 3: fy = fSub(fMul(fy, 2.0f), 1.5f); fy = fMul(fy, e); break;
+      default: break;
+    }
+    face = (quarter == 1 || quarter == 3) ? TOP : BOTTOM;
+  }
+  const float dx = fSub(fx, 0.5f), dy = fSub(fy, 0.5f);
+  if (fAdd(fMul(dx, dx), fMul(dy, dy)) > fMul(fMul(0.25f, e), e)) return false;
+  q = onCubeFace(g, false, face, fx, fy);
+  return true;
+}
+
 // The sampling record {col0, rowPhase} of output pixel (i, j), as HostPlan::samples holds it.  colTab / rowTab: the plan's
-// tables (buildSphereTables) at column and row offset.
+// tables (buildSphereTables) at column and row offset.  BARREL = false leaves the barrel layouts out of the code (the
+// orientation kernel's instantiations for the other layouts).
+template <bool BARREL = true>
 T360_HD void sphereSample(const SphereGeometry& g, const Rotation& r, const float* colTab, const float* rowTab, int i, int j,
                           int32_t* col0, int32_t* rowPhase) {
   float x = pixelCentre(j, g.mapW), y = pixelCentre(i, g.mapH);
@@ -224,10 +301,13 @@ T360_HD void sphereSample(const SphereGeometry& g, const Rotation& r, const floa
   if (g.splitLR) eye = splitEye(x, false);
   else if (g.splitTB) eye = splitEye(y, g.vflip);
   y = fSub(1.0f, y);
+  const bool barrel = BARREL && barrelLayout(g.outputLayout);
   SphereVec q;
-  if (g.outputLayout == LAYOUT_EQUIRECT) {  // cpp:1095-1101: (sin yaw cos pitch, sin pitch, cos yaw cos pitch)
-    const float sy = colTab[2 * j], cy = colTab[2 * j + 1], sp = rowTab[2 * i], cp = rowTab[2 * i + 1];
-    q = SphereVec{fMul(sy, cp), sp, fMul(cy, cp)};
+  bool mapped = true;
+  if (barrel) {
+    mapped = barrelPoint(g, colTab, rowTab, i, j, x, y, q);
+  } else if (g.outputLayout == LAYOUT_EQUIRECT) {
+    q = onSphereHD(colTab + 2 * j, rowTab + 2 * i);
   } else if (g.outputLayout == LAYOUT_CUBEMAP_23_OFFCENTER) {  // cpp:951-958
     const int row = truncToInt(fMul(y, 3.0f)), col = truncToInt(fMul(x, 2.0f));
     q = onCubeFace(g, true, clampFace(col + (2 - row) * 2), fSub(fMul(x, 2.0f), static_cast<float>(col)),
@@ -244,27 +324,34 @@ T360_HD void sphereSample(const SphereGeometry& g, const Rotation& r, const floa
     }
     q = onCubeFace(g, false, clampFace(col + (1 - row) * 3), fx, fy);
   }
-  if (g.offCentre) warpOffCentreHD(g, q);
-  const float tx = fAdd(fSub(fMul(q.x, r.xx), fMul(q.y, r.xy)), fMul(q.z, r.xz));
-  const float ty = -fAdd(fSub(fMul(q.x, r.yx), fMul(q.y, r.yy)), fMul(q.z, r.yz));
-  const float tz = fAdd(fSub(fMul(q.x, r.zx), fMul(q.y, r.zy)), fMul(q.z, r.zz));
-  const float n = fSqrt(fAdd(fAdd(fMul(tx, tx), fMul(ty, ty)), fMul(tz, tz)));  // cpp:863-891
-  float u, v;
-  if (g.cubeInput) {
-    cubeInputHD(g, fDiv(tx, n), fDiv(ty, n), fDiv(tz, n), &u, &v);
-  } else {
-    const float lon = -libmAtan2f(fDiv(-tx, n), fDiv(tz, n));
-    const float lat = libmAsinf(fDiv(-ty, n));
+  float u = -1.0f, v = 0.0f;  // the dead zone's position, not re-packed (cpp:1304-1306)
+  if (mapped) {
+    if (g.offCentre) warpOffCentreHD(g, q);
+    const float tx = fAdd(fSub(fMul(q.x, r.xx), fMul(q.y, r.xy)), fMul(q.z, r.xz));
+    const float ty = -fAdd(fSub(fMul(q.x, r.yx), fMul(q.y, r.yy)), fMul(q.z, r.yz));
+    const float tz = fAdd(fSub(fMul(q.x, r.zx), fMul(q.y, r.zy)), fMul(q.z, r.zz));
+    const float n = fSqrt(fAdd(fAdd(fMul(tx, tx), fMul(ty, ty)), fMul(tz, tz)));  // cpp:863-891
+    if (g.cubeInput) {
+      cubeInputHD(g, fDiv(tx, n), fDiv(ty, n), fDiv(tz, n), &u, &v);
+    } else {
+      const float lon = -libmAtan2f(fDiv(-tx, n), fDiv(tz, n));
+      const float lat = libmAsinf(fDiv(-ty, n));
 #ifdef __CUDA_ARCH__
-    u = __double2float_rn(__dadd_rn(__ddiv_rn(static_cast<double>(lon), M_PI * 2.0f), 0.5));
-    v = __double2float_rn(__dadd_rn(__ddiv_rn(static_cast<double>(lat), M_PI), 0.5));
+      u = __double2float_rn(__dadd_rn(__ddiv_rn(static_cast<double>(lon), M_PI * 2.0f), 0.5));
+      v = __double2float_rn(__dadd_rn(__ddiv_rn(static_cast<double>(lat), M_PI), 0.5));
 #else
-    u = static_cast<float>(lon / (M_PI * 2.0f) + 0.5f);
-    v = static_cast<float>(lat / M_PI + 0.5f);
+      u = static_cast<float>(lon / (M_PI * 2.0f) + 0.5f);
+      v = static_cast<float>(lat / M_PI + 0.5f);
 #endif
+      if (barrel) {  // std::min, then std::max, as the ternaries they are: a NaN u stays NaN (cpp:881-886)
+        const float lo = fMul(g.inPixelWidth, 0.5f), hi = fSub(1.0f, lo);
+        u = hi < u ? hi : u;
+        u = u < lo ? lo : u;
+      }
+    }
+    if (g.packTB) v = packEye(v, eye);  // cpp:1278-1300
+    else if (g.packLR) u = packEye(u, eye);
   }
-  if (g.packTB) v = packEye(v, eye);  // cpp:1278-1300
-  else if (g.packLR) u = packEye(u, eye);
   int c0, fracX, r0, fracY;
   quantizeAxis(toPixel(u, g.inW), g.kernelSize, &c0, &fracX);
   quantizeAxis(toPixel(v, g.inH), g.kernelSize, &r0, &fracY);
@@ -292,6 +379,8 @@ inline SphereGeometry sphereGeometry(const FrameTransformContext& ctx, int mapW,
   g.expand = ctx.expand_coef;
   g.inputExpand = ctx.input_expand_coef;
   g.ox = ctx.fixed_cube_offcenter_x; g.oy = ctx.fixed_cube_offcenter_y; g.oz = ctx.fixed_cube_offcenter_z;
+  g.inPixelWidth = 1.0f / inW;  // cpp:528-531, as buildWarpMap
+  if (g.packLR) g.inPixelWidth *= 2;
   return g;
 }
 

@@ -115,7 +115,8 @@ struct DevicePlan {
   };
   bool resizeNeeded = false;  // for the size the map was generated for
   mutable std::map<std::pair<int, int>, Resize> resizes;
-  // the per-frame orientation path's view-independent tables (oriented_view.h: buildSphereTables), EAC_32 and EQUIRECT
+  // the per-frame orientation path's view-independent tables (oriented_view.h: buildSphereTables): EAC_32, EQUIRECT, BARREL,
+  // BARREL_SPLIT
   DeviceBuffer<float> sphereTables;
   size_t deviceBytes() const {
     return samples.bytes() + records.bytes() + gatherJobs.bytes() + blur.image.bytes();
@@ -877,136 +878,110 @@ class VideoFrameTransform {
     return false;
   }
 
-  // Whole frame with a per-frame FLAT_FIXED view, device to device, asynchronous on `stream`: the frame a fresh transform
-  // would give for the context with fixed_yaw / pitch / hfov / vfov replaced by `view`, with no re-plan.  The gather
-  // computes its sampling records from the view (view_gather.cu); the low-pass, which depends on the view, is re-planned
-  // on the host (the segment rectangles do not change, the taps do) and its lists go to the device through the slot's
-  // page-locked rings, in stream order.  Nothing here synchronises the device, and the plans' sampling data is not read.
+  // Whole frame with a per-frame FLAT_FIXED view (T360B200_transformFrameViewAsync): the frame a fresh transform would give
+  // for the context with fixed_yaw / pitch / hfov / vfov replaced by `view`, with no re-plan (perFrame).
   bool transformFrameView(const t360::FlatView& view, int numPlanes, const uint8_t* const* dIn, uint8_t* const* dOut, const int* inW,
                           const int* inH, const int* inPitch, const int* outW, const int* outH, const int* outPitch, cudaStream_t stream) {
-    try {
-      if (numPlanes < 1 || numPlanes > kPlaneLanes) {
-        std::printf("Could not transform the frame with a view. Error: %d planes (1..%d supported)\n", numPlanes, kPlaneLanes);
-        return false;
-      }
+    auto substitute = [&](FrameTransformContext& ctx) {
       if (!std::isfinite(view.yaw) || !std::isfinite(view.pitch) || !std::isfinite(view.hfov) || !std::isfinite(view.vfov)) {
         std::printf("Could not transform the frame with a view. Error: the view (yaw %g, pitch %g, hfov %g, vfov %g) is not finite\n",
                     view.yaw, view.pitch, view.hfov, view.vfov);
         return false;
       }
-      std::shared_lock<std::shared_mutex> config(configMu_);
-      if (ctx_.output_layout != LAYOUT_FLAT_FIXED) {
+      if (ctx.output_layout != LAYOUT_FLAT_FIXED) {
         std::printf("Could not transform the frame with a view. Error: per-frame views need output_layout FLAT_FIXED (%d), the transform has %d\n",
-                    static_cast<int>(LAYOUT_FLAT_FIXED), static_cast<int>(ctx_.output_layout));
+                    static_cast<int>(LAYOUT_FLAT_FIXED), static_cast<int>(ctx.output_layout));
         return false;
       }
-      FrameTransformContext ctx = ctx_;
       ctx.fixed_yaw = view.yaw;
       ctx.fixed_pitch = view.pitch;
       ctx.fixed_hfov = view.hfov;
       ctx.fixed_vfov = view.vfov;
-      const DevicePlan* plans[kPlaneLanes];
-      for (int p = 0; p < numPlanes; ++p) {
-        if (!(plans[p] = findPlan(p ? 1 : 0, p))) return false;
-        if (inW[p] != plans[p]->inW || inH[p] != plans[p]->inH) {
-          std::printf("Could not transform the frame with a view. Error: input plane %d is %dx%d, its map was generated for %dx%d\n", p, inW[p],
-                      inH[p], plans[p]->inW, plans[p]->inH);
-          return false;
-        }
-        if (plans[p]->kernelSize == 0) {
-          std::printf("Could not transform the frame with a view. Error: no interpolation algorithm %d\n", ctx.interpolation_alg);
-          return false;
-        }
-      }
-      const DeviceRestore restoreDevice = ensureDevice();
-      cudaStream_t s = stream ? stream : stream_;
-      StreamSlot& slot = slotFor(s);
-      const uint8_t* src[kPlaneLanes];
-      int srcPitch[kPlaneLanes];
-      for (int p = 0; p < numPlanes; ++p) { src[p] = dIn[p]; srcPitch[p] = inPitch[p]; }
-      if (plans[0]->lowPass && !viewLowPass(ctx, plans, numPlanes, dIn, inW, inH, inPitch, slot, s, src, srcPitch)) return false;
-
-      t360::ViewGatherParams vp{};
-      for (int p = 0; p < numPlanes; ++p) {
-        const DevicePlan& plan = *plans[p];
-        t360::ViewPlane& v = vp.plane[p];
-        v.src = src[p];
-        v.srcPitch = srcPitch[p];
-        v.dst = dOut[p];
-        v.dstPitch = outPitch[p];
-        if (outW[p] != plan.mapW || outH[p] != plan.mapH) {  // render at the map's size, then cv::resize(INTER_AREA) (cpp:755-777)
-          const int sp = alignedPitch(plan.mapW);
-          slot.lanes[p].scaled.reserve(static_cast<size_t>(sp) * plan.mapH + 64);
-          v.dst = slot.lanes[p].scaled.ptr;
-          v.dstPitch = sp;
-        }
-        const bool stereoIn = ctx.input_stereo_format != STEREO_FORMAT_MONO;
-        v.geometry = t360::FlatGeometry{plan.mapW, plan.mapH, plan.inW, plan.inH, plan.kernelSize,
-                                        stereoIn && ctx.output_stereo_format == STEREO_FORMAT_LR, stereoIn && ctx.output_stereo_format == STEREO_FORMAT_TB,
-                                        ctx.vflip != 0, ctx.input_stereo_format == STEREO_FORMAT_LR, ctx.input_stereo_format == STEREO_FORMAT_TB};
-      }
-      vp.numPlanes = numPlanes;
-      vp.view = view;
-      vp.kernelSize = plans[0]->kernelSize;
-      vp.weights = deviceWeights(ctx.interpolation_alg);
-      CU(t360::launchViewGather(vp, numSMs_, s));
-      for (int p = 0; p < numPlanes; ++p) {
-        if (vp.plane[p].dst == dOut[p]) continue;
-        const DevicePlan& plan = *plans[p];
-        const DevicePlan::Resize& r = resizeFor(plan, outW[p], outH[p]);
-        t360::AreaParams ap{vp.plane[p].dst, dOut[p], plan.mapW, plan.mapH, vp.plane[p].dstPitch, outW[p], outH[p], outPitch[p],
-                            r.cellW, r.cellH, r.xTaps.ptr, r.xFirst.ptr, r.yTaps.ptr, r.yFirst.ptr, r.xLinear.ptr, r.yLinear.ptr, r.xMax};
-        CU(t360::launchAreaResize(ap, s));
-      }
       return true;
-    } catch (const CudaFail& f) {
-      std::printf("Could not transform the frame with a view. Error: CUDA %s (%s) in %s\n", cudaGetErrorName(f.err), cudaGetErrorString(f.err), f.what);
-      cudaGetLastError();
-    } catch (const std::exception& ex) {
-      std::printf("Could not transform the frame with a view. Error: %s\n", ex.what());
-    }
-    return false;
+    };
+    return perFrame("with a view", substitute, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, stream);
   }
 
-  // Whole frame of a CUBEMAP_32, CUBEMAP_23_OFFCENTER, EAC_32 or EQUIRECT transform with a per-frame orientation, device
-  // to device, asynchronous on `stream`: the frame a fresh transform would give for the context with fixed_yaw / pitch /
-  // roll replaced by `o`, with no re-plan.  The gather computes every sampling record from the rotation and the plan's
-  // tables (oriented_view.h); the low-pass, whose adjust_kernel taps depend on yaw and pitch, is re-planned on the host as
-  // in transformFrameView.  Nothing here synchronises the device, and the plans' sampling data is not read.
+  // Whole frame of a CUBEMAP_32, CUBEMAP_23_OFFCENTER, EAC_32 or EQUIRECT transform with a per-frame orientation
+  // (T360B200_transformFrameOrientedAsync): the frame a fresh transform would give for the context with fixed_yaw / pitch /
+  // roll replaced by `o`, with no re-plan (perFrame).
   bool transformFrameOriented(const t360::Orientation& o, int numPlanes, const uint8_t* const* dIn, uint8_t* const* dOut, const int* inW,
                               const int* inH, const int* inPitch, const int* outW, const int* outH, const int* outPitch, cudaStream_t stream) {
-    try {
-      if (numPlanes < 1 || numPlanes > kPlaneLanes) {
-        std::printf("Could not transform the frame with an orientation. Error: %d planes (1..%d supported)\n", numPlanes, kPlaneLanes);
-        return false;
-      }
+    auto substitute = [&](FrameTransformContext& ctx) {
       if (!std::isfinite(o.yaw) || !std::isfinite(o.pitch) || !std::isfinite(o.roll)) {
         std::printf("Could not transform the frame with an orientation. Error: the orientation (yaw %g, pitch %g, roll %g) is not finite\n",
                     o.yaw, o.pitch, o.roll);
         return false;
       }
-      std::shared_lock<std::shared_mutex> config(configMu_);
-      if (!t360::orientedLayouts(ctx_)) {
+      if (!t360::orientedLayouts(ctx)) {
         std::printf("Could not transform the frame with an orientation. Error: per-frame orientations need output_layout CUBEMAP_32, "
                     "CUBEMAP_23_OFFCENTER, EAC_32 or EQUIRECT and input_layout EQUIRECT or CUBEMAP_32, the transform has %d -> %d%s\n",
-                    static_cast<int>(ctx_.input_layout), static_cast<int>(ctx_.output_layout),
-                    ctx_.output_layout == LAYOUT_FLAT_FIXED ? " (FLAT_FIXED views: T360B200_transformFrameViewAsync)" : "");
+                    static_cast<int>(ctx.input_layout), static_cast<int>(ctx.output_layout),
+                    ctx.output_layout == LAYOUT_FLAT_FIXED ? " (FLAT_FIXED views: T360B200_transformFrameViewAsync)" : "");
         return false;
       }
-      FrameTransformContext ctx = ctx_;
       ctx.fixed_yaw = o.yaw;
       ctx.fixed_pitch = o.pitch;
       ctx.fixed_roll = o.roll;
+      return true;
+    };
+    return perFrame("with an orientation", substitute, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, stream);
+  }
+
+  // Whole frame of any transform with a per-frame pose (T360B200_transformFramePoseAsync): the frame a fresh transform would
+  // give for the context with its five view fields replaced by `pose`, with no re-plan (perFrame).  FLAT_FIXED takes the
+  // view kernel (roll plays no part there, as in the planner), every other layout the orientation kernel.
+  bool transformFramePose(const T360Pose& pose, int numPlanes, const uint8_t* const* dIn, uint8_t* const* dOut, const int* inW,
+                          const int* inH, const int* inPitch, const int* outW, const int* outH, const int* outPitch, cudaStream_t stream) {
+    auto substitute = [&](FrameTransformContext& ctx) {
+      if (!std::isfinite(pose.yaw) || !std::isfinite(pose.pitch) || !std::isfinite(pose.roll) || !std::isfinite(pose.hfov) ||
+          !std::isfinite(pose.vfov)) {
+        std::printf("Could not transform the frame with a pose. Error: the pose (yaw %g, pitch %g, roll %g, hfov %g, vfov %g) is not finite\n",
+                    pose.yaw, pose.pitch, pose.roll, pose.hfov, pose.vfov);
+        return false;
+      }
+      substitutePose(ctx, pose);
+      return true;
+    };
+    return perFrame("with a pose", substitute, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, stream);
+  }
+
+  static void substitutePose(FrameTransformContext& ctx, const T360Pose& pose) {
+    ctx.fixed_yaw = pose.yaw;
+    ctx.fixed_pitch = pose.pitch;
+    ctx.fixed_roll = pose.roll;
+    ctx.fixed_hfov = pose.hfov;
+    ctx.fixed_vfov = pose.vfov;
+  }
+
+  // The frame of a per-frame call (view, orientation, pose), device to device, asynchronous on `stream`.  Under the reader
+  // lock, `substitute` checks the call's arguments against the current context and puts the frame's view fields into a
+  // copy of it (false: refused, with a message); `what` names the call in the messages.  The gather computes its sampling
+  // records itself (view_gather.cu): for FLAT_FIXED from the view (flat_view.h), for every other layout from the rotation
+  // and the plan's tables (oriented_view.h).  The low-pass, which depends on the view, is re-planned on the host
+  // (viewLowPass).  Scale factors render at the map's size, then resize with INTER_AREA.  Every refusal comes before the
+  // first CUDA call.  Nothing here synchronises the device, and the plans' sampling data is not read.
+  template <class Substitute>
+  bool perFrame(const char* what, Substitute& substitute, int numPlanes, const uint8_t* const* dIn, uint8_t* const* dOut, const int* inW,
+                const int* inH, const int* inPitch, const int* outW, const int* outH, const int* outPitch, cudaStream_t stream) {
+    try {
+      if (numPlanes < 1 || numPlanes > kPlaneLanes) {
+        std::printf("Could not transform the frame %s. Error: %d planes (1..%d supported)\n", what, numPlanes, kPlaneLanes);
+        return false;
+      }
+      std::shared_lock<std::shared_mutex> config(configMu_);
+      FrameTransformContext ctx = ctx_;
+      if (!substitute(ctx)) return false;
       const DevicePlan* plans[kPlaneLanes];
       for (int p = 0; p < numPlanes; ++p) {
         if (!(plans[p] = findPlan(p ? 1 : 0, p))) return false;
         if (inW[p] != plans[p]->inW || inH[p] != plans[p]->inH) {
-          std::printf("Could not transform the frame with an orientation. Error: input plane %d is %dx%d, its map was generated for %dx%d\n", p,
+          std::printf("Could not transform the frame %s. Error: input plane %d is %dx%d, its map was generated for %dx%d\n", what, p,
                       inW[p], inH[p], plans[p]->inW, plans[p]->inH);
           return false;
         }
         if (plans[p]->kernelSize == 0) {
-          std::printf("Could not transform the frame with an orientation. Error: no interpolation algorithm %d\n", ctx.interpolation_alg);
+          std::printf("Could not transform the frame %s. Error: no interpolation algorithm %d\n", what, ctx.interpolation_alg);
           return false;
         }
       }
@@ -1018,44 +993,78 @@ class VideoFrameTransform {
       for (int p = 0; p < numPlanes; ++p) { src[p] = dIn[p]; srcPitch[p] = inPitch[p]; }
       if (plans[0]->lowPass && !viewLowPass(ctx, plans, numPlanes, dIn, inW, inH, inPitch, slot, s, src, srcPitch)) return false;
 
-      t360::OrientedGatherParams op{};
+      // render targets: the output, or when its size is not the map's the slot's plane at the map's size (cpp:755-777).
+      // Barrel plans (BORDER_TRANSPARENT) leave a pixel whose anchor tap is outside the source as they find it, so the
+      // targets are pre-filled as in the whole-frame path: chroma outputs with 128 (cpp:743-747), scaled planes with 0 (luma)
+      // or 128 (chroma) (cpp:759-762); luma outputs keep the caller's bytes.
+      uint8_t* dst[kPlaneLanes];
+      int dstPitch[kPlaneLanes];
       for (int p = 0; p < numPlanes; ++p) {
         const DevicePlan& plan = *plans[p];
-        t360::OrientedPlane& v = op.plane[p];
-        v.src = src[p];
-        v.srcPitch = srcPitch[p];
-        v.dst = dOut[p];
-        v.dstPitch = outPitch[p];
-        if (outW[p] != plan.mapW || outH[p] != plan.mapH) {  // render at the map's size, then cv::resize(INTER_AREA) (cpp:755-777)
+        dst[p] = dOut[p];
+        dstPitch[p] = outPitch[p];
+        if (outW[p] != plan.mapW || outH[p] != plan.mapH) {
           const int sp = alignedPitch(plan.mapW);
           slot.lanes[p].scaled.reserve(static_cast<size_t>(sp) * plan.mapH + 64);
-          v.dst = slot.lanes[p].scaled.ptr;
-          v.dstPitch = sp;
+          dst[p] = slot.lanes[p].scaled.ptr;
+          dstPitch[p] = sp;
+          if (plan.transparent) CU(cudaMemset2DAsync(dst[p], sp, p ? 128 : 0, plan.mapW, plan.mapH, s));
+        } else if (plan.transparent && p) {
+          CU(cudaMemset2DAsync(dst[p], dstPitch[p], 128, outW[p], outH[p], s));
         }
-        v.geometry = t360::sphereGeometry(ctx, plan.mapW, plan.mapH, plan.inW, plan.inH, plan.kernelSize);
-        v.colTable = plan.sphereTables.ptr;
-        v.rowTable = plan.sphereTables.ptr ? plan.sphereTables.ptr + t360::sphereTableRowOffset(v.geometry) : nullptr;
       }
-      op.numPlanes = numPlanes;
-      op.rotation = t360::rotationFromAngles(o.yaw, o.pitch, o.roll);
-      op.kernelSize = plans[0]->kernelSize;
-      op.weights = deviceWeights(ctx.interpolation_alg);
-      CU(t360::launchOrientedGather(op, numSMs_, s));
+      const bool stereoIn = ctx.input_stereo_format != STEREO_FORMAT_MONO;
+      if (ctx.output_layout == LAYOUT_FLAT_FIXED) {
+        t360::ViewGatherParams vp{};
+        for (int p = 0; p < numPlanes; ++p) {
+          const DevicePlan& plan = *plans[p];
+          vp.plane[p] = t360::ViewPlane{src[p], dst[p], srcPitch[p], dstPitch[p],
+                                        t360::FlatGeometry{plan.mapW, plan.mapH, plan.inW, plan.inH, plan.kernelSize,
+                                                           stereoIn && ctx.output_stereo_format == STEREO_FORMAT_LR,
+                                                           stereoIn && ctx.output_stereo_format == STEREO_FORMAT_TB, ctx.vflip != 0,
+                                                           ctx.input_stereo_format == STEREO_FORMAT_LR,
+                                                           ctx.input_stereo_format == STEREO_FORMAT_TB},
+                                        0, 0};
+        }
+        vp.numPlanes = numPlanes;
+        vp.view = t360::FlatView{ctx.fixed_yaw, ctx.fixed_pitch, ctx.fixed_hfov, ctx.fixed_vfov};
+        vp.kernelSize = plans[0]->kernelSize;
+        vp.weights = deviceWeights(ctx.interpolation_alg);
+        CU(t360::launchViewGather(vp, numSMs_, s));
+      } else {
+        t360::OrientedGatherParams op{};
+        for (int p = 0; p < numPlanes; ++p) {
+          const DevicePlan& plan = *plans[p];
+          t360::OrientedPlane& v = op.plane[p];
+          v.src = src[p];
+          v.srcPitch = srcPitch[p];
+          v.dst = dst[p];
+          v.dstPitch = dstPitch[p];
+          v.geometry = t360::sphereGeometry(ctx, plan.mapW, plan.mapH, plan.inW, plan.inH, plan.kernelSize);
+          v.colTable = plan.sphereTables.ptr;
+          v.rowTable = plan.sphereTables.ptr ? plan.sphereTables.ptr + t360::sphereTableRowOffset(v.geometry) : nullptr;
+        }
+        op.numPlanes = numPlanes;
+        op.rotation = t360::rotationFromAngles(ctx.fixed_yaw, ctx.fixed_pitch, ctx.fixed_roll);
+        op.kernelSize = plans[0]->kernelSize;
+        op.weights = deviceWeights(ctx.interpolation_alg);
+        CU(t360::launchOrientedGather(op, numSMs_, s));
+      }
       for (int p = 0; p < numPlanes; ++p) {
-        if (op.plane[p].dst == dOut[p]) continue;
+        if (dst[p] == dOut[p]) continue;
         const DevicePlan& plan = *plans[p];
         const DevicePlan::Resize& r = resizeFor(plan, outW[p], outH[p]);
-        t360::AreaParams ap{op.plane[p].dst, dOut[p], plan.mapW, plan.mapH, op.plane[p].dstPitch, outW[p], outH[p], outPitch[p],
+        t360::AreaParams ap{dst[p], dOut[p], plan.mapW, plan.mapH, dstPitch[p], outW[p], outH[p], outPitch[p],
                             r.cellW, r.cellH, r.xTaps.ptr, r.xFirst.ptr, r.yTaps.ptr, r.yFirst.ptr, r.xLinear.ptr, r.yLinear.ptr, r.xMax};
         CU(t360::launchAreaResize(ap, s));
       }
       return true;
     } catch (const CudaFail& f) {
-      std::printf("Could not transform the frame with an orientation. Error: CUDA %s (%s) in %s\n", cudaGetErrorName(f.err),
-                  cudaGetErrorString(f.err), f.what);
+      std::printf("Could not transform the frame %s. Error: CUDA %s (%s) in %s\n", what, cudaGetErrorName(f.err), cudaGetErrorString(f.err),
+                  f.what);
       cudaGetLastError();
     } catch (const std::exception& ex) {
-      std::printf("Could not transform the frame with an orientation. Error: %s\n", ex.what());
+      std::printf("Could not transform the frame %s. Error: %s\n", what, ex.what());
     }
     return false;
   }
@@ -1240,7 +1249,7 @@ class VideoFrameTransform {
     }
     d.resizeNeeded = h.resize.needed;
     if (d.resizeNeeded) resizeFor(d, d.outW, d.outH);
-    if (d.kernelSize > 0 && t360::orientedLayouts(ctx)) {
+    if (d.kernelSize > 0 && ctx.output_layout != LAYOUT_FLAT_FIXED) {
       const std::vector<float> t = t360::buildSphereTables(t360::sphereGeometry(ctx, h.mapW, h.mapH, h.inW, h.inH, h.kernelSize));
       if (!t.empty()) {
         d.sphereTables.reserve(t.size());
@@ -1906,6 +1915,41 @@ T360_API int T360B200_transformFrameViewAsync(VideoFrameTransform* t, const T360
   const t360::FlatView v{view->yaw, view->pitch, view->hfov, view->vfov};
   return t->transformFrameView(v, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, static_cast<cudaStream_t>(stream));
 }
+// The sampling records of one plane of `ctx` as the per-frame kernels compute them, with the frame's view fields already in
+// ctx: FLAT_FIXED by flat_view.h, every other layout by oriented_view.h.  `what` names the call in the messages.
+static int perFrameSamples(const char* what, const FrameTransformContext& ctx, int inW, int inH, int outW, int outH, int32_t* samples) {
+  const int k = t360::kernelSizeOf(ctx.interpolation_alg);
+  const int mapW = static_cast<int>(ctx.width_scale_factor * outW + 0.5), mapH = static_cast<int>(ctx.height_scale_factor * outH + 0.5);
+  if (k == 0 || inW <= 0 || inH <= 0 || outW <= 0 || outH <= 0 || mapW <= 0 || mapH <= 0) {
+    std::printf("Could not compute the %s's samples. Error: invalid interpolation or plane sizes\n", what);
+    return 0;
+  }
+  if (ctx.output_layout == LAYOUT_FLAT_FIXED) {
+    const bool stereoIn = ctx.input_stereo_format != STEREO_FORMAT_MONO;
+    const t360::FlatGeometry g{mapW, mapH, inW, inH, k, stereoIn && ctx.output_stereo_format == STEREO_FORMAT_LR,
+                               stereoIn && ctx.output_stereo_format == STEREO_FORMAT_TB, ctx.vflip != 0,
+                               ctx.input_stereo_format == STEREO_FORMAT_LR, ctx.input_stereo_format == STEREO_FORMAT_TB};
+    const t360::FlatView v{ctx.fixed_yaw, ctx.fixed_pitch, ctx.fixed_hfov, ctx.fixed_vfov};
+    for (int i = 0; i < mapH; ++i)
+      for (int j = 0; j < mapW; ++j) {
+        int32_t* out = samples + 2 * (static_cast<size_t>(i) * mapW + j);
+        t360::flatSample(v, g, i, j, out, out + 1);
+      }
+    return 1;
+  }
+  const t360::SphereGeometry g = t360::sphereGeometry(ctx, mapW, mapH, inW, inH, k);
+  const std::vector<float> tables = t360::buildSphereTables(g);
+  const float* colTab = tables.data();
+  const float* rowTab = tables.empty() ? nullptr : tables.data() + t360::sphereTableRowOffset(g);
+  const t360::Rotation r = t360::rotationFromAngles(ctx.fixed_yaw, ctx.fixed_pitch, ctx.fixed_roll);
+  for (int i = 0; i < mapH; ++i)
+    for (int j = 0; j < mapW; ++j) {
+      int32_t* out = samples + 2 * (static_cast<size_t>(i) * mapW + j);
+      t360::sphereSample(g, r, colTab, rowTab, i, j, out, out + 1);
+    }
+  return 1;
+}
+
 T360_API int T360B200_viewSamples(const FrameTransformContext* ctx, const T360View* view, int inW, int inH, int outW, int outH, int32_t* samples) {
   if (!ctx || !view || !samples) return 0;
   if (ctx->output_layout != LAYOUT_FLAT_FIXED) {
@@ -1916,23 +1960,12 @@ T360_API int T360B200_viewSamples(const FrameTransformContext* ctx, const T360Vi
     std::printf("Could not compute the view's samples. Error: the view is not finite\n");
     return 0;
   }
-  const int k = t360::kernelSizeOf(ctx->interpolation_alg);
-  const int mapW = static_cast<int>(ctx->width_scale_factor * outW + 0.5), mapH = static_cast<int>(ctx->height_scale_factor * outH + 0.5);
-  if (k == 0 || inW <= 0 || inH <= 0 || outW <= 0 || outH <= 0 || mapW <= 0 || mapH <= 0) {
-    std::printf("Could not compute the view's samples. Error: invalid interpolation or plane sizes\n");
-    return 0;
-  }
-  const bool stereoIn = ctx->input_stereo_format != STEREO_FORMAT_MONO;
-  const t360::FlatGeometry g{mapW, mapH, inW, inH, k, stereoIn && ctx->output_stereo_format == STEREO_FORMAT_LR,
-                             stereoIn && ctx->output_stereo_format == STEREO_FORMAT_TB, ctx->vflip != 0,
-                             ctx->input_stereo_format == STEREO_FORMAT_LR, ctx->input_stereo_format == STEREO_FORMAT_TB};
-  const t360::FlatView v{view->yaw, view->pitch, view->hfov, view->vfov};
-  for (int i = 0; i < mapH; ++i)
-    for (int j = 0; j < mapW; ++j) {
-      int32_t* out = samples + 2 * (static_cast<size_t>(i) * mapW + j);
-      t360::flatSample(v, g, i, j, out, out + 1);
-    }
-  return 1;
+  FrameTransformContext c = *ctx;
+  c.fixed_yaw = view->yaw;
+  c.fixed_pitch = view->pitch;
+  c.fixed_hfov = view->hfov;
+  c.fixed_vfov = view->vfov;
+  return perFrameSamples("view", c, inW, inH, outW, outH, samples);
 }
 T360_API int T360B200_transformFrameOrientedAsync(VideoFrameTransform* t, const T360Orientation* orientation, int numPlanes,
                                                   const uint8_t* const* dIn, uint8_t* const* dOut, const int* inW, const int* inH,
@@ -1953,23 +1986,32 @@ T360_API int T360B200_orientedSamples(const FrameTransformContext* ctx, const T3
     std::printf("Could not compute the orientation's samples. Error: the orientation is not finite\n");
     return 0;
   }
-  const int k = t360::kernelSizeOf(ctx->interpolation_alg);
-  const int mapW = static_cast<int>(ctx->width_scale_factor * outW + 0.5), mapH = static_cast<int>(ctx->height_scale_factor * outH + 0.5);
-  if (k == 0 || inW <= 0 || inH <= 0 || outW <= 0 || outH <= 0 || mapW <= 0 || mapH <= 0) {
-    std::printf("Could not compute the orientation's samples. Error: invalid interpolation or plane sizes\n");
+  FrameTransformContext c = *ctx;
+  c.fixed_yaw = orientation->yaw;
+  c.fixed_pitch = orientation->pitch;
+  c.fixed_roll = orientation->roll;
+  return perFrameSamples("orientation", c, inW, inH, outW, outH, samples);
+}
+T360_API int T360B200_transformFramePoseAsync(VideoFrameTransform* t, const T360Pose* pose, int numPlanes, const uint8_t* const* dIn,
+                                              uint8_t* const* dOut, const int* inW, const int* inH, const int* inPitch, const int* outW,
+                                              const int* outH, const int* outPitch, void* stream) {
+  if (!t || !pose || !dIn || !dOut || !inW || !inH || !inPitch || !outW || !outH || !outPitch) return 0;
+  return t->transformFramePose(*pose, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, static_cast<cudaStream_t>(stream));
+}
+T360_API int T360B200_poseSamples(const FrameTransformContext* ctx, const T360Pose* pose, int inW, int inH, int outW, int outH, int32_t* samples) {
+  if (!ctx || !pose || !samples) return 0;
+  if (ctx->output_layout < 0 || ctx->output_layout >= LAYOUT_N) {
+    std::printf("Could not compute the pose's samples. Error: output_layout %d is not a layout\n", static_cast<int>(ctx->output_layout));
     return 0;
   }
-  const t360::SphereGeometry g = t360::sphereGeometry(*ctx, mapW, mapH, inW, inH, k);
-  const std::vector<float> tables = t360::buildSphereTables(g);
-  const float* colTab = tables.data();
-  const float* rowTab = tables.empty() ? nullptr : tables.data() + t360::sphereTableRowOffset(g);
-  const t360::Rotation r = t360::rotationFromAngles(orientation->yaw, orientation->pitch, orientation->roll);
-  for (int i = 0; i < mapH; ++i)
-    for (int j = 0; j < mapW; ++j) {
-      int32_t* out = samples + 2 * (static_cast<size_t>(i) * mapW + j);
-      t360::sphereSample(g, r, colTab, rowTab, i, j, out, out + 1);
-    }
-  return 1;
+  if (!std::isfinite(pose->yaw) || !std::isfinite(pose->pitch) || !std::isfinite(pose->roll) || !std::isfinite(pose->hfov) ||
+      !std::isfinite(pose->vfov)) {
+    std::printf("Could not compute the pose's samples. Error: the pose is not finite\n");
+    return 0;
+  }
+  FrameTransformContext c = *ctx;
+  VideoFrameTransform::substitutePose(c, *pose);
+  return perFrameSamples("pose", c, inW, inH, outW, outH, samples);
 }
 T360_API void T360B200_setPinHostPlanes(VideoFrameTransform* t, int enable) { if (t) t->setPinHostPlanes(enable != 0); }
 T360_API void T360B200_debugTrace(VideoFrameTransform* t, int enable) { if (t) t->enableTrace(enable != 0); }

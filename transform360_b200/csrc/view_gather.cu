@@ -1,10 +1,10 @@
 // sm_90a kernels of the per-frame paths: every plane of a frame in one launch, with the view (FLAT_FIXED) or the
-// orientation (cube maps, EAC, equirect) as a launch parameter instead of a sampling plan.
+// orientation (cube maps, EAC, equirect, barrel) as a launch parameter instead of a sampling plan.
 //
 // Both share one persistent tile loop (gatherViewTiles): a CTA takes tiles of 32 columns x viewTileRows(k) rows over the
 // planes of the frame, a thread takes one column of a tile and walks down kViewRowsPerThread rows of it.  The taps go
 // through the read-only path with gatherPixel (gather_common.cuh): whole aligned words for interior windows, per-tap
-// wrapping (BORDER_WRAP, the only border mode of these layouts) for windows that cross the seam or a plane edge.  The
+// wrapping (BORDER_WRAP) for windows that cross the seam or a plane edge, or BORDER_TRANSPARENT for the barrel layouts.  The
 // weight table is staged once per CTA (stageWeights).  Where the kernels differ is where a pixel's sampling record comes
 // from:
 //   - FLAT_FIXED (FlatPositions): the source column and its phase depend only on the output column (and on the pole fold
@@ -20,7 +20,8 @@
 namespace t360 {
 namespace {
 
-template <int K, class Params, class Positions>
+// TRANSPARENT (barrel layouts): BORDER_TRANSPARENT, a pixel whose anchor tap lies outside the source keeps its byte
+template <int K, bool TRANSPARENT, class Params, class Positions>
 __device__ __forceinline__ void gatherViewTiles(const Params& p, int numTiles, unsigned char* smem, Positions& pos) {
   constexpr int kRows = viewTileRows(K);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -48,9 +49,16 @@ __device__ __forceinline__ void gatherViewTiles(const Params& p, int numTiles, u
       pos.record(p, v, lane, r, i, j, &col0, &rowPhase);
       int value;
       if constexpr (K == 1) {  // nearest: the rounded position, wrapped like cv::remap's BORDER_WRAP
-        value = __ldg(s.bytes + (size_t)wrapIndex(rowPhase >> 10, s.h) * s.pitch + wrapIndex(col0, s.w));
+        if constexpr (TRANSPARENT) {
+          const int sx = col0, sy = rowPhase >> 10;
+          if ((unsigned)sx >= (unsigned)s.w || (unsigned)sy >= (unsigned)s.h) continue;
+          value = __ldg(s.bytes + (size_t)sy * s.pitch + sx);
+        } else {
+          value = __ldg(s.bytes + (size_t)wrapIndex(rowPhase >> 10, s.h) * s.pitch + wrapIndex(col0, s.w));
+        }
       } else {
-        value = gatherPixel<K, false, 16384>(s, smem, col0, rowPhase);
+        value = gatherPixel<K, TRANSPARENT, 16384>(s, smem, col0, rowPhase);
+        if (TRANSPARENT && value < 0) continue;
       }
       v.dst[(size_t)i * v.dstPitch + j] = (uint8_t)value;
     }
@@ -95,12 +103,13 @@ struct FlatPositions {
   }
 };
 
-// Sphere outputs: the whole chain per pixel, no shared tables
+// Sphere and barrel outputs: the whole chain per pixel, no shared tables
+template <bool BARREL>
 struct SpherePositions {
   __device__ void beginTile(const OrientedGatherParams&, const OrientedPlane&, int, int) {}
   __device__ void beginColumn(int) {}
   __device__ void record(const OrientedGatherParams& p, const OrientedPlane& v, int, int, int i, int j, int* col0, int* rowPhase) const {
-    sphereSample(v.geometry, p.rotation, v.colTable, v.rowTable, i, j, col0, rowPhase);
+    sphereSample<BARREL>(v.geometry, p.rotation, v.colTable, v.rowTable, i, j, col0, rowPhase);
   }
 };
 
@@ -110,18 +119,19 @@ __global__ void __launch_bounds__(gatherThreads(K), K == 8 ? 1 : 4) viewGatherKe
   constexpr int kWeightBytes = K >= 2 ? weightBytes<K>() : 0;
   FlatPositions<K> pos(smem + kWeightBytes);
   if constexpr (K >= 2) stageWeights<K>(p.weights, smem);  // (the first tile's __syncthreads publishes them)
-  gatherViewTiles<K>(p, numTiles, smem, pos);
+  gatherViewTiles<K, false>(p, numTiles, smem, pos);
 }
 
-template <int K>
+// TRANSPARENT: the barrel layouts, with their positions and BORDER_TRANSPARENT; the other layouts use BORDER_WRAP
+template <int K, bool TRANSPARENT>
 __global__ void __launch_bounds__(gatherThreads(K), K == 8 ? 1 : 4) orientedGatherKernel(const __grid_constant__ OrientedGatherParams p, int numTiles) {
   extern __shared__ __align__(16) unsigned char smem[];
-  SpherePositions pos;
+  SpherePositions<TRANSPARENT> pos;
   if constexpr (K >= 2) {
     stageWeights<K>(p.weights, smem);
     __syncthreads();  // (no tile synchronises after this)
   }
-  gatherViewTiles<K>(p, numTiles, smem, pos);
+  gatherViewTiles<K, TRANSPARENT>(p, numTiles, smem, pos);
 }
 
 template <int K>
@@ -138,16 +148,16 @@ cudaError_t launchViewK(const ViewGatherParams& p, int numTiles, int numSMs, cud
   return cudaGetLastError();
 }
 
-template <int K>
+template <int K, bool TRANSPARENT>
 cudaError_t launchOrientedK(const OrientedGatherParams& p, int numTiles, int numSMs, cudaStream_t stream) {
   static DeviceLaunchCfg cfgs;
   constexpr int threads = gatherThreads(K);
   constexpr int smemBytes = K >= 2 ? weightBytes<K>() : 0;
   LaunchCfg cfg;
-  cudaError_t err = prepare<orientedGatherKernel<K>>(cfgs, threads, smemBytes, cfg);
+  cudaError_t err = prepare<orientedGatherKernel<K, TRANSPARENT>>(cfgs, threads, smemBytes, cfg);
   if (err != cudaSuccess) return err;
   const int grid = std::min(numSMs * cfg.perSM, numTiles);
-  orientedGatherKernel<K><<<grid, threads, smemBytes, stream>>>(p, numTiles);
+  orientedGatherKernel<K, TRANSPARENT><<<grid, threads, smemBytes, stream>>>(p, numTiles);
   gLaunches.fetch_add(1, std::memory_order_relaxed);
   return cudaGetLastError();
 }
@@ -185,11 +195,12 @@ cudaError_t launchOrientedGather(OrientedGatherParams p, int numSMs, cudaStream_
   if (p.numPlanes < 1 || p.numPlanes > kMaxFramePlanes) return cudaErrorInvalidValue;
   const int numTiles = assignTiles(p);
   if (numTiles <= 0) return cudaSuccess;
+  const bool barrel = barrelLayout(p.plane[0].geometry.outputLayout);  // (every plane of a frame has the same layout)
   switch (p.kernelSize) {
-    case 1: return launchOrientedK<1>(p, numTiles, numSMs, stream);
-    case 2: return launchOrientedK<2>(p, numTiles, numSMs, stream);
-    case 4: return launchOrientedK<4>(p, numTiles, numSMs, stream);
-    case 8: return launchOrientedK<8>(p, numTiles, numSMs, stream);
+    case 1: return barrel ? launchOrientedK<1, true>(p, numTiles, numSMs, stream) : launchOrientedK<1, false>(p, numTiles, numSMs, stream);
+    case 2: return barrel ? launchOrientedK<2, true>(p, numTiles, numSMs, stream) : launchOrientedK<2, false>(p, numTiles, numSMs, stream);
+    case 4: return barrel ? launchOrientedK<4, true>(p, numTiles, numSMs, stream) : launchOrientedK<4, false>(p, numTiles, numSMs, stream);
+    case 8: return barrel ? launchOrientedK<8, true>(p, numTiles, numSMs, stream) : launchOrientedK<8, false>(p, numTiles, numSMs, stream);
     default: return cudaErrorInvalidValue;
   }
 }

@@ -46,7 +46,7 @@ typedef struct T360CudaContext {
 
   VideoFrameTransform* transform;
   int maps_ready;
-  int view_frames; /* a FLAT_FIXED view command arrived after the first frame: every frame passes its view */
+  int pose_frames; /* a yaw, pitch, roll, hfov or vfov command arrived after the first frame: every frame passes its pose */
   int sw_format, num_planes;
   AVBufferRef* out_frames;
   AVCUDADeviceContext* cuda;
@@ -234,9 +234,10 @@ static int t360_filter_frame(AVFilterLink* inlink, AVFrame* in) {
       in_pitch[p] = in->linesize[p];
       out_pitch[p] = out->linesize[p];
     }
-    if (s->view_frames) {
-      const T360View view = {s->params.fixed_yaw, s->params.fixed_pitch, s->params.fixed_hfov, s->params.fixed_vfov};
-      rc = T360B200_transformFrameViewAsync(s->transform, &view, s->num_planes, src, dst, in_w, in_h, in_pitch, out_w, out_h,
+    if (s->pose_frames) {
+      const T360Pose pose = {s->params.fixed_yaw, s->params.fixed_pitch, s->params.fixed_roll, s->params.fixed_hfov,
+                             s->params.fixed_vfov};
+      rc = T360B200_transformFramePoseAsync(s->transform, &pose, s->num_planes, src, dst, in_w, in_h, in_pitch, out_w, out_h,
                                             out_pitch, s->cuda->stream)
                ? 0
                : AVERROR_EXTERNAL;
@@ -266,9 +267,11 @@ done:
  * (T360B200_reconfigure: frames filtered before the command keep the old view, every later frame has the new one).
  * Options that could change the output link's size or format (size, cube edge, layouts, stereo formats, scale factors)
  * are refused with ENOSYS, invalid values with EINVAL; a refused command leaves every parameter as it was.
- * In a FLAT_FIXED filter the view commands (yaw, pitch, hfov, vfov) after the first frame re-plan nothing: they update the
- * parameters, and from then on every frame goes through T360B200_transformFrameViewAsync with the current view, so a
- * view can change every frame (head tracking, a camera path) at the cost of a frame, not of a re-plan.
+ * The pose commands (yaw, pitch, roll, hfov, vfov) after the first frame re-plan nothing, whatever the layout: they update
+ * the parameters, and from then on every frame goes through T360B200_transformFramePoseAsync with the current pose, so
+ * the camera can move every frame (head tracking, a camera path, stabilisation) at the cost of a frame, not of a re-plan.
+ * The filter then stays on the per-frame kernels, which take longer per frame than the planned one (DESIGN.md 6); later
+ * commands of other options reconfigure with parameters that already hold the current pose.
  * This needs AV_OPT_FLAG_RUNTIME_PARAM and ff_filter_process_command (FFmpeg 4.2 and later).  A libavfilter without
  * runtime options builds the filter without commands: the options are then fixed at init, as in the reference filter. */
 #ifdef AV_OPT_FLAG_RUNTIME_PARAM
@@ -291,9 +294,8 @@ static int t360_process_command(AVFilterContext* ctx, const char* cmd, const cha
     return AVERROR(EINVAL);
   }
   if (!s->maps_ready) return 0;
-  if (s->params.output_layout == LAYOUT_FLAT_FIXED &&
-      (!strcmp(cmd, "yaw") || !strcmp(cmd, "pitch") || !strcmp(cmd, "hfov") || !strcmp(cmd, "vfov"))) {
-    s->view_frames = 1;
+  if (!strcmp(cmd, "yaw") || !strcmp(cmd, "pitch") || !strcmp(cmd, "roll") || !strcmp(cmd, "hfov") || !strcmp(cmd, "vfov")) {
+    s->pose_frames = 1;
     return 0;
   }
   CudaFunctions* cu = s->cuda->internal->cuda_dl;

@@ -75,6 +75,16 @@ def as_orientation(orientation) -> T360Orientation:
     return T360Orientation(*[float(v) for v in orientation])
 
 
+class T360Pose(C.Structure):
+    """A camera pose in degrees (include/transform360_b200.h), as the context's fixed_yaw / pitch / roll / hfov / vfov."""
+    _fields_ = [("yaw", C.c_float), ("pitch", C.c_float), ("roll", C.c_float), ("hfov", C.c_float), ("vfov", C.c_float)]
+
+
+def as_pose(pose) -> T360Pose:
+    """A T360Pose from a T360Pose or a (yaw, pitch, roll, hfov, vfov) sequence."""
+    return pose if isinstance(pose, T360Pose) else T360Pose(*[float(v) for v in pose])
+
+
 def make_context(**overrides) -> FrameTransformContext:
     vals = dict(FILTER_DEFAULTS)
     for k in overrides:
@@ -144,6 +154,10 @@ def load(path: os.PathLike | None = None):
     L.T360B200_transformFrameOrientedAsync.argtypes = [vp, C.POINTER(T360Orientation), ci, vp, vp] + [vp] * 6 + [vp]
     L.T360B200_orientedSamples.restype = ci
     L.T360B200_orientedSamples.argtypes = [C.POINTER(FrameTransformContext), C.POINTER(T360Orientation)] + [ci] * 4 + [vp]
+    L.T360B200_transformFramePoseAsync.restype = ci
+    L.T360B200_transformFramePoseAsync.argtypes = [vp, C.POINTER(T360Pose), ci, vp, vp] + [vp] * 6 + [vp]
+    L.T360B200_poseSamples.restype = ci
+    L.T360B200_poseSamples.argtypes = [C.POINTER(FrameTransformContext), C.POINTER(T360Pose)] + [ci] * 4 + [vp]
     L.T360B200_setPinHostPlanes.restype = None
     L.T360B200_setPinHostPlanes.argtypes = [vp, ci]
     L.T360B200_debugTrace.restype = None
@@ -173,7 +187,7 @@ EXPORTED_SYMBOLS = [
     "T360B200_hostPlanGather", "T360B200_hostPlanPoleCaps", "T360B200_hostPlanBlurLists", "T360B200_weightImage", "T360B200_dealLanes",
     "T360B200_remapTable", "T360B200_transformFramePlaneAsync", "T360B200_transformFrameAsync",
     "T360B200_lowPassPlaneAsync", "T360B200_reconfigure", "T360B200_transformFrameViewAsync", "T360B200_viewSamples",
-    "T360B200_transformFrameOrientedAsync", "T360B200_orientedSamples",
+    "T360B200_transformFrameOrientedAsync", "T360B200_orientedSamples", "T360B200_transformFramePoseAsync", "T360B200_poseSamples",
     "T360B200_setPinHostPlanes", "T360B200_debugTrace", "T360B200_debugTraceRead", "T360B200_synchronize", "T360B200_stream", "T360B200_kernelLaunchCount", "T360B200_planDeviceBytes",
     "T360B200_planTileCounts", "T360B200_deviceCount", "T360B200_version",
 ]
@@ -285,6 +299,23 @@ class VideoFrameTransform:
 
         def call(orientation, stream: int = 0, _keep=(d_in, d_out, arrs)) -> bool:
             return bool(fn(h, C.byref(as_orientation(orientation)), n, pin, pout, *ptrs, stream))
+        return call
+
+    def make_pose_frame_call(self, in_planes, out_planes, dims):
+        """Like make_frame_call, for T360B200_transformFramePoseAsync (every output layout): returns a callable
+        f(pose, stream) -> bool that enqueues the whole frame with `pose` (a T360Pose or (yaw, pitch, roll, hfov, vfov))."""
+        n = len(in_planes)
+        VP, IA = C.c_void_p * n, C.c_int * n
+        d_in = VP(*[p[0] for p in in_planes])
+        d_out = VP(*[p[0] for p in out_planes])
+        arrs = [IA(*[d[0] for d in dims]), IA(*[d[1] for d in dims]), IA(*[p[1] for p in in_planes]),
+                IA(*[d[2] for d in dims]), IA(*[d[3] for d in dims]), IA(*[p[1] for p in out_planes])]
+        fn, h = self._lib.T360B200_transformFramePoseAsync, self._h
+        ptrs = [C.cast(a, C.c_void_p) for a in arrs]
+        pin, pout = C.cast(d_in, C.c_void_p), C.cast(d_out, C.c_void_p)
+
+        def call(pose, stream: int = 0, _keep=(d_in, d_out, arrs)) -> bool:
+            return bool(fn(h, C.byref(as_pose(pose)), n, pin, pout, *ptrs, stream))
         return call
 
     def low_pass_async(self, d_in: int, d_out: int, w, h, in_pitch, out_pitch, plan_index, stream: int = 0) -> bool:
@@ -443,6 +474,17 @@ def oriented_samples(ctx: FrameTransformContext, orientation, in_w, in_h, out_w,
     if not load().T360B200_orientedSamples(C.byref(ctx), C.byref(as_orientation(orientation)), in_w, in_h, out_w, out_h,
                                            out.ctypes.data):
         raise ValueError("T360B200_orientedSamples refused the arguments (message on stdout)")
+    return out
+
+
+def pose_samples(ctx: FrameTransformContext, pose, in_w, in_h, out_w, out_h) -> np.ndarray:
+    """The sampling records the per-frame kernels compute for one plane with `pose` (T360B200_poseSamples, no CUDA):
+    int32 [map_h][map_w][2] like HostPlan.samples."""
+    scaled = lambda f, n: int(float(np.float32(f) * np.float32(n)) + 0.5)  # (float product, double sum: buildHostPlan)
+    map_w, map_h = scaled(ctx.width_scale_factor, out_w), scaled(ctx.height_scale_factor, out_h)
+    out = np.zeros((max(map_h, 0), max(map_w, 0), 2), np.int32)
+    if not load().T360B200_poseSamples(C.byref(ctx), C.byref(as_pose(pose)), in_w, in_h, out_w, out_h, out.ctypes.data):
+        raise ValueError("T360B200_poseSamples refused the arguments (message on stdout)")
     return out
 
 

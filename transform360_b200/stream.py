@@ -136,6 +136,12 @@ class FrameTransformer:
         dims = [self.spec.plane_dims(p)[:4] for p in range(self.spec.num_planes)]
         return self.vft.make_oriented_frame_call(in_planes, out_planes, dims)
 
+    def pose_frame_call(self, in_planes, out_planes):
+        """Prebuilt whole-frame call with a per-frame pose (T360B200_transformFramePoseAsync: every output layout) for one
+        (input, output) buffer pair.  Returns f(pose, stream) -> bool; pose: T360Pose or (yaw, pitch, roll, hfov, vfov)."""
+        dims = [self.spec.plane_dims(p)[:4] for p in range(self.spec.num_planes)]
+        return self.vft.make_pose_frame_call(in_planes, out_planes, dims)
+
     def transform_frame_device(self, in_planes, out_planes, stream: int = 0):
         """in_planes / out_planes: per plane (device_address, pitch).  Asynchronous on `stream`; the planes of
         the frame run concurrently on the transform's internal lanes."""
