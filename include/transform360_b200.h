@@ -83,7 +83,7 @@ int T360B200_transformFramePlaneAsync(VideoFrameTransform* transform, const uint
  * planes run side by side (chroma on internal streams); one gather launch then takes the tiles of every plane;
  * `cudaStream` observes the completion of all of it.  Arrays have numPlanes (1..3) entries: device pointers, per-plane
  * widths / heights / pitches in bytes.  Scratch planes and schedulers are per stream (see above); generateMapForPlane
- * must not run concurrently with frames in flight (T360B200_reconfigure may). */
+ * must not run concurrently with frames in flight (T360B200_reconfigure and T360B200_reconfigureAsync may). */
 int T360B200_transformFrameAsync(VideoFrameTransform* transform, int numPlanes, const uint8_t* const* deviceInputs,
                                  uint8_t* const* deviceOutputs, const int* inputWidths, const int* inputHeights,
                                  const int* inputPitches, const int* outputWidths, const int* outputHeights,
@@ -97,11 +97,32 @@ int T360B200_lowPassPlaneAsync(VideoFrameTransform* transform, const uint8_t* de
  * still fully in effect.
  * Frame-exact: work enqueued before the call (any entry point, any stream) completes with the old configuration, work
  * enqueued after it returns uses the new one.  The call may overlap frames in flight and calls on other threads: host
- * planning runs while they continue; the call then waits for the device's work enqueued so far, swaps the plans and
- * releases the old ones.  Any field may change as long as the caller keeps the plane sizes it generated the maps for
+ * planning and the upload run while they continue; the call then swaps the plans, waits for the device's work enqueued so
+ * far and releases the old ones.  Any field may change as long as the caller keeps the plane sizes it generated the maps for
  * (layouts, stereo formats and scale factors included).  Before any generateMapForPlane only the context is replaced
  * and no CUDA call is made. */
 int T360B200_reconfigure(VideoFrameTransform* transform, const FrameTransformContext* ctx);
+/* Replaces the transform's FrameTransformContext without waiting for a re-plan.  Returns 1 after checks on the host only
+ * (no device wait, no planning): every frame enqueued after the call, through any entry point and on any stream, equals bit
+ * for bit what a fresh transform made with *ctx gives; work enqueued before it uses the old context.  Until the new plans
+ * are in, whole frames (T360B200_transformFrameAsync, and the view, orientation and pose calls) are served by the per-frame
+ * kernels, which compute every sampling position from the context; the per-plane entry points (transformFramePlane,
+ * T360B200_transformFramePlaneAsync, T360B200_lowPassPlaneAsync) and whole frames of another plane size than planned
+ * wait for the plans.  A background thread plans the latest context once no newer call has arrived for a settle
+ * interval (0.25 s), uploads the plans into fresh buffers, swaps them in without stalling the threads that enqueue frames
+ * and releases the old ones after a device wait of its own; from then on frames take the planned frame kernel again.  A
+ * plan superseded while it was being made is discarded.  Any field may change except the ones that size the planes and
+ * maps (input / output layout, both stereo formats, both scale factors: use T360B200_reconfigure).  Refused, before any
+ * CUDA call, with 0 and a message on stdout and the old context left in effect: a change of one of those fields, an
+ * unknown interpolation_alg, a float field that is not finite, and a context the low-pass planner refuses for one of the
+ * generated plan indices.  Before any generateMapForPlane only the context is replaced and no CUDA call is made.
+ * T360B200_reconfigure and generateMapForPlane discard / finish a pending plan first; VideoFrameTransform_delete waits
+ * for at most the plan being made. */
+int T360B200_reconfigureAsync(VideoFrameTransform* transform, const FrameTransformContext* ctx);
+/* Whether the plans of the current context are in effect: 1 yes; 0 not yet (block == 0); -1 the background planner failed on
+ * it (message on stdout; frames keep being served by the per-frame kernels).  With block != 0 it plans at once, without the
+ * settle interval, and returns 1 or -1 when done. */
+int T360B200_reconfigureWait(VideoFrameTransform* transform, int block);
 /* A FLAT_FIXED view, in degrees, as the context's fixed_yaw, fixed_pitch, fixed_hfov and fixed_vfov. */
 typedef struct T360View {
   float yaw, pitch, hfov, vfov;

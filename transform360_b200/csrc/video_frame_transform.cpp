@@ -9,8 +9,10 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <chrono>
 #include <climits>
 #include <cmath>
+#include <condition_variable>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -123,15 +125,15 @@ struct DevicePlan {
   }
 };
 
-// Whether the low-pass of a frame's planes runs as one strip launch per vertical half-size for all of them: every plane
-// has low-pass at the size it was planned for, the plan is not transparent, its segments cover the plane and its lists
-// (lists[p]) hold strip jobs only.
-bool mergeable(const DevicePlan* const* plans, const t360::BlurLists* const* lists, int numPlanes, const int* inW, const int* inH) {
+// Whether the low-pass of a frame's planes, every one of which has low-pass, runs as one strip launch per vertical
+// half-size for all of them: every plane has the size it was planned for, the plan is not transparent, its segments cover
+// the plane (!clear[p]) and its lists (lists[p]) hold strip jobs only.
+bool mergeable(const DevicePlan* const* plans, const t360::BlurLists* const* lists, const bool* clear, int numPlanes, const int* inW,
+               const int* inH) {
   if (numPlanes < 2) return false;
   for (int p = 0; p < numPlanes; ++p) {
     const DevicePlan& d = *plans[p];
-    if (!d.lowPass || d.transparent || inW[p] != d.inW || inH[p] != d.inH || d.blur.needsClear || !lists[p]->tiles.empty() ||
-        !lists[p]->direct.empty())
+    if (d.transparent || inW[p] != d.inW || inH[p] != d.inH || clear[p] || !lists[p]->tiles.empty() || !lists[p]->direct.empty())
       return false;
   }
   return true;
@@ -147,6 +149,22 @@ bool planOnHost(const FrameTransformContext& ctx, int inW, int inH, int outW, in
   if (p.host.kernelSize > 0) t360::buildGatherPlan(p.host, p.host.kernelSize >= 2 && !p.host.transparentBorder, p.gather);
   return true;
 }
+
+// A driver API function through the runtime's entry point table (nullptr if the driver has none): libcuda is never linked.
+void* driverEntry(const char* name) {
+  void* p = nullptr;
+  cudaDriverEntryPointQueryResult q{};
+  if (cudaGetDriverEntryPoint(name, &p, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess) {
+    cudaGetLastError();
+    p = nullptr;
+  }
+  return p;
+}
+
+// How long the background planner waits after a reconfigureAsync before it plans that context: a camera path or a slider
+// sends a command every frame, and restarting a re-plan of about a second for each of them would keep the host's cores
+// busy for the whole move while the frames are served on the per-frame kernels anyway.
+constexpr std::chrono::milliseconds kSettleInterval{250};
 
 using EncodeTiledFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                    const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -246,6 +264,17 @@ struct WavePlan {
   std::vector<std::vector<Rect>> rects;
 };
 
+// The streamed host-plane call is ~100 runtime calls (chunk copies, events, wave launches, rectangle copies); issued one by
+// one the host thread becomes the bottleneck (measured: no faster than the plain path).  For page-locked caller planes the
+// whole sequence is captured once per (plan, buffers) into a CUDA graph and replayed with one launch.
+struct PlaneGraph {
+  const void* plan; unsigned long long generation; const void* in; const void* out; int inPitch, outPitch;
+  const void* stagingIn; const void* stagingOut;  // (the staging planes grow on demand: a graph made for old ones is stale)
+  int inW, inH, outW, outH;
+  int kernels;
+  cudaGraphExec_t exec; unsigned long long lastUse;
+};
+
 // The per-view low-pass lists of a stream slot's previous frame and what they were made from.  The jobs (rectangles, tap
 // counts and offsets) depend on the view only through the segments' tap counts and on which neighbouring segments carry
 // identical taps; when those agree with the previous frame's, the jobs are reused and only the taps are refilled.
@@ -255,6 +284,7 @@ struct ViewBlurCache {
   std::vector<uint8_t> jobs;
   std::vector<int> tapCodes;  // per float of the tap image: plane << kTapPlaneShift | (1 + plan tap), 0 for a zero
   t360::BlurLayout layout[2];  // merged: [0]; else per plan index
+  bool clear[2] = {false, false};  // per plan index: some pixel lies under no segment
 };
 
 // Page-locked staging of lists that change from frame to frame (the per-view low-pass jobs and taps): a few entries, each
@@ -284,6 +314,14 @@ struct StreamSlot {
   cudaEvent_t fork = nullptr;
   UploadRing viewJobs, viewTaps;  // the per-view low-pass lists (VideoFrameTransform::transformFrameView)
   ViewBlurCache viewBlur;
+  // the per-frame orientation kernel's tables while a reconfigureAsync is pending (the plans' tables are for the old context),
+  // and the context and plan generation they were built for
+  UploadRing sphereTables;
+  std::vector<uint8_t> sphereBytes;
+  size_t sphereAt[2] = {SIZE_MAX, SIZE_MAX};  // per plan index: where its tables start in sphereBytes
+  FrameTransformContext sphereCtx{};
+  unsigned long long sphereGeneration = ~0ull;
+  int sphereIndices = 0;
 };
 
 constexpr int kPitchAlign = 256;
@@ -305,6 +343,12 @@ class VideoFrameTransform {
   void setPinHostPlanes(bool on) { pinHostPlanes_ = on; }
 
   ~VideoFrameTransform() {
+    {  // the background planner finishes the plan it is making, if any, and installs nothing more
+      std::lock_guard<std::mutex> async(asyncMu_);
+      asyncStop_ = true;
+    }
+    asyncCv_.notify_all();
+    if (worker_.joinable()) worker_.join();
     if (deviceReady_) {
       cudaSetDevice(device_);
       plans_.clear();
@@ -323,7 +367,7 @@ class VideoFrameTransform {
         }
         kv.second->frameClaim.release();
         if (kv.second->fork) cudaEventDestroy(kv.second->fork);
-        for (UploadRing* ring : {&kv.second->viewJobs, &kv.second->viewTaps})
+        for (UploadRing* ring : {&kv.second->viewJobs, &kv.second->viewTaps, &kv.second->sphereTables})
           for (UploadRing::Entry& e : ring->entries) {
             if (e.released) cudaEventSynchronize(e.released);
             if (e.device) cudaFree(e.device);
@@ -351,11 +395,17 @@ class VideoFrameTransform {
   // reference generateMapForPlane (cpp:504-576): plan on the host, upload once.
   bool generateMapForPlane(int inW, int inH, int outW, int outH, int planIndex) {
     try {
+      reconfigureWait(true);  // a pending reconfigureAsync re-plans the other indices: it is finished first
       std::lock_guard<std::mutex> planLock(planMu_);
+      FrameTransformContext ctx;
+      {
+        std::shared_lock<std::shared_mutex> config(configMu_);
+        ctx = ctx_;
+      }
       HostIndexPlan host;
-      if (!planOnHost(ctx_, inW, inH, outW, outH, host)) return false;
+      if (!planOnHost(ctx, inW, inH, outW, outH, host)) return false;
       const DeviceRestore restoreDevice = ensureDevice();
-      DevicePlan plan = upload(host, ctx_);
+      DevicePlan plan = upload(host, ctx);
       std::lock_guard<std::mutex> lock(mu_);
       plans_[planIndex] = std::move(plan);
       ++planGeneration_;
@@ -370,57 +420,31 @@ class VideoFrameTransform {
   }
 
   // Replaces the context of a running transform: every plan index is re-planned for `next` with the sizes it was
-  // generated with.  Host planning (all indices at once) runs while other threads keep enqueuing frames with the old
-  // plans; the entry points are held off only while the device waits for the work enqueued so far (it reads the old
-  // plans and lists) and the plans are swapped.  On any failure the old configuration stays in effect.
+  // generated with.  Host planning (all indices at once) and the upload run while other threads keep enqueuing frames with
+  // the old plans; the entry points are held off only while the plans are swapped (install), and the old plans are
+  // released once the device has finished the work enqueued before the swap (retire).  A pending reconfigureAsync is
+  // discarded.  On any failure the old configuration stays in effect.
   bool reconfigure(const FrameTransformContext& next) {
     try {
       std::lock_guard<std::mutex> planLock(planMu_);  // (one re-plan at a time, also against generateMapForPlane)
-      struct Sizes { int index, inW, inH, outW, outH; };
-      std::vector<Sizes> sizes;
+      unsigned long long seq;
       {
-        std::lock_guard<std::mutex> lock(mu_);
-        for (const auto& kv : plans_) sizes.push_back({kv.first, kv.second.inW, kv.second.inH, kv.second.outW, kv.second.outH});
+        std::lock_guard<std::mutex> async(asyncMu_);
+        seq = asyncSeq_;
       }
+      const std::vector<PlanSizes> sizes = plannedSizes();
       if (sizes.empty()) {  // nothing planned yet: the next generateMapForPlane uses the new context (no CUDA call here)
-        std::unique_lock<std::shared_mutex> config(configMu_);  // (the per-view entry point reads the context under it)
+        std::unique_lock<std::shared_mutex> config(configMu_);
         std::memcpy(&ctx_, &next, sizeof(ctx_));
         return true;
       }
-      std::vector<HostIndexPlan> host(sizes.size());
-      std::vector<int> planned(sizes.size(), 0);
-      std::vector<std::string> errors(sizes.size());
-      auto planOne = [&](size_t i) {
-        try {
-          planned[i] = planOnHost(next, sizes[i].inW, sizes[i].inH, sizes[i].outW, sizes[i].outH, host[i]);
-        } catch (const std::exception& ex) {
-          errors[i] = ex.what();
-        }
-      };
-      std::vector<std::thread> pool;  // luma and chroma side by side (each planner is multi-threaded over rows as well)
-      for (size_t i = 1; i < sizes.size(); ++i) pool.emplace_back(planOne, i);
-      planOne(0);
-      for (std::thread& t : pool) t.join();
-      for (size_t i = 0; i < sizes.size(); ++i)
-        if (!planned[i]) {
-          std::printf("Could not reconfigure the transform. Error: no plan for index %d%s%s\n", sizes[i].index, errors[i].empty() ? "" : ": ",
-                      errors[i].c_str());
-          return false;
-        }
+      std::vector<HostIndexPlan> host;
+      if (!planAll(next, sizes, host, "Could not reconfigure the transform")) return false;
       const DeviceRestore restoreDevice = ensureDevice();
-      std::map<int, DevicePlan> plans;
-      for (size_t i = 0; i < sizes.size(); ++i) plans.emplace(sizes[i].index, upload(host[i], next));
-      {
-        std::unique_lock<std::shared_mutex> config(configMu_);  // no call of an entry point is in progress from here on
-        CU(cudaDeviceSynchronize());  // everything enqueued before this call has finished with the old plans
-        std::lock_guard<std::mutex> lock(mu_);
-        plans_.swap(plans);
-        std::memcpy(&ctx_, &next, sizeof(ctx_));
-        ++planGeneration_;  // the merged job and strip lists and the wave plans are rebuilt on first use
-        for (PlaneGraph& g : planeGraphs_) cudaGraphExecDestroy(g.exec);  // (they launch the old plans' jobs)
-        planeGraphs_.clear();
-      }
-      return true;  // (`plans` now holds the old plans: released here, nothing reads them any more)
+      PlanSet set = makePlanSet(next, sizes, host);
+      install(set, next, seq, true);
+      retire(set);
+      return true;
     } catch (const CudaFail& f) {
       std::printf("Could not reconfigure the transform. Error: CUDA %s (%s) in %s\n", cudaGetErrorName(f.err), cudaGetErrorString(f.err), f.what);
       cudaGetLastError();
@@ -428,6 +452,51 @@ class VideoFrameTransform {
       std::printf("Could not reconfigure the transform. Error: %s\n", ex.what());
     }
     return false;
+  }
+
+  // T360B200_reconfigureAsync: `next` is in effect for every frame enqueued after the call returns; until its plans are in,
+  // whole frames take the per-frame kernels (perFrameLocked) and the per-plane entry points wait for the plans.  The plans are
+  // made by the background planner (planInBackground).  Host checks only: every refusal comes before any CUDA call, and so
+  // does the return.
+  bool reconfigureAsync(const FrameTransformContext& next) {
+    const std::vector<PlanSizes> sizes = plannedSizes();
+    if (const char* why = asyncRefusal(next, sizes)) {
+      std::printf("Could not reconfigure the transform asynchronously. Error: %s\n", why);
+      return false;
+    }
+    {
+      std::unique_lock<std::shared_mutex> config(configMu_);  // no call of an entry point is in progress from here on
+      if (ctx_.input_layout != next.input_layout || ctx_.output_layout != next.output_layout ||
+          ctx_.input_stereo_format != next.input_stereo_format || ctx_.output_stereo_format != next.output_stereo_format ||
+          ctx_.width_scale_factor != next.width_scale_factor || ctx_.height_scale_factor != next.height_scale_factor) {
+        std::printf("Could not reconfigure the transform asynchronously. Error: the layouts, stereo formats and scale factors size "
+                    "the planes and maps and cannot change here (T360B200_reconfigure can change them)\n");
+        return false;
+      }
+      std::memcpy(&ctx_, &next, sizeof(ctx_));
+      if (sizes.empty()) return true;  // nothing planned yet: the next generateMapForPlane uses the new context
+      perFrameOnly_ = true;
+      std::lock_guard<std::mutex> async(asyncMu_);
+      ++asyncSeq_;
+      asyncCtx_ = next;
+      asyncLast_ = std::chrono::steady_clock::now();
+      if (!worker_.joinable()) worker_ = std::thread(&VideoFrameTransform::planInBackground, this);
+    }
+    asyncCv_.notify_all();
+    return true;
+  }
+
+  // T360B200_reconfigureWait: 1 when the plans of the current context are in effect, -1 when the background planner failed
+  // on it, else 0 (block = false) or, with block, the result once the planner has finished -- without the settle interval.
+  int reconfigureWait(bool block) {
+    std::unique_lock<std::mutex> async(asyncMu_);
+    if (asyncSettled_ != asyncSeq_ && block) {
+      asyncHurry_ = true;
+      asyncCv_.notify_all();
+      asyncCv_.wait(async, [this] { return asyncSettled_ == asyncSeq_ || asyncStop_; });
+    }
+    if (asyncSettled_ != asyncSeq_) return 0;
+    return asyncFailed_ ? -1 : 1;
   }
 
   // reference transformFramePlane (cpp:1319-1351): host or device planes, synchronous.
@@ -438,7 +507,8 @@ class VideoFrameTransform {
         std::printf("Could not transform the plane %d. Error: invalid plane description\n", imagePlaneIndex);
         return false;
       }
-      std::shared_lock<std::shared_mutex> config(configMu_);
+      std::shared_lock<std::shared_mutex> config = lockPlanned("Could not transform the plane");
+      if (!config.owns_lock()) return false;
       const DeviceRestore restoreDevice = ensureDevice();
       const DevicePlan* plan = findPlan(planIndex, imagePlaneIndex);
       if (!plan) return false;
@@ -765,7 +835,8 @@ class VideoFrameTransform {
   bool transformDevice(const uint8_t* dIn, uint8_t* dOut, int inW, int inH, int inPitch, int outW, int outH,
                        int outPitch, int planIndex, cudaStream_t stream) {
     try {
-      std::shared_lock<std::shared_mutex> config(configMu_);
+      std::shared_lock<std::shared_mutex> config = lockPlanned("Could not transform the plane");
+      if (!config.owns_lock()) return false;
       const DeviceRestore restoreDevice = ensureDevice();
       const DevicePlan* plan = findPlan(planIndex, planIndex);
       if (!plan) return false;
@@ -792,6 +863,16 @@ class VideoFrameTransform {
         return false;
       }
       std::shared_lock<std::shared_mutex> config(configMu_);
+      while (perFrameOnly_) {  // a reconfigureAsync is pending: the per-frame kernels serve planes of the planned sizes
+        if (planesOfPlannedSize(numPlanes, inW, inH))
+          return perFrameLocked("while its plan is pending", ctx_, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, stream);
+        config.unlock();
+        if (reconfigureWait(true) < 0) {
+          std::printf("Could not transform the frame. Error: the background planner failed on the current context\n");
+          return false;
+        }
+        config.lock();
+      }
       const DeviceRestore restoreDevice = ensureDevice();
       cudaStream_t s = stream ? stream : stream_;
       StreamSlot& slot = slotFor(s);
@@ -805,8 +886,13 @@ class VideoFrameTransform {
       }
       // Low-pass of all planes in one launch per vertical kernel size when every plane takes the strip kernel only
       const t360::BlurLists* lists[kPlaneLanes];
-      for (int p = 0; p < numPlanes; ++p) lists[p] = &plans[p]->blur.lists;
-      const bool mergedBlur = mergeable(plans, lists, numPlanes, inW, inH);
+      bool clear[kPlaneLanes], lowPass = true;
+      for (int p = 0; p < numPlanes; ++p) {
+        lists[p] = &plans[p]->blur.lists;
+        clear[p] = plans[p]->blur.needsClear;
+        lowPass = lowPass && plans[p]->lowPass;
+      }
+      const bool mergedBlur = lowPass && mergeable(plans, lists, clear, numPlanes, inW, inH);
       if (mergedBlur) {
         blurFrame(plans, numPlanes, dIn, inW, inH, inPitch, lanes_, s);
         sideWork = false;
@@ -860,7 +946,8 @@ class VideoFrameTransform {
   bool lowPassDevice(const uint8_t* dIn, uint8_t* dOut, int w, int h, int inPitch, int outPitch, int planIndex,
                      cudaStream_t stream) {
     try {
-      std::shared_lock<std::shared_mutex> config(configMu_);
+      std::shared_lock<std::shared_mutex> config = lockPlanned("Could not filter the plane");
+      if (!config.owns_lock()) return false;
       const DeviceRestore restoreDevice = ensureDevice();
       const DevicePlan* plan = findPlan(planIndex, planIndex);
       if (!plan) return false;
@@ -956,22 +1043,33 @@ class VideoFrameTransform {
 
   // The frame of a per-frame call (view, orientation, pose), device to device, asynchronous on `stream`.  Under the reader
   // lock, `substitute` checks the call's arguments against the current context and puts the frame's view fields into a
-  // copy of it (false: refused, with a message); `what` names the call in the messages.  The gather computes its sampling
-  // records itself (view_gather.cu): for FLAT_FIXED from the view (flat_view.h), for every other layout from the rotation
-  // and the plan's tables (oriented_view.h).  The low-pass, which depends on the view, is re-planned on the host
-  // (viewLowPass).  Scale factors render at the map's size, then resize with INTER_AREA.  Every refusal comes before the
-  // first CUDA call.  Nothing here synchronises the device, and the plans' sampling data is not read.
+  // copy of it (false: refused, with a message); `what` names the call in the messages.  The frame is then perFrameLocked's.
   template <class Substitute>
   bool perFrame(const char* what, Substitute& substitute, int numPlanes, const uint8_t* const* dIn, uint8_t* const* dOut, const int* inW,
                 const int* inH, const int* inPitch, const int* outW, const int* outH, const int* outPitch, cudaStream_t stream) {
+    std::shared_lock<std::shared_mutex> config(configMu_);
+    FrameTransformContext ctx = ctx_;
+    if (!substitute(ctx)) return false;
+    return perFrameLocked(what, ctx, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, stream);
+  }
+
+  // The frame a fresh transform made with `ctx` would give, on the per-frame kernels, with the reader lock held: the
+  // per-frame calls' frames, and every whole frame while a reconfigureAsync is pending.  The gather computes its sampling
+  // records itself (view_gather.cu): for FLAT_FIXED from the view (flat_view.h), for every other layout from the rotation
+  // and per-plan tables (oriented_view.h).  Everything that ctx may change against the plans comes from ctx: the kernel size
+  // and weights, low-pass on or off and its segments (re-planned on the host, viewLowPass), and while a reconfigureAsync is
+  // pending the tables (built on the host and uploaded in stream order, sphereTablesFor); only the plane and map sizes, which
+  // ctx cannot change, come from the plans.  Scale factors render at the map's size, then resize with INTER_AREA.  Every
+  // refusal comes before the first CUDA call.  Nothing here synchronises the device, and the plans' sampling data is not read.
+  bool perFrameLocked(const char* what, const FrameTransformContext& ctx, int numPlanes, const uint8_t* const* dIn, uint8_t* const* dOut,
+                      const int* inW, const int* inH, const int* inPitch, const int* outW, const int* outH, const int* outPitch,
+                      cudaStream_t stream) {
     try {
       if (numPlanes < 1 || numPlanes > kPlaneLanes) {
         std::printf("Could not transform the frame %s. Error: %d planes (1..%d supported)\n", what, numPlanes, kPlaneLanes);
         return false;
       }
-      std::shared_lock<std::shared_mutex> config(configMu_);
-      FrameTransformContext ctx = ctx_;
-      if (!substitute(ctx)) return false;
+      const int k = t360::kernelSizeOf(ctx.interpolation_alg);
       const DevicePlan* plans[kPlaneLanes];
       for (int p = 0; p < numPlanes; ++p) {
         if (!(plans[p] = findPlan(p ? 1 : 0, p))) return false;
@@ -980,7 +1078,7 @@ class VideoFrameTransform {
                       inW[p], inH[p], plans[p]->inW, plans[p]->inH);
           return false;
         }
-        if (plans[p]->kernelSize == 0) {
+        if (k == 0) {
           std::printf("Could not transform the frame %s. Error: no interpolation algorithm %d\n", what, ctx.interpolation_alg);
           return false;
         }
@@ -991,7 +1089,7 @@ class VideoFrameTransform {
       const uint8_t* src[kPlaneLanes];
       int srcPitch[kPlaneLanes];
       for (int p = 0; p < numPlanes; ++p) { src[p] = dIn[p]; srcPitch[p] = inPitch[p]; }
-      if (plans[0]->lowPass && !viewLowPass(ctx, plans, numPlanes, dIn, inW, inH, inPitch, slot, s, src, srcPitch)) return false;
+      if (ctx.enable_low_pass_filter && !viewLowPass(what, ctx, plans, numPlanes, dIn, inW, inH, inPitch, slot, s, src, srcPitch)) return false;
 
       // render targets: the output, or when its size is not the map's the slot's plane at the map's size (cpp:755-777).
       // Barrel plans (BORDER_TRANSPARENT) leave a pixel whose anchor tap is outside the source as they find it, so the
@@ -1019,7 +1117,7 @@ class VideoFrameTransform {
         for (int p = 0; p < numPlanes; ++p) {
           const DevicePlan& plan = *plans[p];
           vp.plane[p] = t360::ViewPlane{src[p], dst[p], srcPitch[p], dstPitch[p],
-                                        t360::FlatGeometry{plan.mapW, plan.mapH, plan.inW, plan.inH, plan.kernelSize,
+                                        t360::FlatGeometry{plan.mapW, plan.mapH, plan.inW, plan.inH, k,
                                                            stereoIn && ctx.output_stereo_format == STEREO_FORMAT_LR,
                                                            stereoIn && ctx.output_stereo_format == STEREO_FORMAT_TB, ctx.vflip != 0,
                                                            ctx.input_stereo_format == STEREO_FORMAT_LR,
@@ -1028,11 +1126,15 @@ class VideoFrameTransform {
         }
         vp.numPlanes = numPlanes;
         vp.view = t360::FlatView{ctx.fixed_yaw, ctx.fixed_pitch, ctx.fixed_hfov, ctx.fixed_vfov};
-        vp.kernelSize = plans[0]->kernelSize;
+        vp.kernelSize = k;
         vp.weights = deviceWeights(ctx.interpolation_alg);
         CU(t360::launchViewGather(vp, numSMs_, s));
       } else {
         t360::OrientedGatherParams op{};
+        const float* tables[kPlaneLanes];
+        UploadRing::Entry* staged = nullptr;  // (pending: the tables come through the slot's ring)
+        for (int p = 0; p < numPlanes; ++p) tables[p] = plans[p]->sphereTables.ptr;
+        if (perFrameOnly_) sphereTablesFor(ctx, plans, numPlanes, slot, s, tables, &staged);
         for (int p = 0; p < numPlanes; ++p) {
           const DevicePlan& plan = *plans[p];
           t360::OrientedPlane& v = op.plane[p];
@@ -1040,15 +1142,19 @@ class VideoFrameTransform {
           v.srcPitch = srcPitch[p];
           v.dst = dst[p];
           v.dstPitch = dstPitch[p];
-          v.geometry = t360::sphereGeometry(ctx, plan.mapW, plan.mapH, plan.inW, plan.inH, plan.kernelSize);
-          v.colTable = plan.sphereTables.ptr;
-          v.rowTable = plan.sphereTables.ptr ? plan.sphereTables.ptr + t360::sphereTableRowOffset(v.geometry) : nullptr;
+          v.geometry = t360::sphereGeometry(ctx, plan.mapW, plan.mapH, plan.inW, plan.inH, k);
+          v.colTable = tables[p];
+          v.rowTable = tables[p] ? tables[p] + t360::sphereTableRowOffset(v.geometry) : nullptr;
         }
         op.numPlanes = numPlanes;
         op.rotation = t360::rotationFromAngles(ctx.fixed_yaw, ctx.fixed_pitch, ctx.fixed_roll);
-        op.kernelSize = plans[0]->kernelSize;
+        op.kernelSize = k;
         op.weights = deviceWeights(ctx.interpolation_alg);
         CU(t360::launchOrientedGather(op, numSMs_, s));
+        if (staged) {  // the entry may be refilled once this launch has finished
+          CU(cudaEventRecord(staged->released, s));
+          staged->inFlight = true;
+        }
       }
       for (int p = 0; p < numPlanes; ++p) {
         if (dst[p] == dOut[p]) continue;
@@ -1148,6 +1254,7 @@ class VideoFrameTransform {
     CU(cudaGetDeviceProperties(&prop, device_));
     numSMs_ = prop.multiProcessorCount;
     CU(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
+    if (auto getCurrent = reinterpret_cast<CUresult (*)(CUcontext*)>(driverEntry("cuCtxGetCurrent"))) getCurrent(&cuContext_);
     deviceReady_ = true;
     return guard;
   }
@@ -1197,6 +1304,7 @@ class VideoFrameTransform {
     const int16_t* host = nullptr;
     const int k = t360::remapTable(interpolationAlg, &host);
     if (k < 2) return nullptr;
+    std::lock_guard<std::mutex> lock(lazyMu_);  // (a frame served for a pending context may be the first of its kernel size)
     auto& buf = weights_[k];
     if (!buf.ptr) {
       buf.reserve(static_cast<size_t>(1024) * k * k);
@@ -1482,8 +1590,8 @@ class VideoFrameTransform {
   // job lists cut from them, uploaded through the slot's rings, and the launches -- one per vertical kernel size for all
   // planes when every plane takes the strip kernel only (as blurFrame), else per plane (as runLowPass).  src / srcPitch
   // receive the blurred planes.
-  bool viewLowPass(const FrameTransformContext& ctx, const DevicePlan* const* plans, int numPlanes, const uint8_t* const* dIn, const int* inW,
-                   const int* inH, const int* inPitch, StreamSlot& slot, cudaStream_t s, const uint8_t** src, int* srcPitch) {
+  bool viewLowPass(const char* what, const FrameTransformContext& ctx, const DevicePlan* const* plans, int numPlanes, const uint8_t* const* dIn,
+                   const int* inW, const int* inH, const int* inPitch, StreamSlot& slot, cudaStream_t s, const uint8_t** src, int* srcPitch) {
     const int indices = numPlanes > 1 ? 2 : 1;
     HostPlan h[2];
     // what the job lists depend on: the plans (generation), the planes, and per segment its rectangle, tap counts and
@@ -1494,7 +1602,7 @@ class VideoFrameTransform {
       h[idx].ctx = ctx;
       h[idx].inW = plan.inW; h[idx].inH = plan.inH; h[idx].outW = plan.outW; h[idx].outH = plan.outH; h[idx].mapW = plan.mapW; h[idx].mapH = plan.mapH;
       if (!t360::buildLowPassPlan(h[idx])) {
-        std::printf("Could not transform the frame with a view. Error: no low-pass plan for index %d\n", idx);
+        std::printf("Could not transform the frame %s. Error: no low-pass plan for index %d\n", what, idx);
         return false;
       }
       key.push_back(reinterpret_cast<intptr_t>(&plan));
@@ -1522,11 +1630,19 @@ class VideoFrameTransform {
     } else {
       c = ViewBlurCache{};
       t360::BlurLists lists[2];
-      for (int idx = 0; idx < indices; ++idx)  // (coverage: plan.blur.needsClear, computed once per plan)
-        t360::buildBlurLists(h[idx].segments, h[idx].taps, plans[idx]->inW, plans[idx]->inH, plans[idx]->stereoFormat, lists[idx], nullptr);
+      // coverage: the plan's, computed once per plan, unless a reconfigureAsync is pending (its segment counts may differ)
+      for (int idx = 0; idx < indices; ++idx) {
+        c.clear[idx] = plans[idx]->blur.needsClear;
+        t360::buildBlurLists(h[idx].segments, h[idx].taps, plans[idx]->inW, plans[idx]->inH, plans[idx]->stereoFormat, lists[idx],
+                             perFrameOnly_ ? &c.clear[idx] : nullptr);
+      }
       const t360::BlurLists* perPlane[kPlaneLanes];
-      for (int p = 0; p < numPlanes; ++p) perPlane[p] = &lists[p ? 1 : 0];
-      c.merged = mergeable(plans, perPlane, numPlanes, inW, inH);
+      bool clear[kPlaneLanes];
+      for (int p = 0; p < numPlanes; ++p) {
+        perPlane[p] = &lists[p ? 1 : 0];
+        clear[p] = c.clear[p ? 1 : 0];
+      }
+      c.merged = mergeable(plans, perPlane, clear, numPlanes, inW, inH);
       // one byte image of the jobs and one of the taps, with the provenance of every tap (tapSource; in a merged list it
       // carries the plane already)
       auto appendCodes = [&](const t360::BlurLists& l, const t360::BlurLayout& at, int plane) {
@@ -1563,7 +1679,7 @@ class VideoFrameTransform {
       for (int p = 0; p < numPlanes; ++p) {
         t360::FrameStripParams one{};
         one.plane[0] = fp.plane[p];
-        launchLowPass(c.layout[p ? 1 : 0], plans[p]->blur.needsClear, dJobs, dTaps, one, 1, s);
+        launchLowPass(c.layout[p ? 1 : 0], c.clear[p ? 1 : 0], dJobs, dTaps, one, 1, s);
       }
     }
     for (UploadRing::Entry* e : used) {  // the entries may be refilled once these launches have finished
@@ -1613,28 +1729,33 @@ class VideoFrameTransform {
     std::lock_guard<std::mutex> lock(frameListsMu_);
     FrameLists& f = frameLists_[numPlanes - 2];
     if (f.generation != planGeneration_) {
-      std::vector<GatherJob> jobs;
-      const t360::BlurLists* lists[kPlaneLanes];
-      for (int p = 0; p < numPlanes; ++p) {
-        for (GatherJob t : plans[p]->hostJobs) {
-          t.outY |= p << t360::kJobPlaneShift;
-          jobs.push_back(t);
-        }
-        lists[p] = &plans[p]->blur.lists;
-      }
-      std::stable_sort(jobs.begin(), jobs.end(), [](const GatherJob& a, const GatherJob& b) { return t360::jobLaunchRank(a) < t360::jobLaunchRank(b); });
-      std::vector<uint8_t> image;
-      const t360::BlurLayout layout = t360::packBlurLists(t360::mergeBlurLists(lists, numPlanes), image, image);
       if (f.generation != ~0ull) CU(cudaDeviceSynchronize());
-      f.gatherJobs.reserve(jobs.size());
-      if (!jobs.empty()) CU(cudaMemcpy(f.gatherJobs.ptr, jobs.data(), jobs.size() * sizeof(GatherJob), cudaMemcpyHostToDevice));
-      f.blurImage.reserve(image.size());
-      if (!image.empty()) CU(cudaMemcpy(f.blurImage.ptr, image.data(), image.size(), cudaMemcpyHostToDevice));
-      f.numGatherJobs = static_cast<int>(jobs.size());
-      f.blurLayout = layout;
+      buildFrameLists(plans, numPlanes, f);
       f.generation = planGeneration_;
     }
     return FrameListRefs{f.gatherJobs.ptr, f.numGatherJobs, f.blurImage.ptr, f.blurLayout};
+  }
+
+  // Fills `f` with the merged lists of frames of numPlanes planes (f's buffers are not read by any work in flight).
+  void buildFrameLists(const DevicePlan* const* plans, int numPlanes, FrameLists& f) {
+    std::vector<GatherJob> jobs;
+    const t360::BlurLists* lists[kPlaneLanes];
+    for (int p = 0; p < numPlanes; ++p) {
+      for (GatherJob t : plans[p]->hostJobs) {
+        t.outY |= p << t360::kJobPlaneShift;
+        jobs.push_back(t);
+      }
+      lists[p] = &plans[p]->blur.lists;
+    }
+    std::stable_sort(jobs.begin(), jobs.end(), [](const GatherJob& a, const GatherJob& b) { return t360::jobLaunchRank(a) < t360::jobLaunchRank(b); });
+    std::vector<uint8_t> image;
+    const t360::BlurLayout layout = t360::packBlurLists(t360::mergeBlurLists(lists, numPlanes), image, image);
+    f.gatherJobs.reserve(jobs.size());
+    if (!jobs.empty()) CU(cudaMemcpy(f.gatherJobs.ptr, jobs.data(), jobs.size() * sizeof(GatherJob), cudaMemcpyHostToDevice));
+    f.blurImage.reserve(image.size());
+    if (!image.empty()) CU(cudaMemcpy(f.blurImage.ptr, image.data(), image.size(), cudaMemcpyHostToDevice));
+    f.numGatherJobs = static_cast<int>(jobs.size());
+    f.blurLayout = layout;
   }
 
   // The gathers of all planes of a frame as ONE launch (every plane staged).
@@ -1670,6 +1791,247 @@ class VideoFrameTransform {
     CU(t360::launchAreaResize(ap, s));
   }
 
+  // ---- re-planning: reconfigure and the background planner of reconfigureAsync --------------------------------------
+  struct PlanSizes { int index, inW, inH, outW, outH; };
+  std::vector<PlanSizes> plannedSizes() {
+    std::lock_guard<std::mutex> lock(mu_);
+    std::vector<PlanSizes> sizes;
+    for (const auto& kv : plans_) sizes.push_back({kv.first, kv.second.inW, kv.second.inH, kv.second.outW, kv.second.outH});
+    return sizes;
+  }
+
+  // Whether frame planes of these sizes can take the per-frame kernels (the planned input sizes; a missing plan index is
+  // reported by the path that follows).
+  bool planesOfPlannedSize(int numPlanes, const int* inW, const int* inH) {
+    std::lock_guard<std::mutex> lock(mu_);
+    for (int p = 0; p < numPlanes; ++p) {
+      auto it = plans_.find(p ? 1 : 0);
+      if (it != plans_.end() && (inW[p] != it->second.inW || inH[p] != it->second.inH)) return false;
+    }
+    return true;
+  }
+
+  // The reader lock for an entry point that needs the plans of the current context: while a reconfigureAsync is pending it
+  // first waits for them (without the settle interval).  Not owning the lock: the background planner failed (message).
+  std::shared_lock<std::shared_mutex> lockPlanned(const char* what) {
+    for (;;) {
+      std::shared_lock<std::shared_mutex> config(configMu_);
+      if (!perFrameOnly_) return config;
+      config.unlock();
+      if (reconfigureWait(true) < 0) {
+        std::printf("%s. Error: the background planner failed on the current context\n", what);
+        return {};
+      }
+    }
+  }
+
+  // Why reconfigureAsync refuses `next` (nullptr: accepted).  A refused context would leave frames on the per-frame kernels
+  // with no plan ever to follow, so everything the planner can refuse is refused here, on the host.  With the layouts, stereo
+  // formats and scale factors unchanged (checked under the writer lock) every plane and map size is the planned one, and what
+  // buildHostPlan (sampling.cpp) refuses comes down to:
+  //   - a non-positive plane or map size, and an invalid output layout (buildWarpMap): planned already, cannot occur;
+  //   - with low-pass on, num_vertical_segments < 1, and whatever buildLowPassPlan (lowpass_plan.cpp) refuses: the same
+  //     count, an invalid layout, a band of no rows.  It is run here for every planned index, so a refusal it may add later
+  //     is caught too.
+  // Refused besides: an interpolation_alg that is not NEAREST, LINEAR, CUBIC or LANCZOS4 (buildHostPlan makes a plan without
+  // gather for it; the per-frame kernels need a kernel size), and a float field that is not finite.
+  static const char* asyncRefusal(const FrameTransformContext& next, const std::vector<PlanSizes>& sizes) {
+    if (t360::kernelSizeOf(next.interpolation_alg) == 0) return "unknown interpolation_alg";
+    for (float v : {next.input_expand_coef, next.expand_coef, next.width_scale_factor, next.height_scale_factor, next.fixed_yaw,
+                    next.fixed_pitch, next.fixed_roll, next.fixed_hfov, next.fixed_vfov, next.fixed_cube_offcenter_x,
+                    next.fixed_cube_offcenter_y, next.fixed_cube_offcenter_z, next.kernel_height_scale_factor, next.min_kernel_half_height,
+                    next.max_kernel_half_height, next.kernel_adjust_factor})
+      if (!std::isfinite(v)) return "a float field is not finite";
+    if (!next.enable_low_pass_filter) return nullptr;
+    if (next.num_vertical_segments < 1) return "num_vertical_segments must be positive";
+    for (const PlanSizes& z : sizes) {
+      HostPlan h;
+      h.ctx = next;
+      h.inW = z.inW; h.inH = z.inH; h.outW = z.outW; h.outH = z.outH;
+      h.mapW = static_cast<int>(next.width_scale_factor * z.outW + 0.5);
+      h.mapH = static_cast<int>(next.height_scale_factor * z.outH + 0.5);
+      if (!t360::buildLowPassPlan(h)) return "the low-pass planner refuses the context";
+    }
+    return nullptr;
+  }
+
+  // Host planning of every index in `sizes` for `next`, side by side (false: message, prefixed with `what`).
+  static bool planAll(const FrameTransformContext& next, const std::vector<PlanSizes>& sizes, std::vector<HostIndexPlan>& host,
+                      const char* what) {
+    host.assign(sizes.size(), HostIndexPlan{});
+    std::vector<int> planned(sizes.size(), 0);
+    std::vector<std::string> errors(sizes.size());
+    auto planOne = [&](size_t i) {
+      try {
+        planned[i] = planOnHost(next, sizes[i].inW, sizes[i].inH, sizes[i].outW, sizes[i].outH, host[i]);
+      } catch (const std::exception& ex) {
+        errors[i] = ex.what();
+      }
+    };
+    std::vector<std::thread> pool;  // luma and chroma side by side (each planner is multi-threaded over rows as well)
+    for (size_t i = 1; i < sizes.size(); ++i) pool.emplace_back(planOne, i);
+    planOne(0);
+    for (std::thread& t : pool) t.join();
+    for (size_t i = 0; i < sizes.size(); ++i)
+      if (!planned[i]) {
+        std::printf("%s. Error: no plan for index %d%s%s\n", what, sizes[i].index, errors[i].empty() ? "" : ": ", errors[i].c_str());
+        return false;
+      }
+    return true;
+  }
+
+  // Everything a context's plans are on the device, made off the enqueue path into fresh buffers: the plans of every index
+  // and the merged lists of 2- and 3-plane frames (so the first frame after the swap does not rebuild them in frameLists,
+  // which waits for the device).  After install() it holds what was swapped out.
+  struct PlanSet {
+    std::map<int, DevicePlan> plans;
+    FrameLists lists[kPlaneLanes - 1];
+    std::vector<PlaneGraph> graphs;
+  };
+  PlanSet makePlanSet(const FrameTransformContext& next, const std::vector<PlanSizes>& sizes, std::vector<HostIndexPlan>& host) {
+    PlanSet set;
+    for (size_t i = 0; i < sizes.size(); ++i) set.plans.emplace(sizes[i].index, upload(host[i], next));
+    auto luma = set.plans.find(0), chroma = set.plans.find(1);
+    if (luma != set.plans.end() && chroma != set.plans.end()) {
+      const DevicePlan* planes[kPlaneLanes] = {&luma->second, &chroma->second, &chroma->second};
+      for (int n = 2; n <= kPlaneLanes; ++n) {
+        buildFrameLists(planes, n, set.lists[n - 2]);
+        set.lists[n - 2].generation = planGeneration_ + 1;  // (the generation install() starts: planMu_ is held until then)
+      }
+    }
+    return set;
+  }
+
+  // Swaps `set` in under the writer lock, with no device wait: from here on every entry point uses its plans.  `next`, the
+  // context they were made for, becomes the current one unless a reconfigureAsync newer than `seq` has arrived since; then
+  // the current context stays the newer one and whole frames stay on the per-frame kernels.  With `evenIfSuperseded`
+  // false such a set is not swapped in (false returned).  Either way `set` then holds what retire() must release.
+  bool install(PlanSet& set, const FrameTransformContext& next, unsigned long long seq, bool evenIfSuperseded) {
+    std::unique_lock<std::shared_mutex> config(configMu_);  // no call of an entry point is in progress from here on
+    std::lock_guard<std::mutex> async(asyncMu_);
+    const bool current = asyncSeq_ == seq;
+    if (!current && !evenIfSuperseded) return false;
+    {
+      std::lock_guard<std::mutex> lock(mu_);
+      std::lock_guard<std::mutex> listsLock(frameListsMu_);
+      plans_.swap(set.plans);
+      for (int i = 0; i < kPlaneLanes - 1; ++i) std::swap(frameLists_[i], set.lists[i]);
+      set.graphs.swap(planeGraphs_);  // (they launch the old plans' jobs)
+      ++planGeneration_;  // the wave plans and the per-view low-pass caches are rebuilt on first use
+    }
+    if (current) {
+      std::memcpy(&ctx_, &next, sizeof(ctx_));
+      perFrameOnly_ = false;
+      asyncSettled_ = seq;
+      asyncFailed_ = false;
+      asyncCv_.notify_all();
+    }
+    return true;
+  }
+
+  // Releases what install() swapped out (or a set that was never swapped in) once the device has finished everything
+  // enqueued so far: frames enqueued before the swap may still read the old plans and lists.
+  void retire(PlanSet& old) {
+    CU(cudaDeviceSynchronize());
+    for (PlaneGraph& g : old.graphs) cudaGraphExecDestroy(g.exec);
+    old.graphs.clear();
+    old.plans.clear();
+    for (FrameLists& f : old.lists) f = FrameLists{};
+  }
+
+  // The background planner (one thread per transform, started by the first reconfigureAsync after a plan): plans the
+  // latest pending context once no newer one has arrived for kSettleInterval (at once when someone waits for it), and
+  // installs it unless it has been superseded meanwhile.
+  void planInBackground() {
+    std::unique_lock<std::mutex> async(asyncMu_);
+    bool contextSet = false;
+    while (!asyncStop_) {
+      if (asyncSettled_ == asyncSeq_) {
+        asyncCv_.wait(async);
+        continue;
+      }
+      const auto due = asyncLast_ + kSettleInterval;
+      if (!asyncHurry_ && std::chrono::steady_clock::now() < due) {
+        asyncCv_.wait_until(async, due);
+        continue;
+      }
+      asyncHurry_ = false;
+      const unsigned long long seq = asyncSeq_;
+      const FrameTransformContext next = asyncCtx_;
+      async.unlock();
+      if (!contextSet && cuContext_) {  // the context the transform's frames live in (a caller may have made its own)
+        if (auto setCurrent = reinterpret_cast<CUresult (*)(CUcontext)>(driverEntry("cuCtxSetCurrent"))) setCurrent(cuContext_);
+        contextSet = true;
+      }
+      const bool failed = !planPending(next, seq);
+      async.lock();
+      if (failed && asyncSeq_ == seq && asyncSettled_ != seq) {
+        asyncSettled_ = seq;
+        asyncFailed_ = true;
+        asyncCv_.notify_all();
+      }
+    }
+  }
+
+  // One background plan of `next` (reconfigureAsync number `seq`): false when planning or the upload failed (message).
+  bool planPending(const FrameTransformContext& next, unsigned long long seq) {
+    const char* what = "Could not reconfigure the transform in the background";
+    auto superseded = [&] {
+      std::lock_guard<std::mutex> async(asyncMu_);
+      return asyncSeq_ != seq || asyncSettled_ == seq || asyncStop_;  // (settled: T360B200_reconfigure took over)
+    };
+    try {
+      std::lock_guard<std::mutex> planLock(planMu_);
+      if (superseded()) return true;
+      const std::vector<PlanSizes> sizes = plannedSizes();
+      std::vector<HostIndexPlan> host;
+      if (!planAll(next, sizes, host, what)) return false;
+      if (superseded()) return true;
+      const DeviceRestore restoreDevice = ensureDevice();
+      PlanSet set = makePlanSet(next, sizes, host);
+      install(set, next, seq, false);
+      retire(set);
+      return true;
+    } catch (const CudaFail& f) {
+      std::printf("%s. Error: CUDA %s (%s) in %s\n", what, cudaGetErrorName(f.err), cudaGetErrorString(f.err), f.what);
+      cudaGetLastError();
+    } catch (const std::exception& ex) {
+      std::printf("%s. Error: %s\n", what, ex.what());
+    }
+    return false;
+  }
+
+  // The per-frame orientation kernel's tables of the planes for a context the plans were not made with (a pending
+  // reconfigureAsync): built on the host when the context or the plans change, staged through the slot's upload ring on `s`.
+  // tables[p] receive the device tables (nullptr for layouts without any); *used the ring entry to release after the launch.
+  void sphereTablesFor(const FrameTransformContext& ctx, const DevicePlan* const* plans, int numPlanes, StreamSlot& slot, cudaStream_t s,
+                       const float** tables, UploadRing::Entry** used) {
+    const int indices = numPlanes > 1 ? 2 : 1;
+    FrameTransformContext key = ctx;  // (the orientation plays no part in the tables)
+    key.fixed_yaw = key.fixed_pitch = key.fixed_roll = key.fixed_hfov = key.fixed_vfov = 0;
+    if (slot.sphereGeneration != planGeneration_ || slot.sphereIndices != indices || std::memcmp(&slot.sphereCtx, &key, sizeof(key)) != 0) {
+      slot.sphereBytes.clear();
+      for (int idx = 0; idx < indices; ++idx) {
+        const DevicePlan& plan = *plans[idx];
+        const std::vector<float> t =
+            t360::buildSphereTables(t360::sphereGeometry(ctx, plan.mapW, plan.mapH, plan.inW, plan.inH, t360::kernelSizeOf(ctx.interpolation_alg)));
+        slot.sphereAt[idx] = t.empty() ? SIZE_MAX : slot.sphereBytes.size();
+        const uint8_t* bytes = reinterpret_cast<const uint8_t*>(t.data());
+        slot.sphereBytes.insert(slot.sphereBytes.end(), bytes, bytes + t.size() * sizeof(float));
+      }
+      slot.sphereCtx = key;
+      slot.sphereGeneration = planGeneration_;
+      slot.sphereIndices = indices;
+    }
+    for (int p = 0; p < numPlanes; ++p) tables[p] = nullptr;
+    if (slot.sphereBytes.empty()) return;
+    const uint8_t* d = stageUpload(slot.sphereTables, slot.sphereBytes, s, used);
+    for (int p = 0; p < numPlanes; ++p) {
+      const size_t at = slot.sphereAt[p ? 1 : 0];
+      if (at != SIZE_MAX) tables[p] = reinterpret_cast<const float*>(d + at);
+    }
+  }
+
   int planIndexOf(const DevicePlan& plan) {  // the transformMatPlaneIndex a plan was generated for
     std::lock_guard<std::mutex> lock(mu_);
     for (auto& kv : plans_)
@@ -1678,13 +2040,14 @@ class VideoFrameTransform {
   }
 
   FrameTransformContext ctx_;
-  // Every entry point that enqueues work holds configMu_ shared for as long as it uses a plan; reconfigure() swaps the
-  // plans under it exclusively.  planMu_ serialises planning (generateMapForPlane, reconfigure) and guards ctx_.  Lock
-  // order: planMu_, configMu_, hostCallMu_, then the others.
+  // Every entry point that enqueues work holds configMu_ shared for as long as it uses a plan or ctx_; install() swaps the
+  // plans and reconfigureAsync replaces ctx_ under it exclusively.  planMu_ serialises planning (generateMapForPlane,
+  // reconfigure, the background planner).  Lock order: planMu_, configMu_, asyncMu_, hostCallMu_, then the others.
+  // Nothing waits for the background planner while holding configMu_ or planMu_.
   std::shared_mutex configMu_;
   std::mutex planMu_;
   std::mutex mu_;
-  std::mutex lazyMu_;  // per-size tables made on first use (resizeFor, blurFor)
+  std::mutex lazyMu_;  // tables made on first use (resizeFor, blurFor, deviceWeights)
   std::map<int, DevicePlan> plans_;
   DeviceBuffer<int16_t> weights_[9];       // OpenCV's tables [1024][k][k] (general kernels), by kernel size
   DeviceBuffer<uint8_t> weightImages_[9];  // their shared-memory images for the frame kernel
@@ -1696,17 +2059,7 @@ class VideoFrameTransform {
   long long pipelineMinBytes_ = 6ll << 20;
   int pipelineChunks_ = 0, pipelineBlocks_ = 0;  // 0: automatic
   int pipelineInStreams_ = 1;
-  // The streamed call is ~100 runtime calls (chunk copies, events, wave launches, rectangle copies); issued one by one
-  // the host thread becomes the bottleneck (measured: no faster than the plain path).  For page-locked caller planes the
-  // whole sequence is captured once per (plan, buffers) into a CUDA graph and replayed with one launch.
-  struct PlaneGraph {
-    const void* plan; unsigned long long generation; const void* in; const void* out; int inPitch, outPitch;
-    const void* stagingIn; const void* stagingOut;  // (the staging planes grow on demand: a graph made for old ones is stale)
-    int inW, inH, outW, outH;
-    int kernels;
-    cudaGraphExec_t exec; unsigned long long lastUse;
-  };
-  std::vector<PlaneGraph> planeGraphs_;
+  std::vector<PlaneGraph> planeGraphs_;  // (see PlaneGraph)
   unsigned long long graphClock_ = 0;
   cudaEvent_t graphFork_ = nullptr, graphJoinIn_ = nullptr, graphJoinOut_ = nullptr;
   // opt-in page-locking of recurring pageable caller planes (ffmpeg recycles its frame pool): see pinIfRecurring()
@@ -1723,6 +2076,18 @@ class VideoFrameTransform {
   cudaStream_t stream_ = nullptr;
   int device_ = 0, numSMs_ = 0;
   bool deviceReady_ = false;
+  CUcontext cuContext_ = nullptr;  // the context current when the transform first touched CUDA (the background planner's)
+  // reconfigureAsync: ctx_ is not the context the plans were made with, so whole frames take the per-frame kernels (configMu_)
+  bool perFrameOnly_ = false;
+  // the background planner (planInBackground), under asyncMu_: reconfigureAsync calls accepted after a plan existed, and the
+  // number of the last one settled (installed, taken over by reconfigure, or failed: asyncFailed_)
+  std::mutex asyncMu_;
+  std::condition_variable asyncCv_;
+  std::thread worker_;
+  unsigned long long asyncSeq_ = 0, asyncSettled_ = 0;
+  bool asyncFailed_ = false, asyncHurry_ = false, asyncStop_ = false;
+  FrameTransformContext asyncCtx_{};
+  std::chrono::steady_clock::time_point asyncLast_{};
 };
 
 // ---- the reference C-ABI (VideoFrameTransformHandler.h:22-47) ------------------------------------------
@@ -1907,6 +2272,14 @@ T360_API int T360B200_lowPassPlaneAsync(VideoFrameTransform* t, const uint8_t* d
 T360_API int T360B200_reconfigure(VideoFrameTransform* t, const FrameTransformContext* ctx) {
   if (!t || !ctx) return 0;
   return t->reconfigure(*ctx);
+}
+T360_API int T360B200_reconfigureAsync(VideoFrameTransform* t, const FrameTransformContext* ctx) {
+  if (!t || !ctx) return 0;
+  return t->reconfigureAsync(*ctx);
+}
+T360_API int T360B200_reconfigureWait(VideoFrameTransform* t, int block) {
+  if (!t) return -1;
+  return t->reconfigureWait(block != 0);
 }
 T360_API int T360B200_transformFrameViewAsync(VideoFrameTransform* t, const T360View* view, int numPlanes, const uint8_t* const* dIn,
                                               uint8_t* const* dOut, const int* inW, const int* inH, const int* inPitch, const int* outW,

@@ -46,7 +46,6 @@ typedef struct T360CudaContext {
 
   VideoFrameTransform* transform;
   int maps_ready;
-  int pose_frames; /* a yaw, pitch, roll, hfov or vfov command arrived after the first frame: every frame passes its pose */
   int sw_format, num_planes;
   AVBufferRef* out_frames;
   AVCUDADeviceContext* cuda;
@@ -234,19 +233,10 @@ static int t360_filter_frame(AVFilterLink* inlink, AVFrame* in) {
       in_pitch[p] = in->linesize[p];
       out_pitch[p] = out->linesize[p];
     }
-    if (s->pose_frames) {
-      const T360Pose pose = {s->params.fixed_yaw, s->params.fixed_pitch, s->params.fixed_roll, s->params.fixed_hfov,
-                             s->params.fixed_vfov};
-      rc = T360B200_transformFramePoseAsync(s->transform, &pose, s->num_planes, src, dst, in_w, in_h, in_pitch, out_w, out_h,
-                                            out_pitch, s->cuda->stream)
-               ? 0
-               : AVERROR_EXTERNAL;
-    } else {
-      rc = T360B200_transformFrameAsync(s->transform, s->num_planes, src, dst, in_w, in_h, in_pitch, out_w, out_h, out_pitch,
-                                        s->cuda->stream)
-               ? 0
-               : AVERROR_EXTERNAL;
-    }
+    rc = T360B200_transformFrameAsync(s->transform, s->num_planes, src, dst, in_w, in_h, in_pitch, out_w, out_h, out_pitch,
+                                      s->cuda->stream)
+             ? 0
+             : AVERROR_EXTERNAL;
     /* `in` is released below: its buffer goes back to the decoder's pool, which may hand it out again while the
      * gather still reads it unless the stream is drained first */
     if (!rc && s->sync && cu->cuStreamSynchronize(s->cuda->stream)) rc = AVERROR_EXTERNAL;
@@ -263,15 +253,15 @@ done:
 }
 
 /* Runtime commands (sendcmd, zmq): the view and quality options below are marked AV_OPT_FLAG_RUNTIME_PARAM.  Before the
- * first frame a command only updates the parameters; after it the running transform is re-planned for them
- * (T360B200_reconfigure: frames filtered before the command keep the old view, every later frame has the new one).
+ * first frame a command only updates the parameters.  After it, every accepted command hands the updated parameters to
+ * T360B200_reconfigureAsync, which returns in microseconds without re-planning: frames filtered before the command keep
+ * the old parameters, every later frame has the new ones.  The transform serves those frames on its per-frame kernels
+ * while it plans the new parameters in the background, once commands have paused for a quarter of a second, and then
+ * returns to the planned frame kernel by itself; the frames are the same either way.  So the camera can move every frame
+ * (head tracking, a camera path, stabilisation) and a quality change does not stall the pipeline for a re-plan.
  * Options that could change the output link's size or format (size, cube edge, layouts, stereo formats, scale factors)
- * are refused with ENOSYS, invalid values with EINVAL; a refused command leaves every parameter as it was.
- * The pose commands (yaw, pitch, roll, hfov, vfov) after the first frame re-plan nothing, whatever the layout: they update
- * the parameters, and from then on every frame goes through T360B200_transformFramePoseAsync with the current pose, so
- * the camera can move every frame (head tracking, a camera path, stabilisation) at the cost of a frame, not of a re-plan.
- * The filter then stays on the per-frame kernels, which take longer per frame than the planned one (DESIGN.md 6); later
- * commands of other options reconfigure with parameters that already hold the current pose.
+ * are refused with ENOSYS, invalid values (including parameters the transform refuses) with EINVAL; a refused command
+ * leaves every parameter as it was.
  * This needs AV_OPT_FLAG_RUNTIME_PARAM and ff_filter_process_command (FFmpeg 4.2 and later).  A libavfilter without
  * runtime options builds the filter without commands: the options are then fixed at init, as in the reference filter. */
 #ifdef AV_OPT_FLAG_RUNTIME_PARAM
@@ -294,18 +284,7 @@ static int t360_process_command(AVFilterContext* ctx, const char* cmd, const cha
     return AVERROR(EINVAL);
   }
   if (!s->maps_ready) return 0;
-  if (!strcmp(cmd, "yaw") || !strcmp(cmd, "pitch") || !strcmp(cmd, "roll") || !strcmp(cmd, "hfov") || !strcmp(cmd, "vfov")) {
-    s->pose_frames = 1;
-    return 0;
-  }
-  CudaFunctions* cu = s->cuda->internal->cuda_dl;
-  CUcontext popped;
-  if (cu->cuCtxPushCurrent(s->cuda->cuda_ctx)) {
-    s->params = before;
-    return AVERROR_EXTERNAL;
-  }
-  rc = T360B200_reconfigure(s->transform, &s->params) ? 0 : AVERROR(EINVAL);
-  cu->cuCtxPopCurrent(&popped);
+  rc = T360B200_reconfigureAsync(s->transform, &s->params) ? 0 : AVERROR(EINVAL); /* (host checks only: no CUDA call) */
   if (rc) {
     s->params = before;
     av_log(ctx, AV_LOG_ERROR, "the transform refused %s=%s; the previous configuration stays in effect\n", cmd, arg);

@@ -146,6 +146,10 @@ def load(path: os.PathLike | None = None):
     L.T360B200_lowPassPlaneAsync.argtypes = [vp, vp, vp] + [ci] * 5 + [vp]
     L.T360B200_reconfigure.restype = ci
     L.T360B200_reconfigure.argtypes = [vp, C.POINTER(FrameTransformContext)]
+    L.T360B200_reconfigureAsync.restype = ci
+    L.T360B200_reconfigureAsync.argtypes = [vp, C.POINTER(FrameTransformContext)]
+    L.T360B200_reconfigureWait.restype = ci
+    L.T360B200_reconfigureWait.argtypes = [vp, ci]
     L.T360B200_transformFrameViewAsync.restype = ci
     L.T360B200_transformFrameViewAsync.argtypes = [vp, C.POINTER(T360View), ci, vp, vp] + [vp] * 6 + [vp]
     L.T360B200_viewSamples.restype = ci
@@ -186,7 +190,8 @@ EXPORTED_SYMBOLS = [
     "T360B200_hostPlanInfo", "T360B200_hostPlanMap", "T360B200_hostPlanSamples", "T360B200_hostPlanSegment",
     "T360B200_hostPlanGather", "T360B200_hostPlanPoleCaps", "T360B200_hostPlanBlurLists", "T360B200_weightImage", "T360B200_dealLanes",
     "T360B200_remapTable", "T360B200_transformFramePlaneAsync", "T360B200_transformFrameAsync",
-    "T360B200_lowPassPlaneAsync", "T360B200_reconfigure", "T360B200_transformFrameViewAsync", "T360B200_viewSamples",
+    "T360B200_lowPassPlaneAsync", "T360B200_reconfigure", "T360B200_reconfigureAsync", "T360B200_reconfigureWait",
+    "T360B200_transformFrameViewAsync", "T360B200_viewSamples",
     "T360B200_transformFrameOrientedAsync", "T360B200_orientedSamples", "T360B200_transformFramePoseAsync", "T360B200_poseSamples",
     "T360B200_setPinHostPlanes", "T360B200_debugTrace", "T360B200_debugTraceRead", "T360B200_synchronize", "T360B200_stream", "T360B200_kernelLaunchCount", "T360B200_planDeviceBytes",
     "T360B200_planTileCounts", "T360B200_deviceCount", "T360B200_version",
@@ -329,6 +334,20 @@ class VideoFrameTransform:
         if not self._lib.T360B200_reconfigure(self._h, C.byref(ctx)):
             raise RuntimeError("T360B200_reconfigure returned 0 (message on stdout); the old configuration is still in effect")
         self.ctx = ctx
+
+    def reconfigure_async(self, ctx: FrameTransformContext) -> None:
+        """Replaces the context without waiting for a re-plan (T360B200_reconfigureAsync): frames enqueued after the call
+        use `ctx`, served by the per-frame kernels until its plans, made in the background, are in.  Raises on refusal
+        (layouts, stereo formats or scale factors changed, unknown interpolation, non-finite fields, a context the
+        low-pass planner refuses), which leaves the old context in effect."""
+        if not self._lib.T360B200_reconfigureAsync(self._h, C.byref(ctx)):
+            raise RuntimeError("T360B200_reconfigureAsync returned 0 (message on stdout); the old context is still in effect")
+        self.ctx = ctx
+
+    def reconfigure_wait(self, block: bool = True) -> int:
+        """T360B200_reconfigureWait: 1 when the current context's plans are in effect, 0 while they are pending (only with
+        block=False), -1 when the background planner failed (frames are still served, by the per-frame kernels)."""
+        return self._lib.T360B200_reconfigureWait(self._h, 1 if block else 0)
 
     def set_pin_host_planes(self, enable: bool) -> None:
         self._lib.T360B200_setPinHostPlanes(self._h, 1 if enable else 0)
