@@ -21,6 +21,14 @@ typedef struct T360HostPlan T360HostPlan;
  * for one plane and keeps the result in host memory. */
 T360HostPlan* T360B200_hostPlanCreate(const FrameTransformContext* ctx, int inputWidth, int inputHeight,
                                       int outputWidth, int outputHeight);
+/* cv::remap's border modes for a caller's warp map (OpenCV's values) */
+#define T360_BORDER_WRAP 3
+#define T360_BORDER_TRANSPARENT 5
+/* The host twin of T360B200_generateMapFromWarp: the plan of one plane from the caller's map, in host memory, for the
+ * inspectors above and below (map = the caller's map, mapWidth x mapHeight, no low-pass segments).  NULL, with a message on
+ * stdout, for whatever T360B200_generateMapFromWarp refuses. */
+T360HostPlan* T360B200_hostPlanCreateFromWarp(const FrameTransformContext* ctx, const float* map, int mapWidth, int mapHeight,
+                                              int inputWidth, int inputHeight, int border);
 void T360B200_hostPlanDestroy(T360HostPlan* plan);
 /* info[0..5] = mapWidth, mapHeight, numSegments, numTaps, kernelSizeOfInterpolation, numTileJobs */
 int T360B200_hostPlanInfo(const T360HostPlan* plan, int info[6]);
@@ -68,6 +76,34 @@ int T360B200_hostPlanSegment(const T360HostPlan* plan, int i, int rect[4], int n
                              const float** ky);
 /* OpenCV-compatible fixed-point interpolation table: int16 [1024][k][k]; returns k (0 if unsupported) */
 int T360B200_remapTable(int interpolationAlg, const int16_t** table);
+
+/* ---- warp maps: remap through the caller's own map ------------------------------------------------ */
+/* Installs the plan of plan index transformMatPlaneIndex, as VideoFrameTransform_generateMapForPlane does, from the caller's
+ * map instead of the context's geometry: `map` (host memory, float32 [mapHeight][mapWidth][2], cv::remap's CV_32FC2 map: the
+ * source x, y of every output pixel) is sampled from planes of inputWidth x inputHeight with the context's interpolation_alg
+ * and `border` (T360_BORDER_WRAP or T360_BORDER_TRANSPARENT), bit for bit as cv::remap does (NaN, infinities and coordinates
+ * beyond the int16 range included).  Every frame entry point then serves the index unchanged (transformFramePlane with host
+ * or device planes, T360B200_transformFramePlaneAsync, T360B200_transformFrameAsync); an output size other than the map's
+ * takes the INTER_AREA resize, and under BORDER_TRANSPARENT chroma outputs (plan index 1) are pre-filled with 128 while luma
+ * outputs keep the caller's bytes where no source pixel lands.  Returns 1 on success; 0 with a message on stdout, before any
+ * CUDA call, for a NULL map, non-positive sizes, a map larger than 65536 in a dimension, another border, an unknown
+ * interpolation_alg or enable_low_pass_filter != 0.  While an index holds such a plan, T360B200_reconfigure,
+ * T360B200_reconfigureAsync and the view, orientation and pose calls are refused (0, a message, no CUDA call);
+ * VideoFrameTransform_generateMapForPlane on the index replaces the warp plan. */
+int T360B200_generateMapFromWarp(VideoFrameTransform* transform, const float* map, int mapWidth, int mapHeight, int inputWidth,
+                                 int inputHeight, int border, int transformMatPlaneIndex);
+/* One frame through per-plane maps in device memory, a map per plane of its output plane's size (float32 pairs, row r at
+ * deviceMaps[p] + r * mapPitches[p] bytes; the base 8-byte aligned, the pitch a multiple of 8 of at least 8 x the output
+ * width): the frame T360B200_generateMapFromWarp with the same maps would give, with the context's interpolation_alg and
+ * `border`, BORDER_TRANSPARENT's chroma pre-fill included, and no plan: one kernel launch gathers every plane, each pixel's
+ * sampling record computed from its map entry.  The asynchronous contract of T360B200_transformFrameAsync: the call never
+ * synchronises the device, so the maps may change every frame (keep them alive until the frame is done).  Returns 1 if
+ * everything was enqueued; 0 with a message on stdout, before any CUDA call, for 0 or more than 3 planes, NULL maps or
+ * planes, a map pitch or alignment as above violated, another border, an unknown interpolation_alg or low-pass on. */
+int T360B200_remapFrameAsync(VideoFrameTransform* transform, int numPlanes, const float* const* deviceMaps, const int* mapPitches,
+                             int border, const uint8_t* const* deviceInputs, uint8_t* const* deviceOutputs, const int* inputWidths,
+                             const int* inputHeights, const int* inputPitches, const int* outputWidths, const int* outputHeights,
+                             const int* outputPitches, void* cudaStream);
 
 /* ---- device-resident / asynchronous entry points ----------------------------------------------- */
 /* Same contract as VideoFrameTransform_transformFramePlane, but both planes are CUDA device pointers,

@@ -63,7 +63,8 @@ struct HostPlan {
   int outW = 0, outH = 0;   // as requested by the caller
   int mapW = 0, mapH = 0;   // scaled output size (== outW x outH unless *_scale_factor != 1)
   int kernelSize = 0;       // 1, 2, 4, 8 taps per axis
-  bool transparentBorder = false;  // barrel layouts (reference cpp:716-719)
+  bool transparentBorder = false;  // barrel layouts (reference cpp:716-719), or a caller's warp map with BORDER_TRANSPARENT
+  bool warp = false;               // map is a caller's warp map (buildWarpHostPlan): ctx contributes its interpolation only
   std::vector<float> map;          // [mapH][mapW][2]
   std::vector<SamplePoint> samples;  // [mapH][mapW]
   std::vector<LowPassSegment> segments;
@@ -101,5 +102,17 @@ void buildAreaResizePlan(HostPlan& plan);
 
 // Whole plan for one plane; returns false (message on stdout) on invalid parameters.
 bool buildHostPlan(const FrameTransformContext& ctx, int inW, int inH, int outW, int outH, HostPlan& plan);
+
+// cv::remap's border modes a caller's warp map may use (OpenCV's values)
+constexpr int kBorderWrap = 3, kBorderTransparent = 5;
+// The largest warp map per axis: pole-cap records hold 16-bit output positions.
+constexpr int kMaxWarpMapSide = 65536;
+// Whole plan for one plane from a caller's CV_32FC2 map [mapH][mapW][2] (host memory) instead of the context's geometry:
+// the map is sampled from an inW x inH plane with ctx's interpolation and `border`, rendered at mapW x mapH (outW x outH
+// = the map's size), without low-pass.  Returns false (message on stdout) for a null map, non-positive sizes, a map side
+// above kMaxWarpMapSide, a border other than kBorderWrap / kBorderTransparent, an unknown interpolation_alg and low-pass
+// on (the reference derives its segments from the output layout, which a caller's map does not have).
+bool buildWarpHostPlan(const FrameTransformContext& ctx, const float* map, int mapW, int mapH, int inW, int inH, int border,
+                       HostPlan& plan);
 
 }  // namespace t360

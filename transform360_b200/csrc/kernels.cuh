@@ -366,6 +366,31 @@ struct OrientedGatherParams {
 };
 cudaError_t launchOrientedGather(OrientedGatherParams p, int numSMs, cudaStream_t stream);
 
+// ---- the per-frame warp-map gather (view_gather.cu) -----------------------------------------------------------------
+// Frames remapped through the caller's own CV_32FC2 map, one per plane and of the output plane's size, in device memory:
+// the kernel converts every pixel's map entry into its sampling record with quantizeAxis (flat_view.h), as quantizeWarpMap
+// does for a planned map.  Same tiles, threads and taps as the per-view gather; BORDER_WRAP or BORDER_TRANSPARENT.
+struct MapGeometry {
+  int mapW, mapH, inW, inH;
+};
+struct MapPlane {
+  const uint8_t* src;  // input plane, geometry.inW x geometry.inH
+  uint8_t* dst;        // output plane, geometry.mapW x geometry.mapH
+  int srcPitch, dstPitch;
+  const float2* map;   // [mapH][mapPitch] (x, y) source positions
+  int mapPitch;        // in float2
+  MapGeometry geometry;
+  int tilesX, firstTile;  // filled by launchMapGather
+};
+struct MapGatherParams {
+  MapPlane plane[kMaxFramePlanes];
+  int numPlanes;
+  bool transparent;
+  const int16_t* weights;  // device copy of the [1024][k][k] table (nullptr for nearest)
+  int kernelSize;
+};
+cudaError_t launchMapGather(MapGatherParams p, int numSMs, cudaStream_t stream);
+
 // bytes of dynamic shared memory a blur tile of (w x h) with the given tap counts needs
 inline int blurTileSmem(int w, int h, int nkx, int nky) {
   const int hx = nkx / 2, hy = nky / 2;

@@ -212,6 +212,40 @@ void buildAreaResize(int srcW, int srcH, int dstW, int dstH, AreaResizePlan& r) 
 
 void buildAreaResizePlan(HostPlan& plan) { buildAreaResize(plan.mapW, plan.mapH, plan.outW, plan.outH, plan.resize); }
 
+namespace {
+// What every plan does with its float map: the fixed-point records (when there is an interpolator) and the area resize.
+void samplePlan(HostPlan& plan) {
+  if (plan.kernelSize > 0) quantizeWarpMap(plan);
+  buildAreaResizePlan(plan);
+}
+}  // namespace
+
+bool buildWarpHostPlan(const FrameTransformContext& ctx, const float* map, int mapW, int mapH, int inW, int inH, int border,
+                       HostPlan& plan) {
+  plan = HostPlan{};
+  plan.ctx = ctx;
+  const char* why = nullptr;
+  if (!map) why = "the map is NULL";
+  else if (mapW <= 0 || mapH <= 0 || inW <= 0 || inH <= 0) why = "non-positive map or input size";
+  else if (mapW > kMaxWarpMapSide || mapH > kMaxWarpMapSide) why = "the map is larger than 65536 in a dimension";
+  else if (border != kBorderWrap && border != kBorderTransparent) why = "border must be 3 (BORDER_WRAP) or 5 (BORDER_TRANSPARENT)";
+  else if (kernelSizeOf(ctx.interpolation_alg) == 0) why = "unknown interpolation_alg";
+  else if (ctx.enable_low_pass_filter) why = "the low-pass filter needs an output layout (set enable_low_pass_filter = 0)";
+  if (why) {
+    std::printf("Could not generate map from a warp map: %s (map %dx%d, input %dx%d, border %d).\n", why, mapW, mapH, inW, inH, border);
+    return false;
+  }
+  plan.inW = inW; plan.inH = inH;
+  plan.outW = plan.mapW = mapW;
+  plan.outH = plan.mapH = mapH;
+  plan.kernelSize = kernelSizeOf(ctx.interpolation_alg);
+  plan.transparentBorder = border == kBorderTransparent;
+  plan.warp = true;
+  plan.map.assign(map, map + static_cast<size_t>(mapW) * mapH * 2);
+  samplePlan(plan);
+  return true;
+}
+
 bool buildHostPlan(const FrameTransformContext& ctx, int inW, int inH, int outW, int outH, HostPlan& plan) {
   plan = HostPlan{};
   plan.ctx = ctx;
@@ -230,8 +264,7 @@ bool buildHostPlan(const FrameTransformContext& ctx, int inW, int inH, int outW,
   plan.kernelSize = kernelSizeOf(ctx.interpolation_alg);
   plan.transparentBorder = ctx.output_layout == LAYOUT_BARREL || ctx.output_layout == LAYOUT_BARREL_SPLIT;
   if (!buildWarpMap(plan)) return false;
-  if (plan.kernelSize > 0) quantizeWarpMap(plan);
-  buildAreaResizePlan(plan);
+  samplePlan(plan);
   if (ctx.enable_low_pass_filter) {
     // (num_horizontal_segments <= 0 is not an error in the reference: with adjust_kernel its tile loop simply does not
     // run, cpp:235, so every band is left without tiles and the "blurred" plane stays zero; without adjust_kernel the

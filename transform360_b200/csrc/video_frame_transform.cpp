@@ -85,6 +85,7 @@ struct DevicePlan {
   int inW = 0, inH = 0, outW = 0, outH = 0, mapW = 0, mapH = 0;
   int kernelSize = 0;
   bool transparent = false, lowPass = false;
+  bool warp = false;  // made from a caller's warp map (generateMapFromWarp): no geometry to re-plan or to compute per frame
   int stereoFormat = STEREO_FORMAT_MONO;  // input_stereo_format of the context the plan was made with (low-pass passes)
   DeviceBuffer<int2> samples;      // full records: tile-major, lane-ordered, 8 bytes per pixel (whole-plane general kernels)
   DeviceBuffer<uint32_t> records;  // compact records of the frame kernel's jobs (kernels.cuh): 2.5 - 4 bytes per pixel (pole caps: 8)
@@ -144,9 +145,19 @@ struct HostIndexPlan {
   HostPlan host;
   t360::GatherPlan gather;
 };
+// The gather plan of a host plan: staged (the persistent frame kernel's jobs) for k >= 2 under BORDER_WRAP.
+void gatherOnHost(HostIndexPlan& p) {
+  if (p.host.kernelSize > 0) t360::buildGatherPlan(p.host, p.host.kernelSize >= 2 && !p.host.transparentBorder, p.gather);
+}
 bool planOnHost(const FrameTransformContext& ctx, int inW, int inH, int outW, int outH, HostIndexPlan& p) {
   if (!t360::buildHostPlan(ctx, inW, inH, outW, outH, p.host)) return false;
-  if (p.host.kernelSize > 0) t360::buildGatherPlan(p.host, p.host.kernelSize >= 2 && !p.host.transparentBorder, p.gather);
+  gatherOnHost(p);
+  return true;
+}
+// ... from a caller's warp map instead of the context's geometry (T360B200_generateMapFromWarp)
+bool planWarpOnHost(const FrameTransformContext& ctx, const float* map, int mapW, int mapH, int inW, int inH, int border, HostIndexPlan& p) {
+  if (!t360::buildWarpHostPlan(ctx, map, mapW, mapH, inW, inH, border, p.host)) return false;
+  gatherOnHost(p);
   return true;
 }
 
@@ -394,6 +405,23 @@ class VideoFrameTransform {
 
   // reference generateMapForPlane (cpp:504-576): plan on the host, upload once.
   bool generateMapForPlane(int inW, int inH, int outW, int outH, int planIndex) {
+    return installPlan(planIndex, [&](const FrameTransformContext& ctx, HostIndexPlan& host) {
+      return planOnHost(ctx, inW, inH, outW, outH, host);
+    });
+  }
+
+  // T360B200_generateMapFromWarp: as generateMapForPlane, from the caller's map (buildWarpHostPlan refuses before any CUDA
+  // call)
+  bool generateMapFromWarp(const float* map, int mapW, int mapH, int inW, int inH, int border, int planIndex) {
+    return installPlan(planIndex, [&](const FrameTransformContext& c, HostIndexPlan& host) {
+      return planWarpOnHost(c, map, mapW, mapH, inW, inH, border, host);
+    });
+  }
+
+  // Plans index planIndex on the host with the current context (plan(ctx, host), false: refused with a message), uploads it
+  // and installs it in place of the index's previous plan.
+  template <class Plan>
+  bool installPlan(int planIndex, Plan&& plan) {
     try {
       reconfigureWait(true);  // a pending reconfigureAsync re-plans the other indices: it is finished first
       std::lock_guard<std::mutex> planLock(planMu_);
@@ -403,11 +431,11 @@ class VideoFrameTransform {
         ctx = ctx_;
       }
       HostIndexPlan host;
-      if (!planOnHost(ctx, inW, inH, outW, outH, host)) return false;
+      if (!plan(ctx, host)) return false;
       const DeviceRestore restoreDevice = ensureDevice();
-      DevicePlan plan = upload(host, ctx);
+      DevicePlan d = upload(host, ctx);
       std::lock_guard<std::mutex> lock(mu_);
-      plans_[planIndex] = std::move(plan);
+      plans_[planIndex] = std::move(d);
       ++planGeneration_;
       return true;
     } catch (const CudaFail& f) {
@@ -427,6 +455,7 @@ class VideoFrameTransform {
   bool reconfigure(const FrameTransformContext& next) {
     try {
       std::lock_guard<std::mutex> planLock(planMu_);  // (one re-plan at a time, also against generateMapForPlane)
+      if (refuseWarpPlans("Could not reconfigure the transform")) return false;
       unsigned long long seq;
       {
         std::lock_guard<std::mutex> async(asyncMu_);
@@ -459,6 +488,7 @@ class VideoFrameTransform {
   // made by the background planner (planInBackground).  Host checks only: every refusal comes before any CUDA call, and so
   // does the return.
   bool reconfigureAsync(const FrameTransformContext& next) {
+    if (refuseWarpPlans("Could not reconfigure the transform asynchronously")) return false;
     const std::vector<PlanSizes> sizes = plannedSizes();
     if (const char* why = asyncRefusal(next, sizes)) {
       std::printf("Could not reconfigure the transform asynchronously. Error: %s\n", why);
@@ -1033,6 +1063,71 @@ class VideoFrameTransform {
     return perFrame("with a pose", substitute, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, stream);
   }
 
+  // Whole frame through the caller's per-plane device maps (T360B200_remapFrameAsync): one gather launch for all planes,
+  // every record computed from its map entry as quantizeWarpMap does, so a map gives what generateMapFromWarp plans for it.
+  // Needs no plan; the interpolation comes from the current context.  Every refusal comes before the first CUDA call, and
+  // nothing here synchronises the device.
+  bool remapFrame(int numPlanes, const float* const* maps, const int* mapPitch, int border, const uint8_t* const* dIn, uint8_t* const* dOut,
+                  const int* inW, const int* inH, const int* inPitch, const int* outW, const int* outH, const int* outPitch, cudaStream_t stream) {
+    const char* what = "Could not remap the frame";
+    try {
+      if (numPlanes < 1 || numPlanes > kPlaneLanes) {
+        std::printf("%s. Error: %d planes (1..%d supported)\n", what, numPlanes, kPlaneLanes);
+        return false;
+      }
+      if (border != t360::kBorderWrap && border != t360::kBorderTransparent) {
+        std::printf("%s. Error: border %d (3: BORDER_WRAP, 5: BORDER_TRANSPARENT)\n", what, border);
+        return false;
+      }
+      for (int p = 0; p < numPlanes; ++p) {
+        if (!maps[p] || !dIn[p] || !dOut[p] || inW[p] <= 0 || inH[p] <= 0 || outW[p] <= 0 || outH[p] <= 0 || inPitch[p] < inW[p] ||
+            outPitch[p] < outW[p]) {
+          std::printf("%s. Error: invalid description of plane %d\n", what, p);
+          return false;
+        }
+        if (mapPitch[p] % 8 != 0 || mapPitch[p] / 8 < outW[p] || (reinterpret_cast<uintptr_t>(maps[p]) & 7)) {
+          std::printf("%s. Error: the map of plane %d (pitch %d bytes) must be 8-byte aligned with a pitch that is a multiple of 8 and at "
+                      "least 8 x the output width %d\n", what, p, mapPitch[p], outW[p]);
+          return false;
+        }
+      }
+      std::shared_lock<std::shared_mutex> config(configMu_);
+      const FrameTransformContext ctx = ctx_;
+      const int k = t360::kernelSizeOf(ctx.interpolation_alg);
+      if (k == 0) {
+        std::printf("%s. Error: no interpolation algorithm %d\n", what, ctx.interpolation_alg);
+        return false;
+      }
+      if (ctx.enable_low_pass_filter) {
+        std::printf("%s. Error: the low-pass filter needs an output layout (set enable_low_pass_filter = 0)\n", what);
+        return false;
+      }
+      const DeviceRestore restoreDevice = ensureDevice();
+      cudaStream_t s = stream ? stream : stream_;
+      const bool transparent = border == t360::kBorderTransparent;
+      t360::MapGatherParams mp{};
+      for (int p = 0; p < numPlanes; ++p) {
+        // BORDER_TRANSPARENT leaves a pixel whose anchor tap lies outside the source as it finds it: chroma outputs start at
+        // 128 as in the planned path (reference cpp:743-747), luma outputs keep the caller's bytes
+        if (transparent && p) CU(cudaMemset2DAsync(dOut[p], outPitch[p], 128, outW[p], outH[p], s));
+        mp.plane[p] = t360::MapPlane{dIn[p], dOut[p], inPitch[p], outPitch[p], reinterpret_cast<const float2*>(maps[p]), mapPitch[p] / 8,
+                                     t360::MapGeometry{outW[p], outH[p], inW[p], inH[p]}, 0, 0};
+      }
+      mp.numPlanes = numPlanes;
+      mp.kernelSize = k;
+      mp.transparent = transparent;
+      mp.weights = deviceWeights(ctx.interpolation_alg);
+      CU(t360::launchMapGather(mp, numSMs_, s));
+      return true;
+    } catch (const CudaFail& f) {
+      std::printf("%s. Error: CUDA %s (%s) in %s\n", what, cudaGetErrorName(f.err), cudaGetErrorString(f.err), f.what);
+      cudaGetLastError();
+    } catch (const std::exception& ex) {
+      std::printf("%s. Error: %s\n", what, ex.what());
+    }
+    return false;
+  }
+
   static void substitutePose(FrameTransformContext& ctx, const T360Pose& pose) {
     ctx.fixed_yaw = pose.yaw;
     ctx.fixed_pitch = pose.pitch;
@@ -1048,6 +1143,7 @@ class VideoFrameTransform {
   bool perFrame(const char* what, Substitute& substitute, int numPlanes, const uint8_t* const* dIn, uint8_t* const* dOut, const int* inW,
                 const int* inH, const int* inPitch, const int* outW, const int* outH, const int* outPitch, cudaStream_t stream) {
     std::shared_lock<std::shared_mutex> config(configMu_);
+    if (refuseWarpPlans((std::string("Could not transform the frame ") + what).c_str())) return false;
     FrameTransformContext ctx = ctx_;
     if (!substitute(ctx)) return false;
     return perFrameLocked(what, ctx, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, stream);
@@ -1324,6 +1420,7 @@ class VideoFrameTransform {
     d.inW = h.inW; d.inH = h.inH; d.outW = h.outW; d.outH = h.outH; d.mapW = h.mapW; d.mapH = h.mapH;
     d.kernelSize = h.kernelSize;
     d.transparent = h.transparentBorder;
+    d.warp = h.warp;
     d.stereoFormat = ctx.input_stereo_format;
     if (d.kernelSize > 0) {
       deviceWeights(ctx.interpolation_alg);
@@ -1357,7 +1454,7 @@ class VideoFrameTransform {
     }
     d.resizeNeeded = h.resize.needed;
     if (d.resizeNeeded) resizeFor(d, d.outW, d.outH);
-    if (d.kernelSize > 0 && ctx.output_layout != LAYOUT_FLAT_FIXED) {
+    if (d.kernelSize > 0 && !d.warp && ctx.output_layout != LAYOUT_FLAT_FIXED) {  // (a warp map has no layout)
       const std::vector<float> t = t360::buildSphereTables(t360::sphereGeometry(ctx, h.mapW, h.mapH, h.inW, h.inH, h.kernelSize));
       if (!t.empty()) {
         d.sphereTables.reserve(t.size());
@@ -1811,6 +1908,19 @@ class VideoFrameTransform {
     return true;
   }
 
+  // Whether some plan index holds a plan made from a caller's warp map; if so the calls that derive positions from the
+  // context (re-plans, per-frame views, orientations and poses) are refused with a message prefixed by `what`.
+  bool refuseWarpPlans(const char* what) {
+    std::lock_guard<std::mutex> lock(mu_);
+    for (const auto& kv : plans_)
+      if (kv.second.warp) {
+        std::printf("%s. Error: plan index %d was generated from a warp map, which has no geometry to re-plan or to move "
+                    "(generateMapForPlane on the index replaces it)\n", what, kv.first);
+        return true;
+      }
+    return false;
+  }
+
   // The reader lock for an entry point that needs the plans of the current context: while a reconfigureAsync is pending it
   // first waits for them (without the settle interval).  Not owning the lock: the background planner failed (message).
   std::shared_lock<std::shared_mutex> lockPlanned(const char* what) {
@@ -2104,6 +2214,12 @@ T360_API int VideoFrameTransform_generateMapForPlane(VideoFrameTransform* transf
   return transform->generateMapForPlane(inputWidth, inputHeight, outputWidth, outputHeight, transformMatPlaneIndex);
 }
 
+T360_API int T360B200_generateMapFromWarp(VideoFrameTransform* t, const float* map, int mapW, int mapH, int inW, int inH, int border,
+                                          int planIndex) {
+  if (!t) return 0;
+  return t->generateMapFromWarp(map, mapW, mapH, inW, inH, border, planIndex);
+}
+
 T360_API int VideoFrameTransform_transformFramePlane(VideoFrameTransform* transform, uint8_t* inputData,
                                                      uint8_t* outputData, int inputWidth, int inputHeight,
                                                      int inputWidthWithPadding, int outputWidth, int outputHeight,
@@ -2129,6 +2245,19 @@ T360_API T360HostPlan* T360B200_hostPlanCreate(const FrameTransformContext* ctx,
   if (!p) return nullptr;
   try {
     if (!t360::buildHostPlan(*ctx, inW, inH, outW, outH, p->plan)) return nullptr;
+  } catch (const std::exception& ex) {
+    std::printf("Could not build the host plan. Error: %s\n", ex.what());
+    return nullptr;
+  }
+  return p.release();
+}
+T360_API T360HostPlan* T360B200_hostPlanCreateFromWarp(const FrameTransformContext* ctx, const float* map, int mapW, int mapH, int inW,
+                                                       int inH, int border) {
+  if (!ctx) return nullptr;
+  std::unique_ptr<T360HostPlan> p(new (std::nothrow) T360HostPlan);
+  if (!p) return nullptr;
+  try {
+    if (!t360::buildWarpHostPlan(*ctx, map, mapW, mapH, inW, inH, border, p->plan)) return nullptr;
   } catch (const std::exception& ex) {
     std::printf("Could not build the host plan. Error: %s\n", ex.what());
     return nullptr;
@@ -2385,6 +2514,16 @@ T360_API int T360B200_poseSamples(const FrameTransformContext* ctx, const T360Po
   FrameTransformContext c = *ctx;
   VideoFrameTransform::substitutePose(c, *pose);
   return perFrameSamples("pose", c, inW, inH, outW, outH, samples);
+}
+T360_API int T360B200_remapFrameAsync(VideoFrameTransform* t, int numPlanes, const float* const* maps, const int* mapPitches, int border,
+                                      const uint8_t* const* dIn, uint8_t* const* dOut, const int* inW, const int* inH, const int* inPitch,
+                                      const int* outW, const int* outH, const int* outPitch, void* stream) {
+  if (!t || !maps || !mapPitches || !dIn || !dOut || !inW || !inH || !inPitch || !outW || !outH || !outPitch) {
+    std::printf("Could not remap the frame. Error: a NULL argument\n");
+    return 0;
+  }
+  return t->remapFrame(numPlanes, maps, mapPitches, border, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch,
+                       static_cast<cudaStream_t>(stream));
 }
 T360_API void T360B200_setPinHostPlanes(VideoFrameTransform* t, int enable) { if (t) t->setPinHostPlanes(enable != 0); }
 T360_API void T360B200_debugTrace(VideoFrameTransform* t, int enable) { if (t) t->enableTrace(enable != 0); }

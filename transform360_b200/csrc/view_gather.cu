@@ -12,7 +12,8 @@
 //     column table (32 columns x fold x eye) and a row table (rows x eye) in shared memory and each pixel combines them.
 //   - sphere outputs (SpherePositions): the rotation mixes both axes, so every pixel runs the whole chain
 //     (oriented_view.h: sphereSample), with the plan's per-column / per-row tables for the view-independent libm steps.
-// In both, the records come from the same host/device functions the planner (or its host twin) uses: bit-identical.
+//   - a caller's warp map (MapPositions): the pixel's map entry, quantised by quantizeAxis.
+// In all three, the records come from the same host/device functions the planner (or its host twin) uses: bit-identical.
 #include "gather_common.cuh"
 
 #include <algorithm>
@@ -113,6 +114,21 @@ struct SpherePositions {
   }
 };
 
+// A caller's warp map: the pixel's (x, y) from the map (a warp's lanes read 32 consecutive entries of a row: one coalesced
+// 256-byte load), quantised as quantizeWarpMap quantises a planned map, NaN, infinities and out-of-range values included
+template <int K>
+struct MapPositions {
+  __device__ void beginTile(const MapGatherParams&, const MapPlane&, int, int) {}
+  __device__ void beginColumn(int) {}
+  __device__ void record(const MapGatherParams&, const MapPlane& v, int, int, int i, int j, int* col0, int* rowPhase) const {
+    const float2 m = __ldg(v.map + (size_t)i * v.mapPitch + j);
+    int row0, fracX, fracY;
+    quantizeAxis(m.x, K, col0, &fracX);
+    quantizeAxis(m.y, K, &row0, &fracY);
+    *rowPhase = row0 * 1024 + fracY * 32 + fracX;
+  }
+};
+
 template <int K>
 __global__ void __launch_bounds__(gatherThreads(K), K == 8 ? 1 : 4) viewGatherKernel(const __grid_constant__ ViewGatherParams p, int numTiles) {
   extern __shared__ __align__(16) unsigned char smem[];
@@ -134,6 +150,18 @@ __global__ void __launch_bounds__(gatherThreads(K), K == 8 ? 1 : 4) orientedGath
   gatherViewTiles<K, TRANSPARENT>(p, numTiles, smem, pos);
 }
 
+// TRANSPARENT: the caller's border, BORDER_TRANSPARENT instead of BORDER_WRAP
+template <int K, bool TRANSPARENT>
+__global__ void __launch_bounds__(gatherThreads(K), K == 8 ? 1 : 4) mapGatherKernel(const __grid_constant__ MapGatherParams p, int numTiles) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  MapPositions<K> pos;
+  if constexpr (K >= 2) {
+    stageWeights<K>(p.weights, smem);
+    __syncthreads();  // (no tile synchronises after this)
+  }
+  gatherViewTiles<K, TRANSPARENT>(p, numTiles, smem, pos);
+}
+
 template <int K>
 cudaError_t launchViewK(const ViewGatherParams& p, int numTiles, int numSMs, cudaStream_t stream) {
   static DeviceLaunchCfg cfgs;  // per kernel instantiation, one entry per device
@@ -148,18 +176,28 @@ cudaError_t launchViewK(const ViewGatherParams& p, int numTiles, int numSMs, cud
   return cudaGetLastError();
 }
 
-template <int K, bool TRANSPARENT>
-cudaError_t launchOrientedK(const OrientedGatherParams& p, int numTiles, int numSMs, cudaStream_t stream) {
+// The kernels whose only shared memory is the weight table (orientedGatherKernel, mapGatherKernel): instantiation Kern of
+// kernel size K, one CTA per tile up to the occupancy the __launch_bounds__ allow
+template <int K, auto Kern, class Params>
+cudaError_t launchPositionsK(const Params& p, int numTiles, int numSMs, cudaStream_t stream) {
   static DeviceLaunchCfg cfgs;
   constexpr int threads = gatherThreads(K);
   constexpr int smemBytes = K >= 2 ? weightBytes<K>() : 0;
   LaunchCfg cfg;
-  cudaError_t err = prepare<orientedGatherKernel<K, TRANSPARENT>>(cfgs, threads, smemBytes, cfg);
+  cudaError_t err = prepare<Kern>(cfgs, threads, smemBytes, cfg);
   if (err != cudaSuccess) return err;
   const int grid = std::min(numSMs * cfg.perSM, numTiles);
-  orientedGatherKernel<K, TRANSPARENT><<<grid, threads, smemBytes, stream>>>(p, numTiles);
+  Kern<<<grid, threads, smemBytes, stream>>>(p, numTiles);
   gLaunches.fetch_add(1, std::memory_order_relaxed);
   return cudaGetLastError();
+}
+template <int K, bool TRANSPARENT>
+cudaError_t launchOrientedK(const OrientedGatherParams& p, int numTiles, int numSMs, cudaStream_t stream) {
+  return launchPositionsK<K, orientedGatherKernel<K, TRANSPARENT>>(p, numTiles, numSMs, stream);
+}
+template <int K, bool TRANSPARENT>
+cudaError_t launchMapK(const MapGatherParams& p, int numTiles, int numSMs, cudaStream_t stream) {
+  return launchPositionsK<K, mapGatherKernel<K, TRANSPARENT>>(p, numTiles, numSMs, stream);
 }
 
 // tiles of every plane, in plane order
@@ -201,6 +239,20 @@ cudaError_t launchOrientedGather(OrientedGatherParams p, int numSMs, cudaStream_
     case 2: return barrel ? launchOrientedK<2, true>(p, numTiles, numSMs, stream) : launchOrientedK<2, false>(p, numTiles, numSMs, stream);
     case 4: return barrel ? launchOrientedK<4, true>(p, numTiles, numSMs, stream) : launchOrientedK<4, false>(p, numTiles, numSMs, stream);
     case 8: return barrel ? launchOrientedK<8, true>(p, numTiles, numSMs, stream) : launchOrientedK<8, false>(p, numTiles, numSMs, stream);
+    default: return cudaErrorInvalidValue;
+  }
+}
+
+cudaError_t launchMapGather(MapGatherParams p, int numSMs, cudaStream_t stream) {
+  if (p.numPlanes < 1 || p.numPlanes > kMaxFramePlanes) return cudaErrorInvalidValue;
+  const int numTiles = assignTiles(p);
+  if (numTiles <= 0) return cudaSuccess;
+  const bool t = p.transparent;
+  switch (p.kernelSize) {
+    case 1: return t ? launchMapK<1, true>(p, numTiles, numSMs, stream) : launchMapK<1, false>(p, numTiles, numSMs, stream);
+    case 2: return t ? launchMapK<2, true>(p, numTiles, numSMs, stream) : launchMapK<2, false>(p, numTiles, numSMs, stream);
+    case 4: return t ? launchMapK<4, true>(p, numTiles, numSMs, stream) : launchMapK<4, false>(p, numTiles, numSMs, stream);
+    case 8: return t ? launchMapK<8, true>(p, numTiles, numSMs, stream) : launchMapK<8, false>(p, numTiles, numSMs, stream);
     default: return cudaErrorInvalidValue;
   }
 }

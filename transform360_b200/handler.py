@@ -22,6 +22,15 @@ LAYOUT_CUBEMAP_32, LAYOUT_CUBEMAP_23_OFFCENTER, LAYOUT_FLAT_FIXED, LAYOUT_EQUIRE
 LAYOUT_BARREL, LAYOUT_BARREL_SPLIT, LAYOUT_EAC_32, LAYOUT_N = 4, 5, 6, 7
 STEREO_FORMAT_TB, STEREO_FORMAT_LR, STEREO_FORMAT_MONO, STEREO_FORMAT_GUESS, STEREO_FORMAT_N = 0, 1, 2, 3, 4
 NEAREST, LINEAR, CUBIC, LANCZOS4 = 0, 1, 2, 4
+BORDER_WRAP, BORDER_TRANSPARENT = 3, 5  # cv::remap's border modes for a caller's warp map (include/transform360_b200.h)
+
+
+def _warp_map(map) -> np.ndarray:
+    """A caller's CV_32FC2 warp map as a C-contiguous float32 [h][w][2] array."""
+    m = np.ascontiguousarray(map, np.float32)
+    if m.ndim != 3 or m.shape[2] != 2:
+        raise ValueError(f"a warp map is float32 [h][w][2] (x, y per output pixel), got shape {m.shape}")
+    return m
 
 
 class FrameTransformContext(C.Structure):
@@ -118,6 +127,12 @@ def load(path: os.PathLike | None = None):
     L.VideoFrameTransform_transformFramePlane.argtypes = [vp, vp, vp] + [ci] * 8
     L.T360B200_hostPlanCreate.restype = vp
     L.T360B200_hostPlanCreate.argtypes = [C.POINTER(FrameTransformContext)] + [ci] * 4
+    L.T360B200_hostPlanCreateFromWarp.restype = vp
+    L.T360B200_hostPlanCreateFromWarp.argtypes = [C.POINTER(FrameTransformContext), vp] + [ci] * 5
+    L.T360B200_generateMapFromWarp.restype = ci
+    L.T360B200_generateMapFromWarp.argtypes = [vp, vp] + [ci] * 6
+    L.T360B200_remapFrameAsync.restype = ci
+    L.T360B200_remapFrameAsync.argtypes = [vp, ci, vp, vp, ci] + [vp] * 8 + [vp]
     L.T360B200_hostPlanDestroy.restype = None
     L.T360B200_hostPlanDestroy.argtypes = [vp]
     L.T360B200_hostPlanInfo.restype = ci
@@ -186,7 +201,8 @@ def load(path: os.PathLike | None = None):
 
 EXPORTED_SYMBOLS = [
     "VideoFrameTransform_new", "VideoFrameTransform_delete", "VideoFrameTransform_generateMapForPlane",
-    "VideoFrameTransform_transformFramePlane", "T360B200_hostPlanCreate", "T360B200_hostPlanDestroy",
+    "VideoFrameTransform_transformFramePlane", "T360B200_hostPlanCreate", "T360B200_hostPlanCreateFromWarp", "T360B200_hostPlanDestroy",
+    "T360B200_generateMapFromWarp", "T360B200_remapFrameAsync",
     "T360B200_hostPlanInfo", "T360B200_hostPlanMap", "T360B200_hostPlanSamples", "T360B200_hostPlanSegment",
     "T360B200_hostPlanGather", "T360B200_hostPlanPoleCaps", "T360B200_hostPlanBlurLists", "T360B200_weightImage", "T360B200_dealLanes",
     "T360B200_remapTable", "T360B200_transformFramePlaneAsync", "T360B200_transformFrameAsync",
@@ -323,6 +339,44 @@ class VideoFrameTransform:
             return bool(fn(h, C.byref(as_pose(pose)), n, pin, pout, *ptrs, stream))
         return call
 
+    def generate_map_from_warp(self, map, in_w: int, in_h: int, plan_index: int, border: int = BORDER_WRAP) -> bool:
+        """T360B200_generateMapFromWarp: installs plan index `plan_index` from a caller's warp map (float32 [h][w][2], the
+        source x, y of every output pixel) for input planes of in_w x in_h, sampled with the context's interpolation and
+        `border` (BORDER_WRAP or BORDER_TRANSPARENT).  Every frame entry point then serves it.  False: refused (message on
+        stdout)."""
+        m = _warp_map(map)
+        return bool(self._lib.T360B200_generateMapFromWarp(self._h, m.ctypes.data, m.shape[1], m.shape[0], in_w, in_h, border,
+                                                           plan_index))
+
+    def make_remap_frame_call(self, in_planes, out_planes, dims, border: int = BORDER_WRAP):
+        """Like make_frame_call, for T360B200_remapFrameAsync: returns a callable f(maps, stream) -> bool that enqueues the whole
+        frame through one device map per plane, each the size of its output plane.  maps: per plane a CUDA float32 tensor
+        [out_h][>= out_w][2] (its row stride gives the pitch), a (device address, pitch in bytes) pair, or a device address
+        of a dense map."""
+        n = len(in_planes)
+        VP, IA = C.c_void_p * n, C.c_int * n
+        d_in = VP(*[p[0] for p in in_planes])
+        d_out = VP(*[p[0] for p in out_planes])
+        arrs = [IA(*[d[0] for d in dims]), IA(*[d[1] for d in dims]), IA(*[p[1] for p in in_planes]),
+                IA(*[d[2] for d in dims]), IA(*[d[3] for d in dims]), IA(*[p[1] for p in out_planes])]
+        fn, h = self._lib.T360B200_remapFrameAsync, self._h
+        ptrs = [C.cast(a, C.c_void_p) for a in arrs]
+        pin, pout = C.cast(d_in, C.c_void_p), C.cast(d_out, C.c_void_p)
+        dense = [8 * d[2] for d in dims]
+
+        def as_map(m, p):
+            if hasattr(m, "data_ptr"):
+                return m.data_ptr(), m.stride(0) * m.element_size()
+            return (int(m[0]), int(m[1])) if isinstance(m, (tuple, list)) else (int(m), dense[p])
+
+        def call(maps, stream: int = 0, _keep=(d_in, d_out, arrs)) -> bool:
+            if len(maps) != n:
+                raise ValueError(f"{len(maps)} maps for {n} planes")
+            desc = [as_map(m, p) for p, m in enumerate(maps)]
+            dmaps, pitches = VP(*[d[0] for d in desc]), IA(*[d[1] for d in desc])
+            return bool(fn(h, n, dmaps, pitches, border, pin, pout, *ptrs, stream))
+        return call
+
     def low_pass_async(self, d_in: int, d_out: int, w, h, in_pitch, out_pitch, plan_index, stream: int = 0) -> bool:
         return bool(self._lib.T360B200_lowPassPlaneAsync(self._h, d_in, d_out, w, h, in_pitch, out_pitch, plan_index,
                                                          stream))
@@ -383,14 +437,24 @@ class VideoFrameTransform:
 class HostPlan:
     """Host-side plan of one plane, computed without touching CUDA (T360B200_hostPlan*)."""
 
-    def __init__(self, ctx: FrameTransformContext, in_w, in_h, out_w, out_h):
+    def __init__(self, ctx: FrameTransformContext, in_w, in_h, out_w, out_h, _handle=None):
         self._lib = load()
-        self._h = self._lib.T360B200_hostPlanCreate(C.byref(ctx), in_w, in_h, out_w, out_h)
+        self._h = _handle or self._lib.T360B200_hostPlanCreate(C.byref(ctx), in_w, in_h, out_w, out_h)
         if not self._h:
             raise ValueError("T360B200_hostPlanCreate failed (message on stdout)")
         info = (C.c_int * 6)()
         self._lib.T360B200_hostPlanInfo(self._h, info)
         self.map_w, self.map_h, self.num_segments, self.num_taps, self.kernel_size = info[0], info[1], info[2], info[3], info[4]
+
+    @classmethod
+    def from_warp(cls, ctx: FrameTransformContext, map, in_w, in_h, border: int = BORDER_WRAP) -> "HostPlan":
+        """The host plan T360B200_generateMapFromWarp installs for a caller's warp map (T360B200_hostPlanCreateFromWarp, no
+        CUDA).  Raises ValueError when it is refused (message on stdout)."""
+        m = _warp_map(map)
+        h = load().T360B200_hostPlanCreateFromWarp(C.byref(ctx), m.ctypes.data, m.shape[1], m.shape[0], in_w, in_h, border)
+        if not h:
+            raise ValueError("T360B200_hostPlanCreateFromWarp failed (message on stdout)")
+        return cls(ctx, in_w, in_h, m.shape[1], m.shape[0], _handle=h)
 
     def close(self):
         if getattr(self, "_h", None):

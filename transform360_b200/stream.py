@@ -142,6 +142,13 @@ class FrameTransformer:
         dims = [self.spec.plane_dims(p)[:4] for p in range(self.spec.num_planes)]
         return self.vft.make_pose_frame_call(in_planes, out_planes, dims)
 
+    def remap_frame_call(self, in_planes, out_planes, border: int = H.BORDER_WRAP):
+        """Prebuilt whole-frame call through per-frame warp maps (T360B200_remapFrameAsync: one device map per plane, the size
+        of its output plane) for one (input, output) buffer pair.  Returns f(maps, stream) -> bool; maps: per plane a CUDA
+        float32 tensor [out_h][out_w][2], a (device address, pitch) pair or the device address of a dense map."""
+        dims = [self.spec.plane_dims(p)[:4] for p in range(self.spec.num_planes)]
+        return self.vft.make_remap_frame_call(in_planes, out_planes, dims, border)
+
     def transform_frame_device(self, in_planes, out_planes, stream: int = 0):
         """in_planes / out_planes: per plane (device_address, pitch).  Asynchronous on `stream`; the planes of
         the frame run concurrently on the transform's internal lanes."""
