@@ -157,7 +157,7 @@ int T360B200_reconfigure(VideoFrameTransform* transform, const FrameTransformCon
 int T360B200_reconfigureAsync(VideoFrameTransform* transform, const FrameTransformContext* ctx);
 /* Whether the plans of the current context are in effect: 1 yes; 0 not yet (block == 0); -1 the background planner failed on
  * it (message on stdout; frames keep being served by the per-frame kernels).  With block != 0 it plans at once, without the
- * settle interval, and returns 1 or -1 when done. */
+ * settle interval, and returns 1 or -1 when done, after the device memory of the plans it replaced has been released. */
 int T360B200_reconfigureWait(VideoFrameTransform* transform, int block);
 /* A FLAT_FIXED view, in degrees, as the context's fixed_yaw, fixed_pitch, fixed_hfov and fixed_vfov. */
 typedef struct T360View {
@@ -233,6 +233,62 @@ int T360B200_transformFramePoseAsync(VideoFrameTransform* transform, const T360P
  * success; 0 (message on stdout) for an unknown output layout, a non-finite pose or invalid sizes. */
 int T360B200_poseSamples(const FrameTransformContext* ctx, const T360Pose* pose, int inputWidth, int inputHeight,
                          int outputWidth, int outputHeight, int32_t* samples);
+/* ---- fisheye camera input -------------------------------------------------------------------------
+ * One or two fisheye lenses with OpenCV's fisheye (Kannala-Brandt) calibration, the K and D of cv2.fisheye.calibrate, as
+ * the input of a sphere output.
+ *
+ * Rig frame: the frame of the direction the output chain hands to the input lookup (after the off-centre warp and the
+ * rotation by the orientation, which turn the output exactly as for an equirect input): x right, y up, z forward; an
+ * equirect input would show direction d at u = atan2(x, z) / 2pi + 0.5, v = 0.5 - asin(y / |d|) / pi.
+ *
+ * Lens i: R = Ry(yaw) Rx(-pitch) Rz(roll) (Ry(a) = [[c,0,s],[0,1,0],[-s,0,c]], Rx(b) = [[1,0,0],[0,c,-s],[0,s,c]],
+ * Rz(g) = [[c,-s,0],[s,c,0],[0,0,1]]), so its optical axis is (cos pitch sin yaw, sin pitch, cos pitch cos yaw) and a back
+ * lens has yaw 180.  (X, Y', Z) = R^T d, and (X, Y, Z) = (X, -Y', Z) are OpenCV's camera coordinates (y down).
+ * rho = sqrt(X^2 + Y^2), theta = atan2(rho, Z), theta_d = theta (1 + k1 theta^2 + k2 theta^4 + k3 theta^6 + k4 theta^8),
+ * (x', y') = theta_d / rho (X, Y) ((0, 0) at rho = 0).  In a plane of inW x inH the source position is
+ * ((fx x' + cx + 0.5) / calibWidth) inW - 0.5, and likewise for y: at the calibration size fx x' + cx, which is
+ * cv2.fisheye.projectPoints (skew 0) for Z > 0; chroma planes scale the calibration as the planned layouts do.
+ * A direction goes to the lens with the larger Z / |d| (ties: lens 0), with a hard seam; theta > maxAngle, and a barrel
+ * dead zone, are uncovered.  Sampling is BORDER_TRANSPARENT: uncovered pixels and pixels whose anchor tap lies outside the
+ * source keep what the output holds (luma the caller's bytes, chroma 128, pre-filled).
+ *
+ * The context supplies the output: output_layout (CUBEMAP_32, CUBEMAP_23_OFFCENTER, EAC_32, EQUIRECT, BARREL or
+ * BARREL_SPLIT) and its geometry fields (expand_coef, fixed_cube_offcenter_*, is_horizontal_offset), vflip and
+ * interpolation_alg; the orientation comes with each call.  Not read: input_layout, input_expand_coef, both stereo formats
+ * and both scale factors (the rig is mono, and output planes are rendered at their own size).
+ *
+ * Refused, with 0 and a message on stdout before any CUDA call: a NULL rig or orientation, numLenses other than 1 or 2,
+ * non-positive calibration sizes, a non-finite field (of the orientation or of a used lens), fx or fy <= 0, maxAngle outside
+ * (0, 180], a distortion whose theta_d(theta) is not strictly increasing on [0, maxAngle] (it would mirror the image),
+ * FLAT_FIXED or an unknown output layout, enable_low_pass_filter != 0 and an unknown interpolation_alg. */
+typedef struct T360Lens {
+  float fx, fy, cx, cy; /* intrinsics in pixels of a calibWidth x calibHeight frame */
+  float k[4];           /* k1 .. k4 */
+  float yaw, pitch, roll; /* extrinsics, degrees */
+  float maxAngle;       /* half field of view covered, degrees */
+} T360Lens;
+typedef struct T360LensRig {
+  int numLenses, calibWidth, calibHeight;
+  T360Lens lens[2];
+} T360LensRig;
+/* Host only, no CUDA: the CV_32FC2 map (float32 [outputHeight][outputWidth][2], NaN where uncovered) of one plane of
+ * inputWidth x inputHeight.  T360B200_generateMapFromWarp(map, ..., T360_BORDER_TRANSPARENT, index) plans it for a fixed
+ * pose: every frame entry point, the streamed host path and the INTER_AREA resize then serve it, and frames equal, bit for
+ * bit, those of T360B200_transformFrameLensAsync for the same rig and orientation.  Returns 1; 0 (message) for the refusals
+ * above, a NULL map or non-positive sizes. */
+int T360B200_lensMap(const FrameTransformContext* ctx, const T360LensRig* rig, const T360Orientation* orientation, int inputWidth,
+                     int inputHeight, int outputWidth, int outputHeight, float* map);
+/* One frame of a lens rig, every plane in one gather launch: the arguments and the asynchronous contract of
+ * T360B200_transformFrameAsync, plus `rig` and `orientation`, both of which may change every frame.  Needs no plan: it works
+ * on a transform that was never planned as on one holding context or warp plans, and does not touch them.  The output
+ * layout's tables are built on the host and uploaded in stream order when the context or an output size changes.  Takes the
+ * reader lock, so it is frame-exact against T360B200_reconfigure and T360B200_reconfigureAsync, and never synchronises the
+ * device.  Returns 1 if everything was enqueued; 0 with a message on stdout, before any CUDA call, for the refusals above,
+ * 0 or more than 3 planes, or an invalid plane description. */
+int T360B200_transformFrameLensAsync(VideoFrameTransform* transform, const T360LensRig* rig, const T360Orientation* orientation,
+                                     int numPlanes, const uint8_t* const* deviceInputs, uint8_t* const* deviceOutputs,
+                                     const int* inputWidths, const int* inputHeights, const int* inputPitches,
+                                     const int* outputWidths, const int* outputHeights, const int* outputPitches, void* cudaStream);
 /* Opt-in (also: environment T360B200_PIN_HOST_PLANES=1): page-lock pageable caller planes in place the second time
  * the same buffer is seen (cudaHostRegister), so that recycled frame-pool buffers are DMA'd at full PCIe speed.  The
  * caller must keep such buffers alive until VideoFrameTransform_delete. */

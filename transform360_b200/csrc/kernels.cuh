@@ -391,6 +391,20 @@ struct MapGatherParams {
 };
 cudaError_t launchMapGather(MapGatherParams p, int numSMs, cudaStream_t stream);
 
+// ---- the per-frame lens gather (view_gather.cu) ----------------------------------------------------------------------
+// Frames of a fisheye lens rig to a sphere output (every layout but FLAT_FIXED) with the orientation and the rig as launch
+// parameters: every pixel runs spherePoint and the lens model (oriented_view.h: lensSample), with the output layout's
+// tables built on the host.  Same tiles, threads and taps as the per-view gather; BORDER_TRANSPARENT.
+struct LensGatherParams {
+  OrientedPlane plane[kMaxFramePlanes];  // geometry: the lens context's (sphereGeometry of lensContext), inW / inH the plane's
+  int numPlanes;
+  Rotation rotation;
+  LensRigModel rig;
+  const int16_t* weights;  // device copy of the [1024][k][k] table (nullptr for nearest)
+  int kernelSize;
+};
+cudaError_t launchLensGather(LensGatherParams p, int numSMs, cudaStream_t stream);
+
 // bytes of dynamic shared memory a blur tile of (w x h) with the given tap counts needs
 inline int blurTileSmem(int w, int h, int nkx, int nky) {
   const int hx = nkx / 2, hy = nky / 2;

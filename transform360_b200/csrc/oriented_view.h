@@ -290,16 +290,17 @@ T360_HD bool barrelPoint(const SphereGeometry& g, const float* colTab, const flo
   return true;
 }
 
-// The sampling record {col0, rowPhase} of output pixel (i, j), as HostPlan::samples holds it.  colTab / rowTab: the plan's
-// tables (buildSphereTables) at column and row offset.  BARREL = false leaves the barrel layouts out of the code (the
-// orientation kernel's instantiations for the other layouts).
+// The output half of the chain for output pixel (i, j): pixel centre -> output eye split -> point on the cube / sphere ->
+// off-centre warp -> rotation by r.  *eye: the output eye; *t: the rotated direction (not normalised), the vector the input
+// lookup maps.  Returns false for a barrel dead zone (*t is then not set).  colTab / rowTab: the plan's tables
+// (buildSphereTables) at column and row offset.  BARREL = false leaves the barrel layouts out of the code.
 template <bool BARREL = true>
-T360_HD void sphereSample(const SphereGeometry& g, const Rotation& r, const float* colTab, const float* rowTab, int i, int j,
-                          int32_t* col0, int32_t* rowPhase) {
+T360_HD bool spherePoint(const SphereGeometry& g, const Rotation& r, const float* colTab, const float* rowTab, int i, int j, bool* eye,
+                         SphereVec* t) {
   float x = pixelCentre(j, g.mapW), y = pixelCentre(i, g.mapH);
-  bool eye = false;
-  if (g.splitLR) eye = splitEye(x, false);
-  else if (g.splitTB) eye = splitEye(y, g.vflip);
+  *eye = false;
+  if (g.splitLR) *eye = splitEye(x, false);
+  else if (g.splitTB) *eye = splitEye(y, g.vflip);
   y = fSub(1.0f, y);
   const bool barrel = BARREL && barrelLayout(g.outputLayout);
   SphereVec q;
@@ -324,12 +325,28 @@ T360_HD void sphereSample(const SphereGeometry& g, const Rotation& r, const floa
     }
     q = onCubeFace(g, false, clampFace(col + (1 - row) * 3), fx, fy);
   }
-  float u = -1.0f, v = 0.0f;  // the dead zone's position, not re-packed (cpp:1304-1306)
   if (mapped) {
     if (g.offCentre) warpOffCentreHD(g, q);
-    const float tx = fAdd(fSub(fMul(q.x, r.xx), fMul(q.y, r.xy)), fMul(q.z, r.xz));
-    const float ty = -fAdd(fSub(fMul(q.x, r.yx), fMul(q.y, r.yy)), fMul(q.z, r.yz));
-    const float tz = fAdd(fSub(fMul(q.x, r.zx), fMul(q.y, r.zy)), fMul(q.z, r.zz));
+    t->x = fAdd(fSub(fMul(q.x, r.xx), fMul(q.y, r.xy)), fMul(q.z, r.xz));
+    t->y = -fAdd(fSub(fMul(q.x, r.yx), fMul(q.y, r.yy)), fMul(q.z, r.yz));
+    t->z = fAdd(fSub(fMul(q.x, r.zx), fMul(q.y, r.zy)), fMul(q.z, r.zz));
+  }
+  return mapped;
+}
+
+// The sampling record {col0, rowPhase} of output pixel (i, j), as HostPlan::samples holds it: spherePoint, then the input
+// lookup.  BARREL = false leaves the barrel layouts out of the code (the orientation kernel's instantiations for the other
+// layouts).
+template <bool BARREL = true>
+T360_HD void sphereSample(const SphereGeometry& g, const Rotation& r, const float* colTab, const float* rowTab, int i, int j,
+                          int32_t* col0, int32_t* rowPhase) {
+  const bool barrel = BARREL && barrelLayout(g.outputLayout);
+  bool eye;
+  SphereVec t;
+  const bool mapped = spherePoint<BARREL>(g, r, colTab, rowTab, i, j, &eye, &t);
+  float u = -1.0f, v = 0.0f;  // the dead zone's position, not re-packed (cpp:1304-1306)
+  if (mapped) {
+    const float tx = t.x, ty = t.y, tz = t.z;
     const float n = fSqrt(fAdd(fAdd(fMul(tx, tx), fMul(ty, ty)), fMul(tz, tz)));  // cpp:863-891
     if (g.cubeInput) {
       cubeInputHD(g, fDiv(tx, n), fDiv(ty, n), fDiv(tz, n), &u, &v);
@@ -382,6 +399,77 @@ inline SphereGeometry sphereGeometry(const FrameTransformContext& ctx, int mapW,
   g.inPixelWidth = 1.0f / inW;  // cpp:528-531, as buildWarpMap
   if (g.packLR) g.inPixelWidth *= 2;
   return g;
+}
+
+// ---- fisheye lens input ---------------------------------------------------------------------------------------------
+// A rig of one or two fisheye lenses with OpenCV's fisheye (Kannala-Brandt) calibration replaces the input lookup: the
+// rotated direction d = (tx, ty, tz) of spherePoint (the rig frame: x right, y up, z forward, the frame an equirect input
+// shows at u = atan2(x, z) / 2pi + 0.5) goes to the lens whose axis it is closest to (the larger Z; ties to lens 0), then
+//   (X, Y, Z) = M d               (M: the lens's R^T with its y row negated: OpenCV camera coordinates, y down)
+//   rho = sqrt(X^2 + Y^2), theta = atan2(rho, Z)         (theta > thetaMax: not covered, NaN)
+//   theta_d = theta (1 + t (k1 + t (k2 + t (k3 + t k4)))), t = theta^2      (Horner)
+//   (x', y') = theta_d / rho (X, Y), (0, 0) at rho = 0
+//   position = ((fx x' + cx + 0.5) / calibWidth) inW - 0.5 = (ax x' + bx) inW - 0.5, and likewise for y
+// Only + - * /, sqrt and atan2 (libmAtan2f), so host and device give the same bits; the constants are computed on the
+// host in double and stored as float (lensRigModel, video_frame_transform.cpp).
+struct LensModel {
+  float m[9];              // rig direction -> camera coordinates, row major
+  float ax, bx, ay, by;    // fx / calibWidth, (cx + 0.5) / calibWidth, fy / calibHeight, (cy + 0.5) / calibHeight
+  float k[4];              // k1 .. k4
+  float thetaMax;          // maxAngle in radians
+};
+struct LensRigModel {
+  int numLenses;  // 1 or 2
+  LensModel lens[2];
+};
+
+T360_HD float lensRow(const float* m, const SphereVec& d) { return fAdd(fAdd(fMul(m[0], d.x), fMul(m[1], d.y)), fMul(m[2], d.z)); }
+
+// The source position (*px, *py) of rig direction d in an inW x inH plane; NaN for both where no lens covers d.
+T360_HD void lensPosition(const LensRigModel& rig, const SphereVec& d, int inW, int inH, float* px, float* py) {
+  const float z0 = lensRow(rig.lens[0].m + 6, d);
+  const float z1 = rig.numLenses > 1 ? lensRow(rig.lens[1].m + 6, d) : z0;
+  const bool second = z1 > z0;
+  const LensModel& L = second ? rig.lens[1] : rig.lens[0];
+  const float X = lensRow(L.m, d), Y = lensRow(L.m + 3, d), Z = second ? z1 : z0;
+  const float rho = fSqrt(fAdd(fMul(X, X), fMul(Y, Y)));
+  const float theta = libmAtan2f(rho, Z);
+  if (!(theta <= L.thetaMax)) {
+    *px = *py = bitsFloat(0x7fc00000u);
+    return;
+  }
+  const float t = fMul(theta, theta);
+  const float poly = fAdd(1.0f, fMul(t, fAdd(L.k[0], fMul(t, fAdd(L.k[1], fMul(t, fAdd(L.k[2], fMul(t, L.k[3]))))))));
+  const float s = rho > 0.0f ? fDiv(fMul(theta, poly), rho) : 0.0f;
+  *px = toPixel(fAdd(fMul(L.ax, fMul(s, X)), L.bx), inW);
+  *py = toPixel(fAdd(fMul(L.ay, fMul(s, Y)), L.by), inH);
+}
+
+// The map entry of output pixel (i, j) of a lens rig: spherePoint, then lensPosition; NaN in a barrel dead zone.  The
+// geometry's input fields other than inW / inH play no part.
+template <bool BARREL = true>
+T360_HD void lensPoint(const SphereGeometry& g, const Rotation& r, const LensRigModel& rig, const float* colTab, const float* rowTab, int i,
+                       int j, float* px, float* py) {
+  bool eye;
+  SphereVec d;
+  if (!spherePoint<BARREL>(g, r, colTab, rowTab, i, j, &eye, &d)) {
+    *px = *py = bitsFloat(0x7fc00000u);
+    return;
+  }
+  lensPosition(rig, d, g.inW, g.inH, px, py);
+}
+
+// The sampling record of output pixel (i, j) of a lens rig: its map entry, quantised as quantizeWarpMap quantises a
+// caller's map, so T360B200_lensMap -> T360B200_generateMapFromWarp plans the records the lens kernel computes.
+template <bool BARREL = true>
+T360_HD void lensSample(const SphereGeometry& g, const Rotation& r, const LensRigModel& rig, const float* colTab, const float* rowTab, int i,
+                        int j, int32_t* col0, int32_t* rowPhase) {
+  float px, py;
+  lensPoint<BARREL>(g, r, rig, colTab, rowTab, i, j, &px, &py);
+  int r0, fracX, fracY;
+  quantizeAxis(px, g.kernelSize, col0, &fracX);
+  quantizeAxis(py, g.kernelSize, &r0, &fracY);
+  *rowPhase = r0 * 1024 + fracY * 32 + fracX;
 }
 
 // Whether the per-frame orientation chain covers the layouts of `ctx`

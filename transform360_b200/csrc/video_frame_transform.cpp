@@ -327,16 +327,96 @@ struct StreamSlot {
   ViewBlurCache viewBlur;
   // the per-frame orientation kernel's tables while a reconfigureAsync is pending (the plans' tables are for the old context),
   // and the context and plan generation they were built for
+  // (also the lens kernel's tables, which have no plan to come from), and the context and map sizes they were built for
   UploadRing sphereTables;
   std::vector<uint8_t> sphereBytes;
-  size_t sphereAt[2] = {SIZE_MAX, SIZE_MAX};  // per plan index: where its tables start in sphereBytes
+  size_t sphereAt[kPlaneLanes] = {SIZE_MAX, SIZE_MAX, SIZE_MAX};  // per plane: where its tables start in sphereBytes
   FrameTransformContext sphereCtx{};
-  unsigned long long sphereGeneration = ~0ull;
-  int sphereIndices = 0;
+  std::vector<int> sphereSizes;  // mapW, mapH per plane
 };
 
 constexpr int kPitchAlign = 256;
 inline int alignedPitch(int w) { return (w + kPitchAlign - 1) / kPitchAlign * kPitchAlign; }
+
+// ---- fisheye lens rigs (T360B200_lensMap, T360B200_transformFrameLensAsync; oriented_view.h: lensSample) ----------------
+// true, with the reason in *why, when the lens path cannot serve ctx with this rig and orientation
+bool lensRefused(const FrameTransformContext& ctx, const T360LensRig* rig, const T360Orientation* o, std::string* why) {
+  char buf[256];
+  auto refuse = [&](const char* fmt, auto... args) {
+    std::snprintf(buf, sizeof(buf), fmt, args...);
+    *why = buf;
+    return true;
+  };
+  if (!rig || !o) return refuse("%s", "a NULL rig or orientation");
+  if (!std::isfinite(o->yaw) || !std::isfinite(o->pitch) || !std::isfinite(o->roll))
+    return refuse("the orientation (yaw %g, pitch %g, roll %g) is not finite", o->yaw, o->pitch, o->roll);
+  if (rig->numLenses != 1 && rig->numLenses != 2) return refuse("numLenses %d (1 or 2 supported)", rig->numLenses);
+  if (rig->calibWidth <= 0 || rig->calibHeight <= 0) return refuse("calibration size %dx%d is not positive", rig->calibWidth, rig->calibHeight);
+  for (int i = 0; i < rig->numLenses; ++i) {
+    const T360Lens& L = rig->lens[i];
+    for (float v : {L.fx, L.fy, L.cx, L.cy, L.k[0], L.k[1], L.k[2], L.k[3], L.yaw, L.pitch, L.roll, L.maxAngle})
+      if (!std::isfinite(v)) return refuse("lens %d has a field that is not finite", i);
+    if (!(L.fx > 0.0f) || !(L.fy > 0.0f)) return refuse("lens %d: fx %g and fy %g must be positive", i, L.fx, L.fy);
+    if (!(L.maxAngle > 0.0f && L.maxAngle <= 180.0f)) return refuse("lens %d: maxAngle %g is outside (0, 180]", i, L.maxAngle);
+    // theta_d(theta) must be strictly increasing on [0, maxAngle], or the lens would fold the image over: its derivative
+    // 1 + 3 k1 t^2 + 5 k2 t^4 + 7 k3 t^6 + 9 k4 t^8 > 0 on a fine grid
+    constexpr int kSteps = 4096;
+    const double tMax = L.maxAngle * M_PI / 180.0;
+    for (int s = 0; s <= kSteps; ++s) {
+      const double t = tMax * s / kSteps, t2 = t * t;
+      const double d = 1.0 + t2 * (3.0 * L.k[0] + t2 * (5.0 * L.k[1] + t2 * (7.0 * L.k[2] + t2 * 9.0 * L.k[3])));
+      if (!(d > 0.0))
+        return refuse("lens %d: theta_d(theta) of k = (%g, %g, %g, %g) stops increasing at %.3f degrees, inside maxAngle %g (it would mirror "
+                      "the image)", i, L.k[0], L.k[1], L.k[2], L.k[3], t * 180.0 / M_PI, L.maxAngle);
+    }
+  }
+  const int layout = ctx.output_layout;
+  if (layout == LAYOUT_FLAT_FIXED || layout < 0 || layout >= LAYOUT_N)
+    return refuse("output_layout %d (a lens rig needs CUBEMAP_32, CUBEMAP_23_OFFCENTER, EAC_32, EQUIRECT, BARREL or BARREL_SPLIT)", layout);
+  if (ctx.enable_low_pass_filter) return refuse("%s", "the low-pass filter is not available for a lens rig (set enable_low_pass_filter = 0)");
+  if (t360::kernelSizeOf(ctx.interpolation_alg) == 0) return refuse("no interpolation algorithm %d", static_cast<int>(ctx.interpolation_alg));
+  return false;
+}
+
+// The per-frame constants of a rig (oriented_view.h: LensModel), in double and stored as float
+t360::LensRigModel lensRigModel(const T360LensRig& rig) {
+  t360::LensRigModel m{};
+  m.numLenses = rig.numLenses;
+  for (int i = 0; i < rig.numLenses; ++i) {
+    const T360Lens& L = rig.lens[i];
+    const double a = L.yaw * M_PI / 180.0, b = -L.pitch * M_PI / 180.0, g = L.roll * M_PI / 180.0;
+    const double ry[3][3] = {{std::cos(a), 0, std::sin(a)}, {0, 1, 0}, {-std::sin(a), 0, std::cos(a)}};
+    const double rx[3][3] = {{1, 0, 0}, {0, std::cos(b), -std::sin(b)}, {0, std::sin(b), std::cos(b)}};
+    const double rz[3][3] = {{std::cos(g), -std::sin(g), 0}, {std::sin(g), std::cos(g), 0}, {0, 0, 1}};
+    double ryx[3][3], r[3][3];
+    for (int u = 0; u < 3; ++u)
+      for (int v = 0; v < 3; ++v) ryx[u][v] = ry[u][0] * rx[0][v] + ry[u][1] * rx[1][v] + ry[u][2] * rx[2][v];
+    for (int u = 0; u < 3; ++u)
+      for (int v = 0; v < 3; ++v) r[u][v] = ryx[u][0] * rz[0][v] + ryx[u][1] * rz[1][v] + ryx[u][2] * rz[2][v];
+    t360::LensModel& l = m.lens[i];
+    for (int u = 0; u < 3; ++u)  // R^T, the y row negated: OpenCV's camera coordinates
+      for (int v = 0; v < 3; ++v) l.m[3 * u + v] = static_cast<float>(u == 1 ? -r[v][u] : r[v][u]);
+    l.ax = static_cast<float>(static_cast<double>(L.fx) / rig.calibWidth);
+    l.bx = static_cast<float>((static_cast<double>(L.cx) + 0.5) / rig.calibWidth);
+    l.ay = static_cast<float>(static_cast<double>(L.fy) / rig.calibHeight);
+    l.by = static_cast<float>((static_cast<double>(L.cy) + 0.5) / rig.calibHeight);
+    for (int j = 0; j < 4; ++j) l.k[j] = L.k[j];
+    l.thetaMax = static_cast<float>(L.maxAngle * M_PI / 180.0);
+  }
+  return m;
+}
+
+// The context the lens path renders with: the output fields of ctx, a mono equirect-like input (the fields the rig
+// replaces, which play no part in the output half of the chain), no scaling
+FrameTransformContext lensContext(const FrameTransformContext& ctx) {
+  FrameTransformContext c = ctx;
+  c.input_layout = LAYOUT_EQUIRECT;
+  c.input_stereo_format = STEREO_FORMAT_MONO;
+  c.output_stereo_format = STEREO_FORMAT_MONO;
+  c.input_expand_coef = 1.0f;
+  c.width_scale_factor = c.height_scale_factor = 1.0f;
+  return c;
+}
 
 }  // namespace
 
@@ -517,13 +597,16 @@ class VideoFrameTransform {
   }
 
   // T360B200_reconfigureWait: 1 when the plans of the current context are in effect, -1 when the background planner failed
-  // on it, else 0 (block = false) or, with block, the result once the planner has finished -- without the settle interval.
+  // on it, else 0 (block = false) or, with block, the result once the planner has finished -- without the settle interval,
+  // and only after the plans the swap replaced have been released (asyncRetiring_), so device memory is back when it returns.
   int reconfigureWait(bool block) {
     std::unique_lock<std::mutex> async(asyncMu_);
-    if (asyncSettled_ != asyncSeq_ && block) {
-      asyncHurry_ = true;
-      asyncCv_.notify_all();
-      asyncCv_.wait(async, [this] { return asyncSettled_ == asyncSeq_ || asyncStop_; });
+    if (block) {
+      if (asyncSettled_ != asyncSeq_) {
+        asyncHurry_ = true;
+        asyncCv_.notify_all();
+      }
+      asyncCv_.wait(async, [this] { return (asyncSettled_ == asyncSeq_ && !asyncRetiring_) || asyncStop_; });
     }
     if (asyncSettled_ != asyncSeq_) return 0;
     return asyncFailed_ ? -1 : 1;
@@ -1128,6 +1211,73 @@ class VideoFrameTransform {
     return false;
   }
 
+  // Whole frame of a fisheye lens rig (T360B200_transformFrameLensAsync): one gather launch for all planes, every record
+  // computed by lensSample (oriented_view.h), so a rig gives what lensMap -> generateMapFromWarp plans for it.  Needs no
+  // plan and leaves the plans alone; the output layout's tables come through the slot's upload ring.  Every refusal comes
+  // before the first CUDA call, and nothing here synchronises the device.
+  bool transformFrameLens(const T360LensRig* rig, const T360Orientation* o, int numPlanes, const uint8_t* const* dIn, uint8_t* const* dOut,
+                          const int* inW, const int* inH, const int* inPitch, const int* outW, const int* outH, const int* outPitch,
+                          cudaStream_t stream) {
+    const char* what = "Could not transform the frame with a lens rig";
+    try {
+      if (numPlanes < 1 || numPlanes > kPlaneLanes) {
+        std::printf("%s. Error: %d planes (1..%d supported)\n", what, numPlanes, kPlaneLanes);
+        return false;
+      }
+      for (int p = 0; p < numPlanes; ++p) {
+        if (!dIn[p] || !dOut[p] || inW[p] <= 0 || inH[p] <= 0 || outW[p] <= 0 || outH[p] <= 0 || inPitch[p] < inW[p] || outPitch[p] < outW[p]) {
+          std::printf("%s. Error: invalid description of plane %d\n", what, p);
+          return false;
+        }
+      }
+      std::shared_lock<std::shared_mutex> config(configMu_);
+      const FrameTransformContext ctx = ctx_;
+      std::string why;
+      if (lensRefused(ctx, rig, o, &why)) {
+        std::printf("%s. Error: %s\n", what, why.c_str());
+        return false;
+      }
+      const FrameTransformContext lens = lensContext(ctx);
+      const int k = t360::kernelSizeOf(ctx.interpolation_alg);
+      const DeviceRestore restoreDevice = ensureDevice();
+      cudaStream_t s = stream ? stream : stream_;
+      StreamSlot& slot = slotFor(s);
+      const float* tables[kPlaneLanes];
+      UploadRing::Entry* staged = nullptr;
+      sphereTablesFor(lens, numPlanes, outW, outH, slot, s, tables, &staged);
+      t360::LensGatherParams lp{};
+      for (int p = 0; p < numPlanes; ++p) {
+        // BORDER_TRANSPARENT: chroma outputs start at 128 as in the planned path, luma outputs keep the caller's bytes
+        if (p) CU(cudaMemset2DAsync(dOut[p], outPitch[p], 128, outW[p], outH[p], s));
+        t360::OrientedPlane& v = lp.plane[p];
+        v.src = dIn[p];
+        v.srcPitch = inPitch[p];
+        v.dst = dOut[p];
+        v.dstPitch = outPitch[p];
+        v.geometry = t360::sphereGeometry(lens, outW[p], outH[p], inW[p], inH[p], k);
+        v.colTable = tables[p];
+        v.rowTable = tables[p] ? tables[p] + t360::sphereTableRowOffset(v.geometry) : nullptr;
+      }
+      lp.numPlanes = numPlanes;
+      lp.rotation = t360::rotationFromAngles(o->yaw, o->pitch, o->roll);
+      lp.rig = lensRigModel(*rig);
+      lp.kernelSize = k;
+      lp.weights = deviceWeights(ctx.interpolation_alg);
+      CU(t360::launchLensGather(lp, numSMs_, s));
+      if (staged) {  // the entry may be refilled once this launch has finished
+        CU(cudaEventRecord(staged->released, s));
+        staged->inFlight = true;
+      }
+      return true;
+    } catch (const CudaFail& f) {
+      std::printf("%s. Error: CUDA %s (%s) in %s\n", what, cudaGetErrorName(f.err), cudaGetErrorString(f.err), f.what);
+      cudaGetLastError();
+    } catch (const std::exception& ex) {
+      std::printf("%s. Error: %s\n", what, ex.what());
+    }
+    return false;
+  }
+
   static void substitutePose(FrameTransformContext& ctx, const T360Pose& pose) {
     ctx.fixed_yaw = pose.yaw;
     ctx.fixed_pitch = pose.pitch;
@@ -1230,7 +1380,11 @@ class VideoFrameTransform {
         const float* tables[kPlaneLanes];
         UploadRing::Entry* staged = nullptr;  // (pending: the tables come through the slot's ring)
         for (int p = 0; p < numPlanes; ++p) tables[p] = plans[p]->sphereTables.ptr;
-        if (perFrameOnly_) sphereTablesFor(ctx, plans, numPlanes, slot, s, tables, &staged);
+        if (perFrameOnly_) {
+          int mapW[kPlaneLanes], mapH[kPlaneLanes];
+          for (int p = 0; p < numPlanes; ++p) { mapW[p] = plans[p]->mapW; mapH[p] = plans[p]->mapH; }
+          sphereTablesFor(ctx, numPlanes, mapW, mapH, slot, s, tables, &staged);
+        }
         for (int p = 0; p < numPlanes; ++p) {
           const DevicePlan& plan = *plans[p];
           t360::OrientedPlane& v = op.plane[p];
@@ -2099,6 +2253,19 @@ class VideoFrameTransform {
       if (superseded()) return true;
       const DeviceRestore restoreDevice = ensureDevice();
       PlanSet set = makePlanSet(next, sizes, host);
+      // a blocking reconfigureWait that the swap wakes returns only once the old plans are released as well
+      struct Retiring {
+        VideoFrameTransform* t;
+        explicit Retiring(VideoFrameTransform* self) : t(self) {
+          std::lock_guard<std::mutex> async(t->asyncMu_);
+          t->asyncRetiring_ = true;
+        }
+        ~Retiring() {
+          std::lock_guard<std::mutex> async(t->asyncMu_);
+          t->asyncRetiring_ = false;
+          t->asyncCv_.notify_all();
+        }
+      } retiring(this);
       install(set, next, seq, false);
       retire(set);
       return true;
@@ -2111,33 +2278,40 @@ class VideoFrameTransform {
     return false;
   }
 
-  // The per-frame orientation kernel's tables of the planes for a context the plans were not made with (a pending
-  // reconfigureAsync): built on the host when the context or the plans change, staged through the slot's upload ring on `s`.
-  // tables[p] receive the device tables (nullptr for layouts without any); *used the ring entry to release after the launch.
-  void sphereTablesFor(const FrameTransformContext& ctx, const DevicePlan* const* plans, int numPlanes, StreamSlot& slot, cudaStream_t s,
+  // The per-frame kernels' sphere tables of the planes when no plan holds them (a pending reconfigureAsync, whose context
+  // the plans were not made with, and lens frames): planes of mapW[p] x mapH[p], built on the host when the context or a size
+  // changes (planes of the same size share them), staged through the slot's upload ring on `s`.  tables[p] receive the
+  // device tables (nullptr for layouts without any); *used the ring entry to release after the launch.
+  void sphereTablesFor(const FrameTransformContext& ctx, int numPlanes, const int* mapW, const int* mapH, StreamSlot& slot, cudaStream_t s,
                        const float** tables, UploadRing::Entry** used) {
-    const int indices = numPlanes > 1 ? 2 : 1;
     FrameTransformContext key = ctx;  // (the orientation plays no part in the tables)
     key.fixed_yaw = key.fixed_pitch = key.fixed_roll = key.fixed_hfov = key.fixed_vfov = 0;
-    if (slot.sphereGeneration != planGeneration_ || slot.sphereIndices != indices || std::memcmp(&slot.sphereCtx, &key, sizeof(key)) != 0) {
+    std::vector<int> sizes;
+    for (int p = 0; p < numPlanes; ++p) sizes.insert(sizes.end(), {mapW[p], mapH[p]});
+    if (slot.sphereSizes != sizes || std::memcmp(&slot.sphereCtx, &key, sizeof(key)) != 0) {
       slot.sphereBytes.clear();
-      for (int idx = 0; idx < indices; ++idx) {
-        const DevicePlan& plan = *plans[idx];
+      for (int p = 0; p < numPlanes; ++p) {
+        int same = 0;
+        while (same < p && (mapW[same] != mapW[p] || mapH[same] != mapH[p])) ++same;
+        if (same < p) {
+          slot.sphereAt[p] = slot.sphereAt[same];
+          continue;
+        }
+        // (the tables depend on the map, not on the input)
         const std::vector<float> t =
-            t360::buildSphereTables(t360::sphereGeometry(ctx, plan.mapW, plan.mapH, plan.inW, plan.inH, t360::kernelSizeOf(ctx.interpolation_alg)));
-        slot.sphereAt[idx] = t.empty() ? SIZE_MAX : slot.sphereBytes.size();
+            t360::buildSphereTables(t360::sphereGeometry(ctx, mapW[p], mapH[p], 1, 1, t360::kernelSizeOf(ctx.interpolation_alg)));
+        slot.sphereAt[p] = t.empty() ? SIZE_MAX : slot.sphereBytes.size();
         const uint8_t* bytes = reinterpret_cast<const uint8_t*>(t.data());
         slot.sphereBytes.insert(slot.sphereBytes.end(), bytes, bytes + t.size() * sizeof(float));
       }
       slot.sphereCtx = key;
-      slot.sphereGeneration = planGeneration_;
-      slot.sphereIndices = indices;
+      slot.sphereSizes = sizes;
     }
     for (int p = 0; p < numPlanes; ++p) tables[p] = nullptr;
     if (slot.sphereBytes.empty()) return;
     const uint8_t* d = stageUpload(slot.sphereTables, slot.sphereBytes, s, used);
     for (int p = 0; p < numPlanes; ++p) {
-      const size_t at = slot.sphereAt[p ? 1 : 0];
+      const size_t at = slot.sphereAt[p];
       if (at != SIZE_MAX) tables[p] = reinterpret_cast<const float*>(d + at);
     }
   }
@@ -2196,6 +2370,7 @@ class VideoFrameTransform {
   std::thread worker_;
   unsigned long long asyncSeq_ = 0, asyncSettled_ = 0;
   bool asyncFailed_ = false, asyncHurry_ = false, asyncStop_ = false;
+  bool asyncRetiring_ = false;  // the background planner has swapped in a set and is releasing the one it replaced
   FrameTransformContext asyncCtx_{};
   std::chrono::steady_clock::time_point asyncLast_{};
 };
@@ -2524,6 +2699,41 @@ T360_API int T360B200_remapFrameAsync(VideoFrameTransform* t, int numPlanes, con
   }
   return t->remapFrame(numPlanes, maps, mapPitches, border, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch,
                        static_cast<cudaStream_t>(stream));
+}
+T360_API int T360B200_lensMap(const FrameTransformContext* ctx, const T360LensRig* rig, const T360Orientation* orientation, int inW, int inH,
+                              int outW, int outH, float* map) {
+  const char* what = "Could not compute the lens map";
+  std::string why;
+  if (!ctx) why = "a NULL context";
+  else if (lensRefused(*ctx, rig, orientation, &why)) {}
+  else if (!map || inW <= 0 || inH <= 0 || outW <= 0 || outH <= 0) why = "a NULL map or a plane size that is not positive";
+  if (!why.empty()) {
+    std::printf("%s. Error: %s\n", what, why.c_str());
+    return 0;
+  }
+  const FrameTransformContext lens = lensContext(*ctx);
+  const t360::SphereGeometry g = t360::sphereGeometry(lens, outW, outH, inW, inH, t360::kernelSizeOf(ctx->interpolation_alg));
+  const std::vector<float> tables = t360::buildSphereTables(g);
+  const float* colTab = tables.data();
+  const float* rowTab = tables.empty() ? nullptr : tables.data() + t360::sphereTableRowOffset(g);
+  const t360::Rotation r = t360::rotationFromAngles(orientation->yaw, orientation->pitch, orientation->roll);
+  const t360::LensRigModel model = lensRigModel(*rig);
+  for (int i = 0; i < outH; ++i)
+    for (int j = 0; j < outW; ++j) {
+      float* out = map + 2 * (static_cast<size_t>(i) * outW + j);
+      t360::lensPoint(g, r, model, colTab, rowTab, i, j, out, out + 1);
+    }
+  return 1;
+}
+T360_API int T360B200_transformFrameLensAsync(VideoFrameTransform* t, const T360LensRig* rig, const T360Orientation* orientation, int numPlanes,
+                                              const uint8_t* const* dIn, uint8_t* const* dOut, const int* inW, const int* inH, const int* inPitch,
+                                              const int* outW, const int* outH, const int* outPitch, void* stream) {
+  if (!t || !dIn || !dOut || !inW || !inH || !inPitch || !outW || !outH || !outPitch) {
+    std::printf("Could not transform the frame with a lens rig. Error: a NULL argument\n");
+    return 0;
+  }
+  return t->transformFrameLens(rig, orientation, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch,
+                               static_cast<cudaStream_t>(stream));
 }
 T360_API void T360B200_setPinHostPlanes(VideoFrameTransform* t, int enable) { if (t) t->setPinHostPlanes(enable != 0); }
 T360_API void T360B200_debugTrace(VideoFrameTransform* t, int enable) { if (t) t->enableTrace(enable != 0); }

@@ -13,7 +13,9 @@
 //   - sphere outputs (SpherePositions): the rotation mixes both axes, so every pixel runs the whole chain
 //     (oriented_view.h: sphereSample), with the plan's per-column / per-row tables for the view-independent libm steps.
 //   - a caller's warp map (MapPositions): the pixel's map entry, quantised by quantizeAxis.
-// In all three, the records come from the same host/device functions the planner (or its host twin) uses: bit-identical.
+//   - a fisheye lens rig (LensPositions): the output half of the sphere chain, then the lens model (oriented_view.h:
+//     lensSample), quantised like a map entry.
+// In all four, the records come from the same host/device functions the planner (or its host twin) uses: bit-identical.
 #include "gather_common.cuh"
 
 #include <algorithm>
@@ -129,6 +131,16 @@ struct MapPositions {
   }
 };
 
+// A fisheye lens rig: the whole chain per pixel, no shared tables
+template <bool BARREL>
+struct LensPositions {
+  __device__ void beginTile(const LensGatherParams&, const OrientedPlane&, int, int) {}
+  __device__ void beginColumn(int) {}
+  __device__ void record(const LensGatherParams& p, const OrientedPlane& v, int, int, int i, int j, int* col0, int* rowPhase) const {
+    lensSample<BARREL>(v.geometry, p.rotation, p.rig, v.colTable, v.rowTable, i, j, col0, rowPhase);
+  }
+};
+
 template <int K>
 __global__ void __launch_bounds__(gatherThreads(K), K == 8 ? 1 : 4) viewGatherKernel(const __grid_constant__ ViewGatherParams p, int numTiles) {
   extern __shared__ __align__(16) unsigned char smem[];
@@ -160,6 +172,18 @@ __global__ void __launch_bounds__(gatherThreads(K), K == 8 ? 1 : 4) mapGatherKer
     __syncthreads();  // (no tile synchronises after this)
   }
   gatherViewTiles<K, TRANSPARENT>(p, numTiles, smem, pos);
+}
+
+// BARREL: the barrel layouts' positions (dead zones included); always BORDER_TRANSPARENT
+template <int K, bool BARREL>
+__global__ void __launch_bounds__(gatherThreads(K), K == 8 ? 1 : 4) lensGatherKernel(const __grid_constant__ LensGatherParams p, int numTiles) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  LensPositions<BARREL> pos;
+  if constexpr (K >= 2) {
+    stageWeights<K>(p.weights, smem);
+    __syncthreads();  // (no tile synchronises after this)
+  }
+  gatherViewTiles<K, true>(p, numTiles, smem, pos);
 }
 
 template <int K>
@@ -198,6 +222,11 @@ cudaError_t launchOrientedK(const OrientedGatherParams& p, int numTiles, int num
 template <int K, bool TRANSPARENT>
 cudaError_t launchMapK(const MapGatherParams& p, int numTiles, int numSMs, cudaStream_t stream) {
   return launchPositionsK<K, mapGatherKernel<K, TRANSPARENT>>(p, numTiles, numSMs, stream);
+}
+
+template <int K, bool BARREL>
+cudaError_t launchLensK(const LensGatherParams& p, int numTiles, int numSMs, cudaStream_t stream) {
+  return launchPositionsK<K, lensGatherKernel<K, BARREL>>(p, numTiles, numSMs, stream);
 }
 
 // tiles of every plane, in plane order
@@ -253,6 +282,20 @@ cudaError_t launchMapGather(MapGatherParams p, int numSMs, cudaStream_t stream) 
     case 2: return t ? launchMapK<2, true>(p, numTiles, numSMs, stream) : launchMapK<2, false>(p, numTiles, numSMs, stream);
     case 4: return t ? launchMapK<4, true>(p, numTiles, numSMs, stream) : launchMapK<4, false>(p, numTiles, numSMs, stream);
     case 8: return t ? launchMapK<8, true>(p, numTiles, numSMs, stream) : launchMapK<8, false>(p, numTiles, numSMs, stream);
+    default: return cudaErrorInvalidValue;
+  }
+}
+
+cudaError_t launchLensGather(LensGatherParams p, int numSMs, cudaStream_t stream) {
+  if (p.numPlanes < 1 || p.numPlanes > kMaxFramePlanes) return cudaErrorInvalidValue;
+  const int numTiles = assignTiles(p);
+  if (numTiles <= 0) return cudaSuccess;
+  const bool barrel = barrelLayout(p.plane[0].geometry.outputLayout);  // (every plane of a frame has the same layout)
+  switch (p.kernelSize) {
+    case 1: return barrel ? launchLensK<1, true>(p, numTiles, numSMs, stream) : launchLensK<1, false>(p, numTiles, numSMs, stream);
+    case 2: return barrel ? launchLensK<2, true>(p, numTiles, numSMs, stream) : launchLensK<2, false>(p, numTiles, numSMs, stream);
+    case 4: return barrel ? launchLensK<4, true>(p, numTiles, numSMs, stream) : launchLensK<4, false>(p, numTiles, numSMs, stream);
+    case 8: return barrel ? launchLensK<8, true>(p, numTiles, numSMs, stream) : launchLensK<8, false>(p, numTiles, numSMs, stream);
     default: return cudaErrorInvalidValue;
   }
 }

@@ -94,6 +94,18 @@ def as_pose(pose) -> T360Pose:
     return pose if isinstance(pose, T360Pose) else T360Pose(*[float(v) for v in pose])
 
 
+class T360Lens(C.Structure):
+    """One fisheye lens (include/transform360_b200.h): OpenCV fisheye intrinsics fx, fy, cx, cy in pixels of the rig's
+    calibration frame, distortion k1..k4, extrinsics yaw / pitch / roll in degrees, and the half field of view it covers."""
+    _fields_ = [("fx", C.c_float), ("fy", C.c_float), ("cx", C.c_float), ("cy", C.c_float), ("k", C.c_float * 4),
+                ("yaw", C.c_float), ("pitch", C.c_float), ("roll", C.c_float), ("maxAngle", C.c_float)]
+
+
+class T360LensRig(C.Structure):
+    """One or two fisheye lenses calibrated on a calibWidth x calibHeight frame (include/transform360_b200.h)."""
+    _fields_ = [("numLenses", C.c_int), ("calibWidth", C.c_int), ("calibHeight", C.c_int), ("lens", T360Lens * 2)]
+
+
 def make_context(**overrides) -> FrameTransformContext:
     vals = dict(FILTER_DEFAULTS)
     for k in overrides:
@@ -177,6 +189,10 @@ def load(path: os.PathLike | None = None):
     L.T360B200_transformFramePoseAsync.argtypes = [vp, C.POINTER(T360Pose), ci, vp, vp] + [vp] * 6 + [vp]
     L.T360B200_poseSamples.restype = ci
     L.T360B200_poseSamples.argtypes = [C.POINTER(FrameTransformContext), C.POINTER(T360Pose)] + [ci] * 4 + [vp]
+    L.T360B200_lensMap.restype = ci
+    L.T360B200_lensMap.argtypes = [C.POINTER(FrameTransformContext), C.POINTER(T360LensRig), C.POINTER(T360Orientation)] + [ci] * 4 + [vp]
+    L.T360B200_transformFrameLensAsync.restype = ci
+    L.T360B200_transformFrameLensAsync.argtypes = [vp, C.POINTER(T360LensRig), C.POINTER(T360Orientation), ci, vp, vp] + [vp] * 6 + [vp]
     L.T360B200_setPinHostPlanes.restype = None
     L.T360B200_setPinHostPlanes.argtypes = [vp, ci]
     L.T360B200_debugTrace.restype = None
@@ -209,6 +225,7 @@ EXPORTED_SYMBOLS = [
     "T360B200_lowPassPlaneAsync", "T360B200_reconfigure", "T360B200_reconfigureAsync", "T360B200_reconfigureWait",
     "T360B200_transformFrameViewAsync", "T360B200_viewSamples",
     "T360B200_transformFrameOrientedAsync", "T360B200_orientedSamples", "T360B200_transformFramePoseAsync", "T360B200_poseSamples",
+    "T360B200_lensMap", "T360B200_transformFrameLensAsync",
     "T360B200_setPinHostPlanes", "T360B200_debugTrace", "T360B200_debugTraceRead", "T360B200_synchronize", "T360B200_stream", "T360B200_kernelLaunchCount", "T360B200_planDeviceBytes",
     "T360B200_planTileCounts", "T360B200_deviceCount", "T360B200_version",
 ]
@@ -337,6 +354,24 @@ class VideoFrameTransform:
 
         def call(pose, stream: int = 0, _keep=(d_in, d_out, arrs)) -> bool:
             return bool(fn(h, C.byref(as_pose(pose)), n, pin, pout, *ptrs, stream))
+        return call
+
+    def make_lens_frame_call(self, in_planes, out_planes, dims):
+        """Like make_frame_call, for T360B200_transformFrameLensAsync (a fisheye lens rig to any sphere output, no plan
+        needed): returns a callable f(rig, orientation, stream) -> bool that enqueues the whole frame with `rig` (a
+        T360LensRig) and `orientation` (a T360Orientation or (yaw, pitch, roll))."""
+        n = len(in_planes)
+        VP, IA = C.c_void_p * n, C.c_int * n
+        d_in = VP(*[p[0] for p in in_planes])
+        d_out = VP(*[p[0] for p in out_planes])
+        arrs = [IA(*[d[0] for d in dims]), IA(*[d[1] for d in dims]), IA(*[p[1] for p in in_planes]),
+                IA(*[d[2] for d in dims]), IA(*[d[3] for d in dims]), IA(*[p[1] for p in out_planes])]
+        fn, h = self._lib.T360B200_transformFrameLensAsync, self._h
+        ptrs = [C.cast(a, C.c_void_p) for a in arrs]
+        pin, pout = C.cast(d_in, C.c_void_p), C.cast(d_out, C.c_void_p)
+
+        def call(rig, orientation, stream: int = 0, _keep=(d_in, d_out, arrs)) -> bool:
+            return bool(fn(h, C.byref(rig), C.byref(as_orientation(orientation)), n, pin, pout, *ptrs, stream))
         return call
 
     def generate_map_from_warp(self, map, in_w: int, in_h: int, plan_index: int, border: int = BORDER_WRAP) -> bool:
@@ -568,6 +603,17 @@ def pose_samples(ctx: FrameTransformContext, pose, in_w, in_h, out_w, out_h) -> 
     out = np.zeros((max(map_h, 0), max(map_w, 0), 2), np.int32)
     if not load().T360B200_poseSamples(C.byref(ctx), C.byref(as_pose(pose)), in_w, in_h, out_w, out_h, out.ctypes.data):
         raise ValueError("T360B200_poseSamples refused the arguments (message on stdout)")
+    return out
+
+
+def lens_map(ctx: FrameTransformContext, rig: T360LensRig, orientation, in_w, in_h, out_w, out_h) -> np.ndarray:
+    """The CV_32FC2 map of one plane of a fisheye lens rig (T360B200_lensMap, no CUDA): float32 [out_h][out_w][2], the
+    source x, y of every output pixel in a plane of in_w x in_h, NaN where no lens covers it.  generate_map_from_warp(map,
+    in_w, in_h, index, BORDER_TRANSPARENT) plans it for a fixed pose."""
+    out = np.zeros((max(out_h, 0), max(out_w, 0), 2), np.float32)
+    if not load().T360B200_lensMap(C.byref(ctx), C.byref(rig), C.byref(as_orientation(orientation)), in_w, in_h, out_w, out_h,
+                                   out.ctypes.data):
+        raise ValueError("T360B200_lensMap refused the arguments (message on stdout)")
     return out
 
 
