@@ -18,7 +18,8 @@ import numpy as np
 import pytest
 
 import transform360_b200 as t360
-from tests.test_view import (_assert_planes, _host, _inputs, _outputs, _planes, torch_cuda)  # noqa: F401 (fixture)
+from tests.test_view import (_assert_planes, _bad_planes_are_refused, _host, _inputs, _outputs, _planes, _refused_for,  # noqa: F401 (fixture)
+                             torch_cuda)
 from oracle import c_oracle as co
 from oracle import ref_harness as rh
 from transform360_b200.stream import FrameTransformer, StreamSpec
@@ -123,21 +124,22 @@ def test_oriented_samples_refuse_other_layouts_and_non_finite_orientations():
             t360.oriented_samples(t360.make_context(), bad, 64, 32, 16, 16)
 
 
-def test_oriented_frames_are_refused_before_any_device_work():
-    """FLAT_FIXED, BARREL and BARREL_SPLIT transforms, non-finite orientations and plan indices that were never generated
-    are refused (return 0) before the call touches CUDA, so this needs no device."""
-    dummy = [(1 << 20, 256)] * 3
+def test_oriented_frames_are_refused_before_any_device_work(capfd):
+    """FLAT_FIXED, BARREL and BARREL_SPLIT transforms, non-finite orientations, plan indices that were never generated and
+    invalid planes are refused (return 0) before the call touches CUDA, so this needs no device."""
+    dummy = [(1 << 20, 512)] * 3
     dims = [(512, 256, 192, 128), (256, 128, 96, 64), (256, 128, 96, 64)]
     for layout in (t360.LAYOUT_FLAT_FIXED, t360.LAYOUT_BARREL, t360.LAYOUT_BARREL_SPLIT):
         vft = t360.VideoFrameTransform(t360.make_context(output_layout=layout, enable_low_pass_filter=0))
-        assert not vft.make_oriented_frame_call(dummy, dummy, dims)((10.0, 0.0, 0.0)), layout
+        _refused_for(capfd, "per-frame orientations need", vft.make_oriented_frame_call(dummy, dummy, dims), (10.0, 0.0, 0.0))
         vft.close()
     cube = t360.VideoFrameTransform(t360.make_context())
     call = cube.make_oriented_frame_call(dummy, dummy, dims)
-    assert not call((math.nan, 0.0, 0.0))
-    assert not call((0.0, math.inf, 0.0))
-    assert not call((0.0, 0.0, -math.inf))
-    assert not call((10.0, 0.0, 5.0))  # no map generated for index 0
+    _refused_for(capfd, "is not finite", call, (math.nan, 0.0, 0.0))
+    _refused_for(capfd, "is not finite", call, (0.0, math.inf, 0.0))
+    _refused_for(capfd, "is not finite", call, (0.0, 0.0, -math.inf))
+    _refused_for(capfd, "no map was generated for index 0", call, (10.0, 0.0, 5.0))
+    _bad_planes_are_refused(capfd, cube.make_oriented_frame_call, ((10.0, 0.0, 5.0),), dummy, dims)
     cube.close()
 
 

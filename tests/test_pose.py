@@ -24,7 +24,7 @@ from oracle import ff_harness as ff
 from oracle import ref_harness as rh
 from tests.test_oriented import _angle, _jitter, _sweep
 from tests.test_reconfigure import ROOT, _command, _params, command_filter, commands_library  # noqa: F401 (fixtures)
-from tests.test_view import _assert_planes, _host, _inputs, _pitch, _planes, torch_cuda  # noqa: F401 (fixture)
+from tests.test_view import _assert_planes, _bad_planes_are_refused, _host, _inputs, _pitch, _planes, _refused_for, torch_cuda  # noqa: F401 (fixture)
 from transform360_b200.stream import FrameTransformer, StreamSpec
 
 BARREL, SPLIT = t360.LAYOUT_BARREL, t360.LAYOUT_BARREL_SPLIT
@@ -139,11 +139,11 @@ def test_pose_samples_refuse_non_finite_poses_and_unknown_layouts():
         t360.pose_samples(t360.make_context(output_layout=BARREL, interpolation_alg=3), (0, 0, 0, 120, 110), 64, 32, 16, 16)
 
 
-def test_pose_frames_are_refused_before_any_device_work():
-    """Non-finite poses (each of the five fields), plane counts outside 1..3 and plan indices that were never generated are
-    refused (return 0) before the call touches CUDA, so this needs no device.  (A transform without interpolation
-    algorithm needs a generated plan: tested on the GPU.)"""
-    dummy = [(1 << 20, 256)] * 3
+def test_pose_frames_are_refused_before_any_device_work(capfd):
+    """Non-finite poses (each of the five fields), plane counts outside 1..3, plan indices that were never generated and
+    invalid planes are refused (return 0) before the call touches CUDA, so this needs no device.  (A transform without
+    interpolation algorithm needs a generated plan: tested on the GPU.)"""
+    dummy = [(1 << 20, 512)] * 3
     dims = [(512, 256, 160, 64), (256, 128, 80, 32), (256, 128, 80, 32)]
     for layout in ALL_OUTPUTS:
         vft = t360.VideoFrameTransform(t360.make_context(output_layout=layout, enable_low_pass_filter=0))
@@ -152,10 +152,11 @@ def test_pose_frames_are_refused_before_any_device_work():
             for bad in (math.nan, math.inf, -math.inf):
                 pose = [10.0, 0.0, 5.0, 120.0, 110.0]
                 pose[f] = bad
-                assert not call(pose), (layout, pose)
-        assert not call((10.0, 0.0, 5.0, 120.0, 110.0)), layout  # no map generated for index 0
-        assert not vft.make_pose_frame_call([], [], [])((10.0, 0.0, 5.0, 120.0, 110.0))
-        assert not vft.make_pose_frame_call(dummy * 2, dummy * 2, dims * 2)((10.0, 0.0, 5.0, 120.0, 110.0))
+                _refused_for(capfd, "is not finite", call, pose)
+        _refused_for(capfd, "no map was generated for index 0", call, (10.0, 0.0, 5.0, 120.0, 110.0))
+        _refused_for(capfd, "0 planes", vft.make_pose_frame_call([], [], []), (10.0, 0.0, 5.0, 120.0, 110.0))
+        _refused_for(capfd, "6 planes", vft.make_pose_frame_call(dummy * 2, dummy * 2, dims * 2), (10.0, 0.0, 5.0, 120.0, 110.0))
+        _bad_planes_are_refused(capfd, vft.make_pose_frame_call, ((10.0, 0.0, 5.0, 120.0, 110.0),), dummy, dims)
         vft.close()
 
 

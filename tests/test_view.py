@@ -21,6 +21,7 @@ from oracle import c_oracle as co
 from oracle import ff_harness as ff
 from oracle import ref_harness as rh
 from tests.test_reconfigure import ROOT, _command, _params, command_filter, commands_library  # noqa: F401 (fixtures)
+from tests.test_warp_map import _stdout
 from transform360_b200.stream import FrameTransformer, StreamSpec
 
 FLAT = dict(output_layout=t360.LAYOUT_FLAT_FIXED)
@@ -84,19 +85,41 @@ def test_view_samples_refuse_other_layouts_and_non_finite_views():
             t360.view_samples(t360.make_context(**FLAT), bad, 64, 32, 16, 16)
 
 
-def test_view_frames_are_refused_before_any_device_work():
-    """A non-FLAT_FIXED transform, a NaN view and plan indices that were never generated are refused (return 0) before the
-    call touches CUDA, so this needs no device."""
-    dummy = [(1 << 20, 256)] * 3
+def _refused_for(capfd, reason, call, *args):
+    """call(*args) is refused (returns 0) with a message that names `reason`."""
+    assert not call(*args)
+    out = _stdout(capfd)
+    assert reason in out, (reason, out)
+
+
+def _bad_planes_are_refused(capfd, make_call, args, planes, dims):
+    """make_call(in_planes, out_planes, dims)(*args) refuses a NULL plane, a plane without pixels and a pitch short of the
+    width, naming the plane, before any CUDA call: the fake addresses of `planes` are never dereferenced."""
+    def with_plane(rows, p, value):
+        return [value if i == p else r for i, r in enumerate(rows)]
+    in_w, _, out_w, _ = dims[0]
+    cases = [(with_plane(planes, 0, (None, planes[0][1])), planes, dims, 0), (planes, with_plane(planes, 2, (None, planes[2][1])), dims, 2),
+             (planes, planes, with_plane(dims, 0, (0,) + dims[0][1:]), 0), (planes, planes, with_plane(dims, 1, dims[1][:3] + (-1,)), 1),
+             (with_plane(planes, 0, (planes[0][0], in_w - 1)), planes, dims, 0), (planes, with_plane(planes, 0, (planes[0][0], out_w - 1)), dims, 0)]
+    for ins, outs, d, p in cases:
+        _refused_for(capfd, f"invalid description of plane {p}", make_call(ins, outs, d), *args)
+
+
+def test_view_frames_are_refused_before_any_device_work(capfd):
+    """A non-FLAT_FIXED transform, a NaN view, plan indices that were never generated and invalid planes are refused (return
+    0) before the call touches CUDA, so this needs no device."""
+    dummy = [(1 << 20, 512)] * 3
     dims = [(512, 256, 160, 120), (256, 128, 80, 60), (256, 128, 80, 60)]
     cube = t360.VideoFrameTransform(t360.make_context(enable_low_pass_filter=0))
-    assert not cube.make_view_frame_call(dummy, dummy, dims)((10.0, 0.0, 120.0, 110.0))
+    _refused_for(capfd, "per-frame views need output_layout FLAT_FIXED", cube.make_view_frame_call(dummy, dummy, dims), (10.0, 0.0, 120.0, 110.0))
     cube.close()
     flat = t360.VideoFrameTransform(t360.make_context(**FLAT))
     call = flat.make_view_frame_call(dummy, dummy, dims)
-    assert not call((math.nan, 0.0, 120.0, 110.0))
-    assert not call((0.0, 0.0, math.inf, 110.0))
-    assert not call((10.0, 0.0, 120.0, 110.0))  # no map generated for index 0
+    _refused_for(capfd, "is not finite", call, (math.nan, 0.0, 120.0, 110.0))
+    _refused_for(capfd, "is not finite", call, (0.0, 0.0, math.inf, 110.0))
+    _refused_for(capfd, "no map was generated for index 0", call, (10.0, 0.0, 120.0, 110.0))
+    _bad_planes_are_refused(capfd, flat.make_view_frame_call, ((10.0, 0.0, 120.0, 110.0),), dummy, dims)
+    _bad_planes_are_refused(capfd, flat.make_frame_call, (), dummy, dims)
     flat.close()
 
 

@@ -30,10 +30,6 @@
 
 namespace t360 {
 
-struct Orientation {
-  float yaw, pitch, roll;  // degrees, as FrameTransformContext::fixed_*
-};
-
 // q' = (q.x * xx - q.y * xy + q.z * xz, ...): the planner's rotation (reference cpp:1233-1244)
 struct Rotation {
   float xx, xy, xz, yx, yy, yz, zx, zy, zz;
@@ -399,6 +395,14 @@ inline SphereGeometry sphereGeometry(const FrameTransformContext& ctx, int mapW,
   g.inPixelWidth = 1.0f / inW;  // cpp:528-531, as buildWarpMap
   if (g.packLR) g.inPixelWidth *= 2;
   return g;
+}
+
+// The FLAT_FIXED geometry of a plan for `ctx` (flat_view.h), as sphereGeometry
+inline FlatGeometry flatGeometry(const FrameTransformContext& ctx, int mapW, int mapH, int inW, int inH, int kernelSize) {
+  const bool stereoIn = ctx.input_stereo_format != STEREO_FORMAT_MONO;
+  return FlatGeometry{mapW, mapH, inW, inH, kernelSize, stereoIn && ctx.output_stereo_format == STEREO_FORMAT_LR,
+                      stereoIn && ctx.output_stereo_format == STEREO_FORMAT_TB, ctx.vflip != 0, ctx.input_stereo_format == STEREO_FORMAT_LR,
+                      ctx.input_stereo_format == STEREO_FORMAT_TB};
 }
 
 // ---- fisheye lens input ---------------------------------------------------------------------------------------------

@@ -13,6 +13,7 @@
 #include <climits>
 #include <cmath>
 #include <condition_variable>
+#include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -23,6 +24,7 @@
 #include <shared_mutex>
 #include <stdexcept>
 #include <string>
+#include <string_view>
 #include <thread>
 #include <vector>
 
@@ -51,6 +53,22 @@ struct CudaFail {
     cudaError_t e__ = (call);                          \
     if (e__ != cudaSuccess) throw CudaFail{e__, #call}; \
   } while (0)
+
+// body()'s result, or false with a message prefixed by `what` when it throws.  A CUDA error is cleared, so that the
+// caller's next runtime call does not report it again.
+template <class Body>
+bool guarded(std::string_view what, Body&& body) {
+  const int n = static_cast<int>(what.size());
+  try {
+    return body();
+  } catch (const CudaFail& f) {
+    std::printf("%.*s. Error: CUDA %s (%s) in %s\n", n, what.data(), cudaGetErrorName(f.err), cudaGetErrorString(f.err), f.what);
+    cudaGetLastError();
+  } catch (const std::exception& ex) {
+    std::printf("%.*s. Error: %s\n", n, what.data(), ex.what());
+  }
+  return false;
+}
 
 template <typename T>
 struct DeviceBuffer {
@@ -184,15 +202,7 @@ using EncodeTiledFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t
 // cuTensorMapEncodeTiled through the runtime's driver entry point table: the library must still dlopen()
 // on a machine without libcuda.so (CPU-only planning, tests), so libcuda is never linked.
 EncodeTiledFn tensorMapEncoder() {
-  static EncodeTiledFn fn = [] {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q{};
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess) {
-      cudaGetLastError();
-      p = nullptr;
-    }
-    return reinterpret_cast<EncodeTiledFn>(p);
-  }();
+  static const EncodeTiledFn fn = reinterpret_cast<EncodeTiledFn>(driverEntry("cuTensorMapEncodeTiled"));
   return fn;
 }
 
@@ -323,7 +333,7 @@ struct StreamSlot {
   PlaneLane lanes[kPlaneLanes];
   DeviceBuffer<int> frameClaim;
   cudaEvent_t fork = nullptr;
-  UploadRing viewJobs, viewTaps;  // the per-view low-pass lists (VideoFrameTransform::transformFrameView)
+  UploadRing viewJobs, viewTaps;  // the per-frame calls' low-pass lists (VideoFrameTransform::viewLowPass)
   ViewBlurCache viewBlur;
   // the per-frame orientation kernel's tables while a reconfigureAsync is pending (the plans' tables are for the old context),
   // and the context and plan generation they were built for
@@ -337,6 +347,113 @@ struct StreamSlot {
 
 constexpr int kPitchAlign = 256;
 inline int alignedPitch(int w) { return (w + kPitchAlign - 1) / kPitchAlign * kPitchAlign; }
+
+// The device planes of a whole-frame call: plane p is read from in[p] (inW x inH, inPitch bytes per row) and written to
+// out[p].
+struct FramePlanes {
+  int numPlanes = 0;
+  const uint8_t* in[kPlaneLanes];
+  uint8_t* out[kPlaneLanes];
+  int inW[kPlaneLanes], inH[kPlaneLanes], inPitch[kPlaneLanes], outW[kPlaneLanes], outH[kPlaneLanes], outPitch[kPlaneLanes];
+};
+
+// The frame of a whole-frame call's arrays, checked on the host: false, with a message prefixed by `what`, for a NULL
+// array, a plane count outside 1..kPlaneLanes, or a plane that is NULL, has no pixels or a pitch short of its width.
+bool describeFrame(const char* what, int numPlanes, const uint8_t* const* dIn, uint8_t* const* dOut, const int* inW, const int* inH,
+                   const int* inPitch, const int* outW, const int* outH, const int* outPitch, FramePlanes& f) {
+  if (!dIn || !dOut || !inW || !inH || !inPitch || !outW || !outH || !outPitch) {
+    std::printf("%s. Error: a NULL argument\n", what);
+    return false;
+  }
+  if (numPlanes < 1 || numPlanes > kPlaneLanes) {
+    std::printf("%s. Error: %d planes (1..%d supported)\n", what, numPlanes, kPlaneLanes);
+    return false;
+  }
+  f.numPlanes = numPlanes;
+  for (int p = 0; p < numPlanes; ++p) {
+    if (!dIn[p] || !dOut[p] || inW[p] <= 0 || inH[p] <= 0 || outW[p] <= 0 || outH[p] <= 0 || inPitch[p] < inW[p] || outPitch[p] < outW[p]) {
+      std::printf("%s. Error: invalid description of plane %d\n", what, p);
+      return false;
+    }
+    f.in[p] = dIn[p]; f.out[p] = dOut[p];
+    f.inW[p] = inW[p]; f.inH[p] = inH[p]; f.inPitch[p] = inPitch[p];
+    f.outW[p] = outW[p]; f.outH[p] = outH[p]; f.outPitch[p] = outPitch[p];
+  }
+  return true;
+}
+
+// ---- per-frame views, orientations and poses: their checks against a context and the context they render with ---------
+// The context with the five view fields replaced
+void setPose(FrameTransformContext& ctx, const T360Pose& pose) {
+  ctx.fixed_yaw = pose.yaw;
+  ctx.fixed_pitch = pose.pitch;
+  ctx.fixed_roll = pose.roll;
+  ctx.fixed_hfov = pose.hfov;
+  ctx.fixed_vfov = pose.vfov;
+}
+
+std::string formatted(const char* fmt, ...) __attribute__((format(printf, 1, 2)));
+std::string formatted(const char* fmt, ...) {
+  char buf[320];
+  va_list args;
+  va_start(args, fmt);
+  std::vsnprintf(buf, sizeof(buf), fmt, args);
+  va_end(args);
+  return buf;
+}
+
+// Each puts its fields into ctx and returns "", or returns why ctx cannot take them.  A view is a pose with the context's
+// roll (which the FLAT_FIXED chain does not use), an orientation one with the context's fields of view.
+std::string withFields(FrameTransformContext& ctx, const T360Pose& pose) {
+  if (!std::isfinite(pose.yaw) || !std::isfinite(pose.pitch) || !std::isfinite(pose.roll) || !std::isfinite(pose.hfov) ||
+      !std::isfinite(pose.vfov))
+    return formatted("the pose (yaw %g, pitch %g, roll %g, hfov %g, vfov %g) is not finite", pose.yaw, pose.pitch, pose.roll, pose.hfov,
+                     pose.vfov);
+  if (ctx.output_layout < 0 || ctx.output_layout >= LAYOUT_N) return formatted("output_layout %d is not a layout", static_cast<int>(ctx.output_layout));
+  setPose(ctx, pose);
+  return {};
+}
+std::string withFields(FrameTransformContext& ctx, const T360View& view) {
+  if (!std::isfinite(view.yaw) || !std::isfinite(view.pitch) || !std::isfinite(view.hfov) || !std::isfinite(view.vfov))
+    return formatted("the view (yaw %g, pitch %g, hfov %g, vfov %g) is not finite", view.yaw, view.pitch, view.hfov, view.vfov);
+  if (ctx.output_layout != LAYOUT_FLAT_FIXED)
+    return formatted("per-frame views need output_layout FLAT_FIXED (%d), the transform has %d", static_cast<int>(LAYOUT_FLAT_FIXED),
+                     static_cast<int>(ctx.output_layout));
+  setPose(ctx, T360Pose{view.yaw, view.pitch, ctx.fixed_roll, view.hfov, view.vfov});
+  return {};
+}
+std::string withFields(FrameTransformContext& ctx, const T360Orientation& o) {
+  if (!std::isfinite(o.yaw) || !std::isfinite(o.pitch) || !std::isfinite(o.roll))
+    return formatted("the orientation (yaw %g, pitch %g, roll %g) is not finite", o.yaw, o.pitch, o.roll);
+  if (!t360::orientedLayouts(ctx))
+    return formatted("per-frame orientations need output_layout CUBEMAP_32, CUBEMAP_23_OFFCENTER, EAC_32 or EQUIRECT and input_layout "
+                     "EQUIRECT or CUBEMAP_32, the transform has %d -> %d%s", static_cast<int>(ctx.input_layout),
+                     static_cast<int>(ctx.output_layout),
+                     ctx.output_layout == LAYOUT_FLAT_FIXED ? " (FLAT_FIXED views: T360B200_transformFrameViewAsync)" : "");
+  setPose(ctx, T360Pose{o.yaw, o.pitch, o.roll, ctx.fixed_hfov, ctx.fixed_vfov});
+  return {};
+}
+
+// One plane of the orientation or lens kernel: src -> dst through geometry g, with its sphere tables (nullptr: none)
+t360::OrientedPlane orientedPlane(const uint8_t* src, int srcPitch, uint8_t* dst, int dstPitch, const t360::SphereGeometry& g,
+                                  const float* tables) {
+  t360::OrientedPlane v{};
+  v.src = src;
+  v.srcPitch = srcPitch;
+  v.dst = dst;
+  v.dstPitch = dstPitch;
+  v.geometry = g;
+  v.colTable = tables;
+  v.rowTable = tables ? tables + t360::sphereTableRowOffset(g) : nullptr;
+  return v;
+}
+
+// The upload ring entry may be refilled once the work enqueued on s so far has finished (nullptr: nothing to release)
+void releaseAfter(UploadRing::Entry* e, cudaStream_t s) {
+  if (!e) return;
+  CU(cudaEventRecord(e->released, s));
+  e->inFlight = true;
+}
 
 // ---- fisheye lens rigs (T360B200_lensMap, T360B200_transformFrameLensAsync; oriented_view.h: lensSample) ----------------
 // true, with the reason in *why, when the lens path cannot serve ctx with this rig and orientation
@@ -502,7 +619,7 @@ class VideoFrameTransform {
   // and installs it in place of the index's previous plan.
   template <class Plan>
   bool installPlan(int planIndex, Plan&& plan) {
-    try {
+    return guarded("Could not generate map for plane " + std::to_string(planIndex), [&] {
       reconfigureWait(true);  // a pending reconfigureAsync re-plans the other indices: it is finished first
       std::lock_guard<std::mutex> planLock(planMu_);
       FrameTransformContext ctx;
@@ -518,13 +635,7 @@ class VideoFrameTransform {
       plans_[planIndex] = std::move(d);
       ++planGeneration_;
       return true;
-    } catch (const CudaFail& f) {
-      std::printf("Could not generate map for plane %d. Error: CUDA %s (%s) in %s\n", planIndex,
-                  cudaGetErrorName(f.err), cudaGetErrorString(f.err), f.what);
-    } catch (const std::exception& ex) {
-      std::printf("Could not generate map for plane %d. Error: %s\n", planIndex, ex.what());
-    }
-    return false;
+    });
   }
 
   // Replaces the context of a running transform: every plan index is re-planned for `next` with the sizes it was
@@ -533,7 +644,7 @@ class VideoFrameTransform {
   // released once the device has finished the work enqueued before the swap (retire).  A pending reconfigureAsync is
   // discarded.  On any failure the old configuration stays in effect.
   bool reconfigure(const FrameTransformContext& next) {
-    try {
+    return guarded("Could not reconfigure the transform", [&] {
       std::lock_guard<std::mutex> planLock(planMu_);  // (one re-plan at a time, also against generateMapForPlane)
       if (refuseWarpPlans("Could not reconfigure the transform")) return false;
       unsigned long long seq;
@@ -554,13 +665,7 @@ class VideoFrameTransform {
       install(set, next, seq, true);
       retire(set);
       return true;
-    } catch (const CudaFail& f) {
-      std::printf("Could not reconfigure the transform. Error: CUDA %s (%s) in %s\n", cudaGetErrorName(f.err), cudaGetErrorString(f.err), f.what);
-      cudaGetLastError();
-    } catch (const std::exception& ex) {
-      std::printf("Could not reconfigure the transform. Error: %s\n", ex.what());
-    }
-    return false;
+    });
   }
 
   // T360B200_reconfigureAsync: `next` is in effect for every frame enqueued after the call returns; until its plans are in,
@@ -615,9 +720,10 @@ class VideoFrameTransform {
   // reference transformFramePlane (cpp:1319-1351): host or device planes, synchronous.
   bool transformFramePlane(uint8_t* in, uint8_t* out, int inW, int inH, int inPitch, int outW, int outH, int outPitch,
                            int planIndex, int imagePlaneIndex) {
-    try {
+    const std::string what = "Could not transform the plane " + std::to_string(imagePlaneIndex);
+    return guarded(what, [&] {
       if (!in || !out || inW <= 0 || inH <= 0 || outW <= 0 || outH <= 0 || inPitch < inW || outPitch < outW) {
-        std::printf("Could not transform the plane %d. Error: invalid plane description\n", imagePlaneIndex);
+        std::printf("%s. Error: invalid plane description\n", what.c_str());
         return false;
       }
       std::shared_lock<std::shared_mutex> config = lockPlanned("Could not transform the plane");
@@ -667,14 +773,7 @@ class VideoFrameTransform {
         CU(cudaMemcpy2DAsync(out, outPitch, dOut, dOutPitch, outW, outH, cudaMemcpyDeviceToHost, stream_));
       CU(cudaStreamSynchronize(stream_));
       return true;
-    } catch (const CudaFail& f) {
-      std::printf("Could not transform the plane %d. Error: CUDA %s (%s) in %s\n", imagePlaneIndex,
-                  cudaGetErrorName(f.err), cudaGetErrorString(f.err), f.what);
-      cudaGetLastError();
-    } catch (const std::exception& ex) {
-      std::printf("Could not transform the plane %d. Error: %s\n", imagePlaneIndex, ex.what());
-    }
-    return false;
+    });
   }
 
   // ---- streaming a large host plane through the device -------------------------------------------------------
@@ -947,7 +1046,7 @@ class VideoFrameTransform {
   // device to device, asynchronous
   bool transformDevice(const uint8_t* dIn, uint8_t* dOut, int inW, int inH, int inPitch, int outW, int outH,
                        int outPitch, int planIndex, cudaStream_t stream) {
-    try {
+    return guarded("Could not transform the plane " + std::to_string(planIndex), [&] {
       std::shared_lock<std::shared_mutex> config = lockPlanned("Could not transform the plane");
       if (!config.owns_lock()) return false;
       const DeviceRestore restoreDevice = ensureDevice();
@@ -956,29 +1055,18 @@ class VideoFrameTransform {
       cudaStream_t s = stream ? stream : stream_;
       if (plan->transparent && planIndex) CU(cudaMemset2DAsync(dOut, outPitch, 128, outW, outH, s));
       return enqueue(*plan, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, s, planIndex, slotFor(s).lanes[0]);
-    } catch (const CudaFail& f) {
-      std::printf("Could not transform the plane %d. Error: CUDA %s (%s) in %s\n", planIndex, cudaGetErrorName(f.err),
-                  cudaGetErrorString(f.err), f.what);
-      cudaGetLastError();
-    } catch (const std::exception& ex) {
-      std::printf("Could not transform the plane %d. Error: %s\n", planIndex, ex.what());
-    }
-    return false;
+    });
   }
 
   // Whole frame, device to device, asynchronous: plane 0 with plan 0 on the caller's stream, planes 1.. with plan 1
   // on their own lanes (the planes are independent: reference vf_transform360.c:368-397 loops over them).
-  bool transformFrameDevice(int numPlanes, const uint8_t* const* dIn, uint8_t* const* dOut, const int* inW, const int* inH,
-                            const int* inPitch, const int* outW, const int* outH, const int* outPitch, cudaStream_t stream) {
-    try {
-      if (numPlanes < 1 || numPlanes > kPlaneLanes) {
-        std::printf("Could not transform the frame. Error: %d planes (1..%d supported)\n", numPlanes, kPlaneLanes);
-        return false;
-      }
+  bool transformFrameDevice(const FramePlanes& f, cudaStream_t stream) {
+    const int numPlanes = f.numPlanes;
+    return guarded("Could not transform the frame", [&] {
       std::shared_lock<std::shared_mutex> config(configMu_);
       while (perFrameOnly_) {  // a reconfigureAsync is pending: the per-frame kernels serve planes of the planned sizes
-        if (planesOfPlannedSize(numPlanes, inW, inH))
-          return perFrameLocked("while its plan is pending", ctx_, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, stream);
+        if (planesOfPlannedSize(f))
+          return perFrameLocked("Could not transform the frame while its plan is pending", ctx_, f, stream);
         config.unlock();
         if (reconfigureWait(true) < 0) {
           std::printf("Could not transform the frame. Error: the background planner failed on the current context\n");
@@ -1005,9 +1093,9 @@ class VideoFrameTransform {
         clear[p] = plans[p]->blur.needsClear;
         lowPass = lowPass && plans[p]->lowPass;
       }
-      const bool mergedBlur = lowPass && mergeable(plans, lists, clear, numPlanes, inW, inH);
+      const bool mergedBlur = lowPass && mergeable(plans, lists, clear, numPlanes, f.inW, f.inH);
       if (mergedBlur) {
-        blurFrame(plans, numPlanes, dIn, inW, inH, inPitch, lanes_, s);
+        blurFrame(plans, f, lanes_, s);
         sideWork = false;
       }
       // Stage 1, planes side by side (chroma on its own lanes): everything before the gather.
@@ -1018,8 +1106,9 @@ class VideoFrameTransform {
       for (int p = numPlanes - 1; p >= 0; --p) {
         cudaStream_t ps = (p && fork) ? lanes_[p].main : s;
         if (p && fork) CU(cudaStreamWaitEvent(ps, frameFork_, 0));
-        if (plans[p]->transparent && p) CU(cudaMemset2DAsync(dOut[p], outPitch[p], 128, outW[p], outH[p], ps));
-        if (!prepareGather(*plans[p], dIn[p], dOut[p], inW[p], inH[p], inPitch[p], outW[p], outH[p], outPitch[p], ps, p, lanes_[p], work[p], mergedBlur))
+        if (plans[p]->transparent && p) CU(cudaMemset2DAsync(f.out[p], f.outPitch[p], 128, f.outW[p], f.outH[p], ps));
+        if (!prepareGather(*plans[p], f.in[p], f.out[p], f.inW[p], f.inH[p], f.inPitch[p], f.outW[p], f.outH[p], f.outPitch[p], ps, p, lanes_[p],
+                           work[p], mergedBlur))
           return false;
         allStaged = allStaged && work[p].staged;
       }
@@ -1047,18 +1136,12 @@ class VideoFrameTransform {
       }
       for (int p = 1; p < numPlanes; ++p) CU(cudaStreamWaitEvent(s, lanes_[p].done, 0));
       return true;
-    } catch (const CudaFail& f) {
-      std::printf("Could not transform the frame. Error: CUDA %s (%s) in %s\n", cudaGetErrorName(f.err), cudaGetErrorString(f.err), f.what);
-      cudaGetLastError();
-    } catch (const std::exception& ex) {
-      std::printf("Could not transform the frame. Error: %s\n", ex.what());
-    }
-    return false;
+    });
   }
 
   bool lowPassDevice(const uint8_t* dIn, uint8_t* dOut, int w, int h, int inPitch, int outPitch, int planIndex,
                      cudaStream_t stream) {
-    try {
+    return guarded("Could not filter plane " + std::to_string(planIndex), [&] {
       std::shared_lock<std::shared_mutex> config = lockPlanned("Could not filter the plane");
       if (!config.owns_lock()) return false;
       const DeviceRestore restoreDevice = ensureDevice();
@@ -1070,107 +1153,44 @@ class VideoFrameTransform {
       }
       runLowPass(*plan, dIn, dOut, w, h, inPitch, outPitch, stream ? stream : stream_);
       return true;
-    } catch (const CudaFail& f) {
-      std::printf("Could not filter plane %d. Error: CUDA %s (%s) in %s\n", planIndex, cudaGetErrorName(f.err),
-                  cudaGetErrorString(f.err), f.what);
-      cudaGetLastError();
+    });
+  }
+
+  // Whole frame with per-frame view fields (T360B200_transformFrameViewAsync, ...OrientedAsync, ...PoseAsync): the frame a
+  // fresh transform would give for the context with the fields of `fields` (a T360View, T360Orientation or T360Pose, checked
+  // by withFields) substituted, with no re-plan (perFrameLocked).  `what` names the call in the messages.
+  template <class Fields>
+  bool transformFrameWith(const char* what, const Fields& fields, const FramePlanes& f, cudaStream_t stream) {
+    std::shared_lock<std::shared_mutex> config(configMu_);
+    if (refuseWarpPlans(what)) return false;
+    FrameTransformContext ctx = ctx_;
+    const std::string why = withFields(ctx, fields);
+    if (!why.empty()) {
+      std::printf("%s. Error: %s\n", what, why.c_str());
+      return false;
     }
-    return false;
-  }
-
-  // Whole frame with a per-frame FLAT_FIXED view (T360B200_transformFrameViewAsync): the frame a fresh transform would give
-  // for the context with fixed_yaw / pitch / hfov / vfov replaced by `view`, with no re-plan (perFrame).
-  bool transformFrameView(const t360::FlatView& view, int numPlanes, const uint8_t* const* dIn, uint8_t* const* dOut, const int* inW,
-                          const int* inH, const int* inPitch, const int* outW, const int* outH, const int* outPitch, cudaStream_t stream) {
-    auto substitute = [&](FrameTransformContext& ctx) {
-      if (!std::isfinite(view.yaw) || !std::isfinite(view.pitch) || !std::isfinite(view.hfov) || !std::isfinite(view.vfov)) {
-        std::printf("Could not transform the frame with a view. Error: the view (yaw %g, pitch %g, hfov %g, vfov %g) is not finite\n",
-                    view.yaw, view.pitch, view.hfov, view.vfov);
-        return false;
-      }
-      if (ctx.output_layout != LAYOUT_FLAT_FIXED) {
-        std::printf("Could not transform the frame with a view. Error: per-frame views need output_layout FLAT_FIXED (%d), the transform has %d\n",
-                    static_cast<int>(LAYOUT_FLAT_FIXED), static_cast<int>(ctx.output_layout));
-        return false;
-      }
-      ctx.fixed_yaw = view.yaw;
-      ctx.fixed_pitch = view.pitch;
-      ctx.fixed_hfov = view.hfov;
-      ctx.fixed_vfov = view.vfov;
-      return true;
-    };
-    return perFrame("with a view", substitute, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, stream);
-  }
-
-  // Whole frame of a CUBEMAP_32, CUBEMAP_23_OFFCENTER, EAC_32 or EQUIRECT transform with a per-frame orientation
-  // (T360B200_transformFrameOrientedAsync): the frame a fresh transform would give for the context with fixed_yaw / pitch /
-  // roll replaced by `o`, with no re-plan (perFrame).
-  bool transformFrameOriented(const t360::Orientation& o, int numPlanes, const uint8_t* const* dIn, uint8_t* const* dOut, const int* inW,
-                              const int* inH, const int* inPitch, const int* outW, const int* outH, const int* outPitch, cudaStream_t stream) {
-    auto substitute = [&](FrameTransformContext& ctx) {
-      if (!std::isfinite(o.yaw) || !std::isfinite(o.pitch) || !std::isfinite(o.roll)) {
-        std::printf("Could not transform the frame with an orientation. Error: the orientation (yaw %g, pitch %g, roll %g) is not finite\n",
-                    o.yaw, o.pitch, o.roll);
-        return false;
-      }
-      if (!t360::orientedLayouts(ctx)) {
-        std::printf("Could not transform the frame with an orientation. Error: per-frame orientations need output_layout CUBEMAP_32, "
-                    "CUBEMAP_23_OFFCENTER, EAC_32 or EQUIRECT and input_layout EQUIRECT or CUBEMAP_32, the transform has %d -> %d%s\n",
-                    static_cast<int>(ctx.input_layout), static_cast<int>(ctx.output_layout),
-                    ctx.output_layout == LAYOUT_FLAT_FIXED ? " (FLAT_FIXED views: T360B200_transformFrameViewAsync)" : "");
-        return false;
-      }
-      ctx.fixed_yaw = o.yaw;
-      ctx.fixed_pitch = o.pitch;
-      ctx.fixed_roll = o.roll;
-      return true;
-    };
-    return perFrame("with an orientation", substitute, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, stream);
-  }
-
-  // Whole frame of any transform with a per-frame pose (T360B200_transformFramePoseAsync): the frame a fresh transform would
-  // give for the context with its five view fields replaced by `pose`, with no re-plan (perFrame).  FLAT_FIXED takes the
-  // view kernel (roll plays no part there, as in the planner), every other layout the orientation kernel.
-  bool transformFramePose(const T360Pose& pose, int numPlanes, const uint8_t* const* dIn, uint8_t* const* dOut, const int* inW,
-                          const int* inH, const int* inPitch, const int* outW, const int* outH, const int* outPitch, cudaStream_t stream) {
-    auto substitute = [&](FrameTransformContext& ctx) {
-      if (!std::isfinite(pose.yaw) || !std::isfinite(pose.pitch) || !std::isfinite(pose.roll) || !std::isfinite(pose.hfov) ||
-          !std::isfinite(pose.vfov)) {
-        std::printf("Could not transform the frame with a pose. Error: the pose (yaw %g, pitch %g, roll %g, hfov %g, vfov %g) is not finite\n",
-                    pose.yaw, pose.pitch, pose.roll, pose.hfov, pose.vfov);
-        return false;
-      }
-      substitutePose(ctx, pose);
-      return true;
-    };
-    return perFrame("with a pose", substitute, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, stream);
+    return perFrameLocked(what, ctx, f, stream);
   }
 
   // Whole frame through the caller's per-plane device maps (T360B200_remapFrameAsync): one gather launch for all planes,
   // every record computed from its map entry as quantizeWarpMap does, so a map gives what generateMapFromWarp plans for it.
   // Needs no plan; the interpolation comes from the current context.  Every refusal comes before the first CUDA call, and
   // nothing here synchronises the device.
-  bool remapFrame(int numPlanes, const float* const* maps, const int* mapPitch, int border, const uint8_t* const* dIn, uint8_t* const* dOut,
-                  const int* inW, const int* inH, const int* inPitch, const int* outW, const int* outH, const int* outPitch, cudaStream_t stream) {
+  bool remapFrame(const float* const* maps, const int* mapPitch, int border, const FramePlanes& f, cudaStream_t stream) {
     const char* what = "Could not remap the frame";
-    try {
-      if (numPlanes < 1 || numPlanes > kPlaneLanes) {
-        std::printf("%s. Error: %d planes (1..%d supported)\n", what, numPlanes, kPlaneLanes);
-        return false;
-      }
+    return guarded(what, [&] {
       if (border != t360::kBorderWrap && border != t360::kBorderTransparent) {
         std::printf("%s. Error: border %d (3: BORDER_WRAP, 5: BORDER_TRANSPARENT)\n", what, border);
         return false;
       }
-      for (int p = 0; p < numPlanes; ++p) {
-        if (!maps[p] || !dIn[p] || !dOut[p] || inW[p] <= 0 || inH[p] <= 0 || outW[p] <= 0 || outH[p] <= 0 || inPitch[p] < inW[p] ||
-            outPitch[p] < outW[p]) {
+      for (int p = 0; p < f.numPlanes; ++p) {
+        if (!maps[p]) {
           std::printf("%s. Error: invalid description of plane %d\n", what, p);
           return false;
         }
-        if (mapPitch[p] % 8 != 0 || mapPitch[p] / 8 < outW[p] || (reinterpret_cast<uintptr_t>(maps[p]) & 7)) {
+        if (mapPitch[p] % 8 != 0 || mapPitch[p] / 8 < f.outW[p] || (reinterpret_cast<uintptr_t>(maps[p]) & 7)) {
           std::printf("%s. Error: the map of plane %d (pitch %d bytes) must be 8-byte aligned with a pitch that is a multiple of 8 and at "
-                      "least 8 x the output width %d\n", what, p, mapPitch[p], outW[p]);
+                      "least 8 x the output width %d\n", what, p, mapPitch[p], f.outW[p]);
           return false;
         }
       }
@@ -1189,47 +1209,29 @@ class VideoFrameTransform {
       cudaStream_t s = stream ? stream : stream_;
       const bool transparent = border == t360::kBorderTransparent;
       t360::MapGatherParams mp{};
-      for (int p = 0; p < numPlanes; ++p) {
+      for (int p = 0; p < f.numPlanes; ++p) {
         // BORDER_TRANSPARENT leaves a pixel whose anchor tap lies outside the source as it finds it: chroma outputs start at
         // 128 as in the planned path (reference cpp:743-747), luma outputs keep the caller's bytes
-        if (transparent && p) CU(cudaMemset2DAsync(dOut[p], outPitch[p], 128, outW[p], outH[p], s));
-        mp.plane[p] = t360::MapPlane{dIn[p], dOut[p], inPitch[p], outPitch[p], reinterpret_cast<const float2*>(maps[p]), mapPitch[p] / 8,
-                                     t360::MapGeometry{outW[p], outH[p], inW[p], inH[p]}, 0, 0};
+        if (transparent && p) CU(cudaMemset2DAsync(f.out[p], f.outPitch[p], 128, f.outW[p], f.outH[p], s));
+        mp.plane[p] = t360::MapPlane{f.in[p], f.out[p], f.inPitch[p], f.outPitch[p], reinterpret_cast<const float2*>(maps[p]), mapPitch[p] / 8,
+                                     t360::MapGeometry{f.outW[p], f.outH[p], f.inW[p], f.inH[p]}, 0, 0};
       }
-      mp.numPlanes = numPlanes;
+      mp.numPlanes = f.numPlanes;
       mp.kernelSize = k;
       mp.transparent = transparent;
       mp.weights = deviceWeights(ctx.interpolation_alg);
       CU(t360::launchMapGather(mp, numSMs_, s));
       return true;
-    } catch (const CudaFail& f) {
-      std::printf("%s. Error: CUDA %s (%s) in %s\n", what, cudaGetErrorName(f.err), cudaGetErrorString(f.err), f.what);
-      cudaGetLastError();
-    } catch (const std::exception& ex) {
-      std::printf("%s. Error: %s\n", what, ex.what());
-    }
-    return false;
+    });
   }
 
   // Whole frame of a fisheye lens rig (T360B200_transformFrameLensAsync): one gather launch for all planes, every record
   // computed by lensSample (oriented_view.h), so a rig gives what lensMap -> generateMapFromWarp plans for it.  Needs no
   // plan and leaves the plans alone; the output layout's tables come through the slot's upload ring.  Every refusal comes
   // before the first CUDA call, and nothing here synchronises the device.
-  bool transformFrameLens(const T360LensRig* rig, const T360Orientation* o, int numPlanes, const uint8_t* const* dIn, uint8_t* const* dOut,
-                          const int* inW, const int* inH, const int* inPitch, const int* outW, const int* outH, const int* outPitch,
-                          cudaStream_t stream) {
+  bool transformFrameLens(const T360LensRig* rig, const T360Orientation* o, const FramePlanes& f, cudaStream_t stream) {
     const char* what = "Could not transform the frame with a lens rig";
-    try {
-      if (numPlanes < 1 || numPlanes > kPlaneLanes) {
-        std::printf("%s. Error: %d planes (1..%d supported)\n", what, numPlanes, kPlaneLanes);
-        return false;
-      }
-      for (int p = 0; p < numPlanes; ++p) {
-        if (!dIn[p] || !dOut[p] || inW[p] <= 0 || inH[p] <= 0 || outW[p] <= 0 || outH[p] <= 0 || inPitch[p] < inW[p] || outPitch[p] < outW[p]) {
-          std::printf("%s. Error: invalid description of plane %d\n", what, p);
-          return false;
-        }
-      }
+    return guarded(what, [&] {
       std::shared_lock<std::shared_mutex> config(configMu_);
       const FrameTransformContext ctx = ctx_;
       std::string why;
@@ -1244,59 +1246,23 @@ class VideoFrameTransform {
       StreamSlot& slot = slotFor(s);
       const float* tables[kPlaneLanes];
       UploadRing::Entry* staged = nullptr;
-      sphereTablesFor(lens, numPlanes, outW, outH, slot, s, tables, &staged);
+      sphereTablesFor(lens, f.numPlanes, f.outW, f.outH, slot, s, tables, &staged);
       t360::LensGatherParams lp{};
-      for (int p = 0; p < numPlanes; ++p) {
+      for (int p = 0; p < f.numPlanes; ++p) {
         // BORDER_TRANSPARENT: chroma outputs start at 128 as in the planned path, luma outputs keep the caller's bytes
-        if (p) CU(cudaMemset2DAsync(dOut[p], outPitch[p], 128, outW[p], outH[p], s));
-        t360::OrientedPlane& v = lp.plane[p];
-        v.src = dIn[p];
-        v.srcPitch = inPitch[p];
-        v.dst = dOut[p];
-        v.dstPitch = outPitch[p];
-        v.geometry = t360::sphereGeometry(lens, outW[p], outH[p], inW[p], inH[p], k);
-        v.colTable = tables[p];
-        v.rowTable = tables[p] ? tables[p] + t360::sphereTableRowOffset(v.geometry) : nullptr;
+        if (p) CU(cudaMemset2DAsync(f.out[p], f.outPitch[p], 128, f.outW[p], f.outH[p], s));
+        lp.plane[p] = orientedPlane(f.in[p], f.inPitch[p], f.out[p], f.outPitch[p],
+                                    t360::sphereGeometry(lens, f.outW[p], f.outH[p], f.inW[p], f.inH[p], k), tables[p]);
       }
-      lp.numPlanes = numPlanes;
+      lp.numPlanes = f.numPlanes;
       lp.rotation = t360::rotationFromAngles(o->yaw, o->pitch, o->roll);
       lp.rig = lensRigModel(*rig);
       lp.kernelSize = k;
       lp.weights = deviceWeights(ctx.interpolation_alg);
       CU(t360::launchLensGather(lp, numSMs_, s));
-      if (staged) {  // the entry may be refilled once this launch has finished
-        CU(cudaEventRecord(staged->released, s));
-        staged->inFlight = true;
-      }
+      releaseAfter(staged, s);
       return true;
-    } catch (const CudaFail& f) {
-      std::printf("%s. Error: CUDA %s (%s) in %s\n", what, cudaGetErrorName(f.err), cudaGetErrorString(f.err), f.what);
-      cudaGetLastError();
-    } catch (const std::exception& ex) {
-      std::printf("%s. Error: %s\n", what, ex.what());
-    }
-    return false;
-  }
-
-  static void substitutePose(FrameTransformContext& ctx, const T360Pose& pose) {
-    ctx.fixed_yaw = pose.yaw;
-    ctx.fixed_pitch = pose.pitch;
-    ctx.fixed_roll = pose.roll;
-    ctx.fixed_hfov = pose.hfov;
-    ctx.fixed_vfov = pose.vfov;
-  }
-
-  // The frame of a per-frame call (view, orientation, pose), device to device, asynchronous on `stream`.  Under the reader
-  // lock, `substitute` checks the call's arguments against the current context and puts the frame's view fields into a
-  // copy of it (false: refused, with a message); `what` names the call in the messages.  The frame is then perFrameLocked's.
-  template <class Substitute>
-  bool perFrame(const char* what, Substitute& substitute, int numPlanes, const uint8_t* const* dIn, uint8_t* const* dOut, const int* inW,
-                const int* inH, const int* inPitch, const int* outW, const int* outH, const int* outPitch, cudaStream_t stream) {
-    std::shared_lock<std::shared_mutex> config(configMu_);
-    if (refuseWarpPlans((std::string("Could not transform the frame ") + what).c_str())) return false;
-    FrameTransformContext ctx = ctx_;
-    if (!substitute(ctx)) return false;
-    return perFrameLocked(what, ctx, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, stream);
+    });
   }
 
   // The frame a fresh transform made with `ctx` would give, on the per-frame kernels, with the reader lock held: the
@@ -1306,26 +1272,22 @@ class VideoFrameTransform {
   // and weights, low-pass on or off and its segments (re-planned on the host, viewLowPass), and while a reconfigureAsync is
   // pending the tables (built on the host and uploaded in stream order, sphereTablesFor); only the plane and map sizes, which
   // ctx cannot change, come from the plans.  Scale factors render at the map's size, then resize with INTER_AREA.  Every
-  // refusal comes before the first CUDA call.  Nothing here synchronises the device, and the plans' sampling data is not read.
-  bool perFrameLocked(const char* what, const FrameTransformContext& ctx, int numPlanes, const uint8_t* const* dIn, uint8_t* const* dOut,
-                      const int* inW, const int* inH, const int* inPitch, const int* outW, const int* outH, const int* outPitch,
-                      cudaStream_t stream) {
-    try {
-      if (numPlanes < 1 || numPlanes > kPlaneLanes) {
-        std::printf("Could not transform the frame %s. Error: %d planes (1..%d supported)\n", what, numPlanes, kPlaneLanes);
-        return false;
-      }
+  // refusal comes before the first CUDA call, with a message prefixed by `what`.  Nothing here synchronises the device, and
+  // the plans' sampling data is not read.
+  bool perFrameLocked(const char* what, const FrameTransformContext& ctx, const FramePlanes& f, cudaStream_t stream) {
+    return guarded(what, [&] {
+      const int numPlanes = f.numPlanes;
       const int k = t360::kernelSizeOf(ctx.interpolation_alg);
       const DevicePlan* plans[kPlaneLanes];
       for (int p = 0; p < numPlanes; ++p) {
         if (!(plans[p] = findPlan(p ? 1 : 0, p))) return false;
-        if (inW[p] != plans[p]->inW || inH[p] != plans[p]->inH) {
-          std::printf("Could not transform the frame %s. Error: input plane %d is %dx%d, its map was generated for %dx%d\n", what, p,
-                      inW[p], inH[p], plans[p]->inW, plans[p]->inH);
+        if (f.inW[p] != plans[p]->inW || f.inH[p] != plans[p]->inH) {
+          std::printf("%s. Error: input plane %d is %dx%d, its map was generated for %dx%d\n", what, p, f.inW[p], f.inH[p], plans[p]->inW,
+                      plans[p]->inH);
           return false;
         }
         if (k == 0) {
-          std::printf("Could not transform the frame %s. Error: no interpolation algorithm %d\n", what, ctx.interpolation_alg);
+          std::printf("%s. Error: no interpolation algorithm %d\n", what, ctx.interpolation_alg);
           return false;
         }
       }
@@ -1334,8 +1296,8 @@ class VideoFrameTransform {
       StreamSlot& slot = slotFor(s);
       const uint8_t* src[kPlaneLanes];
       int srcPitch[kPlaneLanes];
-      for (int p = 0; p < numPlanes; ++p) { src[p] = dIn[p]; srcPitch[p] = inPitch[p]; }
-      if (ctx.enable_low_pass_filter && !viewLowPass(what, ctx, plans, numPlanes, dIn, inW, inH, inPitch, slot, s, src, srcPitch)) return false;
+      for (int p = 0; p < numPlanes; ++p) { src[p] = f.in[p]; srcPitch[p] = f.inPitch[p]; }
+      if (ctx.enable_low_pass_filter && !viewLowPass(what, ctx, plans, f, slot, s, src, srcPitch)) return false;
 
       // render targets: the output, or when its size is not the map's the slot's plane at the map's size (cpp:755-777).
       // Barrel plans (BORDER_TRANSPARENT) leave a pixel whose anchor tap is outside the source as they find it, so the
@@ -1345,29 +1307,23 @@ class VideoFrameTransform {
       int dstPitch[kPlaneLanes];
       for (int p = 0; p < numPlanes; ++p) {
         const DevicePlan& plan = *plans[p];
-        dst[p] = dOut[p];
-        dstPitch[p] = outPitch[p];
-        if (outW[p] != plan.mapW || outH[p] != plan.mapH) {
+        dst[p] = f.out[p];
+        dstPitch[p] = f.outPitch[p];
+        if (f.outW[p] != plan.mapW || f.outH[p] != plan.mapH) {
           const int sp = alignedPitch(plan.mapW);
           slot.lanes[p].scaled.reserve(static_cast<size_t>(sp) * plan.mapH + 64);
           dst[p] = slot.lanes[p].scaled.ptr;
           dstPitch[p] = sp;
           if (plan.transparent) CU(cudaMemset2DAsync(dst[p], sp, p ? 128 : 0, plan.mapW, plan.mapH, s));
         } else if (plan.transparent && p) {
-          CU(cudaMemset2DAsync(dst[p], dstPitch[p], 128, outW[p], outH[p], s));
+          CU(cudaMemset2DAsync(dst[p], dstPitch[p], 128, f.outW[p], f.outH[p], s));
         }
       }
-      const bool stereoIn = ctx.input_stereo_format != STEREO_FORMAT_MONO;
       if (ctx.output_layout == LAYOUT_FLAT_FIXED) {
         t360::ViewGatherParams vp{};
         for (int p = 0; p < numPlanes; ++p) {
           const DevicePlan& plan = *plans[p];
-          vp.plane[p] = t360::ViewPlane{src[p], dst[p], srcPitch[p], dstPitch[p],
-                                        t360::FlatGeometry{plan.mapW, plan.mapH, plan.inW, plan.inH, k,
-                                                           stereoIn && ctx.output_stereo_format == STEREO_FORMAT_LR,
-                                                           stereoIn && ctx.output_stereo_format == STEREO_FORMAT_TB, ctx.vflip != 0,
-                                                           ctx.input_stereo_format == STEREO_FORMAT_LR,
-                                                           ctx.input_stereo_format == STEREO_FORMAT_TB},
+          vp.plane[p] = t360::ViewPlane{src[p], dst[p], srcPitch[p], dstPitch[p], t360::flatGeometry(ctx, plan.mapW, plan.mapH, plan.inW, plan.inH, k),
                                         0, 0};
         }
         vp.numPlanes = numPlanes;
@@ -1387,42 +1343,26 @@ class VideoFrameTransform {
         }
         for (int p = 0; p < numPlanes; ++p) {
           const DevicePlan& plan = *plans[p];
-          t360::OrientedPlane& v = op.plane[p];
-          v.src = src[p];
-          v.srcPitch = srcPitch[p];
-          v.dst = dst[p];
-          v.dstPitch = dstPitch[p];
-          v.geometry = t360::sphereGeometry(ctx, plan.mapW, plan.mapH, plan.inW, plan.inH, k);
-          v.colTable = tables[p];
-          v.rowTable = tables[p] ? tables[p] + t360::sphereTableRowOffset(v.geometry) : nullptr;
+          op.plane[p] = orientedPlane(src[p], srcPitch[p], dst[p], dstPitch[p], t360::sphereGeometry(ctx, plan.mapW, plan.mapH, plan.inW, plan.inH, k),
+                                      tables[p]);
         }
         op.numPlanes = numPlanes;
         op.rotation = t360::rotationFromAngles(ctx.fixed_yaw, ctx.fixed_pitch, ctx.fixed_roll);
         op.kernelSize = k;
         op.weights = deviceWeights(ctx.interpolation_alg);
         CU(t360::launchOrientedGather(op, numSMs_, s));
-        if (staged) {  // the entry may be refilled once this launch has finished
-          CU(cudaEventRecord(staged->released, s));
-          staged->inFlight = true;
-        }
+        releaseAfter(staged, s);
       }
       for (int p = 0; p < numPlanes; ++p) {
-        if (dst[p] == dOut[p]) continue;
+        if (dst[p] == f.out[p]) continue;
         const DevicePlan& plan = *plans[p];
-        const DevicePlan::Resize& r = resizeFor(plan, outW[p], outH[p]);
-        t360::AreaParams ap{dst[p], dOut[p], plan.mapW, plan.mapH, dstPitch[p], outW[p], outH[p], outPitch[p],
+        const DevicePlan::Resize& r = resizeFor(plan, f.outW[p], f.outH[p]);
+        t360::AreaParams ap{dst[p], f.out[p], plan.mapW, plan.mapH, dstPitch[p], f.outW[p], f.outH[p], f.outPitch[p],
                             r.cellW, r.cellH, r.xTaps.ptr, r.xFirst.ptr, r.yTaps.ptr, r.yFirst.ptr, r.xLinear.ptr, r.yLinear.ptr, r.xMax};
         CU(t360::launchAreaResize(ap, s));
       }
       return true;
-    } catch (const CudaFail& f) {
-      std::printf("Could not transform the frame %s. Error: CUDA %s (%s) in %s\n", what, cudaGetErrorName(f.err), cudaGetErrorString(f.err),
-                  f.what);
-      cudaGetLastError();
-    } catch (const std::exception& ex) {
-      std::printf("Could not transform the frame %s. Error: %s\n", what, ex.what());
-    }
-    return false;
+    });
   }
 
   // tuning aid: a timeline of the consumer groups of the last frame gather (see StagedParams::trace)
@@ -1825,24 +1765,24 @@ class VideoFrameTransform {
   }
 
   // The low-pass of all planes of a frame (mergeable): one launch per vertical kernel half-size.
-  void blurFrame(const DevicePlan* const* plans, int numPlanes, const uint8_t* const* dIn, const int* inW, const int* inH, const int* inPitch,
-                 PlaneLane* lanes, cudaStream_t s) {
-    const FrameListRefs f = frameLists(plans, numPlanes);
+  void blurFrame(const DevicePlan* const* plans, const FramePlanes& f, PlaneLane* lanes, cudaStream_t s) {
+    const FrameListRefs l = frameLists(plans, f.numPlanes);
     t360::FrameStripParams fp{};
-    for (int p = 0; p < numPlanes; ++p) {
-      const int bp = alignedPitch(inW[p]);
-      lanes[p].blurred.reserve(static_cast<size_t>(bp) * inH[p] + 64);
-      fp.plane[p] = {dIn[p], lanes[p].blurred.ptr, inW[p], inH[p], inPitch[p], bp};
+    for (int p = 0; p < f.numPlanes; ++p) {
+      const int bp = alignedPitch(f.inW[p]);
+      lanes[p].blurred.reserve(static_cast<size_t>(bp) * f.inH[p] + 64);
+      fp.plane[p] = {f.in[p], lanes[p].blurred.ptr, f.inW[p], f.inH[p], f.inPitch[p], bp};
     }
-    launchLowPass(f.blurLayout, false, f.blurImage, f.blurImage, fp, numPlanes, s);
+    launchLowPass(l.blurLayout, false, l.blurImage, l.blurImage, fp, f.numPlanes, s);
   }
 
-  // The low-pass of a per-view frame (transformFrameView): the segments and taps of every plan index for the view, the
-  // job lists cut from them, uploaded through the slot's rings, and the launches -- one per vertical kernel size for all
+  // The low-pass of a per-frame call's frame (perFrameLocked): the segments and taps of every plan index for the context,
+  // the job lists cut from them, uploaded through the slot's rings, and the launches -- one per vertical kernel size for all
   // planes when every plane takes the strip kernel only (as blurFrame), else per plane (as runLowPass).  src / srcPitch
   // receive the blurred planes.
-  bool viewLowPass(const char* what, const FrameTransformContext& ctx, const DevicePlan* const* plans, int numPlanes, const uint8_t* const* dIn,
-                   const int* inW, const int* inH, const int* inPitch, StreamSlot& slot, cudaStream_t s, const uint8_t** src, int* srcPitch) {
+  bool viewLowPass(const char* what, const FrameTransformContext& ctx, const DevicePlan* const* plans, const FramePlanes& f, StreamSlot& slot,
+                   cudaStream_t s, const uint8_t** src, int* srcPitch) {
+    const int numPlanes = f.numPlanes;
     const int indices = numPlanes > 1 ? 2 : 1;
     HostPlan h[2];
     // what the job lists depend on: the plans (generation), the planes, and per segment its rectangle, tap counts and
@@ -1853,7 +1793,7 @@ class VideoFrameTransform {
       h[idx].ctx = ctx;
       h[idx].inW = plan.inW; h[idx].inH = plan.inH; h[idx].outW = plan.outW; h[idx].outH = plan.outH; h[idx].mapW = plan.mapW; h[idx].mapH = plan.mapH;
       if (!t360::buildLowPassPlan(h[idx])) {
-        std::printf("Could not transform the frame %s. Error: no low-pass plan for index %d\n", what, idx);
+        std::printf("%s. Error: no low-pass plan for index %d\n", what, idx);
         return false;
       }
       key.push_back(reinterpret_cast<intptr_t>(&plan));
@@ -1893,7 +1833,7 @@ class VideoFrameTransform {
         perPlane[p] = &lists[p ? 1 : 0];
         clear[p] = c.clear[p ? 1 : 0];
       }
-      c.merged = mergeable(plans, perPlane, clear, numPlanes, inW, inH);
+      c.merged = mergeable(plans, perPlane, clear, numPlanes, f.inW, f.inH);
       // one byte image of the jobs and one of the taps, with the provenance of every tap (tapSource; in a merged list it
       // carries the plane already)
       auto appendCodes = [&](const t360::BlurLists& l, const t360::BlurLayout& at, int plane) {
@@ -1918,11 +1858,11 @@ class VideoFrameTransform {
     const uint8_t* dTaps = stageUpload(slot.viewTaps, taps, s, &used[1]);
     t360::FrameStripParams fp{};
     for (int p = 0; p < numPlanes; ++p) {
-      const int bp = alignedPitch(inW[p]);
-      slot.lanes[p].blurred.reserve(static_cast<size_t>(bp) * inH[p] + 64);
+      const int bp = alignedPitch(f.inW[p]);
+      slot.lanes[p].blurred.reserve(static_cast<size_t>(bp) * f.inH[p] + 64);
       src[p] = slot.lanes[p].blurred.ptr;
       srcPitch[p] = bp;
-      fp.plane[p] = {dIn[p], slot.lanes[p].blurred.ptr, inW[p], inH[p], inPitch[p], bp};
+      fp.plane[p] = {f.in[p], slot.lanes[p].blurred.ptr, f.inW[p], f.inH[p], f.inPitch[p], bp};
     }
     if (c.merged) {
       launchLowPass(c.layout[0], false, dJobs, dTaps, fp, numPlanes, s);
@@ -1933,10 +1873,7 @@ class VideoFrameTransform {
         launchLowPass(c.layout[p ? 1 : 0], c.clear[p ? 1 : 0], dJobs, dTaps, one, 1, s);
       }
     }
-    for (UploadRing::Entry* e : used) {  // the entries may be refilled once these launches have finished
-      CU(cudaEventRecord(e->released, s));
-      e->inFlight = true;
-    }
+    for (UploadRing::Entry* e : used) releaseAfter(e, s);
     return true;
   }
 
@@ -2053,11 +1990,11 @@ class VideoFrameTransform {
 
   // Whether frame planes of these sizes can take the per-frame kernels (the planned input sizes; a missing plan index is
   // reported by the path that follows).
-  bool planesOfPlannedSize(int numPlanes, const int* inW, const int* inH) {
+  bool planesOfPlannedSize(const FramePlanes& f) {
     std::lock_guard<std::mutex> lock(mu_);
-    for (int p = 0; p < numPlanes; ++p) {
+    for (int p = 0; p < f.numPlanes; ++p) {
       auto it = plans_.find(p ? 1 : 0);
-      if (it != plans_.end() && (inW[p] != it->second.inW || inH[p] != it->second.inH)) return false;
+      if (it != plans_.end() && (f.inW[p] != it->second.inW || f.inH[p] != it->second.inH)) return false;
     }
     return true;
   }
@@ -2244,7 +2181,7 @@ class VideoFrameTransform {
       std::lock_guard<std::mutex> async(asyncMu_);
       return asyncSeq_ != seq || asyncSettled_ == seq || asyncStop_;  // (settled: T360B200_reconfigure took over)
     };
-    try {
+    return guarded(what, [&] {
       std::lock_guard<std::mutex> planLock(planMu_);
       if (superseded()) return true;
       const std::vector<PlanSizes> sizes = plannedSizes();
@@ -2269,13 +2206,7 @@ class VideoFrameTransform {
       install(set, next, seq, false);
       retire(set);
       return true;
-    } catch (const CudaFail& f) {
-      std::printf("%s. Error: CUDA %s (%s) in %s\n", what, cudaGetErrorName(f.err), cudaGetErrorString(f.err), f.what);
-      cudaGetLastError();
-    } catch (const std::exception& ex) {
-      std::printf("%s. Error: %s\n", what, ex.what());
-    }
-    return false;
+    });
   }
 
   // The per-frame kernels' sphere tables of the planes when no plan holds them (a pending reconfigureAsync, whose context
@@ -2560,18 +2491,14 @@ T360_API int T360B200_transformFramePlaneAsync(VideoFrameTransform* t, const uin
 T360_API int T360B200_transformFrameAsync(VideoFrameTransform* t, int numPlanes, const uint8_t* const* dIn, uint8_t* const* dOut,
                                           const int* inW, const int* inH, const int* inPitch, const int* outW, const int* outH,
                                           const int* outPitch, void* stream) {
-  if (!t || !dIn || !dOut || !inW || !inH || !inPitch || !outW || !outH || !outPitch) return 0;
-  return t->transformFrameDevice(numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, static_cast<cudaStream_t>(stream));
+  FramePlanes f;
+  if (!t || !describeFrame("Could not transform the frame", numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, f)) return 0;
+  return t->transformFrameDevice(f, static_cast<cudaStream_t>(stream));
 }
 T360_API int T360B200_lowPassPlaneAsync(VideoFrameTransform* t, const uint8_t* dIn, uint8_t* dOut, int w, int h, int inPitch,
                                         int outPitch, int planIndex, void* stream) {
   if (!t || !dIn || !dOut) return 0;
-  try {
-    return t->lowPassDevice(dIn, dOut, w, h, inPitch, outPitch, planIndex, static_cast<cudaStream_t>(stream));
-  } catch (const std::exception& ex) {
-    std::printf("Could not filter plane %d. Error: %s\n", planIndex, ex.what());
-    return 0;
-  }
+  return t->lowPassDevice(dIn, dOut, w, h, inPitch, outPitch, planIndex, static_cast<cudaStream_t>(stream));
 }
 T360_API int T360B200_reconfigure(VideoFrameTransform* t, const FrameTransformContext* ctx) {
   if (!t || !ctx) return 0;
@@ -2588,13 +2515,23 @@ T360_API int T360B200_reconfigureWait(VideoFrameTransform* t, int block) {
 T360_API int T360B200_transformFrameViewAsync(VideoFrameTransform* t, const T360View* view, int numPlanes, const uint8_t* const* dIn,
                                               uint8_t* const* dOut, const int* inW, const int* inH, const int* inPitch, const int* outW,
                                               const int* outH, const int* outPitch, void* stream) {
-  if (!t || !view || !dIn || !dOut || !inW || !inH || !inPitch || !outW || !outH || !outPitch) return 0;
-  const t360::FlatView v{view->yaw, view->pitch, view->hfov, view->vfov};
-  return t->transformFrameView(v, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, static_cast<cudaStream_t>(stream));
+  const char* what = "Could not transform the frame with a view";
+  FramePlanes f;
+  if (!t || !view || !describeFrame(what, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, f)) return 0;
+  return t->transformFrameWith(what, *view, f, static_cast<cudaStream_t>(stream));
 }
-// The sampling records of one plane of `ctx` as the per-frame kernels compute them, with the frame's view fields already in
-// ctx: FLAT_FIXED by flat_view.h, every other layout by oriented_view.h.  `what` names the call in the messages.
-static int perFrameSamples(const char* what, const FrameTransformContext& ctx, int inW, int inH, int outW, int outH, int32_t* samples) {
+// The sampling records of one plane of `ctx` with the frame's view fields `fields` (withFields) as the per-frame kernels
+// compute them: FLAT_FIXED by flat_view.h, every other layout by oriented_view.h.  `what` names the call in the messages.
+template <class Fields>
+static int perFrameSamples(const char* what, const FrameTransformContext* context, const Fields* fields, int inW, int inH, int outW, int outH,
+                           int32_t* samples) {
+  if (!context || !fields || !samples) return 0;
+  FrameTransformContext ctx = *context;
+  const std::string why = withFields(ctx, *fields);
+  if (!why.empty()) {
+    std::printf("Could not compute the %s's samples. Error: %s\n", what, why.c_str());
+    return 0;
+  }
   const int k = t360::kernelSizeOf(ctx.interpolation_alg);
   const int mapW = static_cast<int>(ctx.width_scale_factor * outW + 0.5), mapH = static_cast<int>(ctx.height_scale_factor * outH + 0.5);
   if (k == 0 || inW <= 0 || inH <= 0 || outW <= 0 || outH <= 0 || mapW <= 0 || mapH <= 0) {
@@ -2602,10 +2539,7 @@ static int perFrameSamples(const char* what, const FrameTransformContext& ctx, i
     return 0;
   }
   if (ctx.output_layout == LAYOUT_FLAT_FIXED) {
-    const bool stereoIn = ctx.input_stereo_format != STEREO_FORMAT_MONO;
-    const t360::FlatGeometry g{mapW, mapH, inW, inH, k, stereoIn && ctx.output_stereo_format == STEREO_FORMAT_LR,
-                               stereoIn && ctx.output_stereo_format == STEREO_FORMAT_TB, ctx.vflip != 0,
-                               ctx.input_stereo_format == STEREO_FORMAT_LR, ctx.input_stereo_format == STEREO_FORMAT_TB};
+    const t360::FlatGeometry g = t360::flatGeometry(ctx, mapW, mapH, inW, inH, k);
     const t360::FlatView v{ctx.fixed_yaw, ctx.fixed_pitch, ctx.fixed_hfov, ctx.fixed_vfov};
     for (int i = 0; i < mapH; ++i)
       for (int j = 0; j < mapW; ++j) {
@@ -2628,77 +2562,42 @@ static int perFrameSamples(const char* what, const FrameTransformContext& ctx, i
 }
 
 T360_API int T360B200_viewSamples(const FrameTransformContext* ctx, const T360View* view, int inW, int inH, int outW, int outH, int32_t* samples) {
-  if (!ctx || !view || !samples) return 0;
-  if (ctx->output_layout != LAYOUT_FLAT_FIXED) {
-    std::printf("Could not compute the view's samples. Error: output_layout %d is not FLAT_FIXED\n", static_cast<int>(ctx->output_layout));
-    return 0;
-  }
-  if (!std::isfinite(view->yaw) || !std::isfinite(view->pitch) || !std::isfinite(view->hfov) || !std::isfinite(view->vfov)) {
-    std::printf("Could not compute the view's samples. Error: the view is not finite\n");
-    return 0;
-  }
-  FrameTransformContext c = *ctx;
-  c.fixed_yaw = view->yaw;
-  c.fixed_pitch = view->pitch;
-  c.fixed_hfov = view->hfov;
-  c.fixed_vfov = view->vfov;
-  return perFrameSamples("view", c, inW, inH, outW, outH, samples);
+  return perFrameSamples("view", ctx, view, inW, inH, outW, outH, samples);
 }
 T360_API int T360B200_transformFrameOrientedAsync(VideoFrameTransform* t, const T360Orientation* orientation, int numPlanes,
                                                   const uint8_t* const* dIn, uint8_t* const* dOut, const int* inW, const int* inH,
                                                   const int* inPitch, const int* outW, const int* outH, const int* outPitch, void* stream) {
-  if (!t || !orientation || !dIn || !dOut || !inW || !inH || !inPitch || !outW || !outH || !outPitch) return 0;
-  const t360::Orientation o{orientation->yaw, orientation->pitch, orientation->roll};
-  return t->transformFrameOriented(o, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, static_cast<cudaStream_t>(stream));
+  const char* what = "Could not transform the frame with an orientation";
+  FramePlanes f;
+  if (!t || !orientation || !describeFrame(what, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, f)) return 0;
+  return t->transformFrameWith(what, *orientation, f, static_cast<cudaStream_t>(stream));
 }
 T360_API int T360B200_orientedSamples(const FrameTransformContext* ctx, const T360Orientation* orientation, int inW, int inH, int outW,
                                       int outH, int32_t* samples) {
-  if (!ctx || !orientation || !samples) return 0;
-  if (!t360::orientedLayouts(*ctx)) {
-    std::printf("Could not compute the orientation's samples. Error: layouts %d -> %d have no per-frame orientation\n",
-                static_cast<int>(ctx->input_layout), static_cast<int>(ctx->output_layout));
-    return 0;
-  }
-  if (!std::isfinite(orientation->yaw) || !std::isfinite(orientation->pitch) || !std::isfinite(orientation->roll)) {
-    std::printf("Could not compute the orientation's samples. Error: the orientation is not finite\n");
-    return 0;
-  }
-  FrameTransformContext c = *ctx;
-  c.fixed_yaw = orientation->yaw;
-  c.fixed_pitch = orientation->pitch;
-  c.fixed_roll = orientation->roll;
-  return perFrameSamples("orientation", c, inW, inH, outW, outH, samples);
+  return perFrameSamples("orientation", ctx, orientation, inW, inH, outW, outH, samples);
 }
 T360_API int T360B200_transformFramePoseAsync(VideoFrameTransform* t, const T360Pose* pose, int numPlanes, const uint8_t* const* dIn,
                                               uint8_t* const* dOut, const int* inW, const int* inH, const int* inPitch, const int* outW,
                                               const int* outH, const int* outPitch, void* stream) {
-  if (!t || !pose || !dIn || !dOut || !inW || !inH || !inPitch || !outW || !outH || !outPitch) return 0;
-  return t->transformFramePose(*pose, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, static_cast<cudaStream_t>(stream));
+  const char* what = "Could not transform the frame with a pose";
+  FramePlanes f;
+  if (!t || !pose || !describeFrame(what, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, f)) return 0;
+  return t->transformFrameWith(what, *pose, f, static_cast<cudaStream_t>(stream));
 }
 T360_API int T360B200_poseSamples(const FrameTransformContext* ctx, const T360Pose* pose, int inW, int inH, int outW, int outH, int32_t* samples) {
-  if (!ctx || !pose || !samples) return 0;
-  if (ctx->output_layout < 0 || ctx->output_layout >= LAYOUT_N) {
-    std::printf("Could not compute the pose's samples. Error: output_layout %d is not a layout\n", static_cast<int>(ctx->output_layout));
-    return 0;
-  }
-  if (!std::isfinite(pose->yaw) || !std::isfinite(pose->pitch) || !std::isfinite(pose->roll) || !std::isfinite(pose->hfov) ||
-      !std::isfinite(pose->vfov)) {
-    std::printf("Could not compute the pose's samples. Error: the pose is not finite\n");
-    return 0;
-  }
-  FrameTransformContext c = *ctx;
-  VideoFrameTransform::substitutePose(c, *pose);
-  return perFrameSamples("pose", c, inW, inH, outW, outH, samples);
+  return perFrameSamples("pose", ctx, pose, inW, inH, outW, outH, samples);
 }
 T360_API int T360B200_remapFrameAsync(VideoFrameTransform* t, int numPlanes, const float* const* maps, const int* mapPitches, int border,
                                       const uint8_t* const* dIn, uint8_t* const* dOut, const int* inW, const int* inH, const int* inPitch,
                                       const int* outW, const int* outH, const int* outPitch, void* stream) {
-  if (!t || !maps || !mapPitches || !dIn || !dOut || !inW || !inH || !inPitch || !outW || !outH || !outPitch) {
-    std::printf("Could not remap the frame. Error: a NULL argument\n");
+  const char* what = "Could not remap the frame";
+  if (!t || !maps || !mapPitches) {
+    std::printf("%s. Error: a NULL argument\n", what);
     return 0;
   }
-  return t->remapFrame(numPlanes, maps, mapPitches, border, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch,
-                       static_cast<cudaStream_t>(stream));
+  FramePlanes f;
+  if (!describeFrame(what, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, f)) return 0;
+  return t->remapFrame(maps, mapPitches, border, f, static_cast<cudaStream_t>(stream));
 }
 T360_API int T360B200_lensMap(const FrameTransformContext* ctx, const T360LensRig* rig, const T360Orientation* orientation, int inW, int inH,
                               int outW, int outH, float* map) {
@@ -2728,12 +2627,14 @@ T360_API int T360B200_lensMap(const FrameTransformContext* ctx, const T360LensRi
 T360_API int T360B200_transformFrameLensAsync(VideoFrameTransform* t, const T360LensRig* rig, const T360Orientation* orientation, int numPlanes,
                                               const uint8_t* const* dIn, uint8_t* const* dOut, const int* inW, const int* inH, const int* inPitch,
                                               const int* outW, const int* outH, const int* outPitch, void* stream) {
-  if (!t || !dIn || !dOut || !inW || !inH || !inPitch || !outW || !outH || !outPitch) {
-    std::printf("Could not transform the frame with a lens rig. Error: a NULL argument\n");
+  const char* what = "Could not transform the frame with a lens rig";
+  if (!t) {
+    std::printf("%s. Error: a NULL argument\n", what);
     return 0;
   }
-  return t->transformFrameLens(rig, orientation, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch,
-                               static_cast<cudaStream_t>(stream));
+  FramePlanes f;
+  if (!describeFrame(what, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, f)) return 0;
+  return t->transformFrameLens(rig, orientation, f, static_cast<cudaStream_t>(stream));
 }
 T360_API void T360B200_setPinHostPlanes(VideoFrameTransform* t, int enable) { if (t) t->setPinHostPlanes(enable != 0); }
 T360_API void T360B200_debugTrace(VideoFrameTransform* t, int enable) { if (t) t->enableTrace(enable != 0); }

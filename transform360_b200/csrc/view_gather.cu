@@ -19,6 +19,7 @@
 #include "gather_common.cuh"
 
 #include <algorithm>
+#include <type_traits>
 
 namespace t360 {
 namespace {
@@ -109,6 +110,7 @@ struct FlatPositions {
 // Sphere and barrel outputs: the whole chain per pixel, no shared tables
 template <bool BARREL>
 struct SpherePositions {
+  static constexpr int kTableBytes = 0;
   __device__ void beginTile(const OrientedGatherParams&, const OrientedPlane&, int, int) {}
   __device__ void beginColumn(int) {}
   __device__ void record(const OrientedGatherParams& p, const OrientedPlane& v, int, int, int i, int j, int* col0, int* rowPhase) const {
@@ -120,6 +122,7 @@ struct SpherePositions {
 // 256-byte load), quantised as quantizeWarpMap quantises a planned map, NaN, infinities and out-of-range values included
 template <int K>
 struct MapPositions {
+  static constexpr int kTableBytes = 0;
   __device__ void beginTile(const MapGatherParams&, const MapPlane&, int, int) {}
   __device__ void beginColumn(int) {}
   __device__ void record(const MapGatherParams&, const MapPlane& v, int, int, int i, int j, int* col0, int* rowPhase) const {
@@ -134,6 +137,7 @@ struct MapPositions {
 // A fisheye lens rig: the whole chain per pixel, no shared tables
 template <bool BARREL>
 struct LensPositions {
+  static constexpr int kTableBytes = 0;
   __device__ void beginTile(const LensGatherParams&, const OrientedPlane&, int, int) {}
   __device__ void beginColumn(int) {}
   __device__ void record(const LensGatherParams& p, const OrientedPlane& v, int, int, int i, int j, int* col0, int* rowPhase) const {
@@ -186,27 +190,13 @@ __global__ void __launch_bounds__(gatherThreads(K), K == 8 ? 1 : 4) lensGatherKe
   gatherViewTiles<K, true>(p, numTiles, smem, pos);
 }
 
-template <int K>
-cudaError_t launchViewK(const ViewGatherParams& p, int numTiles, int numSMs, cudaStream_t stream) {
+// Instantiation Kern of kernel size K, one CTA per tile up to the occupancy the __launch_bounds__ allow; its shared memory
+// is the weight table and the per-tile tables of its Positions
+template <int K, auto Kern, class Positions, class Params>
+cudaError_t launchPositionsK(const Params& p, int numTiles, int numSMs, cudaStream_t stream) {
   static DeviceLaunchCfg cfgs;  // per kernel instantiation, one entry per device
   constexpr int threads = gatherThreads(K);
-  constexpr int smemBytes = (K >= 2 ? weightBytes<K>() : 0) + FlatPositions<K>::kTableBytes;
-  LaunchCfg cfg;
-  cudaError_t err = prepare<viewGatherKernel<K>>(cfgs, threads, smemBytes, cfg);
-  if (err != cudaSuccess) return err;
-  const int grid = std::min(numSMs * cfg.perSM, numTiles);
-  viewGatherKernel<K><<<grid, threads, smemBytes, stream>>>(p, numTiles);
-  gLaunches.fetch_add(1, std::memory_order_relaxed);
-  return cudaGetLastError();
-}
-
-// The kernels whose only shared memory is the weight table (orientedGatherKernel, mapGatherKernel): instantiation Kern of
-// kernel size K, one CTA per tile up to the occupancy the __launch_bounds__ allow
-template <int K, auto Kern, class Params>
-cudaError_t launchPositionsK(const Params& p, int numTiles, int numSMs, cudaStream_t stream) {
-  static DeviceLaunchCfg cfgs;
-  constexpr int threads = gatherThreads(K);
-  constexpr int smemBytes = K >= 2 ? weightBytes<K>() : 0;
+  constexpr int smemBytes = (K >= 2 ? weightBytes<K>() : 0) + Positions::kTableBytes;
   LaunchCfg cfg;
   cudaError_t err = prepare<Kern>(cfgs, threads, smemBytes, cfg);
   if (err != cudaSuccess) return err;
@@ -214,19 +204,6 @@ cudaError_t launchPositionsK(const Params& p, int numTiles, int numSMs, cudaStre
   Kern<<<grid, threads, smemBytes, stream>>>(p, numTiles);
   gLaunches.fetch_add(1, std::memory_order_relaxed);
   return cudaGetLastError();
-}
-template <int K, bool TRANSPARENT>
-cudaError_t launchOrientedK(const OrientedGatherParams& p, int numTiles, int numSMs, cudaStream_t stream) {
-  return launchPositionsK<K, orientedGatherKernel<K, TRANSPARENT>>(p, numTiles, numSMs, stream);
-}
-template <int K, bool TRANSPARENT>
-cudaError_t launchMapK(const MapGatherParams& p, int numTiles, int numSMs, cudaStream_t stream) {
-  return launchPositionsK<K, mapGatherKernel<K, TRANSPARENT>>(p, numTiles, numSMs, stream);
-}
-
-template <int K, bool BARREL>
-cudaError_t launchLensK(const LensGatherParams& p, int numTiles, int numSMs, cudaStream_t stream) {
-  return launchPositionsK<K, lensGatherKernel<K, BARREL>>(p, numTiles, numSMs, stream);
 }
 
 // tiles of every plane, in plane order
@@ -243,61 +220,54 @@ int assignTiles(Params& p) {
   return numTiles;
 }
 
+// The tiles of every plane of p, in one launch of launch(K, FLAG, numTiles): K = p.kernelSize and FLAG = flag as
+// compile-time constants (std::integral_constant / std::bool_constant)
+template <class Params, class Launch>
+cudaError_t launchTiles(Params& p, bool flag, Launch&& launch) {
+  if (p.numPlanes < 1 || p.numPlanes > kMaxFramePlanes) return cudaErrorInvalidValue;
+  const int numTiles = assignTiles(p);
+  if (numTiles <= 0) return cudaSuccess;
+  auto withFlag = [&](auto k) { return flag ? launch(k, std::true_type{}, numTiles) : launch(k, std::false_type{}, numTiles); };
+  switch (p.kernelSize) {
+    case 1: return withFlag(std::integral_constant<int, 1>{});
+    case 2: return withFlag(std::integral_constant<int, 2>{});
+    case 4: return withFlag(std::integral_constant<int, 4>{});
+    case 8: return withFlag(std::integral_constant<int, 8>{});
+    default: return cudaErrorInvalidValue;
+  }
+}
+
 }  // namespace
 
 cudaError_t launchViewGather(ViewGatherParams p, int numSMs, cudaStream_t stream) {
-  if (p.numPlanes < 1 || p.numPlanes > kMaxFramePlanes) return cudaErrorInvalidValue;
-  const int numTiles = assignTiles(p);
-  if (numTiles <= 0) return cudaSuccess;
-  switch (p.kernelSize) {
-    case 1: return launchViewK<1>(p, numTiles, numSMs, stream);
-    case 2: return launchViewK<2>(p, numTiles, numSMs, stream);
-    case 4: return launchViewK<4>(p, numTiles, numSMs, stream);
-    case 8: return launchViewK<8>(p, numTiles, numSMs, stream);
-    default: return cudaErrorInvalidValue;
-  }
+  return launchTiles(p, false, [&](auto k, auto, int numTiles) {
+    constexpr int K = decltype(k)::value;
+    return launchPositionsK<K, viewGatherKernel<K>, FlatPositions<K>>(p, numTiles, numSMs, stream);
+  });
 }
 
+// (every plane of a frame has the same layout)
 cudaError_t launchOrientedGather(OrientedGatherParams p, int numSMs, cudaStream_t stream) {
-  if (p.numPlanes < 1 || p.numPlanes > kMaxFramePlanes) return cudaErrorInvalidValue;
-  const int numTiles = assignTiles(p);
-  if (numTiles <= 0) return cudaSuccess;
-  const bool barrel = barrelLayout(p.plane[0].geometry.outputLayout);  // (every plane of a frame has the same layout)
-  switch (p.kernelSize) {
-    case 1: return barrel ? launchOrientedK<1, true>(p, numTiles, numSMs, stream) : launchOrientedK<1, false>(p, numTiles, numSMs, stream);
-    case 2: return barrel ? launchOrientedK<2, true>(p, numTiles, numSMs, stream) : launchOrientedK<2, false>(p, numTiles, numSMs, stream);
-    case 4: return barrel ? launchOrientedK<4, true>(p, numTiles, numSMs, stream) : launchOrientedK<4, false>(p, numTiles, numSMs, stream);
-    case 8: return barrel ? launchOrientedK<8, true>(p, numTiles, numSMs, stream) : launchOrientedK<8, false>(p, numTiles, numSMs, stream);
-    default: return cudaErrorInvalidValue;
-  }
+  return launchTiles(p, barrelLayout(p.plane[0].geometry.outputLayout), [&](auto k, auto barrel, int numTiles) {
+    constexpr int K = decltype(k)::value;
+    constexpr bool B = decltype(barrel)::value;
+    return launchPositionsK<K, orientedGatherKernel<K, B>, SpherePositions<B>>(p, numTiles, numSMs, stream);
+  });
 }
 
 cudaError_t launchMapGather(MapGatherParams p, int numSMs, cudaStream_t stream) {
-  if (p.numPlanes < 1 || p.numPlanes > kMaxFramePlanes) return cudaErrorInvalidValue;
-  const int numTiles = assignTiles(p);
-  if (numTiles <= 0) return cudaSuccess;
-  const bool t = p.transparent;
-  switch (p.kernelSize) {
-    case 1: return t ? launchMapK<1, true>(p, numTiles, numSMs, stream) : launchMapK<1, false>(p, numTiles, numSMs, stream);
-    case 2: return t ? launchMapK<2, true>(p, numTiles, numSMs, stream) : launchMapK<2, false>(p, numTiles, numSMs, stream);
-    case 4: return t ? launchMapK<4, true>(p, numTiles, numSMs, stream) : launchMapK<4, false>(p, numTiles, numSMs, stream);
-    case 8: return t ? launchMapK<8, true>(p, numTiles, numSMs, stream) : launchMapK<8, false>(p, numTiles, numSMs, stream);
-    default: return cudaErrorInvalidValue;
-  }
+  return launchTiles(p, p.transparent, [&](auto k, auto transparent, int numTiles) {
+    constexpr int K = decltype(k)::value;
+    return launchPositionsK<K, mapGatherKernel<K, decltype(transparent)::value>, MapPositions<K>>(p, numTiles, numSMs, stream);
+  });
 }
 
 cudaError_t launchLensGather(LensGatherParams p, int numSMs, cudaStream_t stream) {
-  if (p.numPlanes < 1 || p.numPlanes > kMaxFramePlanes) return cudaErrorInvalidValue;
-  const int numTiles = assignTiles(p);
-  if (numTiles <= 0) return cudaSuccess;
-  const bool barrel = barrelLayout(p.plane[0].geometry.outputLayout);  // (every plane of a frame has the same layout)
-  switch (p.kernelSize) {
-    case 1: return barrel ? launchLensK<1, true>(p, numTiles, numSMs, stream) : launchLensK<1, false>(p, numTiles, numSMs, stream);
-    case 2: return barrel ? launchLensK<2, true>(p, numTiles, numSMs, stream) : launchLensK<2, false>(p, numTiles, numSMs, stream);
-    case 4: return barrel ? launchLensK<4, true>(p, numTiles, numSMs, stream) : launchLensK<4, false>(p, numTiles, numSMs, stream);
-    case 8: return barrel ? launchLensK<8, true>(p, numTiles, numSMs, stream) : launchLensK<8, false>(p, numTiles, numSMs, stream);
-    default: return cudaErrorInvalidValue;
-  }
+  return launchTiles(p, barrelLayout(p.plane[0].geometry.outputLayout), [&](auto k, auto barrel, int numTiles) {
+    constexpr int K = decltype(k)::value;
+    constexpr bool B = decltype(barrel)::value;
+    return launchPositionsK<K, lensGatherKernel<K, B>, LensPositions<B>>(p, numTiles, numSMs, stream);
+  });
 }
 
 }  // namespace t360

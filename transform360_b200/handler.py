@@ -33,6 +33,30 @@ def _warp_map(map) -> np.ndarray:
     return m
 
 
+def _frame_args(in_planes, out_planes, dims):
+    """The arguments of a whole-frame call after the transform: (number of planes, input and output plane arrays, the six
+    size and pitch arrays), and the ctypes arrays they point into, which must outlive the call."""
+    n = len(in_planes)
+    VP, IA = C.c_void_p * n, C.c_int * n
+    d_in = VP(*[p[0] for p in in_planes])
+    d_out = VP(*[p[0] for p in out_planes])
+    arrs = [IA(*[d[0] for d in dims]), IA(*[d[1] for d in dims]), IA(*[p[1] for p in in_planes]),
+            IA(*[d[2] for d in dims]), IA(*[d[3] for d in dims]), IA(*[p[1] for p in out_planes])]
+    ptrs = [C.cast(a, C.c_void_p) for a in arrs]
+    return n, C.cast(d_in, C.c_void_p), C.cast(d_out, C.c_void_p), ptrs, (d_in, d_out, arrs)
+
+
+def _samples(fn, ctx, fields, in_w, in_h, out_w, out_h) -> np.ndarray:
+    """int32 [map_h][map_w][2] sampling records from fn(ctx, fields, in_w, in_h, out_w, out_h, out), a T360B200_*Samples
+    call; ValueError when it refuses the arguments."""
+    scaled = lambda f, n: int(float(np.float32(f) * np.float32(n)) + 0.5)  # (float product, double sum: buildHostPlan)
+    map_w, map_h = scaled(ctx.width_scale_factor, out_w), scaled(ctx.height_scale_factor, out_h)
+    out = np.zeros((max(map_h, 0), max(map_w, 0), 2), np.int32)
+    if not fn(C.byref(ctx), C.byref(fields), in_w, in_h, out_w, out_h, out.ctypes.data):
+        raise ValueError(f"{fn.__name__} refused the arguments (message on stdout)")
+    return out
+
+
 class FrameTransformContext(C.Structure):
     """28 x 4 bytes, field for field the reference's struct (VideoFrameTransformHelper.h:56-90)."""
     _fields_ = [
@@ -290,34 +314,20 @@ class VideoFrameTransform:
         """Prebuilds the argument arrays of T360B200_transformFrameAsync for one (input frame, output frame) pair.
         in_planes / out_planes: per plane (device_address, pitch); dims: per plane (in_w, in_h, out_w, out_h).
         Returns a callable f(stream) -> bool that enqueues the whole frame."""
-        n = len(in_planes)
-        VP, IA = C.c_void_p * n, C.c_int * n
-        d_in = VP(*[p[0] for p in in_planes])
-        d_out = VP(*[p[0] for p in out_planes])
-        arrs = [IA(*[d[0] for d in dims]), IA(*[d[1] for d in dims]), IA(*[p[1] for p in in_planes]),
-                IA(*[d[2] for d in dims]), IA(*[d[3] for d in dims]), IA(*[p[1] for p in out_planes])]
+        n, pin, pout, ptrs, keep = _frame_args(in_planes, out_planes, dims)
         fn, h = self._lib.T360B200_transformFrameAsync, self._h
-        ptrs = [C.cast(a, C.c_void_p) for a in arrs]
-        pin, pout = C.cast(d_in, C.c_void_p), C.cast(d_out, C.c_void_p)
 
-        def call(stream: int = 0, _keep=(d_in, d_out, arrs)) -> bool:
+        def call(stream: int = 0, _keep=keep) -> bool:
             return bool(fn(h, n, pin, pout, *ptrs, stream))
         return call
 
     def make_view_frame_call(self, in_planes, out_planes, dims):
         """Like make_frame_call, for T360B200_transformFrameViewAsync (FLAT_FIXED transforms): returns a callable
         f(view, stream) -> bool that enqueues the whole frame with `view` (a T360View or (yaw, pitch, hfov, vfov))."""
-        n = len(in_planes)
-        VP, IA = C.c_void_p * n, C.c_int * n
-        d_in = VP(*[p[0] for p in in_planes])
-        d_out = VP(*[p[0] for p in out_planes])
-        arrs = [IA(*[d[0] for d in dims]), IA(*[d[1] for d in dims]), IA(*[p[1] for p in in_planes]),
-                IA(*[d[2] for d in dims]), IA(*[d[3] for d in dims]), IA(*[p[1] for p in out_planes])]
+        n, pin, pout, ptrs, keep = _frame_args(in_planes, out_planes, dims)
         fn, h = self._lib.T360B200_transformFrameViewAsync, self._h
-        ptrs = [C.cast(a, C.c_void_p) for a in arrs]
-        pin, pout = C.cast(d_in, C.c_void_p), C.cast(d_out, C.c_void_p)
 
-        def call(view, stream: int = 0, _keep=(d_in, d_out, arrs)) -> bool:
+        def call(view, stream: int = 0, _keep=keep) -> bool:
             return bool(fn(h, C.byref(as_view(view)), n, pin, pout, *ptrs, stream))
         return call
 
@@ -325,34 +335,20 @@ class VideoFrameTransform:
         """Like make_frame_call, for T360B200_transformFrameOrientedAsync (cube-map, EAC and equirect outputs): returns a
         callable f(orientation, stream) -> bool that enqueues the whole frame with `orientation` (a T360Orientation or
         (yaw, pitch, roll))."""
-        n = len(in_planes)
-        VP, IA = C.c_void_p * n, C.c_int * n
-        d_in = VP(*[p[0] for p in in_planes])
-        d_out = VP(*[p[0] for p in out_planes])
-        arrs = [IA(*[d[0] for d in dims]), IA(*[d[1] for d in dims]), IA(*[p[1] for p in in_planes]),
-                IA(*[d[2] for d in dims]), IA(*[d[3] for d in dims]), IA(*[p[1] for p in out_planes])]
+        n, pin, pout, ptrs, keep = _frame_args(in_planes, out_planes, dims)
         fn, h = self._lib.T360B200_transformFrameOrientedAsync, self._h
-        ptrs = [C.cast(a, C.c_void_p) for a in arrs]
-        pin, pout = C.cast(d_in, C.c_void_p), C.cast(d_out, C.c_void_p)
 
-        def call(orientation, stream: int = 0, _keep=(d_in, d_out, arrs)) -> bool:
+        def call(orientation, stream: int = 0, _keep=keep) -> bool:
             return bool(fn(h, C.byref(as_orientation(orientation)), n, pin, pout, *ptrs, stream))
         return call
 
     def make_pose_frame_call(self, in_planes, out_planes, dims):
         """Like make_frame_call, for T360B200_transformFramePoseAsync (every output layout): returns a callable
         f(pose, stream) -> bool that enqueues the whole frame with `pose` (a T360Pose or (yaw, pitch, roll, hfov, vfov))."""
-        n = len(in_planes)
-        VP, IA = C.c_void_p * n, C.c_int * n
-        d_in = VP(*[p[0] for p in in_planes])
-        d_out = VP(*[p[0] for p in out_planes])
-        arrs = [IA(*[d[0] for d in dims]), IA(*[d[1] for d in dims]), IA(*[p[1] for p in in_planes]),
-                IA(*[d[2] for d in dims]), IA(*[d[3] for d in dims]), IA(*[p[1] for p in out_planes])]
+        n, pin, pout, ptrs, keep = _frame_args(in_planes, out_planes, dims)
         fn, h = self._lib.T360B200_transformFramePoseAsync, self._h
-        ptrs = [C.cast(a, C.c_void_p) for a in arrs]
-        pin, pout = C.cast(d_in, C.c_void_p), C.cast(d_out, C.c_void_p)
 
-        def call(pose, stream: int = 0, _keep=(d_in, d_out, arrs)) -> bool:
+        def call(pose, stream: int = 0, _keep=keep) -> bool:
             return bool(fn(h, C.byref(as_pose(pose)), n, pin, pout, *ptrs, stream))
         return call
 
@@ -360,17 +356,10 @@ class VideoFrameTransform:
         """Like make_frame_call, for T360B200_transformFrameLensAsync (a fisheye lens rig to any sphere output, no plan
         needed): returns a callable f(rig, orientation, stream) -> bool that enqueues the whole frame with `rig` (a
         T360LensRig) and `orientation` (a T360Orientation or (yaw, pitch, roll))."""
-        n = len(in_planes)
-        VP, IA = C.c_void_p * n, C.c_int * n
-        d_in = VP(*[p[0] for p in in_planes])
-        d_out = VP(*[p[0] for p in out_planes])
-        arrs = [IA(*[d[0] for d in dims]), IA(*[d[1] for d in dims]), IA(*[p[1] for p in in_planes]),
-                IA(*[d[2] for d in dims]), IA(*[d[3] for d in dims]), IA(*[p[1] for p in out_planes])]
+        n, pin, pout, ptrs, keep = _frame_args(in_planes, out_planes, dims)
         fn, h = self._lib.T360B200_transformFrameLensAsync, self._h
-        ptrs = [C.cast(a, C.c_void_p) for a in arrs]
-        pin, pout = C.cast(d_in, C.c_void_p), C.cast(d_out, C.c_void_p)
 
-        def call(rig, orientation, stream: int = 0, _keep=(d_in, d_out, arrs)) -> bool:
+        def call(rig, orientation, stream: int = 0, _keep=keep) -> bool:
             return bool(fn(h, C.byref(rig), C.byref(as_orientation(orientation)), n, pin, pout, *ptrs, stream))
         return call
 
@@ -388,15 +377,8 @@ class VideoFrameTransform:
         frame through one device map per plane, each the size of its output plane.  maps: per plane a CUDA float32 tensor
         [out_h][>= out_w][2] (its row stride gives the pitch), a (device address, pitch in bytes) pair, or a device address
         of a dense map."""
-        n = len(in_planes)
-        VP, IA = C.c_void_p * n, C.c_int * n
-        d_in = VP(*[p[0] for p in in_planes])
-        d_out = VP(*[p[0] for p in out_planes])
-        arrs = [IA(*[d[0] for d in dims]), IA(*[d[1] for d in dims]), IA(*[p[1] for p in in_planes]),
-                IA(*[d[2] for d in dims]), IA(*[d[3] for d in dims]), IA(*[p[1] for p in out_planes])]
+        n, pin, pout, ptrs, keep = _frame_args(in_planes, out_planes, dims)
         fn, h = self._lib.T360B200_remapFrameAsync, self._h
-        ptrs = [C.cast(a, C.c_void_p) for a in arrs]
-        pin, pout = C.cast(d_in, C.c_void_p), C.cast(d_out, C.c_void_p)
         dense = [8 * d[2] for d in dims]
 
         def as_map(m, p):
@@ -404,11 +386,11 @@ class VideoFrameTransform:
                 return m.data_ptr(), m.stride(0) * m.element_size()
             return (int(m[0]), int(m[1])) if isinstance(m, (tuple, list)) else (int(m), dense[p])
 
-        def call(maps, stream: int = 0, _keep=(d_in, d_out, arrs)) -> bool:
+        def call(maps, stream: int = 0, _keep=keep) -> bool:
             if len(maps) != n:
                 raise ValueError(f"{len(maps)} maps for {n} planes")
             desc = [as_map(m, p) for p, m in enumerate(maps)]
-            dmaps, pitches = VP(*[d[0] for d in desc]), IA(*[d[1] for d in desc])
+            dmaps, pitches = (C.c_void_p * n)(*[d[0] for d in desc]), (C.c_int * n)(*[d[1] for d in desc])
             return bool(fn(h, n, dmaps, pitches, border, pin, pout, *ptrs, stream))
         return call
 
@@ -575,35 +557,19 @@ class HostPlan:
 def view_samples(ctx: FrameTransformContext, view, in_w, in_h, out_w, out_h) -> np.ndarray:
     """The sampling records the per-view kernel computes for one plane (T360B200_viewSamples, no CUDA):
     int32 [map_h][map_w][2] like HostPlan.samples."""
-    scaled = lambda f, n: int(float(np.float32(f) * np.float32(n)) + 0.5)  # (float product, double sum: buildHostPlan)
-    map_w, map_h = scaled(ctx.width_scale_factor, out_w), scaled(ctx.height_scale_factor, out_h)
-    out = np.zeros((max(map_h, 0), max(map_w, 0), 2), np.int32)
-    if not load().T360B200_viewSamples(C.byref(ctx), C.byref(as_view(view)), in_w, in_h, out_w, out_h, out.ctypes.data):
-        raise ValueError("T360B200_viewSamples refused the arguments (message on stdout)")
-    return out
+    return _samples(load().T360B200_viewSamples, ctx, as_view(view), in_w, in_h, out_w, out_h)
 
 
 def oriented_samples(ctx: FrameTransformContext, orientation, in_w, in_h, out_w, out_h) -> np.ndarray:
     """The sampling records the per-frame orientation kernel computes for one plane (T360B200_orientedSamples, no CUDA):
     int32 [map_h][map_w][2] like HostPlan.samples."""
-    scaled = lambda f, n: int(float(np.float32(f) * np.float32(n)) + 0.5)  # (float product, double sum: buildHostPlan)
-    map_w, map_h = scaled(ctx.width_scale_factor, out_w), scaled(ctx.height_scale_factor, out_h)
-    out = np.zeros((max(map_h, 0), max(map_w, 0), 2), np.int32)
-    if not load().T360B200_orientedSamples(C.byref(ctx), C.byref(as_orientation(orientation)), in_w, in_h, out_w, out_h,
-                                           out.ctypes.data):
-        raise ValueError("T360B200_orientedSamples refused the arguments (message on stdout)")
-    return out
+    return _samples(load().T360B200_orientedSamples, ctx, as_orientation(orientation), in_w, in_h, out_w, out_h)
 
 
 def pose_samples(ctx: FrameTransformContext, pose, in_w, in_h, out_w, out_h) -> np.ndarray:
     """The sampling records the per-frame kernels compute for one plane with `pose` (T360B200_poseSamples, no CUDA):
     int32 [map_h][map_w][2] like HostPlan.samples."""
-    scaled = lambda f, n: int(float(np.float32(f) * np.float32(n)) + 0.5)  # (float product, double sum: buildHostPlan)
-    map_w, map_h = scaled(ctx.width_scale_factor, out_w), scaled(ctx.height_scale_factor, out_h)
-    out = np.zeros((max(map_h, 0), max(map_w, 0), 2), np.int32)
-    if not load().T360B200_poseSamples(C.byref(ctx), C.byref(as_pose(pose)), in_w, in_h, out_w, out_h, out.ctypes.data):
-        raise ValueError("T360B200_poseSamples refused the arguments (message on stdout)")
-    return out
+    return _samples(load().T360B200_poseSamples, ctx, as_pose(pose), in_w, in_h, out_w, out_h)
 
 
 def lens_map(ctx: FrameTransformContext, rig: T360LensRig, orientation, in_w, in_h, out_w, out_h) -> np.ndarray:

@@ -117,37 +117,36 @@ class FrameTransformer:
     def close(self):
         self.vft.close()
 
+    def _dims(self):
+        """(in_w, in_h, out_w, out_h) of every plane, as the frame calls take them."""
+        return [self.spec.plane_dims(p)[:4] for p in range(self.spec.num_planes)]
+
     def frame_call(self, in_planes, out_planes):
         """Prebuilt whole-frame call (T360B200_transformFrameAsync) for one (input, output) buffer pair:
         in_planes / out_planes are per plane (device_address, pitch).  Returns f(stream) -> bool."""
-        dims = [self.spec.plane_dims(p)[:4] for p in range(self.spec.num_planes)]
-        return self.vft.make_frame_call(in_planes, out_planes, dims)
+        return self.vft.make_frame_call(in_planes, out_planes, self._dims())
 
     def view_frame_call(self, in_planes, out_planes):
         """Prebuilt whole-frame call with a per-frame view (T360B200_transformFrameViewAsync, FLAT_FIXED contexts) for one
         (input, output) buffer pair.  Returns f(view, stream) -> bool; view: T360View or (yaw, pitch, hfov, vfov)."""
-        dims = [self.spec.plane_dims(p)[:4] for p in range(self.spec.num_planes)]
-        return self.vft.make_view_frame_call(in_planes, out_planes, dims)
+        return self.vft.make_view_frame_call(in_planes, out_planes, self._dims())
 
     def oriented_frame_call(self, in_planes, out_planes):
         """Prebuilt whole-frame call with a per-frame orientation (T360B200_transformFrameOrientedAsync: cube-map, EAC and
         equirect outputs) for one (input, output) buffer pair.  Returns f(orientation, stream) -> bool; orientation:
         T360Orientation or (yaw, pitch, roll)."""
-        dims = [self.spec.plane_dims(p)[:4] for p in range(self.spec.num_planes)]
-        return self.vft.make_oriented_frame_call(in_planes, out_planes, dims)
+        return self.vft.make_oriented_frame_call(in_planes, out_planes, self._dims())
 
     def pose_frame_call(self, in_planes, out_planes):
         """Prebuilt whole-frame call with a per-frame pose (T360B200_transformFramePoseAsync: every output layout) for one
         (input, output) buffer pair.  Returns f(pose, stream) -> bool; pose: T360Pose or (yaw, pitch, roll, hfov, vfov)."""
-        dims = [self.spec.plane_dims(p)[:4] for p in range(self.spec.num_planes)]
-        return self.vft.make_pose_frame_call(in_planes, out_planes, dims)
+        return self.vft.make_pose_frame_call(in_planes, out_planes, self._dims())
 
     def remap_frame_call(self, in_planes, out_planes, border: int = H.BORDER_WRAP):
         """Prebuilt whole-frame call through per-frame warp maps (T360B200_remapFrameAsync: one device map per plane, the size
         of its output plane) for one (input, output) buffer pair.  Returns f(maps, stream) -> bool; maps: per plane a CUDA
         float32 tensor [out_h][out_w][2], a (device address, pitch) pair or the device address of a dense map."""
-        dims = [self.spec.plane_dims(p)[:4] for p in range(self.spec.num_planes)]
-        return self.vft.make_remap_frame_call(in_planes, out_planes, dims, border)
+        return self.vft.make_remap_frame_call(in_planes, out_planes, self._dims(), border)
 
     def transform_frame_device(self, in_planes, out_planes, stream: int = 0):
         """in_planes / out_planes: per plane (device_address, pitch).  Asynchronous on `stream`; the planes of
