@@ -55,6 +55,12 @@ int T360B200_hostPlanGather(T360HostPlan* plan, int info[10], const int32_t** jo
  * Returns 1 on success; the pointers stay valid until T360B200_hostPlanDestroy. */
 int T360B200_hostPlanPoleCaps(T360HostPlan* plan, int info[4], const int32_t** capJobs, const uint32_t** capRecords,
                               const int32_t** launchJobs);
+/* The job list and record buffer the frame kernel reads (csrc/gather_plan.h: deviceJobs, deviceRecords): the launch list
+ * of T360B200_hostPlanPoleCaps with the width of each class-0 source box (csrc/kernels.cuh: class0BoxW) in bits 28-31
+ * of recordOffset, and the compact records followed by the pole-cap records, the window offsets of a job with a narrow
+ * box at that box's pitch.  info = {jobs, words of records}.  Returns 1 on success; the pointers stay valid until
+ * T360B200_hostPlanDestroy. */
+int T360B200_hostPlanDeviceLists(T360HostPlan* plan, int info[2], const int32_t** jobs, const uint32_t** records);
 /* How the host deals the n <= 32 pixels of one warp step to lanes and copies of the weight table (csrc/gather_plan.h:
  * dealLanes): phases[i] = (fracY32 << 5) | fracX32 of pixel i; laneOf[i] / copyOf[i] receive its lane and table copy.
  * Returns the modelled shared-memory wavefronts of one 128-bit weight load of the warp (0 when n < 32: identity deal). */

@@ -303,8 +303,9 @@ __device__ __forceinline__ void computeBorderJob(const PlaneView& pv, uint32_t r
   }
 }
 
+template <int K>
 struct FrameTensorMaps {
-  CUtensorMap map[kMaxFramePlanes][kNumBoxClasses][kBoxVariants];
+  CUtensorMap map[kMaxFramePlanes][boxMaps(K)];  // (only the box shapes of kernel size K: fewer kernel-parameter bytes)
 };
 
 __device__ __forceinline__ void mbarArrive(uint64_t* bar) {
@@ -338,7 +339,7 @@ struct FrameLayout {
 
 template <int K, int COPIES, int GROUPS>
 __global__ void __launch_bounds__(GROUPS * (kGroupWarps + 1) * 32, 1)
-gatherFrameKernel(const __grid_constant__ FrameGatherParams p, StagedParams jobs, const __grid_constant__ FrameTensorMaps maps) {
+gatherFrameKernel(const __grid_constant__ FrameGatherParams p, StagedParams jobs, const __grid_constant__ FrameTensorMaps<K> maps) {
   using L = FrameLayout<K, COPIES, GROUPS>;
   constexpr int VS = weightVectorStride(K, COPIES), kStage = L::kStage, kRec = L::kRec, S = L::kStages;
   constexpr uint32_t kBox0 = stageBoxW(K, 0) * stageBoxH(K, 0), kBox1 = stageBoxW(K, 1) * stageBoxH(K, 1),
@@ -442,15 +443,17 @@ gatherFrameKernel(const __grid_constant__ FrameGatherParams p, StagedParams jobs
           if (kind == kJobBorder) {  // records only: its taps are read through L1
             mbarExpectTx(full + st, recBytes);
           } else {
-            // the source box: the lowest variant of its class that holds the rows the job's windows span (kernels.cuh)
+            // the source box: the lowest variant of its class that holds the rows the job's windows span, for a class-0
+            // job also the narrowest width that holds its columns (kernels.cuh)
             const int cls = boxClassOf(kind), variant = jobBoxVariant(h.z), boxX = jobBoxX(h.z), boxY = jobBoxY(h.z);
-            const uint32_t boxBytes = (uint32_t)(stageBoxW(K, cls) * boxVariantRows(K, cls, variant));
+            const int width = (int)((unsigned)h.w >> kJobWidthShift);
+            const uint32_t boxBytes = (uint32_t)((cls == 0 ? class0BoxW(width) : stageBoxW(K, cls)) * boxVariantRows(K, cls, variant));
             mbarExpectTx(full + st, (kind == kJobSeam ? 2 : 1) * boxBytes + recBytes);
-            tmaLoadBox(groupBase + st * kStage, &maps.map[pl][cls][variant], boxX, boxY, full + st);
+            tmaLoadBox(groupBase + st * kStage, &maps.map[pl][boxMapIndex(K, cls, width, variant)], boxX, boxY, full + st);
             if (kind == kJobSeam)  // the part of the window beyond the right border, from the left of the plane
-              tmaLoadBox(groupBase + (st + 1) * kStage, &maps.map[pl][0][variant], boxX - planes[pl].srcW, boxY, full + st);
+              tmaLoadBox(groupBase + (st + 1) * kStage, &maps.map[pl][boxMapIndex(K, 0, 0, variant)], boxX - planes[pl].srcW, boxY, full + st);
           }
-          bulkCopyToShared(rec + 128, planes[pl].records + (unsigned)h.w, recBytes, full + st);
+          bulkCopyToShared(rec + 128, planes[pl].records + ((unsigned)h.w & kJobRecordMask), recBytes, full + st);
         }
       }
       advance();
@@ -517,7 +520,11 @@ gatherFrameKernel(const __grid_constant__ FrameGatherParams p, StagedParams jobs
           if (quad & 1) { r.z = v.x; r.w = v.y; } else { r.x = v.x; r.y = v.y; }
         }
       }
-      computeTileJob<K, stageBoxW(K, 0), VS>(pv, boxAddr + st * kStage, outX, outY, r, wAddr, warp);
+      const int width = (int)(h.w >> kJobWidthShift);  // the pitch of its box: one instantiation per width
+      staticFor<class0Widths(K)>([&](auto W) {
+        constexpr int w = decltype(W)::value;
+        if (width == w) computeTileJob<K, class0BoxW(w), VS>(pv, boxAddr + st * kStage, outX, outY, r, wAddr, warp);
+      });
     } else if (kind == kJobClass1) {
       computeTileJob<K, stageBoxW(K, 1), VS>(pv, boxAddr + st * kStage, outX, outY, ldsVec(rec + 128 + warp * 512 + lane * 16), wAddr, warp);
     } else if (kind == kJobSeam) {
@@ -559,8 +566,12 @@ cudaError_t prepareFrameK(LaunchCfg& cfg) {
 }
 
 template <int K, int COPIES, int GROUPS>
-cudaError_t launchFrameK(const FrameGatherParams& p, const StagedParams& jobs, const FrameTensorMaps& maps, int numSMs,
+cudaError_t launchFrameK(const FrameGatherParams& p, const StagedParams& jobs, const void* tensorMaps, int numSMs,
                          cudaStream_t stream, bool programmatic) {
+  FrameTensorMaps<K> maps;
+  for (int i = 0; i < kMaxFramePlanes; ++i)  // unused planes: valid descriptors that no job refers to
+    std::memcpy(maps.map[i], static_cast<const CUtensorMap*>(tensorMaps) + (size_t)(i < p.numPlanes ? i : 0) * kMaxBoxMaps,
+                sizeof(maps.map[i]));
   constexpr int threads = GROUPS * (kGroupWarps + 1) * 32, smemBytes = FrameLayout<K, COPIES, GROUPS>::kTotal;
   LaunchCfg cfg;
   cudaError_t err = prepareFrameK<K, COPIES, GROUPS>(cfg);
@@ -597,15 +608,10 @@ cudaError_t launchGatherFrame(const FrameGatherParams& p, const StagedParams& jo
                               cudaStream_t stream, bool programmatic) {
   if (jobs.numTiles <= 0) return cudaSuccess;
   if (p.numPlanes < 1 || p.numPlanes > kMaxFramePlanes) return cudaErrorInvalidValue;
-  FrameTensorMaps maps;
-  std::memcpy(&maps, tensorMaps, sizeof(CUtensorMap) * kNumBoxClasses * kBoxVariants * p.numPlanes);
-  for (int i = p.numPlanes; i < kMaxFramePlanes; ++i)  // unused entries: valid descriptors that no job refers to
-    for (int c = 0; c < kNumBoxClasses; ++c)
-      for (int v = 0; v < kBoxVariants; ++v) maps.map[i][c][v] = maps.map[0][c][v];
   switch (p.kernelSize) {
-    case 2: return launchFrameK<2, weightCopies(2), gatherGroups(2)>(p, jobs, maps, numSMs, stream, programmatic);
-    case 4: return launchFrameK<4, weightCopies(4), gatherGroups(4)>(p, jobs, maps, numSMs, stream, programmatic);
-    case 8: return launchFrameK<8, weightCopies(8), gatherGroups(8)>(p, jobs, maps, numSMs, stream, programmatic);
+    case 2: return launchFrameK<2, weightCopies(2), gatherGroups(2)>(p, jobs, tensorMaps, numSMs, stream, programmatic);
+    case 4: return launchFrameK<4, weightCopies(4), gatherGroups(4)>(p, jobs, tensorMaps, numSMs, stream, programmatic);
+    case 8: return launchFrameK<8, weightCopies(8), gatherGroups(8)>(p, jobs, tensorMaps, numSMs, stream, programmatic);
     default: return cudaErrorInvalidValue;
   }
 }

@@ -660,6 +660,7 @@ void buildGatherPlan(const HostPlan& h, bool stageTiles, GatherPlan& g) {
   g.compact.assign(offset / 4, 0u);
   std::vector<int> needRows(g.jobs.size(), h.inH);
   std::vector<JobRect> rects(g.jobs.size());
+  std::vector<uint8_t> widths(g.jobs.size(), 0);
   parallelRanges(static_cast<int>(g.jobs.size()), 2048, [&](int begin, int end) {
     for (int i = begin; i < end; ++i) {
       const GatherJob& job = g.jobs[i];
@@ -672,6 +673,7 @@ void buildGatherPlan(const HostPlan& h, bool stageTiles, GatherPlan& g) {
       // the source rows the job reads: what a caller that streams the plane in must have delivered before it runs
       const Extent e = extentOf(h, r.x0, r.y0, r.x1, r.y1);
       if (e.minR >= 0 && e.maxR + k <= h.inH) needRows[i] = e.maxR + k;
+      if (kind == kJobClass0) widths[i] = static_cast<uint8_t>(class0WidthFor(k, e.maxC + k - jobBoxX(job.boxXY)));
       uint32_t* out = g.compact.data() + static_cast<size_t>(job.recordOffset) * 4;
       if (boxClassOf(kind) == 2) writeShareRecords(h, job, out);
       else writeTileRecords(h, job, out);
@@ -701,7 +703,33 @@ void buildGatherPlan(const HostPlan& h, bool stageTiles, GatherPlan& g) {
     g.launchJobs.push_back(jobOf(i));
     g.launchNeedRows.push_back(i >= 0 ? needRows[i] : pixelJobs[-1 - i].needRows);
     g.launchRects.push_back(i >= 0 ? rects[i] : pixelJobs[-1 - i].rect);
+    g.launchBoxWidths.push_back(i >= 0 ? widths[i] : 0);
   }
+  if (offset / 16 > static_cast<size_t>(kJobRecordMask)) throw std::invalid_argument("gather plan: too many sampling records");
+}
+
+std::vector<GatherJob> deviceJobs(const GatherPlan& g) {
+  std::vector<GatherJob> out(g.launchJobs);
+  for (size_t i = 0; i < out.size(); ++i) out[i].recordOffset |= static_cast<int>(g.launchBoxWidths[i]) << kJobWidthShift;
+  return out;
+}
+
+std::vector<uint32_t> deviceRecords(const GatherPlan& g, int k) {
+  std::vector<uint32_t> out(g.compact);
+  out.insert(out.end(), g.capRecords.begin(), g.capRecords.end());
+  const int wide = stageBoxW(k, 0);
+  for (size_t i = 0; i < g.launchJobs.size(); ++i) {
+    if (g.launchBoxWidths[i] == 0) continue;
+    const GatherJob& job = g.launchJobs[i];
+    const uint32_t narrow = static_cast<uint32_t>(class0BoxW(g.launchBoxWidths[i]));
+    uint32_t* w = out.data() + static_cast<size_t>(job.recordOffset) * 4;
+    for (int j = 0; j < jobRecordBytes(k, kJobClass0, job.outX) / 4; ++j) {
+      if (w[j] & kRecordSkip) continue;
+      const uint32_t off = w[j] & 0x7fffu;
+      w[j] = (w[j] & ~0x7fffu) | (off / wide * narrow + off % wide);
+    }
+  }
+  return out;
 }
 
 }  // namespace t360

@@ -32,6 +32,10 @@ struct GatherPlan {
   std::vector<GatherJob> launchJobs;
   std::vector<int> launchNeedRows;
   std::vector<JobRect> launchRects;
+  // per launch job the width of its class-0 box (kernels.cuh: class0BoxW; 0 for every other kind), which the device's
+  // copy of the list carries in GatherJob::recordOffset (deviceJobs) and the device's records in their pitch
+  // (deviceRecords)
+  std::vector<uint8_t> launchBoxWidths;
   int numStaged[2] = {}, numSeam = 0, numGeneral = 0, numShare = 0, numCap = 0, numBorder = 0;
   int totalStaged() const { return numSeam + numShare + numStaged[0] + numStaged[1] + numCap; }
 };
@@ -39,6 +43,12 @@ struct GatherPlan {
 // stageTiles: cut the plane into jobs for the persistent kernel (kernel size >= 2 and BORDER_WRAP); otherwise only the
 // full records are produced (nearest neighbour, barrel layouts: whole-plane general kernels).
 void buildGatherPlan(const HostPlan& h, bool stageTiles, GatherPlan& g);
+
+// The job list the frame kernel claims from: launchJobs with each class-0 box width in the top bits of recordOffset.
+std::vector<GatherJob> deviceJobs(const GatherPlan& g);
+// The record buffer the frame kernel reads: compact ++ capRecords, with the window offsets of a job that loads a narrow
+// class-0 box at that box's pitch instead of the stage buffer's 208 bytes (kernels.cuh: class0BoxW).
+std::vector<uint32_t> deviceRecords(const GatherPlan& g, int k);
 
 // Launch order of the jobs: border (latency-bound reads through L1, few; in the tile list: the general tiles), seam and class 1 (both need the two stage
 // buffers of a group), pole caps, share jobs, and finally the small class-0 tiles through the double-buffered TMA

@@ -36,7 +36,8 @@ struct GatherParams {
 struct GatherJob {
   int outX, outY;    // outY carries the job kind (kJobKindShift) and the image plane (kJobPlaneShift)
   int boxXY;         // boxX | boxY << 16 | box variant: boxX % 16 == 0, its low four bits name the tensor map (box height)
-  int recordOffset;  // of the job's compact records, in 16-byte units from the plane's record buffer
+  int recordOffset;  // of the job's compact records, in 16-byte units from the plane's record buffer; in the device's
+                     // list bits kJobWidthShift.. name the width of a class-0 box (class0BoxW)
 };
 // A job's source box is ONE TMA box, but not always the whole stage buffer: every box class has kBoxVariants tensor maps
 // of decreasing height (boxVariantRows below), and a job names the lowest one that still holds the rows its windows span
@@ -99,6 +100,42 @@ __host__ __device__ constexpr int boxVariantFor(int k, int cls, int rows) {
   while (v + 1 < kBoxVariants && cls != 1 && boxVariantRows(k, cls, v + 1) >= rows) ++v;
   return v;
 }
+// A class-0 tile or quadrant job also loads a box of one of kClass0Widths widths, the narrowest that holds the columns its
+// windows span: a polar tile's windows cover a rotated patch of the source whose columns are mostly far fewer than 208
+// bytes (cfg2: 80 / 112 / 144 / 208 B hold 12 / 55 / 23 / 10 % of the tiles and quadrants; their boxes lose 39 % of their
+// bytes; profiles/box_footprint.py).  The box lands in shared memory at a pitch of its width, and the device's copy of
+// the job's records holds its window offsets at that pitch (gather_plan.h: deviceRecords; the plan itself keeps the stage
+// buffer's 208 B).  Every width is 4 * odd words, like 208 B (bank model of the tile jobs' window loads:
+// profiles/box_footprint.py).  Seam jobs (two boxes ORed together) and pole-cap jobs (cut to fill 208 B) keep the whole
+// width.  The device's job list carries the width in the top bits of GatherJob::recordOffset (0: 208 B).
+constexpr int kClass0Widths = 4, kJobWidthShift = 28, kJobRecordMask = (1 << kJobWidthShift) - 1;
+__host__ __device__ constexpr int class0BoxW(int w) { return w == 0 ? 208 : (w == 1 ? 144 : (w == 2 ? 112 : 80)); }
+// Widths a kernel size uses: Lanczos4 (K = 8) keeps the whole width (with the narrow boxes cfg4 was 6 % slower in an
+// A/B on an H100 SXM at 700 W; DESIGN.md section 6)
+__host__ __device__ constexpr int class0Widths(int k) { return k == 8 ? 1 : kClass0Widths; }
+// the narrowest width that holds `cols` bytes of a row
+__host__ __device__ constexpr int class0WidthFor(int k, int cols) {
+  int w = 0;
+  while (w + 1 < class0Widths(k) && class0BoxW(w + 1) >= cols) ++w;
+  return w;
+}
+// The tensor maps of a plane for kernel size k, one per box shape it uses: class 0 (width w, height variant v) at
+// w * kBoxVariants + v, class 1, then the share box's heights (16 maps for K = 2 and 4, 7 for K = 8).
+__host__ __device__ constexpr int boxMaps(int k) { return class0Widths(k) * kBoxVariants + 1 + kBoxVariants; }
+constexpr int kMaxBoxMaps = kClass0Widths * kBoxVariants + 1 + kBoxVariants;
+__host__ __device__ constexpr int boxMapIndex(int k, int cls, int width, int variant) {
+  return cls == 0 ? width * kBoxVariants + variant : (cls == 1 ? class0Widths(k) * kBoxVariants : class0Widths(k) * kBoxVariants + 1 + variant);
+}
+__host__ __device__ constexpr int boxMapClass(int k, int i) {
+  return i < class0Widths(k) * kBoxVariants ? 0 : (i == class0Widths(k) * kBoxVariants ? 1 : 2);
+}
+__host__ __device__ constexpr int boxMapW(int k, int i) { return boxMapClass(k, i) == 0 ? class0BoxW(i / kBoxVariants) : stageBoxW(k, boxMapClass(k, i)); }
+__host__ __device__ constexpr int boxMapRows(int k, int i) {
+  return boxMapClass(k, i) == 0 ? boxVariantRows(k, 0, i % kBoxVariants)
+         : boxMapClass(k, i) == 1 ? stageBoxH(k, 1)
+                                  : boxVariantRows(k, 2, i - class0Widths(k) * kBoxVariants - 1);
+}
+
 // Stages of a group's ring (a stage = one box + one record buffer).  Three fit beside the cubic tables if the boxes lose
 // a few rows (not measured since no job reads its windows through L1 any more; at the time the third stage left too
 // little L1 for those reads and made the frame slower, measured on the B200).
@@ -307,8 +344,10 @@ constexpr int kBlurMaxSmem = 96 * 1024;
 // General path for a whole plane: taps through L1, every border mode (BORDER_WRAP, BORDER_TRANSPARENT), nearest.
 cudaError_t launchGather(const GatherParams& p, int numSMs, cudaStream_t stream);
 // Whole planes in one persistent kernel: `jobs` lists the jobs of every plane in launch order (gather_plan.h:
-// jobLaunchRank).  tensorMaps: per plane kNumBoxClasses CUtensorMap (128 bytes each) describing its source with the
-// staging boxes of p.kernelSize, i.e. [numPlanes][kNumBoxClasses].  BORDER_WRAP only.
+// jobLaunchRank).  tensorMaps: per plane kMaxBoxMaps CUtensorMap (128 bytes each), of which the first
+// boxMaps(p.kernelSize) describe its source with the staging boxes of p.kernelSize (boxMapIndex), i.e.
+// [numPlanes][kMaxBoxMaps].  BORDER_WRAP only.  The kernel takes boxMaps(k) maps per plane as a parameter: 6 KB for
+// K = 2 and 4, more than 4 KB of kernel parameters, which needs CUDA 12.1 and a driver of the R530 series or newer.
 // programmatic: allow the launch to overlap the tail of the previous kernel on the stream (programmatic dependent launch).
 cudaError_t launchGatherFrame(const FrameGatherParams& p, const StagedParams& jobs, const void* tensorMaps, int numSMs,
                               cudaStream_t stream, bool programmatic = true);

@@ -206,15 +206,14 @@ EncodeTiledFn tensorMapEncoder() {
   return fn;
 }
 
-// Describes a pitch-linear 8-bit plane to the TMA unit with variant `variant` of the staging box of class `cls` of kernel
-// size k (kernels.cuh: boxVariantRows).
-bool encodePlaneMap(CUtensorMap* map, const uint8_t* base, int w, int h, int pitch, int k, int cls, int variant) {
+// Describes a pitch-linear 8-bit plane to the TMA unit with box shape `index` of kernel size k (kernels.cuh: boxMapIndex).
+bool encodePlaneMap(CUtensorMap* map, const uint8_t* base, int w, int h, int pitch, int k, int index) {
   EncodeTiledFn enc = tensorMapEncoder();
   if (!enc) return false;
   if ((reinterpret_cast<uintptr_t>(base) & 15) || (pitch & 15)) return false;
   const cuuint64_t dims[2] = {static_cast<cuuint64_t>(w), static_cast<cuuint64_t>(h)};
   const cuuint64_t strides[1] = {static_cast<cuuint64_t>(pitch)};
-  const cuuint32_t box[2] = {static_cast<cuuint32_t>(t360::stageBoxW(k, cls)), static_cast<cuuint32_t>(t360::boxVariantRows(k, cls, variant))};
+  const cuuint32_t box[2] = {static_cast<cuuint32_t>(t360::boxMapW(k, index)), static_cast<cuuint32_t>(t360::boxMapRows(k, index))};
   const cuuint32_t elem[2] = {1, 1};
   return enc(map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<uint8_t*>(base), dims, strides, box, elem,
              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,  // (none / 64 / 256 B: no difference)
@@ -225,13 +224,13 @@ bool encodePlaneMap(CUtensorMap* map, const uint8_t* base, int w, int h, int pit
 // luma plane on the caller's stream and the two chroma planes on their own lanes.
 constexpr int kPlaneLanes = 3;
 static_assert(kPlaneLanes == t360::kMaxFramePlanes, "the frame kernel takes one PlaneView per lane");
-// The tensor maps of one source plane (every box class and variant): encoding one takes the driver about a
-// microsecond, a frame needs 21, and callers come back with the same few planes (a decoder's surface pool, the
+// The tensor maps of one source plane (every box shape of its kernel size): encoding one takes the driver about a
+// microsecond, a frame needs up to 48, and callers come back with the same few planes (a decoder's surface pool, the
 // library's own low-pass plane), so every lane remembers the last few.
 struct PlaneMaps {
   const uint8_t* base = nullptr;
   int w = 0, h = 0, pitch = 0, k = 0;
-  CUtensorMap maps[t360::kNumBoxClasses][t360::kBoxVariants];
+  CUtensorMap maps[t360::kMaxBoxMaps];
 };
 struct PlaneLane {
   static constexpr int kMapCache = 32;  // (a decoder's surface pool holds 10 - 20 frames)
@@ -249,7 +248,7 @@ struct GatherWork {
   const DevicePlan* plan = nullptr;
   t360::PlaneView view{};
   bool staged = false;                       // TMA-describable: may run in the persistent (per-plane / per-frame) kernel
-  CUtensorMap maps[t360::kNumBoxClasses][t360::kBoxVariants];
+  CUtensorMap maps[t360::kMaxBoxMaps];
   uint8_t* finalOut = nullptr;               // where the area resize (if any) delivers
   int finalPitch = 0, finalW = 0, finalH = 0, imagePlane = 0;
   const void* resizeTables = nullptr;
@@ -1525,18 +1524,16 @@ class VideoFrameTransform {
       d.numStaged = g.totalStaged();
       d.numBorder = g.numBorder;
       d.numJobs = static_cast<int>(g.launchJobs.size());
-      if (!g.launchJobs.empty()) {
-        d.gatherJobs.reserve(g.launchJobs.size());
-        CU(cudaMemcpy(d.gatherJobs.ptr, g.launchJobs.data(), g.launchJobs.size() * sizeof(GatherJob), cudaMemcpyHostToDevice));
+      d.hostJobs = t360::deviceJobs(g);
+      if (!d.hostJobs.empty()) {
+        d.gatherJobs.reserve(d.hostJobs.size());
+        CU(cudaMemcpy(d.gatherJobs.ptr, d.hostJobs.data(), d.hostJobs.size() * sizeof(GatherJob), cudaMemcpyHostToDevice));
       }
       if (!g.compact.empty() || !g.capRecords.empty()) {  // one buffer: the tiles' records, then the pole caps'
-        d.records.reserve(g.compact.size() + g.capRecords.size());
-        if (!g.compact.empty())
-          CU(cudaMemcpy(d.records.ptr, g.compact.data(), g.compact.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
-        if (!g.capRecords.empty())
-          CU(cudaMemcpy(d.records.ptr + g.compact.size(), g.capRecords.data(), g.capRecords.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+        const std::vector<uint32_t> records = t360::deviceRecords(g, d.kernelSize);
+        d.records.reserve(records.size());
+        CU(cudaMemcpy(d.records.ptr, records.data(), records.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
       }
-      d.hostJobs = std::move(g.launchJobs);
       d.jobNeedRows = std::move(g.launchNeedRows);
       d.jobRects = std::move(g.launchRects);
     }
@@ -1661,21 +1658,15 @@ class VideoFrameTransform {
 
   // the tensor maps of a source plane, from the lane's cache or freshly encoded (false: not TMA-describable)
   static bool planeMaps(PlaneLane& lane, const uint8_t* src, int w, int h, int pitch, int k,
-                        CUtensorMap (&out)[t360::kNumBoxClasses][t360::kBoxVariants]) {
+                        CUtensorMap (&out)[t360::kMaxBoxMaps]) {
     for (const PlaneMaps& e : lane.mapCache)
       if (e.base == src && e.w == w && e.h == h && e.pitch == pitch && e.k == k) {
         std::memcpy(out, e.maps, sizeof(e.maps));
         return true;
       }
     PlaneMaps fresh;
-    for (int c = 0; c < t360::kNumBoxClasses; ++c)
-      for (int v = 0; v < t360::kBoxVariants; ++v) {
-        if (v > 0 && t360::boxVariantRows(k, c, v) == t360::boxVariantRows(k, c, 0)) {
-          fresh.maps[c][v] = fresh.maps[c][0];  // (class 1 has one height)
-          continue;
-        }
-        if (!encodePlaneMap(&fresh.maps[c][v], src, w, h, pitch, k, c, v)) return false;
-      }
+    for (int m = 0; m < t360::boxMaps(k); ++m)
+      if (!encodePlaneMap(&fresh.maps[m], src, w, h, pitch, k, m)) return false;
     fresh.base = src; fresh.w = w; fresh.h = h; fresh.pitch = pitch; fresh.k = k;
     lane.mapCache[lane.mapCacheNext] = fresh;
     lane.mapCacheNext = (lane.mapCacheNext + 1) % PlaneLane::kMapCache;
@@ -1953,7 +1944,7 @@ class VideoFrameTransform {
     const FrameListRefs f = frameLists(plans, numPlanes);
     armScheduler(slot.frameClaim, s);
     t360::FrameGatherParams fp{};
-    CUtensorMap maps[kPlaneLanes][t360::kNumBoxClasses][t360::kBoxVariants];
+    CUtensorMap maps[kPlaneLanes][t360::kMaxBoxMaps];
     for (int p = 0; p < numPlanes; ++p) {
       fp.plane[p] = work[p].view;
       std::memcpy(maps[p], work[p].maps, sizeof(work[p].maps));
@@ -2342,6 +2333,8 @@ struct T360HostPlan {
   HostPlan plan;
   t360::GatherPlan gather;  // built on first use by T360B200_hostPlanGather
   bool gatherBuilt = false;
+  std::vector<GatherJob> deviceJobs;      // built on first use by T360B200_hostPlanDeviceLists
+  std::vector<uint32_t> deviceRecords;
   std::vector<uint8_t> blurImage;  // the last T360B200_hostPlanBlurLists image made with this plan first
 };
 
@@ -2415,6 +2408,20 @@ T360_API int T360B200_hostPlanPoleCaps(T360HostPlan* plan, int info[4], const in
   if (capJobs) *capJobs = g.capJobs.empty() ? nullptr : reinterpret_cast<const int32_t*>(g.capJobs.data());
   if (capRecords) *capRecords = g.capRecords.empty() ? nullptr : g.capRecords.data();
   if (launchJobs) *launchJobs = g.launchJobs.empty() ? nullptr : reinterpret_cast<const int32_t*>(g.launchJobs.data());
+  return 1;
+}
+T360_API int T360B200_hostPlanDeviceLists(T360HostPlan* plan, int info[2], const int32_t** jobs, const uint32_t** records) {
+  int gatherInfo[10];
+  if (!plan || !info || !jobs || !records || !T360B200_hostPlanGather(plan, gatherInfo, nullptr, nullptr, nullptr)) return 0;
+  const t360::GatherPlan& g = plan->gather;
+  if (plan->deviceJobs.size() != g.launchJobs.size()) {
+    plan->deviceJobs = t360::deviceJobs(g);
+    plan->deviceRecords = t360::deviceRecords(g, plan->plan.kernelSize);
+  }
+  info[0] = static_cast<int>(plan->deviceJobs.size());
+  info[1] = static_cast<int>(plan->deviceRecords.size());
+  *jobs = plan->deviceJobs.empty() ? nullptr : reinterpret_cast<const int32_t*>(plan->deviceJobs.data());
+  *records = plan->deviceRecords.empty() ? nullptr : plan->deviceRecords.data();
   return 1;
 }
 T360_API int T360B200_hostPlanBlurLists(T360HostPlan* const* plans, int numPlans, int width, int height, int layout[15],

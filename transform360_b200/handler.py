@@ -185,6 +185,8 @@ def load(path: os.PathLike | None = None):
     L.T360B200_hostPlanBlurLists.restype = ci
     L.T360B200_hostPlanBlurLists.argtypes = [vp, ci, ci, ci, C.POINTER(ci), C.POINTER(vp)]
     L.T360B200_hostPlanPoleCaps.argtypes = [vp, C.POINTER(ci), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]
+    L.T360B200_hostPlanDeviceLists.restype = ci
+    L.T360B200_hostPlanDeviceLists.argtypes = [vp, C.POINTER(ci), C.POINTER(vp), C.POINTER(vp)]
     L.T360B200_weightImage.restype = ci
     L.T360B200_weightImage.argtypes = [ci, C.POINTER(vp)]
     L.T360B200_remapTable.restype = ci
@@ -244,7 +246,7 @@ EXPORTED_SYMBOLS = [
     "VideoFrameTransform_transformFramePlane", "T360B200_hostPlanCreate", "T360B200_hostPlanCreateFromWarp", "T360B200_hostPlanDestroy",
     "T360B200_generateMapFromWarp", "T360B200_remapFrameAsync",
     "T360B200_hostPlanInfo", "T360B200_hostPlanMap", "T360B200_hostPlanSamples", "T360B200_hostPlanSegment",
-    "T360B200_hostPlanGather", "T360B200_hostPlanPoleCaps", "T360B200_hostPlanBlurLists", "T360B200_weightImage", "T360B200_dealLanes",
+    "T360B200_hostPlanGather", "T360B200_hostPlanPoleCaps", "T360B200_hostPlanDeviceLists", "T360B200_hostPlanBlurLists", "T360B200_weightImage", "T360B200_dealLanes",
     "T360B200_remapTable", "T360B200_transformFramePlaneAsync", "T360B200_transformFrameAsync",
     "T360B200_lowPassPlaneAsync", "T360B200_reconfigure", "T360B200_reconfigureAsync", "T360B200_reconfigureWait",
     "T360B200_transformFrameViewAsync", "T360B200_viewSamples",
@@ -525,6 +527,18 @@ class HostPlan:
         as_jobs = lambda p, k: np.frombuffer((C.c_int32 * (k * 4)).from_address(p.value), np.int32).reshape(k, 4).copy() if k and p.value else np.zeros((0, 4), np.int32)
         records = np.frombuffer((C.c_uint32 * info[2]).from_address(recs.value), np.uint32).copy() if info[2] and recs.value else np.zeros(0, np.uint32)
         return dict(counts=dict(cap=info[0], border=info[1]), jobs=as_jobs(jobs, n), records=records, launch=as_jobs(launch, m))
+
+    def device_lists(self):
+        """The job list and record buffer the frame kernel reads (T360B200_hostPlanDeviceLists): a dict of jobs int32[m][4]
+        (pole_caps()["launch"] with the class-0 box width index in bits 28-31 of recordOffset) and records uint32[]
+        (compact records, then the pole caps', a narrow box's window offsets at its pitch)."""
+        info = (C.c_int * 2)()
+        jobs, recs = C.c_void_p(), C.c_void_p()
+        if not self._lib.T360B200_hostPlanDeviceLists(self._h, info, C.byref(jobs), C.byref(recs)):
+            raise ValueError("T360B200_hostPlanDeviceLists failed")
+        j = np.frombuffer((C.c_int32 * (info[0] * 4)).from_address(jobs.value), np.int32).reshape(-1, 4).copy() if info[0] and jobs.value else np.zeros((0, 4), np.int32)
+        r = np.frombuffer((C.c_uint32 * info[1]).from_address(recs.value), np.uint32).copy() if info[1] and recs.value else np.zeros(0, np.uint32)
+        return dict(jobs=j, records=r)
 
     def blur_lists(self, *others, width=0, height=0):
         """The low-pass job lists of this plan -- merged with those of `others` (the other planes of a frame) when given --
