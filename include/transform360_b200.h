@@ -254,7 +254,8 @@ int T360B200_poseSamples(const FrameTransformContext* ctx, const T360Pose* pose,
  * (x', y') = theta_d / rho (X, Y) ((0, 0) at rho = 0).  In a plane of inW x inH the source position is
  * ((fx x' + cx + 0.5) / calibWidth) inW - 0.5, and likewise for y: at the calibration size fx x' + cx, which is
  * cv2.fisheye.projectPoints (skew 0) for Z > 0; chroma planes scale the calibration as the planned layouts do.
- * A direction goes to the lens with the larger Z / |d| (ties: lens 0), with a hard seam; theta > maxAngle, and a barrel
+ * A direction goes to the lens with the larger Z / |d| (ties: lens 0), with a hard seam (feathered: the blend calls
+ * below); theta > maxAngle, and a barrel
  * dead zone, are uncovered.  Sampling is BORDER_TRANSPARENT: uncovered pixels and pixels whose anchor tap lies outside the
  * source keep what the output holds (luma the caller's bytes, chroma 128, pre-filled).
  *
@@ -295,6 +296,44 @@ int T360B200_transformFrameLensAsync(VideoFrameTransform* transform, const T360L
                                      int numPlanes, const uint8_t* const* deviceInputs, uint8_t* const* deviceOutputs,
                                      const int* inputWidths, const int* inputHeights, const int* inputPitches,
                                      const int* outputWidths, const int* outputHeights, const int* outputPitches, void* cudaStream);
+/* ---- fisheye lens rigs with a feathered seam --------------------------------------------------------
+ * A two-lens rig whose lenses are blended across a belt of seamWidth degrees instead of meeting at a hard seam.  Rig,
+ * orientation and context mean what they mean above.  For the rig direction d of an output pixel, each lens i gives
+ * theta_i = atan2(rho, Z) of its camera coordinates, covers d when theta_i <= its maxAngle, and then has the source
+ * position above.  The weight w (0..256) of lens 1:
+ *   - both lenses cover d: t = 0.5 + (theta0 - theta1) s, with s = 1 / (2 seamWidth pi / 180) (computed in double, used
+ *     as float; every float step rounded to nearest), tw = 256 t, w = 0 for tw <= 0, 256 for tw >= 256, else tw rounded
+ *     half to even.  For back-to-back lenses of half-angle A this is a linear ramp across a belt seamWidth degrees wide,
+ *     centred on the seam; it lies inside both lenses' coverage when seamWidth <= 2 (A - 90): 10 for 190-degree lenses;
+ *   - only lens i covers d: w = 0 for lens 0, 256 for lens 1 (this also fills directions the hard seam leaves
+ *     uncovered when the closer lens does not reach them);
+ *   - neither covers d, or d is in a barrel dead zone: uncovered, the pixel keeps what the output holds.
+ * a = lens 0's sample where w < 256, b = lens 1's where w > 0, each interpolated with BORDER_TRANSPARENT as above.  Where
+ * both exist the pixel is (a (256 - w) + b w + 128) >> 8; where BORDER_TRANSPARENT skips one (its anchor tap lies outside
+ * the source), the other alone; where it skips both, the pixel keeps what the output holds.  Pre-fill as above: chroma
+ * 128, luma the caller's bytes.
+ *
+ * Refused, with 0 and a message on stdout before any CUDA call: the refusals of the lens calls above, numLenses other than
+ * 2 (a single lens has no seam: T360B200_transformFrameLensAsync), and a seamWidth that is not finite or lies outside
+ * [0.01, 180]. */
+/* Host only, no CUDA: the host twin of T360B200_transformFrameLensBlendAsync for one plane of inputWidth x inputHeight.
+ * map0, map1: CV_32FC2 maps (float32 [outputHeight][outputWidth][2]) of lens 0 and lens 1, NaN where that lens does not
+ * contribute (it does not cover the pixel's direction, or w gives it no weight); weight: w (uint16 [outputHeight]
+ * [outputWidth], 0 where neither lens covers the pixel).  cv::remap of each map with BORDER_TRANSPARENT, combined as above,
+ * gives the frame call's plane bit for bit.  Returns 1; 0 (message) for the refusals above, a NULL array or non-positive
+ * sizes. */
+int T360B200_lensBlendMaps(const FrameTransformContext* ctx, const T360LensRig* rig, float seamWidth, const T360Orientation* orientation,
+                           int inputWidth, int inputHeight, int outputWidth, int outputHeight, float* map0, float* map1, uint16_t* weight);
+/* One frame of a two-lens rig with a feathered seam, every plane in one gather launch: the arguments and the asynchronous
+ * contract of T360B200_transformFrameLensAsync, plus seamWidth, which may change every frame like the rig and the
+ * orientation.  Needs no plan and does not touch the plans; takes the reader lock; never synchronises the device.  Returns 1
+ * if everything was enqueued; 0 with a message on stdout, before any CUDA call, for the refusals above, 0 or more than 3
+ * planes, or an invalid plane description. */
+int T360B200_transformFrameLensBlendAsync(VideoFrameTransform* transform, const T360LensRig* rig, float seamWidth,
+                                          const T360Orientation* orientation, int numPlanes, const uint8_t* const* deviceInputs,
+                                          uint8_t* const* deviceOutputs, const int* inputWidths, const int* inputHeights,
+                                          const int* inputPitches, const int* outputWidths, const int* outputHeights,
+                                          const int* outputPitches, void* cudaStream);
 /* Opt-in (also: environment T360B200_PIN_HOST_PLANES=1): page-lock pageable caller planes in place the second time
  * the same buffer is seen (cudaHostRegister), so that recycled frame-pool buffers are DMA'd at full PCIe speed.  The
  * caller must keep such buffers alive until VideoFrameTransform_delete. */

@@ -1,8 +1,9 @@
 """What a fisheye lens rig costs on the GPU machine: the per-frame lens call (T360B200_transformFrameLensAsync, a new
 orientation every frame) against the planned path for a fixed pose (T360B200_lensMap -> T360B200_generateMapFromWarp ->
-T360B200_transformFrameAsync) and against T360B200_remapFrameAsync with the same maps resident on the device.  Needs a GPU.
+T360B200_transformFrameAsync), against T360B200_remapFrameAsync with the same maps resident on the device, and (--blend)
+against the feathered seam (T360B200_transformFrameLensBlendAsync) with belts of 4 and 10 degrees.  Needs a GPU.
 
-    python profiles/lens_path.py [--frames 100] [--windows 3] [--out FILE]
+    python profiles/lens_path.py [--frames 100] [--windows 3] [--blend] [--out FILE]
 
 Workload: a 5760x2880 yuv420p dual-fisheye frame, two 2880-pixel circles side by side from back-to-back 190-degree lenses
 with seeded small k1..k4 (calibrated at 5760x2880), bicubic, to EQUIRECT 5760x2880 and to CUBEMAP_32 3840x2560.  Inputs
@@ -11,6 +12,9 @@ come from a ring of frames larger than the L2 cache.  Per target:
 - lens_ms / planned_ms / remap_ms: CUDA-event GPU time per frame of `--frames` frames enqueued back to back on one stream
   after a warm-up, `--windows` windows per arm, the arms alternated window by window (the lens call with a new orientation
   every frame, the other two with the fixed pose their maps were made for);
+- blend4_ms / blend10_ms (--blend): the same for the feathered seam with seamWidth 4 and 10 degrees, a new orientation
+  every frame, alternated with the other arms; blend_share: the share of luma pixels in the belt (0 < w < 256) at the
+  fixed pose, per seamWidth;
 - identical: whether the three arms' outputs for the fixed pose are equal, byte for byte, plane by plane;
 - nan_share: the share of luma map entries no lens covers.
 Prints one JSON line (also appended to --out) with the card's name and power limit read in the same run.
@@ -52,6 +56,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--frames", type=int, default=100, help="frames per timed window")
     ap.add_argument("--windows", type=int, default=3, help="timed windows per arm")
+    ap.add_argument("--blend", action="store_true", help="add the feathered-seam arms")
     ap.add_argument("--out", help="append the JSON line to this file")
     args = ap.parse_args()
     import numpy as np
@@ -93,7 +98,7 @@ def main():
             assert vft.generate_map_from_warp(maps[idx], *dims[idx][:2], idx, t360.BORDER_TRANSPARENT)
             generate_ms.append(round((time.perf_counter() - t0) * 1e3, 1))
         d_maps = [torch.from_numpy(m).cuda() for m in maps]
-        outs = {k: [torch.zeros((d[3], pitch(d[2])), dtype=torch.uint8, device="cuda") for d in dims] for k in ("lens", "planned", "remap")}
+        outs = {k: [torch.zeros((d[3], pitch(d[2])), dtype=torch.uint8, device="cuda") for d in dims] for k in ("lens", "planned", "remap", "blend")}
         out_planes = {k: [(t.data_ptr(), t.stride(0)) for t in v] for k, v in outs.items()}
         lens = [vft.make_lens_frame_call(in_planes[f], out_planes["lens"], dims) for f in range(RING)]
         planned = [vft.make_frame_call(in_planes[f], out_planes["planned"], dims) for f in range(RING)]
@@ -114,6 +119,13 @@ def main():
             "planned_ms": lambda i: planned[i % RING](s),
             "remap_ms": lambda i: remap[i % RING]([d_maps[0], d_maps[1], d_maps[1]], s),
         }
+        extra = {}
+        if args.blend:
+            blend = [vft.make_lens_blend_frame_call(in_planes[f], out_planes["blend"], dims) for f in range(RING)]
+            for seam in (4.0, 10.0):
+                arms[f"blend{seam:g}_ms"] = lambda i, seam=seam: blend[i % RING](rig, seam, path[i], s)
+            extra["blend_share"] = {f"{seam:g}": round(float(((w > 0) & (w < 256)).mean()), 4)
+                                    for seam in (4.0, 10.0) for w in [t360.lens_blend_maps(ctx, rig, seam, fixed, *dims[0])[2]]}
         for call in arms.values():  # warm-up: first launches, weight tables, the lens call's table upload
             for i in range(10):
                 assert call(i)
@@ -129,7 +141,7 @@ def main():
                 b.synchronize()
                 times[k].append(round(a.elapsed_time(b) / args.frames, 4))
         result["cases"][name] = dict(layout=layout, output=[ow, oh], lens_map_ms=lens_map_ms, generate_ms=generate_ms, **times,
-                                     identical=identical, nan_share=round(float(np.isnan(maps[0][..., 0]).mean()), 4))
+                                     identical=identical, nan_share=round(float(np.isnan(maps[0][..., 0]).mean()), 4), **extra)
         vft.close()
         del d_maps, outs
         torch.cuda.empty_cache()

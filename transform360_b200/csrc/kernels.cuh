@@ -444,6 +444,16 @@ struct LensGatherParams {
 };
 cudaError_t launchLensGather(LensGatherParams p, int numSMs, cudaStream_t stream);
 
+// ---- the per-frame lens blend (view_gather.cu) -----------------------------------------------------------------------
+// Frames of a two-lens rig with the seam feathered across a belt (oriented_view.h: lensBlendSample): every pixel computes
+// both lenses' records and the weight of lens 1, gathers the lens that carries it (lens 0 unless w = 256), and a second
+// time, lens 1, only where both carry weight; the two values are blended as (a (256 - w) + b w + 128) >> 8.  The lens
+// gather's tiles, threads, taps and BORDER_TRANSPARENT.
+struct LensBlendGatherParams : LensGatherParams {
+  float seamScale;  // s = 1 / (2 seamWidth), seamWidth in radians
+};
+cudaError_t launchLensBlendGather(LensBlendGatherParams p, int numSMs, cudaStream_t stream);
+
 // bytes of dynamic shared memory a blur tile of (w x h) with the given tap counts needs
 inline int blurTileSmem(int w, int h, int nkx, int nky) {
   const int hx = nkx / 2, hy = nky / 2;

@@ -429,24 +429,61 @@ struct LensRigModel {
 
 T360_HD float lensRow(const float* m, const SphereVec& d) { return fAdd(fAdd(fMul(m[0], d.x), fMul(m[1], d.y)), fMul(m[2], d.z)); }
 
+// What one lens makes of rig direction d: theta, whether it covers d (theta <= thetaMax), and where it does, the source
+// position (px, py) in an inW x inH plane (NaN for both where it does not).  Z = lensRow(L.m + 6, d), which the callers
+// have already computed.  The one place the lens projection is written: the hard seam (lensPosition) and the feathered
+// seam (lensBlendPosition) both call it.
+struct LensHit {
+  float theta, px, py;
+  bool covered;
+};
+T360_HD LensHit lensHit(const LensModel& L, const SphereVec& d, float Z, int inW, int inH) {
+  const float X = lensRow(L.m, d), Y = lensRow(L.m + 3, d);
+  const float rho = fSqrt(fAdd(fMul(X, X), fMul(Y, Y)));
+  LensHit h;
+  h.theta = libmAtan2f(rho, Z);
+  h.covered = h.theta <= L.thetaMax;
+  if (!h.covered) {
+    h.px = h.py = bitsFloat(0x7fc00000u);
+    return h;
+  }
+  const float t = fMul(h.theta, h.theta);
+  const float poly = fAdd(1.0f, fMul(t, fAdd(L.k[0], fMul(t, fAdd(L.k[1], fMul(t, fAdd(L.k[2], fMul(t, L.k[3]))))))));
+  const float s = rho > 0.0f ? fDiv(fMul(h.theta, poly), rho) : 0.0f;
+  h.px = toPixel(fAdd(fMul(L.ax, fMul(s, X)), L.bx), inW);
+  h.py = toPixel(fAdd(fMul(L.ay, fMul(s, Y)), L.by), inH);
+  return h;
+}
+
 // The source position (*px, *py) of rig direction d in an inW x inH plane; NaN for both where no lens covers d.
 T360_HD void lensPosition(const LensRigModel& rig, const SphereVec& d, int inW, int inH, float* px, float* py) {
   const float z0 = lensRow(rig.lens[0].m + 6, d);
   const float z1 = rig.numLenses > 1 ? lensRow(rig.lens[1].m + 6, d) : z0;
   const bool second = z1 > z0;
-  const LensModel& L = second ? rig.lens[1] : rig.lens[0];
-  const float X = lensRow(L.m, d), Y = lensRow(L.m + 3, d), Z = second ? z1 : z0;
-  const float rho = fSqrt(fAdd(fMul(X, X), fMul(Y, Y)));
-  const float theta = libmAtan2f(rho, Z);
-  if (!(theta <= L.thetaMax)) {
-    *px = *py = bitsFloat(0x7fc00000u);
-    return;
+  const LensHit h = lensHit(second ? rig.lens[1] : rig.lens[0], d, second ? z1 : z0, inW, inH);
+  *px = h.px;
+  *py = h.py;
+}
+
+// The feathered seam of a two-lens rig (T360B200_transformFrameLensBlendAsync): both lenses' view of d and the weight w
+// (0..256) of lens 1.  Where both cover d, w is a linear ramp in theta0 - theta1, t = 0.5 + (theta0 - theta1) s rounded to
+// 1/256 and clamped (s = 1 / (2 seamWidth), seamWidth in radians, computed on the host in double: lensSeamScale); where
+// one covers d, that lens alone (w = 0 or 256).  p0 / p1: lens 0's / lens 1's source position, NaN where that lens does
+// not contribute (it does not cover d, or w gives it no weight).  Returns w; 0 where neither lens covers d.
+T360_HD int lensBlendPosition(const LensRigModel& rig, float s, const SphereVec& d, int inW, int inH, float* p0, float* p1) {
+  const LensHit h0 = lensHit(rig.lens[0], d, lensRow(rig.lens[0].m + 6, d), inW, inH);
+  const LensHit h1 = lensHit(rig.lens[1], d, lensRow(rig.lens[1].m + 6, d), inW, inH);
+  int w = h1.covered ? 256 : 0;
+  if (h0.covered && h1.covered) {
+    const float tw = fMul(fAdd(0.5f, fMul(fSub(h0.theta, h1.theta), s)), 256.0f);
+    w = tw <= 0.0f ? 0 : (tw >= 256.0f ? 256 : roundHalfEven(tw));
   }
-  const float t = fMul(theta, theta);
-  const float poly = fAdd(1.0f, fMul(t, fAdd(L.k[0], fMul(t, fAdd(L.k[1], fMul(t, fAdd(L.k[2], fMul(t, L.k[3]))))))));
-  const float s = rho > 0.0f ? fDiv(fMul(theta, poly), rho) : 0.0f;
-  *px = toPixel(fAdd(fMul(L.ax, fMul(s, X)), L.bx), inW);
-  *py = toPixel(fAdd(fMul(L.ay, fMul(s, Y)), L.by), inH);
+  const float nan = bitsFloat(0x7fc00000u);
+  p0[0] = w < 256 ? h0.px : nan;
+  p0[1] = w < 256 ? h0.py : nan;
+  p1[0] = w > 0 ? h1.px : nan;
+  p1[1] = w > 0 ? h1.py : nan;
+  return w;
 }
 
 // The map entry of output pixel (i, j) of a lens rig: spherePoint, then lensPosition; NaN in a barrel dead zone.  The
@@ -474,6 +511,37 @@ T360_HD void lensSample(const SphereGeometry& g, const Rotation& r, const LensRi
   quantizeAxis(px, g.kernelSize, col0, &fracX);
   quantizeAxis(py, g.kernelSize, &r0, &fracY);
   *rowPhase = r0 * 1024 + fracY * 32 + fracX;
+}
+
+// The two map entries and the weight of output pixel (i, j) of a two-lens rig with a feathered seam: spherePoint, then
+// lensBlendPosition; both entries NaN and w = 0 in a barrel dead zone.  (T360B200_lensBlendMaps)
+template <bool BARREL = true>
+T360_HD int lensBlendPoint(const SphereGeometry& g, const Rotation& r, const LensRigModel& rig, float s, const float* colTab,
+                           const float* rowTab, int i, int j, float* p0, float* p1) {
+  bool eye;
+  SphereVec d;
+  if (!spherePoint<BARREL>(g, r, colTab, rowTab, i, j, &eye, &d)) {
+    p0[0] = p0[1] = p1[0] = p1[1] = bitsFloat(0x7fc00000u);
+    return 0;
+  }
+  return lensBlendPosition(rig, s, d, g.inW, g.inH, p0, p1);
+}
+
+// The sampling records of output pixel (i, j) of a two-lens rig with a feathered seam, lens 0's in rec0 and lens 1's in
+// rec1 ({col0, rowPhase}, quantised as lensSample quantises its entry), and the weight w of lens 1 (the return value).
+template <bool BARREL = true>
+T360_HD int lensBlendSample(const SphereGeometry& g, const Rotation& r, const LensRigModel& rig, float s, const float* colTab,
+                            const float* rowTab, int i, int j, int32_t* rec0, int32_t* rec1) {
+  float p[2][2];
+  const int w = lensBlendPoint<BARREL>(g, r, rig, s, colTab, rowTab, i, j, p[0], p[1]);
+  int32_t* rec[2] = {rec0, rec1};
+  for (int l = 0; l < 2; ++l) {
+    int r0, fracX, fracY;
+    quantizeAxis(p[l][0], g.kernelSize, &rec[l][0], &fracX);
+    quantizeAxis(p[l][1], g.kernelSize, &r0, &fracY);
+    rec[l][1] = r0 * 1024 + fracY * 32 + fracX;
+  }
+  return w;
 }
 
 // Whether the per-frame orientation chain covers the layouts of `ctx`

@@ -494,6 +494,26 @@ bool lensRefused(const FrameTransformContext& ctx, const T360LensRig* rig, const
   return false;
 }
 
+// lensRefused, plus what the feathered seam needs: two lenses, and a belt width in [0.01, 180] degrees (the lower bound
+// keeps lensSeamScale finite)
+bool lensBlendRefused(const FrameTransformContext& ctx, const T360LensRig* rig, float seamWidth, const T360Orientation* o, std::string* why) {
+  if (lensRefused(ctx, rig, o, why)) return true;
+  if (rig->numLenses != 2) {
+    *why = formatted("numLenses %d: a feathered seam needs two lenses (one lens: T360B200_transformFrameLensAsync)", rig->numLenses);
+    return true;
+  }
+  if (!(seamWidth >= 0.01f && seamWidth <= 180.0f)) {
+    *why = formatted("seamWidth %g degrees is outside [0.01, 180]", seamWidth);
+    return true;
+  }
+  return false;
+}
+
+// s = 1 / (2 seamWidth), seamWidth in radians: lens 1's weight rises from 0 to 1 while theta0 - theta1 goes from
+// -seamWidth to +seamWidth, so a back-to-back pair blends across a belt seamWidth degrees wide (oriented_view.h:
+// lensBlendPosition)
+float lensSeamScale(float seamWidth) { return static_cast<float>(1.0 / (2.0 * static_cast<double>(seamWidth) * M_PI / 180.0)); }
+
 // The per-frame constants of a rig (oriented_view.h: LensModel), in double and stored as float
 t360::LensRigModel lensRigModel(const T360LensRig& rig) {
   t360::LensRigModel m{};
@@ -532,6 +552,19 @@ FrameTransformContext lensContext(const FrameTransformContext& ctx) {
   c.input_expand_coef = 1.0f;
   c.width_scale_factor = c.height_scale_factor = 1.0f;
   return c;
+}
+
+// The host twin of the lens kernels for one outW x outH plane of an inW x inH input: point(g, r, colTab, rowTab, i, j,
+// i * outW + j) for every output pixel, with the geometry, tables and rotation those kernels get for ctx and o
+template <class Point>
+void forLensPixels(const FrameTransformContext& ctx, const T360Orientation& o, int inW, int inH, int outW, int outH, Point&& point) {
+  const t360::SphereGeometry g = t360::sphereGeometry(lensContext(ctx), outW, outH, inW, inH, t360::kernelSizeOf(ctx.interpolation_alg));
+  const std::vector<float> tables = t360::buildSphereTables(g);
+  const float* colTab = tables.data();
+  const float* rowTab = tables.empty() ? nullptr : tables.data() + t360::sphereTableRowOffset(g);
+  const t360::Rotation r = t360::rotationFromAngles(o.yaw, o.pitch, o.roll);
+  for (int i = 0; i < outH; ++i)
+    for (int j = 0; j < outW; ++j) point(g, r, colTab, rowTab, i, j, static_cast<size_t>(i) * outW + j);
 }
 
 }  // namespace
@@ -1228,13 +1261,15 @@ class VideoFrameTransform {
   // computed by lensSample (oriented_view.h), so a rig gives what lensMap -> generateMapFromWarp plans for it.  Needs no
   // plan and leaves the plans alone; the output layout's tables come through the slot's upload ring.  Every refusal comes
   // before the first CUDA call, and nothing here synchronises the device.
-  bool transformFrameLens(const T360LensRig* rig, const T360Orientation* o, const FramePlanes& f, cudaStream_t stream) {
-    const char* what = "Could not transform the frame with a lens rig";
+  // seamWidth: nullptr for the hard seam; else the belt in degrees across which two lenses are blended
+  // (T360B200_transformFrameLensBlendAsync: lensBlendSample), the same steps with the blend kernel.
+  bool transformFrameLens(const char* what, const T360LensRig* rig, const float* seamWidth, const T360Orientation* o, const FramePlanes& f,
+                          cudaStream_t stream) {
     return guarded(what, [&] {
       std::shared_lock<std::shared_mutex> config(configMu_);
       const FrameTransformContext ctx = ctx_;
       std::string why;
-      if (lensRefused(ctx, rig, o, &why)) {
+      if (seamWidth ? lensBlendRefused(ctx, rig, *seamWidth, o, &why) : lensRefused(ctx, rig, o, &why)) {
         std::printf("%s. Error: %s\n", what, why.c_str());
         return false;
       }
@@ -1258,7 +1293,8 @@ class VideoFrameTransform {
       lp.rig = lensRigModel(*rig);
       lp.kernelSize = k;
       lp.weights = deviceWeights(ctx.interpolation_alg);
-      CU(t360::launchLensGather(lp, numSMs_, s));
+      if (seamWidth) CU(t360::launchLensBlendGather(t360::LensBlendGatherParams{lp, lensSeamScale(*seamWidth)}, numSMs_, s));
+      else CU(t360::launchLensGather(lp, numSMs_, s));
       releaseAfter(staged, s);
       return true;
     });
@@ -2617,18 +2653,31 @@ T360_API int T360B200_lensMap(const FrameTransformContext* ctx, const T360LensRi
     std::printf("%s. Error: %s\n", what, why.c_str());
     return 0;
   }
-  const FrameTransformContext lens = lensContext(*ctx);
-  const t360::SphereGeometry g = t360::sphereGeometry(lens, outW, outH, inW, inH, t360::kernelSizeOf(ctx->interpolation_alg));
-  const std::vector<float> tables = t360::buildSphereTables(g);
-  const float* colTab = tables.data();
-  const float* rowTab = tables.empty() ? nullptr : tables.data() + t360::sphereTableRowOffset(g);
-  const t360::Rotation r = t360::rotationFromAngles(orientation->yaw, orientation->pitch, orientation->roll);
   const t360::LensRigModel model = lensRigModel(*rig);
-  for (int i = 0; i < outH; ++i)
-    for (int j = 0; j < outW; ++j) {
-      float* out = map + 2 * (static_cast<size_t>(i) * outW + j);
-      t360::lensPoint(g, r, model, colTab, rowTab, i, j, out, out + 1);
-    }
+  forLensPixels(*ctx, *orientation, inW, inH, outW, outH, [&](const t360::SphereGeometry& g, const t360::Rotation& r, const float* colTab,
+                                                              const float* rowTab, int i, int j, size_t at) {
+    t360::lensPoint(g, r, model, colTab, rowTab, i, j, map + 2 * at, map + 2 * at + 1);
+  });
+  return 1;
+}
+T360_API int T360B200_lensBlendMaps(const FrameTransformContext* ctx, const T360LensRig* rig, float seamWidth, const T360Orientation* orientation,
+                                    int inW, int inH, int outW, int outH, float* map0, float* map1, uint16_t* weight) {
+  const char* what = "Could not compute the lens blend maps";
+  std::string why;
+  if (!ctx) why = "a NULL context";
+  else if (lensBlendRefused(*ctx, rig, seamWidth, orientation, &why)) {}
+  else if (!map0 || !map1 || !weight || inW <= 0 || inH <= 0 || outW <= 0 || outH <= 0)
+    why = "a NULL map or weight array or a plane size that is not positive";
+  if (!why.empty()) {
+    std::printf("%s. Error: %s\n", what, why.c_str());
+    return 0;
+  }
+  const t360::LensRigModel model = lensRigModel(*rig);
+  const float s = lensSeamScale(seamWidth);
+  forLensPixels(*ctx, *orientation, inW, inH, outW, outH, [&](const t360::SphereGeometry& g, const t360::Rotation& r, const float* colTab,
+                                                              const float* rowTab, int i, int j, size_t at) {
+    weight[at] = static_cast<uint16_t>(t360::lensBlendPoint(g, r, model, s, colTab, rowTab, i, j, map0 + 2 * at, map1 + 2 * at));
+  });
   return 1;
 }
 T360_API int T360B200_transformFrameLensAsync(VideoFrameTransform* t, const T360LensRig* rig, const T360Orientation* orientation, int numPlanes,
@@ -2641,7 +2690,19 @@ T360_API int T360B200_transformFrameLensAsync(VideoFrameTransform* t, const T360
   }
   FramePlanes f;
   if (!describeFrame(what, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, f)) return 0;
-  return t->transformFrameLens(rig, orientation, f, static_cast<cudaStream_t>(stream));
+  return t->transformFrameLens(what, rig, nullptr, orientation, f, static_cast<cudaStream_t>(stream));
+}
+T360_API int T360B200_transformFrameLensBlendAsync(VideoFrameTransform* t, const T360LensRig* rig, float seamWidth, const T360Orientation* orientation,
+                                                   int numPlanes, const uint8_t* const* dIn, uint8_t* const* dOut, const int* inW, const int* inH,
+                                                   const int* inPitch, const int* outW, const int* outH, const int* outPitch, void* stream) {
+  const char* what = "Could not blend the frame of a lens rig";
+  if (!t) {
+    std::printf("%s. Error: a NULL argument\n", what);
+    return 0;
+  }
+  FramePlanes f;
+  if (!describeFrame(what, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, f)) return 0;
+  return t->transformFrameLens(what, rig, &seamWidth, orientation, f, static_cast<cudaStream_t>(stream));
 }
 T360_API void T360B200_setPinHostPlanes(VideoFrameTransform* t, int enable) { if (t) t->setPinHostPlanes(enable != 0); }
 T360_API void T360B200_debugTrace(VideoFrameTransform* t, int enable) { if (t) t->enableTrace(enable != 0); }

@@ -15,7 +15,9 @@
 //   - a caller's warp map (MapPositions): the pixel's map entry, quantised by quantizeAxis.
 //   - a fisheye lens rig (LensPositions): the output half of the sphere chain, then the lens model (oriented_view.h:
 //     lensSample), quantised like a map entry.
-// In all four, the records come from the same host/device functions the planner (or its host twin) uses: bit-identical.
+//   - a two-lens rig with a feathered seam (LensBlendPositions): both lenses' records and a weight (lensBlendSample); the
+//     tile loop gathers the second record only where the weight blends the two.
+// In all five, the records come from the same host/device functions the planner (or its host twin) uses: bit-identical.
 #include "gather_common.cuh"
 
 #include <algorithm>
@@ -24,7 +26,26 @@
 namespace t360 {
 namespace {
 
-// TRANSPARENT (barrel layouts): BORDER_TRANSPARENT, a pixel whose anchor tap lies outside the source keeps its byte
+// One pixel of record {col0, rowPhase}: its value, or -1 where BORDER_TRANSPARENT leaves it alone
+template <int K, bool TRANSPARENT>
+__device__ __forceinline__ int viewPixel(const SrcView& s, const unsigned char* smem, int col0, int rowPhase) {
+  if constexpr (K == 1) {  // nearest: the rounded position, wrapped like cv::remap's BORDER_WRAP
+    if constexpr (TRANSPARENT) {
+      const int sx = col0, sy = rowPhase >> 10;
+      if ((unsigned)sx >= (unsigned)s.w || (unsigned)sy >= (unsigned)s.h) return -1;
+      return __ldg(s.bytes + (size_t)sy * s.pitch + sx);
+    } else {
+      return __ldg(s.bytes + (size_t)wrapIndex(rowPhase >> 10, s.h) * s.pitch + wrapIndex(col0, s.w));
+    }
+  } else {
+    return gatherPixel<K, TRANSPARENT, 16384>(s, smem, col0, rowPhase);
+  }
+}
+
+// TRANSPARENT (barrel layouts): BORDER_TRANSPARENT, a pixel whose anchor tap lies outside the source keeps its byte.
+// Positions::kBlend: its record() hands over two records and the weight w (0..256) of the second; the first is gathered
+// for every pixel, the second only where 0 < w < 256, and the two values are blended (LensBlendGatherParams).  Where
+// BORDER_TRANSPARENT skips one of the two, the other stands alone.
 template <int K, bool TRANSPARENT, class Params, class Positions>
 __device__ __forceinline__ void gatherViewTiles(const Params& p, int numTiles, unsigned char* smem, Positions& pos) {
   constexpr int kRows = viewTileRows(K);
@@ -50,19 +71,26 @@ __device__ __forceinline__ void gatherViewTiles(const Params& p, int numTiles, u
       const int i = y0 + r;
       if (i >= v.geometry.mapH) break;
       int col0, rowPhase;
-      pos.record(p, v, lane, r, i, j, &col0, &rowPhase);
       int value;
-      if constexpr (K == 1) {  // nearest: the rounded position, wrapped like cv::remap's BORDER_WRAP
-        if constexpr (TRANSPARENT) {
+      if constexpr (Positions::kBlend) {
+        int col1, rowPhase1, w;
+        pos.record(p, v, lane, r, i, j, &col0, &rowPhase, &col1, &rowPhase1, &w);
+        value = viewPixel<K, TRANSPARENT>(s, smem, col0, rowPhase);
+        if (w > 0 && w < 256) {
+          const int b = viewPixel<K, TRANSPARENT>(s, smem, col1, rowPhase1);
+          value = value < 0 ? b : (b < 0 ? value : (value * (256 - w) + b * w + 128) >> 8);
+        }
+        if (value < 0) continue;
+      } else {
+        pos.record(p, v, lane, r, i, j, &col0, &rowPhase);
+        if constexpr (K == 1 && TRANSPARENT) {  // (nearest: the bounds test skips the store directly, without viewPixel's -1)
           const int sx = col0, sy = rowPhase >> 10;
           if ((unsigned)sx >= (unsigned)s.w || (unsigned)sy >= (unsigned)s.h) continue;
           value = __ldg(s.bytes + (size_t)sy * s.pitch + sx);
         } else {
-          value = __ldg(s.bytes + (size_t)wrapIndex(rowPhase >> 10, s.h) * s.pitch + wrapIndex(col0, s.w));
+          value = viewPixel<K, TRANSPARENT>(s, smem, col0, rowPhase);
+          if (TRANSPARENT && value < 0) continue;
         }
-      } else {
-        value = gatherPixel<K, TRANSPARENT, 16384>(s, smem, col0, rowPhase);
-        if (TRANSPARENT && value < 0) continue;
       }
       v.dst[(size_t)i * v.dstPitch + j] = (uint8_t)value;
     }
@@ -74,6 +102,7 @@ template <int K>
 struct FlatPositions {
   static constexpr int kRows = viewTileRows(K);
   static constexpr int kTableBytes = 4 * 32 * (int)sizeof(FlatColumn) + 2 * kRows * (int)sizeof(FlatRow) + 32;
+  static constexpr bool kBlend = false;
   FlatColumn* colTab;  // [eye][fold][32]
   FlatRow* rowTab;     // [column eye][kRows]
   bool* colEye;        // [32]
@@ -111,6 +140,7 @@ struct FlatPositions {
 template <bool BARREL>
 struct SpherePositions {
   static constexpr int kTableBytes = 0;
+  static constexpr bool kBlend = false;
   __device__ void beginTile(const OrientedGatherParams&, const OrientedPlane&, int, int) {}
   __device__ void beginColumn(int) {}
   __device__ void record(const OrientedGatherParams& p, const OrientedPlane& v, int, int, int i, int j, int* col0, int* rowPhase) const {
@@ -123,6 +153,7 @@ struct SpherePositions {
 template <int K>
 struct MapPositions {
   static constexpr int kTableBytes = 0;
+  static constexpr bool kBlend = false;
   __device__ void beginTile(const MapGatherParams&, const MapPlane&, int, int) {}
   __device__ void beginColumn(int) {}
   __device__ void record(const MapGatherParams&, const MapPlane& v, int, int, int i, int j, int* col0, int* rowPhase) const {
@@ -138,10 +169,31 @@ struct MapPositions {
 template <bool BARREL>
 struct LensPositions {
   static constexpr int kTableBytes = 0;
+  static constexpr bool kBlend = false;
   __device__ void beginTile(const LensGatherParams&, const OrientedPlane&, int, int) {}
   __device__ void beginColumn(int) {}
   __device__ void record(const LensGatherParams& p, const OrientedPlane& v, int, int, int i, int j, int* col0, int* rowPhase) const {
     lensSample<BARREL>(v.geometry, p.rotation, p.rig, v.colTable, v.rowTable, i, j, col0, rowPhase);
+  }
+};
+
+// A two-lens rig with a feathered seam: both lenses' records and lens 1's weight per pixel (lensBlendSample).  The first
+// record is the lens that carries the pixel: lens 1 where w = 256, lens 0 everywhere else (also where neither lens covers
+// the pixel: its NaN record is skipped by BORDER_TRANSPARENT).  So a warp gathers twice only for its belt pixels.
+template <bool BARREL>
+struct LensBlendPositions {
+  static constexpr int kTableBytes = 0;
+  static constexpr bool kBlend = true;
+  __device__ void beginTile(const LensBlendGatherParams&, const OrientedPlane&, int, int) {}
+  __device__ void beginColumn(int) {}
+  __device__ void record(const LensBlendGatherParams& p, const OrientedPlane& v, int, int, int i, int j, int* col0, int* rowPhase, int* col1,
+                         int* rowPhase1, int* w) const {
+    int32_t rec0[2], rec1[2];
+    *w = lensBlendSample<BARREL>(v.geometry, p.rotation, p.rig, p.seamScale, v.colTable, v.rowTable, i, j, rec0, rec1);
+    *col0 = *w == 256 ? rec1[0] : rec0[0];
+    *rowPhase = *w == 256 ? rec1[1] : rec0[1];
+    *col1 = rec1[0];
+    *rowPhase1 = rec1[1];
   }
 };
 
@@ -183,6 +235,18 @@ template <int K, bool BARREL>
 __global__ void __launch_bounds__(gatherThreads(K), K == 8 ? 1 : 4) lensGatherKernel(const __grid_constant__ LensGatherParams p, int numTiles) {
   extern __shared__ __align__(16) unsigned char smem[];
   LensPositions<BARREL> pos;
+  if constexpr (K >= 2) {
+    stageWeights<K>(p.weights, smem);
+    __syncthreads();  // (no tile synchronises after this)
+  }
+  gatherViewTiles<K, true>(p, numTiles, smem, pos);
+}
+
+// BARREL: as lensGatherKernel
+template <int K, bool BARREL>
+__global__ void __launch_bounds__(gatherThreads(K), K == 8 ? 1 : 4) lensBlendGatherKernel(const __grid_constant__ LensBlendGatherParams p, int numTiles) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  LensBlendPositions<BARREL> pos;
   if constexpr (K >= 2) {
     stageWeights<K>(p.weights, smem);
     __syncthreads();  // (no tile synchronises after this)
@@ -267,6 +331,14 @@ cudaError_t launchLensGather(LensGatherParams p, int numSMs, cudaStream_t stream
     constexpr int K = decltype(k)::value;
     constexpr bool B = decltype(barrel)::value;
     return launchPositionsK<K, lensGatherKernel<K, B>, LensPositions<B>>(p, numTiles, numSMs, stream);
+  });
+}
+
+cudaError_t launchLensBlendGather(LensBlendGatherParams p, int numSMs, cudaStream_t stream) {
+  return launchTiles(p, barrelLayout(p.plane[0].geometry.outputLayout), [&](auto k, auto barrel, int numTiles) {
+    constexpr int K = decltype(k)::value;
+    constexpr bool B = decltype(barrel)::value;
+    return launchPositionsK<K, lensBlendGatherKernel<K, B>, LensBlendPositions<B>>(p, numTiles, numSMs, stream);
   });
 }
 

@@ -219,6 +219,10 @@ def load(path: os.PathLike | None = None):
     L.T360B200_lensMap.argtypes = [C.POINTER(FrameTransformContext), C.POINTER(T360LensRig), C.POINTER(T360Orientation)] + [ci] * 4 + [vp]
     L.T360B200_transformFrameLensAsync.restype = ci
     L.T360B200_transformFrameLensAsync.argtypes = [vp, C.POINTER(T360LensRig), C.POINTER(T360Orientation), ci, vp, vp] + [vp] * 6 + [vp]
+    L.T360B200_lensBlendMaps.restype = ci
+    L.T360B200_lensBlendMaps.argtypes = [C.POINTER(FrameTransformContext), C.POINTER(T360LensRig), C.c_float, C.POINTER(T360Orientation)] + [ci] * 4 + [vp] * 3
+    L.T360B200_transformFrameLensBlendAsync.restype = ci
+    L.T360B200_transformFrameLensBlendAsync.argtypes = [vp, C.POINTER(T360LensRig), C.c_float, C.POINTER(T360Orientation), ci, vp, vp] + [vp] * 6 + [vp]
     L.T360B200_setPinHostPlanes.restype = None
     L.T360B200_setPinHostPlanes.argtypes = [vp, ci]
     L.T360B200_debugTrace.restype = None
@@ -251,7 +255,7 @@ EXPORTED_SYMBOLS = [
     "T360B200_lowPassPlaneAsync", "T360B200_reconfigure", "T360B200_reconfigureAsync", "T360B200_reconfigureWait",
     "T360B200_transformFrameViewAsync", "T360B200_viewSamples",
     "T360B200_transformFrameOrientedAsync", "T360B200_orientedSamples", "T360B200_transformFramePoseAsync", "T360B200_poseSamples",
-    "T360B200_lensMap", "T360B200_transformFrameLensAsync",
+    "T360B200_lensMap", "T360B200_transformFrameLensAsync", "T360B200_lensBlendMaps", "T360B200_transformFrameLensBlendAsync",
     "T360B200_setPinHostPlanes", "T360B200_debugTrace", "T360B200_debugTraceRead", "T360B200_synchronize", "T360B200_stream", "T360B200_kernelLaunchCount", "T360B200_planDeviceBytes",
     "T360B200_planTileCounts", "T360B200_deviceCount", "T360B200_version",
 ]
@@ -363,6 +367,17 @@ class VideoFrameTransform:
 
         def call(rig, orientation, stream: int = 0, _keep=keep) -> bool:
             return bool(fn(h, C.byref(rig), C.byref(as_orientation(orientation)), n, pin, pout, *ptrs, stream))
+        return call
+
+    def make_lens_blend_frame_call(self, in_planes, out_planes, dims):
+        """Like make_lens_frame_call, for T360B200_transformFrameLensBlendAsync (a two-lens rig whose seam is feathered
+        across a belt of seam_width degrees): returns a callable f(rig, seam_width, orientation, stream) -> bool that
+        enqueues the whole frame."""
+        n, pin, pout, ptrs, keep = _frame_args(in_planes, out_planes, dims)
+        fn, h = self._lib.T360B200_transformFrameLensBlendAsync, self._h
+
+        def call(rig, seam_width, orientation, stream: int = 0, _keep=keep) -> bool:
+            return bool(fn(h, C.byref(rig), seam_width, C.byref(as_orientation(orientation)), n, pin, pout, *ptrs, stream))
         return call
 
     def generate_map_from_warp(self, map, in_w: int, in_h: int, plan_index: int, border: int = BORDER_WRAP) -> bool:
@@ -595,6 +610,20 @@ def lens_map(ctx: FrameTransformContext, rig: T360LensRig, orientation, in_w, in
                                    out.ctypes.data):
         raise ValueError("T360B200_lensMap refused the arguments (message on stdout)")
     return out
+
+
+def lens_blend_maps(ctx: FrameTransformContext, rig: T360LensRig, seam_width, orientation, in_w, in_h, out_w,
+                    out_h) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """The host twin of one plane of a two-lens rig with a feathered seam (T360B200_lensBlendMaps, no CUDA): (map0, map1,
+    weight).  map0 / map1: float32 [out_h][out_w][2] CV_32FC2 maps of lens 0 / lens 1, NaN where that lens does not
+    contribute; weight: uint16 [out_h][out_w], the weight w (0..256) of lens 1.  cv::remap of each map under
+    BORDER_TRANSPARENT, blended as (a (256 - w) + b w + 128) >> 8 where both are sampled, gives the frame call's plane."""
+    shape = (max(out_h, 0), max(out_w, 0))
+    map0, map1, weight = np.zeros(shape + (2,), np.float32), np.zeros(shape + (2,), np.float32), np.zeros(shape, np.uint16)
+    if not load().T360B200_lensBlendMaps(C.byref(ctx), C.byref(rig), seam_width, C.byref(as_orientation(orientation)), in_w, in_h,
+                                         out_w, out_h, map0.ctypes.data, map1.ctypes.data, weight.ctypes.data):
+        raise ValueError("T360B200_lensBlendMaps refused the arguments (message on stdout)")
+    return map0, map1, weight
 
 
 def remap_table(interpolation_alg: int) -> np.ndarray | None:
