@@ -196,7 +196,7 @@ def groups_of(k):
 
 
 def boundary_targets(k, planes, num_sms):
-    """Launch-list lengths around the static capacity S = N * G * 2 (two jobs per producer warp; kClaimBatch = 1)."""
+    """Launch-list lengths around the static capacity S = N * G * 2 (two static jobs per producer warp)."""
     g = groups_of(k)
     s = num_sms * g * 2
     # (a 3-plane frame has a job per plane at least; for K = 8, where 2G - 1 = 3, it takes 2G: one CTA's producers full)

@@ -1,6 +1,6 @@
 """Builds transform360_b200/lib/libTransform360.so (the drop-in C-ABI library) in-tree with nvcc for sm_90a (H100).
 
-    python -m transform360_b200.build [--force] [--verbose]
+    python -m transform360_b200.build [--force] [--verbose] [--out=PATH]
 
 The artifact name follows the reference's CMake target (Transform360/CMakeLists.txt:9: libTransform360).
 The .so is a build product (git-ignored): build() makes it in the tree.
@@ -37,18 +37,18 @@ def needs_build() -> bool:
     return any(d.stat().st_mtime > t for d in deps)
 
 
-def build(force: bool = False, verbose: bool = False, defines: tuple = (), out: Path | None = None) -> Path:
-    """defines / out: experiment variants (e.g. defines=("T360_CLAIM_BATCH=2",), out=lib/libTransform360_c2.so), loaded
-    with T360B200_LIB=<path>."""
-    out = out or LIB
-    if not force and not defines and not needs_build():
+def build(force: bool = False, verbose: bool = False, out: Path | None = None) -> Path:
+    """out: a library built elsewhere than LIB (e.g. a parent commit's build for an A/B run), loaded with
+    T360B200_LIB=<path>; it is always built."""
+    if out is None and not force and not needs_build():
         return LIB
+    out = out or LIB
     LIB_DIR.mkdir(exist_ok=True)
     # host code: -ffp-contract=off keeps the planner's float sequence identical to the reference's build
     host_flags = "-fPIC,-fvisibility=hidden,-ffp-contract=off,-fno-fast-math,-Wall"
     cmd = [nvcc_path(), *ARCH, "-O3", "-lineinfo", "-std=c++17", "--shared", "-Xcompiler", host_flags,
            "-Xptxas", "-v" if verbose else "-warn-spills", "-I", str(ROOT / "include"), "-I", str(CSRC),
-           *[f"-D{d}" for d in defines], "-o", str(out)] + [str(CSRC / s) for s in SOURCES]
+           "-o", str(out)] + [str(CSRC / s) for s in SOURCES]
     env = dict(os.environ)
     r = subprocess.run(cmd, capture_output=True, text=True, env=env)
     if verbose or r.returncode != 0:
@@ -110,7 +110,6 @@ if __name__ == "__main__":
         install(pre[0])
         print("installed under", pre[0])
         sys.exit(0)
-    defs = tuple(a[2:] for a in sys.argv[1:] if a.startswith("-D"))
     outs = [a.split("=", 1)[1] for a in sys.argv[1:] if a.startswith("--out=")]
-    p = build(force="--force" in sys.argv, verbose="--verbose" in sys.argv, defines=defs, out=Path(outs[0]) if outs else None)
+    p = build(force="--force" in sys.argv, verbose="--verbose" in sys.argv, out=Path(outs[0]) if outs else None)
     print(p)

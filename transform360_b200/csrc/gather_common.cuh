@@ -6,7 +6,6 @@
 #include "kernels.cuh"
 
 #include <atomic>
-#include <cstdlib>
 #include <mutex>
 
 namespace t360 {
@@ -37,10 +36,6 @@ cudaError_t prepare(DeviceLaunchCfg& cfgs, int threads, int smemBytes, LaunchCfg
   if (!cfg.ready) {
     if (smemBytes > 48 * 1024) {
       err = cudaFuncSetAttribute(Kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smemBytes);
-      if (err != cudaSuccess) return err;
-    }
-    if (const char* c = std::getenv("T360B200_SMEM_CARVEOUT")) {  // tuning aid: percent of the L1 / shared-memory array
-      err = cudaFuncSetAttribute(Kern, cudaFuncAttributePreferredSharedMemoryCarveout, std::atoi(c));
       if (err != cudaSuccess) return err;
     }
     err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&cfg.perSM, Kern, threads, smemBytes);

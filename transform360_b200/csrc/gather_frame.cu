@@ -381,27 +381,26 @@ gatherFrameKernel(const __grid_constant__ FrameGatherParams p, StagedParams jobs
       for (int i = 0; i < 4; ++i)
         bulkCopyToShared(wsmem + i * kChunk, reinterpret_cast<const unsigned char*>(p.weightImage) + i * kChunk, kChunk, weightBar);
     }
-    // Jobs are claimed kClaimBatch at a time: the first two batches of a producer are static, every further one comes
-    // from the global counter.  Lane i holds the header of job i of the batch.  The claim runs two batches ahead and the
-    // header loads one, so neither the atomic nor the loads are waited for.  (Asking L2 for a job's records and source
+    // Jobs are claimed one at a time: the first two jobs of a producer are static, every further one comes from the
+    // global counter.  Lane 0 holds the headers of the current and the next job.  The claim runs two jobs ahead and the
+    // header load one, so neither the atomic nor the loads are waited for.  (Asking L2 for a job's records and source
     // box a job ahead with cp.async.bulk.prefetch paid while a job's box was the whole stage buffer; with the boxes cut
     // to the rows a job needs the copies are not waited for either, and the prefetches only add producer work.)
-    const int producer = blockIdx.x * GROUPS + g, dynamicBase = gridDim.x * GROUPS * 2 * kClaimBatch;
-    auto loadBatch = [&](int base) {
+    const int producer = blockIdx.x * GROUPS + g, dynamicBase = gridDim.x * GROUPS * 2;
+    auto loadJob = [&](int i) {
       int4 h = make_int4(0, kJobExit << kJobKindShift, 0, 0);
-      if (lane < kClaimBatch && base + lane < jobs.numTiles) h = __ldg(reinterpret_cast<const int4*>(jobs.tiles) + base + lane);
+      if (lane == 0 && i < jobs.numTiles) h = __ldg(reinterpret_cast<const int4*>(jobs.tiles) + i);
       return h;
     };
-    // (the first TWO batches are static, so that the first job is not held up by the round trip of an atomic)
-    int4 batch = loadBatch(producer * 2 * kClaimBatch);
-    int4 batchNext = loadBatch((producer * 2 + 1) * kClaimBatch);
+    // (the first TWO jobs are static, so that the first job is not held up by the round trip of an atomic)
+    int4 header = loadJob(producer * 2);
+    int4 headerNext = loadJob(producer * 2 + 1);
     asm volatile("griddepcontrol.wait;" ::: "memory");  // earlier kernels on the stream are complete and visible from here on
-    int claimed = 0;  // lane 0: the claim for the batch after next, issued one batch before it is looked at
-    if (lane == 0) claimed = atomicAdd(jobs.claimCounter, kClaimBatch);
+    int claimed = 0;  // lane 0: the claim for the job after next, issued one job before it is looked at
+    if (lane == 0) claimed = atomicAdd(jobs.claimCounter, 1);
     unsigned char* groupBase = smem + L::kWeights + g * L::kGroupBytes;
     uint64_t* full = barBase + g * 2 * S;
     uint64_t* empty = full + S;
-    int pos = 0;
     uint32_t st = 0, phase = 0;  // the stage the next job goes to, and the parity of its use count
     auto advance = [&]() { if (++st == S) { st = 0; phase ^= 1; } };
     auto postEmptyJob = [&](int kind) {  // header only (lane 0)
@@ -409,16 +408,9 @@ gatherFrameKernel(const __grid_constant__ FrameGatherParams p, StagedParams jobs
       mbarArrive(full + st);
     };
     for (;;) {
-      if (pos == kClaimBatch) {  // next batch; start claiming the one after
-        batch = batchNext;
-        pos = 0;
-        batchNext = loadBatch(dynamicBase + __shfl_sync(0xffffffffu, claimed, 0));
-        if (lane == 0) claimed = atomicAdd(jobs.claimCounter, kClaimBatch);
-      }
       int4 h;
-      h.x = __shfl_sync(0xffffffffu, batch.x, pos); h.y = __shfl_sync(0xffffffffu, batch.y, pos);
-      h.z = __shfl_sync(0xffffffffu, batch.z, pos); h.w = __shfl_sync(0xffffffffu, batch.w, pos);
-      ++pos;
+      h.x = __shfl_sync(0xffffffffu, header.x, 0); h.y = __shfl_sync(0xffffffffu, header.y, 0);
+      h.z = __shfl_sync(0xffffffffu, header.z, 0); h.w = __shfl_sync(0xffffffffu, header.w, 0);
       const int kind = (h.y >> kJobKindShift) & kJobKindMask;
       mbarWait(empty + st, phase ^ 1);
       const bool twoStages = kind == kJobClass1 || kind == kJobSeam;
@@ -463,6 +455,9 @@ gatherFrameKernel(const __grid_constant__ FrameGatherParams p, StagedParams jobs
       }
       __syncwarp();
       if (kind == kJobExit) break;
+      header = headerNext;  // next job; start claiming the one after
+      headerNext = loadJob(dynamicBase + __shfl_sync(0xffffffffu, claimed, 0));
+      if (lane == 0) claimed = atomicAdd(jobs.claimCounter, 1);
     }
     // the producer that finishes last re-arms the scheduler for the next launch (claimCounter[0] = claims, [1] = finished)
     if (lane == 0 && atomicAdd(jobs.claimCounter + 1, 1) == (int)(gridDim.x * GROUPS) - 1) {
@@ -576,7 +571,7 @@ cudaError_t launchFrameK(const FrameGatherParams& p, const StagedParams& jobs, c
   LaunchCfg cfg;
   cudaError_t err = prepareFrameK<K, COPIES, GROUPS>(cfg);
   if (err != cudaSuccess) return err;
-  const int grid = std::min(numSMs * cfg.perSM, (jobs.numTiles + GROUPS * 2 * kClaimBatch - 1) / (GROUPS * 2 * kClaimBatch));  // persistent: one CTA per SM
+  const int grid = std::min(numSMs * cfg.perSM, (jobs.numTiles + GROUPS * 2 - 1) / (GROUPS * 2));  // persistent: one CTA per SM
   cudaLaunchConfig_t lc{};
   lc.gridDim = dim3(grid);
   lc.blockDim = dim3(threads);

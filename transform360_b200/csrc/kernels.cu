@@ -138,23 +138,10 @@ __global__ void __launch_bounds__(256) blurTileKernel(BlurParams p) {
 //   sm_90 has no packed single-precision FFMA2 / FADD2 / FMUL2: every operation is a scalar round-to-nearest
 //   instruction, in the oracle's order.
 // ---------------------------------------------------------------------------------------------------
-#ifndef T360_BLUR_I2F
-#define T360_BLUR_I2F 1
-#endif
-#ifndef T360_BLUR_L2_AHEAD
-#define T360_BLUR_L2_AHEAD 2
-#endif
+constexpr int kStripL2RowsAhead = 2;  // the strip kernel asks L2 for the source row this far below the next one
 
 __device__ __forceinline__ float byteToFloat(uint32_t word, int k) {
-#if T360_BLUR_I2F == 1
   return __uint2float_rn((word >> (8 * k)) & 0xFFu);  // I2F.U8 with a byte selector: one instruction, on the XU pipe
-#elif T360_BLUR_I2F == 2
-  if (k & 1) return __uint2float_rn((word >> (8 * k)) & 0xFFu);
-  return __uint_as_float(__byte_perm(word, 0x4B000000u, 0x7440 | k)) - 8388608.0f;
-#else
-  // (float)byte k of word: place it in the low mantissa byte of 8388608.0f, subtract 8388608.0f
-  return __uint_as_float(__byte_perm(word, 0x4B000000u, 0x7440 | k)) - 8388608.0f;
-#endif
 }
 
 // Source bytes of one strip row as seen by one lane.  Interior strips read aligned 32-bit words through the
@@ -285,13 +272,11 @@ __device__ __forceinline__ void stripBody(const StripParams& p, const StripJob& 
 #pragma unroll
         for (int i = 0; i < 4; ++i) raw[i] = rawNext[i];
         if (j + 1 < rowsTotal) StripRowReader<EDGE>(p, job.y0 - HY + j + 1, firstByte).head(rawNext);
-#if T360_BLUR_L2_AHEAD > 0
         {  // rows further down are first touches of DRAM lines as well: ask L2 for them now (no register is held)
-          const int yAhead = min(max(job.y0 - HY + j + 1 + T360_BLUR_L2_AHEAD, 0), p.height - 1);
+          const int yAhead = min(max(job.y0 - HY + j + 1 + kStripL2RowsAhead, 0), p.height - 1);
           const uint8_t* ahead = p.src + (size_t)yAhead * p.srcPitch + max(firstByte, 0);
           asm volatile("prefetch.global.L2 [%0];" ::"l"(ahead));
         }
-#endif
         stripRow<EDGE>(p, job, rd, raw, R[u]);
         if (j >= 2 * HY) {
           // centre row is the one computed HY steps ago: ring slot (u - HY) mod L
@@ -324,21 +309,13 @@ __device__ __forceinline__ void stripBody(const StripParams& p, const StripJob& 
   }
 }
 
-#ifndef T360_BLUR_PDL
-#define T360_BLUR_PDL 0
-#endif
-#ifndef T360_BLUR_MINBLOCKS
-#define T360_BLUR_MINBLOCKS 6  // H100 at 700 W: 80 registers (with spills), 142.4 us per cfg3 frame; 4 blocks 144.4 us, 3 blocks 157.2 us
-#endif
+// Blocks per SM the strip kernel is compiled for.  H100 at 700 W: 80 registers (with spills), 142.4 us per cfg3 frame;
+// 4 blocks 144.4 us, 3 blocks 157.2 us
+constexpr int kStripMinBlocks = 6;
 // MULTI: the jobs name planes 0..2 in `edge`; otherwise every job is plane 0's (no per-job plane selection: as many
 // registers and spills as a kernel written for one plane)
 template <int HY, bool MULTI>
-__global__ void __launch_bounds__(128, T360_BLUR_MINBLOCKS) blurFrameStripKernel(const __grid_constant__ FrameStripParams fp) {
-#if T360_BLUR_PDL
-  // the frame gather that follows on the stream may place its CTAs on SMs this grid has already left and run its
-  // prologue there (it waits for this grid's completion before it touches the planes)
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-#endif
+__global__ void __launch_bounds__(128, kStripMinBlocks) blurFrameStripKernel(const __grid_constant__ FrameStripParams fp) {
   const int job = blockIdx.x * 4 + (threadIdx.x >> 5);
   if (job >= fp.numJobs) return;
   const StripJob j = fp.jobs[job];

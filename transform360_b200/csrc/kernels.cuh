@@ -25,7 +25,7 @@ struct GatherParams {
 
 // ---- the persistent frame gather (gatherFrameKernel) -------------------------------------------------------------
 // One CTA per SM: gatherGroups(k) GROUPS of 8 consumer warps + 1 producer warp each, all sharing one copy of the weight
-// tables in shared memory.  A producer claims jobs from the frame's job list (an atomic counter, one job at a time: batches of 2 / 4, T360_CLAIM_BATCH, left groups idle at the end of a frame on the B200, where this
+// tables in shared memory.  A producer claims jobs from the frame's job list (an atomic counter, one job at a time: batches of 2 / 4 left groups idle at the end of a frame on the B200, where this
 // was chosen; not re-measured on the H100),
 // and for every job fills one stage of its group's two-stage ring: the job header (st.shared), the job's
 // compact sampling records (cp.async.bulk) and its source window (ONE cp.async.bulk.tensor.2d box from the
@@ -68,10 +68,6 @@ constexpr int kJobPlaneShift = 28, kJobKindMask = (1 << (kJobPlaneShift - kJobKi
 constexpr int kGroupThreads = 256, kGroupWarps = kGroupThreads / 32;
 // consumer groups per CTA (+ one producer warp): as many as the rings fit beside the weight tables in 227 KB
 __host__ __device__ constexpr int gatherGroups(int k) { return k == 8 ? 2 : 3; }
-#ifndef T360_CLAIM_BATCH
-#define T360_CLAIM_BATCH 1
-#endif
-constexpr int kClaimBatch = T360_CLAIM_BATCH;  // jobs a producer warp claims with one atomic
 constexpr int kGatherTileW = 32, kFrameTileH = 32;  // generic jobs: 32 x 32, four pixels per thread
 // a warp of a 32 x 32 job takes its 32 x 4 pixels in four steps of one 8 x 4 patch each
 constexpr int kTilePatchW = 8, kTilePatchH = 4, kRowsPerPatchStep = 4;

@@ -576,9 +576,6 @@ class VideoFrameTransform {
     const char* e = std::getenv("T360B200_PIN_HOST_PLANES");
     pinHostPlanes_ = e && *e && *e != '0';
     if (const char* m = std::getenv("T360B200_PIPELINE_MIN_BYTES")) pipelineMinBytes_ = std::atoll(m);  // tests: 0 = always
-    if (const char* m = std::getenv("T360B200_PIPELINE_CHUNKS")) pipelineChunks_ = std::atoi(m);       // tuning
-    if (const char* m = std::getenv("T360B200_PIPELINE_BLOCKS")) pipelineBlocks_ = std::atoi(m);
-    if (const char* m = std::getenv("T360B200_PIPELINE_IN_STREAMS")) pipelineInStreams_ = std::atoi(m);
   }
   void setPinHostPlanes(bool on) { pinHostPlanes_ = on; }
 
@@ -626,7 +623,6 @@ class VideoFrameTransform {
       for (PlaneGraph& g : planeGraphs_) cudaGraphExecDestroy(g.exec);
       for (cudaEvent_t e : {graphFork_, graphJoinIn_, graphJoinOut_}) if (e) cudaEventDestroy(e);
       if (copyIn_) cudaStreamDestroy(copyIn_);
-      if (copyIn2_) cudaStreamDestroy(copyIn2_);
       if (copyOut_) cudaStreamDestroy(copyOut_);
       if (stream_) cudaStreamDestroy(stream_);
     }
@@ -765,7 +761,7 @@ class VideoFrameTransform {
       if (!plan) return false;
       {  // the same plan and caller buffers as in an earlier streamed call: replay its graph (no driver query, no set-up)
         std::lock_guard<std::mutex> hostLock(hostCallMu_);
-        if (replayPlaneGraph(*plan, in, out, inW, inH, inPitch, outW, outH, outPitch)) return true;
+        if (PlaneGraph* g = findPlaneGraph(*plan, in, out, inW, inH, inPitch, outW, outH, outPitch)) return replayPlaneGraph(*g);
       }
       const bool inOnDevice = isDevicePointer(in), outOnDevice = isDevicePointer(out);
       if (plan->kernelSize == 0) {  // reference cpp:780-784: message, output untouched, true
@@ -829,23 +825,16 @@ class VideoFrameTransform {
       return c;
     };
     std::vector<std::vector<GatherJob>> byWave(chunks);
-    // Which output rectangles are complete after which wave: 32-row bands of the full width by default (contiguous
-    // copies: a band split into the three faces of a cube-map row finishes earlier per face, but strided rectangle
-    // copies are much slower than whole contiguous bands; T360B200_PIPELINE_BLOCKS > 1 splits anyway).
-    int blocks = 1;
-    for (int nb : {4, 3, 2})
-      if (plan.mapW % (nb * t360::kShareW) == 0 && nb <= pipelineBlocks_) { blocks = nb; break; }
-    const int blockW = plan.mapW / blocks, bands = (plan.mapH + 31) / 32;
-    std::vector<int> complete(static_cast<size_t>(bands) * blocks, 0);
+    // Which output rectangles are complete after which wave: 32-row bands of the full width (contiguous copies: a band
+    // split into the three faces of a cube-map row finishes earlier per face, but strided rectangle copies are much
+    // slower than whole contiguous bands).
+    const int bands = (plan.mapH + 31) / 32;
+    std::vector<int> complete(bands, 0);  // per band: the wave after which it is complete
     for (size_t i = 0; i < plan.hostJobs.size(); ++i) {
       const int c = waveOf(plan.jobNeedRows[i]);
       byWave[c].push_back(plan.hostJobs[i]);
-      const t360::JobRect& r = plan.jobRects[i];  // (a pole-cap job's pixels may spread over several blocks)
-      for (int band = r.y0 / 32; band <= (r.y1 - 1) / 32; ++band)
-        for (int b = r.x0 / blockW; b <= (r.x1 - 1) / blockW; ++b) {
-          int& slot = complete[static_cast<size_t>(band) * blocks + b];
-          slot = std::max(slot, c);
-        }
+      const t360::JobRect& r = plan.jobRects[i];
+      for (int band = r.y0 / 32; band <= (r.y1 - 1) / 32; ++band) complete[band] = std::max(complete[band], c);
     }
     std::vector<GatherJob> all;
     w.waveStart.assign(chunks + 1, 0);
@@ -857,51 +846,52 @@ class VideoFrameTransform {
     w.jobs.reserve(all.size());
     CU(cudaMemcpy(w.jobs.ptr, all.data(), all.size() * sizeof(GatherJob), cudaMemcpyHostToDevice));
     w.rects.assign(chunks, {});
-    for (int b = 0; b < blocks; ++b)
-      for (int band = 0; band < bands;) {  // vertically adjacent bands of a block that complete together: one copy
-        const int c = complete[static_cast<size_t>(band) * blocks + b];
-        int end = band + 1;
-        while (end < bands && complete[static_cast<size_t>(end) * blocks + b] == c) ++end;
-        w.rects[c].push_back(WavePlan::Rect{b * blockW, band * 32, blockW, std::min(plan.mapH, end * 32) - band * 32});
-        band = end;
-      }
+    for (int band = 0; band < bands;) {  // adjacent bands that complete together: one copy
+      const int c = complete[band];
+      int end = band + 1;
+      while (end < bands && complete[end] == c) ++end;
+      w.rects[c].push_back(WavePlan::Rect{0, band * 32, plan.mapW, std::min(plan.mapH, end * 32) - band * 32});
+      band = end;
+    }
     return w;
   }
 
-  static bool isPinnedHost(const void* p) {
-    cudaPointerAttributes a{};
-    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
-      cudaGetLastError();
-      return false;
+  // The graph of an earlier streamed call with this plan, these caller planes and the current staging planes, or nullptr.
+  // Graphs made for replaced plans or staging planes are forgotten first.
+  PlaneGraph* findPlaneGraph(const DevicePlan& plan, const uint8_t* in, const uint8_t* out, int inW, int inH, int inPitch, int outW, int outH,
+                             int outPitch) {
+    PlaneGraph* g = nullptr;
+    for (size_t i = 0; i < planeGraphs_.size();) {
+      PlaneGraph& c = planeGraphs_[i];
+      if (c.stagingIn != stagingIn_.ptr || c.stagingOut != stagingOut_.ptr || c.generation != planGeneration_) {
+        cudaGraphExecDestroy(c.exec);
+        planeGraphs_.erase(planeGraphs_.begin() + static_cast<long>(i));
+        continue;
+      }
+      if (c.plan == &plan && c.in == in && c.out == out && c.inPitch == inPitch && c.outPitch == outPitch && c.inW == inW && c.inH == inH &&
+          c.outW == outW && c.outH == outH)
+        g = &c;
+      ++i;
     }
-    return a.type == cudaMemoryTypeHost;
+    return g;
   }
 
-  bool replayPlaneGraph(const DevicePlan& plan, const uint8_t* in, const uint8_t* out, int inW, int inH, int inPitch, int outW, int outH,
-                        int outPitch) {
-    for (PlaneGraph& c : planeGraphs_) {
-      if (c.plan != &plan || c.in != in || c.out != out || c.inPitch != inPitch || c.outPitch != outPitch || c.generation != planGeneration_ ||
-          c.stagingIn != stagingIn_.ptr || c.stagingOut != stagingOut_.ptr || c.inW != inW || c.inH != inH || c.outW != outW || c.outH != outH)
-        continue;
-      c.lastUse = ++graphClock_;
-      CU(cudaGraphLaunch(c.exec, stream_));
-      t360::countKernelLaunches(c.kernels);
-      CU(cudaStreamSynchronize(stream_));
-      return true;
-    }
-    return false;
+  bool replayPlaneGraph(PlaneGraph& g) {
+    g.lastUse = ++graphClock_;
+    CU(cudaGraphLaunch(g.exec, stream_));
+    t360::countKernelLaunches(g.kernels);
+    CU(cudaStreamSynchronize(stream_));
+    return true;
   }
 
   // reference transformFramePlane for large host planes (same result as the plain path): chunked H2D || gather || D2H
   bool transformHostPlanePipelined(const DevicePlan& plan, uint8_t* in, uint8_t* out, int inW, int inH, int inPitch, int outW, int outH,
                                    int outPitch, int planIndex, int imagePlaneIndex) {
     const long long bytes = static_cast<long long>(inW) * inH;
-    const int chunks = pipelineChunks_ > 1 ? std::min(pipelineChunks_, 32)
-                                           : static_cast<int>(std::min<long long>(8, std::max<long long>(2, bytes / (3ll << 20))));
+    const int chunks = static_cast<int>(std::min<long long>(8, std::max<long long>(2, bytes / (3ll << 20))));
     WavePlan& w = wavePlanFor(plan, planIndex, chunks);
     if (!copyIn_) {
       CU(cudaStreamCreateWithFlags(&copyIn_, cudaStreamNonBlocking));
-      CU(cudaStreamCreateWithFlags(&copyIn2_, cudaStreamNonBlocking));
       CU(cudaStreamCreateWithFlags(&copyOut_, cudaStreamNonBlocking));
       for (cudaEvent_t* e : {&graphFork_, &graphJoinIn_, &graphJoinOut_}) CU(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
     }
@@ -934,7 +924,6 @@ class VideoFrameTransform {
       if (forkJoin) {  // (capture: the side streams become branches of the graph)
         CU(cudaEventRecord(graphFork_, stream_));
         CU(cudaStreamWaitEvent(copyIn_, graphFork_, 0));
-        if (pipelineInStreams_ > 1) CU(cudaStreamWaitEvent(copyIn2_, graphFork_, 0));
         CU(cudaStreamWaitEvent(copyOut_, graphFork_, 0));
       }
       t360::FrameGatherParams fp{};
@@ -944,12 +933,10 @@ class VideoFrameTransform {
       fp.numPlanes = 1;
       for (int c = 0; c < chunks; ++c) {
         const int r0 = c ? w.chunkRowEnd[c - 1] : 0, r1 = w.chunkRowEnd[c];
-        // (with two inbound streams the set-up of band c + 1 hides under the transfer of band c)
-        cudaStream_t inStream = (pipelineInStreams_ > 1 && (c & 1)) ? copyIn2_ : copyIn_;
         if (r1 > r0)
           CU(cudaMemcpy2DAsync(stagingIn_.ptr + static_cast<size_t>(r0) * dInPitch, dInPitch, in + static_cast<size_t>(r0) * inPitch, inPitch, inW,
-                               r1 - r0, cudaMemcpyHostToDevice, inStream));
-        CU(cudaEventRecord(chunkIn_[c], inStream));
+                               r1 - r0, cudaMemcpyHostToDevice, copyIn_));
+        CU(cudaEventRecord(chunkIn_[c], copyIn_));
         CU(cudaStreamWaitEvent(stream_, chunkIn_[c], 0));
         const int n = w.waveStart[c + 1] - w.waveStart[c];
         if (n > 0) {
@@ -965,75 +952,14 @@ class VideoFrameTransform {
         }
       }
       if (forkJoin) {
-        if (pipelineInStreams_ > 1) {  // (the second inbound stream joins through the first)
-          CU(cudaEventRecord(graphJoinIn_, copyIn2_));
-          CU(cudaStreamWaitEvent(copyIn_, graphJoinIn_, 0));
-        }
         CU(cudaEventRecord(graphJoinIn_, copyIn_));
         CU(cudaEventRecord(graphJoinOut_, copyOut_));
         CU(cudaStreamWaitEvent(stream_, graphJoinIn_, 0));
         CU(cudaStreamWaitEvent(stream_, graphJoinOut_, 0));
       }
     };
-    if (std::getenv("T360B200_PIPELINE_TIMING")) {  // tuning aid: the timeline of one streamed call on stdout
-      std::vector<cudaEvent_t> ev(3 * chunks + 1);
-      for (cudaEvent_t& e : ev) CU(cudaEventCreate(&e));
-      CU(cudaStreamSynchronize(stream_));
-      CU(cudaEventRecord(ev[3 * chunks], stream_));
-      CU(cudaStreamWaitEvent(copyIn_, ev[3 * chunks], 0));
-      CU(cudaStreamWaitEvent(copyOut_, ev[3 * chunks], 0));
-      t360::FrameGatherParams fp{};
-      fp.plane[0] = work.view;
-      fp.weightImage = reinterpret_cast<const uint4*>(weightImages_[plan.kernelSize].ptr);
-      fp.kernelSize = plan.kernelSize;
-      fp.numPlanes = 1;
-      for (int c = 0; c < chunks; ++c) {
-        const int r0 = c ? w.chunkRowEnd[c - 1] : 0, r1 = w.chunkRowEnd[c];
-        CU(cudaMemcpy2DAsync(stagingIn_.ptr + static_cast<size_t>(r0) * dInPitch, dInPitch, in + static_cast<size_t>(r0) * inPitch, inPitch, inW,
-                             r1 - r0, cudaMemcpyHostToDevice, copyIn_));
-        CU(cudaEventRecord(ev[3 * c], copyIn_));
-        CU(cudaStreamWaitEvent(stream_, ev[3 * c], 0));
-        const int n = w.waveStart[c + 1] - w.waveStart[c];
-        if (n > 0) {
-          t360::StagedParams jobs{w.jobs.ptr + w.waveStart[c], n, hostLane.claimCounter.ptr, nullptr};
-          CU(t360::launchGatherFrame(fp, jobs, work.maps, numSMs_, stream_, false));
-        }
-        CU(cudaEventRecord(ev[3 * c + 1], stream_));
-        CU(cudaStreamWaitEvent(copyOut_, ev[3 * c + 1], 0));
-        for (const WavePlan::Rect& r : w.rects[c])
-          CU(cudaMemcpy2DAsync(out + static_cast<size_t>(r.y) * outPitch + r.x, outPitch, stagingOut_.ptr + static_cast<size_t>(r.y) * dOutPitch + r.x,
-                               dOutPitch, r.w, r.h, cudaMemcpyDeviceToHost, copyOut_));
-        CU(cudaEventRecord(ev[3 * c + 2], copyOut_));
-      }
-      CU(cudaStreamSynchronize(stream_));
-      CU(cudaStreamSynchronize(copyOut_));
-      std::printf("streamed plane %d (%dx%d -> %dx%d, %d chunks): chunk | H2D done | wave done (jobs) | D2H done (rects, bytes) [us]\n", imagePlaneIndex, inW,
-                  inH, outW, outH, chunks);
-      for (int c = 0; c < chunks; ++c) {
-        float a = 0, b = 0, d = 0;
-        cudaEventElapsedTime(&a, ev[3 * chunks], ev[3 * c]);
-        cudaEventElapsedTime(&b, ev[3 * chunks], ev[3 * c + 1]);
-        cudaEventElapsedTime(&d, ev[3 * chunks], ev[3 * c + 2]);
-        long long bytes = 0;
-        for (const WavePlan::Rect& r : w.rects[c]) bytes += static_cast<long long>(r.w) * r.h;
-        std::printf("  %2d | %7.1f | %7.1f (%5d) | %7.1f (%2zu, %lld)\n", c, a * 1e3, b * 1e3, w.waveStart[c + 1] - w.waveStart[c], d * 1e3,
-                    w.rects[c].size(), bytes);
-      }
-      for (cudaEvent_t e : ev) cudaEventDestroy(e);
-      return true;
-    }
-    if (isPinnedHost(in) && isPinnedHost(out)) {
-      PlaneGraph* g = nullptr;
-      for (size_t i = 0; i < planeGraphs_.size();) {
-        PlaneGraph& c = planeGraphs_[i];
-        if (c.stagingIn != stagingIn_.ptr || c.stagingOut != stagingOut_.ptr || c.generation != planGeneration_) {
-          cudaGraphExecDestroy(c.exec);
-          planeGraphs_.erase(planeGraphs_.begin() + static_cast<long>(i));
-          continue;
-        }
-        if (c.plan == &plan && c.in == in && c.out == out && c.inPitch == inPitch && c.outPitch == outPitch) g = &c;
-        ++i;
-      }
+    if (memoryTypeOf(in) == cudaMemoryTypeHost && memoryTypeOf(out) == cudaMemoryTypeHost) {
+      PlaneGraph* g = findPlaneGraph(plan, in, out, inW, inH, inPitch, outW, outH, outPitch);
       if (!g) {
         if (planeGraphs_.size() >= 24) {  // (a frame pool recycles a handful of buffers; forget the least recently used)
           auto oldest = std::min_element(planeGraphs_.begin(), planeGraphs_.end(), [](const PlaneGraph& a, const PlaneGraph& b) { return a.lastUse < b.lastUse; });
@@ -1060,18 +986,13 @@ class VideoFrameTransform {
         planeGraphs_.push_back(PlaneGraph{&plan, planGeneration_, in, out, inPitch, outPitch, stagingIn_.ptr, stagingOut_.ptr, inW, inH, outW, outH,
                                           kernels, exec, 0});
         g = &planeGraphs_.back();
-        t360::countKernelLaunches(-kernels);  // (counted once while capturing; every replay counts below)
+        t360::countKernelLaunches(-kernels);  // (counted once while capturing; every replay counts)
       }
-      g->lastUse = ++graphClock_;
-      CU(cudaGraphLaunch(g->exec, stream_));
-      t360::countKernelLaunches(g->kernels);
-      CU(cudaStreamSynchronize(stream_));
-      return true;
+      return replayPlaneGraph(*g);
     }
     issue(false);
     CU(cudaStreamSynchronize(stream_));
     CU(cudaStreamSynchronize(copyOut_));
-    if (pipelineInStreams_ > 1) CU(cudaStreamSynchronize(copyIn2_));
     return true;
   }
 
@@ -1489,10 +1410,7 @@ class VideoFrameTransform {
   // in place with cudaHostRegister so that later frames in the same buffer are DMA'd directly.  Opt-in because the
   // caller must not free such a buffer while the transform is alive (it is unregistered in the destructor).
   void pinIfRecurring(const void* ptr, size_t bytes) {
-    if (!pinHostPlanes_ || !ptr || !bytes) return;
-    cudaPointerAttributes a{};
-    if (cudaPointerGetAttributes(&a, ptr) != cudaSuccess) { cudaGetLastError(); return; }
-    if (a.type != cudaMemoryTypeUnregistered) return;
+    if (!pinHostPlanes_ || !ptr || !bytes || memoryTypeOf(ptr) != cudaMemoryTypeUnregistered) return;
     const uintptr_t page = 4096, lo = reinterpret_cast<uintptr_t>(ptr) & ~(page - 1);
     const size_t len = ((reinterpret_cast<uintptr_t>(ptr) + bytes + page - 1) & ~(page - 1)) - lo;
     for (HostRange& r : hostRanges_) {
@@ -1506,13 +1424,19 @@ class VideoFrameTransform {
     if (hostRanges_.size() < 64) hostRanges_.push_back(HostRange{lo, len, 1, false});
   }
 
-  static bool isDevicePointer(const void* p) {
+  // The kind of memory p points into, or -1 (the error cleared) when the runtime cannot tell
+  static int memoryTypeOf(const void* p) {
     cudaPointerAttributes a{};
     if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
       cudaGetLastError();
-      return false;
+      return -1;
     }
-    return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
+    return a.type;
+  }
+
+  static bool isDevicePointer(const void* p) {
+    const int t = memoryTypeOf(p);
+    return t == cudaMemoryTypeDevice || t == cudaMemoryTypeManaged;
   }
 
   const DevicePlan* findPlan(int planIndex, int imagePlaneIndex) {
@@ -2295,12 +2219,10 @@ class VideoFrameTransform {
   DeviceBuffer<uint8_t> weightImages_[9];  // their shared-memory images for the frame kernel
   DeviceBuffer<uint8_t> stagingIn_, stagingOut_;
   std::mutex hostCallMu_;  // the synchronous host-pointer path shares the staging planes and the streams: one call at a time
-  cudaStream_t copyIn_ = nullptr, copyIn2_ = nullptr, copyOut_ = nullptr;
+  cudaStream_t copyIn_ = nullptr, copyOut_ = nullptr;
   std::vector<cudaEvent_t> chunkIn_, waveDone_;
   WavePlan wavePlans_[2];  // plan index 0 / 1
   long long pipelineMinBytes_ = 6ll << 20;
-  int pipelineChunks_ = 0, pipelineBlocks_ = 0;  // 0: automatic
-  int pipelineInStreams_ = 1;
   std::vector<PlaneGraph> planeGraphs_;  // (see PlaneGraph)
   unsigned long long graphClock_ = 0;
   cudaEvent_t graphFork_ = nullptr, graphJoinIn_ = nullptr, graphJoinOut_ = nullptr;
