@@ -336,6 +336,48 @@ def test_frame_entry_point_every_path(name, planes, torch_cuda):
     ft.close()
 
 
+def test_unknown_interpolation_leaves_barrel_outputs_untouched(torch_cuda, capfd):
+    """A barrel plan (BORDER_TRANSPARENT) with an interpolation algorithm outside NEAREST / LINEAR / CUBIC / LANCZOS4 has
+    nothing to gather: like the reference's transformPlane, every planned call prints the message, succeeds and writes
+    nothing, so the pre-fill of a transparent chroma output does not happen either: the synchronous call with device and
+    host planes, the asynchronous plane call and the whole-frame call."""
+    torch = torch_cuda
+    from transform360_b200.stream import FrameTransformer, StreamSpec
+    case = SMALL["barrel"]
+    ctx = t360.make_context(**dict(case["ov"], interpolation_alg=3))
+    spec = StreamSpec(case["inp"][0], case["inp"][1], case["out"][0], case["out"][1])
+    ft = FrameTransformer(ctx, spec)
+    srcs = [co.noise_plane(*spec.plane_dims(p)[:2], plane=p, frame=4) for p in range(3)]
+    pads = [spec.plane_dims(p)[2] + 9 for p in range(3)]
+    patterns = [((np.arange(spec.plane_dims(p)[3] * pads[p]) * 7 + 3 * p + 1) % 251).astype(np.uint8).reshape(-1, pads[p])
+                for p in range(3)]
+    d_in = [_pitched(torch, srcs[p], spec.plane_dims(p)[0] + 5) for p in range(3)]
+    d_out = [torch.from_numpy(patterns[p]).cuda() for p in range(3)]
+    torch.cuda.synchronize()
+
+    def unchanged(what):
+        torch.cuda.synchronize()
+        for p in range(3):
+            assert np.array_equal(d_out[p].cpu().numpy(), patterns[p]), f"{what}: plane {p} was written"
+
+    for p in range(3):
+        iw, ih, ow, oh, idx = spec.plane_dims(p)
+        assert ft.vft.transformFramePlane(d_in[p].data_ptr(), d_out[p].data_ptr(), iw, ih, d_in[p].stride(0), ow, oh, pads[p], idx, p)
+        host_out = patterns[p].copy()
+        assert ft.vft.transformFramePlane(srcs[p].ctypes.data, host_out.ctypes.data, iw, ih, srcs[p].strides[0], ow, oh, pads[p], idx, p)
+        assert np.array_equal(host_out, patterns[p]), f"host plane {p} was written"
+    unchanged("synchronous call")
+    iw, ih, ow, oh, idx = spec.plane_dims(1)
+    assert ft.vft.transform_plane_async(d_in[1].data_ptr(), d_out[1].data_ptr(), iw, ih, d_in[1].stride(0), ow, oh, pads[1], idx)
+    unchanged("asynchronous plane call")
+    assert ft.frame_call([(t.data_ptr(), t.stride(0)) for t in d_in], [(t.data_ptr(), t.stride(0)) for t in d_out])(0)
+    unchanged("frame call")
+    import ctypes
+    ctypes.CDLL(None).fflush(None)  # (the library prints with printf: flush the C stream before reading the captured fd)
+    assert "Could not find interpolation algorithm" in capfd.readouterr().out
+    ft.close()
+
+
 def test_frame_entry_point_survives_map_regeneration(torch_cuda):
     """generateMapForPlane again (other parameters) between frames: the merged job list is rebuilt."""
     torch = torch_cuda

@@ -243,15 +243,24 @@ struct PlaneLane {
   DeviceBuffer<int> claimCounter;                    // dynamic tile scheduler of this lane's gather launch
 };
 
+// Where the gather of one plane writes (dst, at the map's size) and where its result must end up (out, the caller's
+// plane): the same plane, or a lane's plane and the INTER_AREA tables from it to the caller's (see
+// VideoFrameTransform::renderTarget).
+struct PlaneTarget {
+  uint8_t* dst = nullptr;
+  int dstPitch = 0, dstW = 0, dstH = 0;
+  uint8_t* out = nullptr;
+  int outPitch = 0, outW = 0, outH = 0;
+  const DevicePlan::Resize* resize = nullptr;
+};
+
 // What the gather stage of one image plane needs once its source is ready (see VideoFrameTransform::prepareGather).
 struct GatherWork {
   const DevicePlan* plan = nullptr;
   t360::PlaneView view{};
   bool staged = false;                       // TMA-describable: may run in the persistent (per-plane / per-frame) kernel
   CUtensorMap maps[t360::kMaxBoxMaps];
-  uint8_t* finalOut = nullptr;               // where the area resize (if any) delivers
-  int finalPitch = 0, finalW = 0, finalH = 0, imagePlane = 0;
-  const void* resizeTables = nullptr;
+  PlaneTarget target;
 };
 
 // The merged lists of a frame of 2 or 3 planes, built once per plan generation: the gather jobs of every plane in one
@@ -344,8 +353,13 @@ struct StreamSlot {
   std::vector<int> sphereSizes;  // mapW, mapH per plane
 };
 
-constexpr int kPitchAlign = 256;
-inline int alignedPitch(int w) { return (w + kPitchAlign - 1) / kPitchAlign * kPitchAlign; }
+// A w x h scratch plane in buf (a lane's or the staging planes), grown on demand: its pitch, 256-byte aligned
+int scratchPlane(DeviceBuffer<uint8_t>& buf, int w, int h) {
+  constexpr int kPitchAlign = 256;
+  const int pitch = (w + kPitchAlign - 1) / kPitchAlign * kPitchAlign;
+  buf.reserve(static_cast<size_t>(pitch) * h + 64);
+  return pitch;
+}
 
 // The device planes of a whole-frame call: plane p is read from in[p] (inW x inH, inPitch bytes per row) and written to
 // out[p].
@@ -777,26 +791,21 @@ class VideoFrameTransform {
       int dInPitch = inPitch, dOutPitch = outPitch;
       if (!inOnDevice) {
         pinIfRecurring(in, static_cast<size_t>(inPitch) * (inH - 1) + inW);
-        dInPitch = alignedPitch(inW);
-        stagingIn_.reserve(static_cast<size_t>(dInPitch) * inH + 64);
+        dInPitch = scratchPlane(stagingIn_, inW, inH);
         CU(cudaMemcpy2DAsync(stagingIn_.ptr, dInPitch, in, inPitch, inW, inH, cudaMemcpyHostToDevice, stream_));
         dIn = stagingIn_.ptr;
       }
       if (!outOnDevice) {
         pinIfRecurring(out, static_cast<size_t>(outPitch) * (outH - 1) + outW);
-        dOutPitch = alignedPitch(outW);
-        stagingOut_.reserve(static_cast<size_t>(dOutPitch) * outH + 64);
+        dOutPitch = scratchPlane(stagingOut_, outW, outH);
         dOut = stagingOut_.ptr;
-        if (plan->transparent) {
-          // barrel layouts leave unmapped pixels untouched: chroma planes start at 128 (reference cpp:743-747),
-          // the luma plane keeps whatever the caller's buffer holds
-          if (planIndex) CU(cudaMemset2DAsync(dOut, dOutPitch, 128, outW, outH, stream_));
-          else CU(cudaMemcpy2DAsync(dOut, dOutPitch, out, outPitch, outW, outH, cudaMemcpyHostToDevice, stream_));
-        }
-      } else if (plan->transparent && planIndex) {
-        CU(cudaMemset2DAsync(dOut, dOutPitch, 128, outW, outH, stream_));
+        // a transparent luma plane keeps the caller's bytes (renderTarget): they go into the staging plane first
+        if (plan->transparent && !planIndex)
+          CU(cudaMemcpy2DAsync(dOut, dOutPitch, out, outPitch, outW, outH, cudaMemcpyHostToDevice, stream_));
       }
-      if (!enqueue(*plan, dIn, dOut, inW, inH, dInPitch, outW, outH, dOutPitch, stream_, imagePlaneIndex, slotFor(stream_).lanes[0])) return false;
+      if (!enqueue(*plan, planIndex != 0, dIn, dOut, inW, inH, dInPitch, outW, outH, dOutPitch, stream_, imagePlaneIndex,
+                   slotFor(stream_).lanes[0]))
+        return false;
       if (!outOnDevice)
         CU(cudaMemcpy2DAsync(out, outPitch, dOut, dOutPitch, outW, outH, cudaMemcpyDeviceToHost, stream_));
       CU(cudaStreamSynchronize(stream_));
@@ -904,12 +913,11 @@ class VideoFrameTransform {
     }
     pinIfRecurring(in, static_cast<size_t>(inPitch) * (inH - 1) + inW);
     pinIfRecurring(out, static_cast<size_t>(outPitch) * (outH - 1) + outW);
-    const int dInPitch = alignedPitch(inW), dOutPitch = alignedPitch(outW);
-    stagingIn_.reserve(static_cast<size_t>(dInPitch) * inH + 64);
-    stagingOut_.reserve(static_cast<size_t>(dOutPitch) * outH + 64);
+    const int dInPitch = scratchPlane(stagingIn_, inW, inH), dOutPitch = scratchPlane(stagingOut_, outW, outH);
     PlaneLane& hostLane = slotFor(stream_).lanes[0];
     GatherWork work;
-    if (!prepareGather(plan, stagingIn_.ptr, stagingOut_.ptr, inW, inH, dInPitch, outW, outH, dOutPitch, stream_, imagePlaneIndex, hostLane, work))
+    if (!prepareGather(plan, planIndex != 0, stagingIn_.ptr, stagingOut_.ptr, inW, inH, dInPitch, outW, outH, dOutPitch, stream_,
+                       imagePlaneIndex, hostLane, work))
       return false;
     if (!work.staged) {  // the plane cannot be described to the TMA unit after all: plain path
       CU(cudaMemcpy2DAsync(stagingIn_.ptr, dInPitch, in, inPitch, inW, inH, cudaMemcpyHostToDevice, stream_));
@@ -1006,8 +1014,7 @@ class VideoFrameTransform {
       const DevicePlan* plan = findPlan(planIndex, planIndex);
       if (!plan) return false;
       cudaStream_t s = stream ? stream : stream_;
-      if (plan->transparent && planIndex) CU(cudaMemset2DAsync(dOut, outPitch, 128, outW, outH, s));
-      return enqueue(*plan, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, s, planIndex, slotFor(s).lanes[0]);
+      return enqueue(*plan, planIndex != 0, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, s, planIndex, slotFor(s).lanes[0]);
     });
   }
 
@@ -1059,9 +1066,8 @@ class VideoFrameTransform {
       for (int p = numPlanes - 1; p >= 0; --p) {
         cudaStream_t ps = (p && fork) ? lanes_[p].main : s;
         if (p && fork) CU(cudaStreamWaitEvent(ps, frameFork_, 0));
-        if (plans[p]->transparent && p) CU(cudaMemset2DAsync(f.out[p], f.outPitch[p], 128, f.outW[p], f.outH[p], ps));
-        if (!prepareGather(*plans[p], f.in[p], f.out[p], f.inW[p], f.inH[p], f.inPitch[p], f.outW[p], f.outH[p], f.outPitch[p], ps, p, lanes_[p],
-                           work[p], mergedBlur))
+        if (!prepareGather(*plans[p], p > 0, f.in[p], f.out[p], f.inW[p], f.inH[p], f.inPitch[p], f.outW[p], f.outH[p], f.outPitch[p], ps, p,
+                           lanes_[p], work[p], mergedBlur))
           return false;
         allStaged = allStaged && work[p].staged;
       }
@@ -1073,7 +1079,7 @@ class VideoFrameTransform {
             CU(cudaStreamWaitEvent(s, lanes_[p].done, 0));
           }
         gatherFrame(work, numPlanes, s, slot);
-        for (int p = 0; p < numPlanes; ++p) finishGather(work[p], s);
+        for (int p = 0; p < numPlanes; ++p) finishTarget(work[p].target, s);
         return true;
       }
       // some plane needs the general kernel (barrel layouts, nearest, unaligned planes): per-plane launches
@@ -1083,7 +1089,7 @@ class VideoFrameTransform {
         if (p && !fork) CU(cudaStreamWaitEvent(ps, frameFork_, 0));
         if (work[p].plan->kernelSize) {
           gatherPlane(work[p], lanes_[p], ps);
-          finishGather(work[p], ps);
+          finishTarget(work[p].target, ps);
         }
         if (p) CU(cudaEventRecord(lanes_[p].done, ps));
       }
@@ -1163,9 +1169,7 @@ class VideoFrameTransform {
       const bool transparent = border == t360::kBorderTransparent;
       t360::MapGatherParams mp{};
       for (int p = 0; p < f.numPlanes; ++p) {
-        // BORDER_TRANSPARENT leaves a pixel whose anchor tap lies outside the source as it finds it: chroma outputs start at
-        // 128 as in the planned path (reference cpp:743-747), luma outputs keep the caller's bytes
-        if (transparent && p) CU(cudaMemset2DAsync(f.out[p], f.outPitch[p], 128, f.outW[p], f.outH[p], s));
+        renderTarget(nullptr, p > 0, transparent, f.out[p], f.outPitch[p], f.outW[p], f.outH[p], nullptr, s);
         mp.plane[p] = t360::MapPlane{f.in[p], f.out[p], f.inPitch[p], f.outPitch[p], reinterpret_cast<const float2*>(maps[p]), mapPitch[p] / 8,
                                      t360::MapGeometry{f.outW[p], f.outH[p], f.inW[p], f.inH[p]}, 0, 0};
       }
@@ -1204,8 +1208,7 @@ class VideoFrameTransform {
       sphereTablesFor(lens, f.numPlanes, f.outW, f.outH, slot, s, tables, &staged);
       t360::LensGatherParams lp{};
       for (int p = 0; p < f.numPlanes; ++p) {
-        // BORDER_TRANSPARENT: chroma outputs start at 128 as in the planned path, luma outputs keep the caller's bytes
-        if (p) CU(cudaMemset2DAsync(f.out[p], f.outPitch[p], 128, f.outW[p], f.outH[p], s));
+        renderTarget(nullptr, p > 0, /*transparent=*/true, f.out[p], f.outPitch[p], f.outW[p], f.outH[p], nullptr, s);
         lp.plane[p] = orientedPlane(f.in[p], f.inPitch[p], f.out[p], f.outPitch[p],
                                     t360::sphereGeometry(lens, f.outW[p], f.outH[p], f.inW[p], f.inH[p], k), tables[p]);
       }
@@ -1255,32 +1258,15 @@ class VideoFrameTransform {
       for (int p = 0; p < numPlanes; ++p) { src[p] = f.in[p]; srcPitch[p] = f.inPitch[p]; }
       if (ctx.enable_low_pass_filter && !viewLowPass(what, ctx, plans, f, slot, s, src, srcPitch)) return false;
 
-      // render targets: the output, or when its size is not the map's the slot's plane at the map's size (cpp:755-777).
-      // Barrel plans (BORDER_TRANSPARENT) leave a pixel whose anchor tap is outside the source as they find it, so the
-      // targets are pre-filled as in the whole-frame path: chroma outputs with 128 (cpp:743-747), scaled planes with 0 (luma)
-      // or 128 (chroma) (cpp:759-762); luma outputs keep the caller's bytes.
-      uint8_t* dst[kPlaneLanes];
-      int dstPitch[kPlaneLanes];
-      for (int p = 0; p < numPlanes; ++p) {
-        const DevicePlan& plan = *plans[p];
-        dst[p] = f.out[p];
-        dstPitch[p] = f.outPitch[p];
-        if (f.outW[p] != plan.mapW || f.outH[p] != plan.mapH) {
-          const int sp = alignedPitch(plan.mapW);
-          slot.lanes[p].scaled.reserve(static_cast<size_t>(sp) * plan.mapH + 64);
-          dst[p] = slot.lanes[p].scaled.ptr;
-          dstPitch[p] = sp;
-          if (plan.transparent) CU(cudaMemset2DAsync(dst[p], sp, p ? 128 : 0, plan.mapW, plan.mapH, s));
-        } else if (plan.transparent && p) {
-          CU(cudaMemset2DAsync(dst[p], dstPitch[p], 128, f.outW[p], f.outH[p], s));
-        }
-      }
+      PlaneTarget dst[kPlaneLanes];
+      for (int p = 0; p < numPlanes; ++p)
+        dst[p] = renderTarget(plans[p], p > 0, plans[p]->transparent, f.out[p], f.outPitch[p], f.outW[p], f.outH[p], &slot.lanes[p].scaled, s);
       if (ctx.output_layout == LAYOUT_FLAT_FIXED) {
         t360::ViewGatherParams vp{};
         for (int p = 0; p < numPlanes; ++p) {
           const DevicePlan& plan = *plans[p];
-          vp.plane[p] = t360::ViewPlane{src[p], dst[p], srcPitch[p], dstPitch[p], t360::flatGeometry(ctx, plan.mapW, plan.mapH, plan.inW, plan.inH, k),
-                                        0, 0};
+          vp.plane[p] = t360::ViewPlane{src[p], dst[p].dst, srcPitch[p], dst[p].dstPitch,
+                                        t360::flatGeometry(ctx, plan.mapW, plan.mapH, plan.inW, plan.inH, k), 0, 0};
         }
         vp.numPlanes = numPlanes;
         vp.view = t360::FlatView{ctx.fixed_yaw, ctx.fixed_pitch, ctx.fixed_hfov, ctx.fixed_vfov};
@@ -1299,8 +1285,8 @@ class VideoFrameTransform {
         }
         for (int p = 0; p < numPlanes; ++p) {
           const DevicePlan& plan = *plans[p];
-          op.plane[p] = orientedPlane(src[p], srcPitch[p], dst[p], dstPitch[p], t360::sphereGeometry(ctx, plan.mapW, plan.mapH, plan.inW, plan.inH, k),
-                                      tables[p]);
+          op.plane[p] = orientedPlane(src[p], srcPitch[p], dst[p].dst, dst[p].dstPitch,
+                                      t360::sphereGeometry(ctx, plan.mapW, plan.mapH, plan.inW, plan.inH, k), tables[p]);
         }
         op.numPlanes = numPlanes;
         op.rotation = t360::rotationFromAngles(ctx.fixed_yaw, ctx.fixed_pitch, ctx.fixed_roll);
@@ -1309,14 +1295,7 @@ class VideoFrameTransform {
         CU(t360::launchOrientedGather(op, numSMs_, s));
         releaseAfter(staged, s);
       }
-      for (int p = 0; p < numPlanes; ++p) {
-        if (dst[p] == f.out[p]) continue;
-        const DevicePlan& plan = *plans[p];
-        const DevicePlan::Resize& r = resizeFor(plan, f.outW[p], f.outH[p]);
-        t360::AreaParams ap{dst[p], f.out[p], plan.mapW, plan.mapH, dstPitch[p], f.outW[p], f.outH[p], f.outPitch[p],
-                            r.cellW, r.cellH, r.xTaps.ptr, r.xFirst.ptr, r.yTaps.ptr, r.yFirst.ptr, r.xLinear.ptr, r.yLinear.ptr, r.xMax};
-        CU(t360::launchAreaResize(ap, s));
-      }
+      for (int p = 0; p < numPlanes; ++p) finishTarget(dst[p], s);
       return true;
     });
   }
@@ -1635,53 +1614,35 @@ class VideoFrameTransform {
   }
 
   // reference transformPlane (cpp:707-794): [low-pass] -> gather [-> area resize].  Device pointers, asynchronous.
-  bool enqueue(const DevicePlan& plan, const uint8_t* dIn, uint8_t* dOut, int inW, int inH, int inPitch, int outW,
+  bool enqueue(const DevicePlan& plan, bool chroma, const uint8_t* dIn, uint8_t* dOut, int inW, int inH, int inPitch, int outW,
                int outH, int outPitch, cudaStream_t s, int imagePlaneIndex, PlaneLane& lane) {
     GatherWork w;
-    if (!prepareGather(plan, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, s, imagePlaneIndex, lane, w)) return false;
+    if (!prepareGather(plan, chroma, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, s, imagePlaneIndex, lane, w)) return false;
     if (plan.kernelSize == 0) return true;
     gatherPlane(w, lane, s);
-    finishGather(w, s);
+    finishTarget(w.target, s);
     return true;
   }
 
-  // Everything before the gather of one plane: argument checks, the render target, the low-pass stage.
-  bool prepareGather(const DevicePlan& plan, const uint8_t* dIn, uint8_t* dOut, int inW, int inH, int inPitch, int outW,
+  // Everything before the gather of one plane: argument checks, the render target, the low-pass stage.  chroma: the plane
+  // is a chroma plane (plan index != 0).
+  bool prepareGather(const DevicePlan& plan, bool chroma, const uint8_t* dIn, uint8_t* dOut, int inW, int inH, int inPitch, int outW,
                      int outH, int outPitch, cudaStream_t s, int imagePlaneIndex, PlaneLane& lane, GatherWork& w, bool blurDone = false) {
     w.plan = &plan;
-    w.imagePlane = imagePlaneIndex;
     if (plan.kernelSize == 0) {
       std::printf("Could not find interpolation algorithm for plane %d", imagePlaneIndex);  // reference cpp:780-784
       return true;
     }
-    // reference cpp:735-737, 755-777: whenever the requested output size is not the map's (scale factors, or a caller
-    // that asks for another size than it planned), render at the map's size into a plane pre-filled with 0 (plan index
-    // 0) / 128 (others), then cv::resize(INTER_AREA) to the requested size
-    w.finalOut = dOut;
-    w.finalPitch = outPitch;
-    w.finalW = outW;
-    w.finalH = outH;
-    w.resizeTables = nullptr;
-    if (outW != plan.mapW || outH != plan.mapH) {
-      w.resizeTables = &resizeFor(plan, outW, outH);
-      const int sp = alignedPitch(plan.mapW);
-      lane.scaled.reserve(static_cast<size_t>(sp) * plan.mapH + 64);
-      if (plan.transparent) CU(cudaMemset2DAsync(lane.scaled.ptr, sp, planIndexOf(plan) ? 128 : 0, plan.mapW, plan.mapH, s));
-      dOut = lane.scaled.ptr;
-      outPitch = sp;
-      outW = plan.mapW;
-      outH = plan.mapH;
-    }
+    const PlaneTarget& t = w.target = renderTarget(&plan, chroma, plan.transparent, dOut, outPitch, outW, outH, &lane.scaled, s);
     const uint8_t* src = dIn;
     int srcPitch = inPitch;
     if (plan.lowPass) {
-      const int bp = alignedPitch(inW);
-      lane.blurred.reserve(static_cast<size_t>(bp) * inH + 64);
+      const int bp = scratchPlane(lane.blurred, inW, inH);
       if (!blurDone) runLowPass(plan, dIn, lane.blurred.ptr, inW, inH, inPitch, bp, s);
       src = lane.blurred.ptr;
       srcPitch = bp;
     }
-    w.view = t360::PlaneView{src, dOut, reinterpret_cast<const uint4*>(plan.records.ptr), inW, inH, srcPitch, outW, outH, outPitch};
+    w.view = t360::PlaneView{src, t.dst, reinterpret_cast<const uint4*>(plan.records.ptr), inW, inH, srcPitch, t.dstW, t.dstH, t.dstPitch};
     // staged tiles need the plane the plan was made for (their windows were proven in-bounds for it) and a
     // TMA-describable layout (16-byte aligned base and pitch); otherwise every tile takes the general kernel
     w.staged = plan.numJobs > 0 && !plan.transparent && inW == plan.inW && inH == plan.inH;
@@ -1720,8 +1681,7 @@ class VideoFrameTransform {
     const FrameListRefs l = frameLists(plans, f.numPlanes);
     t360::FrameStripParams fp{};
     for (int p = 0; p < f.numPlanes; ++p) {
-      const int bp = alignedPitch(f.inW[p]);
-      lanes[p].blurred.reserve(static_cast<size_t>(bp) * f.inH[p] + 64);
+      const int bp = scratchPlane(lanes[p].blurred, f.inW[p], f.inH[p]);
       fp.plane[p] = {f.in[p], lanes[p].blurred.ptr, f.inW[p], f.inH[p], f.inPitch[p], bp};
     }
     launchLowPass(l.blurLayout, false, l.blurImage, l.blurImage, fp, f.numPlanes, s);
@@ -1809,8 +1769,7 @@ class VideoFrameTransform {
     const uint8_t* dTaps = stageUpload(slot.viewTaps, taps, s, &used[1]);
     t360::FrameStripParams fp{};
     for (int p = 0; p < numPlanes; ++p) {
-      const int bp = alignedPitch(f.inW[p]);
-      slot.lanes[p].blurred.reserve(static_cast<size_t>(bp) * f.inH[p] + 64);
+      const int bp = scratchPlane(slot.lanes[p].blurred, f.inW[p], f.inH[p]);
       src[p] = slot.lanes[p].blurred.ptr;
       srcPitch[p] = bp;
       fp.plane[p] = {f.in[p], slot.lanes[p].blurred.ptr, f.inW[p], f.inH[p], f.inPitch[p], bp};
@@ -1920,12 +1879,34 @@ class VideoFrameTransform {
     CU(t360::launchGatherFrame(fp, jobs, maps, numSMs_, s));
   }
 
-  // What follows the gather: the INTER_AREA down-scale when the map was rendered at a scaled size.
-  void finishGather(const GatherWork& w, cudaStream_t s) {
-    const DevicePlan& plan = *w.plan;
-    if (!w.resizeTables) return;
-    const DevicePlan::Resize& r = *static_cast<const DevicePlan::Resize*>(w.resizeTables);
-    t360::AreaParams ap{w.view.dst, w.finalOut, plan.mapW, plan.mapH, w.view.dstPitch, w.finalW, w.finalH, w.finalPitch,
+  // The render target of one plane's gather into the caller's plane `out`, pre-filled on s (reference transformPlane,
+  // cpp:735-777).  When the caller's size is the map's, the gather writes into `out`; else (scale factors, or a caller that
+  // asks for another size than it planned) into the scratch plane at the map's size, and finishTarget resizes it into `out`
+  // with INTER_AREA.  BORDER_TRANSPARENT (`transparent`) leaves a pixel whose anchor tap lies outside the source as it
+  // finds it, so the target is filled first: `out` with 128 for a chroma plane, nothing for luma (it keeps the caller's
+  // bytes); the scratch plane with 0 (luma) or 128 (chroma).  plan: nullptr for the calls without one, which render at
+  // the output's size (remap, lens rigs).
+  PlaneTarget renderTarget(const DevicePlan* plan, bool chroma, bool transparent, uint8_t* out, int outPitch, int outW, int outH,
+                           DeviceBuffer<uint8_t>* scratch, cudaStream_t s) {
+    PlaneTarget t{out, outPitch, outW, outH, out, outPitch, outW, outH, nullptr};
+    if (plan && (outW != plan->mapW || outH != plan->mapH)) {
+      t.resize = &resizeFor(*plan, outW, outH);
+      t.dstPitch = scratchPlane(*scratch, plan->mapW, plan->mapH);
+      t.dst = scratch->ptr;
+      t.dstW = plan->mapW;
+      t.dstH = plan->mapH;
+      if (transparent) CU(cudaMemset2DAsync(t.dst, t.dstPitch, chroma ? 128 : 0, t.dstW, t.dstH, s));
+    } else if (transparent && chroma) {
+      CU(cudaMemset2DAsync(out, outPitch, 128, outW, outH, s));
+    }
+    return t;
+  }
+
+  // What follows the gather: the INTER_AREA resize when the plane was rendered at the map's size into a scratch plane.
+  void finishTarget(const PlaneTarget& t, cudaStream_t s) {
+    if (!t.resize) return;
+    const DevicePlan::Resize& r = *t.resize;
+    t360::AreaParams ap{t.dst, t.out, t.dstW, t.dstH, t.dstPitch, t.outW, t.outH, t.outPitch,
                         r.cellW, r.cellH, r.xTaps.ptr, r.xFirst.ptr, r.yTaps.ptr, r.yFirst.ptr, r.xLinear.ptr, r.yLinear.ptr, r.xMax};
     CU(t360::launchAreaResize(ap, s));
   }
@@ -2196,13 +2177,6 @@ class VideoFrameTransform {
       const size_t at = slot.sphereAt[p];
       if (at != SIZE_MAX) tables[p] = reinterpret_cast<const float*>(d + at);
     }
-  }
-
-  int planIndexOf(const DevicePlan& plan) {  // the transformMatPlaneIndex a plan was generated for
-    std::lock_guard<std::mutex> lock(mu_);
-    for (auto& kv : plans_)
-      if (&kv.second == &plan) return kv.first;
-    return 0;
   }
 
   FrameTransformContext ctx_;
