@@ -334,6 +334,50 @@ int T360B200_transformFrameLensBlendAsync(VideoFrameTransform* transform, const 
                                           uint8_t* const* deviceOutputs, const int* inputWidths, const int* inputHeights,
                                           const int* inputPitches, const int* outputWidths, const int* outputHeights,
                                           const int* outputPitches, void* cudaStream);
+/* ---- rectilinear views -------------------------------------------------------------------------------
+ * A perspective (pinhole) virtual camera looking into 360-degree or fisheye footage: reframing with pan, tilt, roll and
+ * zoom, or undistortion of a fisheye lens.  The camera is a T360Pose (degrees).  For output pixel (i, j) of a plane of
+ * mapW x mapH (the output plane's own size):
+ *   1. x = (j + 0.5) / mapW, y = (i + 0.5) / mapH (float);
+ *   2. the output eye split of the sphere outputs: a stereo input with output_stereo_format LR or TB gives two views of
+ *      the same pose, side by side (x folded) or stacked (y folded, flipped with vflip); with a mono output, eye 0;
+ *   3. y' = 1 - y;
+ *   4. the ray q = ((2x - 1) tx, (2y' - 1) ty, 1), tx = tan(hfov / 2), ty = tan(vfov / 2), computed in double and stored
+ *      as float.  So hfov and vfov are the full angles between the plane's outer pixel edges, and pixels are square when
+ *      tan(vfov / 2) / tan(hfov / 2) = mapH / mapW;
+ *   5. q rotated by yaw, pitch and roll exactly as the sphere outputs rotate their points: with hfov = vfov = 90 the view
+ *      of an N x N plane is the FRONT face (bottom row, middle) of a 3N x 2N CUBEMAP_32 output of the same orientation;
+ *   6. the input:
+ *      - without a rig, the context's input: CUBEMAP_32 (gnomonic, with input_expand_coef) or, for any other
+ *        input_layout, equirect (u = atan2(x, z) / 2pi + 0.5 of the rotated ray, as the sphere outputs); the input eye
+ *        re-pack of a stereo input, then u inW - 0.5, v inH - 0.5.  Sampled with BORDER_WRAP;
+ *      - with a rig (the rig frame above), the lens with the larger Z and its projection, a hard seam, NaN where no lens
+ *        covers the ray.  Sampled with BORDER_TRANSPARENT: chroma planes are pre-filled with 128, luma keeps the caller's
+ *        bytes where no source pixel lands.
+ * Not read: output_layout, expand_coef, fixed_yaw .. fixed_vfov (the pose replaces them), fixed_cube_offcenter_*,
+ * is_horizontal_offset and both scale factors (each plane renders at its own output size: no INTER_AREA resize); with a rig
+ * also input_layout, input_expand_coef and both stereo formats (the rig is mono).
+ *
+ * Refused, with 0 and a message on stdout before any CUDA call: a NULL pose, a pose field that is not finite, hfov or vfov
+ * outside (0, 179], enable_low_pass_filter != 0, an unknown interpolation_alg, and with a rig every refusal of the lens
+ * calls about the rig itself (numLenses, calibration size, lens fields, distortion). */
+/* Host only, no CUDA: the CV_32FC2 map (float32 [outputHeight][outputWidth][2]; with a rig NaN where uncovered) of one plane
+ * of inputWidth x inputHeight, rig = NULL for the context's input.  T360B200_generateMapFromWarp(map, ..., T360_BORDER_WRAP,
+ * or T360_BORDER_TRANSPARENT with a rig, index) plans it for a fixed pose: every frame entry point, the streamed host path
+ * included, then gives the frames of T360B200_transformFrameRectilinearAsync bit for bit.  Returns 1; 0 (message) for the
+ * refusals above, a NULL context or map, or non-positive sizes. */
+int T360B200_rectilinearMap(const FrameTransformContext* ctx, const T360LensRig* rig, const T360Pose* pose, int inputWidth, int inputHeight,
+                            int outputWidth, int outputHeight, float* map);
+/* One frame of a rectilinear view, every plane in one gather launch: the arguments and the asynchronous contract of
+ * T360B200_transformFrameAsync, plus `rig` (NULL: the context's input) and `pose`, both of which may change every frame.
+ * Needs no plan: it works on a transform that was never planned as on one holding context or warp plans, and does not touch
+ * them.  Takes the reader lock, so it is frame-exact against T360B200_reconfigure and T360B200_reconfigureAsync, and never
+ * synchronises the device.  Returns 1 if everything was enqueued; 0 with a message on stdout, before any CUDA call, for the
+ * refusals above, 0 or more than 3 planes, or an invalid plane description. */
+int T360B200_transformFrameRectilinearAsync(VideoFrameTransform* transform, const T360LensRig* rig, const T360Pose* pose, int numPlanes,
+                                            const uint8_t* const* deviceInputs, uint8_t* const* deviceOutputs, const int* inputWidths,
+                                            const int* inputHeights, const int* inputPitches, const int* outputWidths,
+                                            const int* outputHeights, const int* outputPitches, void* cudaStream);
 /* Opt-in (also: environment T360B200_PIN_HOST_PLANES=1): page-lock pageable caller planes in place the second time
  * the same buffer is seen (cudaHostRegister), so that recycled frame-pool buffers are DMA'd at full PCIe speed.  The
  * caller must keep such buffers alive until VideoFrameTransform_delete. */

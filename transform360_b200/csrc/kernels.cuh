@@ -450,6 +450,21 @@ struct LensBlendGatherParams : LensGatherParams {
 };
 cudaError_t launchLensBlendGather(LensBlendGatherParams p, int numSMs, cudaStream_t stream);
 
+// ---- the per-frame rectilinear gather (view_gather.cu) ---------------------------------------------------------------
+// Perspective views posed per frame (oriented_view.h: rectilinearSample): every pixel computes its pinhole ray from the
+// camera (a column term and a row term, no tables), rotates it and looks it up in the context's input (BORDER_WRAP) or, with
+// a rig, in the lenses (BORDER_TRANSPARENT).  The per-view gather's tiles, threads and taps.
+struct RectilinearGatherParams {
+  OrientedPlane plane[kMaxFramePlanes];  // geometry: sphereGeometry of the context (of lensContext with a rig); no tables
+  int numPlanes;
+  bool lens;                 // the rig's lenses instead of the context's input
+  RectilinearCamera camera;
+  LensRigModel rig;          // read only when lens is set
+  const int16_t* weights;    // device copy of the [1024][k][k] table (nullptr for nearest)
+  int kernelSize;
+};
+cudaError_t launchRectilinearGather(RectilinearGatherParams p, int numSMs, cudaStream_t stream);
+
 // bytes of dynamic shared memory a blur tile of (w x h) with the given tap counts needs
 inline int blurTileSmem(int w, int h, int nkx, int nky) {
   const int hx = nkx / 2, hy = nky / 2;

@@ -286,6 +286,13 @@ T360_HD bool barrelPoint(const SphereGeometry& g, const float* colTab, const flo
   return true;
 }
 
+// q rotated by r: the planner's rotation, its y row negated (cpp:1233-1244)
+T360_HD SphereVec rotateHD(const Rotation& r, const SphereVec& q) {
+  return SphereVec{fAdd(fSub(fMul(q.x, r.xx), fMul(q.y, r.xy)), fMul(q.z, r.xz)),
+                   -fAdd(fSub(fMul(q.x, r.yx), fMul(q.y, r.yy)), fMul(q.z, r.yz)),
+                   fAdd(fSub(fMul(q.x, r.zx), fMul(q.y, r.zy)), fMul(q.z, r.zz))};
+}
+
 // The output half of the chain for output pixel (i, j): pixel centre -> output eye split -> point on the cube / sphere ->
 // off-centre warp -> rotation by r.  *eye: the output eye; *t: the rotated direction (not normalised), the vector the input
 // lookup maps.  Returns false for a barrel dead zone (*t is then not set).  colTab / rowTab: the plan's tables
@@ -323,11 +330,38 @@ T360_HD bool spherePoint(const SphereGeometry& g, const Rotation& r, const float
   }
   if (mapped) {
     if (g.offCentre) warpOffCentreHD(g, q);
-    t->x = fAdd(fSub(fMul(q.x, r.xx), fMul(q.y, r.xy)), fMul(q.z, r.xz));
-    t->y = -fAdd(fSub(fMul(q.x, r.yx), fMul(q.y, r.yy)), fMul(q.z, r.yz));
-    t->z = fAdd(fSub(fMul(q.x, r.zx), fMul(q.y, r.zy)), fMul(q.z, r.zz));
+    *t = rotateHD(r, q);
   }
   return mapped;
+}
+
+// The input lookup of rotated direction t (not normalised) in output eye `eye`: (*u, *v) in the input, re-packed for a
+// stereo input (cpp:863-891, 1278-1300).  EQUIRECT (any input but CUBEMAP_32): atan2f / asinf, and with `barrel` u kept
+// half an input pixel clear of 0 and 1; CUBEMAP_32: gnomonic face coordinates.  Shared by the sphere outputs (sphereSample)
+// and the rectilinear views (rectilinearPosition).
+T360_HD void sphereInputHD(const SphereGeometry& g, bool barrel, bool eye, const SphereVec& t, float* u, float* v) {
+  const float tx = t.x, ty = t.y, tz = t.z;
+  const float n = fSqrt(fAdd(fAdd(fMul(tx, tx), fMul(ty, ty)), fMul(tz, tz)));  // cpp:863-891
+  if (g.cubeInput) {
+    cubeInputHD(g, fDiv(tx, n), fDiv(ty, n), fDiv(tz, n), u, v);
+  } else {
+    const float lon = -libmAtan2f(fDiv(-tx, n), fDiv(tz, n));
+    const float lat = libmAsinf(fDiv(-ty, n));
+#ifdef __CUDA_ARCH__
+    *u = __double2float_rn(__dadd_rn(__ddiv_rn(static_cast<double>(lon), M_PI * 2.0f), 0.5));
+    *v = __double2float_rn(__dadd_rn(__ddiv_rn(static_cast<double>(lat), M_PI), 0.5));
+#else
+    *u = static_cast<float>(lon / (M_PI * 2.0f) + 0.5f);
+    *v = static_cast<float>(lat / M_PI + 0.5f);
+#endif
+    if (barrel) {  // std::min, then std::max, as the ternaries they are: a NaN u stays NaN (cpp:881-886)
+      const float lo = fMul(g.inPixelWidth, 0.5f), hi = fSub(1.0f, lo);
+      *u = hi < *u ? hi : *u;
+      *u = *u < lo ? lo : *u;
+    }
+  }
+  if (g.packTB) *v = packEye(*v, eye);  // cpp:1278-1300
+  else if (g.packLR) *u = packEye(*u, eye);
 }
 
 // The sampling record {col0, rowPhase} of output pixel (i, j), as HostPlan::samples holds it: spherePoint, then the input
@@ -341,30 +375,7 @@ T360_HD void sphereSample(const SphereGeometry& g, const Rotation& r, const floa
   SphereVec t;
   const bool mapped = spherePoint<BARREL>(g, r, colTab, rowTab, i, j, &eye, &t);
   float u = -1.0f, v = 0.0f;  // the dead zone's position, not re-packed (cpp:1304-1306)
-  if (mapped) {
-    const float tx = t.x, ty = t.y, tz = t.z;
-    const float n = fSqrt(fAdd(fAdd(fMul(tx, tx), fMul(ty, ty)), fMul(tz, tz)));  // cpp:863-891
-    if (g.cubeInput) {
-      cubeInputHD(g, fDiv(tx, n), fDiv(ty, n), fDiv(tz, n), &u, &v);
-    } else {
-      const float lon = -libmAtan2f(fDiv(-tx, n), fDiv(tz, n));
-      const float lat = libmAsinf(fDiv(-ty, n));
-#ifdef __CUDA_ARCH__
-      u = __double2float_rn(__dadd_rn(__ddiv_rn(static_cast<double>(lon), M_PI * 2.0f), 0.5));
-      v = __double2float_rn(__dadd_rn(__ddiv_rn(static_cast<double>(lat), M_PI), 0.5));
-#else
-      u = static_cast<float>(lon / (M_PI * 2.0f) + 0.5f);
-      v = static_cast<float>(lat / M_PI + 0.5f);
-#endif
-      if (barrel) {  // std::min, then std::max, as the ternaries they are: a NaN u stays NaN (cpp:881-886)
-        const float lo = fMul(g.inPixelWidth, 0.5f), hi = fSub(1.0f, lo);
-        u = hi < u ? hi : u;
-        u = u < lo ? lo : u;
-      }
-    }
-    if (g.packTB) v = packEye(v, eye);  // cpp:1278-1300
-    else if (g.packLR) u = packEye(u, eye);
-  }
+  if (mapped) sphereInputHD(g, barrel, eye, t, &u, &v);
   int c0, fracX, r0, fracY;
   quantizeAxis(toPixel(u, g.inW), g.kernelSize, &c0, &fracX);
   quantizeAxis(toPixel(v, g.inH), g.kernelSize, &r0, &fracY);
@@ -542,6 +553,60 @@ T360_HD int lensBlendSample(const SphereGeometry& g, const Rotation& r, const Le
     rec[l][1] = r0 * 1024 + fracY * 32 + fracX;
   }
   return w;
+}
+
+// ---- rectilinear views -----------------------------------------------------------------------------------------------
+// A perspective (pinhole) camera in place of the cube / sphere output: output pixel (i, j) of a mapW x mapH plane looks
+// along q = ((2x - 1) tx, (2y' - 1) ty, 1), x and y its centre after the output eye split (as spherePoint), y' = 1 - y,
+// tx = tan(hfov / 2), ty = tan(vfov / 2) (double on the host, stored as float: rectilinearCamera), rotated by the pose as
+// spherePoint rotates its point.  So with hfov = vfov = 90 an N x N view is the FRONT face of a 3N x 2N CUBEMAP_32 output
+// of the same orientation.  The input is the context's (sphereInputHD, BORDER_WRAP) or a lens rig (lensPosition,
+// BORDER_TRANSPARENT).  Only + - * / on the output half, so host and device agree bit for bit.
+struct RectilinearCamera {
+  Rotation r;
+  float tx, ty;  // tan(hfov / 2), tan(vfov / 2)
+};
+
+// Steps 1-5 of the contract for output pixel (i, j): the rotated ray (not normalised) and the output eye.  The geometry's
+// mapW, mapH, splitLR, splitTB and vflip play a part.
+T360_HD SphereVec rectilinearPoint(const SphereGeometry& g, const RectilinearCamera& c, int i, int j, bool* eye) {
+  float x = pixelCentre(j, g.mapW), y = pixelCentre(i, g.mapH);
+  *eye = false;
+  if (g.splitLR) *eye = splitEye(x, false);
+  else if (g.splitTB) *eye = splitEye(y, g.vflip);
+  y = fSub(1.0f, y);
+  const SphereVec q{fMul(fSub(fMul(2.0f, x), 1.0f), c.tx), fMul(fSub(fMul(2.0f, y), 1.0f), c.ty), 1.0f};
+  return rotateHD(c.r, q);
+}
+
+// The CV_32FC2 map entry (*px, *py) of output pixel (i, j) of a rectilinear view: LENS = false the context's input
+// (sphereInputHD, no barrel clamp), LENS = true the rig's hard seam (NaN where no lens covers the ray).
+template <bool LENS>
+T360_HD void rectilinearPosition(const SphereGeometry& g, const RectilinearCamera& c, const LensRigModel& rig, int i, int j, float* px,
+                                 float* py) {
+  bool eye;
+  const SphereVec d = rectilinearPoint(g, c, i, j, &eye);
+  if constexpr (LENS) {
+    lensPosition(rig, d, g.inW, g.inH, px, py);
+  } else {
+    float u, v;
+    sphereInputHD(g, false, eye, d, &u, &v);
+    *px = toPixel(u, g.inW);
+    *py = toPixel(v, g.inH);
+  }
+}
+
+// The sampling record of output pixel (i, j) of a rectilinear view: its map entry quantised as quantizeWarpMap quantises a
+// caller's map, so T360B200_rectilinearMap -> T360B200_generateMapFromWarp plans the records the kernel computes.
+template <bool LENS>
+T360_HD void rectilinearSample(const SphereGeometry& g, const RectilinearCamera& c, const LensRigModel& rig, int i, int j, int32_t* col0,
+                               int32_t* rowPhase) {
+  float px, py;
+  rectilinearPosition<LENS>(g, c, rig, i, j, &px, &py);
+  int r0, fracX, fracY;
+  quantizeAxis(px, g.kernelSize, col0, &fracX);
+  quantizeAxis(py, g.kernelSize, &r0, &fracY);
+  *rowPhase = r0 * 1024 + fracY * 32 + fracX;
 }
 
 // Whether the per-frame orientation chain covers the layouts of `ctx`

@@ -469,17 +469,14 @@ void releaseAfter(UploadRing::Entry* e, cudaStream_t s) {
 }
 
 // ---- fisheye lens rigs (T360B200_lensMap, T360B200_transformFrameLensAsync; oriented_view.h: lensSample) ----------------
-// true, with the reason in *why, when the lens path cannot serve ctx with this rig and orientation
-bool lensRefused(const FrameTransformContext& ctx, const T360LensRig* rig, const T360Orientation* o, std::string* why) {
+// true, with the reason in *why, when the rig's lenses cannot be used (the rig itself, whatever the output)
+bool rigRefused(const T360LensRig* rig, std::string* why) {
   char buf[256];
   auto refuse = [&](const char* fmt, auto... args) {
     std::snprintf(buf, sizeof(buf), fmt, args...);
     *why = buf;
     return true;
   };
-  if (!rig || !o) return refuse("%s", "a NULL rig or orientation");
-  if (!std::isfinite(o->yaw) || !std::isfinite(o->pitch) || !std::isfinite(o->roll))
-    return refuse("the orientation (yaw %g, pitch %g, roll %g) is not finite", o->yaw, o->pitch, o->roll);
   if (rig->numLenses != 1 && rig->numLenses != 2) return refuse("numLenses %d (1 or 2 supported)", rig->numLenses);
   if (rig->calibWidth <= 0 || rig->calibHeight <= 0) return refuse("calibration size %dx%d is not positive", rig->calibWidth, rig->calibHeight);
   for (int i = 0; i < rig->numLenses; ++i) {
@@ -500,11 +497,33 @@ bool lensRefused(const FrameTransformContext& ctx, const T360LensRig* rig, const
                       "the image)", i, L.k[0], L.k[1], L.k[2], L.k[3], t * 180.0 / M_PI, L.maxAngle);
     }
   }
+  return false;
+}
+
+// true, with the reason in *why, when the lens path cannot serve ctx with this rig and orientation
+bool lensRefused(const FrameTransformContext& ctx, const T360LensRig* rig, const T360Orientation* o, std::string* why) {
+  if (!rig || !o) {
+    *why = "a NULL rig or orientation";
+    return true;
+  }
+  if (!std::isfinite(o->yaw) || !std::isfinite(o->pitch) || !std::isfinite(o->roll)) {
+    *why = formatted("the orientation (yaw %g, pitch %g, roll %g) is not finite", o->yaw, o->pitch, o->roll);
+    return true;
+  }
+  if (rigRefused(rig, why)) return true;
   const int layout = ctx.output_layout;
-  if (layout == LAYOUT_FLAT_FIXED || layout < 0 || layout >= LAYOUT_N)
-    return refuse("output_layout %d (a lens rig needs CUBEMAP_32, CUBEMAP_23_OFFCENTER, EAC_32, EQUIRECT, BARREL or BARREL_SPLIT)", layout);
-  if (ctx.enable_low_pass_filter) return refuse("%s", "the low-pass filter is not available for a lens rig (set enable_low_pass_filter = 0)");
-  if (t360::kernelSizeOf(ctx.interpolation_alg) == 0) return refuse("no interpolation algorithm %d", static_cast<int>(ctx.interpolation_alg));
+  if (layout == LAYOUT_FLAT_FIXED || layout < 0 || layout >= LAYOUT_N) {
+    *why = formatted("output_layout %d (a lens rig needs CUBEMAP_32, CUBEMAP_23_OFFCENTER, EAC_32, EQUIRECT, BARREL or BARREL_SPLIT)", layout);
+    return true;
+  }
+  if (ctx.enable_low_pass_filter) {
+    *why = "the low-pass filter is not available for a lens rig (set enable_low_pass_filter = 0)";
+    return true;
+  }
+  if (t360::kernelSizeOf(ctx.interpolation_alg) == 0) {
+    *why = formatted("no interpolation algorithm %d", static_cast<int>(ctx.interpolation_alg));
+    return true;
+  }
   return false;
 }
 
@@ -579,6 +598,50 @@ void forLensPixels(const FrameTransformContext& ctx, const T360Orientation& o, i
   const t360::Rotation r = t360::rotationFromAngles(o.yaw, o.pitch, o.roll);
   for (int i = 0; i < outH; ++i)
     for (int j = 0; j < outW; ++j) point(g, r, colTab, rowTab, i, j, static_cast<size_t>(i) * outW + j);
+}
+
+// ---- rectilinear views (T360B200_rectilinearMap, T360B200_transformFrameRectilinearAsync; oriented_view.h:
+// rectilinearSample) ----------------------------------------------------------------------------------------------------
+// true, with the reason in *why, when a rectilinear view of ctx's input (rig == nullptr) or of the rig cannot be rendered
+// with this pose.  The output layout plays no part: the pose replaces it.
+bool rectilinearRefused(const FrameTransformContext& ctx, const T360LensRig* rig, const T360Pose* pose, std::string* why) {
+  if (!pose) {
+    *why = "a NULL pose";
+    return true;
+  }
+  if (!std::isfinite(pose->yaw) || !std::isfinite(pose->pitch) || !std::isfinite(pose->roll) || !std::isfinite(pose->hfov) ||
+      !std::isfinite(pose->vfov)) {
+    *why = formatted("the pose (yaw %g, pitch %g, roll %g, hfov %g, vfov %g) is not finite", pose->yaw, pose->pitch, pose->roll, pose->hfov,
+                     pose->vfov);
+    return true;
+  }
+  if (!(pose->hfov > 0.0f && pose->hfov <= 179.0f) || !(pose->vfov > 0.0f && pose->vfov <= 179.0f)) {
+    *why = formatted("hfov %g and vfov %g must lie in (0, 179] degrees", pose->hfov, pose->vfov);
+    return true;
+  }
+  if (rig && rigRefused(rig, why)) return true;
+  if (ctx.enable_low_pass_filter) {
+    *why = "the low-pass filter is not available for a rectilinear view (set enable_low_pass_filter = 0)";
+    return true;
+  }
+  if (t360::kernelSizeOf(ctx.interpolation_alg) == 0) {
+    *why = formatted("no interpolation algorithm %d", static_cast<int>(ctx.interpolation_alg));
+    return true;
+  }
+  return false;
+}
+
+// The per-frame constants of a pose: its rotation, and tan(hfov / 2), tan(vfov / 2) in double, stored as float
+t360::RectilinearCamera rectilinearCamera(const T360Pose& pose) {
+  return t360::RectilinearCamera{t360::rotationFromAngles(pose.yaw, pose.pitch, pose.roll),
+                                 static_cast<float>(std::tan(static_cast<double>(pose.hfov) * M_PI / 360.0)),
+                                 static_cast<float>(std::tan(static_cast<double>(pose.vfov) * M_PI / 360.0))};
+}
+
+// The geometry of one outW x outH plane of an inW x inH input in a rectilinear view: ctx's (its stereo formats and input
+// layout, cube-map input_expand_coef), or with a rig lensContext's (mono); no tables
+t360::SphereGeometry rectilinearGeometry(const FrameTransformContext& ctx, bool rig, int inW, int inH, int outW, int outH) {
+  return t360::sphereGeometry(rig ? lensContext(ctx) : ctx, outW, outH, inW, inH, t360::kernelSizeOf(ctx.interpolation_alg));
 }
 
 }  // namespace
@@ -1190,18 +1253,11 @@ class VideoFrameTransform {
   // (T360B200_transformFrameLensBlendAsync: lensBlendSample), the same steps with the blend kernel.
   bool transformFrameLens(const char* what, const T360LensRig* rig, const float* seamWidth, const T360Orientation* o, const FramePlanes& f,
                           cudaStream_t stream) {
-    return guarded(what, [&] {
-      std::shared_lock<std::shared_mutex> config(configMu_);
-      const FrameTransformContext ctx = ctx_;
-      std::string why;
-      if (seamWidth ? lensBlendRefused(ctx, rig, *seamWidth, o, &why) : lensRefused(ctx, rig, o, &why)) {
-        std::printf("%s. Error: %s\n", what, why.c_str());
-        return false;
-      }
+    auto refused = [&](const FrameTransformContext& ctx, std::string* why) {
+      return seamWidth ? lensBlendRefused(ctx, rig, *seamWidth, o, why) : lensRefused(ctx, rig, o, why);
+    };
+    return unplannedFrame(what, stream, refused, [&](const FrameTransformContext& ctx, int k, cudaStream_t s) {
       const FrameTransformContext lens = lensContext(ctx);
-      const int k = t360::kernelSizeOf(ctx.interpolation_alg);
-      const DeviceRestore restoreDevice = ensureDevice();
-      cudaStream_t s = stream ? stream : stream_;
       StreamSlot& slot = slotFor(s);
       const float* tables[kPlaneLanes];
       UploadRing::Entry* staged = nullptr;
@@ -1221,6 +1277,51 @@ class VideoFrameTransform {
       else CU(t360::launchLensGather(lp, numSMs_, s));
       releaseAfter(staged, s);
       return true;
+    });
+  }
+
+  // Whole frame of a rectilinear view (T360B200_transformFrameRectilinearAsync): one gather launch for all planes, every
+  // record computed by rectilinearSample (oriented_view.h), so a pose gives what rectilinearMap -> generateMapFromWarp plans
+  // for it.  rig == nullptr: the context's input under BORDER_WRAP; else the rig's lenses under BORDER_TRANSPARENT, with the
+  // lens call's pre-fill.  Needs no plan and leaves the plans alone; no tables.
+  bool transformFrameRectilinear(const char* what, const T360LensRig* rig, const T360Pose* pose, const FramePlanes& f, cudaStream_t stream) {
+    auto refused = [&](const FrameTransformContext& ctx, std::string* why) { return rectilinearRefused(ctx, rig, pose, why); };
+    return unplannedFrame(what, stream, refused, [&](const FrameTransformContext& ctx, int k, cudaStream_t s) {
+      const bool lens = rig != nullptr;
+      t360::RectilinearGatherParams rp{};
+      for (int p = 0; p < f.numPlanes; ++p) {
+        renderTarget(nullptr, p > 0, lens, f.out[p], f.outPitch[p], f.outW[p], f.outH[p], nullptr, s);
+        rp.plane[p] = orientedPlane(f.in[p], f.inPitch[p], f.out[p], f.outPitch[p],
+                                    rectilinearGeometry(ctx, lens, f.inW[p], f.inH[p], f.outW[p], f.outH[p]), nullptr);
+      }
+      rp.numPlanes = f.numPlanes;
+      rp.lens = lens;
+      rp.camera = rectilinearCamera(*pose);
+      if (lens) rp.rig = lensRigModel(*rig);
+      rp.kernelSize = k;
+      rp.weights = deviceWeights(ctx.interpolation_alg);
+      CU(t360::launchRectilinearGather(rp, numSMs_, s));
+      return true;
+    });
+  }
+
+  // The steps of the per-frame calls that need no plan (lens rigs, rectilinear views): under the reader lock, so frame-exact
+  // against reconfigure and reconfigureAsync, refused(ctx, &why) is asked before any CUDA call (0 and a message prefixed by
+  // `what`); then enqueue(ctx, k, s) sets up the planes and launches the gather on the caller's stream (nullptr: the
+  // transform's).  Nothing here synchronises the device.
+  template <class Refused, class Enqueue>
+  bool unplannedFrame(const char* what, cudaStream_t stream, Refused&& refused, Enqueue&& enqueue) {
+    return guarded(what, [&] {
+      std::shared_lock<std::shared_mutex> config(configMu_);
+      const FrameTransformContext ctx = ctx_;
+      std::string why;
+      if (refused(ctx, &why)) {
+        std::printf("%s. Error: %s\n", what, why.c_str());
+        return false;
+      }
+      const int k = t360::kernelSizeOf(ctx.interpolation_alg);
+      const DeviceRestore restoreDevice = ensureDevice();
+      return enqueue(ctx, k, stream ? stream : stream_);
     });
   }
 
@@ -1885,7 +1986,7 @@ class VideoFrameTransform {
   // with INTER_AREA.  BORDER_TRANSPARENT (`transparent`) leaves a pixel whose anchor tap lies outside the source as it
   // finds it, so the target is filled first: `out` with 128 for a chroma plane, nothing for luma (it keeps the caller's
   // bytes); the scratch plane with 0 (luma) or 128 (chroma).  plan: nullptr for the calls without one, which render at
-  // the output's size (remap, lens rigs).
+  // the output's size (remap, lens rigs, rectilinear views).
   PlaneTarget renderTarget(const DevicePlan* plan, bool chroma, bool transparent, uint8_t* out, int outPitch, int outW, int outH,
                            DeviceBuffer<uint8_t>* scratch, cudaStream_t s) {
     PlaneTarget t{out, outPitch, outW, outH, out, outPitch, outW, outH, nullptr};
@@ -2599,6 +2700,40 @@ T360_API int T360B200_transformFrameLensBlendAsync(VideoFrameTransform* t, const
   FramePlanes f;
   if (!describeFrame(what, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, f)) return 0;
   return t->transformFrameLens(what, rig, &seamWidth, orientation, f, static_cast<cudaStream_t>(stream));
+}
+T360_API int T360B200_rectilinearMap(const FrameTransformContext* ctx, const T360LensRig* rig, const T360Pose* pose, int inW, int inH, int outW,
+                                     int outH, float* map) {
+  const char* what = "Could not compute the rectilinear map";
+  std::string why;
+  if (!ctx) why = "a NULL context";
+  else if (rectilinearRefused(*ctx, rig, pose, &why)) {}
+  else if (!map || inW <= 0 || inH <= 0 || outW <= 0 || outH <= 0) why = "a NULL map or a plane size that is not positive";
+  if (!why.empty()) {
+    std::printf("%s. Error: %s\n", what, why.c_str());
+    return 0;
+  }
+  const t360::SphereGeometry g = rectilinearGeometry(*ctx, rig != nullptr, inW, inH, outW, outH);
+  const t360::RectilinearCamera c = rectilinearCamera(*pose);
+  const t360::LensRigModel model = rig ? lensRigModel(*rig) : t360::LensRigModel{};
+  for (int i = 0; i < outH; ++i)
+    for (int j = 0; j < outW; ++j) {
+      float* at = map + 2 * (static_cast<size_t>(i) * outW + j);
+      if (rig) t360::rectilinearPosition<true>(g, c, model, i, j, at, at + 1);
+      else t360::rectilinearPosition<false>(g, c, model, i, j, at, at + 1);
+    }
+  return 1;
+}
+T360_API int T360B200_transformFrameRectilinearAsync(VideoFrameTransform* t, const T360LensRig* rig, const T360Pose* pose, int numPlanes,
+                                                     const uint8_t* const* dIn, uint8_t* const* dOut, const int* inW, const int* inH,
+                                                     const int* inPitch, const int* outW, const int* outH, const int* outPitch, void* stream) {
+  const char* what = "Could not transform the frame with a rectilinear view";
+  if (!t) {
+    std::printf("%s. Error: a NULL argument\n", what);
+    return 0;
+  }
+  FramePlanes f;
+  if (!describeFrame(what, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, f)) return 0;
+  return t->transformFrameRectilinear(what, rig, pose, f, static_cast<cudaStream_t>(stream));
 }
 T360_API void T360B200_setPinHostPlanes(VideoFrameTransform* t, int enable) { if (t) t->setPinHostPlanes(enable != 0); }
 T360_API void T360B200_debugTrace(VideoFrameTransform* t, int enable) { if (t) t->enableTrace(enable != 0); }

@@ -17,7 +17,9 @@
 //     lensSample), quantised like a map entry.
 //   - a two-lens rig with a feathered seam (LensBlendPositions): both lenses' records and a weight (lensBlendSample); the
 //     tile loop gathers the second record only where the weight blends the two.
-// In all five, the records come from the same host/device functions the planner (or its host twin) uses: bit-identical.
+//   - a rectilinear view (RectilinearPositions): a pinhole ray per pixel, rotated, then the context's input lookup or the
+//     lens model (oriented_view.h: rectilinearSample).
+// In all six, the records come from the same host/device functions the planner (or its host twin) uses: bit-identical.
 #include "gather_common.cuh"
 
 #include <algorithm>
@@ -197,6 +199,19 @@ struct LensBlendPositions {
   }
 };
 
+// A rectilinear view: the pinhole ray, the rotation and the input lookup per pixel, no shared tables.  LENS: the rig's
+// lenses (rectilinearSample<true>) instead of the context's input
+template <bool LENS>
+struct RectilinearPositions {
+  static constexpr int kTableBytes = 0;
+  static constexpr bool kBlend = false;
+  __device__ void beginTile(const RectilinearGatherParams&, const OrientedPlane&, int, int) {}
+  __device__ void beginColumn(int) {}
+  __device__ void record(const RectilinearGatherParams& p, const OrientedPlane& v, int, int, int i, int j, int* col0, int* rowPhase) const {
+    rectilinearSample<LENS>(v.geometry, p.camera, p.rig, i, j, col0, rowPhase);
+  }
+};
+
 template <int K>
 __global__ void __launch_bounds__(gatherThreads(K), K == 8 ? 1 : 4) viewGatherKernel(const __grid_constant__ ViewGatherParams p, int numTiles) {
   extern __shared__ __align__(16) unsigned char smem[];
@@ -252,6 +267,18 @@ __global__ void __launch_bounds__(gatherThreads(K), K == 8 ? 1 : 4) lensBlendGat
     __syncthreads();  // (no tile synchronises after this)
   }
   gatherViewTiles<K, true>(p, numTiles, smem, pos);
+}
+
+// LENS: a lens rig's input with BORDER_TRANSPARENT; else the context's input with BORDER_WRAP
+template <int K, bool LENS>
+__global__ void __launch_bounds__(gatherThreads(K), K == 8 ? 1 : 4) rectilinearGatherKernel(const __grid_constant__ RectilinearGatherParams p, int numTiles) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  RectilinearPositions<LENS> pos;
+  if constexpr (K >= 2) {
+    stageWeights<K>(p.weights, smem);
+    __syncthreads();  // (no tile synchronises after this)
+  }
+  gatherViewTiles<K, LENS>(p, numTiles, smem, pos);
 }
 
 // Instantiation Kern of kernel size K, one CTA per tile up to the occupancy the __launch_bounds__ allow; its shared memory
@@ -339,6 +366,14 @@ cudaError_t launchLensBlendGather(LensBlendGatherParams p, int numSMs, cudaStrea
     constexpr int K = decltype(k)::value;
     constexpr bool B = decltype(barrel)::value;
     return launchPositionsK<K, lensBlendGatherKernel<K, B>, LensBlendPositions<B>>(p, numTiles, numSMs, stream);
+  });
+}
+
+cudaError_t launchRectilinearGather(RectilinearGatherParams p, int numSMs, cudaStream_t stream) {
+  return launchTiles(p, p.lens, [&](auto k, auto lens, int numTiles) {
+    constexpr int K = decltype(k)::value;
+    constexpr bool L = decltype(lens)::value;
+    return launchPositionsK<K, rectilinearGatherKernel<K, L>, RectilinearPositions<L>>(p, numTiles, numSMs, stream);
   });
 }
 

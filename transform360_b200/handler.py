@@ -223,6 +223,10 @@ def load(path: os.PathLike | None = None):
     L.T360B200_lensBlendMaps.argtypes = [C.POINTER(FrameTransformContext), C.POINTER(T360LensRig), C.c_float, C.POINTER(T360Orientation)] + [ci] * 4 + [vp] * 3
     L.T360B200_transformFrameLensBlendAsync.restype = ci
     L.T360B200_transformFrameLensBlendAsync.argtypes = [vp, C.POINTER(T360LensRig), C.c_float, C.POINTER(T360Orientation), ci, vp, vp] + [vp] * 6 + [vp]
+    L.T360B200_rectilinearMap.restype = ci
+    L.T360B200_rectilinearMap.argtypes = [C.POINTER(FrameTransformContext), C.POINTER(T360LensRig), C.POINTER(T360Pose)] + [ci] * 4 + [vp]
+    L.T360B200_transformFrameRectilinearAsync.restype = ci
+    L.T360B200_transformFrameRectilinearAsync.argtypes = [vp, C.POINTER(T360LensRig), C.POINTER(T360Pose), ci, vp, vp] + [vp] * 6 + [vp]
     L.T360B200_setPinHostPlanes.restype = None
     L.T360B200_setPinHostPlanes.argtypes = [vp, ci]
     L.T360B200_debugTrace.restype = None
@@ -256,6 +260,7 @@ EXPORTED_SYMBOLS = [
     "T360B200_transformFrameViewAsync", "T360B200_viewSamples",
     "T360B200_transformFrameOrientedAsync", "T360B200_orientedSamples", "T360B200_transformFramePoseAsync", "T360B200_poseSamples",
     "T360B200_lensMap", "T360B200_transformFrameLensAsync", "T360B200_lensBlendMaps", "T360B200_transformFrameLensBlendAsync",
+    "T360B200_rectilinearMap", "T360B200_transformFrameRectilinearAsync",
     "T360B200_setPinHostPlanes", "T360B200_debugTrace", "T360B200_debugTraceRead", "T360B200_synchronize", "T360B200_stream", "T360B200_kernelLaunchCount", "T360B200_planDeviceBytes",
     "T360B200_planTileCounts", "T360B200_deviceCount", "T360B200_version",
 ]
@@ -378,6 +383,17 @@ class VideoFrameTransform:
 
         def call(rig, seam_width, orientation, stream: int = 0, _keep=keep) -> bool:
             return bool(fn(h, C.byref(rig), seam_width, C.byref(as_orientation(orientation)), n, pin, pout, *ptrs, stream))
+        return call
+
+    def make_rectilinear_frame_call(self, in_planes, out_planes, dims):
+        """Like make_frame_call, for T360B200_transformFrameRectilinearAsync (a perspective view, no plan needed): returns a
+        callable f(pose, stream, rig=None) -> bool that enqueues the whole frame with `pose` (a T360Pose or (yaw, pitch,
+        roll, hfov, vfov)), looking into the context's input, or into `rig` (a T360LensRig) when one is given."""
+        n, pin, pout, ptrs, keep = _frame_args(in_planes, out_planes, dims)
+        fn, h = self._lib.T360B200_transformFrameRectilinearAsync, self._h
+
+        def call(pose, stream: int = 0, rig=None, _keep=keep) -> bool:
+            return bool(fn(h, C.byref(rig) if rig is not None else None, C.byref(as_pose(pose)), n, pin, pout, *ptrs, stream))
         return call
 
     def generate_map_from_warp(self, map, in_w: int, in_h: int, plan_index: int, border: int = BORDER_WRAP) -> bool:
@@ -624,6 +640,24 @@ def lens_blend_maps(ctx: FrameTransformContext, rig: T360LensRig, seam_width, or
                                          out_w, out_h, map0.ctypes.data, map1.ctypes.data, weight.ctypes.data):
         raise ValueError("T360B200_lensBlendMaps refused the arguments (message on stdout)")
     return map0, map1, weight
+
+
+def rectilinear_map(ctx: FrameTransformContext, pose, in_w, in_h, out_w, out_h, rig: T360LensRig | None = None) -> np.ndarray:
+    """The CV_32FC2 map of one plane of a rectilinear view (T360B200_rectilinearMap, no CUDA): float32 [out_h][out_w][2],
+    the source x, y of every output pixel in a plane of in_w x in_h, from the context's input, or from `rig` (NaN where no
+    lens covers the pixel).  generate_map_from_warp(map, in_w, in_h, index, BORDER_WRAP, or BORDER_TRANSPARENT with a rig)
+    plans it for a fixed pose."""
+    out = np.zeros((max(out_h, 0), max(out_w, 0), 2), np.float32)
+    if not load().T360B200_rectilinearMap(C.byref(ctx), C.byref(rig) if rig is not None else None, C.byref(as_pose(pose)), in_w, in_h,
+                                          out_w, out_h, out.ctypes.data):
+        raise ValueError("T360B200_rectilinearMap refused the arguments (message on stdout)")
+    return out
+
+
+def square_pixel_vfov(hfov, width, height) -> float:
+    """The vfov in degrees that gives a width x height rectilinear view with horizontal field of view `hfov` square pixels:
+    tan(vfov / 2) = tan(hfov / 2) height / width."""
+    return float(np.degrees(2.0 * np.arctan(np.tan(np.radians(hfov) / 2.0) * height / width)))
 
 
 def remap_table(interpolation_alg: int) -> np.ndarray | None:
