@@ -30,13 +30,20 @@ struct FlatView {
   float yaw, pitch, hfov, vfov;  // degrees, as FrameTransformContext::fixed_*
 };
 
-// What the FLAT_FIXED chain needs besides the view: the map (scaled output) size, the input plane size, the stereo formats.
-struct FlatGeometry {
+// Everything a position chain needs besides its per-frame constants (oriented_view.h: sphereGeometry).  The FLAT_FIXED
+// chain reads the map (scaled output) size, the input plane size, the kernel size and the stereo fields.
+struct SphereGeometry {
   int mapW, mapH, inW, inH;
-  int kernelSize;       // 1 (nearest), 2, 4, 8
-  bool splitLR, splitTB;  // the output holds two eyes side by side / stacked (only when the input is stereo)
+  int kernelSize;            // 1 (nearest), 2, 4, 8
+  bool splitLR, splitTB;     // the output holds two eyes side by side / stacked (only when the input is stereo)
   bool vflip;
-  bool packLR, packTB;    // the input holds two eyes side by side / stacked
+  bool packLR, packTB;       // the input holds two eyes side by side / stacked
+  bool cubeInput;            // input_layout CUBEMAP_32 (else treated as EQUIRECT, as the planner does)
+  bool offCentre, horizontalOffset;
+  int outputLayout;
+  float expand, inputExpand;  // expand_coef, input_expand_coef
+  float ox, oy, oz;           // fixed_cube_offcenter_*
+  float inPixelWidth;         // 1.0f / inW, doubled for a side-by-side input: barrel outputs keep u half of it clear of 0 and 1
 };
 
 T360_HD float fAdd(float a, float b) {
@@ -152,7 +159,7 @@ T360_HD void quantizeAxis(float f, int k, int* first, int* frac) {
 struct FlatColumn {
   int col0, fracX;
 };
-T360_HD FlatColumn flatColumn(const FlatView& v, const FlatGeometry& g, int j, bool fold, bool eye) {
+T360_HD FlatColumn flatColumn(const FlatView& v, const SphereGeometry& g, int j, bool fold, bool eye) {
   float x = pixelCentre(j, g.mapW);
   if (g.splitLR) eye = splitEye(x, false);
   float u = flatLon(v, x, fold);
@@ -161,7 +168,7 @@ T360_HD FlatColumn flatColumn(const FlatView& v, const FlatGeometry& g, int j, b
   quantizeAxis(toPixel(u, g.inW), g.kernelSize, &c.col0, &c.fracX);
   return c;
 }
-T360_HD bool flatColumnEye(const FlatGeometry& g, int j) {
+T360_HD bool flatColumnEye(const SphereGeometry& g, int j) {
   float x = pixelCentre(j, g.mapW);
   return g.splitLR && splitEye(x, false);
 }
@@ -172,7 +179,7 @@ struct FlatRow {
   int rowPart;
   bool fold, eye;
 };
-T360_HD FlatRow flatRow(const FlatView& v, const FlatGeometry& g, int i, bool columnEye) {
+T360_HD FlatRow flatRow(const FlatView& v, const SphereGeometry& g, int i, bool columnEye) {
   float y = pixelCentre(i, g.mapH);
   FlatRow r;
   r.eye = g.splitTB ? splitEye(y, g.vflip) : columnEye;
@@ -185,7 +192,7 @@ T360_HD FlatRow flatRow(const FlatView& v, const FlatGeometry& g, int i, bool co
 }
 
 // The sampling record {col0, rowPhase} of output pixel (i, j), as HostPlan::samples holds it.
-T360_HD void flatSample(const FlatView& v, const FlatGeometry& g, int i, int j, int32_t* col0, int32_t* rowPhase) {
+T360_HD void flatSample(const FlatView& v, const SphereGeometry& g, int i, int j, int32_t* col0, int32_t* rowPhase) {
   const bool colEye = flatColumnEye(g, j);
   const FlatRow r = flatRow(v, g, i, colEye);
   const FlatColumn c = flatColumn(v, g, j, r.fold, r.eye);

@@ -355,20 +355,45 @@ cudaError_t launchBlurDirect(const BlurParams& p, cudaStream_t stream);  // any 
 unsigned long long kernelLaunchCount();
 void countKernelLaunches(long long n);  // kernels launched through a replayed CUDA graph
 
-// ---- the per-view gather (view_gather.cu) ---------------------------------------------------------------------------
-// FLAT_FIXED frames whose view (yaw, pitch, hfov, vfov) is a launch parameter: the kernel computes every sampling record
-// itself (flat_view.h), so it needs no sampling plan.  One launch gathers every plane of the frame; BORDER_WRAP only.
-struct ViewPlane {
+// ---- the per-frame gathers (view_gather.cu) ------------------------------------------------------------------------
+// Frames rendered without a sampling plan: the kernel computes every pixel's sampling record itself from per-frame
+// constants passed with the launch, so nothing is re-planned when they change.  One launch gathers every plane of the
+// frame.  The source names where a record comes from:
+//   kView         FLAT_FIXED views (yaw, pitch, hfov, vfov: view; flat_view.h), BORDER_WRAP;
+//   kSphere       every other layout with an orientation (rotation) and the plan's view-independent tables
+//                 (oriented_view.h: sphereSample), BORDER_WRAP, or BORDER_TRANSPARENT for BARREL and BARREL_SPLIT;
+//   kMap          the caller's CV_32FC2 map of each plane, quantised as quantizeWarpMap does (quantizeAxis), BORDER_WRAP
+//                 or BORDER_TRANSPARENT (transparent);
+//   kLens         a fisheye lens rig (rotation, rig; oriented_view.h: lensSample) to a sphere output, with the output
+//                 layout's tables, BORDER_TRANSPARENT;
+//   kLensBlend    a two-lens rig with the seam feathered across a belt (rotation, rig, seamScale; lensBlendSample): every
+//                 pixel gathers the lens that carries it (lens 0 unless the weight w of lens 1 is 256), and a second time,
+//                 lens 1, only where both carry weight; the two values are blended as (a (256 - w) + b w + 128) >> 8;
+//   kRectilinear  perspective views posed per frame (camera; rectilinearSample): a pinhole ray per pixel, no tables, looked
+//                 up in the context's input (BORDER_WRAP) or, with lens set, in the rig's lenses (BORDER_TRANSPARENT).
+enum class PerFrameSource { kView, kSphere, kMap, kLens, kLensBlend, kRectilinear };
+struct PerFramePlane {
   const uint8_t* src;  // (blurred) input plane, geometry.inW x geometry.inH
   uint8_t* dst;        // render target, geometry.mapW x geometry.mapH
   int srcPitch, dstPitch;
-  FlatGeometry geometry;
-  int tilesX, firstTile;  // filled by launchViewGather
+  SphereGeometry geometry;  // (kMap reads the four sizes only)
+  const float* colTable;    // sphere tables (buildSphereTables): column entries, then row entries (nullptr: none)
+  const float* rowTable;
+  int tilesX, firstTile;    // filled by launchPerFrameGather
+  const float2* map;        // kMap: [mapH][mapPitch] (x, y) source positions
+  int mapPitch;             // in float2
 };
-struct ViewGatherParams {
-  ViewPlane plane[kMaxFramePlanes];
+// The per-frame constants a source does not read stay zero.
+struct PerFrameGatherParams {
+  PerFramePlane plane[kMaxFramePlanes];
   int numPlanes;
   FlatView view;
+  Rotation rotation;
+  LensRigModel rig;
+  RectilinearCamera camera;
+  float seamScale;   // s = 1 / (2 seamWidth), seamWidth in radians
+  bool transparent;  // kMap: BORDER_TRANSPARENT instead of BORDER_WRAP
+  bool lens;         // kRectilinear: the rig's lenses instead of the context's input
   const int16_t* weights;  // device copy of the [1024][k][k] table (nullptr for nearest)
   int kernelSize;
 };
@@ -376,94 +401,8 @@ struct ViewGatherParams {
 // kViewRowsPerThread of its rows
 constexpr int kViewRowsPerThread = 8;
 __host__ __device__ constexpr int viewTileRows(int k) { return gatherThreads(k) / 32 * kViewRowsPerThread; }
-cudaError_t launchViewGather(ViewGatherParams p, int numSMs, cudaStream_t stream);
-
-// ---- the per-frame orientation gather (view_gather.cu) --------------------------------------------------------------
-// Frames of every layout but FLAT_FIXED whose orientation (yaw, pitch, roll) is a launch parameter, as its rotation
-// coefficients: the kernel computes every pixel's sampling record (oriented_view.h), with the plan's view-independent
-// tables.  Same tiles, threads and taps as the per-view gather; BORDER_WRAP, or BORDER_TRANSPARENT for BARREL and
-// BARREL_SPLIT (chosen from the planes' output layout).
-struct OrientedPlane {
-  const uint8_t* src;  // (blurred) input plane, geometry.inW x geometry.inH
-  uint8_t* dst;        // render target, geometry.mapW x geometry.mapH
-  int srcPitch, dstPitch;
-  SphereGeometry geometry;
-  const float* colTable;  // the plan's tables (buildSphereTables): column entries, then row entries (nullptr: none)
-  const float* rowTable;
-  int tilesX, firstTile;  // filled by launchOrientedGather
-};
-struct OrientedGatherParams {
-  OrientedPlane plane[kMaxFramePlanes];
-  int numPlanes;
-  Rotation rotation;
-  const int16_t* weights;  // device copy of the [1024][k][k] table (nullptr for nearest)
-  int kernelSize;
-};
-cudaError_t launchOrientedGather(OrientedGatherParams p, int numSMs, cudaStream_t stream);
-
-// ---- the per-frame warp-map gather (view_gather.cu) -----------------------------------------------------------------
-// Frames remapped through the caller's own CV_32FC2 map, one per plane and of the output plane's size, in device memory:
-// the kernel converts every pixel's map entry into its sampling record with quantizeAxis (flat_view.h), as quantizeWarpMap
-// does for a planned map.  Same tiles, threads and taps as the per-view gather; BORDER_WRAP or BORDER_TRANSPARENT.
-struct MapGeometry {
-  int mapW, mapH, inW, inH;
-};
-struct MapPlane {
-  const uint8_t* src;  // input plane, geometry.inW x geometry.inH
-  uint8_t* dst;        // output plane, geometry.mapW x geometry.mapH
-  int srcPitch, dstPitch;
-  const float2* map;   // [mapH][mapPitch] (x, y) source positions
-  int mapPitch;        // in float2
-  MapGeometry geometry;
-  int tilesX, firstTile;  // filled by launchMapGather
-};
-struct MapGatherParams {
-  MapPlane plane[kMaxFramePlanes];
-  int numPlanes;
-  bool transparent;
-  const int16_t* weights;  // device copy of the [1024][k][k] table (nullptr for nearest)
-  int kernelSize;
-};
-cudaError_t launchMapGather(MapGatherParams p, int numSMs, cudaStream_t stream);
-
-// ---- the per-frame lens gather (view_gather.cu) ----------------------------------------------------------------------
-// Frames of a fisheye lens rig to a sphere output (every layout but FLAT_FIXED) with the orientation and the rig as launch
-// parameters: every pixel runs spherePoint and the lens model (oriented_view.h: lensSample), with the output layout's
-// tables built on the host.  Same tiles, threads and taps as the per-view gather; BORDER_TRANSPARENT.
-struct LensGatherParams {
-  OrientedPlane plane[kMaxFramePlanes];  // geometry: the lens context's (sphereGeometry of lensContext), inW / inH the plane's
-  int numPlanes;
-  Rotation rotation;
-  LensRigModel rig;
-  const int16_t* weights;  // device copy of the [1024][k][k] table (nullptr for nearest)
-  int kernelSize;
-};
-cudaError_t launchLensGather(LensGatherParams p, int numSMs, cudaStream_t stream);
-
-// ---- the per-frame lens blend (view_gather.cu) -----------------------------------------------------------------------
-// Frames of a two-lens rig with the seam feathered across a belt (oriented_view.h: lensBlendSample): every pixel computes
-// both lenses' records and the weight of lens 1, gathers the lens that carries it (lens 0 unless w = 256), and a second
-// time, lens 1, only where both carry weight; the two values are blended as (a (256 - w) + b w + 128) >> 8.  The lens
-// gather's tiles, threads, taps and BORDER_TRANSPARENT.
-struct LensBlendGatherParams : LensGatherParams {
-  float seamScale;  // s = 1 / (2 seamWidth), seamWidth in radians
-};
-cudaError_t launchLensBlendGather(LensBlendGatherParams p, int numSMs, cudaStream_t stream);
-
-// ---- the per-frame rectilinear gather (view_gather.cu) ---------------------------------------------------------------
-// Perspective views posed per frame (oriented_view.h: rectilinearSample): every pixel computes its pinhole ray from the
-// camera (a column term and a row term, no tables), rotates it and looks it up in the context's input (BORDER_WRAP) or, with
-// a rig, in the lenses (BORDER_TRANSPARENT).  The per-view gather's tiles, threads and taps.
-struct RectilinearGatherParams {
-  OrientedPlane plane[kMaxFramePlanes];  // geometry: sphereGeometry of the context (of lensContext with a rig); no tables
-  int numPlanes;
-  bool lens;                 // the rig's lenses instead of the context's input
-  RectilinearCamera camera;
-  LensRigModel rig;          // read only when lens is set
-  const int16_t* weights;    // device copy of the [1024][k][k] table (nullptr for nearest)
-  int kernelSize;
-};
-cudaError_t launchRectilinearGather(RectilinearGatherParams p, int numSMs, cudaStream_t stream);
+// (every plane of a frame has the same output layout)
+cudaError_t launchPerFrameGather(PerFrameGatherParams p, PerFrameSource source, int numSMs, cudaStream_t stream);
 
 // bytes of dynamic shared memory a blur tile of (w x h) with the given tap counts needs
 inline int blurTileSmem(int w, int h, int nkx, int nky) {

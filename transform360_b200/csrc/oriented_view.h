@@ -62,21 +62,6 @@ inline float barrelSplitYaw(float x, int half, float e) {                       
 }
 inline float barrelSplitPitch(float y, int half, float e) { return static_cast<float>((y - 0.25f - 0.5f * half) * e * M_PI); }
 
-// Everything the chain needs besides the orientation and the tables.
-struct SphereGeometry {
-  int mapW, mapH, inW, inH;
-  int kernelSize;            // 1 (nearest), 2, 4, 8
-  int outputLayout;          // any but LAYOUT_FLAT_FIXED
-  bool cubeInput;            // input_layout CUBEMAP_32 (else treated as EQUIRECT, as the planner does)
-  bool splitLR, splitTB;     // the output holds two eyes side by side / stacked (only when the input is stereo)
-  bool vflip;
-  bool packLR, packTB;       // the input holds two eyes side by side / stacked
-  bool offCentre, horizontalOffset;
-  float expand, inputExpand;  // expand_coef, input_expand_coef
-  float ox, oy, oz;           // fixed_cube_offcenter_*
-  float inPixelWidth;         // 1.0f / inW, doubled for a side-by-side input: barrel outputs keep u half of it clear of 0 and 1
-};
-
 T360_HD bool barrelLayout(int layout) { return layout == LAYOUT_BARREL || layout == LAYOUT_BARREL_SPLIT; }
 
 // Per-plan tables (buildSphereTables), column entries followed by row entries:
@@ -406,14 +391,6 @@ inline SphereGeometry sphereGeometry(const FrameTransformContext& ctx, int mapW,
   g.inPixelWidth = 1.0f / inW;  // cpp:528-531, as buildWarpMap
   if (g.packLR) g.inPixelWidth *= 2;
   return g;
-}
-
-// The FLAT_FIXED geometry of a plan for `ctx` (flat_view.h), as sphereGeometry
-inline FlatGeometry flatGeometry(const FrameTransformContext& ctx, int mapW, int mapH, int inW, int inH, int kernelSize) {
-  const bool stereoIn = ctx.input_stereo_format != STEREO_FORMAT_MONO;
-  return FlatGeometry{mapW, mapH, inW, inH, kernelSize, stereoIn && ctx.output_stereo_format == STEREO_FORMAT_LR,
-                      stereoIn && ctx.output_stereo_format == STEREO_FORMAT_TB, ctx.vflip != 0, ctx.input_stereo_format == STEREO_FORMAT_LR,
-                      ctx.input_stereo_format == STEREO_FORMAT_TB};
 }
 
 // ---- fisheye lens input ---------------------------------------------------------------------------------------------

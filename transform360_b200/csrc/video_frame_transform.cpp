@@ -447,25 +447,41 @@ std::string withFields(FrameTransformContext& ctx, const T360Orientation& o) {
   return {};
 }
 
-// One plane of the orientation or lens kernel: src -> dst through geometry g, with its sphere tables (nullptr: none)
-t360::OrientedPlane orientedPlane(const uint8_t* src, int srcPitch, uint8_t* dst, int dstPitch, const t360::SphereGeometry& g,
-                                  const float* tables) {
-  t360::OrientedPlane v{};
-  v.src = src;
-  v.srcPitch = srcPitch;
-  v.dst = dst;
-  v.dstPitch = dstPitch;
-  v.geometry = g;
-  v.colTable = tables;
-  v.rowTable = tables ? tables + t360::sphereTableRowOffset(g) : nullptr;
-  return v;
-}
-
 // The upload ring entry may be refilled once the work enqueued on s so far has finished (nullptr: nothing to release)
 void releaseAfter(UploadRing::Entry* e, cudaStream_t s) {
   if (!e) return;
   CU(cudaEventRecord(e->released, s));
   e->inFlight = true;
+}
+
+// ---- warp maps (T360B200_remapFrameAsync) ------------------------------------------------------------------------------
+// true, with the reason in *why, when the caller's device maps (mapPitch in bytes) cannot remap frame f with this border
+bool mapRefused(const FrameTransformContext& ctx, const float* const* maps, const int* mapPitch, int border, const FramePlanes& f,
+                std::string* why) {
+  if (border != t360::kBorderWrap && border != t360::kBorderTransparent) {
+    *why = formatted("border %d (3: BORDER_WRAP, 5: BORDER_TRANSPARENT)", border);
+    return true;
+  }
+  for (int p = 0; p < f.numPlanes; ++p) {
+    if (!maps[p]) {
+      *why = formatted("invalid description of plane %d", p);
+      return true;
+    }
+    if (mapPitch[p] % 8 != 0 || mapPitch[p] / 8 < f.outW[p] || (reinterpret_cast<uintptr_t>(maps[p]) & 7)) {
+      *why = formatted("the map of plane %d (pitch %d bytes) must be 8-byte aligned with a pitch that is a multiple of 8 and at least 8 x the "
+                       "output width %d", p, mapPitch[p], f.outW[p]);
+      return true;
+    }
+  }
+  if (t360::kernelSizeOf(ctx.interpolation_alg) == 0) {
+    *why = formatted("no interpolation algorithm %d", static_cast<int>(ctx.interpolation_alg));
+    return true;
+  }
+  if (ctx.enable_low_pass_filter) {
+    *why = "the low-pass filter needs an output layout (set enable_low_pass_filter = 0)";
+    return true;
+  }
+  return false;
 }
 
 // ---- fisheye lens rigs (T360B200_lensMap, T360B200_transformFrameLensAsync; oriented_view.h: lensSample) ----------------
@@ -1199,48 +1215,16 @@ class VideoFrameTransform {
   // Needs no plan; the interpolation comes from the current context.  Every refusal comes before the first CUDA call, and
   // nothing here synchronises the device.
   bool remapFrame(const float* const* maps, const int* mapPitch, int border, const FramePlanes& f, cudaStream_t stream) {
-    const char* what = "Could not remap the frame";
-    return guarded(what, [&] {
-      if (border != t360::kBorderWrap && border != t360::kBorderTransparent) {
-        std::printf("%s. Error: border %d (3: BORDER_WRAP, 5: BORDER_TRANSPARENT)\n", what, border);
-        return false;
-      }
+    auto refused = [&](const FrameTransformContext& ctx, std::string* why) { return mapRefused(ctx, maps, mapPitch, border, f, why); };
+    return unplannedFrame("Could not remap the frame", stream, refused, [&](const FrameTransformContext& ctx, int, cudaStream_t s) {
+      t360::PerFrameGatherParams gp{};
       for (int p = 0; p < f.numPlanes; ++p) {
-        if (!maps[p]) {
-          std::printf("%s. Error: invalid description of plane %d\n", what, p);
-          return false;
-        }
-        if (mapPitch[p] % 8 != 0 || mapPitch[p] / 8 < f.outW[p] || (reinterpret_cast<uintptr_t>(maps[p]) & 7)) {
-          std::printf("%s. Error: the map of plane %d (pitch %d bytes) must be 8-byte aligned with a pitch that is a multiple of 8 and at "
-                      "least 8 x the output width %d\n", what, p, mapPitch[p], f.outW[p]);
-          return false;
-        }
+        gp.plane[p].geometry = t360::SphereGeometry{f.outW[p], f.outH[p], f.inW[p], f.inH[p]};
+        gp.plane[p].map = reinterpret_cast<const float2*>(maps[p]);
+        gp.plane[p].mapPitch = mapPitch[p] / 8;
       }
-      std::shared_lock<std::shared_mutex> config(configMu_);
-      const FrameTransformContext ctx = ctx_;
-      const int k = t360::kernelSizeOf(ctx.interpolation_alg);
-      if (k == 0) {
-        std::printf("%s. Error: no interpolation algorithm %d\n", what, ctx.interpolation_alg);
-        return false;
-      }
-      if (ctx.enable_low_pass_filter) {
-        std::printf("%s. Error: the low-pass filter needs an output layout (set enable_low_pass_filter = 0)\n", what);
-        return false;
-      }
-      const DeviceRestore restoreDevice = ensureDevice();
-      cudaStream_t s = stream ? stream : stream_;
-      const bool transparent = border == t360::kBorderTransparent;
-      t360::MapGatherParams mp{};
-      for (int p = 0; p < f.numPlanes; ++p) {
-        renderTarget(nullptr, p > 0, transparent, f.out[p], f.outPitch[p], f.outW[p], f.outH[p], nullptr, s);
-        mp.plane[p] = t360::MapPlane{f.in[p], f.out[p], f.inPitch[p], f.outPitch[p], reinterpret_cast<const float2*>(maps[p]), mapPitch[p] / 8,
-                                     t360::MapGeometry{f.outW[p], f.outH[p], f.inW[p], f.inH[p]}, 0, 0};
-      }
-      mp.numPlanes = f.numPlanes;
-      mp.kernelSize = k;
-      mp.transparent = transparent;
-      mp.weights = deviceWeights(ctx.interpolation_alg);
-      CU(t360::launchMapGather(mp, numSMs_, s));
+      gp.transparent = border == t360::kBorderTransparent;
+      perFrameGather(t360::PerFrameSource::kMap, gp, ctx, f, f.in, f.inPitch, nullptr, gp.transparent, nullptr, nullptr, nullptr, s);
       return true;
     });
   }
@@ -1250,7 +1234,7 @@ class VideoFrameTransform {
   // plan and leaves the plans alone; the output layout's tables come through the slot's upload ring.  Every refusal comes
   // before the first CUDA call, and nothing here synchronises the device.
   // seamWidth: nullptr for the hard seam; else the belt in degrees across which two lenses are blended
-  // (T360B200_transformFrameLensBlendAsync: lensBlendSample), the same steps with the blend kernel.
+  // (T360B200_transformFrameLensBlendAsync: lensBlendSample), the same steps with the blend source.
   bool transformFrameLens(const char* what, const T360LensRig* rig, const float* seamWidth, const T360Orientation* o, const FramePlanes& f,
                           cudaStream_t stream) {
     auto refused = [&](const FrameTransformContext& ctx, std::string* why) {
@@ -1258,24 +1242,16 @@ class VideoFrameTransform {
     };
     return unplannedFrame(what, stream, refused, [&](const FrameTransformContext& ctx, int k, cudaStream_t s) {
       const FrameTransformContext lens = lensContext(ctx);
-      StreamSlot& slot = slotFor(s);
       const float* tables[kPlaneLanes];
       UploadRing::Entry* staged = nullptr;
-      sphereTablesFor(lens, f.numPlanes, f.outW, f.outH, slot, s, tables, &staged);
-      t360::LensGatherParams lp{};
-      for (int p = 0; p < f.numPlanes; ++p) {
-        renderTarget(nullptr, p > 0, /*transparent=*/true, f.out[p], f.outPitch[p], f.outW[p], f.outH[p], nullptr, s);
-        lp.plane[p] = orientedPlane(f.in[p], f.inPitch[p], f.out[p], f.outPitch[p],
-                                    t360::sphereGeometry(lens, f.outW[p], f.outH[p], f.inW[p], f.inH[p], k), tables[p]);
-      }
-      lp.numPlanes = f.numPlanes;
-      lp.rotation = t360::rotationFromAngles(o->yaw, o->pitch, o->roll);
-      lp.rig = lensRigModel(*rig);
-      lp.kernelSize = k;
-      lp.weights = deviceWeights(ctx.interpolation_alg);
-      if (seamWidth) CU(t360::launchLensBlendGather(t360::LensBlendGatherParams{lp, lensSeamScale(*seamWidth)}, numSMs_, s));
-      else CU(t360::launchLensGather(lp, numSMs_, s));
-      releaseAfter(staged, s);
+      sphereTablesFor(lens, f.numPlanes, f.outW, f.outH, slotFor(s), s, tables, &staged);
+      t360::PerFrameGatherParams gp{};
+      for (int p = 0; p < f.numPlanes; ++p) gp.plane[p].geometry = t360::sphereGeometry(lens, f.outW[p], f.outH[p], f.inW[p], f.inH[p], k);
+      gp.rotation = t360::rotationFromAngles(o->yaw, o->pitch, o->roll);
+      gp.rig = lensRigModel(*rig);
+      if (seamWidth) gp.seamScale = lensSeamScale(*seamWidth);
+      perFrameGather(seamWidth ? t360::PerFrameSource::kLensBlend : t360::PerFrameSource::kLens, gp, ctx, f, f.in, f.inPitch, nullptr,
+                     /*transparent=*/true, tables, staged, nullptr, s);
       return true;
     });
   }
@@ -1286,21 +1262,13 @@ class VideoFrameTransform {
   // lens call's pre-fill.  Needs no plan and leaves the plans alone; no tables.
   bool transformFrameRectilinear(const char* what, const T360LensRig* rig, const T360Pose* pose, const FramePlanes& f, cudaStream_t stream) {
     auto refused = [&](const FrameTransformContext& ctx, std::string* why) { return rectilinearRefused(ctx, rig, pose, why); };
-    return unplannedFrame(what, stream, refused, [&](const FrameTransformContext& ctx, int k, cudaStream_t s) {
-      const bool lens = rig != nullptr;
-      t360::RectilinearGatherParams rp{};
-      for (int p = 0; p < f.numPlanes; ++p) {
-        renderTarget(nullptr, p > 0, lens, f.out[p], f.outPitch[p], f.outW[p], f.outH[p], nullptr, s);
-        rp.plane[p] = orientedPlane(f.in[p], f.inPitch[p], f.out[p], f.outPitch[p],
-                                    rectilinearGeometry(ctx, lens, f.inW[p], f.inH[p], f.outW[p], f.outH[p]), nullptr);
-      }
-      rp.numPlanes = f.numPlanes;
-      rp.lens = lens;
-      rp.camera = rectilinearCamera(*pose);
-      if (lens) rp.rig = lensRigModel(*rig);
-      rp.kernelSize = k;
-      rp.weights = deviceWeights(ctx.interpolation_alg);
-      CU(t360::launchRectilinearGather(rp, numSMs_, s));
+    return unplannedFrame(what, stream, refused, [&](const FrameTransformContext& ctx, int, cudaStream_t s) {
+      t360::PerFrameGatherParams gp{};
+      gp.lens = rig != nullptr;
+      for (int p = 0; p < f.numPlanes; ++p) gp.plane[p].geometry = rectilinearGeometry(ctx, gp.lens, f.inW[p], f.inH[p], f.outW[p], f.outH[p]);
+      gp.camera = rectilinearCamera(*pose);
+      if (rig) gp.rig = lensRigModel(*rig);
+      perFrameGather(t360::PerFrameSource::kRectilinear, gp, ctx, f, f.in, f.inPitch, nullptr, gp.lens, nullptr, nullptr, nullptr, s);
       return true;
     });
   }
@@ -1359,46 +1327,56 @@ class VideoFrameTransform {
       for (int p = 0; p < numPlanes; ++p) { src[p] = f.in[p]; srcPitch[p] = f.inPitch[p]; }
       if (ctx.enable_low_pass_filter && !viewLowPass(what, ctx, plans, f, slot, s, src, srcPitch)) return false;
 
-      PlaneTarget dst[kPlaneLanes];
-      for (int p = 0; p < numPlanes; ++p)
-        dst[p] = renderTarget(plans[p], p > 0, plans[p]->transparent, f.out[p], f.outPitch[p], f.outW[p], f.outH[p], &slot.lanes[p].scaled, s);
-      if (ctx.output_layout == LAYOUT_FLAT_FIXED) {
-        t360::ViewGatherParams vp{};
-        for (int p = 0; p < numPlanes; ++p) {
-          const DevicePlan& plan = *plans[p];
-          vp.plane[p] = t360::ViewPlane{src[p], dst[p].dst, srcPitch[p], dst[p].dstPitch,
-                                        t360::flatGeometry(ctx, plan.mapW, plan.mapH, plan.inW, plan.inH, k), 0, 0};
-        }
-        vp.numPlanes = numPlanes;
-        vp.view = t360::FlatView{ctx.fixed_yaw, ctx.fixed_pitch, ctx.fixed_hfov, ctx.fixed_vfov};
-        vp.kernelSize = k;
-        vp.weights = deviceWeights(ctx.interpolation_alg);
-        CU(t360::launchViewGather(vp, numSMs_, s));
-      } else {
-        t360::OrientedGatherParams op{};
-        const float* tables[kPlaneLanes];
-        UploadRing::Entry* staged = nullptr;  // (pending: the tables come through the slot's ring)
+      const bool flat = ctx.output_layout == LAYOUT_FLAT_FIXED;
+      const float* tables[kPlaneLanes] = {};
+      UploadRing::Entry* staged = nullptr;  // (pending: the tables come through the slot's ring)
+      if (!flat) {
         for (int p = 0; p < numPlanes; ++p) tables[p] = plans[p]->sphereTables.ptr;
         if (perFrameOnly_) {
           int mapW[kPlaneLanes], mapH[kPlaneLanes];
           for (int p = 0; p < numPlanes; ++p) { mapW[p] = plans[p]->mapW; mapH[p] = plans[p]->mapH; }
           sphereTablesFor(ctx, numPlanes, mapW, mapH, slot, s, tables, &staged);
         }
-        for (int p = 0; p < numPlanes; ++p) {
-          const DevicePlan& plan = *plans[p];
-          op.plane[p] = orientedPlane(src[p], srcPitch[p], dst[p].dst, dst[p].dstPitch,
-                                      t360::sphereGeometry(ctx, plan.mapW, plan.mapH, plan.inW, plan.inH, k), tables[p]);
-        }
-        op.numPlanes = numPlanes;
-        op.rotation = t360::rotationFromAngles(ctx.fixed_yaw, ctx.fixed_pitch, ctx.fixed_roll);
-        op.kernelSize = k;
-        op.weights = deviceWeights(ctx.interpolation_alg);
-        CU(t360::launchOrientedGather(op, numSMs_, s));
-        releaseAfter(staged, s);
       }
-      for (int p = 0; p < numPlanes; ++p) finishTarget(dst[p], s);
+      t360::PerFrameGatherParams gp{};
+      for (int p = 0; p < numPlanes; ++p)
+        gp.plane[p].geometry = t360::sphereGeometry(ctx, plans[p]->mapW, plans[p]->mapH, plans[p]->inW, plans[p]->inH, k);
+      if (flat) gp.view = t360::FlatView{ctx.fixed_yaw, ctx.fixed_pitch, ctx.fixed_hfov, ctx.fixed_vfov};
+      else gp.rotation = t360::rotationFromAngles(ctx.fixed_yaw, ctx.fixed_pitch, ctx.fixed_roll);
+      perFrameGather(flat ? t360::PerFrameSource::kView : t360::PerFrameSource::kSphere, gp, ctx, f, src, srcPitch, plans, false, tables,
+                     staged, &slot, s);
       return true;
     });
+  }
+
+  // The one gather launch of a per-frame call (launchPerFrameGather) for the planes of f, on s: gp holds the per-frame
+  // constants and each plane's geometry (and map); src / srcPitch are the planes' inputs.  With plans (the whole-frame
+  // calls) a plane renders at its plan's map size with the plan's border, and a scale factor resizes it into f's plane with
+  // INTER_AREA through the slot's scratch plane; without (remap, lens rigs, rectilinear views) it renders into f's plane
+  // with BORDER_TRANSPARENT where `transparent`.  tables: the planes' sphere tables (nullptr: none); `staged` the upload
+  // ring entry they came through, released after the launch.
+  void perFrameGather(t360::PerFrameSource source, t360::PerFrameGatherParams& gp, const FrameTransformContext& ctx, const FramePlanes& f,
+                      const uint8_t* const* src, const int* srcPitch, const DevicePlan* const* plans, bool transparent,
+                      const float* const* tables, UploadRing::Entry* staged, StreamSlot* slot, cudaStream_t s) {
+    PlaneTarget dst[kPlaneLanes];
+    for (int p = 0; p < f.numPlanes; ++p) {
+      const DevicePlan* plan = plans ? plans[p] : nullptr;
+      dst[p] = renderTarget(plan, p > 0, plan ? plan->transparent : transparent, f.out[p], f.outPitch[p], f.outW[p], f.outH[p],
+                            plan ? &slot->lanes[p].scaled : nullptr, s);
+      t360::PerFramePlane& v = gp.plane[p];
+      v.src = src[p];
+      v.srcPitch = srcPitch[p];
+      v.dst = dst[p].dst;
+      v.dstPitch = dst[p].dstPitch;
+      v.colTable = tables ? tables[p] : nullptr;
+      v.rowTable = v.colTable ? v.colTable + t360::sphereTableRowOffset(v.geometry) : nullptr;
+    }
+    gp.numPlanes = f.numPlanes;
+    gp.kernelSize = t360::kernelSizeOf(ctx.interpolation_alg);
+    gp.weights = deviceWeights(ctx.interpolation_alg);
+    CU(t360::launchPerFrameGather(gp, source, numSMs_, s));
+    releaseAfter(staged, s);
+    for (int p = 0; p < f.numPlanes; ++p) finishTarget(dst[p], s);
   }
 
   // tuning aid: a timeline of the consumer groups of the last frame gather (see StagedParams::trace)
@@ -2578,8 +2556,8 @@ static int perFrameSamples(const char* what, const FrameTransformContext* contex
     std::printf("Could not compute the %s's samples. Error: invalid interpolation or plane sizes\n", what);
     return 0;
   }
+  const t360::SphereGeometry g = t360::sphereGeometry(ctx, mapW, mapH, inW, inH, k);
   if (ctx.output_layout == LAYOUT_FLAT_FIXED) {
-    const t360::FlatGeometry g = t360::flatGeometry(ctx, mapW, mapH, inW, inH, k);
     const t360::FlatView v{ctx.fixed_yaw, ctx.fixed_pitch, ctx.fixed_hfov, ctx.fixed_vfov};
     for (int i = 0; i < mapH; ++i)
       for (int j = 0; j < mapW; ++j) {
@@ -2588,7 +2566,6 @@ static int perFrameSamples(const char* what, const FrameTransformContext* contex
       }
     return 1;
   }
-  const t360::SphereGeometry g = t360::sphereGeometry(ctx, mapW, mapH, inW, inH, k);
   const std::vector<float> tables = t360::buildSphereTables(g);
   const float* colTab = tables.data();
   const float* rowTab = tables.empty() ? nullptr : tables.data() + t360::sphereTableRowOffset(g);

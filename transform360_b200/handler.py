@@ -153,6 +153,8 @@ def load(path: os.PathLike | None = None):
                                 "transform360_b200 has no CPU fallback")
     L = C.CDLL(str(p), mode=os.RTLD_LOCAL)
     vp, ci = C.c_void_p, C.c_int
+    # the tail of every frame entry point: dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, stream
+    planes = [vp, vp] + [vp] * 6 + [vp]
     L.VideoFrameTransform_new.restype = vp
     L.VideoFrameTransform_new.argtypes = [C.POINTER(FrameTransformContext)]
     L.VideoFrameTransform_delete.restype = None
@@ -168,7 +170,7 @@ def load(path: os.PathLike | None = None):
     L.T360B200_generateMapFromWarp.restype = ci
     L.T360B200_generateMapFromWarp.argtypes = [vp, vp] + [ci] * 6
     L.T360B200_remapFrameAsync.restype = ci
-    L.T360B200_remapFrameAsync.argtypes = [vp, ci, vp, vp, ci] + [vp] * 8 + [vp]
+    L.T360B200_remapFrameAsync.argtypes = [vp, ci, vp, vp, ci] + planes
     L.T360B200_hostPlanDestroy.restype = None
     L.T360B200_hostPlanDestroy.argtypes = [vp]
     L.T360B200_hostPlanInfo.restype = ci
@@ -194,7 +196,7 @@ def load(path: os.PathLike | None = None):
     L.T360B200_transformFramePlaneAsync.restype = ci
     L.T360B200_transformFramePlaneAsync.argtypes = [vp, vp, vp] + [ci] * 7 + [vp]
     L.T360B200_transformFrameAsync.restype = ci
-    L.T360B200_transformFrameAsync.argtypes = [vp, ci, vp, vp] + [vp] * 6 + [vp]
+    L.T360B200_transformFrameAsync.argtypes = [vp, ci] + planes
     L.T360B200_lowPassPlaneAsync.restype = ci
     L.T360B200_lowPassPlaneAsync.argtypes = [vp, vp, vp] + [ci] * 5 + [vp]
     L.T360B200_reconfigure.restype = ci
@@ -204,29 +206,29 @@ def load(path: os.PathLike | None = None):
     L.T360B200_reconfigureWait.restype = ci
     L.T360B200_reconfigureWait.argtypes = [vp, ci]
     L.T360B200_transformFrameViewAsync.restype = ci
-    L.T360B200_transformFrameViewAsync.argtypes = [vp, C.POINTER(T360View), ci, vp, vp] + [vp] * 6 + [vp]
+    L.T360B200_transformFrameViewAsync.argtypes = [vp, C.POINTER(T360View), ci] + planes
     L.T360B200_viewSamples.restype = ci
     L.T360B200_viewSamples.argtypes = [C.POINTER(FrameTransformContext), C.POINTER(T360View)] + [ci] * 4 + [vp]
     L.T360B200_transformFrameOrientedAsync.restype = ci
-    L.T360B200_transformFrameOrientedAsync.argtypes = [vp, C.POINTER(T360Orientation), ci, vp, vp] + [vp] * 6 + [vp]
+    L.T360B200_transformFrameOrientedAsync.argtypes = [vp, C.POINTER(T360Orientation), ci] + planes
     L.T360B200_orientedSamples.restype = ci
     L.T360B200_orientedSamples.argtypes = [C.POINTER(FrameTransformContext), C.POINTER(T360Orientation)] + [ci] * 4 + [vp]
     L.T360B200_transformFramePoseAsync.restype = ci
-    L.T360B200_transformFramePoseAsync.argtypes = [vp, C.POINTER(T360Pose), ci, vp, vp] + [vp] * 6 + [vp]
+    L.T360B200_transformFramePoseAsync.argtypes = [vp, C.POINTER(T360Pose), ci] + planes
     L.T360B200_poseSamples.restype = ci
     L.T360B200_poseSamples.argtypes = [C.POINTER(FrameTransformContext), C.POINTER(T360Pose)] + [ci] * 4 + [vp]
     L.T360B200_lensMap.restype = ci
     L.T360B200_lensMap.argtypes = [C.POINTER(FrameTransformContext), C.POINTER(T360LensRig), C.POINTER(T360Orientation)] + [ci] * 4 + [vp]
     L.T360B200_transformFrameLensAsync.restype = ci
-    L.T360B200_transformFrameLensAsync.argtypes = [vp, C.POINTER(T360LensRig), C.POINTER(T360Orientation), ci, vp, vp] + [vp] * 6 + [vp]
+    L.T360B200_transformFrameLensAsync.argtypes = [vp, C.POINTER(T360LensRig), C.POINTER(T360Orientation), ci] + planes
     L.T360B200_lensBlendMaps.restype = ci
     L.T360B200_lensBlendMaps.argtypes = [C.POINTER(FrameTransformContext), C.POINTER(T360LensRig), C.c_float, C.POINTER(T360Orientation)] + [ci] * 4 + [vp] * 3
     L.T360B200_transformFrameLensBlendAsync.restype = ci
-    L.T360B200_transformFrameLensBlendAsync.argtypes = [vp, C.POINTER(T360LensRig), C.c_float, C.POINTER(T360Orientation), ci, vp, vp] + [vp] * 6 + [vp]
+    L.T360B200_transformFrameLensBlendAsync.argtypes = [vp, C.POINTER(T360LensRig), C.c_float, C.POINTER(T360Orientation), ci] + planes
     L.T360B200_rectilinearMap.restype = ci
     L.T360B200_rectilinearMap.argtypes = [C.POINTER(FrameTransformContext), C.POINTER(T360LensRig), C.POINTER(T360Pose)] + [ci] * 4 + [vp]
     L.T360B200_transformFrameRectilinearAsync.restype = ci
-    L.T360B200_transformFrameRectilinearAsync.argtypes = [vp, C.POINTER(T360LensRig), C.POINTER(T360Pose), ci, vp, vp] + [vp] * 6 + [vp]
+    L.T360B200_transformFrameRectilinearAsync.argtypes = [vp, C.POINTER(T360LensRig), C.POINTER(T360Pose), ci] + planes
     L.T360B200_setPinHostPlanes.restype = None
     L.T360B200_setPinHostPlanes.argtypes = [vp, ci]
     L.T360B200_debugTrace.restype = None
@@ -321,80 +323,64 @@ class VideoFrameTransform:
         return bool(self._lib.T360B200_transformFramePlaneAsync(self._h, d_in, d_out, in_w, in_h, in_pitch, out_w,
                                                                 out_h, out_pitch, plan_index, stream))
 
+    def _frame_call(self, entry: str, in_planes, out_planes, dims):
+        """The argument arrays of the frame entry point `entry` for one (input frame, output frame) pair, prebuilt once.
+        Returns (n, enqueue): n planes, and enqueue(lead, stream) -> bool, which calls `entry` with the handle, `lead` (the
+        arguments up to the planes, n included) and the planes."""
+        n, pin, pout, ptrs, keep = _frame_args(in_planes, out_planes, dims)
+        fn, h = getattr(self._lib, entry), self._h
+
+        def enqueue(lead, stream, _keep=keep) -> bool:
+            return bool(fn(h, *lead, pin, pout, *ptrs, stream))
+        return n, enqueue
+
     def make_frame_call(self, in_planes, out_planes, dims):
         """Prebuilds the argument arrays of T360B200_transformFrameAsync for one (input frame, output frame) pair.
         in_planes / out_planes: per plane (device_address, pitch); dims: per plane (in_w, in_h, out_w, out_h).
         Returns a callable f(stream) -> bool that enqueues the whole frame."""
-        n, pin, pout, ptrs, keep = _frame_args(in_planes, out_planes, dims)
-        fn, h = self._lib.T360B200_transformFrameAsync, self._h
-
-        def call(stream: int = 0, _keep=keep) -> bool:
-            return bool(fn(h, n, pin, pout, *ptrs, stream))
-        return call
+        n, enqueue = self._frame_call("T360B200_transformFrameAsync", in_planes, out_planes, dims)
+        return lambda stream=0: enqueue((n,), stream)
 
     def make_view_frame_call(self, in_planes, out_planes, dims):
         """Like make_frame_call, for T360B200_transformFrameViewAsync (FLAT_FIXED transforms): returns a callable
         f(view, stream) -> bool that enqueues the whole frame with `view` (a T360View or (yaw, pitch, hfov, vfov))."""
-        n, pin, pout, ptrs, keep = _frame_args(in_planes, out_planes, dims)
-        fn, h = self._lib.T360B200_transformFrameViewAsync, self._h
-
-        def call(view, stream: int = 0, _keep=keep) -> bool:
-            return bool(fn(h, C.byref(as_view(view)), n, pin, pout, *ptrs, stream))
-        return call
+        n, enqueue = self._frame_call("T360B200_transformFrameViewAsync", in_planes, out_planes, dims)
+        return lambda view, stream=0: enqueue((C.byref(as_view(view)), n), stream)
 
     def make_oriented_frame_call(self, in_planes, out_planes, dims):
         """Like make_frame_call, for T360B200_transformFrameOrientedAsync (cube-map, EAC and equirect outputs): returns a
         callable f(orientation, stream) -> bool that enqueues the whole frame with `orientation` (a T360Orientation or
         (yaw, pitch, roll))."""
-        n, pin, pout, ptrs, keep = _frame_args(in_planes, out_planes, dims)
-        fn, h = self._lib.T360B200_transformFrameOrientedAsync, self._h
-
-        def call(orientation, stream: int = 0, _keep=keep) -> bool:
-            return bool(fn(h, C.byref(as_orientation(orientation)), n, pin, pout, *ptrs, stream))
-        return call
+        n, enqueue = self._frame_call("T360B200_transformFrameOrientedAsync", in_planes, out_planes, dims)
+        return lambda orientation, stream=0: enqueue((C.byref(as_orientation(orientation)), n), stream)
 
     def make_pose_frame_call(self, in_planes, out_planes, dims):
         """Like make_frame_call, for T360B200_transformFramePoseAsync (every output layout): returns a callable
         f(pose, stream) -> bool that enqueues the whole frame with `pose` (a T360Pose or (yaw, pitch, roll, hfov, vfov))."""
-        n, pin, pout, ptrs, keep = _frame_args(in_planes, out_planes, dims)
-        fn, h = self._lib.T360B200_transformFramePoseAsync, self._h
-
-        def call(pose, stream: int = 0, _keep=keep) -> bool:
-            return bool(fn(h, C.byref(as_pose(pose)), n, pin, pout, *ptrs, stream))
-        return call
+        n, enqueue = self._frame_call("T360B200_transformFramePoseAsync", in_planes, out_planes, dims)
+        return lambda pose, stream=0: enqueue((C.byref(as_pose(pose)), n), stream)
 
     def make_lens_frame_call(self, in_planes, out_planes, dims):
         """Like make_frame_call, for T360B200_transformFrameLensAsync (a fisheye lens rig to any sphere output, no plan
         needed): returns a callable f(rig, orientation, stream) -> bool that enqueues the whole frame with `rig` (a
         T360LensRig) and `orientation` (a T360Orientation or (yaw, pitch, roll))."""
-        n, pin, pout, ptrs, keep = _frame_args(in_planes, out_planes, dims)
-        fn, h = self._lib.T360B200_transformFrameLensAsync, self._h
-
-        def call(rig, orientation, stream: int = 0, _keep=keep) -> bool:
-            return bool(fn(h, C.byref(rig), C.byref(as_orientation(orientation)), n, pin, pout, *ptrs, stream))
-        return call
+        n, enqueue = self._frame_call("T360B200_transformFrameLensAsync", in_planes, out_planes, dims)
+        return lambda rig, orientation, stream=0: enqueue((C.byref(rig), C.byref(as_orientation(orientation)), n), stream)
 
     def make_lens_blend_frame_call(self, in_planes, out_planes, dims):
         """Like make_lens_frame_call, for T360B200_transformFrameLensBlendAsync (a two-lens rig whose seam is feathered
         across a belt of seam_width degrees): returns a callable f(rig, seam_width, orientation, stream) -> bool that
         enqueues the whole frame."""
-        n, pin, pout, ptrs, keep = _frame_args(in_planes, out_planes, dims)
-        fn, h = self._lib.T360B200_transformFrameLensBlendAsync, self._h
-
-        def call(rig, seam_width, orientation, stream: int = 0, _keep=keep) -> bool:
-            return bool(fn(h, C.byref(rig), seam_width, C.byref(as_orientation(orientation)), n, pin, pout, *ptrs, stream))
-        return call
+        n, enqueue = self._frame_call("T360B200_transformFrameLensBlendAsync", in_planes, out_planes, dims)
+        return lambda rig, seam_width, orientation, stream=0: enqueue(
+            (C.byref(rig), seam_width, C.byref(as_orientation(orientation)), n), stream)
 
     def make_rectilinear_frame_call(self, in_planes, out_planes, dims):
         """Like make_frame_call, for T360B200_transformFrameRectilinearAsync (a perspective view, no plan needed): returns a
         callable f(pose, stream, rig=None) -> bool that enqueues the whole frame with `pose` (a T360Pose or (yaw, pitch,
         roll, hfov, vfov)), looking into the context's input, or into `rig` (a T360LensRig) when one is given."""
-        n, pin, pout, ptrs, keep = _frame_args(in_planes, out_planes, dims)
-        fn, h = self._lib.T360B200_transformFrameRectilinearAsync, self._h
-
-        def call(pose, stream: int = 0, rig=None, _keep=keep) -> bool:
-            return bool(fn(h, C.byref(rig) if rig is not None else None, C.byref(as_pose(pose)), n, pin, pout, *ptrs, stream))
-        return call
+        n, enqueue = self._frame_call("T360B200_transformFrameRectilinearAsync", in_planes, out_planes, dims)
+        return lambda pose, stream=0, rig=None: enqueue((C.byref(rig) if rig is not None else None, C.byref(as_pose(pose)), n), stream)
 
     def generate_map_from_warp(self, map, in_w: int, in_h: int, plan_index: int, border: int = BORDER_WRAP) -> bool:
         """T360B200_generateMapFromWarp: installs plan index `plan_index` from a caller's warp map (float32 [h][w][2], the
@@ -410,8 +396,7 @@ class VideoFrameTransform:
         frame through one device map per plane, each the size of its output plane.  maps: per plane a CUDA float32 tensor
         [out_h][>= out_w][2] (its row stride gives the pitch), a (device address, pitch in bytes) pair, or a device address
         of a dense map."""
-        n, pin, pout, ptrs, keep = _frame_args(in_planes, out_planes, dims)
-        fn, h = self._lib.T360B200_remapFrameAsync, self._h
+        n, enqueue = self._frame_call("T360B200_remapFrameAsync", in_planes, out_planes, dims)
         dense = [8 * d[2] for d in dims]
 
         def as_map(m, p):
@@ -419,12 +404,12 @@ class VideoFrameTransform:
                 return m.data_ptr(), m.stride(0) * m.element_size()
             return (int(m[0]), int(m[1])) if isinstance(m, (tuple, list)) else (int(m), dense[p])
 
-        def call(maps, stream: int = 0, _keep=keep) -> bool:
+        def call(maps, stream: int = 0) -> bool:
             if len(maps) != n:
                 raise ValueError(f"{len(maps)} maps for {n} planes")
             desc = [as_map(m, p) for p, m in enumerate(maps)]
             dmaps, pitches = (C.c_void_p * n)(*[d[0] for d in desc]), (C.c_int * n)(*[d[1] for d in desc])
-            return bool(fn(h, n, dmaps, pitches, border, pin, pout, *ptrs, stream))
+            return enqueue((n, dmaps, pitches, border), stream)
         return call
 
     def low_pass_async(self, d_in: int, d_out: int, w, h, in_pitch, out_pitch, plan_index, stream: int = 0) -> bool:
