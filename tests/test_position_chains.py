@@ -1,6 +1,8 @@
 """The position chains of the per-frame kernels (view_gather.cu: FlatPositions, SpherePositions<BARREL>, LensPositions,
-LensBlendPositions): every pixel's sampling record {col0, rowPhase}, read back from the device and compared with the host
-twin record for record, at the breadth of the CPU sweeps and at the chains' branch points.
+LensBlendPositions, RectilinearPositions<LENS>, MapPositions<K, TRANSPARENT>): every pixel's sampling record {col0,
+rowPhase}, read back from the device and compared with the host twin record for record, at the breadth of the CPU sweeps
+and at the chains' branch points.  The host twins are the planner's samplers, and for rectilinear views and warp maps
+HostPlan.from_warp of rectilinear_map's map or of the caller's map.
 
 The chains (flat_view.h, oriented_view.h, libm_ports.h) are the one place where device float code must give the host's
 bits, glibc's atan2f / asinf included.  A pixel comparison on noise can miss a record that moved by 1/32 px, and says
@@ -19,8 +21,10 @@ The decode is proven on the CPU against remap_u8 before any of it is trusted on 
 
 The ledger below classifies every pixel of every case by the chain branch it takes, from exact sources: numpy float32
 for the + - * / parts (no contraction), the planner's own float map for ties, saturation and clamps, the lens maps of
-single-lens rigs for coverage and lens choice.  Each (chain, class, K) must be reached; each case must reach one that no
-other case does.
+single-lens rigs for coverage and lens choice, a float32 replica of the rectilinear chain (which must give rectilinear_map's
+bits, or a rig's coverage, on every pixel) and the warp maps' own values.  Each (chain, class, K) must be reached; each
+case family must reach one that no other family does; a class that cannot occur is in UNREACHABLE with a CPU test that
+proves it.  The rectilinear positions read back are also checked against test_rectilinear's float64 model.
 """
 from __future__ import annotations
 
@@ -40,9 +44,16 @@ from tests.test_lens_blend import BLEND_RIGS, SEAMS, composite
 from tests.test_oriented import _angle
 from tests.test_oriented import _sweep_case as oriented_case
 from tests.test_pose import _sweep_case as pose_case
+from tests.test_rectilinear import CONTEXTS as RECT_CONTEXTS
+from tests.test_rectilinear import _in_dims as rect_in_dims
+from tests.test_rectilinear import _poses as rect_poses
+from tests.test_rectilinear import model as rect_model
+from tests.test_rectilinear import rays as rect_model_rays
 from tests.test_tile_gather import records_to_map
 from tests.test_view import _sweep_case as view_case
 from tests.test_view import torch_cuda  # noqa: F401 (fixture)
+from tests.test_warp_map import FAMILIES as MAP_FAMILIES
+from tests.test_warp_map import _sizes as map_sizes
 from transform360_b200.stream import FrameTransformer, StreamSpec
 
 F32 = np.float32
@@ -409,12 +420,211 @@ def boundary_cases():
     return cases
 
 
+# ---- rectilinear views and warp maps: the cases -------------------------------------------------------------------------
+RECT_CTX = dict(enable_low_pass_filter=0)
+
+
+def rect_case(inp, pose, sizes, own_k, **extra):
+    """A rectilinear view (RectilinearPositions) of `inp`: a context input of test_rectilinear (BORDER_WRAP), a rig of
+    test_lens (BORDER_TRANSPARENT) or, with ov= in extra, the context overrides themselves."""
+    ov = extra.pop("ov", None)
+    if inp in RIGS:
+        return dict(kind="rect", ov=dict(RECT_CTX), fields=tuple(pose), rig=inp, sizes=sizes, own_k=own_k, border=TRANSPARENT, **extra)
+    return dict(kind="rect", ov=dict(RECT_CTX, **(RECT_CONTEXTS[inp] if ov is None else ov)), fields=tuple(pose), sizes=sizes, own_k=own_k,
+                border=WRAP, **extra)
+
+
+def rectilinear_sweep():
+    """test_rectilinear's inputs (four contexts, three rigs) x its seeded and fixed poses, at its sizes."""
+    out = []
+    for n, inp in enumerate(sorted(RECT_CONTEXTS) + RIGS):
+        (iw, ih), _ = rect_in_dims(inp)
+        for pose in rect_poses(sum(map(ord, inp))):
+            out.append(rect_case(inp, pose, (iw, ih, 97, 65), [4, 8][n % 2]))
+    return out
+
+
+def rectilinear_large():
+    """The reframing use: a 7680 x 3840 equirect into a 1920 x 1080 view (90 degrees with square pixels, and 179 degrees
+    across the meridian), and a 5760 x 3840 cube map: record columns above 2048, long tile loops and rays up to ~160 times
+    longer than a unit vector."""
+    hd = (7680, 3840, 1920, 1080)
+    return [rect_case("equirect", (35.0, -20.0, 10.0, 90.0, t360.square_pixel_vfov(90.0, 1920, 1080)), hd, 4),
+            rect_case("equirect", (-175.0, 50.0, -30.0, 179.0, 150.0), hd, 8),
+            rect_case("cube", (120.0, -35.0, 15.0, 100.0, 70.0), (5760, 3840, 1920, 1080), 4, ov=dict(input_layout=t360.LAYOUT_CUBEMAP_32))]
+
+
+def _meridian_search():
+    """Rectilinear views of an odd-width equirect whose ray has t.x == +0 (and another t.x == -0) with t.z < 0: the
+    branch cut of atan2f, where u is 1 (column inW - 0.5) or 0 (column -0.5).  Searched over axis-aligned and half-turn
+    poses and odd output sizes."""
+    found = {}
+    angles = (0.0, 90.0, -90.0, 180.0, -180.0, 45.0, -45.0)
+    for yaw in angles:
+        for pitch in angles:
+            for roll in angles:
+                for w, h in ((9, 7), (15, 11), (33, 21)):
+                    c = rect_case("equirect", (yaw, pitch, roll, 60.0, 40.0), (259, 131, w, h), 4)
+                    t, _ = rect_rays(c, 0)
+                    cut = (t[..., 0] == 0) & (t[..., 2] < 0)
+                    for sign in (False, True):
+                        if sign not in found and (cut & (np.signbit(t[..., 0]) == sign)).any():
+                            found[sign] = c
+                    if len(found) == 2:
+                        return [found[False], found[True]]
+    raise AssertionError(f"no pose puts a ray on the branch cut with both signs of zero (found {sorted(found)})")
+
+
+@functools.lru_cache(maxsize=None)
+def _pole_search():
+    """A view with a ray exactly on a pole, t = (0, y, 0): yaw 0 and roll 0 make the centre column of an odd view t.x = qx =
+    0 and t.z = c2 - qy s2, so a row whose qy s2 rounds to c2 is on the pole.  Searched over pitches, output heights and
+    rows, with vfov stepped by floats around the angle that aims that row at the pole."""
+    for pitch in (45.0, 60.0, 30.0, -45.0, 75.0):
+        s2, c2 = (F32(fn(float(F32(pitch)) * math.pi / 180.0)) for fn in (math.sin, math.cos))
+        for h in range(3, 40):
+            y = F32(1.0) - _centres(h)
+            for a in (F32(2.0) * y - F32(1.0))[:h // 2]:
+                v0 = F32(2.0 * math.degrees(math.atan(float(c2) / (float(s2) * float(a)))))
+                if not 0 < v0 < 179:
+                    continue
+                for vfov in v0 + np.arange(-256, 257) * np.spacing(v0):
+                    ty = F32(math.tan(float(vfov) * math.pi / 360.0))
+                    if (a * ty) * s2 == c2:
+                        c = rect_case("equirect", (0.0, pitch, 0.0, 60.0, float(vfov)), (259, 131, 9, h), 8)
+                        t, _ = rect_rays(c, 0)
+                        if ((t[..., 0] == 0) & (t[..., 2] == 0)).any():
+                            return c
+    return None
+
+
+def _rect_lens_search():
+    """Lens cases through the unnormalised pinhole ray: an unrotated single lens with an odd output, so the centre ray is
+    (0, 0, 1) (rho == 0), at 179 x 179 degrees (rays ~160 times longer than a unit vector) with maxAngle searched so that
+    thetaMax equals a pixel's theta; and a back-to-back pair with a pose searched for z1 == z0."""
+    c = rect_case("single_200", (0.0, 0.0, 0.0, 179.0, 179.0), (259, 131, 33, 21), 8)
+    t, _ = rect_rays(c, 0)
+    theta = lens_views(rig_of(c), t)[0][2]
+    edge = None
+    for th in np.unique(theta[(theta > np.radians(85)) & (theta < np.radians(89.5))])[::-1]:
+        a0 = F32(float(th) * 180.0 / math.pi)
+        hit = [a for a in a0 + np.arange(-4, 5) * np.spacing(a0) if F32(float(a) * math.pi / 180.0) == th]
+        if hit:
+            edge = dict(c, max_angle=float(hit[0]))
+            break
+    assert edge is not None, "no maxAngle puts thetaMax on a pixel's theta"
+    rig = make_rig("pair_190", seed=len("pair_190"))
+    pole = _pole_search()
+    cands = [pole] if pole is not None else []
+    cands += [rect_case("pair_190", (y, p, r, 60.0, 40.0), (259, 131, 9, h), 4)
+              for y in (0.0, 90.0, -90.0, 180.0) for p in (45.0, -45.0, 90.0, 0.0) for r in (0.0, 90.0, 180.0) for h in (7, 11)]
+    for c2 in cands:
+        c2 = rect_case("pair_190", c2["fields"], c2["sizes"], 4)
+        (z0, *_), (z1, *_) = lens_views(rig, rect_rays(c2, 0)[0])
+        if (z0 == z1).any():
+            return [edge, c2]
+    raise AssertionError("no pose gives a ray with z1 == z0 on the back-to-back pair")
+
+
+def _cube_edge_cases():
+    """Cube-map input with input_expand_coef 1: a ray with |gx| == 1 (yaw 45: the centre column's t.x and t.z are the
+    same float) and one with |gy| == 1 (pitch 45), the face-selection ties of cubeInputHD."""
+    ov = dict(input_layout=t360.LAYOUT_CUBEMAP_32, input_expand_coef=1.0)
+    return [rect_case("cube", (45.0, 0.0, 0.0, 60.0, 40.0), (261, 174, 9, 7), 4, ov=ov),
+            rect_case("cube", (0.0, 45.0, 0.0, 60.0, 40.0), (261, 174, 9, 7), 8, ov=ov)]
+
+
+def rectilinear_boundary():
+    """Rays put exactly on the chain's decisions, found by the searches above or set by hand, and the one stereo pair the
+    sweep lacks (a side-by-side input into a stacked output without the flip)."""
+    out = _meridian_search() + _cube_edge_cases() + _rect_lens_search()
+    pole = _pole_search()
+    if pole is not None:
+        out.append(pole)
+    out.append(rect_case("lr_to_tb", (-60.0, 10.0, 20.0, 100.0, 80.0), (258, 131, 97, 65), 4,
+                         ov=dict(input_layout=t360.LAYOUT_EQUIRECT, input_stereo_format=LR, output_stereo_format=TB)))
+    return out
+
+
+# The warp maps: test_warp_map's families at their sizes, and hand-placed values.  Each plane has its own map (chroma: the
+# family at the chroma size, plane 2 mirrored left to right) and its own map pitch (entries of row padding per plane), so
+# a plane mix-up or an ignored pitch moves records.
+MAP_PITCH_EXTRA = (3, 0, 5)
+
+
+def _bits(*bits):
+    return np.array(bits, np.uint32).view(F32)
+
+
+# value, and the class it is placed for (at K = 2 the classes of f * 32, at K = 1 those of f)
+EXACT_VALUES = [
+    (F32(-0.0), "neg_zero"), (F32(1e-40), "subnormal"), (F32(-1e-40), "subnormal"), (_bits(1)[0], "subnormal"),
+    (F32(10 + 1 / 64), "tie_even (K 2)"), (F32(10 + 3 / 64), "tie_odd (K 2)"), (F32(12.5), "tie_even (K 1)"), (F32(13.5), "tie_odd (K 1)"),
+    (_bits(0x7FC00000)[0], "nan (quiet)"), (_bits(0xFFC00000)[0], "nan (negative)"), (_bits(0x7FC12345)[0], "nan (payload)"),
+    (_bits(0x7F800001)[0], "nan (signalling)"), (F32(np.inf), "pos_inf"), (F32(-np.inf), "neg_inf"),
+    (F32(40000.5), "sat16_high"), (F32(-40000.5), "sat16_low"),
+    (F32(67108860.0), "int_top (K 2: f * 32 = 2147483520)"), (F32(2147483520.0), "int_top (K 1)"),
+    (F32(2.0 ** 26), "int_over (K 2: f * 32 = 2^31)"), (F32(2.0 ** 31), "int_over (K 1)"),
+    (F32(-(2.0 ** 26)), "int_bottom (K 2: f * 32 = -2^31)"), (F32(-(2.0 ** 31)), "int_bottom (K 1)"),
+    (F32(-67108872.0), "int_under (K 2: f * 32 = -2147483904)"), (F32(-2147483904.0), "int_under (K 1)"),
+]
+
+
+def exact_map(ow, oh, iw, ih, p):
+    """Ordinary positions inside the source (no window leaves it), with every EXACT_VALUES value once as x and once as y, placed at
+    plane-dependent pixels (bits kept: the NaN payloads and signs reach the kernel)."""
+    rng = np.random.default_rng(100 + p)
+    m = np.stack([rng.uniform(8, iw - 9, (oh, ow)), rng.uniform(8, ih - 9, (oh, ow))], -1).astype(F32)
+    bits = m.view(np.uint32)
+    for n, (v, _) in enumerate(EXACT_VALUES):
+        for axis in range(2):
+            i, j = divmod(((2 * n + axis) * 7 + 3 * p + 1) % (ow * oh), ow)
+            bits[i, j, axis] = np.array([v], F32).view(np.uint32)[0]
+    return m
+
+
+@functools.lru_cache(maxsize=None)
+def _case_map(name, sizes, p):
+    iw, ih, ow, oh = StreamSpec(*sizes).plane_dims(p)[:4]
+    if name == "exact":
+        m = exact_map(ow, oh, iw, ih, p)
+    else:
+        m = MAP_FAMILIES[name](ow, oh, iw, ih)
+        if p == 2:
+            m = np.ascontiguousarray(m[:, ::-1])
+    m.setflags(write=False)
+    return m
+
+
+def case_map(c, p):
+    return _case_map(c["maps"], c["sizes"], p)
+
+
+def map_families():
+    """test_warp_map's six families at their sizes, under both borders (MapPositions<K, false> and <K, true>)."""
+    out = []
+    for n, name in enumerate(sorted(MAP_FAMILIES)):
+        mw, mh, iw, ih = map_sizes(name)
+        out += [dict(kind="map", maps=name, ov=dict(RECT_CTX), sizes=(iw, ih, mw, mh), own_k=[4, 8][(n + b) % 2], border=border)
+                for b, border in enumerate((WRAP, TRANSPARENT))]
+    return out
+
+
+def map_exact():
+    """The hand-placed values into a 2403 x 41 source (plane widths 2403 and 1202 do not divide 65535, so the saturated
+    columns 32767 - a and -32768 - a wrap to different columns), under both borders."""
+    return [dict(kind="map", maps="exact", ov=dict(RECT_CTX), sizes=(2403, 41, 75, 53), own_k=k, border=border)
+            for k, border in ((4, WRAP), (8, TRANSPARENT))]
+
+
 @functools.lru_cache(maxsize=None)
 def families():
     """name -> list of cases: each sweep, the lens and blend sets, the large planes and each boundary search."""
     out = dict(view_sweep=view_sweep(), oriented_sweep=oriented_sweep(), pose_sweep=pose_sweep(), lens=lens_cases(), blend=blend_cases(),
                large=large_cases())
     out.update(boundary_cases())
+    out.update(rectilinear_sweep=rectilinear_sweep(), rectilinear_large=rectilinear_large(), rectilinear_boundary=rectilinear_boundary(),
+               map_families=map_families(), map_exact=map_exact())
     return out
 
 
@@ -444,8 +654,8 @@ def rig_of(c, lens=None):
     return one
 
 
-def _quantised(ctx, m, iw, ih):
-    hp = t360.HostPlan.from_warp(ctx, m, iw, ih, TRANSPARENT)
+def _quantised(ctx, m, iw, ih, border=TRANSPARENT):
+    hp = t360.HostPlan.from_warp(ctx, m, iw, ih, border)
     r = hp.samples
     hp.close()
     return r
@@ -464,6 +674,9 @@ def host_plane(c, k, p):
         hp.close()
         return out
     warp = t360.make_context(interpolation_alg=INTERP[k], enable_low_pass_filter=0)
+    if kind in ("rect", "map"):
+        m = t360.rectilinear_map(ctx, c["fields"], iw, ih, ow, oh, rig_of(c) if "rig" in c else None) if kind == "rect" else case_map(c, p)
+        return dict(rec=_quantised(warp, m, iw, ih, c["border"]), map=m)
     alone = [t360.lens_map(ctx, rig_of(c, i), c["fields"], iw, ih, ow, oh) for i in range(rig_of(c).numLenses)]
     if kind == "lens":
         m = t360.lens_map(ctx, rig_of(c), c["fields"], iw, ih, ow, oh)
@@ -673,9 +886,148 @@ def blend_classes(c, k, p, hp):
                              ("neither", ~cov0 & ~cov1)) if hit.any()}
 
 
+_LIBM.asinf.restype, _LIBM.asinf.argtypes = ctypes.c_float, (ctypes.c_float,)
+asinf = np.vectorize(lambda x: F32(_LIBM.asinf(float(x))), otypes=[F32])
+
+
+def rect_rays(c, p):
+    """oriented_view.h: rectilinearPoint of every pixel of plane p, in float32: (t [h][w][3], not normalised; eye [h][w])."""
+    _, _, w, h = plane_dims(c)[p]
+    ov = c["ov"]
+    split_lr, split_tb, _ = _stereo(ov)
+    x, y = _centres(w), _centres(h)
+    eye_x, eye_y = np.zeros(w, bool), np.zeros(h, bool)
+    if split_lr:
+        eye_x, x = x > F32(0.5), _split(x)
+    elif split_tb:
+        eye_y, y = y > F32(0.5), _split(y, bool(ov.get("vflip")))
+    y = (F32(1.0) - y).astype(F32)
+    yaw, pitch, roll, hfov, vfov = (float(F32(v)) for v in c["fields"])
+    tx, ty = (F32(math.tan(f * math.pi / 360.0)) for f in (hfov, vfov))  # (video_frame_transform.cpp: rectilinearCamera)
+    qx = ((F32(2.0) * x - F32(1.0)) * tx)[None, :].repeat(h, 0)
+    qy = ((F32(2.0) * y - F32(1.0)) * ty)[:, None].repeat(w, 1)
+    r = rotation_f32(yaw, pitch, roll)
+    one = F32(1.0)
+    t = np.stack([(qx * r[0][0] - qy * r[0][1]) + one * r[0][2], -((qx * r[1][0] - qy * r[1][1]) + one * r[1][2]),
+                  (qx * r[2][0] - qy * r[2][1]) + one * r[2][2]], -1).astype(F32)
+    return t, eye_x[None, :] | eye_y[:, None]
+
+
+_CUBE_IN = [(2, 0, 1, 5, 3, 1, 1), (2, 0, 1, 3, 3, 1, -1), (0, 2, 1, 3, 1, -1, 1), (0, 2, 1, 1, 1, -1, -1), (1, 0, 2, 1, 3, -1, 1),
+            (1, 0, 2, 5, 1, 1, 1)]  # cubeInputHD: (major, a, b, col, row, su, sv) of faces 0..5 (even faces: major <= -0.5)
+
+
+def cube_input(d, e):
+    """oriented_view.h: cubeInputHD of unit rays d in float32: (face index or -1, gx, gy, u, v) of the face that takes each."""
+    face = np.full(d.shape[:2], -1)
+    gx, gy = np.full(d.shape[:2], np.nan, F32), np.full(d.shape[:2], np.nan, F32)
+    u, v = np.full(d.shape[:2], F32(-1.0)), np.full(d.shape[:2], F32(0.0))
+    with np.errstate(all="ignore"):
+        for f, (mj, a, b, col, row, su, sv) in enumerate(_CUBE_IN):
+            major = d[..., mj]
+            ok = (major <= F32(-0.5)) if f % 2 == 0 else (major >= F32(0.5))
+            fx, fy = d[..., a] / major, d[..., b] / major
+            win = (face < 0) & ok & (fx >= -1) & (fx <= 1) & (fy >= -1) & (fy <= 1)
+            sx, sy = fx / F32(e), fy / F32(e)
+            fu = ((F32(col) + sx) if su > 0 else (F32(col) - sx)) / F32(6.0)
+            fv = ((F32(row) + sy) if sv > 0 else (F32(row) - sy)) / F32(4.0)
+            face, gx, gy = np.where(win, f, face), np.where(win, fx, gx), np.where(win, fy, gy)
+            u, v = np.where(win, fu, u).astype(F32), np.where(win, fv, v).astype(F32)
+    return face, gx, gy, u, v
+
+
+_RECT_REPLICA = {}
+
+
+def rect_classes(c, k, p, hp):
+    """The rectilinear chain's branches from its float32 replica, which must give the host twin's map (context inputs: its
+    bits; rigs: its coverage) on every pixel.  (The map does not depend on K: the replica runs once per plane.)"""
+    key = (repr(sorted(c.items())), p)
+    if key not in _RECT_REPLICA:
+        _RECT_REPLICA[key] = frozenset(_rect_replica_classes(c, p, hp["map"]))
+    out = set(_RECT_REPLICA[key])
+    if "rig" not in c and np.isin(hp["rec"][..., 0] + max(k // 2 - 1, 0), (-32768, 32767)).any():
+        out.add("input_saturated")
+    return out
+
+
+def _rect_replica_classes(c, p, m):
+    ov, f = c["ov"], c["fields"]
+    iw, ih, _, _ = plane_dims(c)[p]
+    t, eye = rect_rays(c, p)
+    split_lr, split_tb, pack = _stereo(ov)
+    out = {n for n, hit in (("mono", not (split_lr or split_tb)), ("split_lr", split_lr), ("split_tb", split_tb and not ov.get("vflip")),
+                            ("split_tb_vflip", split_tb and ov.get("vflip")), ("pack_lr", pack == LR), ("pack_tb", pack == TB),
+                            ("fov_179", max(f[3], f[4]) >= 179.0), ("fov_narrow", min(f[3], f[4]) <= 2.0)) if hit}
+    if "rig" in c:
+        views = lens_views(rig_of(c), t)
+        covered = ~np.isnan(m[..., 0])
+        second = views[1][0] > views[0][0] if len(views) > 1 else np.zeros(covered.shape, bool)
+        chosen = [np.where(second, b, a) for a, b in zip(views[0], views[-1])]
+        assert np.array_equal(chosen[3], covered), f"the lens replica's coverage differs from the host twin's ({c})"
+        tmax = np.where(second, lens_matrix(rig_of(c).lens[len(views) - 1])[1], lens_matrix(rig_of(c).lens[0])[1])
+        return out | {n for n, hit in (("lens0", covered & ~second), ("lens1", covered & second), ("uncovered", ~covered),
+                                       ("tie", (views[1][0] == views[0][0]) if len(views) > 1 else second),
+                                       ("rho_zero", covered & (chosen[1] == 0)), ("theta_at_max", chosen[2] == tmax)) if hit.any()}
+    tx, ty, tz = t[..., 0], t[..., 1], t[..., 2]
+    n = np.sqrt((tx * tx + ty * ty) + tz * tz)
+    if ov.get("input_layout") == t360.LAYOUT_CUBEMAP_32:
+        face, gx, gy, u, v = cube_input(t / n[..., None], case_context(c, 2).input_expand_coef)
+        out |= {f"cube_in_face{i}" for i in np.unique(face) if i >= 0} | ({"cube_in_none"} if (face < 0).any() else set())
+        out |= {name for name, g in (("column_on_face_edge", gx), ("row_on_face_edge", gy)) if (np.abs(g) == 1).any()}
+    else:
+        lon = -atan2f(-tx / n, tz / n)
+        lat = asinf(-ty / n)
+        u = (lon.astype(np.float64) / (2 * math.pi) + 0.5).astype(F32)
+        v = (lat.astype(np.float64) / math.pi + 0.5).astype(F32)
+        if pack == LR:
+            u = np.where(eye, u * F32(0.5) + F32(0.5), u * F32(0.5)).astype(F32)
+        cut = (tx == 0) & (tz < 0)
+        wrap = (tz[:, 1:] < 0) & (tz[:, :-1] < 0) & (np.signbit(tx[:, 1:]) != np.signbit(tx[:, :-1]))
+        polar = np.hypot(tx.astype(np.float64), tz.astype(np.float64)) < 1e-3 * n
+        out |= {name for name, hit in (("lon_plain", tz > 0), ("lon_wrap", wrap), ("lon_cut_pos_zero", cut & ~np.signbit(tx)),
+                                       ("lon_cut_neg_zero", cut & np.signbit(tx)), ("near_pole", polar),
+                                       ("exact_pole", (tx == 0) & (tz == 0))) if hit.any()}
+    if pack == TB:
+        v = np.where(eye, v * F32(0.5) + F32(0.5), v * F32(0.5)).astype(F32)
+    want = np.stack([u * F32(iw) - F32(0.5), v * F32(ih) - F32(0.5)], -1)
+    assert np.array_equal(want.view(np.uint32), m.view(np.uint32)), f"the rectilinear replica's map differs from the host twin's ({c}, plane {p})"
+    return out
+
+
+def map_classes(c, k, p, hp):
+    """The map chain's branches from the map values themselves: f * 32 (K >= 2) or f (K = 1) against roundHalfEven's
+    int range, the int16 clamp and the special floats."""
+    f = hp["map"].reshape(-1)
+    with np.errstate(all="ignore"):
+        q = (f * F32(32.0)).astype(F32) if k > 1 else f
+        fin = np.isfinite(f)
+        inside = fin & (q >= F32(-(2.0 ** 31))) & (q < F32(2.0 ** 31))
+        r = np.where(inside, np.rint(np.where(inside, q, 0).astype(np.float64)), 0).astype(np.int64)
+        first = r >> 5 if k > 1 else r
+    hit = {"interior": inside & (first >= -32768) & (first <= 32767), "neg_zero": (f == 0) & np.signbit(f),
+           "subnormal": (f != 0) & (np.abs(f) < np.finfo(F32).tiny), "nan": np.isnan(f), "pos_inf": f == np.inf, "neg_inf": f == -np.inf,
+           "sat16_high": inside & (first > 32767), "sat16_low": inside & (first < -32768), "int_top": q == F32(2147483520.0),
+           "int_over": fin & (q >= F32(2.0 ** 31)), "int_bottom": q == F32(-(2.0 ** 31)), "int_under": fin & (q < F32(-(2.0 ** 31)))}
+    out = {n for n, h in hit.items() if h.any()}
+    iw, ih, _, _ = plane_dims(c)[p]
+    col0, row0 = hp["rec"][..., 0].astype(np.int64), hp["rec"][..., 1].astype(np.int64) >> 10
+    span = max(k, 1)
+    for first, n, ok in ((col0, iw, inside.reshape(-1, 2)[:, 0]), (row0, ih, inside.reshape(-1, 2)[:, 1])):
+        first = first.reshape(-1)
+        if (ok & (first > -32768) & (first < 32767 - span) & ((first < 0) | (first + span > n))).any():
+            out.add("edge")  # (an ordinary record whose window leaves the source: wrapped, or under BORDER_TRANSPARENT skipped or reflected)
+    out.add("border_wrap" if c["border"] == WRAP else "border_transparent")
+    if MAP_PITCH_EXTRA[p] > 0:
+        out.add("padded_pitch")
+    return out
+
+
 def chain_of(c):
     if c["kind"] in ("lens", "blend"):
         return c["kind"]
+    if c["kind"] in ("rect", "map"):
+        return {"rect": "rectilinear", "map": "map"}[c["kind"]]
     layout = c["ov"].get("output_layout", t360.LAYOUT_CUBEMAP_32)
     return "flat" if layout == t360.LAYOUT_FLAT_FIXED else ("barrel" if layout in BARRELS else "sphere")
 
@@ -694,7 +1046,8 @@ def all_classes(k, hp, iw):
 def plane_classes(c, k, p, hp):
     chain = chain_of(c)
     own = {"flat": lambda: flat_classes(c, k, p), "sphere": lambda: sphere_classes(c, k, p, hp), "barrel": lambda: barrel_classes(c, k, p, hp),
-           "lens": lambda: lens_classes(c, k, p, hp), "blend": lambda: blend_classes(c, k, p, hp)}[chain]()
+           "lens": lambda: lens_classes(c, k, p, hp), "blend": lambda: blend_classes(c, k, p, hp),
+           "rectilinear": lambda: rect_classes(c, k, p, hp), "map": lambda: map_classes(c, k, p, hp)}[chain]()
     if chain == "barrel":
         own |= {f"sphere:{s}" for s in sphere_classes(c, k, p, hp) if s.startswith(("cube_in", "equirect_in", "offcentre"))}
     return {(chain, cls, k) for cls in own | all_classes(k, hp, plane_dims(c)[p][0])}
@@ -720,11 +1073,23 @@ CLASSES = {
                "clamp_high", "sphere:equirect_in", "sphere:cube_in_none", "sphere:offcentre", "sphere:offcentre_horizontal", "sphere:offcentre_nan"),
     "lens": ("lens0", "lens1", "uncovered", "tie", "rho_zero", "theta_at_max"),
     "blend": ("only_lens0", "only_lens1", "clamped_low", "clamped_high", "ramp", "neither", "half_way_tie_even"),
+    "rectilinear": ("mono", "split_lr", "split_tb", "split_tb_vflip", "pack_lr", "pack_tb", "lon_plain", "lon_wrap", "lon_cut_pos_zero",
+                    "lon_cut_neg_zero", "near_pole", "exact_pole") + tuple(f"cube_in_face{f}" for f in range(6)) + (
+        "cube_in_none", "column_on_face_edge", "row_on_face_edge", "lens0", "lens1", "uncovered", "tie", "rho_zero", "theta_at_max", "fov_179",
+        "fov_narrow", "input_saturated"),
+    "map": ("interior", "edge", "neg_zero", "subnormal", "nan", "pos_inf", "neg_inf", "sat16_high", "sat16_low", "int_top", "int_over", "int_bottom",
+            "int_under", "padded_pitch", "border_wrap", "border_transparent"),
 }
 ALL = ("tie_even", "tie_odd", "saturated", "column_above_2048")
 UNREACHABLE = {
     ("barrel", "band_edge"): "no pixel centre (j + 0.5) / W, nor its eye-split image, rounds to 0.8f or to a third of 2 for any W < 8192 "
                              "(test_barrel_band_edges_are_not_reached_by_any_size)",
+    ("rectilinear", "cube_in_none"): "a unit ray's largest component is at least 1/sqrt(3) > 0.5 after the float normalisation, and "
+                                     "|a / major| <= 1 is exact in float division, so its face always takes it "
+                                     "(test_every_unit_ray_has_a_cube_input_face)",
+    ("rectilinear", "input_saturated"): "u and v of a context input lie within 2^-26 of [0, 1] (equirect) or at most (5 + 1 / e) / 4 "
+                                        "from 0 (cube map, input_expand_coef e >= 0.5), so no record of a plane narrower than 8192 columns reaches the int16 clamp "
+                                        "(test_context_input_records_stay_inside_the_int16_range)",
 }
 
 
@@ -827,8 +1192,50 @@ def test_barrel_band_edges_are_not_reached_by_any_size():
             assert not (t == F32(0.8)).any() and not (F32(3.0) * t == F32(2.0)).any(), w
 
 
+def test_every_unit_ray_has_a_cube_input_face():
+    """cube_in_none is unreachable for a rectilinear ray.  The ray t = R q with q = (qx, qy, 1) is finite and at least ~1 long,
+    so n > 0 and d = t / n is a unit vector up to a few float steps; its largest component is then at least 1/sqrt(3) (1 -
+    4 eps) > 0.5, which passes that face's major test, and the other two components are no larger in magnitude, so |a /
+    major| <= 1 (float division is monotonic and x / x == 1): the largest component's face takes d if no earlier face
+    has.  Checked here on the worst case (the eight diagonals and their float neighbours, where the largest component is
+    smallest) and on a million random rays of every length a view makes (up to ~160)."""
+    rng = np.random.default_rng(3)
+    diag = np.array([[sx, sy, sz] for sx in (-1, 1) for sy in (-1, 1) for sz in (-1, 1)], F32)
+    steps = np.array([np.spacing(F32(1.0)) * s for s in range(-4, 5)], F32)
+    near_diag = (diag[:, None, :] * (F32(1.0) + steps[None, :, None])).reshape(-1, 3)
+    rand = (rng.normal(size=(1000000, 3)) * rng.uniform(1, 160, (1000000, 1))).astype(F32)
+    for t in (near_diag, rand):
+        t = t[None]
+        n = np.sqrt((t[..., 0] * t[..., 0] + t[..., 1] * t[..., 1]) + t[..., 2] * t[..., 2])
+        d = t / n[..., None]
+        assert (np.abs(d).max(-1) > F32(0.5)).all()
+        for e in (1.0, 1.04, 0.9):
+            assert (cube_input(d, e)[0] >= 0).all()
+
+
+def test_context_input_records_stay_inside_the_int16_range():
+    """input_saturated is unreachable: atan2f returns at most float(pi) and asinf at most float(pi / 2) in magnitude, and
+    the double steps make u = lon / 2pi + 0.5 and v = lat / pi + 0.5 of those extremes lie within 2^-26 of [0, 1] (float(pi)
+    is a little above pi: u of -float(pi) is -1.4e-8); a cube-map input gives u = (col +- gx / e) / 6 with col in {1, 3, 5},
+    v = (row +- gy / e) / 4 with row in {1, 3}, and |gx|, |gy| <= 1.  So |u inW - 0.5| stays below (5 + 1 / e) inW / 4 + 1,
+    and for inW < 8192 and e >= 0.5 every record is far inside -32768 .. 32767 - 3."""
+    pi_f, half_pi_f = F32(math.pi), F32(math.pi / 2)
+    assert atan2f(F32(0.0), F32(-1.0)) == pi_f and atan2f(F32(-0.0), F32(-1.0)) == -pi_f and asinf(F32(1.0)) == half_pi_f
+    ext = [F32(float(a) / (2 * math.pi) + 0.5) for a in (pi_f, -pi_f)] + [F32(float(a) / math.pi + 0.5) for a in (half_pi_f, -half_pi_f)]
+    assert all(-(2.0 ** -26) <= a <= 1 + 2.0 ** -26 for a in ext), ext
+    for e in (0.5, 1.0, 1.04):
+        d = np.array([[[1.0, 1.0, -1.0], [-1.0, -1.0, 1.0], [1.0, -1.0, 1.0], [-1.0, 1.0, -1.0]]], F32) / F32(math.sqrt(3.0))
+        _, _, _, u, v = cube_input(d, e)
+        assert (np.abs(np.concatenate([u, v])) <= (5 + 1 / e) / 4).all()
+    assert 8191 * 7 / 4 + 1 < 32767 - 3
+    assert all(c["sizes"][0] < 8192 for cases in families().values() for c in cases if c["kind"] == "rect")
+
+
 def test_host_twins_equal_the_planner_on_the_added_cases():
-    """The large and boundary cases (not in the CPU sweeps): the host twin's records equal the planner's."""
+    """The large and boundary cases (not in the CPU sweeps): the host twin's records equal the planner's.  (The rectilinear
+    families' float32 replica is checked against rectilinear_map on every pixel by rect_classes, through the ledger.)"""
+    for name in ("rectilinear_sweep", "rectilinear_large", "rectilinear_boundary"):
+        assert family_classes(name)
     for name, cases in families().items():
         if name in ("view_sweep", "oriented_sweep", "pose_sweep", "lens", "blend"):
             continue
@@ -862,6 +1269,13 @@ def _run_frames(torch, c, k, frames, prefill_luma):
         vft = ft.vft
         make = dict(view=vft.make_view_frame_call, oriented=vft.make_oriented_frame_call, pose=vft.make_pose_frame_call)[c["kind"]]
         args = (c["fields"],)
+    elif c["kind"] == "rect":  # (a never-planned transform)
+        vft = t360.VideoFrameTransform(ctx)
+        rig = rig_of(c) if "rig" in c else None
+        make, args = (lambda i, o, d: lambda pose, stream: vft.make_rectilinear_frame_call(i, o, d)(pose, stream, rig)), (c["fields"],)
+    elif c["kind"] == "map":
+        vft = t360.VideoFrameTransform(ctx)
+        make, args = (lambda i, o, d: vft.make_remap_frame_call(i, o, d, c["border"])), (device_maps(torch, c),)
     else:
         vft = t360.VideoFrameTransform(ctx)
         if c["kind"] == "lens":
@@ -942,6 +1356,52 @@ def check_case(torch, c, k):
                            lambda i, j: f"device {int(dev[axis][i, j])}, host {int(host[axis][i, j])}")
         if c["kind"] == "lens" and k == 2 and p == 0 and iw <= 2048 and ih <= 2048:
             check_against_model(c, hp, dev, valid, ~skip)
+        if c["kind"] == "rect" and k == 2 and p == 0:
+            check_rect_against_model(c, dev, valid, ~skip)
+
+
+def device_maps(torch, c):
+    """The case's map of each plane on the device, with MAP_PITCH_EXTRA entries of row padding (built in numpy and copied
+    whole, so every NaN keeps its bits)."""
+    out = []
+    for p in range(3):
+        m = case_map(c, p)
+        padded = np.zeros((m.shape[0], m.shape[1] + MAP_PITCH_EXTRA[p], 2), F32)
+        padded[:, :m.shape[1]] = m
+        out.append(torch.from_numpy(padded).cuda())
+        assert out[-1].stride(0) * 4 == 8 * (m.shape[1] + MAP_PITCH_EXTRA[p])
+    return out
+
+
+def check_rect_against_model(c, dev, valid, written):
+    """The device's rectilinear positions (column and row + phase / 32, read back, modulo 2048) against test_rectilinear's
+    float64 model of the header's contract, not through the host twin: within 1/64 px of quantisation plus the model's
+    0.01 px (0.02 px for rigs), away from its near-threshold and polar pixels.  Plus the float32 pinhole's own slack: 2x - 1
+    and 2y' - 1 round to 2^-24 before tan(fov / 2) scales them, a direction error of up to 2^-23 max(tx, ty) rad (1.4e-5 rad
+    at 179 degrees), which an equirect input turns into that over 2 pi hypot(x, z) of a row in columns (so a 179-degree view
+    of a 7680-wide input moves by pixels near the poles) and over pi hypot(x, z) in rows."""
+    iw, ih, ow, oh = plane_dims(c)[0]
+    ctx = case_context(c, 2)
+    rig = rig_of(c) if "rig" in c else None
+    with np.errstate(divide="ignore", invalid="ignore"):  # (the model's cube lookup divides by every component)
+        want, near, polar = rect_model(None, ctx, rig, c["fields"], iw, ih, ow, oh)
+    d, eye = rect_model_rays(ctx, c["fields"], ow, oh, mono=rig is not None)
+    if rig is None and ctx.input_stereo_format == LR:  # (the model leaves side-by-side inputs to the caller: re-pack u)
+        want[..., 0] = ((want[..., 0] + 0.5) / iw * 0.5 + np.where(eye, 0.5, 0.0)) * iw - 0.5
+    eps = 2.0 ** -23 * max(float(F32(math.tan(float(F32(f)) * math.pi / 360.0))) for f in c["fields"][3:])
+    if rig is None and ctx.input_layout != t360.LAYOUT_CUBEMAP_32:
+        r = np.maximum(np.hypot(d[..., 0], d[..., 2]), 1e-12)  # (d atan2 and d asin both grow as 1 / r towards the poles)
+        slack = [eps * iw / (2 * math.pi * r), eps * ih / (math.pi * r)]
+    else:
+        slack = [eps * max(iw, ih)] * 2
+    ok = ~np.isnan(want[..., 0]) & ~near & ~polar & written
+    for axis in range(2):
+        sel = ok & valid[axis]
+        err = np.abs(dev[axis][sel] / 32.0 - np.mod(want[..., axis][sel], 2048.0))
+        err = np.minimum(err, 2048.0 - err)
+        over = err - (1 / 64 + (0.02 if rig is not None else 0.01) + np.broadcast_to(slack[axis], want.shape[:2])[sel])
+        assert sel.sum() > 0 and over.max() <= 0, (f"rectilinear positions read back differ from the float64 model by up to "
+                                                   f"{over.max():.4f} px beyond the bound (axis {axis}, case {c})")
 
 
 def check_against_model(c, hp, dev, valid, written):
