@@ -378,6 +378,57 @@ int T360B200_transformFrameRectilinearAsync(VideoFrameTransform* transform, cons
                                             const uint8_t* const* deviceInputs, uint8_t* const* deviceOutputs, const int* inputWidths,
                                             const int* inputHeights, const int* inputPitches, const int* outputWidths,
                                             const int* outputHeights, const int* outputPitches, void* cudaStream);
+/* ---- camera models ---------------------------------------------------------------------------------
+ * The views above with another camera than the pinhole: a fisheye (equidistant) lens for dome masters and virtual
+ * fisheye footage, a stereographic one for "little planet" shots, and Pannini for wide reframing that keeps vertical and
+ * radial lines straight.  Everything is as for the rectilinear views (the pose, the rig, the input lookup and its border,
+ * the pre-fill, the fields not read) except step 4, the ray q before the rotation.  With X = 2x - 1 and Y = 2y' - 1 (+-1
+ * at the plane's outer pixel edges), the per-pose constants computed in double and stored as float, and every per-pixel
+ * step in float rounded to nearest:
+ *   PINHOLE        tx = tan(hfov / 2), ty = tan(vfov / 2); q = (X tx, Y ty, 1): the rectilinear view, bit for bit.
+ *                  hfov, vfov in (0, 179];
+ *   EQUIDISTANT    ax = hfov pi / 360, ay = vfov pi / 360; a = X ax, b = Y ay, rho = sqrt(a^2 + b^2),
+ *                  q = (a S, b S, C) with S = sin rho / rho (1 at rho = 0) and C = cos rho: a pixel's angle to the axis is
+ *                  proportional to its distance from the centre.  With hfov = vfov = 180 on a square plane the inscribed
+ *                  circle is the front hemisphere (a dome master); the plane is full frame, no circular mask.  hfov, vfov
+ *                  in (0, 360];
+ *   STEREOGRAPHIC  sx = tan(hfov / 4), sy = tan(vfov / 4); a = X sx, b = Y sy, q = (2a, 2b, 1 - a^2 - b^2): the angle to
+ *                  the axis is 2 atan(sqrt(a^2 + b^2)).  Looking at the nadir (pitch -90) with 200-300 degrees, a little
+ *                  planet.  hfov, vfov in (0, 359];
+ *   PANNINI        d = pannini in [0, 1], h = hfov / 2; xe = (d + 1) sin h / (d + cos h), ye = tan(vfov / 2); u = X xe,
+ *                  w = Y ye, k = u^2 / (d + 1)^2, c = (-k d + sqrt(k^2 d^2 - (k + 1)(k d^2 - 1))) / (k + 1),
+ *                  q = (u (d + c) / (d + 1), w (d + c) / (d + 1), c), proportional to (sin lon, tan lat, cos lon) with
+ *                  c = cos lon (Sharpless et al.'s inverse; computed as k = (u / (d + 1))^2, c = (-k d + sqrt(1 + k (1 -
+ *                  d^2))) / (k + 1)).  Vertical lines stay vertical and radial lines through the centre straight; d = 0
+ *                  is the pinhole up to rounding, vfov is the field of the centre column.  hfov in (0, 359] with
+ *                  d + cos(hfov / 2) > 0, vfov in (0, 179].
+ * Every model gives every pixel a ray, so a view of the context's input has no NaN in its map.
+ *
+ * Refused, with 0 and a message on stdout before any CUDA call: the refusals of the rectilinear views with the field
+ * ranges above instead of (0, 179], a NULL camera, an unknown model, and for PANNINI a pannini that is not finite or lies
+ * outside [0, 1], and d + cos(hfov / 2) <= 0. */
+#define T360_CAMERA_PINHOLE 0
+#define T360_CAMERA_EQUIDISTANT 1
+#define T360_CAMERA_STEREOGRAPHIC 2
+#define T360_CAMERA_PANNINI 3
+typedef struct T360Camera {
+  int model;     /* T360_CAMERA_* */
+  float pannini; /* d, read by T360_CAMERA_PANNINI only */
+} T360Camera;
+/* Host only, no CUDA: T360B200_rectilinearMap with `camera` (float32 [outputHeight][outputWidth][2]; with a rig NaN where
+ * uncovered).  T360B200_generateMapFromWarp(map, ..., T360_BORDER_WRAP, or T360_BORDER_TRANSPARENT with a rig, index)
+ * plans it for a fixed pose and camera, and then gives the frames of T360B200_transformFrameCameraAsync bit for bit.
+ * Returns 1; 0 (message) for the refusals above, a NULL context or map, or non-positive sizes. */
+int T360B200_cameraMap(const FrameTransformContext* ctx, const T360LensRig* rig, const T360Pose* pose, const T360Camera* camera,
+                       int inputWidth, int inputHeight, int outputWidth, int outputHeight, float* map);
+/* One frame of a camera view, every plane in one gather launch: T360B200_transformFrameRectilinearAsync with `camera`,
+ * which may change every frame like the rig and the pose.  Needs no plan and does not touch the plans; takes the reader
+ * lock; never synchronises the device.  Returns 1 if everything was enqueued; 0 with a message on stdout, before any CUDA
+ * call, for the refusals above, 0 or more than 3 planes, or an invalid plane description. */
+int T360B200_transformFrameCameraAsync(VideoFrameTransform* transform, const T360LensRig* rig, const T360Pose* pose, const T360Camera* camera,
+                                       int numPlanes, const uint8_t* const* deviceInputs, uint8_t* const* deviceOutputs,
+                                       const int* inputWidths, const int* inputHeights, const int* inputPitches, const int* outputWidths,
+                                       const int* outputHeights, const int* outputPitches, void* cudaStream);
 /* Opt-in (also: environment T360B200_PIN_HOST_PLANES=1): page-lock pageable caller planes in place the second time
  * the same buffer is seen (cudaHostRegister), so that recycled frame-pool buffers are DMA'd at full PCIe speed.  The
  * caller must keep such buffers alive until VideoFrameTransform_delete. */

@@ -532,37 +532,105 @@ T360_HD int lensBlendSample(const SphereGeometry& g, const Rotation& r, const Le
   return w;
 }
 
-// ---- rectilinear views -----------------------------------------------------------------------------------------------
-// A perspective (pinhole) camera in place of the cube / sphere output: output pixel (i, j) of a mapW x mapH plane looks
-// along q = ((2x - 1) tx, (2y' - 1) ty, 1), x and y its centre after the output eye split (as spherePoint), y' = 1 - y,
-// tx = tan(hfov / 2), ty = tan(vfov / 2) (double on the host, stored as float: rectilinearCamera), rotated by the pose as
-// spherePoint rotates its point.  So with hfov = vfov = 90 an N x N view is the FRONT face of a 3N x 2N CUBEMAP_32 output
-// of the same orientation.  The input is the context's (sphereInputHD, BORDER_WRAP) or a lens rig (lensPosition,
-// BORDER_TRANSPARENT).  Only + - * / on the output half, so host and device agree bit for bit.
+// ---- camera views (rectilinear and the other camera models) ---------------------------------------------------------
+// A virtual camera in place of the cube / sphere output: output pixel (i, j) of a mapW x mapH plane, x and y its centre
+// after the output eye split (as spherePoint), y' = 1 - y, X = 2x - 1, Y = 2y' - 1 (+-1 at the plane's outer pixel edges),
+// looks along the model's ray q, rotated by the pose as spherePoint rotates its point:
+//   kCameraPinhole        q = (X cx, Y cy, 1), cx = tan(hfov / 2), cy = tan(vfov / 2).  So with hfov = vfov = 90 an N x N
+//                         view is the FRONT face of a 3N x 2N CUBEMAP_32 output of the same orientation;
+//   kCameraEquidistant    a = X cx, b = Y cy (cx = hfov pi / 360, cy = vfov pi / 360: the angle to the axis), rho the
+//                         length of (a, b), q = (a S, b S, C) with S = sin rho / rho, C = cos rho (sincCos);
+//   kCameraStereographic  a = X cx, b = Y cy (cx = tan(hfov / 4), cy = tan(vfov / 4)), q = (2a, 2b, 1 - a^2 - b^2);
+//   kCameraPannini        u = X cx, w = Y cy (cx = (d + 1) sin h / (d + cos h), h = hfov / 2, cy = tan(vfov / 2)),
+//                         k = (u e)^2, c = (-k d + sqrt(1 + k dd)) / (k + 1) (e = 1 / (d + 1), dd = 1 - d^2: Sharpless et
+//                         al.'s inverse with its discriminant k^2 d^2 - (k + 1)(k d^2 - 1) expanded, so it cannot cancel),
+//                         q = (u (d + c) e, w (d + c) e, c), proportional to (sin lon, tan lat, cos lon), c = cos lon.
+// The per-pose constants are computed on the host in double and stored as float (cameraConstants in
+// video_frame_transform.cpp).  The input is the context's (sphereInputHD, BORDER_WRAP) or a lens rig (lensPosition,
+// BORDER_TRANSPARENT).  Only + - * / and sqrt on the output half, so host and device agree bit for bit.
+enum CameraModel { kCameraPinhole = 0, kCameraEquidistant = 1, kCameraStereographic = 2, kCameraPannini = 3 };
 struct RectilinearCamera {
   Rotation r;
-  float tx, ty;  // tan(hfov / 2), tan(vfov / 2)
+  float cx, cy;  // the model's per-axis constants above
+  int model;     // CameraModel (the same for every pixel of a launch: a warp-uniform branch)
+  float d, e, dd;  // kCameraPannini: d, 1 / (d + 1), 1 - d^2
 };
 
+// sin(rho) / rho (1 at rho = 0) and cos(rho) for rho in [0, pi sqrt 2] from + - * / only: h = rho / 4, the Taylor
+// polynomials of sin(h) / h and cos(h) in h^2 (|h| <= 1.12: the first dropped terms are below 1e-9), then two angle
+// doublings: sin 2h / 2h = (sin h / h) cos h, cos 2h = 1 - 2 sin^2 h.  tests/test_camera_models.py compares it with
+// double over every float of the range.
+T360_HD void sincCos(float rho, float* sinc, float* cosine) {
+  const float h = fMul(rho, 0.25f), t = fMul(h, h);
+  float s = fAdd(fMul(t, -1.0f / 6227020800.0f), 1.0f / 39916800.0f);  // sin(h) / h = sum (-t)^n / (2n + 1)!
+  s = fSub(fMul(t, s), 1.0f / 362880.0f);
+  s = fAdd(fMul(t, s), 1.0f / 5040.0f);
+  s = fSub(fMul(t, s), 1.0f / 120.0f);
+  s = fAdd(fMul(t, s), 1.0f / 6.0f);
+  s = fSub(1.0f, fMul(t, s));
+  float c = fAdd(fMul(t, -1.0f / 87178291200.0f), 1.0f / 479001600.0f);  // cos(h) = sum (-t)^n / (2n)!
+  c = fSub(fMul(t, c), 1.0f / 3628800.0f);
+  c = fAdd(fMul(t, c), 1.0f / 40320.0f);
+  c = fSub(fMul(t, c), 1.0f / 720.0f);
+  c = fAdd(fMul(t, c), 1.0f / 24.0f);
+  c = fSub(fMul(t, c), 0.5f);
+  c = fAdd(fMul(t, c), 1.0f);
+  float a = h;
+  for (int k = 0; k < 2; ++k) {  // (s, c) of angle a -> of angle 2a
+    const float sn = fMul(a, s);
+    s = fMul(s, c);
+    c = fSub(1.0f, fMul(2.0f, fMul(sn, sn)));
+    a = fMul(a, 2.0f);
+  }
+  *sinc = s;
+  *cosine = c;
+}
+
+// The ray q (not rotated, not normalised) of the pixel at (X, Y) for the models other than the pinhole
+T360_HD SphereVec cameraRay(const RectilinearCamera& c, float X, float Y) {
+  switch (c.model) {
+    case kCameraEquidistant: {
+      const float a = fMul(X, c.cx), b = fMul(Y, c.cy);
+      float s, co;
+      sincCos(fSqrt(fAdd(fMul(a, a), fMul(b, b))), &s, &co);
+      return SphereVec{fMul(a, s), fMul(b, s), co};
+    }
+    case kCameraStereographic: {
+      const float a = fMul(X, c.cx), b = fMul(Y, c.cy);
+      return SphereVec{fMul(2.0f, a), fMul(2.0f, b), fSub(fSub(1.0f, fMul(a, a)), fMul(b, b))};
+    }
+    default: {  // kCameraPannini
+      const float u = fMul(X, c.cx), w = fMul(Y, c.cy);
+      const float ue = fMul(u, c.e), k = fMul(ue, ue);
+      const float cl = fDiv(fAdd(-fMul(k, c.d), fSqrt(fAdd(1.0f, fMul(k, c.dd)))), fAdd(k, 1.0f));
+      const float f = fMul(fAdd(c.d, cl), c.e);
+      return SphereVec{fMul(u, f), fMul(w, f), cl};
+    }
+  }
+}
+
 // Steps 1-5 of the contract for output pixel (i, j): the rotated ray (not normalised) and the output eye.  The geometry's
-// mapW, mapH, splitLR, splitTB and vflip play a part.
+// mapW, mapH, splitLR, splitTB and vflip play a part.  ANY_MODEL = false: c is a pinhole (the kernel's own loop for
+// pinhole launches, which so keeps the rectilinear view's code).
+template <bool ANY_MODEL = true>
 T360_HD SphereVec rectilinearPoint(const SphereGeometry& g, const RectilinearCamera& c, int i, int j, bool* eye) {
   float x = pixelCentre(j, g.mapW), y = pixelCentre(i, g.mapH);
   *eye = false;
   if (g.splitLR) *eye = splitEye(x, false);
   else if (g.splitTB) *eye = splitEye(y, g.vflip);
   y = fSub(1.0f, y);
-  const SphereVec q{fMul(fSub(fMul(2.0f, x), 1.0f), c.tx), fMul(fSub(fMul(2.0f, y), 1.0f), c.ty), 1.0f};
-  return rotateHD(c.r, q);
+  const float X = fSub(fMul(2.0f, x), 1.0f), Y = fSub(fMul(2.0f, y), 1.0f);
+  if (!ANY_MODEL || c.model == kCameraPinhole) return rotateHD(c.r, SphereVec{fMul(X, c.cx), fMul(Y, c.cy), 1.0f});
+  return rotateHD(c.r, cameraRay(c, X, Y));
 }
 
 // The CV_32FC2 map entry (*px, *py) of output pixel (i, j) of a rectilinear view: LENS = false the context's input
 // (sphereInputHD, no barrel clamp), LENS = true the rig's hard seam (NaN where no lens covers the ray).
-template <bool LENS>
+template <bool LENS, bool ANY_MODEL = true>
 T360_HD void rectilinearPosition(const SphereGeometry& g, const RectilinearCamera& c, const LensRigModel& rig, int i, int j, float* px,
                                  float* py) {
   bool eye;
-  const SphereVec d = rectilinearPoint(g, c, i, j, &eye);
+  const SphereVec d = rectilinearPoint<ANY_MODEL>(g, c, i, j, &eye);
   if constexpr (LENS) {
     lensPosition(rig, d, g.inW, g.inH, px, py);
   } else {
@@ -575,11 +643,11 @@ T360_HD void rectilinearPosition(const SphereGeometry& g, const RectilinearCamer
 
 // The sampling record of output pixel (i, j) of a rectilinear view: its map entry quantised as quantizeWarpMap quantises a
 // caller's map, so T360B200_rectilinearMap -> T360B200_generateMapFromWarp plans the records the kernel computes.
-template <bool LENS>
+template <bool LENS, bool ANY_MODEL = true>
 T360_HD void rectilinearSample(const SphereGeometry& g, const RectilinearCamera& c, const LensRigModel& rig, int i, int j, int32_t* col0,
                                int32_t* rowPhase) {
   float px, py;
-  rectilinearPosition<LENS>(g, c, rig, i, j, &px, &py);
+  rectilinearPosition<LENS, ANY_MODEL>(g, c, rig, i, j, &px, &py);
   int r0, fracX, fracY;
   quantizeAxis(px, g.kernelSize, col0, &fracX);
   quantizeAxis(py, g.kernelSize, &r0, &fracY);

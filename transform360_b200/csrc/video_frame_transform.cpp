@@ -616,11 +616,15 @@ void forLensPixels(const FrameTransformContext& ctx, const T360Orientation& o, i
     for (int j = 0; j < outW; ++j) point(g, r, colTab, rowTab, i, j, static_cast<size_t>(i) * outW + j);
 }
 
-// ---- rectilinear views (T360B200_rectilinearMap, T360B200_transformFrameRectilinearAsync; oriented_view.h:
-// rectilinearSample) ----------------------------------------------------------------------------------------------------
-// true, with the reason in *why, when a rectilinear view of ctx's input (rig == nullptr) or of the rig cannot be rendered
-// with this pose.  The output layout plays no part: the pose replaces it.
-bool rectilinearRefused(const FrameTransformContext& ctx, const T360LensRig* rig, const T360Pose* pose, std::string* why) {
+// ---- camera views (T360B200_cameraMap, T360B200_transformFrameCameraAsync, and the rectilinear pair, which is the
+// pinhole camera; oriented_view.h: rectilinearSample) -------------------------------------------------------------------
+static_assert(T360_CAMERA_PINHOLE == t360::kCameraPinhole && T360_CAMERA_EQUIDISTANT == t360::kCameraEquidistant &&
+              T360_CAMERA_STEREOGRAPHIC == t360::kCameraStereographic && T360_CAMERA_PANNINI == t360::kCameraPannini);
+constexpr T360Camera kPinhole{T360_CAMERA_PINHOLE, 0.0f};
+
+// true, with the reason in *why, when a view of ctx's input (rig == nullptr) or of the rig cannot be rendered with this
+// pose and camera.  The output layout plays no part: the pose replaces it.
+bool cameraRefused(const FrameTransformContext& ctx, const T360LensRig* rig, const T360Pose* pose, const T360Camera* camera, std::string* why) {
   if (!pose) {
     *why = "a NULL pose";
     return true;
@@ -631,13 +635,39 @@ bool rectilinearRefused(const FrameTransformContext& ctx, const T360LensRig* rig
                      pose->vfov);
     return true;
   }
-  if (!(pose->hfov > 0.0f && pose->hfov <= 179.0f) || !(pose->vfov > 0.0f && pose->vfov <= 179.0f)) {
-    *why = formatted("hfov %g and vfov %g must lie in (0, 179] degrees", pose->hfov, pose->vfov);
+  if (!camera) {
+    *why = "a NULL camera";
     return true;
   }
+  const float h = pose->hfov, v = pose->vfov;
+  switch (camera->model) {
+    case T360_CAMERA_PINHOLE:
+      if (!(h > 0.0f && h <= 179.0f) || !(v > 0.0f && v <= 179.0f)) *why = formatted("hfov %g and vfov %g must lie in (0, 179] degrees", h, v);
+      break;
+    case T360_CAMERA_EQUIDISTANT:
+      if (!(h > 0.0f && h <= 360.0f) || !(v > 0.0f && v <= 360.0f))
+        *why = formatted("hfov %g and vfov %g must lie in (0, 360] degrees for an equidistant camera", h, v);
+      break;
+    case T360_CAMERA_STEREOGRAPHIC:
+      if (!(h > 0.0f && h <= 359.0f) || !(v > 0.0f && v <= 359.0f))
+        *why = formatted("hfov %g and vfov %g must lie in (0, 359] degrees for a stereographic camera", h, v);
+      break;
+    case T360_CAMERA_PANNINI: {
+      const float d = camera->pannini;
+      if (!(d >= 0.0f && d <= 1.0f)) *why = formatted("the Pannini distance %g must lie in [0, 1]", d);
+      else if (!(h > 0.0f && h <= 359.0f) || !(v > 0.0f && v <= 179.0f))
+        *why = formatted("hfov %g must lie in (0, 359] and vfov %g in (0, 179] degrees for a Pannini camera", h, v);
+      else if (!(d + std::cos(static_cast<double>(h) * M_PI / 360.0) > 0.0))
+        *why = formatted("a Pannini camera with distance %g sees at most 2 acos(-%g) degrees across, not hfov %g", d, d, h);
+      break;
+    }
+    default:
+      *why = formatted("no camera model %d", camera->model);
+  }
+  if (!why->empty()) return true;
   if (rig && rigRefused(rig, why)) return true;
   if (ctx.enable_low_pass_filter) {
-    *why = "the low-pass filter is not available for a rectilinear view (set enable_low_pass_filter = 0)";
+    *why = "the low-pass filter is not available for a camera view (set enable_low_pass_filter = 0)";
     return true;
   }
   if (t360::kernelSizeOf(ctx.interpolation_alg) == 0) {
@@ -647,11 +677,36 @@ bool rectilinearRefused(const FrameTransformContext& ctx, const T360LensRig* rig
   return false;
 }
 
-// The per-frame constants of a pose: its rotation, and tan(hfov / 2), tan(vfov / 2) in double, stored as float
-t360::RectilinearCamera rectilinearCamera(const T360Pose& pose) {
-  return t360::RectilinearCamera{t360::rotationFromAngles(pose.yaw, pose.pitch, pose.roll),
-                                 static_cast<float>(std::tan(static_cast<double>(pose.hfov) * M_PI / 360.0)),
-                                 static_cast<float>(std::tan(static_cast<double>(pose.vfov) * M_PI / 360.0))};
+// The per-frame constants of a pose and camera (oriented_view.h: RectilinearCamera): the rotation, and the model's
+// constants in double, stored as float
+t360::RectilinearCamera cameraConstants(const T360Pose& pose, const T360Camera& camera) {
+  t360::RectilinearCamera c{};
+  c.r = t360::rotationFromAngles(pose.yaw, pose.pitch, pose.roll);
+  c.model = camera.model;
+  const double h = static_cast<double>(pose.hfov) * M_PI / 360.0, v = static_cast<double>(pose.vfov) * M_PI / 360.0;  // half angles
+  switch (camera.model) {
+    case T360_CAMERA_EQUIDISTANT:
+      c.cx = static_cast<float>(h);
+      c.cy = static_cast<float>(v);
+      break;
+    case T360_CAMERA_STEREOGRAPHIC:
+      c.cx = static_cast<float>(std::tan(h / 2.0));
+      c.cy = static_cast<float>(std::tan(v / 2.0));
+      break;
+    case T360_CAMERA_PANNINI: {
+      const double d = camera.pannini;
+      c.cx = static_cast<float>((d + 1.0) * std::sin(h) / (d + std::cos(h)));
+      c.cy = static_cast<float>(std::tan(v));
+      c.d = camera.pannini;
+      c.e = static_cast<float>(1.0 / (d + 1.0));
+      c.dd = static_cast<float>(1.0 - d * d);
+      break;
+    }
+    default:
+      c.cx = static_cast<float>(std::tan(h));
+      c.cy = static_cast<float>(std::tan(v));
+  }
+  return c;
 }
 
 // The geometry of one outW x outH plane of an inW x inH input in a rectilinear view: ctx's (its stereo formats and input
@@ -1256,17 +1311,18 @@ class VideoFrameTransform {
     });
   }
 
-  // Whole frame of a rectilinear view (T360B200_transformFrameRectilinearAsync): one gather launch for all planes, every
-  // record computed by rectilinearSample (oriented_view.h), so a pose gives what rectilinearMap -> generateMapFromWarp plans
-  // for it.  rig == nullptr: the context's input under BORDER_WRAP; else the rig's lenses under BORDER_TRANSPARENT, with the
-  // lens call's pre-fill.  Needs no plan and leaves the plans alone; no tables.
-  bool transformFrameRectilinear(const char* what, const T360LensRig* rig, const T360Pose* pose, const FramePlanes& f, cudaStream_t stream) {
-    auto refused = [&](const FrameTransformContext& ctx, std::string* why) { return rectilinearRefused(ctx, rig, pose, why); };
+  // Whole frame of a camera view (T360B200_transformFrameCameraAsync, T360B200_transformFrameRectilinearAsync): one gather
+  // launch for all planes, every record computed by rectilinearSample (oriented_view.h), so a pose and camera give what
+  // cameraMap -> generateMapFromWarp plans for them.  rig == nullptr: the context's input under BORDER_WRAP; else the rig's
+  // lenses under BORDER_TRANSPARENT, with the lens call's pre-fill.  Needs no plan and leaves the plans alone; no tables.
+  bool transformFrameCamera(const char* what, const T360LensRig* rig, const T360Pose* pose, const T360Camera* camera, const FramePlanes& f,
+                            cudaStream_t stream) {
+    auto refused = [&](const FrameTransformContext& ctx, std::string* why) { return cameraRefused(ctx, rig, pose, camera, why); };
     return unplannedFrame(what, stream, refused, [&](const FrameTransformContext& ctx, int, cudaStream_t s) {
       t360::PerFrameGatherParams gp{};
       gp.lens = rig != nullptr;
       for (int p = 0; p < f.numPlanes; ++p) gp.plane[p].geometry = rectilinearGeometry(ctx, gp.lens, f.inW[p], f.inH[p], f.outW[p], f.outH[p]);
-      gp.camera = rectilinearCamera(*pose);
+      gp.camera = cameraConstants(*pose, *camera);
       if (rig) gp.rig = lensRigModel(*rig);
       perFrameGather(t360::PerFrameSource::kRectilinear, gp, ctx, f, f.in, f.inPitch, nullptr, gp.lens, nullptr, nullptr, nullptr, s);
       return true;
@@ -2678,19 +2734,19 @@ T360_API int T360B200_transformFrameLensBlendAsync(VideoFrameTransform* t, const
   if (!describeFrame(what, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, f)) return 0;
   return t->transformFrameLens(what, rig, &seamWidth, orientation, f, static_cast<cudaStream_t>(stream));
 }
-T360_API int T360B200_rectilinearMap(const FrameTransformContext* ctx, const T360LensRig* rig, const T360Pose* pose, int inW, int inH, int outW,
-                                     int outH, float* map) {
-  const char* what = "Could not compute the rectilinear map";
+namespace {
+int cameraMap(const char* what, const FrameTransformContext* ctx, const T360LensRig* rig, const T360Pose* pose, const T360Camera* camera,
+              int inW, int inH, int outW, int outH, float* map) {
   std::string why;
   if (!ctx) why = "a NULL context";
-  else if (rectilinearRefused(*ctx, rig, pose, &why)) {}
+  else if (cameraRefused(*ctx, rig, pose, camera, &why)) {}
   else if (!map || inW <= 0 || inH <= 0 || outW <= 0 || outH <= 0) why = "a NULL map or a plane size that is not positive";
   if (!why.empty()) {
     std::printf("%s. Error: %s\n", what, why.c_str());
     return 0;
   }
   const t360::SphereGeometry g = rectilinearGeometry(*ctx, rig != nullptr, inW, inH, outW, outH);
-  const t360::RectilinearCamera c = rectilinearCamera(*pose);
+  const t360::RectilinearCamera c = cameraConstants(*pose, *camera);
   const t360::LensRigModel model = rig ? lensRigModel(*rig) : t360::LensRigModel{};
   for (int i = 0; i < outH; ++i)
     for (int j = 0; j < outW; ++j) {
@@ -2700,17 +2756,37 @@ T360_API int T360B200_rectilinearMap(const FrameTransformContext* ctx, const T36
     }
   return 1;
 }
-T360_API int T360B200_transformFrameRectilinearAsync(VideoFrameTransform* t, const T360LensRig* rig, const T360Pose* pose, int numPlanes,
-                                                     const uint8_t* const* dIn, uint8_t* const* dOut, const int* inW, const int* inH,
-                                                     const int* inPitch, const int* outW, const int* outH, const int* outPitch, void* stream) {
-  const char* what = "Could not transform the frame with a rectilinear view";
+int transformFrameCamera(const char* what, VideoFrameTransform* t, const T360LensRig* rig, const T360Pose* pose, const T360Camera* camera,
+                         int numPlanes, const uint8_t* const* dIn, uint8_t* const* dOut, const int* inW, const int* inH, const int* inPitch,
+                         const int* outW, const int* outH, const int* outPitch, void* stream) {
   if (!t) {
     std::printf("%s. Error: a NULL argument\n", what);
     return 0;
   }
   FramePlanes f;
   if (!describeFrame(what, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, f)) return 0;
-  return t->transformFrameRectilinear(what, rig, pose, f, static_cast<cudaStream_t>(stream));
+  return t->transformFrameCamera(what, rig, pose, camera, f, static_cast<cudaStream_t>(stream));
+}
+}  // namespace
+T360_API int T360B200_cameraMap(const FrameTransformContext* ctx, const T360LensRig* rig, const T360Pose* pose, const T360Camera* camera, int inW,
+                                int inH, int outW, int outH, float* map) {
+  return cameraMap("Could not compute the camera map", ctx, rig, pose, camera, inW, inH, outW, outH, map);
+}
+T360_API int T360B200_transformFrameCameraAsync(VideoFrameTransform* t, const T360LensRig* rig, const T360Pose* pose, const T360Camera* camera,
+                                                int numPlanes, const uint8_t* const* dIn, uint8_t* const* dOut, const int* inW, const int* inH,
+                                                const int* inPitch, const int* outW, const int* outH, const int* outPitch, void* stream) {
+  return transformFrameCamera("Could not transform the frame with a camera view", t, rig, pose, camera, numPlanes, dIn, dOut, inW, inH, inPitch,
+                              outW, outH, outPitch, stream);
+}
+T360_API int T360B200_rectilinearMap(const FrameTransformContext* ctx, const T360LensRig* rig, const T360Pose* pose, int inW, int inH, int outW,
+                                     int outH, float* map) {
+  return cameraMap("Could not compute the rectilinear map", ctx, rig, pose, &kPinhole, inW, inH, outW, outH, map);
+}
+T360_API int T360B200_transformFrameRectilinearAsync(VideoFrameTransform* t, const T360LensRig* rig, const T360Pose* pose, int numPlanes,
+                                                     const uint8_t* const* dIn, uint8_t* const* dOut, const int* inW, const int* inH,
+                                                     const int* inPitch, const int* outW, const int* outH, const int* outPitch, void* stream) {
+  return transformFrameCamera("Could not transform the frame with a rectilinear view", t, rig, pose, &kPinhole, numPlanes, dIn, dOut, inW, inH,
+                              inPitch, outW, outH, outPitch, stream);
 }
 T360_API void T360B200_setPinHostPlanes(VideoFrameTransform* t, int enable) { if (t) t->setPinHostPlanes(enable != 0); }
 T360_API void T360B200_debugTrace(VideoFrameTransform* t, int enable) { if (t) t->enableTrace(enable != 0); }

@@ -17,8 +17,8 @@
 //     lensSample), quantised like a map entry.
 //   - a two-lens rig with a feathered seam (LensBlendPositions): both lenses' records and a weight (lensBlendSample); the
 //     tile loop gathers the second record only where the weight blends the two.
-//   - a rectilinear view (RectilinearPositions): a pinhole ray per pixel, rotated, then the context's input lookup or the
-//     lens model (oriented_view.h: rectilinearSample).
+//   - a camera view (RectilinearPositions): the camera model's ray per pixel (a pinhole launch in a loop of its own),
+//     rotated, then the context's input lookup or the lens model (oriented_view.h: rectilinearSample).
 // In all six, the records come from the same host/device functions the planner (or its host twin) uses: bit-identical.
 #include "gather_common.cuh"
 
@@ -205,16 +205,28 @@ struct LensBlendPositions : NoTables {
   }
 };
 
-// A rectilinear view: the pinhole ray, the rotation and the input lookup per pixel, no tables.  LENS: the rig's lenses
-// (rectilinearSample<true>) with BORDER_TRANSPARENT instead of the context's input with BORDER_WRAP
-template <int, bool LENS>
-struct RectilinearPositions : NoTables {
+// A camera view: the camera model's ray, the rotation and the input lookup per pixel, no tables.  LENS: the rig's lenses
+// (rectilinearSample<true>) with BORDER_TRANSPARENT instead of the context's input with BORDER_WRAP.  ANY_MODEL = false:
+// the launch's camera is a pinhole.
+template <bool LENS, bool ANY_MODEL>
+struct CameraPositions : NoTables {
   static constexpr bool kTransparent = LENS;
   using NoTables::NoTables;
   __device__ void record(const PerFrameGatherParams& p, const PerFramePlane& v, int, int, int i, int j, int* col0, int* rowPhase) const {
-    rectilinearSample<LENS>(v.geometry, p.camera, p.rig, i, j, col0, rowPhase);
+    rectilinearSample<LENS, ANY_MODEL>(v.geometry, p.camera, p.rig, i, j, col0, rowPhase);
   }
 };
+// The kernel runs a pinhole launch (the rectilinear views) through its own tile loop, Pinhole, so the model switch costs
+// those views nothing per pixel; the other models take the loop with the switch.
+template <int, bool LENS>
+struct RectilinearPositions : CameraPositions<LENS, true> {
+  using Pinhole = CameraPositions<LENS, false>;
+  using CameraPositions<LENS, true>::CameraPositions;
+};
+template <class Pos, class = void>
+struct HasPinholeLoop : std::false_type {};
+template <class Pos>
+struct HasPinholeLoop<Pos, std::void_t<typename Pos::Pinhole>> : std::true_type {};
 
 // The weights are staged first.  A policy with per-tile tables publishes them with its first beginTile __syncthreads;
 // without tables no tile synchronises, so the kernel does it here.
@@ -227,6 +239,13 @@ perFrameGatherKernel(const __grid_constant__ PerFrameGatherParams p, int numTile
   if constexpr (K >= 2) {
     stageWeights<K>(p.weights, smem);
     if constexpr (Pos::kTableBytes == 0) __syncthreads();
+  }
+  if constexpr (HasPinholeLoop<Pos>::value) {
+    if (p.camera.model == kCameraPinhole) {
+      typename Pos::Pinhole pinhole(smem + (K >= 2 ? weightBytes<K>() : 0));
+      gatherViewTiles<K, Pos::kTransparent>(p, numTiles, smem, pinhole);
+      return;
+    }
   }
   gatherViewTiles<K, Pos::kTransparent>(p, numTiles, smem, pos);
 }

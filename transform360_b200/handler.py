@@ -118,6 +118,24 @@ def as_pose(pose) -> T360Pose:
     return pose if isinstance(pose, T360Pose) else T360Pose(*[float(v) for v in pose])
 
 
+T360_CAMERA_PINHOLE, T360_CAMERA_EQUIDISTANT, T360_CAMERA_STEREOGRAPHIC, T360_CAMERA_PANNINI = 0, 1, 2, 3
+
+
+class T360Camera(C.Structure):
+    """The camera model of a view (include/transform360_b200.h): T360_CAMERA_*, and Pannini's d (read by T360_CAMERA_PANNINI
+    only)."""
+    _fields_ = [("model", C.c_int), ("pannini", C.c_float)]
+
+
+def as_camera(camera) -> T360Camera:
+    """A T360Camera from a T360Camera, a model, or a (model, pannini) sequence."""
+    if isinstance(camera, T360Camera):
+        return camera
+    if isinstance(camera, (tuple, list)):
+        return T360Camera(int(camera[0]), float(camera[1]))
+    return T360Camera(int(camera), 0.0)
+
+
 class T360Lens(C.Structure):
     """One fisheye lens (include/transform360_b200.h): OpenCV fisheye intrinsics fx, fy, cx, cy in pixels of the rig's
     calibration frame, distortion k1..k4, extrinsics yaw / pitch / roll in degrees, and the half field of view it covers."""
@@ -229,6 +247,11 @@ def load(path: os.PathLike | None = None):
     L.T360B200_rectilinearMap.argtypes = [C.POINTER(FrameTransformContext), C.POINTER(T360LensRig), C.POINTER(T360Pose)] + [ci] * 4 + [vp]
     L.T360B200_transformFrameRectilinearAsync.restype = ci
     L.T360B200_transformFrameRectilinearAsync.argtypes = [vp, C.POINTER(T360LensRig), C.POINTER(T360Pose), ci] + planes
+    L.T360B200_cameraMap.restype = ci
+    L.T360B200_cameraMap.argtypes = [C.POINTER(FrameTransformContext), C.POINTER(T360LensRig), C.POINTER(T360Pose),
+                                     C.POINTER(T360Camera)] + [ci] * 4 + [vp]
+    L.T360B200_transformFrameCameraAsync.restype = ci
+    L.T360B200_transformFrameCameraAsync.argtypes = [vp, C.POINTER(T360LensRig), C.POINTER(T360Pose), C.POINTER(T360Camera), ci] + planes
     L.T360B200_setPinHostPlanes.restype = None
     L.T360B200_setPinHostPlanes.argtypes = [vp, ci]
     L.T360B200_debugTrace.restype = None
@@ -262,7 +285,7 @@ EXPORTED_SYMBOLS = [
     "T360B200_transformFrameViewAsync", "T360B200_viewSamples",
     "T360B200_transformFrameOrientedAsync", "T360B200_orientedSamples", "T360B200_transformFramePoseAsync", "T360B200_poseSamples",
     "T360B200_lensMap", "T360B200_transformFrameLensAsync", "T360B200_lensBlendMaps", "T360B200_transformFrameLensBlendAsync",
-    "T360B200_rectilinearMap", "T360B200_transformFrameRectilinearAsync",
+    "T360B200_rectilinearMap", "T360B200_transformFrameRectilinearAsync", "T360B200_cameraMap", "T360B200_transformFrameCameraAsync",
     "T360B200_setPinHostPlanes", "T360B200_debugTrace", "T360B200_debugTraceRead", "T360B200_synchronize", "T360B200_stream", "T360B200_kernelLaunchCount", "T360B200_planDeviceBytes",
     "T360B200_planTileCounts", "T360B200_deviceCount", "T360B200_version",
 ]
@@ -381,6 +404,14 @@ class VideoFrameTransform:
         roll, hfov, vfov)), looking into the context's input, or into `rig` (a T360LensRig) when one is given."""
         n, enqueue = self._frame_call("T360B200_transformFrameRectilinearAsync", in_planes, out_planes, dims)
         return lambda pose, stream=0, rig=None: enqueue((C.byref(rig) if rig is not None else None, C.byref(as_pose(pose)), n), stream)
+
+    def make_camera_frame_call(self, in_planes, out_planes, dims):
+        """Like make_rectilinear_frame_call, for T360B200_transformFrameCameraAsync: returns a callable f(pose, camera,
+        stream, rig=None) -> bool that enqueues the whole frame with `pose` and `camera` (a T360Camera, a T360_CAMERA_*
+        model, or (model, pannini))."""
+        n, enqueue = self._frame_call("T360B200_transformFrameCameraAsync", in_planes, out_planes, dims)
+        return lambda pose, camera, stream=0, rig=None: enqueue(
+            (C.byref(rig) if rig is not None else None, C.byref(as_pose(pose)), C.byref(as_camera(camera)), n), stream)
 
     def generate_map_from_warp(self, map, in_w: int, in_h: int, plan_index: int, border: int = BORDER_WRAP) -> bool:
         """T360B200_generateMapFromWarp: installs plan index `plan_index` from a caller's warp map (float32 [h][w][2], the
@@ -636,6 +667,16 @@ def rectilinear_map(ctx: FrameTransformContext, pose, in_w, in_h, out_w, out_h, 
     if not load().T360B200_rectilinearMap(C.byref(ctx), C.byref(rig) if rig is not None else None, C.byref(as_pose(pose)), in_w, in_h,
                                           out_w, out_h, out.ctypes.data):
         raise ValueError("T360B200_rectilinearMap refused the arguments (message on stdout)")
+    return out
+
+
+def camera_map(ctx: FrameTransformContext, pose, camera, in_w, in_h, out_w, out_h, rig: T360LensRig | None = None) -> np.ndarray:
+    """rectilinear_map with a camera model (T360B200_cameraMap, no CUDA): `camera` a T360Camera, a T360_CAMERA_* model, or
+    (model, pannini).  generate_map_from_warp plans it for a fixed pose and camera as it plans rectilinear_map's map."""
+    out = np.zeros((max(out_h, 0), max(out_w, 0), 2), np.float32)
+    if not load().T360B200_cameraMap(C.byref(ctx), C.byref(rig) if rig is not None else None, C.byref(as_pose(pose)),
+                                     C.byref(as_camera(camera)), in_w, in_h, out_w, out_h, out.ctypes.data):
+        raise ValueError("T360B200_cameraMap refused the arguments (message on stdout)")
     return out
 
 
