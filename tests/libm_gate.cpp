@@ -11,6 +11,7 @@
 #include <thread>
 #include <vector>
 
+#include "atan2_pairs.h"
 #include "libm_ports.h"
 
 namespace {
@@ -38,31 +39,12 @@ void checkPair(uint32_t yb, uint32_t xb) {
   if (want != got) report("atan2f", yb, xb, want, got);
 }
 
-uint64_t splitmix(uint64_t& s) {
-  uint64_t z = (s += 0x9e3779b97f4a7c15ull);
-  z = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9ull;
-  z = (z ^ (z >> 27)) * 0x94d049bb133111ebull;
-  return z ^ (z >> 31);
-}
-
-// n pairs from stream `seed`: a quarter arbitrary bit patterns, the rest y = x * r with |r| near atanf's range splits
-// (7/16, 11/16, 19/16, 39/16), near 1, and near the 2^+-60 / 2^24 cut-offs, with random signs
-void randomPairs(uint64_t seed, uint64_t n) {
-  static const float kRatios[] = {0.4375f, 0.6875f, 1.1875f, 2.4375f, 1.0f, 0.5f, 0x1p24f, 0x1p60f, 0x1p-60f, 0x1p-29f};
-  uint64_t s = seed;
-  for (uint64_t i = 0; i < n; ++i) {
-    const uint64_t r = splitmix(s);
-    const uint32_t a = static_cast<uint32_t>(r), b = static_cast<uint32_t>(r >> 32);
-    if ((i & 3) == 0) {
-      checkPair(a, b);
-      continue;
-    }
-    // x: any finite float of moderate exponent; y = x * ratio, nudged by a few ulps either way
-    const float x = t360::bitsFloat((a & 0x807fffffu) | ((100u + (a >> 23) % 56u) << 23));
-    const float ratio = kRatios[(b >> 8) % (sizeof(kRatios) / sizeof(kRatios[0]))];
-    const int nudge = static_cast<int>(b & 0x3f) - 32;
-    const uint32_t yb = t360::floatBits(x * ratio) + static_cast<uint32_t>(nudge);
-    checkPair((yb & 0x7fffffffu) | ((b >> 16 & 1u) << 31), t360::floatBits(x));
+// pairs [begin, end) of stream `seed` (atan2_pairs.h)
+void randomPairs(uint64_t seed, uint64_t begin, uint64_t end) {
+  for (uint64_t i = begin; i < end; ++i) {
+    uint32_t y, x;
+    t360gate::atan2RandomPair(seed, i, &y, &x);
+    checkPair(y, x);
   }
 }
 
@@ -74,14 +56,11 @@ int main(int argc, char** argv) {
   const unsigned long long seed = argc > 3 ? std::strtoull(argv[3], nullptr, 10) : 1;
 
   // every combination of the special values
-  std::vector<uint32_t> special = {0x00000000u, 0x00000001u, 0x00000002u, 0x003fffffu, 0x007fffffu, 0x00800000u, 0x00800001u,
-                                   0x3f800000u, 0x3f7fffffu, 0x3f800001u, 0x3ee00000u, 0x3edfffffu, 0x3f300000u, 0x3f2fffffu,
-                                   0x3f980000u, 0x3f97ffffu, 0x401c0000u, 0x401bffffu, 0x4c000000u, 0x4bffffffu, 0x31000000u,
-                                   0x30ffffffu, 0x7f7fffffu, 0x7f800000u, 0x7fc00000u, 0x7f800001u, 0x7fffffffu, 0x3f000000u};
-  const size_t base = special.size();
-  for (size_t i = 0; i < base; ++i) special.push_back(special[i] | 0x80000000u);
-  for (uint32_t y : special)
-    for (uint32_t x : special) checkPair(y, x);
+  for (int k = 0; k < t360gate::kAtan2Specials * t360gate::kAtan2Specials; ++k) {
+    uint32_t y, x;
+    t360gate::atan2SpecialPair(k, &y, &x);
+    checkPair(y, x);
+  }
 
   std::vector<std::thread> pool;
   const uint64_t total = 1ull << 32, chunk = total / threads + 1;
@@ -90,11 +69,11 @@ int main(int argc, char** argv) {
       const uint64_t b = t * chunk, e = b + chunk < total ? b + chunk : total;
       checkUnary("asinf", asinf, t360::libmAsinf, b, e);
       checkUnary("atanf", atanf, t360::libmAtanf, b, e);
-      randomPairs(seed * 1000003ull + t, pairs / threads + (static_cast<unsigned long long>(t) < pairs % threads ? 1 : 0));
+      randomPairs(seed, pairs * t / threads, pairs * (t + 1) / threads);
     });
   }
   for (auto& th : pool) th.join();
-  std::printf("asinf: 2^32 inputs, atanf: 2^32 inputs, atan2f: %llu random + %zu special pairs; %llu mismatches\n", pairs,
-              special.size() * special.size(), gMismatches.load());
+  std::printf("asinf: 2^32 inputs, atanf: 2^32 inputs, atan2f: %llu random + %d special pairs; %llu mismatches\n", pairs,
+              t360gate::kAtan2Specials * t360gate::kAtan2Specials, gMismatches.load());
   return gMismatches.load() ? 1 : 0;
 }

@@ -174,6 +174,30 @@ def test_recurring_pageable_planes_can_be_pinned_in_place(torch_cuda):
             assert np.array_equal(out, co.transform_plane(octx, plan, src, ow, oh))
 
 
+@pytest.mark.parametrize("out_first", [False, True])
+def test_pinned_planes_that_share_a_page(torch_cuda, out_first):
+    """Pinning registers whole pages, so the input plane's registration takes in the first (or last) page of an output
+    plane that shares a page with it.  The output must still be copied, and bit-exact, on every frame: the library merges
+    the two registrations instead of leaving the output partly page-locked."""
+    case = SMALL["lp_tiles"]
+    ctx, octx = _ctxs(case)
+    iw, ih, ow, oh, idx = plane_dims(case, 0)
+    pool = np.zeros(iw * ih + ow * oh + 2 * 4096, np.uint8)
+    base = (-pool.ctypes.data) % 4096 + 1000  # neither plane starts or ends on a page boundary
+    first, second = (ow * oh, iw * ih) if out_first else (iw * ih, ow * oh)
+    a, b = pool[base:base + first], pool[base + first:base + first + second]
+    src, out = (b, a) if out_first else (a, b)
+    src, out = src.reshape(ih, iw), out.reshape(oh, ow)
+    plan = co.OraclePlan(octx, iw, ih, ow, oh)
+    with t360.VideoFrameTransform(ctx) as vft:
+        vft.set_pin_host_planes(True)
+        assert vft.generateMapForPlane(iw, ih, ow, oh, 0)
+        for frame in range(4):
+            src[...] = co.noise_plane(iw, ih, frame=frame)
+            vft.transform_plane(src, ow, oh, 0, out=out)
+            assert np.array_equal(out, co.transform_plane(octx, plan, src, ow, oh)), frame
+
+
 def test_errors_follow_the_reference_contract(torch_cuda):
     ctx = t360.make_context(enable_low_pass_filter=0)
     src = np.zeros((32, 64), np.uint8)

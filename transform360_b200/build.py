@@ -20,6 +20,10 @@ LIB_DIR = PKG / "lib"
 LIB = LIB_DIR / "libTransform360.so"
 SOURCES = ["geometry.cpp", "lowpass_plan.cpp", "lowpass_jobs.cpp", "sampling.cpp", "gather_plan.cpp", "kernels.cu", "gather_frame.cu", "view_gather.cu", "video_frame_transform.cpp"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+# host code: -ffp-contract=off keeps the planner's float sequence identical to the reference's build, and the host twins
+# of the per-frame position chains (csrc/flat_view.h, libm_ports.h, oriented_view.h) plain IEEE operations.
+# tests/test_device_twins.py builds its host / device comparison with the same string.
+HOST_FLAGS = "-fPIC,-fvisibility=hidden,-ffp-contract=off,-fno-fast-math,-Wall"
 
 
 def nvcc_path() -> str:
@@ -44,9 +48,7 @@ def build(force: bool = False, verbose: bool = False, out: Path | None = None) -
         return LIB
     out = out or LIB
     LIB_DIR.mkdir(exist_ok=True)
-    # host code: -ffp-contract=off keeps the planner's float sequence identical to the reference's build
-    host_flags = "-fPIC,-fvisibility=hidden,-ffp-contract=off,-fno-fast-math,-Wall"
-    cmd = [nvcc_path(), *ARCH, "-O3", "-lineinfo", "-std=c++17", "--shared", "-Xcompiler", host_flags,
+    cmd = [nvcc_path(), *ARCH, "-O3", "-lineinfo", "-std=c++17", "--shared", "-Xcompiler", HOST_FLAGS,
            "-Xptxas", "-v" if verbose else "-warn-spills", "-I", str(ROOT / "include"), "-I", str(CSRC),
            "-o", str(out)] + [str(CSRC / s) for s in SOURCES]
     env = dict(os.environ)
@@ -65,11 +67,10 @@ def build_static(verbose: bool = False) -> Path:
     LIB_DIR.mkdir(exist_ok=True)
     obj_dir = LIB_DIR / "obj"
     obj_dir.mkdir(exist_ok=True)
-    host_flags = "-fPIC,-fvisibility=hidden,-ffp-contract=off,-fno-fast-math,-Wall"
     objs = []
     for src in SOURCES:
         o = obj_dir / (Path(src).stem + ".o")
-        cmd = [nvcc_path(), *ARCH, "-O3", "-lineinfo", "-std=c++17", "-c", "-Xcompiler", host_flags, "-I", str(ROOT / "include"),
+        cmd = [nvcc_path(), *ARCH, "-O3", "-lineinfo", "-std=c++17", "-c", "-Xcompiler", HOST_FLAGS, "-I", str(ROOT / "include"),
                "-I", str(CSRC), "-o", str(o), str(CSRC / src)]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if verbose or r.returncode != 0:

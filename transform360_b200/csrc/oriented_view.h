@@ -556,6 +556,38 @@ struct RectilinearCamera {
   float d, e, dd;  // kCameraPannini: d, 1 / (d + 1), 1 - d^2
 };
 
+// The per-frame constants of a pose (degrees) and a camera model: the rotation, and the model's constants in double,
+// stored as float.  Host only: the device receives the result (T360B200_cameraMap and the camera kernels).
+inline RectilinearCamera cameraConstants(int model, float pannini, float yaw, float pitch, float roll, float hfov, float vfov) {
+  RectilinearCamera c{};
+  c.r = rotationFromAngles(yaw, pitch, roll);
+  c.model = model;
+  const double h = static_cast<double>(hfov) * M_PI / 360.0, v = static_cast<double>(vfov) * M_PI / 360.0;  // half angles
+  switch (model) {
+    case kCameraEquidistant:
+      c.cx = static_cast<float>(h);
+      c.cy = static_cast<float>(v);
+      break;
+    case kCameraStereographic:
+      c.cx = static_cast<float>(std::tan(h / 2.0));
+      c.cy = static_cast<float>(std::tan(v / 2.0));
+      break;
+    case kCameraPannini: {
+      const double d = pannini;
+      c.cx = static_cast<float>((d + 1.0) * std::sin(h) / (d + std::cos(h)));
+      c.cy = static_cast<float>(std::tan(v));
+      c.d = pannini;
+      c.e = static_cast<float>(1.0 / (d + 1.0));
+      c.dd = static_cast<float>(1.0 - d * d);
+      break;
+    }
+    default:
+      c.cx = static_cast<float>(std::tan(h));
+      c.cy = static_cast<float>(std::tan(v));
+  }
+  return c;
+}
+
 // sin(rho) / rho (1 at rho = 0) and cos(rho) for rho in [0, pi sqrt 2] from + - * / only: h = rho / 4, the Taylor
 // polynomials of sin(h) / h and cos(h) in h^2 (|h| <= 1.12: the first dropped terms are below 1e-9), then two angle
 // doublings: sin 2h / 2h = (sin h / h) cos h, cos 2h = 1 - 2 sin^2 h.  tests/test_camera_models.py compares it with

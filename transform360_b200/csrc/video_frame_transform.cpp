@@ -677,36 +677,9 @@ bool cameraRefused(const FrameTransformContext& ctx, const T360LensRig* rig, con
   return false;
 }
 
-// The per-frame constants of a pose and camera (oriented_view.h: RectilinearCamera): the rotation, and the model's
-// constants in double, stored as float
+// The per-frame constants of a pose and camera (oriented_view.h: cameraConstants)
 t360::RectilinearCamera cameraConstants(const T360Pose& pose, const T360Camera& camera) {
-  t360::RectilinearCamera c{};
-  c.r = t360::rotationFromAngles(pose.yaw, pose.pitch, pose.roll);
-  c.model = camera.model;
-  const double h = static_cast<double>(pose.hfov) * M_PI / 360.0, v = static_cast<double>(pose.vfov) * M_PI / 360.0;  // half angles
-  switch (camera.model) {
-    case T360_CAMERA_EQUIDISTANT:
-      c.cx = static_cast<float>(h);
-      c.cy = static_cast<float>(v);
-      break;
-    case T360_CAMERA_STEREOGRAPHIC:
-      c.cx = static_cast<float>(std::tan(h / 2.0));
-      c.cy = static_cast<float>(std::tan(v / 2.0));
-      break;
-    case T360_CAMERA_PANNINI: {
-      const double d = camera.pannini;
-      c.cx = static_cast<float>((d + 1.0) * std::sin(h) / (d + std::cos(h)));
-      c.cy = static_cast<float>(std::tan(v));
-      c.d = camera.pannini;
-      c.e = static_cast<float>(1.0 / (d + 1.0));
-      c.dd = static_cast<float>(1.0 - d * d);
-      break;
-    }
-    default:
-      c.cx = static_cast<float>(std::tan(h));
-      c.cy = static_cast<float>(std::tan(v));
-  }
-  return c;
+  return t360::cameraConstants(camera.model, camera.pannini, pose.yaw, pose.pitch, pose.roll, pose.hfov, pose.vfov);
 }
 
 // The geometry of one outW x outH plane of an inW x inH input in a rectilinear view: ctx's (its stereo formats and input
@@ -923,14 +896,15 @@ class VideoFrameTransform {
       const uint8_t* dIn = in;
       uint8_t* dOut = out;
       int dInPitch = inPitch, dOutPitch = outPitch;
+      // (both planes before any copy: pinning one may re-register a range the other one is copied from)
+      if (!inOnDevice) pinIfRecurring(in, static_cast<size_t>(inPitch) * (inH - 1) + inW);
+      if (!outOnDevice) pinIfRecurring(out, static_cast<size_t>(outPitch) * (outH - 1) + outW);
       if (!inOnDevice) {
-        pinIfRecurring(in, static_cast<size_t>(inPitch) * (inH - 1) + inW);
         dInPitch = scratchPlane(stagingIn_, inW, inH);
         CU(cudaMemcpy2DAsync(stagingIn_.ptr, dInPitch, in, inPitch, inW, inH, cudaMemcpyHostToDevice, stream_));
         dIn = stagingIn_.ptr;
       }
       if (!outOnDevice) {
-        pinIfRecurring(out, static_cast<size_t>(outPitch) * (outH - 1) + outW);
         dOutPitch = scratchPlane(stagingOut_, outW, outH);
         dOut = stagingOut_.ptr;
         // a transparent luma plane keeps the caller's bytes (renderTarget): they go into the staging plane first
@@ -1523,10 +1497,32 @@ class VideoFrameTransform {
   // (T360B200_setPinHostPlanes or T360B200_PIN_HOST_PLANES=1), a plane address seen for the second time is page-locked
   // in place with cudaHostRegister so that later frames in the same buffer are DMA'd directly.  Opt-in because the
   // caller must not free such a buffer while the transform is alive (it is unregistered in the destructor).
+  // A registration covers whole pages, so it can take in the first or last page of another caller plane.  The runtime
+  // takes a plane whose first byte is registered for page-locked memory throughout and refuses a copy that runs past
+  // the registration (cudaErrorInvalidValue), so a plane that overlaps one of these registrations without lying inside
+  // it is merged into it (one registration of the union), or, if that fails, the registration is dropped.  Called for
+  // both planes of a call before its first copy, with nothing in flight.
   void pinIfRecurring(const void* ptr, size_t bytes) {
-    if (!pinHostPlanes_ || !ptr || !bytes || memoryTypeOf(ptr) != cudaMemoryTypeUnregistered) return;
+    if (!pinHostPlanes_ || !ptr || !bytes) return;
     const uintptr_t page = 4096, lo = reinterpret_cast<uintptr_t>(ptr) & ~(page - 1);
     const size_t len = ((reinterpret_cast<uintptr_t>(ptr) + bytes + page - 1) & ~(page - 1)) - lo;
+    for (HostRange& r : hostRanges_) {
+      if (!r.pinned || lo + len <= r.base || lo >= r.base + r.bytes) continue;
+      if (lo >= r.base && lo + len <= r.base + r.bytes) return;  // inside a registration: page-locked already
+      for (PlaneGraph& g : planeGraphs_) cudaGraphExecDestroy(g.exec);  // (their copies assumed the old registration)
+      planeGraphs_.clear();
+      cudaHostUnregister(reinterpret_cast<void*>(r.base));
+      const uintptr_t ulo = std::min(lo, r.base), uhi = std::max(lo + len, r.base + r.bytes);
+      if (cudaHostRegister(reinterpret_cast<void*>(ulo), uhi - ulo, cudaHostRegisterDefault) == cudaSuccess) {
+        r.base = ulo;
+        r.bytes = uhi - ulo;
+        return;
+      }
+      cudaGetLastError();
+      r.pinned = false;
+      r.seen = -1000000;  // its planes go through the bounce buffers from now on
+    }
+    if (memoryTypeOf(ptr) != cudaMemoryTypeUnregistered) return;
     for (HostRange& r : hostRanges_) {
       if (r.base != lo || r.bytes != len) continue;
       if (!r.pinned && ++r.seen >= 2) {
