@@ -429,6 +429,72 @@ int T360B200_transformFrameCameraAsync(VideoFrameTransform* transform, const T36
                                        int numPlanes, const uint8_t* const* deviceInputs, uint8_t* const* deviceOutputs,
                                        const int* inputWidths, const int* inputHeights, const int* inputPitches, const int* outputWidths,
                                        const int* outputHeights, const int* outputPitches, void* cudaStream);
+/* ---- anti-aliased camera views ----------------------------------------------------------------------
+ * The camera views above sample the input at one point per output pixel, as cv::remap does, so a view much smaller than
+ * the part of the input it covers (a dome master or a little planet of an 8K input, a thumbnail) aliases.  These calls
+ * sample an input pyramid instead, each pixel at the level its footprint asks for (Williams 1983), the footprint from ray
+ * differentials (Igehy 1999).  For each plane of inW x inH rendered at mapW x mapH:
+ *   1. pyramid: level 0 is the input plane; level l + 1 is cv::resize(level l, (ceil(W_l / 2), ceil(H_l / 2)),
+ *      INTER_AREA) (exact 2 x 2 cells as (sum + 2) >> 2, other sizes with OpenCV's area taps).  The plane's top level T is
+ *      the largest l <= maxLevel whose sides are both >= 8 (0 if none), so a small chroma plane may stop before its luma
+ *      plane.  Each plane has its own pyramid;
+ *   2. footprint: X, Y as in steps 1-3 of the camera views; dX = 2 / mapW (4 / mapW with an LR output split) and dY =
+ *      2 / mapH (4 / mapH with a TB split) are one column / row of one eye, computed on the host in double and stored as
+ *      float (as dX / 2 and dY / 2).  rx = R (q(X + dX/2, Y) - q(X - dX/2, Y)) and ry = R (q(X, Y + dY/2) - q(X, Y - dY/2)),
+ *      q the model's ray of step 4 and R the rotation of step 5.  With t the pixel's rotated ray, a = J rx and b = J ry,
+ *      J the Jacobian at t of the input lookup the pixel takes, in level-0 pixels of the plane (the input eye re-pack's
+ *      halving included):
+ *        equirect    du = inW / 2pi (z dx - x dz) / (x^2 + z^2),
+ *                    dv = inH / pi (dy (x^2 + z^2) - y (x dx + z dz)) / ((x^2 + y^2 + z^2) sqrt(x^2 + z^2));
+ *        CUBEMAP_32  on the face the lookup picks, major component m and face coordinates a, b: du = inW / (6 e)
+ *                    (da m - a dm) / m^2, dv = inH / (4 e) (db m - b dm) / m^2, e = input_expand_coef;
+ *        a rig       on the lens the lookup picks, (X, Y, Z) its camera coordinates, rho = |(X, Y)|, theta = atan2(rho,
+ *                    Z), s = theta_d / rho, theta_d' = 1 + 3 k1 theta^2 + 5 k2 theta^4 + 7 k3 theta^6 + 9 k4 theta^8:
+ *                    drho = (X dX + Y dY) / rho, dtheta = (Z drho - rho dZ) / (rho^2 + Z^2), ds = (theta_d' dtheta -
+ *                    s drho) / rho, dx' = s dX + X ds, dy' = s dY + Y ds, a = (fx / calibWidth inW dx', fy / calibHeight
+ *                    inH dy'); at rho = 0 dx' = dX / Z, dy' = dY / Z (infinite for Z <= 0).
+ *      Every step in float with + - * / and sqrt only (no libm function is differentiated), as the chains above;
+ *   3. level and weight: rho^2 = max(a.a, b.b) (NaN-propagating); lambda = ((int32) bits(rho^2) - 0x3f800000) >> 16
+ *      (arithmetic shift) + round(256 lodBias) (half away from zero, on the host): 1/2 log2 rho^2 in 1/256 of a level, with a
+ *      log2 that is exact at powers of two and linear between them (at most 0.043 level off); lambda = 256 T where rho^2
+ *      is not below +inf (an equirect's exact pole).  level = clamp(lambda >> 8, 0, T); the weight of the next level
+ *      w = lambda & 255 where 0 <= lambda < 256 T, else 0;
+ *   4. records: (px, py) the pixel's T360B200_cameraMap entry; at level l >= 1 px_l = ((px + 0.5) sx_l) - 0.5 and likewise
+ *      py_l, sx_l = W_l / W_0 and sy_l = H_l / H_0 computed in double and stored as float, each step rounded to float (at
+ *      level 0 the entry as it is).  Each entry is quantised as cv::remap quantises a CV_32FC2 map;
+ *   5. pixel: a = the gather of level `level`, b = the gather of level + 1 where w > 0; the pixel is
+ *      (a (256 - w) + b w + 128) >> 8.  Without a rig every level is sampled with BORDER_WRAP at its own size; with a rig
+ *      BORDER_TRANSPARENT, and where one of the two samples is skipped the other stands alone, where both are the output
+ *      keeps its bytes (the pre-fill of the camera views).
+ * maxLevel = 0 is T360B200_transformFrameCameraAsync exactly (one launch, no pyramid); a frame whose planes all have T = 0
+ * is too.  Else a frame takes T_max + 1 launches: one per pyramid level over every plane that has it, then the gather.
+ * There is no planned path for a fixed pose: a plan carries one record per pixel.
+ *
+ * Refused, with 0 and a message on stdout before any CUDA call: every refusal of the camera views, a NULL minify, maxLevel
+ * outside [0, 8], and a lodBias that is not finite or lies outside [-4, 4]. */
+typedef struct T360Minify {
+  int maxLevel;  /* 0..8: pyramid levels above the input; 0 = T360B200_transformFrameCameraAsync exactly */
+  float lodBias; /* levels added to every pixel's level of detail, finite, in [-4, 4] (> 0 blurs, < 0 sharpens) */
+} T360Minify;
+/* Host only, no CUDA: the twin of one plane of inputWidth x inputHeight.  map0 / map1: float32 [outputHeight][outputWidth]
+ * [2], the entry of each pixel in its level's pixels / in level + 1's pixels (NaN where the weight is 0); level: uint8
+ * [outputHeight][outputWidth]; weight: uint16, w of step 3.  cv::remap of each level's entries over the pyramid
+ * (cv::resize with INTER_AREA, repeated), combined as in step 5, gives the plane of T360B200_transformFrameCameraMipAsync
+ * bit for bit.  maxLevel = 0 gives T360B200_cameraMap's map, level 0 and weight 0.  Returns 1; 0 (message) for the refusals
+ * above, a NULL context or array, or non-positive sizes. */
+int T360B200_cameraMipMaps(const FrameTransformContext* ctx, const T360LensRig* rig, const T360Pose* pose, const T360Camera* camera,
+                           const T360Minify* minify, int inputWidth, int inputHeight, int outputWidth, int outputHeight, float* map0,
+                           float* map1, uint8_t* level, uint16_t* weight);
+/* One frame of an anti-aliased camera view: T360B200_transformFrameCameraAsync's arguments and asynchronous contract, plus
+ * `minify`, which may change every frame like the rig, pose and camera.  Needs no plan and does not touch the plans; takes
+ * the reader lock; never synchronises the device.  The pyramids live in per-stream scratch of about a third of the input
+ * planes, grown on demand.  Returns 1 if everything was enqueued; 0 with a message on stdout, before any CUDA call, for
+ * the refusals above, 0 or more than 3 planes, or an invalid plane description. */
+int T360B200_transformFrameCameraMipAsync(VideoFrameTransform* transform, const T360LensRig* rig, const T360Pose* pose,
+                                          const T360Camera* camera, const T360Minify* minify, int numPlanes,
+                                          const uint8_t* const* deviceInputs, uint8_t* const* deviceOutputs, const int* inputWidths,
+                                          const int* inputHeights, const int* inputPitches, const int* outputWidths,
+                                          const int* outputHeights, const int* outputPitches, void* cudaStream);
 /* Opt-in (also: environment T360B200_PIN_HOST_PLANES=1): page-lock pageable caller planes in place the second time
  * the same buffer is seen (cudaHostRegister), so that recycled frame-pool buffers are DMA'd at full PCIe speed.  The
  * caller must keep such buffers alive until VideoFrameTransform_delete. */

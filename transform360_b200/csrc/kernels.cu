@@ -389,6 +389,66 @@ __global__ void __launch_bounds__(256) areaResizeKernel(AreaParams p) {
   p.dst[(size_t)dy * p.dstPitch + dx] = (uint8_t)min(max(v, 0), 255);
 }
 
+// One level of the input pyramids of a frame's planes (PyramidParams): INTER_AREA to half the size, rounded up.  Exact
+// 2 x 2 cells: a thread sums two rows of 8 source bytes (two 8-byte loads where the rows are 8-byte aligned, as the
+// pyramid's own levels always are) into 4 output bytes, (sum + 2) >> 2, stored as one word.  Other sizes (an odd side):
+// areaResizeKernel's tap arithmetic, 4 output pixels per thread 32 columns apart.
+__global__ void __launch_bounds__(256) pyramidLevelKernel(const __grid_constant__ PyramidParams p) {
+  const int b = blockIdx.x;
+  const int pl = (p.numPlanes > 2 && b >= p.plane[2].firstBlock) ? 2 : ((p.numPlanes > 1 && b >= p.plane[1].firstBlock) ? 1 : 0);
+  const PyramidPlane& v = p.plane[pl];
+  const int t = b - v.firstBlock, by = t / v.blocksX, bx = t - by * v.blocksX;
+  const int dy = by * kPyramidBlockH + (threadIdx.x >> 5);
+  if (dy >= v.dstH) return;
+  const int lane = threadIdx.x & 31;
+  uint8_t* drow = v.dst + (size_t)dy * v.dstPitch;
+  if (!v.xTaps) {
+    const int dx = bx * kPyramidBlockW + lane * 4;
+    if (dx >= v.dstW) return;
+    const uint8_t* r0 = v.src + (size_t)(2 * dy) * v.srcPitch + 2 * dx;
+    const uint8_t* r1 = r0 + v.srcPitch;
+    if (dx + 4 <= v.dstW && ((reinterpret_cast<uintptr_t>(r0) | reinterpret_cast<uintptr_t>(r1)) & 7) == 0 &&
+        (reinterpret_cast<uintptr_t>(drow + dx) & 3) == 0) {
+      const uint2 a = __ldg(reinterpret_cast<const uint2*>(r0)), c = __ldg(reinterpret_cast<const uint2*>(r1));
+      uint32_t out = 0;
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const uint32_t wa = k < 2 ? a.x : a.y, wc = k < 2 ? c.x : c.y;
+        const int sh = (k & 1) * 16;
+        const int sum = ((wa >> sh) & 255) + ((wa >> (sh + 8)) & 255) + ((wc >> sh) & 255) + ((wc >> (sh + 8)) & 255);
+        out |= (uint32_t)((sum + 2) >> 2) << (8 * k);
+      }
+      *reinterpret_cast<uint32_t*>(drow + dx) = out;
+    } else {
+      for (int k = 0; k < 4 && dx + k < v.dstW; ++k) {
+        const int sum = __ldg(r0 + 2 * k) + __ldg(r0 + 2 * k + 1) + __ldg(r1 + 2 * k) + __ldg(r1 + 2 * k + 1);
+        drow[dx + k] = (uint8_t)((sum + 2) >> 2);
+      }
+    }
+    return;
+  }
+  const int y0 = __ldg(v.yFirst + dy), y1 = __ldg(v.yFirst + dy + 1);
+#pragma unroll 1
+  for (int k = 0; k < 4; ++k) {
+    const int dx = bx * kPyramidBlockW + k * 32 + lane;
+    if (dx >= v.dstW) break;
+    const int x0 = __ldg(v.xFirst + dx), x1 = __ldg(v.xFirst + dx + 1);
+    float sum = 0.f;
+    for (int j = y0; j < y1; ++j) {
+      const int2 ty = __ldg(v.yTaps + j);
+      const uint8_t* row = v.src + (size_t)ty.x * v.srcPitch;
+      float buf = 0.f;
+      for (int i = x0; i < x1; ++i) {
+        const int2 tx = __ldg(v.xTaps + i);
+        buf = __fadd_rn(buf, __fmul_rn((float)__ldg(row + tx.x), __int_as_float(tx.y)));
+      }
+      const float term = __fmul_rn(__int_as_float(ty.y), buf);
+      sum = j == y0 ? term : __fadd_rn(sum, term);
+    }
+    drow[dx] = (uint8_t)min(max(__float2int_rn(sum), 0), 255);
+  }
+}
+
 template <int K, bool T>
 cudaError_t launchGatherK(const GatherParams& p, int numSMs, cudaStream_t stream) {
   static DeviceLaunchCfg cfgs;  // per kernel instantiation, one entry per device
@@ -458,6 +518,21 @@ cudaError_t launchAreaResize(const AreaParams& p, cudaStream_t stream) {
   const dim3 grid((p.dstW + 31) / 32, (p.dstH + 7) / 8);
   if (p.cellW < 0) areaEnlargeKernel<<<grid, 256, 0, stream>>>(p);
   else areaResizeKernel<<<grid, 256, 0, stream>>>(p);
+  gLaunches.fetch_add(1, std::memory_order_relaxed);
+  return cudaGetLastError();
+}
+
+cudaError_t launchPyramidLevel(PyramidParams p, cudaStream_t stream) {
+  if (p.numPlanes < 1 || p.numPlanes > kMaxFramePlanes) return cudaErrorInvalidValue;
+  int blocks = 0;
+  for (int i = 0; i < p.numPlanes; ++i) {
+    PyramidPlane& v = p.plane[i];
+    v.blocksX = (v.dstW + kPyramidBlockW - 1) / kPyramidBlockW;
+    v.firstBlock = blocks;
+    blocks += v.blocksX * ((v.dstH + kPyramidBlockH - 1) / kPyramidBlockH);
+  }
+  if (blocks <= 0) return cudaSuccess;
+  pyramidLevelKernel<<<blocks, 256, 0, stream>>>(p);
   gLaunches.fetch_add(1, std::memory_order_relaxed);
   return cudaGetLastError();
 }

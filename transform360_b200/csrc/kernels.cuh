@@ -314,6 +314,27 @@ struct AreaParams {
 };
 cudaError_t launchAreaResize(const AreaParams& p, cudaStream_t stream);
 
+// One level of the input pyramids of a frame's planes in ONE launch (T360B200_transformFrameCameraMipAsync): dst =
+// cv::resize(src, (ceil(srcW / 2), ceil(srcH / 2)), INTER_AREA) for every plane listed.  xTaps == nullptr: exact 2 x 2
+// cells, (sum + 2) >> 2, four output bytes per thread; else the tap tables of buildAreaResize (AreaParams' layout) in
+// OpenCV's accumulation order.  A block takes 128 x 8 output pixels; blocks are numbered through the planes in order.
+struct PyramidPlane {
+  const uint8_t* src;
+  uint8_t* dst;
+  int srcW, srcH, srcPitch, dstW, dstH, dstPitch;
+  const int2* xTaps;
+  const int* xFirst;
+  const int2* yTaps;
+  const int* yFirst;
+  int firstBlock, blocksX;  // filled by launchPyramidLevel
+};
+struct PyramidParams {
+  PyramidPlane plane[kMaxFramePlanes];
+  int numPlanes;
+};
+constexpr int kPyramidBlockW = 128, kPyramidBlockH = 8;
+cudaError_t launchPyramidLevel(PyramidParams p, cudaStream_t stream);
+
 // The register-resident low-pass (hy <= kStripMaxHy) of 1-3 planes in ONE launch (StripJob::edge carries the plane in
 // bits 8-9; kxOffset / kyOffset index the tap buffer, merged for several planes: lowpass_jobs.h): a frame takes one launch
 // and one tail instead of three launches on three streams; a single plane's list has plane 0 throughout.
@@ -370,8 +391,11 @@ void countKernelLaunches(long long n);  // kernels launched through a replayed C
 //                 pixel gathers the lens that carries it (lens 0 unless the weight w of lens 1 is 256), and a second time,
 //                 lens 1, only where both carry weight; the two values are blended as (a (256 - w) + b w + 128) >> 8;
 //   kRectilinear  perspective views posed per frame (camera; rectilinearSample): a pinhole ray per pixel, no tables, looked
-//                 up in the context's input (BORDER_WRAP) or, with lens set, in the rig's lenses (BORDER_TRANSPARENT).
-enum class PerFrameSource { kView, kSphere, kMap, kLens, kLensBlend, kRectilinear };
+//                 up in the context's input (BORDER_WRAP) or, with lens set, in the rig's lenses (BORDER_TRANSPARENT);
+//   kCameraMip    anti-aliased camera views (camera, mip, mipBias; mipCameraSample): kRectilinear's chain plus the pixel's
+//                 footprint, which picks a level of the plane's pyramid and the weight w (0..255) of the next one; the
+//                 pixel gathers its level, and the next level only where w > 0, blended as kLensBlend blends.
+enum class PerFrameSource { kView, kSphere, kMap, kLens, kLensBlend, kRectilinear, kCameraMip };
 struct PerFramePlane {
   const uint8_t* src;  // (blurred) input plane, geometry.inW x geometry.inH
   uint8_t* dst;        // render target, geometry.mapW x geometry.mapH
@@ -396,6 +420,17 @@ struct PerFrameGatherParams {
   bool lens;         // kRectilinear: the rig's lenses instead of the context's input
   const int16_t* weights;  // device copy of the [1024][k][k] table (nullptr for nearest)
   int kernelSize;
+  // kCameraMip: per plane its footprint constants and pyramid levels 1..geometry.top (level 0 is the plane's src), and
+  // round(256 lodBias)
+  struct MipLevel {
+    uint8_t* bytes;  // written by the level's pyramid launch, read by the gather
+    int w, h, pitch;
+  };
+  struct MipPlane {
+    MipGeometry geometry;
+    MipLevel level[kMipMaxLevels];  // [l - 1]: level l
+  } mip[kMaxFramePlanes];
+  int mipBias;
 };
 // a CTA takes tiles of 32 output columns x viewTileRows(k) rows; a thread owns one column of a tile and walks down
 // kViewRowsPerThread of its rows

@@ -686,6 +686,246 @@ T360_HD void rectilinearSample(const SphereGeometry& g, const RectilinearCamera&
   *rowPhase = r0 * 1024 + fracY * 32 + fracX;
 }
 
+// ---- anti-aliased camera views (T360B200_cameraMipMaps, T360B200_transformFrameCameraMipAsync) -----------------------
+// A camera view sampled from an input pyramid (level l + 1 = INTER_AREA of level l to half its size, rounded up), each
+// pixel at the level its footprint asks for (Williams 1983), the footprint from ray differentials (Igehy 1999):
+//   rx = R (q(X + dX/2, Y) - q(X - dX/2, Y)), ry = R (q(X, Y + dY/2) - q(X, Y - dY/2)) (q: the model's ray, R: the pose),
+//   a = J rx, b = J ry with J the Jacobian, at the pixel's rotated ray t, of the input lookup the pixel takes, in level-0
+//   pixels of the plane; rho^2 = max(a.a, b.b); lambda = 1/2 log2 rho^2 in 1/256 level from the float's bits.
+// The Jacobians are written out analytically with + - * / and sqrt (the lookup's atan2 / asin are not differentiated
+// through libm; a lens's theta, which its projection needs anyway, is libmAtan2f), so host and device agree bit for bit.
+constexpr int kMipMaxLevels = 8;
+struct MipGeometry {
+  float halfX, halfY;             // dX / 2, dY / 2: one column / row of one eye in X and Y (host, double -> float)
+  int top;                        // the plane's top level T (0: no pyramid)
+  float sx[kMipMaxLevels + 1];    // W_l / W_0, H_l / H_0 (host, double -> float; [0] unused)
+  float sy[kMipMaxLevels + 1];
+};
+
+// The pyramid of a w x h plane for maxLevel: its top level T, the largest l <= maxLevel whose sides ceil(w / 2^l),
+// ceil(h / 2^l) are both >= 8 (0 if there is none), and the sides of levels 0..T.  The one place the level sizes are
+// walked: the host twin's constants (mipGeometry), the frame call's scratch and launches, and the kernel's level table all
+// take them from here.
+struct MipSizes {
+  int top;
+  int w[kMipMaxLevels + 1], h[kMipMaxLevels + 1];
+};
+T360_HD MipSizes mipSizes(int w, int h, int maxLevel) {
+  MipSizes m{};
+  m.w[0] = w;
+  m.h[0] = h;
+  while (m.top < maxLevel && (m.w[m.top] + 1) / 2 >= 8 && (m.h[m.top] + 1) / 2 >= 8) {
+    m.w[m.top + 1] = (m.w[m.top] + 1) / 2;
+    m.h[m.top + 1] = (m.h[m.top] + 1) / 2;
+    ++m.top;
+  }
+  return m;
+}
+
+// The footprint constants of one plane of a camera view (g: the camera view's geometry) for maxLevel: dX / 2 and dY / 2
+// (one column / row of one eye), the top level, and the levels' size ratios, in double and stored as float.  Host only:
+// the device receives the result (T360B200_cameraMipMaps and the frame call).
+inline MipGeometry mipGeometry(const SphereGeometry& g, int maxLevel) {
+  const MipSizes z = mipSizes(g.inW, g.inH, maxLevel);
+  MipGeometry m{};
+  m.halfX = static_cast<float>((g.splitLR ? 2.0 : 1.0) / g.mapW);
+  m.halfY = static_cast<float>((g.splitTB ? 2.0 : 1.0) / g.mapH);
+  m.top = z.top;
+  for (int l = 0; l <= z.top; ++l) {
+    m.sx[l] = static_cast<float>(static_cast<double>(z.w[l]) / g.inW);
+    m.sy[l] = static_cast<float>(static_cast<double>(z.h[l]) / g.inH);
+  }
+  return m;
+}
+
+// The pixel's X, Y (steps 1-3 of the camera contract, +-1 at the plane's outer pixel edges) and its output eye
+T360_HD void cameraXY(const SphereGeometry& g, int i, int j, float* X, float* Y, bool* eye) {
+  float x = pixelCentre(j, g.mapW), y = pixelCentre(i, g.mapH);
+  *eye = false;
+  if (g.splitLR) *eye = splitEye(x, false);
+  else if (g.splitTB) *eye = splitEye(y, g.vflip);
+  y = fSub(1.0f, y);
+  *X = fSub(fMul(2.0f, x), 1.0f);
+  *Y = fSub(fMul(2.0f, y), 1.0f);
+}
+
+// The ray q (not rotated, not normalised) of any model, the pinhole's as rectilinearPoint writes it
+T360_HD SphereVec modelRay(const RectilinearCamera& c, float X, float Y) {
+  if (c.model == kCameraPinhole) return SphereVec{fMul(X, c.cx), fMul(Y, c.cy), 1.0f};
+  return cameraRay(c, X, Y);
+}
+
+// R (q(X1, Y1) - q(X0, Y0)): the rotated ray differential between two points of the image plane
+T360_HD SphereVec rayDifferential(const RectilinearCamera& c, float X0, float Y0, float X1, float Y1) {
+  const SphereVec a = modelRay(c, X1, Y1), b = modelRay(c, X0, Y0);
+  return rotateHD(c.r, SphereVec{fSub(a.x, b.x), fSub(a.y, b.y), fSub(a.z, b.z)});
+}
+
+// The chart Jacobian of the equirect lookup u = atan2(x, z) / 2pi + 1/2, v = 1/2 - asin(y / |t|) / pi at t, applied to
+// ray differential d, in level-0 pixels (the input eye re-pack's halving included):
+//   du = su (z dx - x dz) / (x^2 + z^2),                         su = inW / 2pi
+//   dv = sv (dy (x^2 + z^2) - y (x dx + z dz)) / (|t|^2 sqrt(x^2 + z^2)),  sv = inH / pi  (the sign is dropped)
+// At a pole (x = z = 0) the quotients are infinite or NaN.
+T360_HD void equirectJacobian(const SphereGeometry& g, const SphereVec& t, const SphereVec& d, float* du, float* dv) {
+  const float su = fMul(static_cast<float>(g.inW), g.packLR ? 0.0795774715f : 0.159154943f);
+  const float sv = fMul(static_cast<float>(g.inH), g.packTB ? 0.159154943f : 0.318309886f);
+  const float h2 = fAdd(fMul(t.x, t.x), fMul(t.z, t.z));
+  const float r2 = fAdd(h2, fMul(t.y, t.y));
+  *du = fDiv(fMul(su, fSub(fMul(t.z, d.x), fMul(t.x, d.z))), h2);
+  const float num = fSub(fMul(d.y, h2), fMul(t.y, fAdd(fMul(t.x, d.x), fMul(t.z, d.z))));
+  *dv = fDiv(fMul(sv, num), fMul(r2, fSqrt(h2)));
+}
+
+// The face cubeInputHD picks for the normalised direction (tx, ty, tz), its tests written as there: 0..5, -1 for none
+T360_HD int cubeInputFace(float tx, float ty, float tz) {
+#pragma unroll 1
+  for (int f = 0; f < 6; ++f) {
+    const float major = f < 2 ? tz : (f < 4 ? tx : ty);
+    const float a = f < 4 ? (f < 2 ? tx : tz) : tx, b = f < 4 ? ty : tz;
+    if ((f & 1) == 0 ? !(major <= -0.5f) : !(major >= 0.5f)) continue;
+    const float gx = fDiv(a, major), gy = fDiv(b, major);
+    if (gx >= -1.0f && gx <= 1.0f && gy >= -1.0f && gy <= 1.0f) return f;
+  }
+  return -1;
+}
+
+// The chart Jacobian of the CUBEMAP_32 lookup on face f (the gnomonic quotient rule: d(a / m) = (da m - a dm) / m^2, with
+// u = (col +- gx / e) / 6, v = (row +- gy / e) / 4), applied to d, in level-0 pixels
+T360_HD void cubeJacobian(const SphereGeometry& g, int f, const SphereVec& t, const SphereVec& d, float* du, float* dv) {
+  const float m = f < 2 ? t.z : (f < 4 ? t.x : t.y), dm = f < 2 ? d.z : (f < 4 ? d.x : d.y);
+  const float a = f < 4 ? (f < 2 ? t.x : t.z) : t.x, da = f < 4 ? (f < 2 ? d.x : d.z) : d.x;
+  const float b = f < 4 ? t.y : t.z, db = f < 4 ? d.y : d.z;
+  const float m2 = fMul(m, m);
+  const float su = fDiv(static_cast<float>(g.inW), fMul(g.packLR ? 12.0f : 6.0f, g.inputExpand));
+  const float sv = fDiv(static_cast<float>(g.inH), fMul(g.packTB ? 8.0f : 4.0f, g.inputExpand));
+  *du = fDiv(fMul(su, fSub(fMul(da, m), fMul(a, dm))), m2);
+  *dv = fDiv(fMul(sv, fSub(fMul(db, m), fMul(b, dm))), m2);
+}
+
+// The Kannala-Brandt projection's Jacobian for the lens lensPosition picks, applied to rx and ry, in level-0 pixels.
+// With rho = |(X, Y)|, theta = atan2(rho, Z), s = theta_d / rho (lensHit), theta_d'(theta) = 1 + 3 k1 t + 5 k2 t^2 +
+// 7 k3 t^3 + 9 k4 t^4 (t = theta^2):
+//   drho = (X dX + Y dY) / rho,  dtheta = (Z drho - rho dZ) / (rho^2 + Z^2),  ds = (theta_d' dtheta - s drho) / rho,
+//   dx' = s dX + X ds,  dy' = s dY + Y ds,  a = (ax inW dx', ay inH dy').
+// At rho = 0 (theta = 0 for Z > 0) the limit is dx' = dX / Z, dy' = dY / Z; on the back axis (Z <= 0) it is infinite.
+T360_HD void lensJacobian(const LensRigModel& rig, const SphereVec& t, const SphereVec& rx, const SphereVec& ry, int inW, int inH,
+                          float* a, float* b) {
+  const float z0 = lensRow(rig.lens[0].m + 6, t);
+  const float z1 = rig.numLenses > 1 ? lensRow(rig.lens[1].m + 6, t) : z0;
+  const LensModel& L = z1 > z0 ? rig.lens[1] : rig.lens[0];
+  const float X = lensRow(L.m, t), Y = lensRow(L.m + 3, t), Z = z1 > z0 ? z1 : z0;
+  const float cx = fMul(L.ax, static_cast<float>(inW)), cy = fMul(L.ay, static_cast<float>(inH));
+  const float rho = fSqrt(fAdd(fMul(X, X), fMul(Y, Y)));
+  const SphereVec* d[2] = {&rx, &ry};
+  float* out[2] = {a, b};
+  if (!(rho > 0.0f)) {
+    const float inv = Z > 0.0f ? fDiv(1.0f, Z) : bitsFloat(0x7f800000u);
+    for (int k = 0; k < 2; ++k) {
+      out[k][0] = fMul(cx, fMul(lensRow(L.m, *d[k]), inv));
+      out[k][1] = fMul(cy, fMul(lensRow(L.m + 3, *d[k]), inv));
+    }
+    return;
+  }
+  const float theta = libmAtan2f(rho, Z), tt = fMul(theta, theta);
+  const float poly = fAdd(1.0f, fMul(tt, fAdd(L.k[0], fMul(tt, fAdd(L.k[1], fMul(tt, fAdd(L.k[2], fMul(tt, L.k[3]))))))));
+  const float dpoly = fAdd(1.0f, fMul(tt, fAdd(fMul(3.0f, L.k[0]), fMul(tt, fAdd(fMul(5.0f, L.k[1]), fMul(tt, fAdd(fMul(7.0f, L.k[2]),
+                                                                                                           fMul(tt, fMul(9.0f, L.k[3])))))))));
+  const float s = fDiv(fMul(theta, poly), rho);
+  const float q2 = fAdd(fMul(rho, rho), fMul(Z, Z));
+  for (int k = 0; k < 2; ++k) {
+    const float dX = lensRow(L.m, *d[k]), dY = lensRow(L.m + 3, *d[k]), dZ = lensRow(L.m + 6, *d[k]);
+    const float drho = fDiv(fAdd(fMul(X, dX), fMul(Y, dY)), rho);
+    const float dtheta = fDiv(fSub(fMul(Z, drho), fMul(rho, dZ)), q2);
+    const float ds = fDiv(fSub(fMul(dpoly, dtheta), fMul(s, drho)), rho);
+    out[k][0] = fMul(cx, fAdd(fMul(s, dX), fMul(X, ds)));
+    out[k][1] = fMul(cy, fAdd(fMul(s, dY), fMul(Y, ds)));
+  }
+}
+
+// lambda256 = ((int32) bits(rho^2) - 0x3f800000) >> 16 + bias256 (1/2 log2 rho^2 in 1/256 level, piecewise linear between
+// powers of two), 256 T where rho^2 = max(aa, bb) is not below +inf; then the level clamp(lambda256 >> 8, 0, T) and the
+// weight of the next level, lambda256 & 255 where 0 <= lambda256 < 256 T and 0 elsewhere.  Returns the level.
+T360_HD int mipLevelOf(float aa, float bb, int top, int bias256, int* w) {
+  const float inf = bitsFloat(0x7f800000u);
+  int lam = 256 * top;
+  if (aa < inf && bb < inf) lam = ((static_cast<int32_t>(floatBits(aa > bb ? aa : bb)) - 0x3f800000) >> 16) + bias256;
+  *w = lam >= 0 && lam < 256 * top ? (lam & 255) : 0;
+  const int level = lam >> 8;
+  return level < 0 ? 0 : (level > top ? top : level);
+}
+
+// A level-0 position in level l's pixels, l >= 1: ((p + 0.5) s_l) - 0.5, each step rounded to float
+T360_HD float mipScale(float p, float s) { return fSub(fMul(fAdd(p, 0.5f), s), 0.5f); }
+
+// The footprint, level and map entries of output pixel (i, j) of an anti-aliased camera view: p0 = the camera view's entry
+// (rectilinearPosition's bits) in level `level`'s pixels, p1 = the entry in level + 1's pixels (NaN where *w = 0).
+// Returns the level.
+template <bool LENS>
+T360_HD int mipCameraPoint(const SphereGeometry& g, const RectilinearCamera& c, const LensRigModel& rig, const MipGeometry& m, int bias256,
+                           int i, int j, float* p0, float* p1, int* w) {
+  float X, Y;
+  bool eye;
+  cameraXY(g, i, j, &X, &Y, &eye);
+  const SphereVec t = rotateHD(c.r, modelRay(c, X, Y));
+  float px, py;
+  if constexpr (LENS) {
+    lensPosition(rig, t, g.inW, g.inH, &px, &py);
+  } else {
+    float u, v;
+    sphereInputHD(g, false, eye, t, &u, &v);
+    px = toPixel(u, g.inW);
+    py = toPixel(v, g.inH);
+  }
+  int level = 0;
+  *w = 0;
+  if (m.top > 0) {
+    const SphereVec rx = rayDifferential(c, fSub(X, m.halfX), Y, fAdd(X, m.halfX), Y);
+    const SphereVec ry = rayDifferential(c, X, fSub(Y, m.halfY), X, fAdd(Y, m.halfY));
+    float a[2], b[2];
+    if constexpr (LENS) {
+      lensJacobian(rig, t, rx, ry, g.inW, g.inH, a, b);
+    } else if (g.cubeInput) {
+      const float n = fSqrt(fAdd(fAdd(fMul(t.x, t.x), fMul(t.y, t.y)), fMul(t.z, t.z)));
+      const int f = cubeInputFace(fDiv(t.x, n), fDiv(t.y, n), fDiv(t.z, n));
+      const float nan = bitsFloat(0x7fc00000u);
+      a[0] = a[1] = b[0] = b[1] = nan;
+      if (f >= 0) {
+        cubeJacobian(g, f, t, rx, &a[0], &a[1]);
+        cubeJacobian(g, f, t, ry, &b[0], &b[1]);
+      }
+    } else {
+      equirectJacobian(g, t, rx, &a[0], &a[1]);
+      equirectJacobian(g, t, ry, &b[0], &b[1]);
+    }
+    level = mipLevelOf(fAdd(fMul(a[0], a[0]), fMul(a[1], a[1])), fAdd(fMul(b[0], b[0]), fMul(b[1], b[1])), m.top, bias256, w);
+  }
+  p0[0] = level ? mipScale(px, m.sx[level]) : px;
+  p0[1] = level ? mipScale(py, m.sy[level]) : py;
+  const float nan = bitsFloat(0x7fc00000u);
+  p1[0] = *w ? mipScale(px, m.sx[level + 1]) : nan;
+  p1[1] = *w ? mipScale(py, m.sy[level + 1]) : nan;
+  return level;
+}
+
+// The sampling records of output pixel (i, j) of an anti-aliased camera view: mipCameraPoint's entries quantised as
+// rectilinearSample quantises its entry (rec1 only where *w > 0).  Returns the level.
+template <bool LENS>
+T360_HD int mipCameraSample(const SphereGeometry& g, const RectilinearCamera& c, const LensRigModel& rig, const MipGeometry& m, int bias256,
+                            int i, int j, int32_t* rec0, int32_t* rec1, int* w) {
+  float p0[2], p1[2];
+  const int level = mipCameraPoint<LENS>(g, c, rig, m, bias256, i, j, p0, p1, w);
+  int r0, fracX, fracY;
+  quantizeAxis(p0[0], g.kernelSize, &rec0[0], &fracX);
+  quantizeAxis(p0[1], g.kernelSize, &r0, &fracY);
+  rec0[1] = r0 * 1024 + fracY * 32 + fracX;
+  if (*w) {
+    quantizeAxis(p1[0], g.kernelSize, &rec1[0], &fracX);
+    quantizeAxis(p1[1], g.kernelSize, &r0, &fracY);
+    rec1[1] = r0 * 1024 + fracY * 32 + fracX;
+  }
+  return level;
+}
+
 // Whether the per-frame orientation chain covers the layouts of `ctx`
 inline bool orientedLayouts(const FrameTransformContext& ctx) {
   const int o = ctx.output_layout, in = ctx.input_layout;

@@ -240,6 +240,7 @@ struct PlaneLane {
   cudaEvent_t done = nullptr;                        // recorded when this lane's plane has been enqueued completely
   DeviceBuffer<uint8_t> blurred;                     // low-pass output of this plane
   DeviceBuffer<uint8_t> scaled;                      // render target at map size when an area resize follows
+  DeviceBuffer<uint8_t> pyramid;                     // levels 1..T of this plane's input pyramid (anti-aliased camera views)
   DeviceBuffer<int> claimCounter;                    // dynamic tile scheduler of this lane's gather launch
 };
 
@@ -351,6 +352,14 @@ struct StreamSlot {
   size_t sphereAt[kPlaneLanes] = {SIZE_MAX, SIZE_MAX, SIZE_MAX};  // per plane: where its tables start in sphereBytes
   FrameTransformContext sphereCtx{};
   std::vector<int> sphereSizes;  // mapW, mapH per plane
+  // the INTER_AREA tap tables of the anti-aliased camera views' pyramid levels that are not exact 2 x 2 cells, and the
+  // plane sizes and top levels they were built for (VideoFrameTransform::buildPyramids)
+  UploadRing mipTaps;
+  std::vector<uint8_t> mipTapBytes;
+  struct MipTapsAt {
+    size_t xTaps = SIZE_MAX, xFirst, yTaps, yFirst;  // byte offsets in mipTapBytes (SIZE_MAX: exact 2 x 2 cells)
+  } mipTapAt[kPlaneLanes][t360::kMipMaxLevels];      // per plane and level l (at l - 1)
+  std::vector<int> mipSizes;                         // inW, inH, top per plane
 };
 
 // A w x h scratch plane in buf (a lane's or the staging planes), grown on demand: its pitch, 256-byte aligned
@@ -687,6 +696,32 @@ t360::RectilinearCamera cameraConstants(const T360Pose& pose, const T360Camera& 
 t360::SphereGeometry rectilinearGeometry(const FrameTransformContext& ctx, bool rig, int inW, int inH, int outW, int outH) {
   return t360::sphereGeometry(rig ? lensContext(ctx) : ctx, outW, outH, inW, inH, t360::kernelSizeOf(ctx.interpolation_alg));
 }
+
+// ---- anti-aliased camera views (T360B200_cameraMipMaps, T360B200_transformFrameCameraMipAsync; oriented_view.h:
+// mipCameraSample) -------------------------------------------------------------------------------------------------------
+// true, with the reason in *why, when `minify` is NULL or out of range (the camera's own checks: cameraRefused)
+bool minifyRefused(const T360Minify* minify, std::string* why) {
+  if (!minify) {
+    *why = "a NULL minify";
+    return true;
+  }
+  if (minify->maxLevel < 0 || minify->maxLevel > t360::kMipMaxLevels) {
+    *why = formatted("maxLevel %d is outside [0, %d]", minify->maxLevel, t360::kMipMaxLevels);
+    return true;
+  }
+  if (!std::isfinite(minify->lodBias) || !(minify->lodBias >= -4.0f && minify->lodBias <= 4.0f)) {
+    *why = formatted("lodBias %g must be finite and lie in [-4, 4]", minify->lodBias);
+    return true;
+  }
+  return false;
+}
+bool cameraMipRefused(const FrameTransformContext& ctx, const T360LensRig* rig, const T360Pose* pose, const T360Camera* camera,
+                      const T360Minify* minify, std::string* why) {
+  return cameraRefused(ctx, rig, pose, camera, why) || minifyRefused(minify, why);
+}
+
+// round(256 lodBias), half away from zero: the bias in 1/256 of a level
+int mipBias(const T360Minify& m) { return static_cast<int>(std::lround(256.0 * static_cast<double>(m.lodBias))); }
 
 }  // namespace
 
@@ -1301,6 +1336,129 @@ class VideoFrameTransform {
       perFrameGather(t360::PerFrameSource::kRectilinear, gp, ctx, f, f.in, f.inPitch, nullptr, gp.lens, nullptr, nullptr, nullptr, s);
       return true;
     });
+  }
+
+  // Whole frame of an anti-aliased camera view (T360B200_transformFrameCameraMipAsync): the pyramid of every plane, one
+  // launch per level over the planes that have it (buildPyramids), then one gather launch for all planes, every record
+  // computed by mipCameraSample (oriented_view.h), so a pose, camera and minify give what cameraMipMaps describes.  A frame
+  // whose planes all have top level 0 (maxLevel = 0, or planes too small for a level) is transformFrameCamera's.  Needs no
+  // plan and leaves the plans alone.
+  bool transformFrameCameraMip(const char* what, const T360LensRig* rig, const T360Pose* pose, const T360Camera* camera,
+                               const T360Minify* minify, const FramePlanes& f, cudaStream_t stream) {
+    std::string why;
+    if (minifyRefused(minify, &why)) {
+      std::printf("%s. Error: %s\n", what, why.c_str());
+      return false;
+    }
+    int topMax = 0;
+    for (int p = 0; p < f.numPlanes; ++p) topMax = std::max(topMax, t360::mipSizes(f.inW[p], f.inH[p], minify->maxLevel).top);
+    if (topMax == 0) return transformFrameCamera(what, rig, pose, camera, f, stream);
+    auto refused = [&](const FrameTransformContext& ctx, std::string* why) { return cameraRefused(ctx, rig, pose, camera, why); };
+    return unplannedFrame(what, stream, refused, [&](const FrameTransformContext& ctx, int, cudaStream_t s) {
+      t360::PerFrameGatherParams gp{};
+      gp.lens = rig != nullptr;
+      for (int p = 0; p < f.numPlanes; ++p) {
+        gp.plane[p].geometry = rectilinearGeometry(ctx, gp.lens, f.inW[p], f.inH[p], f.outW[p], f.outH[p]);
+        gp.mip[p].geometry = t360::mipGeometry(gp.plane[p].geometry, minify->maxLevel);
+      }
+      gp.camera = cameraConstants(*pose, *camera);
+      if (rig) gp.rig = lensRigModel(*rig);
+      gp.mipBias = mipBias(*minify);
+      UploadRing::Entry* staged = nullptr;
+      buildPyramids(f, gp, slotFor(s), s, &staged);
+      perFrameGather(t360::PerFrameSource::kCameraMip, gp, ctx, f, f.in, f.inPitch, nullptr, gp.lens, nullptr, nullptr, nullptr, s);
+      releaseAfter(staged, s);
+      return true;
+    });
+  }
+
+  // Levels 1..top of every plane's pyramid (gp.mip[p].geometry.top) into the slot's scratch, on s: level l of all planes
+  // that have it in one launch (launchPyramidLevel), so T_max launches.  Fills gp.mip[p].level.  The tap tables of the
+  // levels that are not exact 2 x 2 cells are built on the host when a plane size or top level changes and staged through
+  // the slot's upload ring (*staged: the entry to release after the gather).
+  void buildPyramids(const FramePlanes& f, t360::PerFrameGatherParams& gp, StreamSlot& slot, cudaStream_t s, UploadRing::Entry** staged) {
+    constexpr int kPitchAlign = 256;
+    // levels 1..top of plane p in its lane's scratch, one after the other, each at a 256-byte pitch
+    std::vector<int> key;
+    int topMax = 0;
+    for (int p = 0; p < f.numPlanes; ++p) {
+      const t360::MipSizes z = t360::mipSizes(f.inW[p], f.inH[p], gp.mip[p].geometry.top);
+      size_t at = 0;
+      for (int l = 1; l <= z.top; ++l) {
+        gp.mip[p].level[l - 1] = {nullptr, z.w[l], z.h[l], (z.w[l] + kPitchAlign - 1) / kPitchAlign * kPitchAlign};
+        at += static_cast<size_t>(gp.mip[p].level[l - 1].pitch) * z.h[l];
+      }
+      if (at) slot.lanes[p].pyramid.reserve(at + 64);
+      at = 0;
+      for (int l = 1; l <= z.top; ++l) {
+        t360::PerFrameGatherParams::MipLevel& L = gp.mip[p].level[l - 1];
+        L.bytes = slot.lanes[p].pyramid.ptr + at;
+        at += static_cast<size_t>(L.pitch) * L.h;
+      }
+      key.insert(key.end(), {f.inW[p], f.inH[p], z.top});
+      topMax = std::max(topMax, z.top);
+    }
+    // the tap tables of the levels that are not exact 2 x 2 cells, rebuilt when a plane size or top level changes
+    if (slot.mipSizes != key) {
+      std::vector<uint8_t>& b = slot.mipTapBytes;
+      b.clear();
+      auto append = [&b](const void* data, size_t bytes) {
+        b.resize((b.size() + 7) & ~size_t{7});
+        const size_t at = b.size();
+        b.insert(b.end(), static_cast<const uint8_t*>(data), static_cast<const uint8_t*>(data) + bytes);
+        return at;
+      };
+      auto packed = [](const t360::AreaAxis& a) {
+        std::vector<int2> v(a.taps.size());
+        for (size_t i = 0; i < v.size(); ++i) {
+          int bits;
+          std::memcpy(&bits, &a.taps[i].alpha, sizeof(bits));
+          v[i] = int2{a.taps[i].src, bits};
+        }
+        return v;
+      };
+      for (int p = 0; p < f.numPlanes; ++p) {
+        for (int l = 1; l <= gp.mip[p].geometry.top; ++l) {
+          const int w = l == 1 ? f.inW[p] : gp.mip[p].level[l - 2].w, h = l == 1 ? f.inH[p] : gp.mip[p].level[l - 2].h;
+          t360::AreaResizePlan r;
+          t360::buildAreaResize(w, h, gp.mip[p].level[l - 1].w, gp.mip[p].level[l - 1].h, r);
+          StreamSlot::MipTapsAt& at = slot.mipTapAt[p][l - 1];
+          at = {};
+          if (r.cellW == 0) {  // (else cellW == cellH == 2: the kernel's exact cells)
+            const std::vector<int2> xt = packed(r.x), yt = packed(r.y);
+            at.xTaps = append(xt.data(), xt.size() * sizeof(int2));
+            at.xFirst = append(r.x.first.data(), r.x.first.size() * sizeof(int));
+            at.yTaps = append(yt.data(), yt.size() * sizeof(int2));
+            at.yFirst = append(r.y.first.data(), r.y.first.size() * sizeof(int));
+          }
+        }
+      }
+      slot.mipSizes = key;
+    }
+    const uint8_t* taps = slot.mipTapBytes.empty() ? nullptr : stageUpload(slot.mipTaps, slot.mipTapBytes, s, staged);
+    for (int l = 1; l <= topMax; ++l) {
+      t360::PyramidParams pp{};
+      for (int p = 0; p < f.numPlanes; ++p) {
+        if (gp.mip[p].geometry.top < l) continue;
+        const t360::PerFrameGatherParams::MipLevel& dst = gp.mip[p].level[l - 1];
+        t360::PyramidPlane& v = pp.plane[pp.numPlanes++];
+        if (l == 1) {
+          v.src = f.in[p]; v.srcW = f.inW[p]; v.srcH = f.inH[p]; v.srcPitch = f.inPitch[p];
+        } else {
+          const t360::PerFrameGatherParams::MipLevel& below = gp.mip[p].level[l - 2];
+          v.src = below.bytes; v.srcW = below.w; v.srcH = below.h; v.srcPitch = below.pitch;
+        }
+        v.dst = dst.bytes; v.dstW = dst.w; v.dstH = dst.h; v.dstPitch = dst.pitch;
+        const StreamSlot::MipTapsAt& at = slot.mipTapAt[p][l - 1];
+        if (at.xTaps != SIZE_MAX) {
+          v.xTaps = reinterpret_cast<const int2*>(taps + at.xTaps);
+          v.xFirst = reinterpret_cast<const int*>(taps + at.xFirst);
+          v.yTaps = reinterpret_cast<const int2*>(taps + at.yTaps);
+          v.yFirst = reinterpret_cast<const int*>(taps + at.yFirst);
+        }
+      }
+      CU(t360::launchPyramidLevel(pp, s));
+    }
   }
 
   // The steps of the per-frame calls that need no plan (lens rigs, rectilinear views): under the reader lock, so frame-exact
@@ -2783,6 +2941,47 @@ T360_API int T360B200_transformFrameRectilinearAsync(VideoFrameTransform* t, con
                                                      const int* inPitch, const int* outW, const int* outH, const int* outPitch, void* stream) {
   return transformFrameCamera("Could not transform the frame with a rectilinear view", t, rig, pose, &kPinhole, numPlanes, dIn, dOut, inW, inH,
                               inPitch, outW, outH, outPitch, stream);
+}
+T360_API int T360B200_cameraMipMaps(const FrameTransformContext* ctx, const T360LensRig* rig, const T360Pose* pose, const T360Camera* camera,
+                                    const T360Minify* minify, int inW, int inH, int outW, int outH, float* map0, float* map1, uint8_t* level,
+                                    uint16_t* weight) {
+  const char* what = "Could not compute the camera mip maps";
+  std::string why;
+  if (!ctx) why = "a NULL context";
+  else if (cameraMipRefused(*ctx, rig, pose, camera, minify, &why)) {}
+  else if (!map0 || !map1 || !level || !weight || inW <= 0 || inH <= 0 || outW <= 0 || outH <= 0)
+    why = "a NULL map, level or weight array or a plane size that is not positive";
+  if (!why.empty()) {
+    std::printf("%s. Error: %s\n", what, why.c_str());
+    return 0;
+  }
+  const t360::SphereGeometry g = rectilinearGeometry(*ctx, rig != nullptr, inW, inH, outW, outH);
+  const t360::RectilinearCamera c = cameraConstants(*pose, *camera);
+  const t360::LensRigModel model = rig ? lensRigModel(*rig) : t360::LensRigModel{};
+  const t360::MipGeometry m = t360::mipGeometry(g, minify->maxLevel);
+  const int bias = mipBias(*minify);
+  for (int i = 0; i < outH; ++i)
+    for (int j = 0; j < outW; ++j) {
+      const size_t at = static_cast<size_t>(i) * outW + j;
+      int w;
+      level[at] = static_cast<uint8_t>(rig ? t360::mipCameraPoint<true>(g, c, model, m, bias, i, j, map0 + 2 * at, map1 + 2 * at, &w)
+                                           : t360::mipCameraPoint<false>(g, c, model, m, bias, i, j, map0 + 2 * at, map1 + 2 * at, &w));
+      weight[at] = static_cast<uint16_t>(w);
+    }
+  return 1;
+}
+T360_API int T360B200_transformFrameCameraMipAsync(VideoFrameTransform* t, const T360LensRig* rig, const T360Pose* pose, const T360Camera* camera,
+                                                   const T360Minify* minify, int numPlanes, const uint8_t* const* dIn, uint8_t* const* dOut,
+                                                   const int* inW, const int* inH, const int* inPitch, const int* outW, const int* outH,
+                                                   const int* outPitch, void* stream) {
+  const char* what = "Could not transform the frame with an anti-aliased camera view";
+  if (!t) {
+    std::printf("%s. Error: a NULL argument\n", what);
+    return 0;
+  }
+  FramePlanes f;
+  if (!describeFrame(what, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, f)) return 0;
+  return t->transformFrameCameraMip(what, rig, pose, camera, minify, f, static_cast<cudaStream_t>(stream));
 }
 T360_API void T360B200_setPinHostPlanes(VideoFrameTransform* t, int enable) { if (t) t->setPinHostPlanes(enable != 0); }
 T360_API void T360B200_debugTrace(VideoFrameTransform* t, int enable) { if (t) t->enableTrace(enable != 0); }

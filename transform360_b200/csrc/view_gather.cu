@@ -18,8 +18,10 @@
 //   - a two-lens rig with a feathered seam (LensBlendPositions): both lenses' records and a weight (lensBlendSample); the
 //     tile loop gathers the second record only where the weight blends the two.
 //   - a camera view (RectilinearPositions): the camera model's ray per pixel (a pinhole launch in a loop of its own),
-//     rotated, then the context's input lookup or the lens model (oriented_view.h: rectilinearSample).
-// In all six, the records come from the same host/device functions the planner (or its host twin) uses: bit-identical.
+//     rotated, then the context's input lookup or the lens model (oriented_view.h: rectilinearSample);
+//   - an anti-aliased camera view (MipCameraPositions): the same chain, the pixel's footprint from ray differentials, and
+//     two records at adjacent levels of the plane's input pyramid, blended by the footprint's weight (mipCameraSample).
+// In all seven, the records come from the same host/device functions the planner (or its host twin) uses: bit-identical.
 #include "gather_common.cuh"
 
 #include <algorithm>
@@ -44,7 +46,24 @@ __device__ __forceinline__ int viewPixel(const SrcView& s, const unsigned char* 
   }
 }
 
+// Level l >= 1 of a plane's pyramid (kCameraMip) as a source
+__device__ __forceinline__ SrcView mipView(const PerFrameGatherParams::MipLevel& l) {
+  SrcView s;
+  s.bytes = l.bytes;
+  s.misalign = (int)(reinterpret_cast<uintptr_t>(l.bytes) & 3);
+  s.words = reinterpret_cast<const uint32_t*>(l.bytes - s.misalign);
+  s.w = l.w; s.h = l.h; s.pitch = l.pitch;
+  return s;
+}
+template <class Pos, class = void>
+struct IsMip : std::false_type {};
+template <class Pos>
+struct IsMip<Pos, std::enable_if_t<Pos::kMip>> : std::true_type {};
+
 // TRANSPARENT (barrel layouts): BORDER_TRANSPARENT, a pixel whose anchor tap lies outside the source keeps its byte.
+// Positions::kMip (IsMip): record() returns the pixel's pyramid level and hands over its record there, the record at the
+// next level and that level's weight w (0..255); the next level is gathered only where w > 0, and blended as kBlend
+// blends.  (A branch of its own, so the other policies' loops are what they were.)
 // Positions::kBlend: its record() hands over two records and the weight w (0..256) of the second; the first is gathered
 // for every pixel, the second only where 0 < w < 256, and the two values are blended (PerFrameSource::kLensBlend).  Where
 // BORDER_TRANSPARENT skips one of the two, the other stands alone.
@@ -74,7 +93,17 @@ __device__ __forceinline__ void gatherViewTiles(const PerFrameGatherParams& p, i
       if (i >= v.geometry.mapH) break;
       int col0, rowPhase;
       int value;
-      if constexpr (Positions::kBlend) {
+      if constexpr (IsMip<Positions>::value) {
+        int32_t rec0[2], rec1[2];
+        int w;
+        const int level = pos.record(p, v, pl, i, j, rec0, rec1, &w);
+        value = viewPixel<K, TRANSPARENT>(level ? mipView(p.mip[pl].level[level - 1]) : s, smem, rec0[0], rec0[1]);
+        if (w > 0) {
+          const int b = viewPixel<K, TRANSPARENT>(mipView(p.mip[pl].level[level]), smem, rec1[0], rec1[1]);
+          value = value < 0 ? b : (b < 0 ? value : (value * (256 - w) + b * w + 128) >> 8);
+        }
+        if (TRANSPARENT && value < 0) continue;
+      } else if constexpr (Positions::kBlend) {
         int col1, rowPhase1, w;
         pos.record(p, v, lane, r, i, j, &col0, &rowPhase, &col1, &rowPhase1, &w);
         value = viewPixel<K, TRANSPARENT>(s, smem, col0, rowPhase);
@@ -223,6 +252,19 @@ struct RectilinearPositions : CameraPositions<LENS, true> {
   using Pinhole = CameraPositions<LENS, false>;
   using CameraPositions<LENS, true>::CameraPositions;
 };
+// An anti-aliased camera view (kCameraMip): the camera view's chain and the pixel's footprint (mipCameraSample) give its
+// pyramid level, its record there and, where the next level has weight, the record at the next level.  Every model in one
+// loop (no pinhole loop of its own).  LENS as for CameraPositions.
+template <int, bool LENS>
+struct MipCameraPositions : NoTables {
+  static constexpr bool kMip = true, kTransparent = LENS;
+  using NoTables::NoTables;
+  __device__ int record(const PerFrameGatherParams& p, const PerFramePlane& v, int pl, int i, int j, int32_t* rec0, int32_t* rec1,
+                        int* w) const {
+    return mipCameraSample<LENS>(v.geometry, p.camera, p.rig, p.mip[pl].geometry, p.mipBias, i, j, rec0, rec1, w);
+  }
+};
+
 template <class Pos, class = void>
 struct HasPinholeLoop : std::false_type {};
 template <class Pos>
@@ -304,6 +346,7 @@ cudaError_t launchPerFrameGather(PerFrameGatherParams p, PerFrameSource source, 
     case PerFrameSource::kLens: return launchPositions<LensPositions>(p, barrel, numTiles, numSMs, stream);
     case PerFrameSource::kLensBlend: return launchPositions<LensBlendPositions>(p, barrel, numTiles, numSMs, stream);
     case PerFrameSource::kRectilinear: return launchPositions<RectilinearPositions>(p, p.lens, numTiles, numSMs, stream);
+    case PerFrameSource::kCameraMip: return launchPositions<MipCameraPositions>(p, p.lens, numTiles, numSMs, stream);
   }
   return cudaErrorInvalidValue;
 }

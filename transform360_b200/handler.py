@@ -136,6 +136,30 @@ def as_camera(camera) -> T360Camera:
     return T360Camera(int(camera), 0.0)
 
 
+class T360Minify(C.Structure):
+    """The pyramid of an anti-aliased camera view (include/transform360_b200.h): maxLevel in 0..8 levels above the input (0:
+    the plain camera view), lodBias in [-4, 4] levels added to every pixel's level of detail."""
+    _fields_ = [("maxLevel", C.c_int), ("lodBias", C.c_float)]
+
+
+def as_minify(minify) -> T360Minify:
+    """A T360Minify from a T360Minify, a max level, or a (max_level, lod_bias) sequence."""
+    if isinstance(minify, T360Minify):
+        return minify
+    if isinstance(minify, (tuple, list)):
+        return T360Minify(int(minify[0]), float(minify[1]))
+    return T360Minify(int(minify), 0.0)
+
+
+def mip_level_sizes(w: int, h: int, max_level: int) -> list[tuple[int, int]]:
+    """The (width, height) of levels 0..T of a w x h plane's pyramid for max_level: each level half the one below, rounded
+    up, and T the largest level <= max_level whose sides are both >= 8."""
+    sizes = [(w, h)]
+    while len(sizes) <= max_level and (sizes[-1][0] + 1) // 2 >= 8 and (sizes[-1][1] + 1) // 2 >= 8:
+        sizes.append(((sizes[-1][0] + 1) // 2, (sizes[-1][1] + 1) // 2))
+    return sizes
+
+
 class T360Lens(C.Structure):
     """One fisheye lens (include/transform360_b200.h): OpenCV fisheye intrinsics fx, fy, cx, cy in pixels of the rig's
     calibration frame, distortion k1..k4, extrinsics yaw / pitch / roll in degrees, and the half field of view it covers."""
@@ -252,6 +276,12 @@ def load(path: os.PathLike | None = None):
                                      C.POINTER(T360Camera)] + [ci] * 4 + [vp]
     L.T360B200_transformFrameCameraAsync.restype = ci
     L.T360B200_transformFrameCameraAsync.argtypes = [vp, C.POINTER(T360LensRig), C.POINTER(T360Pose), C.POINTER(T360Camera), ci] + planes
+    L.T360B200_cameraMipMaps.restype = ci
+    L.T360B200_cameraMipMaps.argtypes = [C.POINTER(FrameTransformContext), C.POINTER(T360LensRig), C.POINTER(T360Pose),
+                                         C.POINTER(T360Camera), C.POINTER(T360Minify)] + [ci] * 4 + [vp] * 4
+    L.T360B200_transformFrameCameraMipAsync.restype = ci
+    L.T360B200_transformFrameCameraMipAsync.argtypes = [vp, C.POINTER(T360LensRig), C.POINTER(T360Pose), C.POINTER(T360Camera),
+                                                        C.POINTER(T360Minify), ci] + planes
     L.T360B200_setPinHostPlanes.restype = None
     L.T360B200_setPinHostPlanes.argtypes = [vp, ci]
     L.T360B200_debugTrace.restype = None
@@ -286,6 +316,7 @@ EXPORTED_SYMBOLS = [
     "T360B200_transformFrameOrientedAsync", "T360B200_orientedSamples", "T360B200_transformFramePoseAsync", "T360B200_poseSamples",
     "T360B200_lensMap", "T360B200_transformFrameLensAsync", "T360B200_lensBlendMaps", "T360B200_transformFrameLensBlendAsync",
     "T360B200_rectilinearMap", "T360B200_transformFrameRectilinearAsync", "T360B200_cameraMap", "T360B200_transformFrameCameraAsync",
+    "T360B200_cameraMipMaps", "T360B200_transformFrameCameraMipAsync",
     "T360B200_setPinHostPlanes", "T360B200_debugTrace", "T360B200_debugTraceRead", "T360B200_synchronize", "T360B200_stream", "T360B200_kernelLaunchCount", "T360B200_planDeviceBytes",
     "T360B200_planTileCounts", "T360B200_deviceCount", "T360B200_version",
 ]
@@ -412,6 +443,15 @@ class VideoFrameTransform:
         n, enqueue = self._frame_call("T360B200_transformFrameCameraAsync", in_planes, out_planes, dims)
         return lambda pose, camera, stream=0, rig=None: enqueue(
             (C.byref(rig) if rig is not None else None, C.byref(as_pose(pose)), C.byref(as_camera(camera)), n), stream)
+
+    def make_camera_mip_frame_call(self, in_planes, out_planes, dims):
+        """Like make_camera_frame_call, for T360B200_transformFrameCameraMipAsync (an anti-aliased camera view): returns a
+        callable f(pose, camera, minify, stream, rig=None) -> bool, `minify` a T360Minify, a max level, or (max_level,
+        lod_bias)."""
+        n, enqueue = self._frame_call("T360B200_transformFrameCameraMipAsync", in_planes, out_planes, dims)
+        return lambda pose, camera, minify, stream=0, rig=None: enqueue(
+            (C.byref(rig) if rig is not None else None, C.byref(as_pose(pose)), C.byref(as_camera(camera)),
+             C.byref(as_minify(minify)), n), stream)
 
     def generate_map_from_warp(self, map, in_w: int, in_h: int, plan_index: int, border: int = BORDER_WRAP) -> bool:
         """T360B200_generateMapFromWarp: installs plan index `plan_index` from a caller's warp map (float32 [h][w][2], the
@@ -678,6 +718,23 @@ def camera_map(ctx: FrameTransformContext, pose, camera, in_w, in_h, out_w, out_
                                      C.byref(as_camera(camera)), in_w, in_h, out_w, out_h, out.ctypes.data):
         raise ValueError("T360B200_cameraMap refused the arguments (message on stdout)")
     return out
+
+
+def camera_mip_maps(ctx: FrameTransformContext, pose, camera, minify, in_w, in_h, out_w, out_h,
+                    rig: T360LensRig | None = None) -> tuple[np.ndarray, np.ndarray, np.ndarray, np.ndarray]:
+    """The host twin of one plane of an anti-aliased camera view (T360B200_cameraMipMaps, no CUDA): (map0, map1, level,
+    weight).  map0 / map1: float32 [out_h][out_w][2], each pixel's entry in its level's pixels / in the next level's (NaN
+    where the weight is 0); level: uint8 [out_h][out_w]; weight: uint16, the next level's weight w (0..255).  cv::remap of
+    each level's entries over the pyramid (cv::resize with INTER_AREA, repeated: mip_level_sizes), blended as
+    (a (256 - w) + b w + 128) >> 8, gives the frame call's plane."""
+    shape = (max(out_h, 0), max(out_w, 0))
+    map0, map1 = np.zeros(shape + (2,), np.float32), np.zeros(shape + (2,), np.float32)
+    level, weight = np.zeros(shape, np.uint8), np.zeros(shape, np.uint16)
+    if not load().T360B200_cameraMipMaps(C.byref(ctx), C.byref(rig) if rig is not None else None, C.byref(as_pose(pose)),
+                                         C.byref(as_camera(camera)), C.byref(as_minify(minify)), in_w, in_h, out_w, out_h,
+                                         map0.ctypes.data, map1.ctypes.data, level.ctypes.data, weight.ctypes.data):
+        raise ValueError("T360B200_cameraMipMaps refused the arguments (message on stdout)")
+    return map0, map1, level, weight
 
 
 def square_pixel_vfov(hfov, width, height) -> float:
