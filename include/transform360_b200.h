@@ -334,6 +334,74 @@ int T360B200_transformFrameLensBlendAsync(VideoFrameTransform* transform, const 
                                           uint8_t* const* deviceOutputs, const int* inputWidths, const int* inputHeights,
                                           const int* inputPitches, const int* outputWidths, const int* outputHeights,
                                           const int* outputPitches, void* cudaStream);
+/* ---- lens photometry ---------------------------------------------------------------------------------
+ * The lens calls above move pixels only: each lens loses light towards its rim, where the seam lies, and the two sensors
+ * of a dual-fisheye camera run their own exposure and white balance, so a seam (hard or feathered) shows a brightness
+ * step.  These calls correct each lens's sample before the seam combines them, and measure the mismatch that is left.
+ * The model is in code values, as the frame holds them: no transfer function is applied.  V is the falloff measured in code
+ * values (for example fitted to a flat-field frame); scaling every plane about its pivot by one factor models a scale of
+ * R'G'B', and the per-plane gains and offsets model the exposure and a colour cast between the lenses.
+ *
+ * For each lens sample s the frame uses (plane p, lens i), every float step rounded to nearest, + - * / only, in this
+ * order on the host and on the device:
+ *   r = theta_d = theta (1 + k1 theta^2 + ...) of the lens calls (so the image radius of the pixel is f r: a falloff
+ *     measured against the pixel radius R at the calibration size is a polynomial in R / f);
+ *   t = r r, V = 1 + t (v1 + t (v2 + t v3)), G = gain_p / V;
+ *   Gq = G 4096 rounded half to even, at most 65535 (G >= 16);
+ *   Oq = round(16 offset_p), computed on the host, half away from zero;
+ *   P = lumaPivot for plane 0, 128 for planes 1 and 2;
+ *   s' = clamp(P + ((((s - P) Gq) + Oq 256 + 2048) >> 12), 0, 255), >> an arithmetic shift.
+ * vignetting = 0, gain = 1 and offset = 0 give Gq = 4096 and s' = s: the frames of the lens calls above, bit for bit.
+ *
+ * Seams: seamWidth == 0 is the hard seam of T360B200_transformFrameLensAsync (1 or 2 lenses, the closer lens carries the
+ * pixel); seamWidth in [0.01, 180] the feathered seam of T360B200_transformFrameLensBlendAsync (2 lenses, its w).  Each
+ * lens's sample is corrected before the combination: the feathered seam gives (a' (256 - w) + b' w + 128) >> 8.  Samples
+ * that BORDER_TRANSPARENT skips stay skipped, and the pre-fill is the lens calls' (chroma 128, luma the caller's bytes).
+ *
+ * Statistics: deviceStats (device memory, NULL: none) receives [numPlanes][6] sums per frame, n, sum a', sum b', sum a'^2,
+ * sum b'^2, sum a' b', over the output pixels where both lenses cover the pixel's direction and neither sample is skipped;
+ * a' and b' are lens 0's and lens 1's corrected samples.  With the hard seam too: there the overlap's pixels gather the
+ * other lens for the statistics only, and the frame is the same as without them.  The call zeroes the buffer in stream
+ * order before the gather; the sums are integers, exact whatever the order of accumulation.  A one-lens rig gives zeros.
+ * Every output pixel weighs the same, whatever solid angle it covers: an equirect output, for example, over-weights the
+ * poles.
+ *
+ * Refused, with 0 and a message on stdout before any CUDA call: every refusal of T360B200_transformFrameLensAsync, and with
+ * seamWidth > 0 every refusal of T360B200_transformFrameLensBlendAsync; a seamWidth that is negative, not finite or in
+ * (0, 0.01); a NULL photometry; lumaPivot outside 0..255; a field of a lens that is read (lens[1] with two lenses) that
+ * is not finite, a gain outside (0, 8] or an offset outside [-64, 64]; a falloff with V(r) <= 0 somewhere on [0,
+ * theta_d(maxAngle)] (checked in double on a 4096-step grid). */
+typedef struct T360LensPhotometry {
+  float vignetting[3]; /* v1..v3 of the falloff V(r) = 1 + v1 r^2 + v2 r^4 + v3 r^6, r = theta_d (radians) */
+  float gain[3];       /* per plane: 0 = luma, 1 and 2 = chroma; finite, in (0, 8] */
+  float offset[3];     /* per plane, in code values; finite, in [-64, 64] */
+} T360LensPhotometry;
+typedef struct T360RigPhotometry {
+  int lumaPivot;              /* 0..255: the level luma scales about (16 limited range, 0 full range); chroma scales about 128 */
+  T360LensPhotometry lens[2]; /* lens[1] is read only with numLenses == 2 */
+} T360RigPhotometry;
+/* Host only, no CUDA: the host twin of T360B200_transformFrameLensPhotoAsync for plane `plane` (0..2) of inputWidth x
+ * inputHeight.  map0, map1: CV_32FC2 maps (float32 [outputHeight][outputWidth][2]) of lens 0 and lens 1, the lens's entry
+ * wherever it covers the pixel's direction, NaN elsewhere; weight: w (uint16 [outputHeight][outputWidth]), 0 or 256 from
+ * the lens choice of the hard seam, the blend weight of the feathered one; gain0, gain1: each lens's Gq for the plane
+ * (uint16), 0 where it does not cover the pixel.  The frame's plane is cv::remap of each map with BORDER_TRANSPARENT, then
+ * s', then: w = 0 lens 0's alone, w = 256 lens 1's alone, else the combination above (the other alone where one is
+ * skipped); the statistics are the sums over the pixels where both maps are finite and neither sample is skipped.
+ * Returns 1; 0 (message) for the refusals above, a plane outside 0..2, a NULL array or non-positive sizes. */
+int T360B200_lensPhotoMaps(const FrameTransformContext* ctx, const T360LensRig* rig, const T360RigPhotometry* photometry, float seamWidth,
+                           const T360Orientation* orientation, int plane, int inputWidth, int inputHeight, int outputWidth,
+                           int outputHeight, float* map0, float* map1, uint16_t* weight, uint16_t* gain0, uint16_t* gain1);
+/* One frame of a lens rig with photometry, every plane in one gather launch: the arguments and the asynchronous contract
+ * of T360B200_transformFrameLensAsync, plus photometry, seamWidth and deviceStats, which may change every frame like the
+ * rig and the orientation.  Needs no plan and does not touch the plans; takes the reader lock; never synchronises the
+ * device.  Zeroing deviceStats is a memset.  There is no planned path: a plan carries one record per pixel.  Returns 1 if
+ * everything was enqueued; 0 with a message on stdout, before any CUDA call, for the refusals above, 0 or more than 3
+ * planes, or an invalid plane description. */
+int T360B200_transformFrameLensPhotoAsync(VideoFrameTransform* transform, const T360LensRig* rig, const T360RigPhotometry* photometry,
+                                          float seamWidth, const T360Orientation* orientation, unsigned long long* deviceStats,
+                                          int numPlanes, const uint8_t* const* deviceInputs, uint8_t* const* deviceOutputs,
+                                          const int* inputWidths, const int* inputHeights, const int* inputPitches,
+                                          const int* outputWidths, const int* outputHeights, const int* outputPitches, void* cudaStream);
 /* ---- rectilinear views -------------------------------------------------------------------------------
  * A perspective (pinhole) virtual camera looking into 360-degree or fisheye footage: reframing with pan, tilt, roll and
  * zoom, or undistortion of a fisheye lens.  The camera is a T360Pose (degrees).  For output pixel (i, j) of a plane of

@@ -395,7 +395,10 @@ void countKernelLaunches(long long n);  // kernels launched through a replayed C
 //   kCameraMip    anti-aliased camera views (camera, mip, mipBias; mipCameraSample): kRectilinear's chain plus the pixel's
 //                 footprint, which picks a level of the plane's pyramid and the weight w (0..255) of the next one; the
 //                 pixel gathers its level, and the next level only where w > 0, blended as kLensBlend blends.
-enum class PerFrameSource { kView, kSphere, kMap, kLens, kLensBlend, kRectilinear, kCameraMip };
+//   kLensPhoto    a lens rig with photometry (rotation, rig, seamScale, photo; lensPhotoSample): the hard seam
+//                 (seamScale = 0) or the feathered one; each lens's sample is corrected with its gain (photoCorrect)
+//                 before the seam combines them, and with photo.stats set the overlap's sums are accumulated.
+enum class PerFrameSource { kView, kSphere, kMap, kLens, kLensBlend, kRectilinear, kCameraMip, kLensPhoto };
 struct PerFramePlane {
   const uint8_t* src;  // (blurred) input plane, geometry.inW x geometry.inH
   uint8_t* dst;        // render target, geometry.mapW x geometry.mapH
@@ -429,9 +432,23 @@ struct PerFrameGatherParams {
   struct MipPlane {
     MipGeometry geometry;
     MipLevel level[kMipMaxLevels];  // [l - 1]: level l
-  } mip[kMaxFramePlanes];
+  };
+  // kLensPhoto: per plane its photometric constants, and the statistics buffer ([numPlanes][6] sums: n, sum a', sum b',
+  // sum a'^2, sum b'^2, sum a'b', zeroed by the caller in stream order; nullptr: none)
+  struct LensPhoto {
+    LensPhotoPlane plane[kMaxFramePlanes];
+    unsigned long long* stats;
+  };
+  // (the two sources' constants share their storage, so the block keeps the size and layout every other source's
+  // kernel was compiled against)
+  union {
+    MipPlane mip[kMaxFramePlanes];
+    LensPhoto photo;
+  };
   int mipBias;
 };
+static_assert(sizeof(PerFrameGatherParams::LensPhoto) <= sizeof(PerFrameGatherParams::MipPlane) * kMaxFramePlanes);
+constexpr int kPhotoStats = 6;  // sums per plane of kLensPhoto's statistics
 // a CTA takes tiles of 32 output columns x viewTileRows(k) rows; a thread owns one column of a tile and walks down
 // kViewRowsPerThread of its rows
 constexpr int kViewRowsPerThread = 8;

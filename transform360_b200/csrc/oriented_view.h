@@ -22,6 +22,7 @@
 
 #include <cmath>
 #include <cstdint>
+#include <type_traits>
 #include <vector>
 
 #include "Transform360/VideoFrameTransformHelper.h"
@@ -420,24 +421,32 @@ T360_HD float lensRow(const float* m, const SphereVec& d) { return fAdd(fAdd(fMu
 // What one lens makes of rig direction d: theta, whether it covers d (theta <= thetaMax), and where it does, the source
 // position (px, py) in an inW x inH plane (NaN for both where it does not).  Z = lensRow(L.m + 6, d), which the callers
 // have already computed.  The one place the lens projection is written: the hard seam (lensPosition) and the feathered
-// seam (lensBlendPosition) both call it.
+// seam (lensBlendPosition) both call it.  R = true also keeps r = theta_d, the distorted angle (so the image radius is
+// f theta_d), for the photometric falloff (lensGain), in a LensHitR; the callers that do not need it compile exactly as
+// they did before it was kept.
 struct LensHit {
   float theta, px, py;
   bool covered;
 };
-T360_HD LensHit lensHit(const LensModel& L, const SphereVec& d, float Z, int inW, int inH) {
+struct LensHitR : LensHit {
+  float r;  // theta_d where covered
+};
+template <bool R = false>
+T360_HD std::conditional_t<R, LensHitR, LensHit> lensHit(const LensModel& L, const SphereVec& d, float Z, int inW, int inH) {
   const float X = lensRow(L.m, d), Y = lensRow(L.m + 3, d);
   const float rho = fSqrt(fAdd(fMul(X, X), fMul(Y, Y)));
-  LensHit h;
+  std::conditional_t<R, LensHitR, LensHit> h;
   h.theta = libmAtan2f(rho, Z);
   h.covered = h.theta <= L.thetaMax;
   if (!h.covered) {
     h.px = h.py = bitsFloat(0x7fc00000u);
+    if constexpr (R) h.r = h.px;
     return h;
   }
   const float t = fMul(h.theta, h.theta);
   const float poly = fAdd(1.0f, fMul(t, fAdd(L.k[0], fMul(t, fAdd(L.k[1], fMul(t, fAdd(L.k[2], fMul(t, L.k[3]))))))));
   const float s = rho > 0.0f ? fDiv(fMul(h.theta, poly), rho) : 0.0f;
+  if constexpr (R) h.r = fMul(h.theta, poly);
   h.px = toPixel(fAdd(fMul(L.ax, fMul(s, X)), L.bx), inW);
   h.py = toPixel(fAdd(fMul(L.ay, fMul(s, Y)), L.by), inH);
   return h;
@@ -522,6 +531,114 @@ T360_HD int lensBlendSample(const SphereGeometry& g, const Rotation& r, const Le
                             const float* rowTab, int i, int j, int32_t* rec0, int32_t* rec1) {
   float p[2][2];
   const int w = lensBlendPoint<BARREL>(g, r, rig, s, colTab, rowTab, i, j, p[0], p[1]);
+  int32_t* rec[2] = {rec0, rec1};
+  for (int l = 0; l < 2; ++l) {
+    int r0, fracX, fracY;
+    quantizeAxis(p[l][0], g.kernelSize, &rec[l][0], &fracX);
+    quantizeAxis(p[l][1], g.kernelSize, &r0, &fracY);
+    rec[l][1] = r0 * 1024 + fracY * 32 + fracX;
+  }
+  return w;
+}
+
+// ---- photometric correction of a lens rig (T360B200_transformFrameLensPhotoAsync, T360B200_lensPhotoMaps) -------------
+// Each lens's sample s of plane p is corrected before the seam combines the two:
+//   V = 1 + t (v1 + t (v2 + t v3)), t = r^2, r = theta_d (lensHit<true>)  the lens's radial falloff
+//   Gq = min(round_half_even(gain_p / V * 4096), 65535)                     (lensGain)
+//   s' = clamp(P + (((s - P) Gq + Oq 256 + 2048) >> 12), 0, 255)          (photoCorrect; Oq = round(16 offset_p))
+// with the pivot P = lumaPivot for luma, 128 for chroma.  The constants of one plane, per lens, are computed on the host
+// (lensPhotoPlane, video_frame_transform.cpp).
+struct LensPhotoPlane {
+  float v[2][3];  // v1..v3 of each lens
+  float gain[2];  // gain_p of each lens
+  int offset[2];  // Oq of each lens: the offset in 1/16 code value
+  int pivot;
+};
+
+// Gq of lens hit h: the one place the falloff is written (the kernel and the host twin both call it).  0 where the lens
+// does not cover the direction; 0 also for a V that is not positive or a NaN (the host refuses falloffs that reach 0).
+T360_HD int lensGain(const LensHitR& h, const float* v, float gain) {
+  if (!h.covered) return 0;
+  const float t = fMul(h.r, h.r);
+  const float V = fAdd(1.0f, fMul(t, fAdd(v[0], fMul(t, fAdd(v[1], fMul(t, v[2]))))));
+  const float q = fMul(fDiv(gain, V), 4096.0f);
+  return q >= 65535.0f ? 65535 : (q > 0.0f ? roundHalfEven(q) : 0);
+}
+
+// s' of sample s (0..255), gain Gq, offset Oq and pivot P, in integers
+T360_HD int photoCorrect(int s, int gq, int oq, int pivot) {
+  const int c = pivot + (((s - pivot) * gq + oq * 256 + 2048) >> 12);
+  return c < 0 ? 0 : (c > 255 ? 255 : c);
+}
+
+// Both lenses' view of rig direction d for the photometric calls, and the weight w (0..256) of lens 1.  s = 0: the hard
+// seam, w = 256 where lens 1 is the closer lens (lensPosition's choice), else 0; s > 0: the feathered seam's w
+// (lensBlendPosition).  p0 / p1: lens 0's / lens 1's source position wherever that lens covers d (NaN elsewhere), g0 / g1
+// its Gq (lensGain; 0 where it does not cover d); *overlap: both lenses cover d.  both = false with the hard seam computes
+// the closer lens only (the other's position NaN, its gain 0, no overlap): all the frame needs when no statistics are taken.
+T360_HD int lensPhotoPosition(const LensRigModel& rig, float s, bool both, const LensPhotoPlane& c, const SphereVec& d, int inW, int inH,
+                              float* p0, float* p1, int* g0, int* g1, bool* overlap) {
+  const float nan = bitsFloat(0x7fc00000u);
+  const float z0 = lensRow(rig.lens[0].m + 6, d);
+  const float z1 = rig.numLenses > 1 ? lensRow(rig.lens[1].m + 6, d) : z0;
+  const bool second = z1 > z0;
+  if (s == 0.0f && !both) {  // the closer lens alone, as lensPosition projects it
+    const int l = second ? 1 : 0;
+    const LensHitR h = lensHit<true>(rig.lens[l], d, second ? z1 : z0, inW, inH);
+    float* p = second ? p1 : p0;
+    float* q = second ? p0 : p1;
+    p[0] = h.px; p[1] = h.py;
+    q[0] = q[1] = nan;
+    *(second ? g1 : g0) = lensGain(h, c.v[l], c.gain[l]);
+    *(second ? g0 : g1) = 0;
+    *overlap = false;
+    return second ? 256 : 0;
+  }
+  LensHitR h0 = lensHit<true>(rig.lens[0], d, z0, inW, inH), h1;
+  h1.covered = false;
+  h1.px = h1.py = h1.r = nan;
+  if (rig.numLenses > 1) h1 = lensHit<true>(rig.lens[1], d, z1, inW, inH);
+  int w = second ? 256 : 0;
+  if (s > 0.0f) {
+    w = h1.covered ? 256 : 0;
+    if (h0.covered && h1.covered) {
+      const float tw = fMul(fAdd(0.5f, fMul(fSub(h0.theta, h1.theta), s)), 256.0f);
+      w = tw <= 0.0f ? 0 : (tw >= 256.0f ? 256 : roundHalfEven(tw));
+    }
+  }
+  p0[0] = h0.px; p0[1] = h0.py;
+  p1[0] = h1.px; p1[1] = h1.py;
+  *g0 = lensGain(h0, c.v[0], c.gain[0]);
+  *g1 = lensGain(h1, c.v[1], c.gain[1]);
+  *overlap = h0.covered && h1.covered;
+  return w;
+}
+
+// The two map entries, the weight and the two gains of output pixel (i, j) of a lens rig with photometry: spherePoint,
+// then lensPhotoPosition; both entries NaN, w = 0, both gains 0 and no overlap in a barrel dead zone.
+// (T360B200_lensPhotoMaps)
+template <bool BARREL = true>
+T360_HD int lensPhotoPoint(const SphereGeometry& g, const Rotation& r, const LensRigModel& rig, float s, bool both, const LensPhotoPlane& c,
+                           const float* colTab, const float* rowTab, int i, int j, float* p0, float* p1, int* g0, int* g1, bool* overlap) {
+  bool eye;
+  SphereVec d;
+  if (!spherePoint<BARREL>(g, r, colTab, rowTab, i, j, &eye, &d)) {
+    p0[0] = p0[1] = p1[0] = p1[1] = bitsFloat(0x7fc00000u);
+    *g0 = *g1 = 0;
+    *overlap = false;
+    return 0;
+  }
+  return lensPhotoPosition(rig, s, both, c, d, g.inW, g.inH, p0, p1, g0, g1, overlap);
+}
+
+// The sampling records of output pixel (i, j) of a lens rig with photometry, lens 0's in rec0 and lens 1's in rec1
+// (quantised as lensSample quantises its entry), the gains, the overlap and the weight w of lens 1 (the return value).
+template <bool BARREL = true>
+T360_HD int lensPhotoSample(const SphereGeometry& g, const Rotation& r, const LensRigModel& rig, float s, bool both, const LensPhotoPlane& c,
+                            const float* colTab, const float* rowTab, int i, int j, int32_t* rec0, int32_t* rec1, int* g0, int* g1,
+                            bool* overlap) {
+  float p[2][2];
+  const int w = lensPhotoPoint<BARREL>(g, r, rig, s, both, c, colTab, rowTab, i, j, p[0], p[1], g0, g1, overlap);
   int32_t* rec[2] = {rec0, rec1};
   for (int l = 0; l < 2; ++l) {
     int r0, fracX, fracY;

@@ -600,6 +600,74 @@ t360::LensRigModel lensRigModel(const T360LensRig& rig) {
   return m;
 }
 
+// true, with the reason in *why, when the photometric lens call cannot serve ctx with this rig, photometry, seam and
+// orientation: the lens call's refusals (seamWidth = 0, the hard seam) or the blend call's (seamWidth > 0), and a
+// photometry that is NULL, out of range, or whose falloff reaches 0 inside a lens's coverage
+bool lensPhotoRefused(const FrameTransformContext& ctx, const T360LensRig* rig, const T360RigPhotometry* ph, float seamWidth,
+                      const T360Orientation* o, std::string* why) {
+  if (!std::isfinite(seamWidth) || seamWidth < 0.0f || (seamWidth > 0.0f && seamWidth < 0.01f)) {
+    *why = formatted("seamWidth %g degrees is neither 0 (the hard seam) nor in [0.01, 180]", seamWidth);
+    return true;
+  }
+  if (seamWidth > 0.0f ? lensBlendRefused(ctx, rig, seamWidth, o, why) : lensRefused(ctx, rig, o, why)) return true;
+  if (!ph) {
+    *why = "a NULL photometry";
+    return true;
+  }
+  if (ph->lumaPivot < 0 || ph->lumaPivot > 255) {
+    *why = formatted("lumaPivot %d is outside 0..255", ph->lumaPivot);
+    return true;
+  }
+  for (int i = 0; i < rig->numLenses; ++i) {
+    const T360LensPhotometry& L = ph->lens[i];
+    for (int k = 0; k < 3; ++k)
+      if (!std::isfinite(L.vignetting[k]) || !std::isfinite(L.gain[k]) || !std::isfinite(L.offset[k])) {
+        *why = formatted("the photometry of lens %d has a field that is not finite", i);
+        return true;
+      }
+    for (int k = 0; k < 3; ++k) {
+      if (!(L.gain[k] > 0.0f && L.gain[k] <= 8.0f)) {
+        *why = formatted("lens %d: gain[%d] %g is outside (0, 8]", i, k, L.gain[k]);
+        return true;
+      }
+      if (!(L.offset[k] >= -64.0f && L.offset[k] <= 64.0f)) {
+        *why = formatted("lens %d: offset[%d] %g is outside [-64, 64]", i, k, L.offset[k]);
+        return true;
+      }
+    }
+    // V(r) = 1 + v1 r^2 + v2 r^4 + v3 r^6 must stay positive for every r = theta_d the lens reaches: [0, theta_d(maxAngle)]
+    // (theta_d increases on [0, maxAngle]: rigRefused), on a fine grid
+    const T360Lens& lens = rig->lens[i];
+    const double tMax = lens.maxAngle * M_PI / 180.0, t2 = tMax * tMax;
+    const double rMax = tMax * (1.0 + t2 * (lens.k[0] + t2 * (lens.k[1] + t2 * (lens.k[2] + t2 * lens.k[3]))));
+    constexpr int kSteps = 4096;
+    for (int s = 0; s <= kSteps; ++s) {
+      const double r = rMax * s / kSteps, q = r * r;
+      const double v = 1.0 + q * (L.vignetting[0] + q * (L.vignetting[1] + q * L.vignetting[2]));
+      if (!(v > 0.0)) {
+        *why = formatted("lens %d: the falloff V(r) of vignetting (%g, %g, %g) reaches %g at r = %.4f, inside the lens's theta_d(maxAngle) %.4f",
+                         i, L.vignetting[0], L.vignetting[1], L.vignetting[2], v, r, rMax);
+        return true;
+      }
+    }
+  }
+  return false;
+}
+
+// The per-frame constants of plane `plane` (0 luma, 1 and 2 chroma) of a rig's photometry (oriented_view.h: LensPhotoPlane);
+// lens 1's stay zero for a one-lens rig
+t360::LensPhotoPlane lensPhotoPlane(const T360RigPhotometry& ph, int numLenses, int plane) {
+  t360::LensPhotoPlane c{};
+  c.pivot = plane == 0 ? ph.lumaPivot : 128;
+  for (int i = 0; i < numLenses; ++i) {
+    const T360LensPhotometry& L = ph.lens[i];
+    for (int k = 0; k < 3; ++k) c.v[i][k] = L.vignetting[k];
+    c.gain[i] = L.gain[plane];
+    c.offset[i] = static_cast<int>(std::lround(16.0 * static_cast<double>(L.offset[plane])));  // (half away from zero)
+  }
+  return c;
+}
+
 // The context the lens path renders with: the output fields of ctx, a mono equirect-like input (the fields the rig
 // replaces, which play no part in the output half of the chain), no scaling
 FrameTransformContext lensContext(const FrameTransformContext& ctx) {
@@ -1299,9 +1367,13 @@ class VideoFrameTransform {
   // before the first CUDA call, and nothing here synchronises the device.
   // seamWidth: nullptr for the hard seam; else the belt in degrees across which two lenses are blended
   // (T360B200_transformFrameLensBlendAsync: lensBlendSample), the same steps with the blend source.
+  // photo: a photometry (T360B200_transformFrameLensPhotoAsync: lensPhotoSample), with *seamWidth 0 for the hard seam; each
+  // lens's sample is corrected before the seam, and with stats set (device, [numPlanes][6]) the overlap's sums are zeroed
+  // with a memset and accumulated by the same gather.
   bool transformFrameLens(const char* what, const T360LensRig* rig, const float* seamWidth, const T360Orientation* o, const FramePlanes& f,
-                          cudaStream_t stream) {
+                          cudaStream_t stream, const T360RigPhotometry* photo = nullptr, unsigned long long* stats = nullptr) {
     auto refused = [&](const FrameTransformContext& ctx, std::string* why) {
+      if (photo) return lensPhotoRefused(ctx, rig, photo, *seamWidth, o, why);
       return seamWidth ? lensBlendRefused(ctx, rig, *seamWidth, o, why) : lensRefused(ctx, rig, o, why);
     };
     return unplannedFrame(what, stream, refused, [&](const FrameTransformContext& ctx, int k, cudaStream_t s) {
@@ -1313,9 +1385,16 @@ class VideoFrameTransform {
       for (int p = 0; p < f.numPlanes; ++p) gp.plane[p].geometry = t360::sphereGeometry(lens, f.outW[p], f.outH[p], f.inW[p], f.inH[p], k);
       gp.rotation = t360::rotationFromAngles(o->yaw, o->pitch, o->roll);
       gp.rig = lensRigModel(*rig);
-      if (seamWidth) gp.seamScale = lensSeamScale(*seamWidth);
-      perFrameGather(seamWidth ? t360::PerFrameSource::kLensBlend : t360::PerFrameSource::kLens, gp, ctx, f, f.in, f.inPitch, nullptr,
-                     /*transparent=*/true, tables, staged, nullptr, s);
+      const bool feathered = seamWidth && *seamWidth > 0.0f;
+      if (feathered) gp.seamScale = lensSeamScale(*seamWidth);
+      t360::PerFrameSource source = feathered ? t360::PerFrameSource::kLensBlend : t360::PerFrameSource::kLens;
+      if (photo) {
+        source = t360::PerFrameSource::kLensPhoto;
+        for (int p = 0; p < f.numPlanes; ++p) gp.photo.plane[p] = lensPhotoPlane(*photo, rig->numLenses, p);
+        gp.photo.stats = stats;
+        if (stats) CU(cudaMemsetAsync(stats, 0, sizeof(unsigned long long) * t360::kPhotoStats * f.numPlanes, s));
+      }
+      perFrameGather(source, gp, ctx, f, f.in, f.inPitch, nullptr, /*transparent=*/true, tables, staged, nullptr, s);
       return true;
     });
   }
@@ -2887,6 +2966,51 @@ T360_API int T360B200_transformFrameLensBlendAsync(VideoFrameTransform* t, const
   FramePlanes f;
   if (!describeFrame(what, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, f)) return 0;
   return t->transformFrameLens(what, rig, &seamWidth, orientation, f, static_cast<cudaStream_t>(stream));
+}
+T360_API int T360B200_lensPhotoMaps(const FrameTransformContext* ctx, const T360LensRig* rig, const T360RigPhotometry* photometry, float seamWidth,
+                                    const T360Orientation* orientation, int plane, int inW, int inH, int outW, int outH, float* map0, float* map1,
+                                    uint16_t* weight, uint16_t* gain0, uint16_t* gain1) {
+  const char* what = "Could not compute the lens photometry maps";
+  std::string why;
+  if (!ctx) why = "a NULL context";
+  else if (lensPhotoRefused(*ctx, rig, photometry, seamWidth, orientation, &why)) {}
+  else if (plane < 0 || plane > 2) why = formatted("plane %d is outside 0..2", plane);
+  else if (!map0 || !map1 || !weight || !gain0 || !gain1 || inW <= 0 || inH <= 0 || outW <= 0 || outH <= 0)
+    why = "a NULL map, weight or gain array or a plane size that is not positive";
+  if (!why.empty()) {
+    std::printf("%s. Error: %s\n", what, why.c_str());
+    return 0;
+  }
+  const t360::LensRigModel model = lensRigModel(*rig);
+  const t360::LensPhotoPlane c = lensPhotoPlane(*photometry, rig->numLenses, plane);
+  const float s = seamWidth > 0.0f ? lensSeamScale(seamWidth) : 0.0f;
+  forLensPixels(*ctx, *orientation, inW, inH, outW, outH, [&](const t360::SphereGeometry& g, const t360::Rotation& r, const float* colTab,
+                                                              const float* rowTab, int i, int j, size_t at) {
+    int g0, g1;
+    bool overlap;
+    weight[at] = static_cast<uint16_t>(
+        t360::lensPhotoPoint(g, r, model, s, /*both=*/true, c, colTab, rowTab, i, j, map0 + 2 * at, map1 + 2 * at, &g0, &g1, &overlap));
+    gain0[at] = static_cast<uint16_t>(g0);
+    gain1[at] = static_cast<uint16_t>(g1);
+  });
+  return 1;
+}
+T360_API int T360B200_transformFrameLensPhotoAsync(VideoFrameTransform* t, const T360LensRig* rig, const T360RigPhotometry* photometry,
+                                                   float seamWidth, const T360Orientation* orientation, unsigned long long* deviceStats,
+                                                   int numPlanes, const uint8_t* const* dIn, uint8_t* const* dOut, const int* inW, const int* inH,
+                                                   const int* inPitch, const int* outW, const int* outH, const int* outPitch, void* stream) {
+  const char* what = "Could not transform the frame of a lens rig with photometry";
+  if (!t) {
+    std::printf("%s. Error: a NULL argument\n", what);
+    return 0;
+  }
+  if (!photometry) {  // (checked here: without a photometry transformFrameLens is the plain lens call)
+    std::printf("%s. Error: a NULL photometry\n", what);
+    return 0;
+  }
+  FramePlanes f;
+  if (!describeFrame(what, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, f)) return 0;
+  return t->transformFrameLens(what, rig, &seamWidth, orientation, f, static_cast<cudaStream_t>(stream), photometry, deviceStats);
 }
 namespace {
 int cameraMap(const char* what, const FrameTransformContext* ctx, const T360LensRig* rig, const T360Pose* pose, const T360Camera* camera,

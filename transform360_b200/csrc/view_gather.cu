@@ -20,8 +20,10 @@
 //   - a camera view (RectilinearPositions): the camera model's ray per pixel (a pinhole launch in a loop of its own),
 //     rotated, then the context's input lookup or the lens model (oriented_view.h: rectilinearSample);
 //   - an anti-aliased camera view (MipCameraPositions): the same chain, the pixel's footprint from ray differentials, and
-//     two records at adjacent levels of the plane's input pyramid, blended by the footprint's weight (mipCameraSample).
-// In all seven, the records come from the same host/device functions the planner (or its host twin) uses: bit-identical.
+//     two records at adjacent levels of the plane's input pyramid, blended by the footprint's weight (mipCameraSample);
+//   - a lens rig with photometry (LensPhotoPositions): both lenses' records and gains (lensPhotoSample); the tile loop
+//     corrects each sample, combines them by the seam and accumulates the overlap's statistics.
+// In all eight, the records come from the same host/device functions the planner (or its host twin) uses: bit-identical.
 #include "gather_common.cuh"
 
 #include <algorithm>
@@ -59,6 +61,10 @@ template <class Pos, class = void>
 struct IsMip : std::false_type {};
 template <class Pos>
 struct IsMip<Pos, std::enable_if_t<Pos::kMip>> : std::true_type {};
+template <class Pos, class = void>
+struct IsPhoto : std::false_type {};
+template <class Pos>
+struct IsPhoto<Pos, std::enable_if_t<Pos::kPhoto>> : std::true_type {};
 
 // TRANSPARENT (barrel layouts): BORDER_TRANSPARENT, a pixel whose anchor tap lies outside the source keeps its byte.
 // Positions::kMip (IsMip): record() returns the pixel's pyramid level and hands over its record there, the record at the
@@ -67,6 +73,11 @@ struct IsMip<Pos, std::enable_if_t<Pos::kMip>> : std::true_type {};
 // Positions::kBlend: its record() hands over two records and the weight w (0..256) of the second; the first is gathered
 // for every pixel, the second only where 0 < w < 256, and the two values are blended (PerFrameSource::kLensBlend).  Where
 // BORDER_TRANSPARENT skips one of the two, the other stands alone.
+// Positions::kPhoto (IsPhoto, kLensPhoto): record() hands over both lenses' records, their gains and w.  Lens 0 is
+// gathered where w < 256, lens 1 where w > 0, and, with statistics, both wherever both cover the pixel; each sample is
+// corrected (photoCorrect) before w combines them.  A thread sums its overlap pixels' six values over its rows of the tile,
+// its warp reduces them (__reduce_add_sync over the warp's live columns), and one lane adds them to the plane's sums with
+// one 64-bit atomic each.  Whether statistics are taken and which seam is used are launch-uniform branches.
 template <int K, bool TRANSPARENT, class Positions>
 __device__ __forceinline__ void gatherViewTiles(const PerFrameGatherParams& p, int numTiles, unsigned char* smem, Positions& pos) {
   constexpr int kRows = viewTileRows(K);
@@ -87,13 +98,36 @@ __device__ __forceinline__ void gatherViewTiles(const PerFrameGatherParams& p, i
     s.w = v.geometry.inW; s.h = v.geometry.inH; s.pitch = v.srcPitch;
     pos.beginColumn(lane);
     const int r0 = warp * kViewRowsPerThread;
+    [[maybe_unused]] uint32_t sums[kPhotoStats] = {};  // (kPhoto: this thread's overlap sums over its rows of the tile)
 #pragma unroll 1
     for (int r = r0; r < r0 + kViewRowsPerThread; ++r) {
       const int i = y0 + r;
       if (i >= v.geometry.mapH) break;
       int col0, rowPhase;
       int value;
-      if constexpr (IsMip<Positions>::value) {
+      if constexpr (IsPhoto<Positions>::value) {
+        int32_t rec0[2], rec1[2];
+        int g0, g1;
+        bool overlap;
+        const int w = pos.record(p, v, pl, i, j, rec0, rec1, &g0, &g1, &overlap);
+        const LensPhotoPlane& c = p.photo.plane[pl];
+        const bool stats = p.photo.stats && overlap;
+        int a = -1, b = -1;
+        if (w < 256 || stats) {
+          a = viewPixel<K, TRANSPARENT>(s, smem, rec0[0], rec0[1]);
+          if (a >= 0) a = photoCorrect(a, g0, c.offset[0], c.pivot);
+        }
+        if (w > 0 || stats) {
+          b = viewPixel<K, TRANSPARENT>(s, smem, rec1[0], rec1[1]);
+          if (b >= 0) b = photoCorrect(b, g1, c.offset[1], c.pivot);
+        }
+        if (stats && a >= 0 && b >= 0) {
+          sums[0] += 1; sums[1] += a; sums[2] += b;
+          sums[3] += a * a; sums[4] += b * b; sums[5] += a * b;
+        }
+        value = w == 0 ? a : (w == 256 ? b : (a < 0 ? b : (b < 0 ? a : (a * (256 - w) + b * w + 128) >> 8)));
+        if (value < 0) continue;
+      } else if constexpr (IsMip<Positions>::value) {
         int32_t rec0[2], rec1[2];
         int w;
         const int level = pos.record(p, v, pl, i, j, rec0, rec1, &w);
@@ -124,6 +158,20 @@ __device__ __forceinline__ void gatherViewTiles(const PerFrameGatherParams& p, i
         }
       }
       v.dst[(size_t)i * v.dstPitch + j] = (uint8_t)value;
+    }
+    if constexpr (IsPhoto<Positions>::value) {
+      if (p.photo.stats) {  // (every lane of the warp's live columns gets here: a row bound breaks the whole warp)
+        const int live = v.geometry.mapW - x0;
+        const unsigned mask = live >= 32 ? 0xffffffffu : (1u << live) - 1u;
+        if (__reduce_add_sync(mask, sums[0])) {
+          unsigned long long* out = p.photo.stats + pl * kPhotoStats;
+#pragma unroll
+          for (int k = 0; k < kPhotoStats; ++k) {
+            const unsigned total = __reduce_add_sync(mask, sums[k]);
+            if (lane == 0) atomicAdd(out + k, (unsigned long long)total);
+          }
+        }
+      }
     }
   }
 }
@@ -265,6 +313,19 @@ struct MipCameraPositions : NoTables {
   }
 };
 
+// A lens rig with photometry (kLensPhoto): both lenses' records, their gains, the overlap and w per pixel
+// (lensPhotoSample); BARREL as for LensPositions.  With the hard seam and no statistics only the closer lens is projected.
+template <int, bool BARREL>
+struct LensPhotoPositions : NoTables {
+  static constexpr bool kPhoto = true, kTransparent = true;
+  using NoTables::NoTables;
+  __device__ int record(const PerFrameGatherParams& p, const PerFramePlane& v, int pl, int i, int j, int32_t* rec0, int32_t* rec1, int* g0,
+                        int* g1, bool* overlap) const {
+    return lensPhotoSample<BARREL>(v.geometry, p.rotation, p.rig, p.seamScale, p.photo.stats != nullptr, p.photo.plane[pl], v.colTable,
+                                   v.rowTable, i, j, rec0, rec1, g0, g1, overlap);
+  }
+};
+
 template <class Pos, class = void>
 struct HasPinholeLoop : std::false_type {};
 template <class Pos>
@@ -347,6 +408,7 @@ cudaError_t launchPerFrameGather(PerFrameGatherParams p, PerFrameSource source, 
     case PerFrameSource::kLensBlend: return launchPositions<LensBlendPositions>(p, barrel, numTiles, numSMs, stream);
     case PerFrameSource::kRectilinear: return launchPositions<RectilinearPositions>(p, p.lens, numTiles, numSMs, stream);
     case PerFrameSource::kCameraMip: return launchPositions<MipCameraPositions>(p, p.lens, numTiles, numSMs, stream);
+    case PerFrameSource::kLensPhoto: return launchPositions<LensPhotoPositions>(p, barrel, numTiles, numSMs, stream);
   }
   return cudaErrorInvalidValue;
 }

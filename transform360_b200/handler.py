@@ -172,6 +172,19 @@ class T360LensRig(C.Structure):
     _fields_ = [("numLenses", C.c_int), ("calibWidth", C.c_int), ("calibHeight", C.c_int), ("lens", T360Lens * 2)]
 
 
+class T360LensPhotometry(C.Structure):
+    """The photometry of one lens (include/transform360_b200.h): vignetting v1..v3 of the falloff V(r) = 1 + v1 r^2 +
+    v2 r^4 + v3 r^6 (r = theta_d in radians), and per plane (0 luma, 1 and 2 chroma) a gain in (0, 8] and an offset in
+    [-64, 64] code values."""
+    _fields_ = [("vignetting", C.c_float * 3), ("gain", C.c_float * 3), ("offset", C.c_float * 3)]
+
+
+class T360RigPhotometry(C.Structure):
+    """The photometry of a rig (include/transform360_b200.h): lumaPivot (0..255, the level luma scales about; chroma scales
+    about 128) and one T360LensPhotometry per lens."""
+    _fields_ = [("lumaPivot", C.c_int), ("lens", T360LensPhotometry * 2)]
+
+
 def make_context(**overrides) -> FrameTransformContext:
     vals = dict(FILTER_DEFAULTS)
     for k in overrides:
@@ -267,6 +280,12 @@ def load(path: os.PathLike | None = None):
     L.T360B200_lensBlendMaps.argtypes = [C.POINTER(FrameTransformContext), C.POINTER(T360LensRig), C.c_float, C.POINTER(T360Orientation)] + [ci] * 4 + [vp] * 3
     L.T360B200_transformFrameLensBlendAsync.restype = ci
     L.T360B200_transformFrameLensBlendAsync.argtypes = [vp, C.POINTER(T360LensRig), C.c_float, C.POINTER(T360Orientation), ci] + planes
+    L.T360B200_lensPhotoMaps.restype = ci
+    L.T360B200_lensPhotoMaps.argtypes = [C.POINTER(FrameTransformContext), C.POINTER(T360LensRig), C.POINTER(T360RigPhotometry), C.c_float,
+                                         C.POINTER(T360Orientation)] + [ci] * 5 + [vp] * 5
+    L.T360B200_transformFrameLensPhotoAsync.restype = ci
+    L.T360B200_transformFrameLensPhotoAsync.argtypes = [vp, C.POINTER(T360LensRig), C.POINTER(T360RigPhotometry), C.c_float,
+                                                        C.POINTER(T360Orientation), vp, ci] + planes
     L.T360B200_rectilinearMap.restype = ci
     L.T360B200_rectilinearMap.argtypes = [C.POINTER(FrameTransformContext), C.POINTER(T360LensRig), C.POINTER(T360Pose)] + [ci] * 4 + [vp]
     L.T360B200_transformFrameRectilinearAsync.restype = ci
@@ -315,6 +334,7 @@ EXPORTED_SYMBOLS = [
     "T360B200_transformFrameViewAsync", "T360B200_viewSamples",
     "T360B200_transformFrameOrientedAsync", "T360B200_orientedSamples", "T360B200_transformFramePoseAsync", "T360B200_poseSamples",
     "T360B200_lensMap", "T360B200_transformFrameLensAsync", "T360B200_lensBlendMaps", "T360B200_transformFrameLensBlendAsync",
+    "T360B200_lensPhotoMaps", "T360B200_transformFrameLensPhotoAsync",
     "T360B200_rectilinearMap", "T360B200_transformFrameRectilinearAsync", "T360B200_cameraMap", "T360B200_transformFrameCameraAsync",
     "T360B200_cameraMipMaps", "T360B200_transformFrameCameraMipAsync",
     "T360B200_setPinHostPlanes", "T360B200_debugTrace", "T360B200_debugTraceRead", "T360B200_synchronize", "T360B200_stream", "T360B200_kernelLaunchCount", "T360B200_planDeviceBytes",
@@ -428,6 +448,15 @@ class VideoFrameTransform:
         n, enqueue = self._frame_call("T360B200_transformFrameLensBlendAsync", in_planes, out_planes, dims)
         return lambda rig, seam_width, orientation, stream=0: enqueue(
             (C.byref(rig), seam_width, C.byref(as_orientation(orientation)), n), stream)
+
+    def make_lens_photo_frame_call(self, in_planes, out_planes, dims):
+        """Like make_lens_frame_call, for T360B200_transformFrameLensPhotoAsync (a rig with photometry: each lens's samples
+        corrected before the seam, seam_width 0 for the hard seam): returns a callable f(rig, photometry, seam_width,
+        orientation, stream, stats=0) -> bool, `photometry` a T360RigPhotometry and `stats` the device address of
+        [planes][6] uint64 sums (0: none)."""
+        n, enqueue = self._frame_call("T360B200_transformFrameLensPhotoAsync", in_planes, out_planes, dims)
+        return lambda rig, photometry, seam_width, orientation, stream=0, stats=0: enqueue(
+            (C.byref(rig), C.byref(photometry), seam_width, C.byref(as_orientation(orientation)), stats or None, n), stream)
 
     def make_rectilinear_frame_call(self, in_planes, out_planes, dims):
         """Like make_frame_call, for T360B200_transformFrameRectilinearAsync (a perspective view, no plan needed): returns a
@@ -696,6 +725,21 @@ def lens_blend_maps(ctx: FrameTransformContext, rig: T360LensRig, seam_width, or
                                          out_w, out_h, map0.ctypes.data, map1.ctypes.data, weight.ctypes.data):
         raise ValueError("T360B200_lensBlendMaps refused the arguments (message on stdout)")
     return map0, map1, weight
+
+
+def lens_photo_maps(ctx: FrameTransformContext, rig: T360LensRig, photometry: T360RigPhotometry, seam_width, orientation, plane, in_w, in_h,
+                    out_w, out_h) -> tuple[np.ndarray, np.ndarray, np.ndarray, np.ndarray, np.ndarray]:
+    """The host twin of one plane (0 luma, 1 and 2 chroma) of a rig with photometry (T360B200_lensPhotoMaps, no CUDA):
+    (map0, map1, weight, gain0, gain1).  map0 / map1: float32 [out_h][out_w][2] CV_32FC2 maps of lens 0 / lens 1, NaN where
+    that lens does not cover the pixel; weight: uint16, w of lens 1 (0 or 256 with seam_width 0, the hard seam); gain0 /
+    gain1: uint16, each lens's Gq (4096 = 1), 0 where it does not cover the pixel."""
+    map0, map1 = np.empty((out_h, out_w, 2), np.float32), np.empty((out_h, out_w, 2), np.float32)
+    weight, gain0, gain1 = (np.empty((out_h, out_w), np.uint16) for _ in range(3))
+    if not load().T360B200_lensPhotoMaps(C.byref(ctx), C.byref(rig), C.byref(photometry), seam_width, C.byref(as_orientation(orientation)),
+                                         plane, in_w, in_h, out_w, out_h, map0.ctypes.data, map1.ctypes.data, weight.ctypes.data,
+                                         gain0.ctypes.data, gain1.ctypes.data):
+        raise ValueError("T360B200_lensPhotoMaps refused the arguments (message on stdout)")
+    return map0, map1, weight, gain0, gain1
 
 
 def rectilinear_map(ctx: FrameTransformContext, pose, in_w, in_h, out_w, out_h, rig: T360LensRig | None = None) -> np.ndarray:
