@@ -8,7 +8,7 @@ What pins what:
   - geometry that does not restate the contract: the equidistant angle-to-radius law, the stereographic little planet's
     nadir and rings, Pannini's straight verticals, its d = 0 limit and the forward Pannini projection;
   - sincCos, the equidistant model's sin(rho) / rho and cos(rho), against double over every float of its range (the host
-    build; tests/test_device_twins.py compares the device build with it over every 32-bit input, and cameraRay and the
+    build; tests/test_twin_gates.py compares the device build with it over every 32-bit input, and cameraRay and the
     rectilinear chains of every model over structured families);
   - the frames against the plain-C oracle's cv::remap of camera_map's map and against the planned path, and the records
     the kernel computes read back through test_position_chains' decode and compared with the host twin's.

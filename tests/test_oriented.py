@@ -6,7 +6,7 @@ context with fixed_yaw / pitch / roll replaced by it -- low-pass and area resize
 synchronising the device.  The kernel computes each pixel's sampling record with csrc/oriented_view.h, whose equirect input
 lookup needs atan2f and asinf exactly as the host libm computes them: csrc/libm_ports.h ports them, and the first test
 compares the ports with the library over every float input (asinf, atanf) and 10^8 seeded pairs (atan2f, drawn by
-tests/atan2_pairs.h).  That pins the host build; tests/test_device_twins.py pins the device build to it, bit for bit.
+tests/atan2_pairs.h).  That pins the host build; tests/test_twin_gates.py pins the device build to it, bit for bit.
 T360B200_orientedSamples runs the chain on the host and is checked against the planner here."""
 import ctypes as C
 import math

@@ -1,100 +1,20 @@
-// Host / device twin gate: the device build of every float function of the per-frame position chains (csrc/flat_view.h,
-// libm_ports.h, oriented_view.h) against its host build, the one the planner runs.  tests/test_device_twins.py builds it
-// with the library's own nvcc flags (transform360_b200/build.py: ARCH, -O3, HOST_FLAGS) and runs it.
-//
-// A probe is a T360_HD function of an index i: it draws its inputs from (probe, i) alone -- a splitmix64 stream seeded
-// with a hash of (seed, probe, i) -- calls one twin function or chain, and packs the result into at most four 32-bit
-// words.  The same probe code runs in a kernel on the device and in a thread pool on the host.  Three tiers:
-//   A. every 32-bit pattern: libmAtanf, libmAsinf, fSqrt, sincCos, truncToInt, roundHalfEven, quantizeAxis (K = 1, 2, 4, 8);
+// Twin gate of the per-frame position chains: the device build of every float function of csrc/flat_view.h, libm_ports.h
+// and oriented_view.h that the per-frame kernels call, against its host build, the one the planner runs.  The harness,
+// its comparison rule and its modes are tests/twin_gate.cuh's.  Three tiers:
+//   A. every 32-bit pattern (fullOnly; under --shift, patternA samples one in 2^S): libmAtanf, libmAsinf, fSqrt, sincCos,
+//      truncToInt, roundHalfEven, quantizeAxis (K = 1, 2, 4, 8);
 //   B. structured families (arbitrary bit patterns, special values, values a few ulps either side of each branch threshold
 //      and realistic values): libmAtan2f, pixelCentre, toPixel, rotateHD, rayToSphereHD, warpOffCentreHD, sphereInputHD,
 //      lensPosition, lensBlendPosition, cameraRay (equidistant, stereographic, Pannini: the pinhole ray is not part of
 //      cameraRay, rectilinearPoint builds it, and tier C covers it);
 //   C. whole chains over geometries from sphereGeometry() of seeded contexts with their buildSphereTables tables:
 //      flatSample, sphereSample, lensSample, lensBlendSample and rectilinearSample in every instantiation the kernels use.
-//
-// Comparison: integer words compare raw, float words bit for bit (-0 against +0 included), with one exception: every NaN
-// equals every NaN (each probe writes a NaN float as 0x7fc00000).  x86 propagates a NaN's payload and sm_90 returns the
-// canonical NaN; no record depends on a payload (roundHalfEven maps every NaN to INT_MIN).  There is no other exception.
-//
-// Each half sums a 64-bit mix of (probe, i, words) over each block of 2^20 inputs: an order-independent fingerprint.  The
-// host compares the fingerprints; for up to 16 mismatching blocks per probe both halves re-evaluate the block element by
-// element, and at most 20 lines `probe i input-bits host-bits device-bits` are printed, then the probes that mismatch.  A mismatching block that is not
-// re-evaluated counts as one mismatch.  The last line is `<P> probes, <N> inputs, <M> mismatches`; the exit status is 1 on
-// any mismatch.
-//
-//   twin_gate [--threads T] [--shift S]     the full gate (tiers B and C have 2^S times fewer inputs, tier A samples
-//                                           one pattern in 2^S)
-//   twin_gate --host-only [--threads T]     the host half of tiers B and C at 2^20 inputs each, per-probe fingerprints
-//                                           printed; no CUDA runtime call
-//   twin_gate --self-test [--threads T]     the host half against a copy of itself with one bit of one word flipped
-//   twin_gate --ledger [--threads T]        per-probe counts of the input classes tiers B and C are meant to reach, over
-//                                           the --host-only inputs (a prefix of the full gate's)
-#include <cuda_runtime.h>
-
-#include <algorithm>
-#include <atomic>
-#include <chrono>
-#include <cinttypes>
-#include <cstdio>
-#include <cstdlib>
-#include <cstring>
-#include <functional>
-#include <string>
-#include <thread>
-#include <vector>
-
-#include "atan2_pairs.h"
-#include "oriented_view.h"
+#include "twin_gate.cuh"
 
 using namespace t360;
-using t360gate::mix64;
+using namespace t360gate;
 
 namespace {
-
-constexpr int kBlockShift = 20;
-constexpr uint64_t kBlock = 1ull << kBlockShift;
-constexpr uint64_t kSeed = 20261017ull;
-constexpr uint64_t kHostOnlyInputs = kBlock;
-
-// ---- inputs -----------------------------------------------------------------------------------------------------------
-// The draws of one (probe, i): a splitmix64 stream from a hash of (seed, probe, i), so inputs do not depend on the order
-// or the thread that evaluates them.  Every float it makes is exact (integer scaling by powers of two) or made with the
-// twin operations, so both halves see the same bits.
-struct Draw {
-  uint64_t s;
-  T360_HD Draw(int probe, uint64_t i) : s(mix64(kSeed ^ (static_cast<uint64_t>(probe) << 56) ^ mix64(i))) {}
-  T360_HD uint32_t u32() {
-    s += 0x9e3779b97f4a7c15ull;
-    return static_cast<uint32_t>(mix64(s) >> 32);
-  }
-  T360_HD int below(int n) { return static_cast<int>(u32() % static_cast<uint32_t>(n)); }
-  T360_HD bool coin() { return u32() & 1u; }
-  T360_HD float unit() { return static_cast<float>(u32() >> 8) * 0x1p-24f; }  // [0, 1), exact
-  T360_HD float range(float a, float b) { return fAdd(a, fMul(fSub(b, a), unit())); }
-  T360_HD float sign(float v) { return coin() ? -v : v; }
-  T360_HD float bits() { return bitsFloat(u32()); }
-  // +-0, +-1, +-0.5, +-inf, NaN, a subnormal, the largest float, a tiny normal
-  T360_HD float special() {
-    const uint32_t v[] = {0x00000000u, 0x3f800000u, 0x3f000000u, 0x7f800000u, 0x7fc00000u, 0x00000001u, 0x007fffffu, 0x7f7fffffu, 0x00800000u};
-    return sign(bitsFloat(v[below(9)]));
-  }
-};
-
-T360_HD uint32_t fw(float f) { return f != f ? 0x7fc00000u : floatBits(f); }  // the canonical word of a float result
-T360_HD uint32_t iw(int v) { return static_cast<uint32_t>(v); }
-
-struct Words {
-  uint32_t in[4];
-  uint32_t out[4];
-  uint64_t cls;  // ledger classes (host only)
-};
-
-#ifdef __CUDA_ARCH__
-#define CLASS(k, cond) ((void)0)
-#else
-#define CLASS(k, cond) (w.cls |= (cond) ? (1ull << (k)) : 0ull)
-#endif
 
 // ---- data the structured probes and the chains share (host-built, copied to the device) ------------------------------
 struct GeoEntry {
@@ -119,15 +39,6 @@ T360_HD uint32_t patternA(const GateData& D, uint64_t i) {
   if (D.shift == 0) return static_cast<uint32_t>(i);
   return static_cast<uint32_t>((i << D.shift) | (mix64(i) & ((1ull << D.shift) - 1)));
 }
-
-enum Probe {
-  kAtanf, kAsinf, kSqrt, kSincCos, kTrunc, kRound, kQuantize,                                  // A
-  kAtan2, kPixelCentre, kToPixel, kRotate, kRayToSphere, kWarpOffCentre, kSphereInput, kLens,  // B
-  kLensBlend0, kLensBlend1, kCameraRay,
-  kFlat, kSphere, kSpherePlain, kLensChain, kLensChainPlain, kBlendChain, kBlendChainPlain,    // C
-  kRectCtx, kRectCtxPinhole, kRectLens, kRectLensPinhole,
-  kProbes
-};
 
 constexpr int kToPixelPlanes = 4;
 T360_HD int toPixelWidth(int k) { return k == 0 ? 1 : k == 1 ? 3 : k == 2 ? 1920 : 7679; }  // odd and even plane widths
@@ -262,12 +173,83 @@ T360_HD SphereVec drawRigDirection(Draw& r, const LensRigModel& rig) {
   }
 }
 
+#define CHAIN_LAYOUTS "cube32 cube23 eac equirect barrel barrelSplit "
+#define CHAIN_PLAIN_LAYOUTS "cube32 cube23 eac equirect - - "
+#define CHAIN_NO_LAYOUTS "- - - - - - "
+#define CHAIN_CLASSES "offCentreHorizontal offCentreFull splitLR splitTBvflip packLR packTB cubeInput oddMap oddInput K1 K2 K4 K8 -"
+
+struct TwinGate {
+  static constexpr uint64_t kSeed = 20261017ull;
+  static constexpr int kOut = 4;
+  enum Probe {
+    kAtanf, kAsinf, kSqrt, kSincCos, kTrunc, kRound, kQuantize,                                  // A
+    kAtan2, kPixelCentre, kToPixel, kRotate, kRayToSphere, kWarpOffCentre, kSphereInput, kLens,  // B
+    kLensBlend0, kLensBlend1, kCameraRay,
+    kFlat, kSphere, kSpherePlain, kLensChain, kLensChainPlain, kBlendChain, kBlendChainPlain,    // C
+    kRectCtx, kRectCtxPinhole, kRectLens, kRectLensPinhole,
+    kProbes
+  };
+  // the classes each probe's ledger names, in CLASS order, and the inputs per probe
+  static constexpr ProbeInfo kInfo[kProbes] = {
+      {"atanf", "", 1ull << 32, true},
+      {"asinf", "", 1ull << 32, true},
+      {"fSqrt", "", 1ull << 32, true},
+      {"sincCos", "", 1ull << 32, true},
+      {"truncToInt", "", 1ull << 32, true},
+      {"roundHalfEven", "", 1ull << 32, true},
+      {"quantizeAxis", "", 1ull << 32, true},
+      {"libmAtan2f", "nan xIsOne zero inf ratioAbove2^60 negativeXRatioBelow2^-60 atanfTiny atanfBelow7/16 atanfBelow11/16 "
+                     "atanfBelow19/16 atanfBelow39/16 atanfBelow2^24 atanfAbove2^24 atanfNearSplit", 1ull << 28},
+      {"pixelCentre", "", 1ull << 28},
+      {"toPixel", "", kToPixelFloats * kToPixelPlanes},
+      {"rotateHD", "angles rawMatrix signedZeroQ", 1ull << 28},
+      {"rayToSphereHD", "discNotPositive discBelowAlong ordinary", 1ull << 28},
+      {"warpOffCentreHD", "horizontalWarped horizontalUnwarped fullWarped fullUnwarped", 1ull << 28},
+      {"sphereInputHD", "cutPlusZero cutMinusZero pole barrelClampLow barrelClampHigh barrelNaN packLR0 packLR1 packTB0 packTB1 "
+                        "face0 face1 face2 face3 face4 face5 gIsOne majorIsHalf noFace noFaceWithoutNaN pickedMajorIsHalf", 1ull << 28},
+      {"lensPosition", "oneLens secondLens z1EqualsZ0 covered uncovered rhoZero thetaIsThetaMax thetaMaxPi", 1ull << 28},
+      {"lensBlendPosition0", "bothCoveredW0 bothCoveredW256 ramp tie only0 only1 neither", 1ull << 27},
+      {"lensBlendPosition1", "bothCoveredW0 bothCoveredW256 ramp tie only0 only1 neither", 1ull << 27},
+      {"cameraRay", "equidistantRho0 equidistantRhoAbovePi/2 equidistantRhoAbovePi stereoBelow1 stereoAt1 stereoAbove1 panniniD0 "
+                    "panniniD1 panniniKAbove1e7 equidistantZeroXY stereoZeroXY panniniZeroXY", 1ull << 28},
+      {"flatSample", CHAIN_NO_LAYOUTS CHAIN_CLASSES " fold noFold", 1ull << 26},
+      {"sphereSample<BARREL>", CHAIN_LAYOUTS CHAIN_CLASSES " deadZone", 1ull << 26},
+      {"sphereSample<plain>", CHAIN_PLAIN_LAYOUTS CHAIN_CLASSES, 1ull << 26},
+      {"lensSample<BARREL>", CHAIN_LAYOUTS CHAIN_CLASSES " covered uncovered", 1ull << 26},
+      {"lensSample<plain>", CHAIN_PLAIN_LAYOUTS CHAIN_CLASSES " covered uncovered", 1ull << 26},
+      {"lensBlendSample<BARREL>", CHAIN_LAYOUTS CHAIN_CLASSES " w0 w256 ramp", 1ull << 26},
+      {"lensBlendSample<plain>", CHAIN_PLAIN_LAYOUTS CHAIN_CLASSES " w0 w256 ramp", 1ull << 26},
+      {"rectilinearSample<ctx,any>", CHAIN_NO_LAYOUTS CHAIN_CLASSES " pinhole equidistant stereographic pannini", 1ull << 26},
+      {"rectilinearSample<ctx,pinhole>", CHAIN_NO_LAYOUTS CHAIN_CLASSES " pinhole", 1ull << 26},
+      {"rectilinearSample<lens,any>", CHAIN_NO_LAYOUTS CHAIN_CLASSES " pinhole equidistant stereographic pannini", 1ull << 26},
+      {"rectilinearSample<lens,pinhole>", CHAIN_NO_LAYOUTS CHAIN_CLASSES " pinhole", 1ull << 26},
+  };
+  // bit 3 of word 1 of a sphereInputHD element in the second block
+  static constexpr Flip kFlip = {kSphereInput, 3 * kBlock / 2 - 12345, 1, 3};
+
+  using Data = GateData;
+  struct HostData {
+    std::vector<Rotation> rot;
+    std::vector<LensRigModel> rig;
+    std::vector<RectilinearCamera> cam;
+    std::vector<GeoEntry> geo;
+    std::vector<float> tab;
+    int nRotReal = 0, nRig2 = 0, nCamPinhole = 0, nGeoPlain = 0;
+  };
+  template <int P>
+  static T360_HD void probe(const Data& D, uint64_t i, Words<kOut>& w);
+  static HostData makeData();
+  static Data view(const HostData& H, int shift);
+  static Data deviceData(const HostData& H, Data D, Uploads& up) {
+    D.rot = up(H.rot); D.rig = up(H.rig); D.cam = up(H.cam); D.geo = up(H.geo); D.tab = up(H.tab);
+    return D;
+  }
+};
+
 // ---- the probes -------------------------------------------------------------------------------------------------------
 template <int P>
-T360_HD void probe(const GateData& D, uint64_t i, Words& w) {
-  for (int k = 0; k < 4; ++k) w.in[k] = w.out[k] = 0;
-  w.cls = 0;
-  Draw r(P, i);
+T360_HD void TwinGate::probe(const GateData& D, uint64_t i, Words<kOut>& w) {
+  Draw r(kSeed, P, i);
   if constexpr (P <= kQuantize) {
     const uint32_t b = patternA(D, i);
     const float x = bitsFloat(b);
@@ -600,136 +582,7 @@ T360_HD void probe(const GateData& D, uint64_t i, Words& w) {
   }
 }
 
-// The classes each probe's ledger names, in CLASS order ("-": not a class of that probe), and the inputs per probe
-struct ProbeInfo {
-  const char* name;
-  const char* classes;
-  uint64_t inputs;
-};
-#define CHAIN_LAYOUTS "cube32 cube23 eac equirect barrel barrelSplit "
-#define CHAIN_PLAIN_LAYOUTS "cube32 cube23 eac equirect - - "
-#define CHAIN_NO_LAYOUTS "- - - - - - "
-#define CHAIN_CLASSES "offCentreHorizontal offCentreFull splitLR splitTBvflip packLR packTB cubeInput oddMap oddInput K1 K2 K4 K8 -"
-const ProbeInfo kInfo[kProbes] = {
-    {"atanf", "", 1ull << 32},
-    {"asinf", "", 1ull << 32},
-    {"fSqrt", "", 1ull << 32},
-    {"sincCos", "", 1ull << 32},
-    {"truncToInt", "", 1ull << 32},
-    {"roundHalfEven", "", 1ull << 32},
-    {"quantizeAxis", "", 1ull << 32},
-    {"libmAtan2f", "nan xIsOne zero inf ratioAbove2^60 negativeXRatioBelow2^-60 atanfTiny atanfBelow7/16 atanfBelow11/16 "
-                   "atanfBelow19/16 atanfBelow39/16 atanfBelow2^24 atanfAbove2^24 atanfNearSplit", 1ull << 28},
-    {"pixelCentre", "", 1ull << 28},
-    {"toPixel", "", kToPixelFloats * kToPixelPlanes},
-    {"rotateHD", "angles rawMatrix signedZeroQ", 1ull << 28},
-    {"rayToSphereHD", "discNotPositive discBelowAlong ordinary", 1ull << 28},
-    {"warpOffCentreHD", "horizontalWarped horizontalUnwarped fullWarped fullUnwarped", 1ull << 28},
-    {"sphereInputHD", "cutPlusZero cutMinusZero pole barrelClampLow barrelClampHigh barrelNaN packLR0 packLR1 packTB0 packTB1 "
-                      "face0 face1 face2 face3 face4 face5 gIsOne majorIsHalf noFace noFaceWithoutNaN pickedMajorIsHalf", 1ull << 28},
-    {"lensPosition", "oneLens secondLens z1EqualsZ0 covered uncovered rhoZero thetaIsThetaMax thetaMaxPi", 1ull << 28},
-    {"lensBlendPosition0", "bothCoveredW0 bothCoveredW256 ramp tie only0 only1 neither", 1ull << 27},
-    {"lensBlendPosition1", "bothCoveredW0 bothCoveredW256 ramp tie only0 only1 neither", 1ull << 27},
-    {"cameraRay", "equidistantRho0 equidistantRhoAbovePi/2 equidistantRhoAbovePi stereoBelow1 stereoAt1 stereoAbove1 panniniD0 "
-                  "panniniD1 panniniKAbove1e7 equidistantZeroXY stereoZeroXY panniniZeroXY", 1ull << 28},
-    {"flatSample", CHAIN_NO_LAYOUTS CHAIN_CLASSES " fold noFold", 1ull << 26},
-    {"sphereSample<BARREL>", CHAIN_LAYOUTS CHAIN_CLASSES " deadZone", 1ull << 26},
-    {"sphereSample<plain>", CHAIN_PLAIN_LAYOUTS CHAIN_CLASSES, 1ull << 26},
-    {"lensSample<BARREL>", CHAIN_LAYOUTS CHAIN_CLASSES " covered uncovered", 1ull << 26},
-    {"lensSample<plain>", CHAIN_PLAIN_LAYOUTS CHAIN_CLASSES " covered uncovered", 1ull << 26},
-    {"lensBlendSample<BARREL>", CHAIN_LAYOUTS CHAIN_CLASSES " w0 w256 ramp", 1ull << 26},
-    {"lensBlendSample<plain>", CHAIN_PLAIN_LAYOUTS CHAIN_CLASSES " w0 w256 ramp", 1ull << 26},
-    {"rectilinearSample<ctx,any>", CHAIN_NO_LAYOUTS CHAIN_CLASSES " pinhole equidistant stereographic pannini", 1ull << 26},
-    {"rectilinearSample<ctx,pinhole>", CHAIN_NO_LAYOUTS CHAIN_CLASSES " pinhole", 1ull << 26},
-    {"rectilinearSample<lens,any>", CHAIN_NO_LAYOUTS CHAIN_CLASSES " pinhole equidistant stereographic pannini", 1ull << 26},
-    {"rectilinearSample<lens,pinhole>", CHAIN_NO_LAYOUTS CHAIN_CLASSES " pinhole", 1ull << 26},
-};
-
-using ProbeFn = void (*)(const GateData&, uint64_t, Words&);
-template <int... P>
-constexpr std::array<ProbeFn, sizeof...(P)> probeTable(std::integer_sequence<int, P...>) {
-  return {&probe<P>...};
-}
-const auto kHostProbe = probeTable(std::make_integer_sequence<int, kProbes>());
-
-T360_HD uint64_t elementMix(int p, uint64_t i, const uint32_t* out) {
-  uint64_t h = mix64((static_cast<uint64_t>(p) << 56) ^ i);
-  for (int k = 0; k < 4; ++k) h = mix64(h ^ (static_cast<uint64_t>(out[k]) << (k & 1 ? 32 : 0)) ^ static_cast<uint64_t>(k));
-  return h;
-}
-
-// ---- the device half --------------------------------------------------------------------------------------------------
-template <int P>
-__global__ void __launch_bounds__(256) fingerprintKernel(GateData D, uint64_t inputs, uint64_t firstBlock, unsigned long long* fp) {
-  const uint64_t block = firstBlock + blockIdx.x, begin = block * kBlock, end = begin + kBlock < inputs ? begin + kBlock : inputs;
-  unsigned long long sum = 0;
-  Words w;
-  for (uint64_t i = begin + threadIdx.x; i < end; i += blockDim.x) {
-    probe<P>(D, i, w);
-    sum += elementMix(P, i, w.out);
-  }
-  for (int o = 16; o > 0; o >>= 1) sum += __shfl_down_sync(0xffffffffu, sum, o);
-  __shared__ unsigned long long warpSum[8];
-  if ((threadIdx.x & 31) == 0) warpSum[threadIdx.x >> 5] = sum;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    for (int k = 1; k < 8; ++k) sum += warpSum[k];
-    fp[block] = sum;
-  }
-}
-template <int P>
-__global__ void wordsKernel(GateData D, uint64_t begin, uint64_t count, uint32_t* out) {
-  for (uint64_t k = blockIdx.x * static_cast<uint64_t>(blockDim.x) + threadIdx.x; k < count; k += gridDim.x * static_cast<uint64_t>(blockDim.x)) {
-    Words w;
-    probe<P>(D, begin + k, w);
-    for (int q = 0; q < 4; ++q) out[4 * k + q] = w.out[q];
-  }
-}
-
-#define CUDA_OK(x)                                                                          \
-  do {                                                                                      \
-    const cudaError_t e_ = (x);                                                             \
-    if (e_ != cudaSuccess) {                                                                \
-      std::fprintf(stderr, "%s:%d %s: %s\n", __FILE__, __LINE__, #x, cudaGetErrorString(e_)); \
-      std::exit(2);                                                                         \
-    }                                                                                       \
-  } while (0)
-
-using LaunchFp = void (*)(const GateData&, uint64_t, uint64_t, uint64_t, unsigned long long*);
-using LaunchWords = void (*)(const GateData&, uint64_t, uint64_t, uint32_t*);
-template <int P>
-void launchFp(const GateData& D, uint64_t inputs, uint64_t first, uint64_t blocks, unsigned long long* fp) {
-  fingerprintKernel<P><<<static_cast<unsigned>(blocks), 256>>>(D, inputs, first, fp);
-  CUDA_OK(cudaGetLastError());
-}
-template <int P>
-void launchWords(const GateData& D, uint64_t begin, uint64_t count, uint32_t* out) {
-  wordsKernel<P><<<1024, 256>>>(D, begin, count, out);
-  CUDA_OK(cudaGetLastError());
-}
-template <int... P>
-constexpr std::array<LaunchFp, sizeof...(P)> fpTable(std::integer_sequence<int, P...>) { return {&launchFp<P>...}; }
-template <int... P>
-constexpr std::array<LaunchWords, sizeof...(P)> wordsTable(std::integer_sequence<int, P...>) { return {&launchWords<P>...}; }
-
-// ---- the shared data --------------------------------------------------------------------------------------------------
-struct HostData {
-  std::vector<Rotation> rot;
-  std::vector<LensRigModel> rig;
-  std::vector<RectilinearCamera> cam;
-  std::vector<GeoEntry> geo;
-  std::vector<float> tab;
-  int nRotReal = 0, nRig2 = 0, nCamPinhole = 0, nGeoPlain = 0;
-};
-
-struct HostRng {  // host-only draws for building the shared data (double, libm: not part of any probe's inputs)
-  uint64_t s;
-  uint64_t next() { return mix64(s++); }
-  double uniform(double a, double b) { return a + (b - a) * static_cast<double>(next() >> 11) * 0x1p-53; }
-  int below(int n) { return static_cast<int>(next() % static_cast<uint64_t>(n)); }
-};
-
-HostData makeData() {
+TwinGate::HostData TwinGate::makeData() {
   HostData H;
   HostRng g{kSeed * 7919};
   const float angles[] = {0.0f, -0.0f, 90.0f, -90.0f, 180.0f, -180.0f, 45.0f, 270.0f, 1e6f};
@@ -841,260 +694,12 @@ HostData makeData() {
   return H;
 }
 
-GateData view(const HostData& H, int shift) {
+GateData TwinGate::view(const HostData& H, int shift) {
   return GateData{H.rot.data(), static_cast<int>(H.rot.size()), H.nRotReal, H.rig.data(), static_cast<int>(H.rig.size()), H.nRig2,
                   H.cam.data(), static_cast<int>(H.cam.size()), H.nCamPinhole, H.geo.data(), static_cast<int>(H.geo.size()), H.nGeoPlain,
                   H.tab.data(), shift};
 }
 
-template <class T>
-T* upload(const std::vector<T>& v) {
-  T* d = nullptr;
-  CUDA_OK(cudaMalloc(&d, v.size() * sizeof(T)));
-  CUDA_OK(cudaMemcpy(d, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
-  return d;
-}
-
-// ---- the halves -------------------------------------------------------------------------------------------------------
-// A half gives the block fingerprints of a probe and, for a drill-down, the words of one block.
-struct Half {
-  std::function<void(int p, uint64_t inputs, std::vector<uint64_t>& fp)> fingerprints;
-  std::function<void(int p, uint64_t begin, uint64_t count, std::vector<uint32_t>& words)> words;
-};
-
-uint64_t blocksOf(uint64_t inputs) { return (inputs + kBlock - 1) / kBlock; }
-
-// fn(p, block) over every block of the given probes on `threads` threads, one block at a time per thread
-void forBlocks(int threads, const std::vector<std::pair<int, uint64_t>>& probes, const std::function<void(int, uint64_t, uint64_t)>& fn) {
-  std::vector<std::pair<int, uint64_t>> tasks;
-  for (auto [p, inputs] : probes)
-    for (uint64_t b = 0; b < blocksOf(inputs); ++b) tasks.push_back({p, b});
-  std::atomic<size_t> next{0};
-  std::vector<std::thread> pool;
-  for (int t = 0; t < threads; ++t)
-    pool.emplace_back([&] {
-      for (size_t k; (k = next.fetch_add(1)) < tasks.size();) {
-        const auto [p, b] = tasks[k];
-        uint64_t inputs = 0;
-        for (auto [q, n] : probes)
-          if (q == p) inputs = n;
-        fn(p, b, inputs);
-      }
-    });
-  for (auto& th : pool) th.join();
-}
-
-uint64_t hostBlock(const GateData& D, int p, uint64_t b, uint64_t inputs) {
-  const uint64_t begin = b * kBlock, end = std::min(inputs, begin + kBlock);
-  uint64_t sum = 0;
-  Words w;
-  for (uint64_t i = begin; i < end; ++i) {
-    kHostProbe[p](D, i, w);
-    sum += elementMix(p, i, w.out);
-  }
-  return sum;
-}
-
-void hostWords(const GateData& D, int p, uint64_t begin, uint64_t count, std::vector<uint32_t>& words) {
-  words.assign(4 * count, 0);
-  Words w;
-  for (uint64_t k = 0; k < count; ++k) {
-    kHostProbe[p](D, begin + k, w);
-    std::memcpy(&words[4 * k], w.out, sizeof(w.out));
-  }
-}
-
-// The host half's fingerprints of every probe in `probes`, computed together so the thread pool stays busy
-std::vector<std::vector<uint64_t>> hostFingerprints(const GateData& D, int threads, const std::vector<std::pair<int, uint64_t>>& probes) {
-  std::vector<std::vector<uint64_t>> fp(kProbes);
-  for (auto [p, inputs] : probes) fp[p].assign(blocksOf(inputs), 0);
-  forBlocks(threads, probes, [&](int p, uint64_t b, uint64_t inputs) { fp[p][b] = hostBlock(D, p, b, inputs); });
-  return fp;
-}
-
-// Compares the host half's fingerprints with the other half's, drills into mismatching blocks; returns the mismatches
-uint64_t compare(const GateData& D, const std::vector<std::pair<int, uint64_t>>& probes, const std::vector<std::vector<uint64_t>>& hostFp,
-                 const Half& other, uint64_t* totalInputs) {
-  uint64_t mismatches = 0;
-  int printed = 0;
-  std::string failing;
-  for (auto [p, inputs] : probes) {
-    const uint64_t before = mismatches;
-    *totalInputs += inputs;
-    std::vector<uint64_t> fp;
-    other.fingerprints(p, inputs, fp);
-    int drilled = 0;
-    for (uint64_t b = 0; b < hostFp[p].size(); ++b) {
-      if (hostFp[p][b] == fp[b]) continue;
-      if (drilled++ >= 16) {
-        ++mismatches;
-        continue;
-      }
-      const uint64_t begin = b * kBlock, count = std::min(inputs, begin + kBlock) - begin;
-      std::vector<uint32_t> hw, ow;
-      hostWords(D, p, begin, count, hw);
-      other.words(p, begin, count, ow);
-      for (uint64_t k = 0; k < count; ++k) {
-        if (std::memcmp(&hw[4 * k], &ow[4 * k], 16) == 0) continue;
-        ++mismatches;
-        if (printed++ < 20) {
-          Words w;
-          kHostProbe[p](D, begin + k, w);
-          std::printf("%s %" PRIu64 " %08x:%08x:%08x:%08x %08x:%08x:%08x:%08x %08x:%08x:%08x:%08x\n", kInfo[p].name, begin + k, w.in[0], w.in[1],
-                      w.in[2], w.in[3], hw[4 * k], hw[4 * k + 1], hw[4 * k + 2], hw[4 * k + 3], ow[4 * k], ow[4 * k + 1], ow[4 * k + 2],
-                      ow[4 * k + 3]);
-        }
-      }
-    }
-    if (mismatches > before) failing += std::string(" ") + kInfo[p].name;
-  }
-  if (!failing.empty()) std::printf("mismatching probes:%s\n", failing.c_str());
-  return mismatches;
-}
-
-double seconds(std::chrono::steady_clock::time_point t0) {
-  return std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-}
-
 }  // namespace
 
-int main(int argc, char** argv) {
-  int threads = static_cast<int>(std::thread::hardware_concurrency());
-  int shift = 0;
-  std::string mode = "full";
-  for (int a = 1; a < argc; ++a) {
-    const std::string s = argv[a];
-    if (s == "--threads" && a + 1 < argc) threads = std::atoi(argv[++a]);
-    else if (s == "--shift" && a + 1 < argc) shift = std::atoi(argv[++a]);
-    else if (s == "--host-only" || s == "--self-test" || s == "--ledger") mode = s.substr(2);
-    else {
-      std::fprintf(stderr, "usage: twin_gate [--threads T] [--shift S] [--host-only | --self-test | --ledger]\n");
-      return 2;
-    }
-  }
-  threads = std::max(1, threads);
-  const HostData H = makeData();
-  const GateData hostD = view(H, shift);
-
-  std::vector<std::pair<int, uint64_t>> probes;
-  for (int p = 0; p < kProbes; ++p) {
-    if (mode != "full" && p <= kQuantize) continue;  // tier A runs in the full gate only
-    uint64_t n = kInfo[p].inputs;
-    if (mode != "full") n = std::min(n, kHostOnlyInputs);
-    else if (p <= kQuantize) n >>= shift;
-    else n = std::max<uint64_t>(n >> shift, 1);
-    probes.push_back({p, n});
-  }
-
-  if (mode == "ledger") {
-    for (auto [p, inputs] : probes) {
-      std::vector<std::atomic<uint64_t>> counts(64);
-      std::vector<std::thread> pool;
-      for (int t = 0; t < threads; ++t)
-        pool.emplace_back([&, t, p = p, inputs = inputs] {
-          std::vector<uint64_t> local(64, 0);
-          Words w;
-          for (uint64_t i = t; i < inputs; i += threads) {
-            kHostProbe[p](hostD, i, w);
-            for (int k = 0; k < 64; ++k) local[k] += (w.cls >> k) & 1u;
-          }
-          for (int k = 0; k < 64; ++k) counts[k] += local[k];
-        });
-      for (auto& th : pool) th.join();
-      const std::string names = kInfo[p].classes;
-      size_t at = 0;
-      for (int k = 0; at < names.size(); ++k) {
-        const size_t sp = names.find(' ', at);
-        const std::string name = names.substr(at, sp == std::string::npos ? std::string::npos : sp - at);
-        at = sp == std::string::npos ? names.size() : sp + 1;
-        if (name != "-") std::printf("class %s %s %" PRIu64 "\n", kInfo[p].name, name.c_str(), counts[k].load());
-      }
-    }
-    return 0;
-  }
-
-  auto t0 = std::chrono::steady_clock::now();
-  const std::vector<std::vector<uint64_t>> hostFp = hostFingerprints(hostD, threads, probes);
-  const double hostSeconds = seconds(t0);
-
-  if (mode == "host-only") {
-    for (auto [p, inputs] : probes) {
-      uint64_t h = 0;
-      for (uint64_t f : hostFp[p]) h = mix64(h ^ f);
-      std::printf("fingerprint %s %" PRIu64 " %016" PRIx64 "\n", kInfo[p].name, inputs, h);
-    }
-    std::printf("host %.1f s on %d threads\n", hostSeconds, threads);
-    return 0;
-  }
-
-  uint64_t totalInputs = 0, mismatches = 0;
-  if (mode == "self-test") {
-    // the other half: the host half with bit 3 of word 1 of one sphereInputHD element flipped
-    const int fp = kSphereInput;
-    const uint64_t fi = 3 * kBlock / 2 - 12345;
-    Half flipped;
-    flipped.words = [&](int p, uint64_t begin, uint64_t count, std::vector<uint32_t>& words) {
-      hostWords(hostD, p, begin, count, words);
-      if (p == fp && fi >= begin && fi < begin + count) words[4 * (fi - begin) + 1] ^= 8u;
-    };
-    flipped.fingerprints = [&](int p, uint64_t inputs, std::vector<uint64_t>& out) {
-      out.assign(blocksOf(inputs), 0);
-      for (uint64_t b = 0; b < out.size(); ++b) {
-        const uint64_t begin = b * kBlock, count = std::min(inputs, begin + kBlock) - begin;
-        std::vector<uint32_t> words;
-        flipped.words(p, begin, count, words);
-        for (uint64_t k = 0; k < count; ++k) out[b] += elementMix(p, begin + k, &words[4 * k]);
-      }
-    };
-    for (auto& pr : probes)
-      if (pr.first == fp) pr.second = 2 * kBlock;  // two blocks: the flip sits in the second
-    const std::vector<std::vector<uint64_t>> fp2 = hostFingerprints(hostD, threads, probes);
-    mismatches = compare(hostD, probes, fp2, flipped, &totalInputs);
-    std::printf("self-test: flipped %s %" PRIu64 " word 1 bit 3\n", kInfo[fp].name, fi);
-  } else {
-    // the device half
-    GateData devD = hostD;
-    Rotation* dRot = upload(H.rot);
-    LensRigModel* dRig = upload(H.rig);
-    RectilinearCamera* dCam = upload(H.cam);
-    GeoEntry* dGeo = upload(H.geo);
-    float* dTab = upload(H.tab);
-    devD.rot = dRot; devD.rig = dRig; devD.cam = dCam; devD.geo = dGeo; devD.tab = dTab;
-    constexpr auto launchFps = fpTable(std::make_integer_sequence<int, kProbes>());
-    constexpr auto launchW = wordsTable(std::make_integer_sequence<int, kProbes>());
-    unsigned long long* dFp = nullptr;
-    uint32_t* dWords = nullptr;
-    uint64_t maxBlocks = 0;
-    for (auto [p, inputs] : probes) maxBlocks = std::max(maxBlocks, blocksOf(inputs));
-    CUDA_OK(cudaMalloc(&dFp, maxBlocks * sizeof(unsigned long long)));
-    CUDA_OK(cudaMalloc(&dWords, 4 * kBlock * sizeof(uint32_t)));
-    cudaEvent_t e0, e1;
-    CUDA_OK(cudaEventCreate(&e0));
-    CUDA_OK(cudaEventCreate(&e1));
-    float deviceMs = 0.0f;
-    Half device;
-    device.fingerprints = [&](int p, uint64_t inputs, std::vector<uint64_t>& out) {
-      const uint64_t blocks = blocksOf(inputs);
-      CUDA_OK(cudaEventRecord(e0));
-      for (uint64_t b = 0; b < blocks; b += 65535) launchFps[p](devD, inputs, b, std::min<uint64_t>(65535, blocks - b), dFp);
-      CUDA_OK(cudaEventRecord(e1));
-      CUDA_OK(cudaEventSynchronize(e1));
-      float ms;
-      CUDA_OK(cudaEventElapsedTime(&ms, e0, e1));
-      deviceMs += ms;
-      out.resize(blocks);
-      CUDA_OK(cudaMemcpy(out.data(), dFp, blocks * sizeof(uint64_t), cudaMemcpyDeviceToHost));
-    };
-    device.words = [&](int p, uint64_t begin, uint64_t count, std::vector<uint32_t>& words) {
-      launchW[p](devD, begin, count, dWords);
-      words.resize(4 * count);
-      CUDA_OK(cudaMemcpy(words.data(), dWords, 4 * count * sizeof(uint32_t), cudaMemcpyDeviceToHost));
-    };
-    mismatches = compare(hostD, probes, hostFp, device, &totalInputs);
-    std::printf("device %.1f s, host %.1f s on %d threads\n", deviceMs / 1000.0, hostSeconds, threads);
-    cudaFree(dFp); cudaFree(dWords); cudaFree(dRot); cudaFree(dRig); cudaFree(dCam); cudaFree(dGeo); cudaFree(dTab);
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
-  }
-  std::printf("%zu probes, %" PRIu64 " inputs, %" PRIu64 " mismatches\n", probes.size(), totalInputs, mismatches);
-  return mismatches ? 1 : 0;
-}
+int main(int argc, char** argv) { return runGate<TwinGate>(argc, argv); }

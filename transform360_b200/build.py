@@ -22,7 +22,7 @@ SOURCES = ["geometry.cpp", "lowpass_plan.cpp", "lowpass_jobs.cpp", "sampling.cpp
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 # host code: -ffp-contract=off keeps the planner's float sequence identical to the reference's build, and the host twins
 # of the per-frame position chains (csrc/flat_view.h, libm_ports.h, oriented_view.h) plain IEEE operations.
-# tests/test_device_twins.py builds its host / device comparison with the same string.
+# tests/test_twin_gates.py builds its host / device comparisons with the same string.
 HOST_FLAGS = "-fPIC,-fvisibility=hidden,-ffp-contract=off,-fno-fast-math,-Wall"
 
 
