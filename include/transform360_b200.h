@@ -563,6 +563,66 @@ int T360B200_transformFrameCameraMipAsync(VideoFrameTransform* transform, const 
                                           const uint8_t* const* deviceInputs, uint8_t* const* deviceOutputs, const int* inputWidths,
                                           const int* inputHeights, const int* inputPitches, const int* outputWidths,
                                           const int* outputHeights, const int* outputPitches, void* cudaStream);
+/* ---- camera views of a lens rig with photometry ----------------------------------------------------------
+ * The camera views above take a rig's hard, uncorrected seam, so a view panned across the seam of a dual-fisheye clip
+ * shows the step the lens photometry removes from sphere outputs.  This call gives the rectilinear view (the pinhole
+ * camera, bit for bit), the other camera models and the anti-aliased views of a rig the photometry and the seam of
+ * T360B200_transformFrameLensPhotoAsync.  Per output pixel of each plane:
+ *   1. ray: steps 1-5 of the camera views (X, Y, the model's ray q, the pose's rotation); the rig is mono, so there is no
+ *      eye split;
+ *   2. lenses: the lens photometry's per-lens step on that ray: each lens's entry (the lens calls' projection, NaN where
+ *      the lens does not cover the ray), its Gq, and the seam weight w of lens 1 (0 or 256 from the closer lens with
+ *      seamWidth = 0; the feathered seam's w otherwise);
+ *   3. pyramid (minify not NULL and the plane's top level T > 0; the pyramid of the anti-aliased views, step 1): each lens
+ *      whose entry is finite takes its own footprint, steps 2-3 of the anti-aliased views with the Jacobian of that lens
+ *      (not the closer lens's), so its own level and next-level weight, and its entries at those levels (step 4).  A lens
+ *      that does not cover the ray has level 0 and weight 0.  A pixel in the seam's belt may so gather four windows, two
+ *      lenses at two levels each;
+ *   4. combining: each lens's sample S_i is the blend of its two levels (step 5 of the anti-aliased views; its level-0
+ *      sample alone without a pyramid), then S_i' = s' of the lens photometry with that lens's Gq and Oq, then the seam
+ *      combines S_0' and S_1' exactly as T360B200_transformFrameLensPhotoAsync does.  Samples that BORDER_TRANSPARENT skips
+ *      stay skipped; the pre-fill and the output bytes that are kept are the lens calls' (chroma 128, luma the caller's);
+ *   5. statistics: deviceStats (device memory, NULL: none) receives the lens photometry's [numPlanes][6] sums over S_0'
+ *      and S_1', where both lenses cover the ray and neither sample is skipped, zeroed with a memset in stream order.
+ *      Every output pixel weighs the same.
+ * With the identity photometry (vignetting 0, gain 1, offset 0) and seamWidth = 0 the frame is
+ * T360B200_transformFrameCameraAsync's with the rig byte for byte without a pyramid (minify NULL or maxLevel 0), and
+ * T360B200_transformFrameCameraMipAsync's with the rig with one.  Taking statistics never changes the frame.  The limits of
+ * the lens photometry (no transfer function, one falloff for every plane, centred; gains chosen by the caller) and of the
+ * anti-aliased views (an isotropic footprint; a lens's dark surround reaches its rim texels at coarse levels) carry over.
+ * A frame takes one launch, or T_max + 1 with a pyramid (one per level, then the gather), plus the memset with statistics.
+ *
+ * Refused, with 0 and a message on stdout before any CUDA call: a NULL rig (the photometry is per lens); every refusal of
+ * T360B200_transformFrameCameraAsync with a rig; a seamWidth that is negative, not finite or in (0, 0.01), and with
+ * seamWidth > 0 a rig of one lens or a seamWidth above 180; every refusal of the photometry of
+ * T360B200_transformFrameLensPhotoAsync; and where minify is not NULL every refusal of T360B200_transformFrameCameraMipAsync
+ * about it, and (frame call only) with maxLevel > 0 an input plane side above 131070. */
+/* Host only, no CUDA: the twin of plane `plane` (0..2) of inputWidth x inputHeight, one lens (0 or 1) per call.  map0,
+ * map1, level, weight: T360B200_cameraMipMaps' four arrays for that lens (the entry in its level's pixels, in level + 1's
+ * pixels, the level, the next level's weight); NaN entries, level 0 and weight 0 where the lens does not cover the ray.
+ * gain: that lens's Gq (uint16, 0 where it does not cover the ray); seamWeight: w of step 2 (uint16).  Both lenses'
+ * entries are given wherever they cover the ray, with either seam.  cv::remap of each level's entries over the pyramid,
+ * blended as in step 4 per lens, then s', then the seam (the other alone where one is skipped) gives the frame's plane bit
+ * for bit; the statistics are the sums over the pixels where both lenses' map0 entries are finite and neither sample is
+ * skipped.  With the identity photometry and seamWidth = 0 the closer lens's arrays are T360B200_cameraMipMaps' with the rig
+ * where it covers the ray (T360B200_cameraMap's entries without a pyramid) and its gain 4096.  Returns 1; 0 (message) for
+ * the refusals above, a lens outside 0..1, a plane outside 0..2, a NULL context or array, or non-positive sizes. */
+int T360B200_cameraPhotoMaps(const FrameTransformContext* ctx, const T360LensRig* rig, const T360RigPhotometry* photometry, float seamWidth,
+                             const T360Pose* pose, const T360Camera* camera, const T360Minify* minify /* NULL: no pyramid */, int lens,
+                             int plane, int inputWidth, int inputHeight, int outputWidth, int outputHeight, float* map0, float* map1,
+                             uint8_t* level, uint16_t* weight, uint16_t* gain, uint16_t* seamWeight);
+/* One frame of a camera view of a lens rig with photometry, every plane in one gather launch after the pyramid's: the
+ * arguments and asynchronous contract of T360B200_transformFrameCameraMipAsync with a rig, plus photometry, seamWidth and
+ * deviceStats; every argument may change every frame.  Needs no plan and does not touch the plans; takes the reader lock;
+ * never synchronises the device.  There is no planned path: a plan carries one record per pixel.  Returns 1 if everything
+ * was enqueued; 0 with a message on stdout, before any CUDA call, for the refusals above, 0 or more than 3 planes, or an
+ * invalid plane description. */
+int T360B200_transformFrameCameraPhotoAsync(VideoFrameTransform* transform, const T360LensRig* rig, const T360RigPhotometry* photometry,
+                                            float seamWidth, const T360Pose* pose, const T360Camera* camera,
+                                            const T360Minify* minify /* NULL: no pyramid */, unsigned long long* deviceStats /* NULL: none */,
+                                            int numPlanes, const uint8_t* const* deviceInputs, uint8_t* const* deviceOutputs,
+                                            const int* inputWidths, const int* inputHeights, const int* inputPitches,
+                                            const int* outputWidths, const int* outputHeights, const int* outputPitches, void* cudaStream);
 /* Opt-in (also: environment T360B200_PIN_HOST_PLANES=1): page-lock pageable caller planes in place the second time
  * the same buffer is seen (cudaHostRegister), so that recycled frame-pool buffers are DMA'd at full PCIe speed.  The
  * caller must keep such buffers alive until VideoFrameTransform_delete. */

@@ -398,7 +398,10 @@ void countKernelLaunches(long long n);  // kernels launched through a replayed C
 //   kLensPhoto    a lens rig with photometry (rotation, rig, seamScale, photo; lensPhotoSample): the hard seam
 //                 (seamScale = 0) or the feathered one; each lens's sample is corrected with its gain (photoCorrect)
 //                 before the seam combines them, and with photo.stats set the overlap's sums are accumulated.
-enum class PerFrameSource { kView, kSphere, kMap, kLens, kLensBlend, kRectilinear, kCameraMip, kLensPhoto };
+//   kCameraPhoto  a camera view of a lens rig with photometry (camera, rig, seamScale, cameraPhoto: the planes' pyramids
+//                 and the photometric constants, mipBias; cameraPhotoSample): each lens's sample is the blend of its own two levels (kCameraMip's
+//                 blend; level 0 alone without a pyramid), then corrected, combined and counted as kLensPhoto's.
+enum class PerFrameSource { kView, kSphere, kMap, kLens, kLensBlend, kRectilinear, kCameraMip, kLensPhoto, kCameraPhoto };
 struct PerFramePlane {
   const uint8_t* src;  // (blurred) input plane, geometry.inW x geometry.inH
   uint8_t* dst;        // render target, geometry.mapW x geometry.mapH
@@ -439,15 +442,32 @@ struct PerFrameGatherParams {
     LensPhotoPlane plane[kMaxFramePlanes];
     unsigned long long* stats;
   };
-  // (the two sources' constants share their storage, so the block keeps the size and layout every other source's
-  // kernel was compiled against)
+  // kCameraPhoto: both of the above, per plane its footprint constants and pyramid levels (a level's sides in 16 bits, so
+  // the two fit in mip's storage), and the photometric constants
+  struct CameraPhotoLevel {
+    uint8_t* bytes;
+    int pitch;
+    uint16_t w, h;
+  };
+  struct CameraPhotoPlane {
+    MipGeometry geometry;
+    CameraPhotoLevel level[kMipMaxLevels];  // [l - 1]: level l
+  };
+  struct CameraPhoto {
+    CameraPhotoPlane mip[kMaxFramePlanes];
+    LensPhoto photo;
+  };
+  // (the three sources' constants share their storage, so the block keeps the size and layout every other source's
+  // kernel was compiled against: a larger block would move the kernels' next parameter)
   union {
     MipPlane mip[kMaxFramePlanes];
     LensPhoto photo;
+    CameraPhoto cameraPhoto;
   };
   int mipBias;
 };
 static_assert(sizeof(PerFrameGatherParams::LensPhoto) <= sizeof(PerFrameGatherParams::MipPlane) * kMaxFramePlanes);
+static_assert(sizeof(PerFrameGatherParams::CameraPhoto) <= sizeof(PerFrameGatherParams::MipPlane) * kMaxFramePlanes);
 constexpr int kPhotoStats = 6;  // sums per plane of kLensPhoto's statistics
 // a CTA takes tiles of 32 output columns x viewTileRows(k) rows; a thread owns one column of a tile and walks down
 // kViewRowsPerThread of its rows

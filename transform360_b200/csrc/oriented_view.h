@@ -919,18 +919,15 @@ T360_HD void cubeJacobian(const SphereGeometry& g, int f, const SphereVec& t, co
   *dv = fDiv(fMul(sv, fSub(fMul(db, m), fMul(b, dm))), m2);
 }
 
-// The Kannala-Brandt projection's Jacobian for the lens lensPosition picks, applied to rx and ry, in level-0 pixels.
-// With rho = |(X, Y)|, theta = atan2(rho, Z), s = theta_d / rho (lensHit), theta_d'(theta) = 1 + 3 k1 t + 5 k2 t^2 +
-// 7 k3 t^3 + 9 k4 t^4 (t = theta^2):
+// The Kannala-Brandt projection's Jacobian for lens L, applied to rx and ry, in level-0 pixels; Z = lensRow(L.m + 6, t),
+// which the callers have already computed.  With rho = |(X, Y)|, theta = atan2(rho, Z), s = theta_d / rho (lensHit),
+// theta_d'(theta) = 1 + 3 k1 t + 5 k2 t^2 + 7 k3 t^3 + 9 k4 t^4 (t = theta^2):
 //   drho = (X dX + Y dY) / rho,  dtheta = (Z drho - rho dZ) / (rho^2 + Z^2),  ds = (theta_d' dtheta - s drho) / rho,
 //   dx' = s dX + X ds,  dy' = s dY + Y ds,  a = (ax inW dx', ay inH dy').
 // At rho = 0 (theta = 0 for Z > 0) the limit is dx' = dX / Z, dy' = dY / Z; on the back axis (Z <= 0) it is infinite.
-T360_HD void lensJacobian(const LensRigModel& rig, const SphereVec& t, const SphereVec& rx, const SphereVec& ry, int inW, int inH,
+T360_HD void lensJacobian(const LensModel& L, float Z, const SphereVec& t, const SphereVec& rx, const SphereVec& ry, int inW, int inH,
                           float* a, float* b) {
-  const float z0 = lensRow(rig.lens[0].m + 6, t);
-  const float z1 = rig.numLenses > 1 ? lensRow(rig.lens[1].m + 6, t) : z0;
-  const LensModel& L = z1 > z0 ? rig.lens[1] : rig.lens[0];
-  const float X = lensRow(L.m, t), Y = lensRow(L.m + 3, t), Z = z1 > z0 ? z1 : z0;
+  const float X = lensRow(L.m, t), Y = lensRow(L.m + 3, t);
   const float cx = fMul(L.ax, static_cast<float>(inW)), cy = fMul(L.ay, static_cast<float>(inH));
   const float rho = fSqrt(fAdd(fMul(X, X), fMul(Y, Y)));
   const SphereVec* d[2] = {&rx, &ry};
@@ -957,6 +954,14 @@ T360_HD void lensJacobian(const LensRigModel& rig, const SphereVec& t, const Sph
     out[k][0] = fMul(cx, fAdd(fMul(s, dX), fMul(X, ds)));
     out[k][1] = fMul(cy, fAdd(fMul(s, dY), fMul(Y, ds)));
   }
+}
+
+// ... for the lens lensPosition picks (the closer lens; ties to lens 0)
+T360_HD void lensJacobian(const LensRigModel& rig, const SphereVec& t, const SphereVec& rx, const SphereVec& ry, int inW, int inH,
+                          float* a, float* b) {
+  const float z0 = lensRow(rig.lens[0].m + 6, t);
+  const float z1 = rig.numLenses > 1 ? lensRow(rig.lens[1].m + 6, t) : z0;
+  lensJacobian(z1 > z0 ? rig.lens[1] : rig.lens[0], z1 > z0 ? z1 : z0, t, rx, ry, inW, inH, a, b);
 }
 
 // lambda256 = ((int32) bits(rho^2) - 0x3f800000) >> 16 + bias256 (1/2 log2 rho^2 in 1/256 level, piecewise linear between
@@ -1041,6 +1046,85 @@ T360_HD int mipCameraSample(const SphereGeometry& g, const RectilinearCamera& c,
     rec1[1] = r0 * 1024 + fracY * 32 + fracX;
   }
   return level;
+}
+
+// ---- camera views of a lens rig with photometry (T360B200_cameraPhotoMaps, T360B200_transformFrameCameraPhotoAsync) ---
+// The camera view's ray (cameraXY, modelRay, rotateHD: the rig is mono), then lensPhotoPosition as the photometric lens
+// call applies it; with a pyramid each lens that covers the ray takes its own footprint from its own Kannala-Brandt
+// Jacobian (lensJacobian of that lens), level (mipLevelOf) and entries (mipScale), as mipCameraPoint takes them for the
+// closer lens.  So a belt pixel may gather up to four windows: two lenses x two levels.
+// One lens's part of a pixel (cameraPhotoPoint): cameraMipMaps's four values for that lens and its gain
+struct CameraPhotoLens {
+  float p0[2], p1[2];  // the entry in level `level`'s pixels and in level + 1's (NaN where w = 0 or the lens is not used)
+  int level, w;        // its level and the weight of the next (0, 0 where the lens is not used)
+  int gain;            // Gq (lensGain; 0 where the lens does not cover the ray)
+};
+// ... quantised (cameraPhotoSample): {col0, rowPhase} at `level` and, where w > 0, at level + 1
+struct CameraPhotoRecords {
+  int32_t rec0[2], rec1[2];
+  int level, w, gain;
+};
+
+// Both lenses' part of output pixel (i, j) of a camera view of a rig with photometry and the seam weight w (0..256) of
+// lens 1 (the return value; lensPhotoPosition's s, both and c).  A lens is used where lensPhotoPosition gives it an entry
+// (it covers the ray; with the hard seam and both = false the closer lens only).  MIP = false, or m.top = 0: no pyramid,
+// every used lens at level 0 with weight 0.  With the identity photometry and s = 0 the closer lens's entries are
+// cameraMipMaps' (cameraMap's without a pyramid) and its gain 4096.
+template <bool MIP>
+T360_HD int cameraPhotoPoint(const SphereGeometry& g, const RectilinearCamera& c, const LensRigModel& rig, const MipGeometry& m, int bias256,
+                             float s, bool both, const LensPhotoPlane& ph, int i, int j, CameraPhotoLens* lens, bool* overlap) {
+  float X, Y;
+  bool eye;
+  cameraXY(g, i, j, &X, &Y, &eye);
+  const SphereVec t = rotateHD(c.r, modelRay(c, X, Y));
+  float p[2][2];
+  const int w = lensPhotoPosition(rig, s, both, ph, t, g.inW, g.inH, p[0], p[1], &lens[0].gain, &lens[1].gain, overlap);
+  const bool used[2] = {p[0][0] == p[0][0], p[1][0] == p[1][0]};
+  const bool footprint = MIP && m.top > 0 && (used[0] || used[1]);
+  SphereVec rx{}, ry{};
+  if (footprint) {
+    rx = rayDifferential(c, fSub(X, m.halfX), Y, fAdd(X, m.halfX), Y);
+    ry = rayDifferential(c, X, fSub(Y, m.halfY), X, fAdd(Y, m.halfY));
+  }
+  const float nan = bitsFloat(0x7fc00000u);
+  for (int l = 0; l < 2; ++l) {
+    CameraPhotoLens& e = lens[l];
+    e.level = e.w = 0;
+    if (footprint && used[l]) {
+      float a[2], b[2];
+      lensJacobian(rig.lens[l], lensRow(rig.lens[l].m + 6, t), t, rx, ry, g.inW, g.inH, a, b);
+      e.level = mipLevelOf(fAdd(fMul(a[0], a[0]), fMul(a[1], a[1])), fAdd(fMul(b[0], b[0]), fMul(b[1], b[1])), m.top, bias256, &e.w);
+    }
+    e.p0[0] = e.level ? mipScale(p[l][0], m.sx[e.level]) : p[l][0];
+    e.p0[1] = e.level ? mipScale(p[l][1], m.sy[e.level]) : p[l][1];
+    e.p1[0] = e.w ? mipScale(p[l][0], m.sx[e.level + 1]) : nan;
+    e.p1[1] = e.w ? mipScale(p[l][1], m.sy[e.level + 1]) : nan;
+  }
+  return w;
+}
+
+// The sampling records of output pixel (i, j): cameraPhotoPoint's entries quantised as mipCameraSample quantises its
+// entries (rec1 only where w > 0).  Returns the seam weight w of lens 1.
+template <bool MIP>
+T360_HD int cameraPhotoSample(const SphereGeometry& g, const RectilinearCamera& c, const LensRigModel& rig, const MipGeometry& m, int bias256,
+                              float s, bool both, const LensPhotoPlane& ph, int i, int j, CameraPhotoRecords* lens, bool* overlap) {
+  CameraPhotoLens e[2];
+  const int w = cameraPhotoPoint<MIP>(g, c, rig, m, bias256, s, both, ph, i, j, e, overlap);
+  for (int l = 0; l < 2; ++l) {
+    int r0, fracX, fracY;
+    quantizeAxis(e[l].p0[0], g.kernelSize, &lens[l].rec0[0], &fracX);
+    quantizeAxis(e[l].p0[1], g.kernelSize, &r0, &fracY);
+    lens[l].rec0[1] = r0 * 1024 + fracY * 32 + fracX;
+    if (e[l].w) {
+      quantizeAxis(e[l].p1[0], g.kernelSize, &lens[l].rec1[0], &fracX);
+      quantizeAxis(e[l].p1[1], g.kernelSize, &r0, &fracY);
+      lens[l].rec1[1] = r0 * 1024 + fracY * 32 + fracX;
+    }
+    lens[l].level = e[l].level;
+    lens[l].w = e[l].w;
+    lens[l].gain = e[l].gain;
+  }
+  return w;
 }
 
 // Whether the per-frame orientation chain covers the layouts of `ctx`

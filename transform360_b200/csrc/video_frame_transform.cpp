@@ -552,12 +552,11 @@ bool lensRefused(const FrameTransformContext& ctx, const T360LensRig* rig, const
   return false;
 }
 
-// lensRefused, plus what the feathered seam needs: two lenses, and a belt width in [0.01, 180] degrees (the lower bound
-// keeps lensSeamScale finite)
-bool lensBlendRefused(const FrameTransformContext& ctx, const T360LensRig* rig, float seamWidth, const T360Orientation* o, std::string* why) {
-  if (lensRefused(ctx, rig, o, why)) return true;
-  if (rig->numLenses != 2) {
-    *why = formatted("numLenses %d: a feathered seam needs two lenses (one lens: T360B200_transformFrameLensAsync)", rig->numLenses);
+// What the feathered seam needs of a rig that is otherwise usable: two lenses, and a belt width in [0.01, 180] degrees (the
+// lower bound keeps lensSeamScale finite)
+bool featherRefused(const T360LensRig& rig, float seamWidth, std::string* why) {
+  if (rig.numLenses != 2) {
+    *why = formatted("numLenses %d: a feathered seam needs two lenses (one lens: T360B200_transformFrameLensAsync)", rig.numLenses);
     return true;
   }
   if (!(seamWidth >= 0.01f && seamWidth <= 180.0f)) {
@@ -565,6 +564,10 @@ bool lensBlendRefused(const FrameTransformContext& ctx, const T360LensRig* rig, 
     return true;
   }
   return false;
+}
+// lensRefused, plus featherRefused
+bool lensBlendRefused(const FrameTransformContext& ctx, const T360LensRig* rig, float seamWidth, const T360Orientation* o, std::string* why) {
+  return lensRefused(ctx, rig, o, why) || featherRefused(*rig, seamWidth, why);
 }
 
 // s = 1 / (2 seamWidth), seamWidth in radians: lens 1's weight rises from 0 to 1 while theta0 - theta1 goes from
@@ -600,16 +603,19 @@ t360::LensRigModel lensRigModel(const T360LensRig& rig) {
   return m;
 }
 
-// true, with the reason in *why, when the photometric lens call cannot serve ctx with this rig, photometry, seam and
-// orientation: the lens call's refusals (seamWidth = 0, the hard seam) or the blend call's (seamWidth > 0), and a
-// photometry that is NULL, out of range, or whose falloff reaches 0 inside a lens's coverage
-bool lensPhotoRefused(const FrameTransformContext& ctx, const T360LensRig* rig, const T360RigPhotometry* ph, float seamWidth,
-                      const T360Orientation* o, std::string* why) {
+// true, with the reason in *why, when seamWidth is neither 0 (the hard seam) nor a feathered seam's width (the photometric
+// calls' seam; featherRefused checks the rest of a feathered seam against the rig)
+bool seamWidthRefused(float seamWidth, std::string* why) {
   if (!std::isfinite(seamWidth) || seamWidth < 0.0f || (seamWidth > 0.0f && seamWidth < 0.01f)) {
     *why = formatted("seamWidth %g degrees is neither 0 (the hard seam) nor in [0.01, 180]", seamWidth);
     return true;
   }
-  if (seamWidth > 0.0f ? lensBlendRefused(ctx, rig, seamWidth, o, why) : lensRefused(ctx, rig, o, why)) return true;
+  return false;
+}
+
+// true, with the reason in *why, when a photometry cannot correct the lenses of a usable rig: NULL, out of range, or a
+// falloff that reaches 0 inside a lens's coverage
+bool photometryRefused(const T360LensRig& rig, const T360RigPhotometry* ph, std::string* why) {
   if (!ph) {
     *why = "a NULL photometry";
     return true;
@@ -618,7 +624,7 @@ bool lensPhotoRefused(const FrameTransformContext& ctx, const T360LensRig* rig, 
     *why = formatted("lumaPivot %d is outside 0..255", ph->lumaPivot);
     return true;
   }
-  for (int i = 0; i < rig->numLenses; ++i) {
+  for (int i = 0; i < rig.numLenses; ++i) {
     const T360LensPhotometry& L = ph->lens[i];
     for (int k = 0; k < 3; ++k)
       if (!std::isfinite(L.vignetting[k]) || !std::isfinite(L.gain[k]) || !std::isfinite(L.offset[k])) {
@@ -637,7 +643,7 @@ bool lensPhotoRefused(const FrameTransformContext& ctx, const T360LensRig* rig, 
     }
     // V(r) = 1 + v1 r^2 + v2 r^4 + v3 r^6 must stay positive for every r = theta_d the lens reaches: [0, theta_d(maxAngle)]
     // (theta_d increases on [0, maxAngle]: rigRefused), on a fine grid
-    const T360Lens& lens = rig->lens[i];
+    const T360Lens& lens = rig.lens[i];
     const double tMax = lens.maxAngle * M_PI / 180.0, t2 = tMax * tMax;
     const double rMax = tMax * (1.0 + t2 * (lens.k[0] + t2 * (lens.k[1] + t2 * (lens.k[2] + t2 * lens.k[3]))));
     constexpr int kSteps = 4096;
@@ -652,6 +658,16 @@ bool lensPhotoRefused(const FrameTransformContext& ctx, const T360LensRig* rig, 
     }
   }
   return false;
+}
+
+// true, with the reason in *why, when the photometric lens call cannot serve ctx with this rig, photometry, seam and
+// orientation: the lens call's refusals (seamWidth = 0, the hard seam) or the blend call's (seamWidth > 0), and
+// photometryRefused's
+bool lensPhotoRefused(const FrameTransformContext& ctx, const T360LensRig* rig, const T360RigPhotometry* ph, float seamWidth,
+                      const T360Orientation* o, std::string* why) {
+  if (seamWidthRefused(seamWidth, why)) return true;
+  if (seamWidth > 0.0f ? lensBlendRefused(ctx, rig, seamWidth, o, why) : lensRefused(ctx, rig, o, why)) return true;
+  return photometryRefused(*rig, ph, why);
 }
 
 // The per-frame constants of plane `plane` (0 luma, 1 and 2 chroma) of a rig's photometry (oriented_view.h: LensPhotoPlane);
@@ -790,6 +806,22 @@ bool cameraMipRefused(const FrameTransformContext& ctx, const T360LensRig* rig, 
 
 // round(256 lodBias), half away from zero: the bias in 1/256 of a level
 int mipBias(const T360Minify& m) { return static_cast<int>(std::lround(256.0 * static_cast<double>(m.lodBias))); }
+
+// ---- camera views of a lens rig with photometry (T360B200_cameraPhotoMaps, T360B200_transformFrameCameraPhotoAsync;
+// oriented_view.h: cameraPhotoSample) ------------------------------------------------------------------------------------
+// true, with the reason in *why, when the view cannot be rendered: a NULL rig (the photometry is per lens), the camera
+// view's refusals with a rig, the photometric lens call's seam and photometry checks, and minifyRefused where minify is
+// not NULL (NULL: no pyramid)
+bool cameraPhotoRefused(const FrameTransformContext& ctx, const T360LensRig* rig, const T360RigPhotometry* ph, float seamWidth, const T360Pose* pose,
+                        const T360Camera* camera, const T360Minify* minify, std::string* why) {
+  if (!rig) {
+    *why = "a NULL rig (the photometry corrects a rig's lenses)";
+    return true;
+  }
+  if (cameraRefused(ctx, rig, pose, camera, why) || seamWidthRefused(seamWidth, why)) return true;
+  if (seamWidth > 0.0f && featherRefused(*rig, seamWidth, why)) return true;
+  return photometryRefused(*rig, ph, why) || (minify && minifyRefused(minify, why));
+}
 
 }  // namespace
 
@@ -1446,6 +1478,54 @@ class VideoFrameTransform {
       UploadRing::Entry* staged = nullptr;
       buildPyramids(f, gp, slotFor(s), s, &staged);
       perFrameGather(t360::PerFrameSource::kCameraMip, gp, ctx, f, f.in, f.inPitch, nullptr, gp.lens, nullptr, nullptr, nullptr, s);
+      releaseAfter(staged, s);
+      return true;
+    });
+  }
+
+  // Whole frame of a camera view of a lens rig with photometry (T360B200_transformFrameCameraPhotoAsync): with a pyramid
+  // (minify not NULL and some plane's top level above 0) the planes' pyramids first (buildPyramids), then one gather launch
+  // for all planes, every record computed by cameraPhotoSample (oriented_view.h), so a rig, photometry, seam, pose, camera
+  // and minify give what cameraPhotoMaps describes.  With stats set (device, [numPlanes][6]) the overlap's sums are zeroed
+  // with a memset and accumulated by the same gather.  Needs no plan and leaves the plans alone; no tables.
+  bool transformFrameCameraPhoto(const char* what, const T360LensRig* rig, const T360RigPhotometry* photo, float seamWidth, const T360Pose* pose,
+                                 const T360Camera* camera, const T360Minify* minify, unsigned long long* stats, const FramePlanes& f,
+                                 cudaStream_t stream) {
+    auto refused = [&](const FrameTransformContext& ctx, std::string* why) {
+      if (cameraPhotoRefused(ctx, rig, photo, seamWidth, pose, camera, minify, why)) return true;
+      for (int p = 0; minify && minify->maxLevel > 0 && p < f.numPlanes; ++p)
+        if (f.inW[p] > 2 * 65535 || f.inH[p] > 2 * 65535) {  // (CameraPhotoLevel keeps a level's sides in 16 bits)
+          *why = formatted("input plane %d is %dx%d: a pyramid needs sides of at most 131070", p, f.inW[p], f.inH[p]);
+          return true;
+        }
+      return false;
+    };
+    return unplannedFrame(what, stream, refused, [&](const FrameTransformContext& ctx, int, cudaStream_t s) {
+      t360::PerFrameGatherParams gp{}, pyramids{};  // (pyramids: buildPyramids' levels, copied into gp.cameraPhoto)
+      t360::PerFrameGatherParams::CameraPhoto& cp = gp.cameraPhoto;
+      int topMax = 0;
+      for (int p = 0; p < f.numPlanes; ++p) {
+        gp.plane[p].geometry = rectilinearGeometry(ctx, true, f.inW[p], f.inH[p], f.outW[p], f.outH[p]);
+        cp.mip[p].geometry = pyramids.mip[p].geometry = t360::mipGeometry(gp.plane[p].geometry, minify ? minify->maxLevel : 0);
+        topMax = std::max(topMax, cp.mip[p].geometry.top);
+        cp.photo.plane[p] = lensPhotoPlane(*photo, rig->numLenses, p);
+      }
+      gp.camera = cameraConstants(*pose, *camera);
+      gp.rig = lensRigModel(*rig);
+      if (seamWidth > 0.0f) gp.seamScale = lensSeamScale(seamWidth);
+      if (minify) gp.mipBias = mipBias(*minify);
+      cp.photo.stats = stats;
+      if (stats) CU(cudaMemsetAsync(stats, 0, sizeof(unsigned long long) * t360::kPhotoStats * f.numPlanes, s));
+      UploadRing::Entry* staged = nullptr;
+      if (topMax > 0) {
+        buildPyramids(f, pyramids, slotFor(s), s, &staged);
+        for (int p = 0; p < f.numPlanes; ++p)
+          for (int l = 1; l <= cp.mip[p].geometry.top; ++l) {
+            const t360::PerFrameGatherParams::MipLevel& L = pyramids.mip[p].level[l - 1];
+            cp.mip[p].level[l - 1] = {L.bytes, L.pitch, static_cast<uint16_t>(L.w), static_cast<uint16_t>(L.h)};
+          }
+      }
+      perFrameGather(t360::PerFrameSource::kCameraPhoto, gp, ctx, f, f.in, f.inPitch, nullptr, /*transparent=*/true, nullptr, nullptr, nullptr, s);
       releaseAfter(staged, s);
       return true;
     });
@@ -3106,6 +3186,59 @@ T360_API int T360B200_transformFrameCameraMipAsync(VideoFrameTransform* t, const
   FramePlanes f;
   if (!describeFrame(what, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, f)) return 0;
   return t->transformFrameCameraMip(what, rig, pose, camera, minify, f, static_cast<cudaStream_t>(stream));
+}
+T360_API int T360B200_cameraPhotoMaps(const FrameTransformContext* ctx, const T360LensRig* rig, const T360RigPhotometry* photometry, float seamWidth,
+                                      const T360Pose* pose, const T360Camera* camera, const T360Minify* minify, int lens, int plane, int inW,
+                                      int inH, int outW, int outH, float* map0, float* map1, uint8_t* level, uint16_t* weight, uint16_t* gain,
+                                      uint16_t* seamWeight) {
+  const char* what = "Could not compute the camera photometry maps";
+  std::string why;
+  if (!ctx) why = "a NULL context";
+  else if (cameraPhotoRefused(*ctx, rig, photometry, seamWidth, pose, camera, minify, &why)) {}
+  else if (lens < 0 || lens > 1) why = formatted("lens %d is outside 0..1", lens);
+  else if (plane < 0 || plane > 2) why = formatted("plane %d is outside 0..2", plane);
+  else if (!map0 || !map1 || !level || !weight || !gain || !seamWeight || inW <= 0 || inH <= 0 || outW <= 0 || outH <= 0)
+    why = "a NULL map, level, weight or gain array or a plane size that is not positive";
+  if (!why.empty()) {
+    std::printf("%s. Error: %s\n", what, why.c_str());
+    return 0;
+  }
+  const t360::SphereGeometry g = rectilinearGeometry(*ctx, true, inW, inH, outW, outH);
+  const t360::RectilinearCamera c = cameraConstants(*pose, *camera);
+  const t360::LensRigModel model = lensRigModel(*rig);
+  const t360::MipGeometry m = t360::mipGeometry(g, minify ? minify->maxLevel : 0);
+  const int bias = minify ? mipBias(*minify) : 0;
+  const t360::LensPhotoPlane ph = lensPhotoPlane(*photometry, rig->numLenses, plane);
+  const float s = seamWidth > 0.0f ? lensSeamScale(seamWidth) : 0.0f;
+  for (int i = 0; i < outH; ++i)
+    for (int j = 0; j < outW; ++j) {
+      const size_t at = static_cast<size_t>(i) * outW + j;
+      t360::CameraPhotoLens e[2];
+      bool overlap;
+      seamWeight[at] = static_cast<uint16_t>(t360::cameraPhotoPoint<true>(g, c, model, m, bias, s, /*both=*/true, ph, i, j, e, &overlap));
+      map0[2 * at] = e[lens].p0[0];
+      map0[2 * at + 1] = e[lens].p0[1];
+      map1[2 * at] = e[lens].p1[0];
+      map1[2 * at + 1] = e[lens].p1[1];
+      level[at] = static_cast<uint8_t>(e[lens].level);
+      weight[at] = static_cast<uint16_t>(e[lens].w);
+      gain[at] = static_cast<uint16_t>(e[lens].gain);
+    }
+  return 1;
+}
+T360_API int T360B200_transformFrameCameraPhotoAsync(VideoFrameTransform* t, const T360LensRig* rig, const T360RigPhotometry* photometry,
+                                                     float seamWidth, const T360Pose* pose, const T360Camera* camera, const T360Minify* minify,
+                                                     unsigned long long* deviceStats, int numPlanes, const uint8_t* const* dIn,
+                                                     uint8_t* const* dOut, const int* inW, const int* inH, const int* inPitch, const int* outW,
+                                                     const int* outH, const int* outPitch, void* stream) {
+  const char* what = "Could not transform the frame with a camera view of a lens rig with photometry";
+  if (!t) {
+    std::printf("%s. Error: a NULL argument\n", what);
+    return 0;
+  }
+  FramePlanes f;
+  if (!describeFrame(what, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, f)) return 0;
+  return t->transformFrameCameraPhoto(what, rig, photometry, seamWidth, pose, camera, minify, deviceStats, f, static_cast<cudaStream_t>(stream));
 }
 T360_API void T360B200_setPinHostPlanes(VideoFrameTransform* t, int enable) { if (t) t->setPinHostPlanes(enable != 0); }
 T360_API void T360B200_debugTrace(VideoFrameTransform* t, int enable) { if (t) t->enableTrace(enable != 0); }

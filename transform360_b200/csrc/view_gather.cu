@@ -22,8 +22,11 @@
 //   - an anti-aliased camera view (MipCameraPositions): the same chain, the pixel's footprint from ray differentials, and
 //     two records at adjacent levels of the plane's input pyramid, blended by the footprint's weight (mipCameraSample);
 //   - a lens rig with photometry (LensPhotoPositions): both lenses' records and gains (lensPhotoSample); the tile loop
-//     corrects each sample, combines them by the seam and accumulates the overlap's statistics.
-// In all eight, the records come from the same host/device functions the planner (or its host twin) uses: bit-identical.
+//     corrects each sample, combines them by the seam and accumulates the overlap's statistics;
+//   - a camera view of a lens rig with photometry (CameraPhotoPositions): the camera view's ray, then both lenses' records,
+//     levels and gains (cameraPhotoSample); each lens's sample is the blend of its two levels, then the tile loop goes on
+//     as for LensPhotoPositions.
+// In all nine, the records come from the same host/device functions the planner (or its host twin) uses: bit-identical.
 #include "gather_common.cuh"
 
 #include <algorithm>
@@ -57,6 +60,28 @@ __device__ __forceinline__ SrcView mipView(const PerFrameGatherParams::MipLevel&
   s.w = l.w; s.h = l.h; s.pitch = l.pitch;
   return s;
 }
+__device__ __forceinline__ SrcView mipView(const PerFrameGatherParams::CameraPhotoLevel& l) {  // (kCameraPhoto)
+  SrcView s;
+  s.bytes = l.bytes;
+  s.misalign = (int)(reinterpret_cast<uintptr_t>(l.bytes) & 3);
+  s.words = reinterpret_cast<const uint32_t*>(l.bytes - s.misalign);
+  s.w = l.w; s.h = l.h; s.pitch = l.pitch;
+  return s;
+}
+// A pixel at pyramid level `level` of a plane (0: the plane's src s; levels[l - 1]: level l) and, where w > 0, at level +
+// 1, blended by w (0..255); where BORDER_TRANSPARENT skips one of the two the other stands alone, -1 where it skips both.
+// (kCameraPhoto's per-lens blend.  kCameraMip's branch writes the same blend inline: through this helper its kernels
+// compile to other register assignments, and they are kept as they were.)
+template <int K, bool TRANSPARENT, class Level>
+__device__ __forceinline__ int levelPixel(const Level* levels, const SrcView& s, const unsigned char* smem, int level, const int32_t* rec0,
+                                          const int32_t* rec1, int w) {
+  int value = viewPixel<K, TRANSPARENT>(level ? mipView(levels[level - 1]) : s, smem, rec0[0], rec0[1]);
+  if (w > 0) {
+    const int b = viewPixel<K, TRANSPARENT>(mipView(levels[level]), smem, rec1[0], rec1[1]);
+    value = value < 0 ? b : (b < 0 ? value : (value * (256 - w) + b * w + 128) >> 8);
+  }
+  return value;
+}
 template <class Pos, class = void>
 struct IsMip : std::false_type {};
 template <class Pos>
@@ -73,8 +98,9 @@ struct IsPhoto<Pos, std::enable_if_t<Pos::kPhoto>> : std::true_type {};
 // Positions::kBlend: its record() hands over two records and the weight w (0..256) of the second; the first is gathered
 // for every pixel, the second only where 0 < w < 256, and the two values are blended (PerFrameSource::kLensBlend).  Where
 // BORDER_TRANSPARENT skips one of the two, the other stands alone.
-// Positions::kPhoto (IsPhoto, kLensPhoto): record() hands over both lenses' records, their gains and w.  Lens 0 is
-// gathered where w < 256, lens 1 where w > 0, and, with statistics, both wherever both cover the pixel; each sample is
+// Positions::kPhoto (IsPhoto, kLensPhoto and kCameraPhoto): record() hands over both lenses' records, their gains and w,
+// and the policy's pixel() gathers a lens's sample from them (photo() names the launch's photometric constants).  Lens 0
+// is gathered where w < 256, lens 1 where w > 0, and, with statistics, both wherever both cover the pixel; each sample is
 // corrected (photoCorrect) before w combines them.  A thread sums its overlap pixels' six values over its rows of the tile,
 // its warp reduces them (__reduce_add_sync over the warp's live columns), and one lane adds them to the plane's sums with
 // one 64-bit atomic each.  Whether statistics are taken and which seam is used are launch-uniform branches.
@@ -110,15 +136,15 @@ __device__ __forceinline__ void gatherViewTiles(const PerFrameGatherParams& p, i
         int g0, g1;
         bool overlap;
         const int w = pos.record(p, v, pl, i, j, rec0, rec1, &g0, &g1, &overlap);
-        const LensPhotoPlane& c = p.photo.plane[pl];
-        const bool stats = p.photo.stats && overlap;
+        const LensPhotoPlane& c = Positions::photo(p).plane[pl];
+        const bool stats = Positions::photo(p).stats && overlap;
         int a = -1, b = -1;
         if (w < 256 || stats) {
-          a = viewPixel<K, TRANSPARENT>(s, smem, rec0[0], rec0[1]);
+          a = pos.template pixel<K, TRANSPARENT>(p, pl, s, smem, 0, rec0);
           if (a >= 0) a = photoCorrect(a, g0, c.offset[0], c.pivot);
         }
         if (w > 0 || stats) {
-          b = viewPixel<K, TRANSPARENT>(s, smem, rec1[0], rec1[1]);
+          b = pos.template pixel<K, TRANSPARENT>(p, pl, s, smem, 1, rec1);
           if (b >= 0) b = photoCorrect(b, g1, c.offset[1], c.pivot);
         }
         if (stats && a >= 0 && b >= 0) {
@@ -160,11 +186,11 @@ __device__ __forceinline__ void gatherViewTiles(const PerFrameGatherParams& p, i
       v.dst[(size_t)i * v.dstPitch + j] = (uint8_t)value;
     }
     if constexpr (IsPhoto<Positions>::value) {
-      if (p.photo.stats) {  // (every lane of the warp's live columns gets here: a row bound breaks the whole warp)
+      if (Positions::photo(p).stats) {  // (every lane of the warp's live columns gets here: a row bound breaks the whole warp)
         const int live = v.geometry.mapW - x0;
         const unsigned mask = live >= 32 ? 0xffffffffu : (1u << live) - 1u;
         if (__reduce_add_sync(mask, sums[0])) {
-          unsigned long long* out = p.photo.stats + pl * kPhotoStats;
+          unsigned long long* out = Positions::photo(p).stats + pl * kPhotoStats;
 #pragma unroll
           for (int k = 0; k < kPhotoStats; ++k) {
             const unsigned total = __reduce_add_sync(mask, sums[k]);
@@ -324,6 +350,39 @@ struct LensPhotoPositions : NoTables {
     return lensPhotoSample<BARREL>(v.geometry, p.rotation, p.rig, p.seamScale, p.photo.stats != nullptr, p.photo.plane[pl], v.colTable,
                                    v.rowTable, i, j, rec0, rec1, g0, g1, overlap);
   }
+  __device__ static const PerFrameGatherParams::LensPhoto& photo(const PerFrameGatherParams& p) { return p.photo; }
+  template <int K, bool TRANSPARENT>
+  __device__ int pixel(const PerFrameGatherParams&, int, const SrcView& s, const unsigned char* smem, int, const int32_t* rec) const {
+    return viewPixel<K, TRANSPARENT>(s, smem, rec[0], rec[1]);
+  }
+};
+
+// A camera view of a lens rig with photometry (kCameraPhoto): the camera view's ray, then both lenses' records, levels and
+// gains, the overlap and w per pixel (cameraPhotoSample).  record() keeps each lens's records, level and level weight in
+// the policy, and pixel() gathers lens l's sample from them: the blend of its two levels (levelPixel).  MIP = false: no
+// pyramid, level 0 alone (a launch whose planes all have top level 0).  Every model in one loop; always
+// BORDER_TRANSPARENT.  With the hard seam and no statistics only the closer lens is projected.
+template <int, bool MIP>
+struct CameraPhotoPositions : NoTables {
+  static constexpr bool kPhoto = true, kTransparent = true;
+  CameraPhotoRecords lens[2];
+  using NoTables::NoTables;
+  __device__ int record(const PerFrameGatherParams& p, const PerFramePlane& v, int pl, int i, int j, int32_t*, int32_t*, int* g0, int* g1,
+                        bool* overlap) {
+    const PerFrameGatherParams::LensPhoto& photo = p.cameraPhoto.photo;
+    const int w = cameraPhotoSample<MIP>(v.geometry, p.camera, p.rig, p.cameraPhoto.mip[pl].geometry, p.mipBias, p.seamScale,
+                                         photo.stats != nullptr, photo.plane[pl], i, j, lens, overlap);
+    *g0 = lens[0].gain;
+    *g1 = lens[1].gain;
+    return w;
+  }
+  __device__ static const PerFrameGatherParams::LensPhoto& photo(const PerFrameGatherParams& p) { return p.cameraPhoto.photo; }
+  template <int K, bool TRANSPARENT>
+  __device__ int pixel(const PerFrameGatherParams& p, int pl, const SrcView& s, const unsigned char* smem, int l, const int32_t*) const {
+    const CameraPhotoRecords& r = lens[l];
+    if constexpr (MIP) return levelPixel<K, TRANSPARENT>(p.cameraPhoto.mip[pl].level, s, smem, r.level, r.rec0, r.rec1, r.w);
+    else return viewPixel<K, TRANSPARENT>(s, smem, r.rec0[0], r.rec0[1]);
+  }
 };
 
 template <class Pos, class = void>
@@ -409,6 +468,11 @@ cudaError_t launchPerFrameGather(PerFrameGatherParams p, PerFrameSource source, 
     case PerFrameSource::kRectilinear: return launchPositions<RectilinearPositions>(p, p.lens, numTiles, numSMs, stream);
     case PerFrameSource::kCameraMip: return launchPositions<MipCameraPositions>(p, p.lens, numTiles, numSMs, stream);
     case PerFrameSource::kLensPhoto: return launchPositions<LensPhotoPositions>(p, barrel, numTiles, numSMs, stream);
+    case PerFrameSource::kCameraPhoto: {
+      bool mip = false;  // (a level table only where some plane has a pyramid)
+      for (int i = 0; i < p.numPlanes; ++i) mip = mip || p.cameraPhoto.mip[i].geometry.top > 0;
+      return launchPositions<CameraPhotoPositions>(p, mip, numTiles, numSMs, stream);
+    }
   }
   return cudaErrorInvalidValue;
 }

@@ -301,6 +301,12 @@ def load(path: os.PathLike | None = None):
     L.T360B200_transformFrameCameraMipAsync.restype = ci
     L.T360B200_transformFrameCameraMipAsync.argtypes = [vp, C.POINTER(T360LensRig), C.POINTER(T360Pose), C.POINTER(T360Camera),
                                                         C.POINTER(T360Minify), ci] + planes
+    L.T360B200_cameraPhotoMaps.restype = ci
+    L.T360B200_cameraPhotoMaps.argtypes = [C.POINTER(FrameTransformContext), C.POINTER(T360LensRig), C.POINTER(T360RigPhotometry), C.c_float,
+                                           C.POINTER(T360Pose), C.POINTER(T360Camera), C.POINTER(T360Minify)] + [ci] * 6 + [vp] * 6
+    L.T360B200_transformFrameCameraPhotoAsync.restype = ci
+    L.T360B200_transformFrameCameraPhotoAsync.argtypes = [vp, C.POINTER(T360LensRig), C.POINTER(T360RigPhotometry), C.c_float,
+                                                          C.POINTER(T360Pose), C.POINTER(T360Camera), C.POINTER(T360Minify), vp, ci] + planes
     L.T360B200_setPinHostPlanes.restype = None
     L.T360B200_setPinHostPlanes.argtypes = [vp, ci]
     L.T360B200_debugTrace.restype = None
@@ -336,7 +342,7 @@ EXPORTED_SYMBOLS = [
     "T360B200_lensMap", "T360B200_transformFrameLensAsync", "T360B200_lensBlendMaps", "T360B200_transformFrameLensBlendAsync",
     "T360B200_lensPhotoMaps", "T360B200_transformFrameLensPhotoAsync",
     "T360B200_rectilinearMap", "T360B200_transformFrameRectilinearAsync", "T360B200_cameraMap", "T360B200_transformFrameCameraAsync",
-    "T360B200_cameraMipMaps", "T360B200_transformFrameCameraMipAsync",
+    "T360B200_cameraMipMaps", "T360B200_transformFrameCameraMipAsync", "T360B200_cameraPhotoMaps", "T360B200_transformFrameCameraPhotoAsync",
     "T360B200_setPinHostPlanes", "T360B200_debugTrace", "T360B200_debugTraceRead", "T360B200_synchronize", "T360B200_stream", "T360B200_kernelLaunchCount", "T360B200_planDeviceBytes",
     "T360B200_planTileCounts", "T360B200_deviceCount", "T360B200_version",
 ]
@@ -481,6 +487,16 @@ class VideoFrameTransform:
         return lambda pose, camera, minify, stream=0, rig=None: enqueue(
             (C.byref(rig) if rig is not None else None, C.byref(as_pose(pose)), C.byref(as_camera(camera)),
              C.byref(as_minify(minify)), n), stream)
+
+    def make_camera_photo_frame_call(self, in_planes, out_planes, dims):
+        """Like make_camera_mip_frame_call, for T360B200_transformFrameCameraPhotoAsync (a camera view of a rig with
+        photometry: each lens's samples corrected before the hard or feathered seam): returns a callable f(rig, photometry,
+        seam_width, pose, camera, minify=None, stream=0, stats=0) -> bool, `minify` as for make_camera_mip_frame_call or None
+        (no pyramid) and `stats` the device address of [planes][6] uint64 sums (0: none)."""
+        n, enqueue = self._frame_call("T360B200_transformFrameCameraPhotoAsync", in_planes, out_planes, dims)
+        return lambda rig, photometry, seam_width, pose, camera, minify=None, stream=0, stats=0: enqueue(
+            (C.byref(rig), C.byref(photometry), seam_width, C.byref(as_pose(pose)), C.byref(as_camera(camera)),
+             C.byref(as_minify(minify)) if minify is not None else None, stats or None, n), stream)
 
     def generate_map_from_warp(self, map, in_w: int, in_h: int, plan_index: int, border: int = BORDER_WRAP) -> bool:
         """T360B200_generateMapFromWarp: installs plan index `plan_index` from a caller's warp map (float32 [h][w][2], the
@@ -779,6 +795,25 @@ def camera_mip_maps(ctx: FrameTransformContext, pose, camera, minify, in_w, in_h
                                          map0.ctypes.data, map1.ctypes.data, level.ctypes.data, weight.ctypes.data):
         raise ValueError("T360B200_cameraMipMaps refused the arguments (message on stdout)")
     return map0, map1, level, weight
+
+
+def camera_photo_maps(ctx: FrameTransformContext, rig: T360LensRig, photometry: T360RigPhotometry, seam_width, pose, camera, minify, lens,
+                      plane, in_w, in_h, out_w, out_h) -> tuple[np.ndarray, np.ndarray, np.ndarray, np.ndarray, np.ndarray, np.ndarray]:
+    """The host twin of one lens (0 or 1) of one plane (0 luma, 1 and 2 chroma) of a camera view of a rig with photometry
+    (T360B200_cameraPhotoMaps, no CUDA): (map0, map1, level, weight, gain, seam_weight).  The first four are
+    camera_mip_maps' arrays for that lens (NaN entries, level 0 and weight 0 where it does not cover the pixel's ray); gain:
+    uint16, the lens's Gq (4096 = 1, 0 where it does not cover the ray); seam_weight: uint16, w of lens 1 (0 or 256 with
+    seam_width 0, the hard seam).  minify as for camera_mip_maps, or None: no pyramid."""
+    shape = (max(out_h, 0), max(out_w, 0))
+    map0, map1 = np.zeros(shape + (2,), np.float32), np.zeros(shape + (2,), np.float32)
+    level = np.zeros(shape, np.uint8)
+    weight, gain, seam_weight = (np.zeros(shape, np.uint16) for _ in range(3))
+    if not load().T360B200_cameraPhotoMaps(C.byref(ctx), C.byref(rig), C.byref(photometry), seam_width, C.byref(as_pose(pose)),
+                                           C.byref(as_camera(camera)), C.byref(as_minify(minify)) if minify is not None else None, lens,
+                                           plane, in_w, in_h, out_w, out_h, map0.ctypes.data, map1.ctypes.data, level.ctypes.data,
+                                           weight.ctypes.data, gain.ctypes.data, seam_weight.ctypes.data):
+        raise ValueError("T360B200_cameraPhotoMaps refused the arguments (message on stdout)")
+    return map0, map1, level, weight, gain, seam_weight
 
 
 def square_pixel_vfov(hfov, width, height) -> float:
