@@ -469,7 +469,12 @@ int T360B200_transformFrameRectilinearAsync(VideoFrameTransform* transform, cons
  *                  c = cos lon (Sharpless et al.'s inverse; computed as k = (u / (d + 1))^2, c = (-k d + sqrt(1 + k (1 -
  *                  d^2))) / (k + 1)).  Vertical lines stay vertical and radial lines through the centre straight; d = 0
  *                  is the pinhole up to rounding, vfov is the field of the centre column.  hfov in (0, 359] with
- *                  d + cos(hfov / 2) > 0, vfov in (0, 179].
+ *                  d + cos(hfov / 2) > 0, vfov in (0, 179];
+ *   EQUIRECT       ax = hfov pi / 360, ay = vfov pi / 360; lon = X ax, lat = Y ay, q = (cos lat sin lon, sin lat,
+ *                  cos lat cos lon), with sin a = a S(a) and cos a = C(a) of the EQUIDISTANT row (S and C are even, and
+ *                  |lon| <= pi): a latitude / longitude window.  With hfov = vfov = 180 it is a VR180 eye's half-equirect;
+ *                  with hfov = 360, vfov = 180 and a zero pose the full equirect.  hfov in (0, 360], vfov in (0, 180].
+ * Model 4 is not assigned and is refused (EQUIRECT was added after it had been pinned as refused).
  * Every model gives every pixel a ray, so a view of the context's input has no NaN in its map.
  *
  * Refused, with 0 and a message on stdout before any CUDA call: the refusals of the rectilinear views with the field
@@ -479,6 +484,7 @@ int T360B200_transformFrameRectilinearAsync(VideoFrameTransform* transform, cons
 #define T360_CAMERA_EQUIDISTANT 1
 #define T360_CAMERA_STEREOGRAPHIC 2
 #define T360_CAMERA_PANNINI 3
+#define T360_CAMERA_EQUIRECT 5
 typedef struct T360Camera {
   int model;     /* T360_CAMERA_* */
   float pannini; /* d, read by T360_CAMERA_PANNINI only */
@@ -623,6 +629,56 @@ int T360B200_transformFrameCameraPhotoAsync(VideoFrameTransform* transform, cons
                                             int numPlanes, const uint8_t* const* deviceInputs, uint8_t* const* deviceOutputs,
                                             const int* inputWidths, const int* inputHeights, const int* inputPitches,
                                             const int* outputWidths, const int* outputHeights, const int* outputPitches, void* cudaStream);
+/* ---- camera views of a stereo rig ---------------------------------------------------------------------------------
+ * A stereo fisheye rig (a VR180 camera, a dual-fisheye cinema lens, a pair of action cameras) has two lenses that both
+ * look forward, lens 0 the left eye and lens 1 the right eye, their circles anywhere in the frame (cx, cy: some cameras put
+ * the left eye's circle on the right).  This call renders one view per eye with the camera views' pose and models and the
+ * photometry and pyramid of T360B200_transformFrameCameraPhotoAsync.  With the EQUIRECT model at 180 x 180 and an LR
+ * output, each eye is a VR180 half-equirect.  Per output pixel of each plane:
+ *   1. eye split: the context's output_stereo_format, whatever input_stereo_format says: LR side by side (x folded), TB
+ *      stacked (y folded, the lower eye's y flipped with vflip), MONO eye 0 alone.  The footprint's dX and dY are one column and
+ *      row of one eye, as in the anti-aliased views;
+ *   2. ray: steps 1-5 of the camera views; the same pose for both eyes (each lens's own extrinsics carry the stereo
+ *      rectification);
+ *   3. lens: eye e takes lens e and only lens e.  Where lens e does not cover the ray, or its samples are skipped
+ *      (BORDER_TRANSPARENT), the pixel keeps its bytes (the pre-fill: chroma 128, luma the caller's); it never falls back to
+ *      the other eye's lens, which would show the wrong parallax;
+ *   4. pyramid, photometry, statistics: steps 3-5 of T360B200_transformFrameCameraPhotoAsync with lens e's footprint, its
+ *      two levels and its Gq and Oq; s' of lens e is the pixel.  With deviceStats each pixel also gathers the other lens
+ *      for the statistics only, so the sums run over the output pixels of both eyes whose ray both lenses cover where
+ *      neither sample is skipped: they measure the exposure and colour mismatch between the eyes over their common field
+ *      (near objects add parallax noise to them: a scene point closer than a few metres lies at other pixels in the two
+ *      eyes).
+ * With MONO output and no statistics the frame is T360B200_transformFrameCameraPhotoAsync's with the one-lens rig {lens
+ * 0} and seamWidth 0, byte for byte, with and without a pyramid.  With the identity photometry and no pyramid, the twin's
+ * two map0 arrays combined by eye (lens 1's where eyeWeight is 256) and planned with T360B200_generateMapFromWarp(...,
+ * T360_BORDER_TRANSPARENT) give the frame through T360B200_transformFrameAsync for a fixed pose.  A frame takes one launch,
+ * or T_max + 1 with a pyramid, plus the memset with statistics.
+ *
+ * Refused, with 0 and a message on stdout before any CUDA call: a NULL rig or numLenses other than 2; an
+ * output_stereo_format other than TB, LR or MONO; every refusal of T360B200_transformFrameCameraPhotoAsync except the seam's;
+ * and (frame call only) with maxLevel > 0 an input plane side above 131070. */
+/* Host only, no CUDA: the twin of plane `plane` (0..2) of inputWidth x inputHeight, one lens (0 or 1) per call.  map0,
+ * map1, level, weight, gain: T360B200_cameraPhotoMaps' arrays for that lens (NaN entries, level 0, weight 0 and gain 0
+ * where it does not cover the ray), given wherever it covers the ray, in both eyes.  eyeWeight (uint16): 0 on eye-0
+ * pixels, 256 on eye-1 pixels.  So the oracle composite of T360B200_cameraPhotoMaps, with eyeWeight as the seam weight,
+ * gives the frame bit for bit, and its statistics the frame's.  Returns 1; 0 (message) for the refusals above, a lens
+ * outside 0..1, a plane outside 0..2, a NULL context or array, or non-positive sizes. */
+int T360B200_stereoCameraMaps(const FrameTransformContext* ctx, const T360LensRig* rig, const T360RigPhotometry* photometry, const T360Pose* pose,
+                              const T360Camera* camera, const T360Minify* minify /* NULL: no pyramid */, int lens, int plane, int inputWidth,
+                              int inputHeight, int outputWidth, int outputHeight, float* map0, float* map1, uint8_t* level, uint16_t* weight,
+                              uint16_t* gain, uint16_t* eyeWeight);
+/* One frame of a camera view of a stereo rig, every plane in one gather launch after the pyramid's: the arguments and
+ * asynchronous contract of T360B200_transformFrameCameraPhotoAsync without seamWidth; every argument may change every
+ * frame.  Needs no plan and does not touch the plans; takes the reader lock; never synchronises the device.  Returns 1 if
+ * everything was enqueued; 0 with a message on stdout, before any CUDA call, for the refusals above, 0 or more than 3
+ * planes, or an invalid plane description. */
+int T360B200_transformFrameStereoCameraAsync(VideoFrameTransform* transform, const T360LensRig* rig, const T360RigPhotometry* photometry,
+                                             const T360Pose* pose, const T360Camera* camera, const T360Minify* minify /* NULL: no pyramid */,
+                                             unsigned long long* deviceStats /* NULL: none */, int numPlanes, const uint8_t* const* deviceInputs,
+                                             uint8_t* const* deviceOutputs, const int* inputWidths, const int* inputHeights,
+                                             const int* inputPitches, const int* outputWidths, const int* outputHeights,
+                                             const int* outputPitches, void* cudaStream);
 /* Opt-in (also: environment T360B200_PIN_HOST_PLANES=1): page-lock pageable caller planes in place the second time
  * the same buffer is seen (cudaHostRegister), so that recycled frame-pool buffers are DMA'd at full PCIe speed.  The
  * caller must keep such buffers alive until VideoFrameTransform_delete. */

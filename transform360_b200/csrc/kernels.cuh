@@ -401,7 +401,9 @@ void countKernelLaunches(long long n);  // kernels launched through a replayed C
 //   kCameraPhoto  a camera view of a lens rig with photometry (camera, rig, seamScale, cameraPhoto: the planes' pyramids
 //                 and the photometric constants, mipBias; cameraPhotoSample): each lens's sample is the blend of its own two levels (kCameraMip's
 //                 blend; level 0 alone without a pyramid), then corrected, combined and counted as kLensPhoto's.
-enum class PerFrameSource { kView, kSphere, kMap, kLens, kLensBlend, kRectilinear, kCameraMip, kLensPhoto, kCameraPhoto };
+//   kStereoCamera a camera view of a stereo rig (kCameraPhoto's constants, no seam; cameraPhotoSample<MIP, true>): the
+//                 output eye split of the context's output_stereo_format, and eye e's pixels take lens e alone.
+enum class PerFrameSource { kView, kSphere, kMap, kLens, kLensBlend, kRectilinear, kCameraMip, kLensPhoto, kCameraPhoto, kStereoCamera };
 struct PerFramePlane {
   const uint8_t* src;  // (blurred) input plane, geometry.inW x geometry.inH
   uint8_t* dst;        // render target, geometry.mapW x geometry.mapH

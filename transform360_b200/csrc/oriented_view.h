@@ -576,12 +576,14 @@ T360_HD int photoCorrect(int s, int gq, int oq, int pivot) {
 // (lensBlendPosition).  p0 / p1: lens 0's / lens 1's source position wherever that lens covers d (NaN elsewhere), g0 / g1
 // its Gq (lensGain; 0 where it does not cover d); *overlap: both lenses cover d.  both = false with the hard seam computes
 // the closer lens only (the other's position NaN, its gain 0, no overlap): all the frame needs when no statistics are taken.
+// STEREO (a stereo rig, s = 0): output eye `eye` picks the lens instead of the closer axis; lens e is eye e's.
+template <bool STEREO = false>
 T360_HD int lensPhotoPosition(const LensRigModel& rig, float s, bool both, const LensPhotoPlane& c, const SphereVec& d, int inW, int inH,
-                              float* p0, float* p1, int* g0, int* g1, bool* overlap) {
+                              float* p0, float* p1, int* g0, int* g1, bool* overlap, bool eye = false) {
   const float nan = bitsFloat(0x7fc00000u);
   const float z0 = lensRow(rig.lens[0].m + 6, d);
   const float z1 = rig.numLenses > 1 ? lensRow(rig.lens[1].m + 6, d) : z0;
-  const bool second = z1 > z0;
+  const bool second = STEREO ? eye : z1 > z0;
   if (s == 0.0f && !both) {  // the closer lens alone, as lensPosition projects it
     const int l = second ? 1 : 0;
     const LensHitR h = lensHit<true>(rig.lens[l], d, second ? z1 : z0, inW, inH);
@@ -661,11 +663,14 @@ T360_HD int lensPhotoSample(const SphereGeometry& g, const Rotation& r, const Le
 //   kCameraPannini        u = X cx, w = Y cy (cx = (d + 1) sin h / (d + cos h), h = hfov / 2, cy = tan(vfov / 2)),
 //                         k = (u e)^2, c = (-k d + sqrt(1 + k dd)) / (k + 1) (e = 1 / (d + 1), dd = 1 - d^2: Sharpless et
 //                         al.'s inverse with its discriminant k^2 d^2 - (k + 1)(k d^2 - 1) expanded, so it cannot cancel),
-//                         q = (u (d + c) e, w (d + c) e, c), proportional to (sin lon, tan lat, cos lon), c = cos lon.
+//                         q = (u (d + c) e, w (d + c) e, c), proportional to (sin lon, tan lat, cos lon), c = cos lon;
+//   kCameraEquirect       lon = X cx, lat = Y cy (cx = hfov pi / 360, cy = vfov pi / 360), q = (cos lat sin lon, sin lat,
+//                         cos lat cos lon), sin a = a S(a) and cos a = C(a) from sincCos (even in a; |lon| <= pi lies in its
+//                         range).  4 is not a model: the model numbers are public, and 4 stays refused.
 // The per-pose constants are computed on the host in double and stored as float (cameraConstants in
 // video_frame_transform.cpp).  The input is the context's (sphereInputHD, BORDER_WRAP) or a lens rig (lensPosition,
 // BORDER_TRANSPARENT).  Only + - * / and sqrt on the output half, so host and device agree bit for bit.
-enum CameraModel { kCameraPinhole = 0, kCameraEquidistant = 1, kCameraStereographic = 2, kCameraPannini = 3 };
+enum CameraModel { kCameraPinhole = 0, kCameraEquidistant = 1, kCameraStereographic = 2, kCameraPannini = 3, kCameraEquirect = 5 };
 struct RectilinearCamera {
   Rotation r;
   float cx, cy;  // the model's per-axis constants above
@@ -682,6 +687,7 @@ inline RectilinearCamera cameraConstants(int model, float pannini, float yaw, fl
   const double h = static_cast<double>(hfov) * M_PI / 360.0, v = static_cast<double>(vfov) * M_PI / 360.0;  // half angles
   switch (model) {
     case kCameraEquidistant:
+    case kCameraEquirect:
       c.cx = static_cast<float>(h);
       c.cy = static_cast<float>(v);
       break;
@@ -735,6 +741,20 @@ T360_HD void sincCos(float rho, float* sinc, float* cosine) {
   *cosine = c;
 }
 
+// The equirect model's ray at longitude lon and latitude lat.  Out of line on the device, and tested inside cameraRay's
+// last case rather than as a case of its own, so the other models' branches compile as they did before the model existed.
+#ifdef __CUDA_ARCH__
+__device__ __noinline__
+#else
+inline
+#endif
+SphereVec equirectRay(float lon, float lat) {
+  float sl, cl, sp, cp;
+  sincCos(lon, &sl, &cl);
+  sincCos(lat, &sp, &cp);
+  return SphereVec{fMul(cp, fMul(lon, sl)), fMul(lat, sp), fMul(cp, cl)};
+}
+
 // The ray q (not rotated, not normalised) of the pixel at (X, Y) for the models other than the pinhole
 T360_HD SphereVec cameraRay(const RectilinearCamera& c, float X, float Y) {
   switch (c.model) {
@@ -748,7 +768,8 @@ T360_HD SphereVec cameraRay(const RectilinearCamera& c, float X, float Y) {
       const float a = fMul(X, c.cx), b = fMul(Y, c.cy);
       return SphereVec{fMul(2.0f, a), fMul(2.0f, b), fSub(fSub(1.0f, fMul(a, a)), fMul(b, b))};
     }
-    default: {  // kCameraPannini
+    default: {  // kCameraPannini, kCameraEquirect
+      if (c.model == kCameraEquirect) return equirectRay(fMul(X, c.cx), fMul(Y, c.cy));
       const float u = fMul(X, c.cx), w = fMul(Y, c.cy);
       const float ue = fMul(u, c.e), k = fMul(ue, ue);
       const float cl = fDiv(fAdd(-fMul(k, c.d), fSqrt(fAdd(1.0f, fMul(k, c.dd)))), fAdd(k, 1.0f));
@@ -1070,7 +1091,9 @@ struct CameraPhotoRecords {
 // (it covers the ray; with the hard seam and both = false the closer lens only).  MIP = false, or m.top = 0: no pyramid,
 // every used lens at level 0 with weight 0.  With the identity photometry and s = 0 the closer lens's entries are
 // cameraMipMaps' (cameraMap's without a pyramid) and its gain 4096.
-template <bool MIP>
+// STEREO (a stereo rig, T360B200_transformFrameStereoCameraAsync; s = 0): the pixel's output eye e picks lens e, so w =
+// 256 e; the other lens is projected only with both (the statistics).
+template <bool MIP, bool STEREO = false>
 T360_HD int cameraPhotoPoint(const SphereGeometry& g, const RectilinearCamera& c, const LensRigModel& rig, const MipGeometry& m, int bias256,
                              float s, bool both, const LensPhotoPlane& ph, int i, int j, CameraPhotoLens* lens, bool* overlap) {
   float X, Y;
@@ -1078,7 +1101,7 @@ T360_HD int cameraPhotoPoint(const SphereGeometry& g, const RectilinearCamera& c
   cameraXY(g, i, j, &X, &Y, &eye);
   const SphereVec t = rotateHD(c.r, modelRay(c, X, Y));
   float p[2][2];
-  const int w = lensPhotoPosition(rig, s, both, ph, t, g.inW, g.inH, p[0], p[1], &lens[0].gain, &lens[1].gain, overlap);
+  const int w = lensPhotoPosition<STEREO>(rig, s, both, ph, t, g.inW, g.inH, p[0], p[1], &lens[0].gain, &lens[1].gain, overlap, eye);
   const bool used[2] = {p[0][0] == p[0][0], p[1][0] == p[1][0]};
   const bool footprint = MIP && m.top > 0 && (used[0] || used[1]);
   SphereVec rx{}, ry{};
@@ -1105,11 +1128,11 @@ T360_HD int cameraPhotoPoint(const SphereGeometry& g, const RectilinearCamera& c
 
 // The sampling records of output pixel (i, j): cameraPhotoPoint's entries quantised as mipCameraSample quantises its
 // entries (rec1 only where w > 0).  Returns the seam weight w of lens 1.
-template <bool MIP>
+template <bool MIP, bool STEREO = false>
 T360_HD int cameraPhotoSample(const SphereGeometry& g, const RectilinearCamera& c, const LensRigModel& rig, const MipGeometry& m, int bias256,
                               float s, bool both, const LensPhotoPlane& ph, int i, int j, CameraPhotoRecords* lens, bool* overlap) {
   CameraPhotoLens e[2];
-  const int w = cameraPhotoPoint<MIP>(g, c, rig, m, bias256, s, both, ph, i, j, e, overlap);
+  const int w = cameraPhotoPoint<MIP, STEREO>(g, c, rig, m, bias256, s, both, ph, i, j, e, overlap);
   for (int l = 0; l < 2; ++l) {
     int r0, fracX, fracY;
     quantizeAxis(e[l].p0[0], g.kernelSize, &lens[l].rec0[0], &fracX);

@@ -712,7 +712,8 @@ void forLensPixels(const FrameTransformContext& ctx, const T360Orientation& o, i
 // ---- camera views (T360B200_cameraMap, T360B200_transformFrameCameraAsync, and the rectilinear pair, which is the
 // pinhole camera; oriented_view.h: rectilinearSample) -------------------------------------------------------------------
 static_assert(T360_CAMERA_PINHOLE == t360::kCameraPinhole && T360_CAMERA_EQUIDISTANT == t360::kCameraEquidistant &&
-              T360_CAMERA_STEREOGRAPHIC == t360::kCameraStereographic && T360_CAMERA_PANNINI == t360::kCameraPannini);
+              T360_CAMERA_STEREOGRAPHIC == t360::kCameraStereographic && T360_CAMERA_PANNINI == t360::kCameraPannini &&
+              T360_CAMERA_EQUIRECT == t360::kCameraEquirect);
 constexpr T360Camera kPinhole{T360_CAMERA_PINHOLE, 0.0f};
 
 // true, with the reason in *why, when a view of ctx's input (rig == nullptr) or of the rig cannot be rendered with this
@@ -754,6 +755,10 @@ bool cameraRefused(const FrameTransformContext& ctx, const T360LensRig* rig, con
         *why = formatted("a Pannini camera with distance %g sees at most 2 acos(-%g) degrees across, not hfov %g", d, d, h);
       break;
     }
+    case T360_CAMERA_EQUIRECT:
+      if (!(h > 0.0f && h <= 360.0f) || !(v > 0.0f && v <= 180.0f))
+        *why = formatted("hfov %g must lie in (0, 360] and vfov %g in (0, 180] degrees for an equirect camera", h, v);
+      break;
     default:
       *why = formatted("no camera model %d", camera->model);
   }
@@ -821,6 +826,70 @@ bool cameraPhotoRefused(const FrameTransformContext& ctx, const T360LensRig* rig
   if (cameraRefused(ctx, rig, pose, camera, why) || seamWidthRefused(seamWidth, why)) return true;
   if (seamWidth > 0.0f && featherRefused(*rig, seamWidth, why)) return true;
   return photometryRefused(*rig, ph, why) || (minify && minifyRefused(minify, why));
+}
+
+// ---- camera views of a stereo rig (T360B200_stereoCameraMaps, T360B200_transformFrameStereoCameraAsync; oriented_view.h:
+// cameraPhotoSample<MIP, true>) -------------------------------------------------------------------------------------------
+// true, with the reason in *why, when the view cannot be rendered: a NULL rig or one without two lenses (lens e is eye
+// e's), an output_stereo_format other than TB, LR or MONO, the camera view's refusals with the rig, the photometry's, and
+// minifyRefused where minify is not NULL.  (There is no seam: each eye takes its own lens.)
+bool stereoCameraRefused(const FrameTransformContext& ctx, const T360LensRig* rig, const T360RigPhotometry* ph, const T360Pose* pose,
+                         const T360Camera* camera, const T360Minify* minify, std::string* why) {
+  if (!rig) {
+    *why = "a NULL rig (a stereo rig's lenses are its eyes)";
+    return true;
+  }
+  if (rig->numLenses != 2) {
+    *why = formatted("numLenses %d: a stereo rig has two lenses, lens 0 the left eye's and lens 1 the right eye's", rig->numLenses);
+    return true;
+  }
+  const int sf = ctx.output_stereo_format;
+  if (sf != STEREO_FORMAT_TB && sf != STEREO_FORMAT_LR && sf != STEREO_FORMAT_MONO) {
+    *why = formatted("output_stereo_format %d (a stereo rig's views are LR, TB or MONO: eye 0 alone)", sf);
+    return true;
+  }
+  return cameraRefused(ctx, rig, pose, camera, why) || photometryRefused(*rig, ph, why) || (minify && minifyRefused(minify, why));
+}
+
+// The geometry of one plane of a camera view of a rig: rectilinearGeometry's (mono, no input eye re-pack) and, for a
+// stereo rig, the output eye split of ctx's output_stereo_format (whatever input_stereo_format says)
+t360::SphereGeometry rigViewGeometry(const FrameTransformContext& ctx, bool stereo, int inW, int inH, int outW, int outH) {
+  t360::SphereGeometry g = rectilinearGeometry(ctx, true, inW, inH, outW, outH);
+  if (stereo) {
+    g.splitLR = ctx.output_stereo_format == STEREO_FORMAT_LR;
+    g.splitTB = ctx.output_stereo_format == STEREO_FORMAT_TB;
+  }
+  return g;
+}
+
+// The host twin of one lens and plane of a camera view of a rig with photometry (STEREO = false, T360B200_cameraPhotoMaps;
+// lensWeight the seam weight) or of a stereo rig (STEREO = true, T360B200_stereoCameraMaps, seamWidth 0; lensWeight the eye
+// weight 256 e): cameraPhotoPoint<true, STEREO> of every pixel with both lenses projected.  The arguments are not refused.
+template <bool STEREO>
+void cameraPhotoTwin(const FrameTransformContext& ctx, const T360LensRig& rig, const T360RigPhotometry& photometry, float seamWidth,
+                     const T360Pose& pose, const T360Camera& camera, const T360Minify* minify, int lens, int plane, int inW, int inH, int outW,
+                     int outH, float* map0, float* map1, uint8_t* level, uint16_t* weight, uint16_t* gain, uint16_t* lensWeight) {
+  const t360::SphereGeometry g = rigViewGeometry(ctx, STEREO, inW, inH, outW, outH);
+  const t360::RectilinearCamera c = cameraConstants(pose, camera);
+  const t360::LensRigModel model = lensRigModel(rig);
+  const t360::MipGeometry m = t360::mipGeometry(g, minify ? minify->maxLevel : 0);
+  const int bias = minify ? mipBias(*minify) : 0;
+  const t360::LensPhotoPlane ph = lensPhotoPlane(photometry, rig.numLenses, plane);
+  const float s = seamWidth > 0.0f ? lensSeamScale(seamWidth) : 0.0f;
+  for (int i = 0; i < outH; ++i)
+    for (int j = 0; j < outW; ++j) {
+      const size_t at = static_cast<size_t>(i) * outW + j;
+      t360::CameraPhotoLens e[2];
+      bool overlap;
+      lensWeight[at] = static_cast<uint16_t>(t360::cameraPhotoPoint<true, STEREO>(g, c, model, m, bias, s, /*both=*/true, ph, i, j, e, &overlap));
+      map0[2 * at] = e[lens].p0[0];
+      map0[2 * at + 1] = e[lens].p0[1];
+      map1[2 * at] = e[lens].p1[0];
+      map1[2 * at + 1] = e[lens].p1[1];
+      level[at] = static_cast<uint8_t>(e[lens].level);
+      weight[at] = static_cast<uint16_t>(e[lens].w);
+      gain[at] = static_cast<uint16_t>(e[lens].gain);
+    }
 }
 
 }  // namespace
@@ -1483,16 +1552,19 @@ class VideoFrameTransform {
     });
   }
 
-  // Whole frame of a camera view of a lens rig with photometry (T360B200_transformFrameCameraPhotoAsync): with a pyramid
-  // (minify not NULL and some plane's top level above 0) the planes' pyramids first (buildPyramids), then one gather launch
-  // for all planes, every record computed by cameraPhotoSample (oriented_view.h), so a rig, photometry, seam, pose, camera
-  // and minify give what cameraPhotoMaps describes.  With stats set (device, [numPlanes][6]) the overlap's sums are zeroed
-  // with a memset and accumulated by the same gather.  Needs no plan and leaves the plans alone; no tables.
-  bool transformFrameCameraPhoto(const char* what, const T360LensRig* rig, const T360RigPhotometry* photo, float seamWidth, const T360Pose* pose,
-                                 const T360Camera* camera, const T360Minify* minify, unsigned long long* stats, const FramePlanes& f,
-                                 cudaStream_t stream) {
+  // Whole frame of a camera view of a lens rig with photometry (T360B200_transformFrameCameraPhotoAsync) or, with stereo
+  // set, of a stereo rig (T360B200_transformFrameStereoCameraAsync, seamWidth 0): with a pyramid (minify not NULL and some
+  // plane's top level above 0) the planes' pyramids first (buildPyramids), then one gather launch for all planes, every
+  // record computed by cameraPhotoSample<MIP, stereo> (oriented_view.h), so a rig, photometry, seam, pose, camera and
+  // minify give what cameraPhotoMaps (stereoCameraMaps) describes.  With stats set (device, [numPlanes][6]) the overlap's
+  // sums are zeroed with a memset and accumulated by the same gather.  Needs no plan and leaves the plans alone; no tables.
+  bool transformFrameCameraPhoto(const char* what, bool stereo, const T360LensRig* rig, const T360RigPhotometry* photo, float seamWidth,
+                                 const T360Pose* pose, const T360Camera* camera, const T360Minify* minify, unsigned long long* stats,
+                                 const FramePlanes& f, cudaStream_t stream) {
     auto refused = [&](const FrameTransformContext& ctx, std::string* why) {
-      if (cameraPhotoRefused(ctx, rig, photo, seamWidth, pose, camera, minify, why)) return true;
+      if (stereo ? stereoCameraRefused(ctx, rig, photo, pose, camera, minify, why)
+                 : cameraPhotoRefused(ctx, rig, photo, seamWidth, pose, camera, minify, why))
+        return true;
       for (int p = 0; minify && minify->maxLevel > 0 && p < f.numPlanes; ++p)
         if (f.inW[p] > 2 * 65535 || f.inH[p] > 2 * 65535) {  // (CameraPhotoLevel keeps a level's sides in 16 bits)
           *why = formatted("input plane %d is %dx%d: a pyramid needs sides of at most 131070", p, f.inW[p], f.inH[p]);
@@ -1505,7 +1577,7 @@ class VideoFrameTransform {
       t360::PerFrameGatherParams::CameraPhoto& cp = gp.cameraPhoto;
       int topMax = 0;
       for (int p = 0; p < f.numPlanes; ++p) {
-        gp.plane[p].geometry = rectilinearGeometry(ctx, true, f.inW[p], f.inH[p], f.outW[p], f.outH[p]);
+        gp.plane[p].geometry = rigViewGeometry(ctx, stereo, f.inW[p], f.inH[p], f.outW[p], f.outH[p]);
         cp.mip[p].geometry = pyramids.mip[p].geometry = t360::mipGeometry(gp.plane[p].geometry, minify ? minify->maxLevel : 0);
         topMax = std::max(topMax, cp.mip[p].geometry.top);
         cp.photo.plane[p] = lensPhotoPlane(*photo, rig->numLenses, p);
@@ -1525,7 +1597,8 @@ class VideoFrameTransform {
             cp.mip[p].level[l - 1] = {L.bytes, L.pitch, static_cast<uint16_t>(L.w), static_cast<uint16_t>(L.h)};
           }
       }
-      perFrameGather(t360::PerFrameSource::kCameraPhoto, gp, ctx, f, f.in, f.inPitch, nullptr, /*transparent=*/true, nullptr, nullptr, nullptr, s);
+      perFrameGather(stereo ? t360::PerFrameSource::kStereoCamera : t360::PerFrameSource::kCameraPhoto, gp, ctx, f, f.in, f.inPitch, nullptr,
+                     /*transparent=*/true, nullptr, nullptr, nullptr, s);
       releaseAfter(staged, s);
       return true;
     });
@@ -3203,27 +3276,8 @@ T360_API int T360B200_cameraPhotoMaps(const FrameTransformContext* ctx, const T3
     std::printf("%s. Error: %s\n", what, why.c_str());
     return 0;
   }
-  const t360::SphereGeometry g = rectilinearGeometry(*ctx, true, inW, inH, outW, outH);
-  const t360::RectilinearCamera c = cameraConstants(*pose, *camera);
-  const t360::LensRigModel model = lensRigModel(*rig);
-  const t360::MipGeometry m = t360::mipGeometry(g, minify ? minify->maxLevel : 0);
-  const int bias = minify ? mipBias(*minify) : 0;
-  const t360::LensPhotoPlane ph = lensPhotoPlane(*photometry, rig->numLenses, plane);
-  const float s = seamWidth > 0.0f ? lensSeamScale(seamWidth) : 0.0f;
-  for (int i = 0; i < outH; ++i)
-    for (int j = 0; j < outW; ++j) {
-      const size_t at = static_cast<size_t>(i) * outW + j;
-      t360::CameraPhotoLens e[2];
-      bool overlap;
-      seamWeight[at] = static_cast<uint16_t>(t360::cameraPhotoPoint<true>(g, c, model, m, bias, s, /*both=*/true, ph, i, j, e, &overlap));
-      map0[2 * at] = e[lens].p0[0];
-      map0[2 * at + 1] = e[lens].p0[1];
-      map1[2 * at] = e[lens].p1[0];
-      map1[2 * at + 1] = e[lens].p1[1];
-      level[at] = static_cast<uint8_t>(e[lens].level);
-      weight[at] = static_cast<uint16_t>(e[lens].w);
-      gain[at] = static_cast<uint16_t>(e[lens].gain);
-    }
+  cameraPhotoTwin<false>(*ctx, *rig, *photometry, seamWidth, *pose, *camera, minify, lens, plane, inW, inH, outW, outH, map0, map1, level, weight,
+                         gain, seamWeight);
   return 1;
 }
 T360_API int T360B200_transformFrameCameraPhotoAsync(VideoFrameTransform* t, const T360LensRig* rig, const T360RigPhotometry* photometry,
@@ -3238,7 +3292,40 @@ T360_API int T360B200_transformFrameCameraPhotoAsync(VideoFrameTransform* t, con
   }
   FramePlanes f;
   if (!describeFrame(what, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, f)) return 0;
-  return t->transformFrameCameraPhoto(what, rig, photometry, seamWidth, pose, camera, minify, deviceStats, f, static_cast<cudaStream_t>(stream));
+  return t->transformFrameCameraPhoto(what, false, rig, photometry, seamWidth, pose, camera, minify, deviceStats, f, static_cast<cudaStream_t>(stream));
+}
+T360_API int T360B200_stereoCameraMaps(const FrameTransformContext* ctx, const T360LensRig* rig, const T360RigPhotometry* photometry, const T360Pose* pose,
+                                       const T360Camera* camera, const T360Minify* minify, int lens, int plane, int inW, int inH, int outW, int outH,
+                                       float* map0, float* map1, uint8_t* level, uint16_t* weight, uint16_t* gain, uint16_t* eyeWeight) {
+  const char* what = "Could not compute the stereo camera maps";
+  std::string why;
+  if (!ctx) why = "a NULL context";
+  else if (stereoCameraRefused(*ctx, rig, photometry, pose, camera, minify, &why)) {}
+  else if (lens < 0 || lens > 1) why = formatted("lens %d is outside 0..1", lens);
+  else if (plane < 0 || plane > 2) why = formatted("plane %d is outside 0..2", plane);
+  else if (!map0 || !map1 || !level || !weight || !gain || !eyeWeight || inW <= 0 || inH <= 0 || outW <= 0 || outH <= 0)
+    why = "a NULL map, level, weight or gain array or a plane size that is not positive";
+  if (!why.empty()) {
+    std::printf("%s. Error: %s\n", what, why.c_str());
+    return 0;
+  }
+  cameraPhotoTwin<true>(*ctx, *rig, *photometry, 0.0f, *pose, *camera, minify, lens, plane, inW, inH, outW, outH, map0, map1, level, weight, gain,
+                        eyeWeight);
+  return 1;
+}
+T360_API int T360B200_transformFrameStereoCameraAsync(VideoFrameTransform* t, const T360LensRig* rig, const T360RigPhotometry* photometry,
+                                                      const T360Pose* pose, const T360Camera* camera, const T360Minify* minify,
+                                                      unsigned long long* deviceStats, int numPlanes, const uint8_t* const* dIn,
+                                                      uint8_t* const* dOut, const int* inW, const int* inH, const int* inPitch, const int* outW,
+                                                      const int* outH, const int* outPitch, void* stream) {
+  const char* what = "Could not transform the frame with a camera view of a stereo rig";
+  if (!t) {
+    std::printf("%s. Error: a NULL argument\n", what);
+    return 0;
+  }
+  FramePlanes f;
+  if (!describeFrame(what, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, f)) return 0;
+  return t->transformFrameCameraPhoto(what, true, rig, photometry, 0.0f, pose, camera, minify, deviceStats, f, static_cast<cudaStream_t>(stream));
 }
 T360_API void T360B200_setPinHostPlanes(VideoFrameTransform* t, int enable) { if (t) t->setPinHostPlanes(enable != 0); }
 T360_API void T360B200_debugTrace(VideoFrameTransform* t, int enable) { if (t) t->enableTrace(enable != 0); }

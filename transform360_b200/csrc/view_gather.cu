@@ -25,8 +25,9 @@
 //     corrects each sample, combines them by the seam and accumulates the overlap's statistics;
 //   - a camera view of a lens rig with photometry (CameraPhotoPositions): the camera view's ray, then both lenses' records,
 //     levels and gains (cameraPhotoSample); each lens's sample is the blend of its two levels, then the tile loop goes on
-//     as for LensPhotoPositions.
-// In all nine, the records come from the same host/device functions the planner (or its host twin) uses: bit-identical.
+//     as for LensPhotoPositions;
+//   - a camera view of a stereo rig (StereoCameraPositions): the same, with the output eye picking the lens.
+// In all ten, the records come from the same host/device functions the planner (or its host twin) uses: bit-identical.
 #include "gather_common.cuh"
 
 #include <algorithm>
@@ -385,6 +386,24 @@ struct CameraPhotoPositions : NoTables {
   }
 };
 
+// A camera view of a stereo rig (kStereoCamera): CameraPhotoPositions with the output eye's lens in place of the closer
+// lens (cameraPhotoSample<MIP, true>): eye e's pixels gather lens e alone, and with statistics the other lens too.  The
+// launch's seamScale is 0.
+template <int K, bool MIP>
+struct StereoCameraPositions : CameraPhotoPositions<K, MIP> {
+  using CameraPhotoPositions<K, MIP>::CameraPhotoPositions;
+  __device__ int record(const PerFrameGatherParams& p, const PerFramePlane& v, int pl, int i, int j, int32_t*, int32_t*, int* g0, int* g1,
+                        bool* overlap) {
+    const PerFrameGatherParams::LensPhoto& photo = p.cameraPhoto.photo;
+    CameraPhotoRecords* lens = this->lens;
+    const int w = cameraPhotoSample<MIP, true>(v.geometry, p.camera, p.rig, p.cameraPhoto.mip[pl].geometry, p.mipBias, 0.0f,
+                                               photo.stats != nullptr, photo.plane[pl], i, j, lens, overlap);
+    *g0 = lens[0].gain;
+    *g1 = lens[1].gain;
+    return w;
+  }
+};
+
 template <class Pos, class = void>
 struct HasPinholeLoop : std::false_type {};
 template <class Pos>
@@ -468,9 +487,11 @@ cudaError_t launchPerFrameGather(PerFrameGatherParams p, PerFrameSource source, 
     case PerFrameSource::kRectilinear: return launchPositions<RectilinearPositions>(p, p.lens, numTiles, numSMs, stream);
     case PerFrameSource::kCameraMip: return launchPositions<MipCameraPositions>(p, p.lens, numTiles, numSMs, stream);
     case PerFrameSource::kLensPhoto: return launchPositions<LensPhotoPositions>(p, barrel, numTiles, numSMs, stream);
-    case PerFrameSource::kCameraPhoto: {
+    case PerFrameSource::kCameraPhoto:
+    case PerFrameSource::kStereoCamera: {
       bool mip = false;  // (a level table only where some plane has a pyramid)
       for (int i = 0; i < p.numPlanes; ++i) mip = mip || p.cameraPhoto.mip[i].geometry.top > 0;
+      if (source == PerFrameSource::kStereoCamera) return launchPositions<StereoCameraPositions>(p, mip, numTiles, numSMs, stream);
       return launchPositions<CameraPhotoPositions>(p, mip, numTiles, numSMs, stream);
     }
   }

@@ -119,6 +119,7 @@ def as_pose(pose) -> T360Pose:
 
 
 T360_CAMERA_PINHOLE, T360_CAMERA_EQUIDISTANT, T360_CAMERA_STEREOGRAPHIC, T360_CAMERA_PANNINI = 0, 1, 2, 3
+T360_CAMERA_EQUIRECT = 5  # (4 is not a model)
 
 
 class T360Camera(C.Structure):
@@ -307,6 +308,12 @@ def load(path: os.PathLike | None = None):
     L.T360B200_transformFrameCameraPhotoAsync.restype = ci
     L.T360B200_transformFrameCameraPhotoAsync.argtypes = [vp, C.POINTER(T360LensRig), C.POINTER(T360RigPhotometry), C.c_float,
                                                           C.POINTER(T360Pose), C.POINTER(T360Camera), C.POINTER(T360Minify), vp, ci] + planes
+    L.T360B200_stereoCameraMaps.restype = ci
+    L.T360B200_stereoCameraMaps.argtypes = [C.POINTER(FrameTransformContext), C.POINTER(T360LensRig), C.POINTER(T360RigPhotometry),
+                                            C.POINTER(T360Pose), C.POINTER(T360Camera), C.POINTER(T360Minify)] + [ci] * 6 + [vp] * 6
+    L.T360B200_transformFrameStereoCameraAsync.restype = ci
+    L.T360B200_transformFrameStereoCameraAsync.argtypes = [vp, C.POINTER(T360LensRig), C.POINTER(T360RigPhotometry), C.POINTER(T360Pose),
+                                                           C.POINTER(T360Camera), C.POINTER(T360Minify), vp, ci] + planes
     L.T360B200_setPinHostPlanes.restype = None
     L.T360B200_setPinHostPlanes.argtypes = [vp, ci]
     L.T360B200_debugTrace.restype = None
@@ -343,6 +350,7 @@ EXPORTED_SYMBOLS = [
     "T360B200_lensPhotoMaps", "T360B200_transformFrameLensPhotoAsync",
     "T360B200_rectilinearMap", "T360B200_transformFrameRectilinearAsync", "T360B200_cameraMap", "T360B200_transformFrameCameraAsync",
     "T360B200_cameraMipMaps", "T360B200_transformFrameCameraMipAsync", "T360B200_cameraPhotoMaps", "T360B200_transformFrameCameraPhotoAsync",
+    "T360B200_stereoCameraMaps", "T360B200_transformFrameStereoCameraAsync",
     "T360B200_setPinHostPlanes", "T360B200_debugTrace", "T360B200_debugTraceRead", "T360B200_synchronize", "T360B200_stream", "T360B200_kernelLaunchCount", "T360B200_planDeviceBytes",
     "T360B200_planTileCounts", "T360B200_deviceCount", "T360B200_version",
 ]
@@ -496,6 +504,15 @@ class VideoFrameTransform:
         n, enqueue = self._frame_call("T360B200_transformFrameCameraPhotoAsync", in_planes, out_planes, dims)
         return lambda rig, photometry, seam_width, pose, camera, minify=None, stream=0, stats=0: enqueue(
             (C.byref(rig), C.byref(photometry), seam_width, C.byref(as_pose(pose)), C.byref(as_camera(camera)),
+             C.byref(as_minify(minify)) if minify is not None else None, stats or None, n), stream)
+
+    def make_stereo_camera_frame_call(self, in_planes, out_planes, dims):
+        """Like make_camera_photo_frame_call, for T360B200_transformFrameStereoCameraAsync (a camera view of a stereo rig:
+        eye e of the context's output_stereo_format takes lens e, no seam): returns a callable f(rig, photometry, pose,
+        camera, minify=None, stream=0, stats=0) -> bool."""
+        n, enqueue = self._frame_call("T360B200_transformFrameStereoCameraAsync", in_planes, out_planes, dims)
+        return lambda rig, photometry, pose, camera, minify=None, stream=0, stats=0: enqueue(
+            (C.byref(rig), C.byref(photometry), C.byref(as_pose(pose)), C.byref(as_camera(camera)),
              C.byref(as_minify(minify)) if minify is not None else None, stats or None, n), stream)
 
     def generate_map_from_warp(self, map, in_w: int, in_h: int, plan_index: int, border: int = BORDER_WRAP) -> bool:
@@ -814,6 +831,23 @@ def camera_photo_maps(ctx: FrameTransformContext, rig: T360LensRig, photometry: 
                                            weight.ctypes.data, gain.ctypes.data, seam_weight.ctypes.data):
         raise ValueError("T360B200_cameraPhotoMaps refused the arguments (message on stdout)")
     return map0, map1, level, weight, gain, seam_weight
+
+
+def stereo_camera_maps(ctx: FrameTransformContext, rig: T360LensRig, photometry: T360RigPhotometry, pose, camera, minify, lens, plane,
+                       in_w, in_h, out_w, out_h) -> tuple[np.ndarray, np.ndarray, np.ndarray, np.ndarray, np.ndarray, np.ndarray]:
+    """The host twin of one lens (0 or 1) of one plane of a camera view of a stereo rig (T360B200_stereoCameraMaps, no
+    CUDA): (map0, map1, level, weight, gain, eye_weight), camera_photo_maps' arrays for that lens wherever it covers the
+    ray, and eye_weight (uint16) 0 on eye-0 pixels and 256 on eye-1 pixels.  minify as for camera_mip_maps, or None."""
+    shape = (max(out_h, 0), max(out_w, 0))
+    map0, map1 = np.zeros(shape + (2,), np.float32), np.zeros(shape + (2,), np.float32)
+    level = np.zeros(shape, np.uint8)
+    weight, gain, eye_weight = (np.zeros(shape, np.uint16) for _ in range(3))
+    if not load().T360B200_stereoCameraMaps(C.byref(ctx), C.byref(rig), C.byref(photometry), C.byref(as_pose(pose)), C.byref(as_camera(camera)),
+                                            C.byref(as_minify(minify)) if minify is not None else None, lens, plane, in_w, in_h, out_w, out_h,
+                                            map0.ctypes.data, map1.ctypes.data, level.ctypes.data, weight.ctypes.data, gain.ctypes.data,
+                                            eye_weight.ctypes.data):
+        raise ValueError("T360B200_stereoCameraMaps refused the arguments (message on stdout)")
+    return map0, map1, level, weight, gain, eye_weight
 
 
 def square_pixel_vfov(hfov, width, height) -> float:
