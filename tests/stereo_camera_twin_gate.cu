@@ -243,7 +243,7 @@ StereoCameraGate::HostData StereoCameraGate::makeData() {
     if (oddSides) mapW |= 1, mapH |= 1;
     StereoGeo e{};
     e.g = sphereGeometry(c, mapW, mapH, 8 + g.below(16000), 8 + g.below(8000), 1 << (k / 2) % 4);
-    e.g.splitLR = split == 1;  // (as rigViewGeometry sets them: the output split alone, no input re-pack)
+    e.g.splitLR = split == 1;  // (as viewGeometry sets them: the output split alone, no input re-pack)
     e.g.splitTB = split >= 2;
     e.m = mipGeometry(e.g, k % 9);
     e.bias = g.below(2049) - 1024;

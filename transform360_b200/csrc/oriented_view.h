@@ -462,6 +462,13 @@ T360_HD void lensPosition(const LensRigModel& rig, const SphereVec& d, int inW, 
   *py = h.py;
 }
 
+// The feathered seam's weight (0..256) of lens 1 where both lenses cover a direction: a linear ramp in theta0 - theta1,
+// t = 0.5 + (theta0 - theta1) s rounded to 1/256 (half to even) and clamped
+T360_HD int seamWeight(float theta0, float theta1, float s) {
+  const float tw = fMul(fAdd(0.5f, fMul(fSub(theta0, theta1), s)), 256.0f);
+  return tw <= 0.0f ? 0 : (tw >= 256.0f ? 256 : roundHalfEven(tw));
+}
+
 // The feathered seam of a two-lens rig (T360B200_transformFrameLensBlendAsync): both lenses' view of d and the weight w
 // (0..256) of lens 1.  Where both cover d, w is a linear ramp in theta0 - theta1, t = 0.5 + (theta0 - theta1) s rounded to
 // 1/256 and clamped (s = 1 / (2 seamWidth), seamWidth in radians, computed on the host in double: lensSeamScale); where
@@ -471,10 +478,7 @@ T360_HD int lensBlendPosition(const LensRigModel& rig, float s, const SphereVec&
   const LensHit h0 = lensHit(rig.lens[0], d, lensRow(rig.lens[0].m + 6, d), inW, inH);
   const LensHit h1 = lensHit(rig.lens[1], d, lensRow(rig.lens[1].m + 6, d), inW, inH);
   int w = h1.covered ? 256 : 0;
-  if (h0.covered && h1.covered) {
-    const float tw = fMul(fAdd(0.5f, fMul(fSub(h0.theta, h1.theta), s)), 256.0f);
-    w = tw <= 0.0f ? 0 : (tw >= 256.0f ? 256 : roundHalfEven(tw));
-  }
+  if (h0.covered && h1.covered) w = seamWeight(h0.theta, h1.theta, s);
   const float nan = bitsFloat(0x7fc00000u);
   p0[0] = w < 256 ? h0.px : nan;
   p0[1] = w < 256 ? h0.py : nan;
@@ -603,10 +607,7 @@ T360_HD int lensPhotoPosition(const LensRigModel& rig, float s, bool both, const
   int w = second ? 256 : 0;
   if (s > 0.0f) {
     w = h1.covered ? 256 : 0;
-    if (h0.covered && h1.covered) {
-      const float tw = fMul(fAdd(0.5f, fMul(fSub(h0.theta, h1.theta), s)), 256.0f);
-      w = tw <= 0.0f ? 0 : (tw >= 256.0f ? 256 : roundHalfEven(tw));
-    }
+    if (h0.covered && h1.covered) w = seamWeight(h0.theta, h1.theta, s);
   }
   p0[0] = h0.px; p0[1] = h0.py;
   p1[0] = h1.px; p1[1] = h1.py;
@@ -781,7 +782,8 @@ T360_HD SphereVec cameraRay(const RectilinearCamera& c, float X, float Y) {
 
 // Steps 1-5 of the contract for output pixel (i, j): the rotated ray (not normalised) and the output eye.  The geometry's
 // mapW, mapH, splitLR, splitTB and vflip play a part.  ANY_MODEL = false: c is a pinhole (the kernel's own loop for
-// pinhole launches, which so keeps the rectilinear view's code).
+// pinhole launches, which so keeps the rectilinear view's code).  (These are cameraXY's steps and modelRay's pinhole ray,
+// written out: built on them, the rectilinear kernels compile to different SASS.)
 template <bool ANY_MODEL = true>
 T360_HD SphereVec rectilinearPoint(const SphereGeometry& g, const RectilinearCamera& c, int i, int j, bool* eye) {
   float x = pixelCentre(j, g.mapW), y = pixelCentre(i, g.mapH);

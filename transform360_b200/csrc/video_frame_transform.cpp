@@ -17,6 +17,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <initializer_list>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -709,86 +710,39 @@ void forLensPixels(const FrameTransformContext& ctx, const T360Orientation& o, i
     for (int j = 0; j < outW; ++j) point(g, r, colTab, rowTab, i, j, static_cast<size_t>(i) * outW + j);
 }
 
-// ---- camera views (T360B200_cameraMap, T360B200_transformFrameCameraAsync, and the rectilinear pair, which is the
-// pinhole camera; oriented_view.h: rectilinearSample) -------------------------------------------------------------------
+// ---- camera views: the rectilinear, camera, anti-aliased (mip), photometric and stereo calls (T360B200_cameraMap and
+// T360B200_transformFrameCameraAsync, the rectilinear pair, which is the pinhole camera, T360B200_cameraMipMaps, ...CameraMip...,
+// ...CameraPhoto... and ...StereoCamera...; oriented_view.h: rectilinearSample, mipCameraSample, cameraPhotoSample) --------
 static_assert(T360_CAMERA_PINHOLE == t360::kCameraPinhole && T360_CAMERA_EQUIDISTANT == t360::kCameraEquidistant &&
               T360_CAMERA_STEREOGRAPHIC == t360::kCameraStereographic && T360_CAMERA_PANNINI == t360::kCameraPannini &&
               T360_CAMERA_EQUIRECT == t360::kCameraEquirect);
 constexpr T360Camera kPinhole{T360_CAMERA_PINHOLE, 0.0f};
 
-// true, with the reason in *why, when a view of ctx's input (rig == nullptr) or of the rig cannot be rendered with this
-// pose and camera.  The output layout plays no part: the pose replaces it.
-bool cameraRefused(const FrameTransformContext& ctx, const T360LensRig* rig, const T360Pose* pose, const T360Camera* camera, std::string* why) {
-  if (!pose) {
-    *why = "a NULL pose";
-    return true;
-  }
-  if (!std::isfinite(pose->yaw) || !std::isfinite(pose->pitch) || !std::isfinite(pose->roll) || !std::isfinite(pose->hfov) ||
-      !std::isfinite(pose->vfov)) {
-    *why = formatted("the pose (yaw %g, pitch %g, roll %g, hfov %g, vfov %g) is not finite", pose->yaw, pose->pitch, pose->roll, pose->hfov,
-                     pose->vfov);
-    return true;
-  }
-  if (!camera) {
-    *why = "a NULL camera";
-    return true;
-  }
-  const float h = pose->hfov, v = pose->vfov;
-  switch (camera->model) {
-    case T360_CAMERA_PINHOLE:
-      if (!(h > 0.0f && h <= 179.0f) || !(v > 0.0f && v <= 179.0f)) *why = formatted("hfov %g and vfov %g must lie in (0, 179] degrees", h, v);
-      break;
-    case T360_CAMERA_EQUIDISTANT:
-      if (!(h > 0.0f && h <= 360.0f) || !(v > 0.0f && v <= 360.0f))
-        *why = formatted("hfov %g and vfov %g must lie in (0, 360] degrees for an equidistant camera", h, v);
-      break;
-    case T360_CAMERA_STEREOGRAPHIC:
-      if (!(h > 0.0f && h <= 359.0f) || !(v > 0.0f && v <= 359.0f))
-        *why = formatted("hfov %g and vfov %g must lie in (0, 359] degrees for a stereographic camera", h, v);
-      break;
-    case T360_CAMERA_PANNINI: {
-      const float d = camera->pannini;
-      if (!(d >= 0.0f && d <= 1.0f)) *why = formatted("the Pannini distance %g must lie in [0, 1]", d);
-      else if (!(h > 0.0f && h <= 359.0f) || !(v > 0.0f && v <= 179.0f))
-        *why = formatted("hfov %g must lie in (0, 359] and vfov %g in (0, 179] degrees for a Pannini camera", h, v);
-      else if (!(d + std::cos(static_cast<double>(h) * M_PI / 360.0) > 0.0))
-        *why = formatted("a Pannini camera with distance %g sees at most 2 acos(-%g) degrees across, not hfov %g", d, d, h);
-      break;
-    }
-    case T360_CAMERA_EQUIRECT:
-      if (!(h > 0.0f && h <= 360.0f) || !(v > 0.0f && v <= 180.0f))
-        *why = formatted("hfov %g must lie in (0, 360] and vfov %g in (0, 180] degrees for an equirect camera", h, v);
-      break;
-    default:
-      *why = formatted("no camera model %d", camera->model);
-  }
-  if (!why->empty()) return true;
-  if (rig && rigRefused(rig, why)) return true;
-  if (ctx.enable_low_pass_filter) {
-    *why = "the low-pass filter is not available for a camera view (set enable_low_pass_filter = 0)";
-    return true;
-  }
-  if (t360::kernelSizeOf(ctx.interpolation_alg) == 0) {
-    *why = formatted("no interpolation algorithm %d", static_cast<int>(ctx.interpolation_alg));
-    return true;
-  }
-  return false;
+// What a camera call was given; the arguments a call does not take stay NULL / 0.  rig == nullptr: a view of the
+// context's input.  photometric: the call corrects the rig's lenses, so it needs a rig and a photometry (the photometric
+// and stereo calls); stereo: each eye takes its own lens (no seam).  minify == nullptr: no pyramid.
+struct CameraView {
+  const T360LensRig* rig = nullptr;
+  const T360RigPhotometry* photometry = nullptr;
+  float seamWidth = 0.0f;
+  const T360Pose* pose = nullptr;
+  const T360Camera* camera = nullptr;
+  const T360Minify* minify = nullptr;
+  unsigned long long* stats = nullptr;
+  bool photometric = false;
+  bool stereo = false;
+};
+// A view of ctx's input (rig == nullptr) or of a rig's lenses as they are: the rectilinear, camera and camera-mip calls
+CameraView plainView(const T360LensRig* rig, const T360Pose* pose, const T360Camera* camera, const T360Minify* minify = nullptr) {
+  return {rig, nullptr, 0.0f, pose, camera, minify};
+}
+// A view of a rig's lenses with photometry: the photometric call, and the stereo call (seamWidth 0)
+CameraView photoView(const T360LensRig* rig, const T360RigPhotometry* photometry, float seamWidth, const T360Pose* pose, const T360Camera* camera,
+                     const T360Minify* minify, unsigned long long* stats, bool stereo) {
+  return {rig, photometry, seamWidth, pose, camera, minify, stats, true, stereo};
 }
 
-// The per-frame constants of a pose and camera (oriented_view.h: cameraConstants)
-t360::RectilinearCamera cameraConstants(const T360Pose& pose, const T360Camera& camera) {
-  return t360::cameraConstants(camera.model, camera.pannini, pose.yaw, pose.pitch, pose.roll, pose.hfov, pose.vfov);
-}
-
-// The geometry of one outW x outH plane of an inW x inH input in a rectilinear view: ctx's (its stereo formats and input
-// layout, cube-map input_expand_coef), or with a rig lensContext's (mono); no tables
-t360::SphereGeometry rectilinearGeometry(const FrameTransformContext& ctx, bool rig, int inW, int inH, int outW, int outH) {
-  return t360::sphereGeometry(rig ? lensContext(ctx) : ctx, outW, outH, inW, inH, t360::kernelSizeOf(ctx.interpolation_alg));
-}
-
-// ---- anti-aliased camera views (T360B200_cameraMipMaps, T360B200_transformFrameCameraMipAsync; oriented_view.h:
-// mipCameraSample) -------------------------------------------------------------------------------------------------------
-// true, with the reason in *why, when `minify` is NULL or out of range (the camera's own checks: cameraRefused)
+// true, with the reason in *why, when `minify` is NULL or out of range
 bool minifyRefused(const T360Minify* minify, std::string* why) {
   if (!minify) {
     *why = "a NULL minify";
@@ -804,92 +758,152 @@ bool minifyRefused(const T360Minify* minify, std::string* why) {
   }
   return false;
 }
-bool cameraMipRefused(const FrameTransformContext& ctx, const T360LensRig* rig, const T360Pose* pose, const T360Camera* camera,
-                      const T360Minify* minify, std::string* why) {
-  return cameraRefused(ctx, rig, pose, camera, why) || minifyRefused(minify, why);
+
+// true, with the reason in *why, when view v of ctx's input or of its rig cannot be rendered, in this order: a photometric
+// view's NULL rig; a stereo rig without two lenses or an output_stereo_format other than TB, LR or MONO; the pose, the
+// camera and its fields of view, the rig (rigRefused), the low-pass filter and the interpolation; a photometric view's
+// seam (seamWidthRefused, featherRefused) and photometry (photometryRefused); the minify where there is one.  The output
+// layout plays no part: the pose replaces it.
+bool viewRefused(const FrameTransformContext& ctx, const CameraView& v, std::string* why) {
+  if (v.photometric && !v.rig) {
+    *why = v.stereo ? "a NULL rig (a stereo rig's lenses are its eyes)" : "a NULL rig (the photometry corrects a rig's lenses)";
+    return true;
+  }
+  if (v.stereo) {
+    if (v.rig->numLenses != 2) {
+      *why = formatted("numLenses %d: a stereo rig has two lenses, lens 0 the left eye's and lens 1 the right eye's", v.rig->numLenses);
+      return true;
+    }
+    const int sf = ctx.output_stereo_format;
+    if (sf != STEREO_FORMAT_TB && sf != STEREO_FORMAT_LR && sf != STEREO_FORMAT_MONO) {
+      *why = formatted("output_stereo_format %d (a stereo rig's views are LR, TB or MONO: eye 0 alone)", sf);
+      return true;
+    }
+  }
+  const T360Pose* pose = v.pose;
+  if (!pose) {
+    *why = "a NULL pose";
+    return true;
+  }
+  if (!std::isfinite(pose->yaw) || !std::isfinite(pose->pitch) || !std::isfinite(pose->roll) || !std::isfinite(pose->hfov) ||
+      !std::isfinite(pose->vfov)) {
+    *why = formatted("the pose (yaw %g, pitch %g, roll %g, hfov %g, vfov %g) is not finite", pose->yaw, pose->pitch, pose->roll, pose->hfov,
+                     pose->vfov);
+    return true;
+  }
+  if (!v.camera) {
+    *why = "a NULL camera";
+    return true;
+  }
+  const float h = pose->hfov, vf = pose->vfov;
+  switch (v.camera->model) {
+    case T360_CAMERA_PINHOLE:
+      if (!(h > 0.0f && h <= 179.0f) || !(vf > 0.0f && vf <= 179.0f)) *why = formatted("hfov %g and vfov %g must lie in (0, 179] degrees", h, vf);
+      break;
+    case T360_CAMERA_EQUIDISTANT:
+      if (!(h > 0.0f && h <= 360.0f) || !(vf > 0.0f && vf <= 360.0f))
+        *why = formatted("hfov %g and vfov %g must lie in (0, 360] degrees for an equidistant camera", h, vf);
+      break;
+    case T360_CAMERA_STEREOGRAPHIC:
+      if (!(h > 0.0f && h <= 359.0f) || !(vf > 0.0f && vf <= 359.0f))
+        *why = formatted("hfov %g and vfov %g must lie in (0, 359] degrees for a stereographic camera", h, vf);
+      break;
+    case T360_CAMERA_PANNINI: {
+      const float d = v.camera->pannini;
+      if (!(d >= 0.0f && d <= 1.0f)) *why = formatted("the Pannini distance %g must lie in [0, 1]", d);
+      else if (!(h > 0.0f && h <= 359.0f) || !(vf > 0.0f && vf <= 179.0f))
+        *why = formatted("hfov %g must lie in (0, 359] and vfov %g in (0, 179] degrees for a Pannini camera", h, vf);
+      else if (!(d + std::cos(static_cast<double>(h) * M_PI / 360.0) > 0.0))
+        *why = formatted("a Pannini camera with distance %g sees at most 2 acos(-%g) degrees across, not hfov %g", d, d, h);
+      break;
+    }
+    case T360_CAMERA_EQUIRECT:
+      if (!(h > 0.0f && h <= 360.0f) || !(vf > 0.0f && vf <= 180.0f))
+        *why = formatted("hfov %g must lie in (0, 360] and vfov %g in (0, 180] degrees for an equirect camera", h, vf);
+      break;
+    default:
+      *why = formatted("no camera model %d", v.camera->model);
+  }
+  if (!why->empty()) return true;
+  if (v.rig && rigRefused(v.rig, why)) return true;
+  if (ctx.enable_low_pass_filter) {
+    *why = "the low-pass filter is not available for a camera view (set enable_low_pass_filter = 0)";
+    return true;
+  }
+  if (t360::kernelSizeOf(ctx.interpolation_alg) == 0) {
+    *why = formatted("no interpolation algorithm %d", static_cast<int>(ctx.interpolation_alg));
+    return true;
+  }
+  if (v.photometric) {
+    if (seamWidthRefused(v.seamWidth, why) || (v.seamWidth > 0.0f && featherRefused(*v.rig, v.seamWidth, why))) return true;
+    if (photometryRefused(*v.rig, v.photometry, why)) return true;
+  }
+  return v.minify && minifyRefused(v.minify, why);
+}
+
+// The per-frame constants of v's pose and camera (oriented_view.h: cameraConstants)
+t360::RectilinearCamera cameraConstants(const CameraView& v) {
+  return t360::cameraConstants(v.camera->model, v.camera->pannini, v.pose->yaw, v.pose->pitch, v.pose->roll, v.pose->hfov, v.pose->vfov);
 }
 
 // round(256 lodBias), half away from zero: the bias in 1/256 of a level
 int mipBias(const T360Minify& m) { return static_cast<int>(std::lround(256.0 * static_cast<double>(m.lodBias))); }
 
-// ---- camera views of a lens rig with photometry (T360B200_cameraPhotoMaps, T360B200_transformFrameCameraPhotoAsync;
-// oriented_view.h: cameraPhotoSample) ------------------------------------------------------------------------------------
-// true, with the reason in *why, when the view cannot be rendered: a NULL rig (the photometry is per lens), the camera
-// view's refusals with a rig, the photometric lens call's seam and photometry checks, and minifyRefused where minify is
-// not NULL (NULL: no pyramid)
-bool cameraPhotoRefused(const FrameTransformContext& ctx, const T360LensRig* rig, const T360RigPhotometry* ph, float seamWidth, const T360Pose* pose,
-                        const T360Camera* camera, const T360Minify* minify, std::string* why) {
-  if (!rig) {
-    *why = "a NULL rig (the photometry corrects a rig's lenses)";
-    return true;
-  }
-  if (cameraRefused(ctx, rig, pose, camera, why) || seamWidthRefused(seamWidth, why)) return true;
-  if (seamWidth > 0.0f && featherRefused(*rig, seamWidth, why)) return true;
-  return photometryRefused(*rig, ph, why) || (minify && minifyRefused(minify, why));
-}
-
-// ---- camera views of a stereo rig (T360B200_stereoCameraMaps, T360B200_transformFrameStereoCameraAsync; oriented_view.h:
-// cameraPhotoSample<MIP, true>) -------------------------------------------------------------------------------------------
-// true, with the reason in *why, when the view cannot be rendered: a NULL rig or one without two lenses (lens e is eye
-// e's), an output_stereo_format other than TB, LR or MONO, the camera view's refusals with the rig, the photometry's, and
-// minifyRefused where minify is not NULL.  (There is no seam: each eye takes its own lens.)
-bool stereoCameraRefused(const FrameTransformContext& ctx, const T360LensRig* rig, const T360RigPhotometry* ph, const T360Pose* pose,
-                         const T360Camera* camera, const T360Minify* minify, std::string* why) {
-  if (!rig) {
-    *why = "a NULL rig (a stereo rig's lenses are its eyes)";
-    return true;
-  }
-  if (rig->numLenses != 2) {
-    *why = formatted("numLenses %d: a stereo rig has two lenses, lens 0 the left eye's and lens 1 the right eye's", rig->numLenses);
-    return true;
-  }
-  const int sf = ctx.output_stereo_format;
-  if (sf != STEREO_FORMAT_TB && sf != STEREO_FORMAT_LR && sf != STEREO_FORMAT_MONO) {
-    *why = formatted("output_stereo_format %d (a stereo rig's views are LR, TB or MONO: eye 0 alone)", sf);
-    return true;
-  }
-  return cameraRefused(ctx, rig, pose, camera, why) || photometryRefused(*rig, ph, why) || (minify && minifyRefused(minify, why));
-}
-
-// The geometry of one plane of a camera view of a rig: rectilinearGeometry's (mono, no input eye re-pack) and, for a
-// stereo rig, the output eye split of ctx's output_stereo_format (whatever input_stereo_format says)
-t360::SphereGeometry rigViewGeometry(const FrameTransformContext& ctx, bool stereo, int inW, int inH, int outW, int outH) {
-  t360::SphereGeometry g = rectilinearGeometry(ctx, true, inW, inH, outW, outH);
-  if (stereo) {
+// The geometry of one outW x outH plane of an inW x inH input in view v: ctx's (its stereo formats and input layout,
+// cube-map input_expand_coef), or with a rig lensContext's (mono); a stereo rig's takes the output eye split of ctx's
+// output_stereo_format (whatever input_stereo_format says).  No tables.
+t360::SphereGeometry viewGeometry(const FrameTransformContext& ctx, const CameraView& v, int inW, int inH, int outW, int outH) {
+  t360::SphereGeometry g = t360::sphereGeometry(v.rig ? lensContext(ctx) : ctx, outW, outH, inW, inH, t360::kernelSizeOf(ctx.interpolation_alg));
+  if (v.stereo) {
     g.splitLR = ctx.output_stereo_format == STEREO_FORMAT_LR;
     g.splitTB = ctx.output_stereo_format == STEREO_FORMAT_TB;
   }
   return g;
 }
 
-// The host twin of one lens and plane of a camera view of a rig with photometry (STEREO = false, T360B200_cameraPhotoMaps;
-// lensWeight the seam weight) or of a stereo rig (STEREO = true, T360B200_stereoCameraMaps, seamWidth 0; lensWeight the eye
-// weight 256 e): cameraPhotoPoint<true, STEREO> of every pixel with both lenses projected.  The arguments are not refused.
-template <bool STEREO>
-void cameraPhotoTwin(const FrameTransformContext& ctx, const T360LensRig& rig, const T360RigPhotometry& photometry, float seamWidth,
-                     const T360Pose& pose, const T360Camera& camera, const T360Minify* minify, int lens, int plane, int inW, int inH, int outW,
-                     int outH, float* map0, float* map1, uint8_t* level, uint16_t* weight, uint16_t* gain, uint16_t* lensWeight) {
-  const t360::SphereGeometry g = rigViewGeometry(ctx, STEREO, inW, inH, outW, outH);
-  const t360::RectilinearCamera c = cameraConstants(pose, camera);
-  const t360::LensRigModel model = lensRigModel(rig);
-  const t360::MipGeometry m = t360::mipGeometry(g, minify ? minify->maxLevel : 0);
-  const int bias = minify ? mipBias(*minify) : 0;
-  const t360::LensPhotoPlane ph = lensPhotoPlane(photometry, rig.numLenses, plane);
-  const float s = seamWidth > 0.0f ? lensSeamScale(seamWidth) : 0.0f;
+// The host twin of the camera kernels for one outW x outH plane of an inW x inH input: point(g, c, model, m, bias, i, j,
+// i * outW + j) for every output pixel, with the geometry, camera constants (oriented_view.h: cameraConstants), rig model
+// (empty without a rig), footprint constants (maxLevel 0 without a minify) and bias those kernels get for ctx and v.  The
+// arguments are not refused.
+template <class Point>
+void forCameraPixels(const FrameTransformContext& ctx, const CameraView& v, int inW, int inH, int outW, int outH, Point&& point) {
+  const t360::SphereGeometry g = viewGeometry(ctx, v, inW, inH, outW, outH);
+  const t360::RectilinearCamera c = cameraConstants(v);
+  const t360::LensRigModel model = v.rig ? lensRigModel(*v.rig) : t360::LensRigModel{};
+  const t360::MipGeometry m = t360::mipGeometry(g, v.minify ? v.minify->maxLevel : 0);
+  const int bias = v.minify ? mipBias(*v.minify) : 0;
   for (int i = 0; i < outH; ++i)
-    for (int j = 0; j < outW; ++j) {
-      const size_t at = static_cast<size_t>(i) * outW + j;
-      t360::CameraPhotoLens e[2];
-      bool overlap;
-      lensWeight[at] = static_cast<uint16_t>(t360::cameraPhotoPoint<true, STEREO>(g, c, model, m, bias, s, /*both=*/true, ph, i, j, e, &overlap));
-      map0[2 * at] = e[lens].p0[0];
-      map0[2 * at + 1] = e[lens].p0[1];
-      map1[2 * at] = e[lens].p1[0];
-      map1[2 * at + 1] = e[lens].p1[1];
-      level[at] = static_cast<uint8_t>(e[lens].level);
-      weight[at] = static_cast<uint16_t>(e[lens].w);
-      gain[at] = static_cast<uint16_t>(e[lens].gain);
-    }
+    for (int j = 0; j < outW; ++j) point(g, c, model, m, bias, i, j, static_cast<size_t>(i) * outW + j);
+}
+
+// ---- the entry points' guards --------------------------------------------------------------------------------------------
+// true, with the reason in *why, when `name` (a lens or plane index) is outside 0..hi
+bool indexRefused(const char* name, int value, int hi, std::string* why) {
+  if (value >= 0 && value <= hi) return false;
+  *why = formatted("%s %d is outside 0..%d", name, value, hi);
+  return true;
+}
+
+// true, with `message` in *why, when an output array is NULL or a plane size is not positive
+bool outputsRefused(std::initializer_list<const void*> arrays, int inW, int inH, int outW, int outH, const char* message, std::string* why) {
+  if (std::find(arrays.begin(), arrays.end(), nullptr) == arrays.end() && inW > 0 && inH > 0 && outW > 0 && outH > 0) return false;
+  *why = message;
+  return true;
+}
+
+// A host twin: a NULL context, then refused(*ctx, &why) (the call's refusals, then its own array, size and index checks),
+// then body(*ctx).  0 and "<what>. Error: <why>" on stdout when refused, else 1.
+template <class Refused, class Body>
+int twinCall(const char* what, const FrameTransformContext* ctx, Refused&& refused, Body&& body) {
+  std::string why;
+  if (!ctx) why = "a NULL context";
+  else refused(*ctx, &why);
+  if (!why.empty()) {
+    std::printf("%s. Error: %s\n", what, why.c_str());
+    return 0;
+  }
+  body(*ctx);
+  return 1;
 }
 
 }  // namespace
@@ -1500,72 +1514,21 @@ class VideoFrameTransform {
     });
   }
 
-  // Whole frame of a camera view (T360B200_transformFrameCameraAsync, T360B200_transformFrameRectilinearAsync): one gather
-  // launch for all planes, every record computed by rectilinearSample (oriented_view.h), so a pose and camera give what
-  // cameraMap -> generateMapFromWarp plans for them.  rig == nullptr: the context's input under BORDER_WRAP; else the rig's
-  // lenses under BORDER_TRANSPARENT, with the lens call's pre-fill.  Needs no plan and leaves the plans alone; no tables.
-  bool transformFrameCamera(const char* what, const T360LensRig* rig, const T360Pose* pose, const T360Camera* camera, const FramePlanes& f,
-                            cudaStream_t stream) {
-    auto refused = [&](const FrameTransformContext& ctx, std::string* why) { return cameraRefused(ctx, rig, pose, camera, why); };
-    return unplannedFrame(what, stream, refused, [&](const FrameTransformContext& ctx, int, cudaStream_t s) {
-      t360::PerFrameGatherParams gp{};
-      gp.lens = rig != nullptr;
-      for (int p = 0; p < f.numPlanes; ++p) gp.plane[p].geometry = rectilinearGeometry(ctx, gp.lens, f.inW[p], f.inH[p], f.outW[p], f.outH[p]);
-      gp.camera = cameraConstants(*pose, *camera);
-      if (rig) gp.rig = lensRigModel(*rig);
-      perFrameGather(t360::PerFrameSource::kRectilinear, gp, ctx, f, f.in, f.inPitch, nullptr, gp.lens, nullptr, nullptr, nullptr, s);
-      return true;
-    });
-  }
-
-  // Whole frame of an anti-aliased camera view (T360B200_transformFrameCameraMipAsync): the pyramid of every plane, one
-  // launch per level over the planes that have it (buildPyramids), then one gather launch for all planes, every record
-  // computed by mipCameraSample (oriented_view.h), so a pose, camera and minify give what cameraMipMaps describes.  A frame
-  // whose planes all have top level 0 (maxLevel = 0, or planes too small for a level) is transformFrameCamera's.  Needs no
-  // plan and leaves the plans alone.
-  bool transformFrameCameraMip(const char* what, const T360LensRig* rig, const T360Pose* pose, const T360Camera* camera,
-                               const T360Minify* minify, const FramePlanes& f, cudaStream_t stream) {
-    std::string why;
-    if (minifyRefused(minify, &why)) {
-      std::printf("%s. Error: %s\n", what, why.c_str());
-      return false;
-    }
-    int topMax = 0;
-    for (int p = 0; p < f.numPlanes; ++p) topMax = std::max(topMax, t360::mipSizes(f.inW[p], f.inH[p], minify->maxLevel).top);
-    if (topMax == 0) return transformFrameCamera(what, rig, pose, camera, f, stream);
-    auto refused = [&](const FrameTransformContext& ctx, std::string* why) { return cameraRefused(ctx, rig, pose, camera, why); };
-    return unplannedFrame(what, stream, refused, [&](const FrameTransformContext& ctx, int, cudaStream_t s) {
-      t360::PerFrameGatherParams gp{};
-      gp.lens = rig != nullptr;
-      for (int p = 0; p < f.numPlanes; ++p) {
-        gp.plane[p].geometry = rectilinearGeometry(ctx, gp.lens, f.inW[p], f.inH[p], f.outW[p], f.outH[p]);
-        gp.mip[p].geometry = t360::mipGeometry(gp.plane[p].geometry, minify->maxLevel);
-      }
-      gp.camera = cameraConstants(*pose, *camera);
-      if (rig) gp.rig = lensRigModel(*rig);
-      gp.mipBias = mipBias(*minify);
-      UploadRing::Entry* staged = nullptr;
-      buildPyramids(f, gp, slotFor(s), s, &staged);
-      perFrameGather(t360::PerFrameSource::kCameraMip, gp, ctx, f, f.in, f.inPitch, nullptr, gp.lens, nullptr, nullptr, nullptr, s);
-      releaseAfter(staged, s);
-      return true;
-    });
-  }
-
-  // Whole frame of a camera view of a lens rig with photometry (T360B200_transformFrameCameraPhotoAsync) or, with stereo
-  // set, of a stereo rig (T360B200_transformFrameStereoCameraAsync, seamWidth 0): with a pyramid (minify not NULL and some
-  // plane's top level above 0) the planes' pyramids first (buildPyramids), then one gather launch for all planes, every
-  // record computed by cameraPhotoSample<MIP, stereo> (oriented_view.h), so a rig, photometry, seam, pose, camera and
-  // minify give what cameraPhotoMaps (stereoCameraMaps) describes.  With stats set (device, [numPlanes][6]) the overlap's
-  // sums are zeroed with a memset and accumulated by the same gather.  Needs no plan and leaves the plans alone; no tables.
-  bool transformFrameCameraPhoto(const char* what, bool stereo, const T360LensRig* rig, const T360RigPhotometry* photo, float seamWidth,
-                                 const T360Pose* pose, const T360Camera* camera, const T360Minify* minify, unsigned long long* stats,
-                                 const FramePlanes& f, cudaStream_t stream) {
+  // Whole frame of camera view v (the rectilinear, camera, camera-mip, camera-photo and stereo calls): one gather launch
+  // for all planes, every record computed by the chain of its source (oriented_view.h), so the view gives what its host
+  // twin describes.  The source follows from v:
+  //   - kRectilinear (rectilinearSample) without a photometry where no plane has a level above 0 (no minify, maxLevel 0,
+  //     or planes too small for a level): cameraMap -> generateMapFromWarp's frame;
+  //   - kCameraMip (mipCameraSample) without a photometry, after the planes' pyramids (buildPyramids);
+  //   - kCameraPhoto / kStereoCamera (cameraPhotoSample<MIP, stereo>) with one, after the pyramids when a plane has a
+  //     level, and with v.stats (device, [numPlanes][6]) the overlap's sums zeroed with a memset first and accumulated by
+  //     the same gather.
+  // rig == nullptr: the context's input under BORDER_WRAP; else the rig's lenses under BORDER_TRANSPARENT, with the lens
+  // call's pre-fill.  Needs no plan and leaves the plans alone; no tables.
+  bool transformFrameView(const char* what, const CameraView& v, const FramePlanes& f, cudaStream_t stream) {
     auto refused = [&](const FrameTransformContext& ctx, std::string* why) {
-      if (stereo ? stereoCameraRefused(ctx, rig, photo, pose, camera, minify, why)
-                 : cameraPhotoRefused(ctx, rig, photo, seamWidth, pose, camera, minify, why))
-        return true;
-      for (int p = 0; minify && minify->maxLevel > 0 && p < f.numPlanes; ++p)
+      if (viewRefused(ctx, v, why)) return true;
+      for (int p = 0; v.photometric && v.minify && v.minify->maxLevel > 0 && p < f.numPlanes; ++p)
         if (f.inW[p] > 2 * 65535 || f.inH[p] > 2 * 65535) {  // (CameraPhotoLevel keeps a level's sides in 16 bits)
           *why = formatted("input plane %d is %dx%d: a pyramid needs sides of at most 131070", p, f.inW[p], f.inH[p]);
           return true;
@@ -1573,32 +1536,42 @@ class VideoFrameTransform {
       return false;
     };
     return unplannedFrame(what, stream, refused, [&](const FrameTransformContext& ctx, int, cudaStream_t s) {
-      t360::PerFrameGatherParams gp{}, pyramids{};  // (pyramids: buildPyramids' levels, copied into gp.cameraPhoto)
-      t360::PerFrameGatherParams::CameraPhoto& cp = gp.cameraPhoto;
+      // (pyramids: the planes' footprint constants and buildPyramids' levels, copied into the source's member of gp's union)
+      t360::PerFrameGatherParams gp{}, pyramids{};
       int topMax = 0;
       for (int p = 0; p < f.numPlanes; ++p) {
-        gp.plane[p].geometry = rigViewGeometry(ctx, stereo, f.inW[p], f.inH[p], f.outW[p], f.outH[p]);
-        cp.mip[p].geometry = pyramids.mip[p].geometry = t360::mipGeometry(gp.plane[p].geometry, minify ? minify->maxLevel : 0);
-        topMax = std::max(topMax, cp.mip[p].geometry.top);
-        cp.photo.plane[p] = lensPhotoPlane(*photo, rig->numLenses, p);
+        gp.plane[p].geometry = viewGeometry(ctx, v, f.inW[p], f.inH[p], f.outW[p], f.outH[p]);
+        pyramids.mip[p].geometry = t360::mipGeometry(gp.plane[p].geometry, v.minify ? v.minify->maxLevel : 0);
+        topMax = std::max(topMax, pyramids.mip[p].geometry.top);
       }
-      gp.camera = cameraConstants(*pose, *camera);
-      gp.rig = lensRigModel(*rig);
-      if (seamWidth > 0.0f) gp.seamScale = lensSeamScale(seamWidth);
-      if (minify) gp.mipBias = mipBias(*minify);
-      cp.photo.stats = stats;
-      if (stats) CU(cudaMemsetAsync(stats, 0, sizeof(unsigned long long) * t360::kPhotoStats * f.numPlanes, s));
+      gp.lens = v.rig != nullptr;
+      gp.camera = cameraConstants(v);
+      if (v.rig) gp.rig = lensRigModel(*v.rig);
+      if (v.seamWidth > 0.0f) gp.seamScale = lensSeamScale(v.seamWidth);
+      if (v.minify) gp.mipBias = mipBias(*v.minify);
+      t360::PerFrameSource source = topMax > 0 ? t360::PerFrameSource::kCameraMip : t360::PerFrameSource::kRectilinear;
+      t360::PerFrameGatherParams::CameraPhoto& cp = gp.cameraPhoto;
+      if (v.photometric) {
+        source = v.stereo ? t360::PerFrameSource::kStereoCamera : t360::PerFrameSource::kCameraPhoto;
+        for (int p = 0; p < f.numPlanes; ++p) {
+          cp.mip[p].geometry = pyramids.mip[p].geometry;
+          cp.photo.plane[p] = lensPhotoPlane(*v.photometry, v.rig->numLenses, p);
+        }
+        cp.photo.stats = v.stats;
+        if (v.stats) CU(cudaMemsetAsync(v.stats, 0, sizeof(unsigned long long) * t360::kPhotoStats * f.numPlanes, s));
+      }
       UploadRing::Entry* staged = nullptr;
       if (topMax > 0) {
         buildPyramids(f, pyramids, slotFor(s), s, &staged);
-        for (int p = 0; p < f.numPlanes; ++p)
-          for (int l = 1; l <= cp.mip[p].geometry.top; ++l) {
+        for (int p = 0; p < f.numPlanes; ++p) {
+          if (!v.photometric) gp.mip[p] = pyramids.mip[p];
+          for (int l = 1; v.photometric && l <= cp.mip[p].geometry.top; ++l) {
             const t360::PerFrameGatherParams::MipLevel& L = pyramids.mip[p].level[l - 1];
             cp.mip[p].level[l - 1] = {L.bytes, L.pitch, static_cast<uint16_t>(L.w), static_cast<uint16_t>(L.h)};
           }
+        }
       }
-      perFrameGather(stereo ? t360::PerFrameSource::kStereoCamera : t360::PerFrameSource::kCameraPhoto, gp, ctx, f, f.in, f.inPitch, nullptr,
-                     /*transparent=*/true, nullptr, nullptr, nullptr, s);
+      perFrameGather(source, gp, ctx, f, f.in, f.inPitch, nullptr, gp.lens, nullptr, nullptr, nullptr, s);
       releaseAfter(staged, s);
       return true;
     });
@@ -3058,274 +3031,234 @@ T360_API int T360B200_remapFrameAsync(VideoFrameTransform* t, int numPlanes, con
   if (!describeFrame(what, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, f)) return 0;
   return t->remapFrame(maps, mapPitches, border, f, static_cast<cudaStream_t>(stream));
 }
-T360_API int T360B200_lensMap(const FrameTransformContext* ctx, const T360LensRig* rig, const T360Orientation* orientation, int inW, int inH,
-                              int outW, int outH, float* map) {
-  const char* what = "Could not compute the lens map";
-  std::string why;
-  if (!ctx) why = "a NULL context";
-  else if (lensRefused(*ctx, rig, orientation, &why)) {}
-  else if (!map || inW <= 0 || inH <= 0 || outW <= 0 || outH <= 0) why = "a NULL map or a plane size that is not positive";
-  if (!why.empty()) {
-    std::printf("%s. Error: %s\n", what, why.c_str());
+namespace {
+// A rig or camera frame call: a NULL transform, then the frame's arrays (describeFrame), then run(*t, f, stream).
+template <class Run>
+int frameCall(const char* what, VideoFrameTransform* t, int numPlanes, const uint8_t* const* dIn, uint8_t* const* dOut, const int* inW,
+              const int* inH, const int* inPitch, const int* outW, const int* outH, const int* outPitch, void* stream, Run&& run) {
+  if (!t) {
+    std::printf("%s. Error: a NULL argument\n", what);
     return 0;
   }
-  const t360::LensRigModel model = lensRigModel(*rig);
-  forLensPixels(*ctx, *orientation, inW, inH, outW, outH, [&](const t360::SphereGeometry& g, const t360::Rotation& r, const float* colTab,
-                                                              const float* rowTab, int i, int j, size_t at) {
-    t360::lensPoint(g, r, model, colTab, rowTab, i, j, map + 2 * at, map + 2 * at + 1);
+  FramePlanes f;
+  if (!describeFrame(what, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, f)) return 0;
+  return run(*t, f, static_cast<cudaStream_t>(stream));
+}
+}  // namespace
+T360_API int T360B200_lensMap(const FrameTransformContext* ctx, const T360LensRig* rig, const T360Orientation* orientation, int inW, int inH,
+                              int outW, int outH, float* map) {
+  auto refused = [&](const FrameTransformContext& c, std::string* why) {
+    return lensRefused(c, rig, orientation, why) ||
+           outputsRefused({map}, inW, inH, outW, outH, "a NULL map or a plane size that is not positive", why);
+  };
+  return twinCall("Could not compute the lens map", ctx, refused, [&](const FrameTransformContext& c) {
+    const t360::LensRigModel model = lensRigModel(*rig);
+    forLensPixels(c, *orientation, inW, inH, outW, outH, [&](const t360::SphereGeometry& g, const t360::Rotation& r, const float* colTab,
+                                                             const float* rowTab, int i, int j, size_t at) {
+      t360::lensPoint(g, r, model, colTab, rowTab, i, j, map + 2 * at, map + 2 * at + 1);
+    });
   });
-  return 1;
 }
 T360_API int T360B200_lensBlendMaps(const FrameTransformContext* ctx, const T360LensRig* rig, float seamWidth, const T360Orientation* orientation,
                                     int inW, int inH, int outW, int outH, float* map0, float* map1, uint16_t* weight) {
-  const char* what = "Could not compute the lens blend maps";
-  std::string why;
-  if (!ctx) why = "a NULL context";
-  else if (lensBlendRefused(*ctx, rig, seamWidth, orientation, &why)) {}
-  else if (!map0 || !map1 || !weight || inW <= 0 || inH <= 0 || outW <= 0 || outH <= 0)
-    why = "a NULL map or weight array or a plane size that is not positive";
-  if (!why.empty()) {
-    std::printf("%s. Error: %s\n", what, why.c_str());
-    return 0;
-  }
-  const t360::LensRigModel model = lensRigModel(*rig);
-  const float s = lensSeamScale(seamWidth);
-  forLensPixels(*ctx, *orientation, inW, inH, outW, outH, [&](const t360::SphereGeometry& g, const t360::Rotation& r, const float* colTab,
-                                                              const float* rowTab, int i, int j, size_t at) {
-    weight[at] = static_cast<uint16_t>(t360::lensBlendPoint(g, r, model, s, colTab, rowTab, i, j, map0 + 2 * at, map1 + 2 * at));
+  auto refused = [&](const FrameTransformContext& c, std::string* why) {
+    return lensBlendRefused(c, rig, seamWidth, orientation, why) ||
+           outputsRefused({map0, map1, weight}, inW, inH, outW, outH, "a NULL map or weight array or a plane size that is not positive", why);
+  };
+  return twinCall("Could not compute the lens blend maps", ctx, refused, [&](const FrameTransformContext& c) {
+    const t360::LensRigModel model = lensRigModel(*rig);
+    const float s = lensSeamScale(seamWidth);
+    forLensPixels(c, *orientation, inW, inH, outW, outH, [&](const t360::SphereGeometry& g, const t360::Rotation& r, const float* colTab,
+                                                             const float* rowTab, int i, int j, size_t at) {
+      weight[at] = static_cast<uint16_t>(t360::lensBlendPoint(g, r, model, s, colTab, rowTab, i, j, map0 + 2 * at, map1 + 2 * at));
+    });
   });
-  return 1;
 }
 T360_API int T360B200_transformFrameLensAsync(VideoFrameTransform* t, const T360LensRig* rig, const T360Orientation* orientation, int numPlanes,
                                               const uint8_t* const* dIn, uint8_t* const* dOut, const int* inW, const int* inH, const int* inPitch,
                                               const int* outW, const int* outH, const int* outPitch, void* stream) {
   const char* what = "Could not transform the frame with a lens rig";
-  if (!t) {
-    std::printf("%s. Error: a NULL argument\n", what);
-    return 0;
-  }
-  FramePlanes f;
-  if (!describeFrame(what, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, f)) return 0;
-  return t->transformFrameLens(what, rig, nullptr, orientation, f, static_cast<cudaStream_t>(stream));
+  return frameCall(what, t, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, stream,
+                   [&](VideoFrameTransform& vft, const FramePlanes& f, cudaStream_t s) { return vft.transformFrameLens(what, rig, nullptr, orientation, f, s); });
 }
 T360_API int T360B200_transformFrameLensBlendAsync(VideoFrameTransform* t, const T360LensRig* rig, float seamWidth, const T360Orientation* orientation,
                                                    int numPlanes, const uint8_t* const* dIn, uint8_t* const* dOut, const int* inW, const int* inH,
                                                    const int* inPitch, const int* outW, const int* outH, const int* outPitch, void* stream) {
   const char* what = "Could not blend the frame of a lens rig";
-  if (!t) {
-    std::printf("%s. Error: a NULL argument\n", what);
-    return 0;
-  }
-  FramePlanes f;
-  if (!describeFrame(what, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, f)) return 0;
-  return t->transformFrameLens(what, rig, &seamWidth, orientation, f, static_cast<cudaStream_t>(stream));
+  return frameCall(what, t, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, stream,
+                   [&](VideoFrameTransform& vft, const FramePlanes& f, cudaStream_t s) { return vft.transformFrameLens(what, rig, &seamWidth, orientation, f, s); });
 }
 T360_API int T360B200_lensPhotoMaps(const FrameTransformContext* ctx, const T360LensRig* rig, const T360RigPhotometry* photometry, float seamWidth,
                                     const T360Orientation* orientation, int plane, int inW, int inH, int outW, int outH, float* map0, float* map1,
                                     uint16_t* weight, uint16_t* gain0, uint16_t* gain1) {
-  const char* what = "Could not compute the lens photometry maps";
-  std::string why;
-  if (!ctx) why = "a NULL context";
-  else if (lensPhotoRefused(*ctx, rig, photometry, seamWidth, orientation, &why)) {}
-  else if (plane < 0 || plane > 2) why = formatted("plane %d is outside 0..2", plane);
-  else if (!map0 || !map1 || !weight || !gain0 || !gain1 || inW <= 0 || inH <= 0 || outW <= 0 || outH <= 0)
-    why = "a NULL map, weight or gain array or a plane size that is not positive";
-  if (!why.empty()) {
-    std::printf("%s. Error: %s\n", what, why.c_str());
-    return 0;
-  }
-  const t360::LensRigModel model = lensRigModel(*rig);
-  const t360::LensPhotoPlane c = lensPhotoPlane(*photometry, rig->numLenses, plane);
-  const float s = seamWidth > 0.0f ? lensSeamScale(seamWidth) : 0.0f;
-  forLensPixels(*ctx, *orientation, inW, inH, outW, outH, [&](const t360::SphereGeometry& g, const t360::Rotation& r, const float* colTab,
-                                                              const float* rowTab, int i, int j, size_t at) {
-    int g0, g1;
-    bool overlap;
-    weight[at] = static_cast<uint16_t>(
-        t360::lensPhotoPoint(g, r, model, s, /*both=*/true, c, colTab, rowTab, i, j, map0 + 2 * at, map1 + 2 * at, &g0, &g1, &overlap));
-    gain0[at] = static_cast<uint16_t>(g0);
-    gain1[at] = static_cast<uint16_t>(g1);
+  auto refused = [&](const FrameTransformContext& c, std::string* why) {
+    return lensPhotoRefused(c, rig, photometry, seamWidth, orientation, why) || indexRefused("plane", plane, 2, why) ||
+           outputsRefused({map0, map1, weight, gain0, gain1}, inW, inH, outW, outH,
+                          "a NULL map, weight or gain array or a plane size that is not positive", why);
+  };
+  return twinCall("Could not compute the lens photometry maps", ctx, refused, [&](const FrameTransformContext& c) {
+    const t360::LensRigModel model = lensRigModel(*rig);
+    const t360::LensPhotoPlane ph = lensPhotoPlane(*photometry, rig->numLenses, plane);
+    const float s = seamWidth > 0.0f ? lensSeamScale(seamWidth) : 0.0f;
+    forLensPixels(c, *orientation, inW, inH, outW, outH, [&](const t360::SphereGeometry& g, const t360::Rotation& r, const float* colTab,
+                                                             const float* rowTab, int i, int j, size_t at) {
+      int g0, g1;
+      bool overlap;
+      weight[at] = static_cast<uint16_t>(
+          t360::lensPhotoPoint(g, r, model, s, /*both=*/true, ph, colTab, rowTab, i, j, map0 + 2 * at, map1 + 2 * at, &g0, &g1, &overlap));
+      gain0[at] = static_cast<uint16_t>(g0);
+      gain1[at] = static_cast<uint16_t>(g1);
+    });
   });
-  return 1;
 }
 T360_API int T360B200_transformFrameLensPhotoAsync(VideoFrameTransform* t, const T360LensRig* rig, const T360RigPhotometry* photometry,
                                                    float seamWidth, const T360Orientation* orientation, unsigned long long* deviceStats,
                                                    int numPlanes, const uint8_t* const* dIn, uint8_t* const* dOut, const int* inW, const int* inH,
                                                    const int* inPitch, const int* outW, const int* outH, const int* outPitch, void* stream) {
   const char* what = "Could not transform the frame of a lens rig with photometry";
-  if (!t) {
-    std::printf("%s. Error: a NULL argument\n", what);
-    return 0;
-  }
-  if (!photometry) {  // (checked here: without a photometry transformFrameLens is the plain lens call)
+  if (t && !photometry) {  // (before the frame's checks: without a photometry transformFrameLens is the plain lens call)
     std::printf("%s. Error: a NULL photometry\n", what);
     return 0;
   }
-  FramePlanes f;
-  if (!describeFrame(what, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, f)) return 0;
-  return t->transformFrameLens(what, rig, &seamWidth, orientation, f, static_cast<cudaStream_t>(stream), photometry, deviceStats);
+  return frameCall(what, t, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, stream,
+                   [&](VideoFrameTransform& vft, const FramePlanes& f, cudaStream_t s) {
+                     return vft.transformFrameLens(what, rig, &seamWidth, orientation, f, s, photometry, deviceStats);
+                   });
 }
 namespace {
-int cameraMap(const char* what, const FrameTransformContext* ctx, const T360LensRig* rig, const T360Pose* pose, const T360Camera* camera,
-              int inW, int inH, int outW, int outH, float* map) {
-  std::string why;
-  if (!ctx) why = "a NULL context";
-  else if (cameraRefused(*ctx, rig, pose, camera, &why)) {}
-  else if (!map || inW <= 0 || inH <= 0 || outW <= 0 || outH <= 0) why = "a NULL map or a plane size that is not positive";
-  if (!why.empty()) {
-    std::printf("%s. Error: %s\n", what, why.c_str());
-    return 0;
-  }
-  const t360::SphereGeometry g = rectilinearGeometry(*ctx, rig != nullptr, inW, inH, outW, outH);
-  const t360::RectilinearCamera c = cameraConstants(*pose, *camera);
-  const t360::LensRigModel model = rig ? lensRigModel(*rig) : t360::LensRigModel{};
-  for (int i = 0; i < outH; ++i)
-    for (int j = 0; j < outW; ++j) {
-      float* at = map + 2 * (static_cast<size_t>(i) * outW + j);
-      if (rig) t360::rectilinearPosition<true>(g, c, model, i, j, at, at + 1);
-      else t360::rectilinearPosition<false>(g, c, model, i, j, at, at + 1);
-    }
-  return 1;
+int cameraMap(const char* what, const FrameTransformContext* ctx, const CameraView& v, int inW, int inH, int outW, int outH, float* map) {
+  auto refused = [&](const FrameTransformContext& c, std::string* why) {
+    return viewRefused(c, v, why) || outputsRefused({map}, inW, inH, outW, outH, "a NULL map or a plane size that is not positive", why);
+  };
+  return twinCall(what, ctx, refused, [&](const FrameTransformContext& c) {
+    forCameraPixels(c, v, inW, inH, outW, outH, [&](const t360::SphereGeometry& g, const t360::RectilinearCamera& cam, const t360::LensRigModel& model,
+                                                    const t360::MipGeometry&, int, int i, int j, size_t at) {
+      if (v.rig) t360::rectilinearPosition<true>(g, cam, model, i, j, map + 2 * at, map + 2 * at + 1);
+      else t360::rectilinearPosition<false>(g, cam, model, i, j, map + 2 * at, map + 2 * at + 1);
+    });
+  });
 }
-int transformFrameCamera(const char* what, VideoFrameTransform* t, const T360LensRig* rig, const T360Pose* pose, const T360Camera* camera,
-                         int numPlanes, const uint8_t* const* dIn, uint8_t* const* dOut, const int* inW, const int* inH, const int* inPitch,
-                         const int* outW, const int* outH, const int* outPitch, void* stream) {
-  if (!t) {
-    std::printf("%s. Error: a NULL argument\n", what);
-    return 0;
-  }
-  FramePlanes f;
-  if (!describeFrame(what, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, f)) return 0;
-  return t->transformFrameCamera(what, rig, pose, camera, f, static_cast<cudaStream_t>(stream));
+// The twin of one lens and plane of a photometric (cameraPhotoMaps) or stereo (stereoCameraMaps) view:
+// cameraPhotoPoint<true, stereo> of every pixel with both lenses projected; lensWeight the seam weight or the eye weight
+// 256 e
+int cameraPhotoMaps(const char* what, const FrameTransformContext* ctx, const CameraView& v, int lens, int plane, int inW, int inH, int outW,
+                    int outH, float* map0, float* map1, uint8_t* level, uint16_t* weight, uint16_t* gain, uint16_t* lensWeight) {
+  auto refused = [&](const FrameTransformContext& c, std::string* why) {
+    return viewRefused(c, v, why) || indexRefused("lens", lens, 1, why) || indexRefused("plane", plane, 2, why) ||
+           outputsRefused({map0, map1, level, weight, gain, lensWeight}, inW, inH, outW, outH,
+                          "a NULL map, level, weight or gain array or a plane size that is not positive", why);
+  };
+  return twinCall(what, ctx, refused, [&](const FrameTransformContext& c) {
+    const t360::LensPhotoPlane ph = lensPhotoPlane(*v.photometry, v.rig->numLenses, plane);
+    const float s = v.seamWidth > 0.0f ? lensSeamScale(v.seamWidth) : 0.0f;
+    forCameraPixels(c, v, inW, inH, outW, outH, [&](const t360::SphereGeometry& g, const t360::RectilinearCamera& cam, const t360::LensRigModel& model,
+                                                    const t360::MipGeometry& m, int bias, int i, int j, size_t at) {
+      t360::CameraPhotoLens e[2];
+      bool overlap;
+      lensWeight[at] = static_cast<uint16_t>(v.stereo ? t360::cameraPhotoPoint<true, true>(g, cam, model, m, bias, s, /*both=*/true, ph, i, j, e, &overlap)
+                                                      : t360::cameraPhotoPoint<true>(g, cam, model, m, bias, s, /*both=*/true, ph, i, j, e, &overlap));
+      map0[2 * at] = e[lens].p0[0];
+      map0[2 * at + 1] = e[lens].p0[1];
+      map1[2 * at] = e[lens].p1[0];
+      map1[2 * at + 1] = e[lens].p1[1];
+      level[at] = static_cast<uint8_t>(e[lens].level);
+      weight[at] = static_cast<uint16_t>(e[lens].w);
+      gain[at] = static_cast<uint16_t>(e[lens].gain);
+    });
+  });
+}
+int transformFrameView(const char* what, VideoFrameTransform* t, const CameraView& v, int numPlanes, const uint8_t* const* dIn, uint8_t* const* dOut,
+                       const int* inW, const int* inH, const int* inPitch, const int* outW, const int* outH, const int* outPitch, void* stream) {
+  return frameCall(what, t, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, stream,
+                   [&](VideoFrameTransform& vft, const FramePlanes& f, cudaStream_t s) { return vft.transformFrameView(what, v, f, s); });
 }
 }  // namespace
 T360_API int T360B200_cameraMap(const FrameTransformContext* ctx, const T360LensRig* rig, const T360Pose* pose, const T360Camera* camera, int inW,
                                 int inH, int outW, int outH, float* map) {
-  return cameraMap("Could not compute the camera map", ctx, rig, pose, camera, inW, inH, outW, outH, map);
+  return cameraMap("Could not compute the camera map", ctx, plainView(rig, pose, camera), inW, inH, outW, outH, map);
 }
 T360_API int T360B200_transformFrameCameraAsync(VideoFrameTransform* t, const T360LensRig* rig, const T360Pose* pose, const T360Camera* camera,
                                                 int numPlanes, const uint8_t* const* dIn, uint8_t* const* dOut, const int* inW, const int* inH,
                                                 const int* inPitch, const int* outW, const int* outH, const int* outPitch, void* stream) {
-  return transformFrameCamera("Could not transform the frame with a camera view", t, rig, pose, camera, numPlanes, dIn, dOut, inW, inH, inPitch,
-                              outW, outH, outPitch, stream);
+  return transformFrameView("Could not transform the frame with a camera view", t, plainView(rig, pose, camera), numPlanes, dIn,
+                            dOut, inW, inH, inPitch, outW, outH, outPitch, stream);
 }
 T360_API int T360B200_rectilinearMap(const FrameTransformContext* ctx, const T360LensRig* rig, const T360Pose* pose, int inW, int inH, int outW,
                                      int outH, float* map) {
-  return cameraMap("Could not compute the rectilinear map", ctx, rig, pose, &kPinhole, inW, inH, outW, outH, map);
+  return cameraMap("Could not compute the rectilinear map", ctx, plainView(rig, pose, &kPinhole), inW, inH, outW, outH, map);
 }
 T360_API int T360B200_transformFrameRectilinearAsync(VideoFrameTransform* t, const T360LensRig* rig, const T360Pose* pose, int numPlanes,
                                                      const uint8_t* const* dIn, uint8_t* const* dOut, const int* inW, const int* inH,
                                                      const int* inPitch, const int* outW, const int* outH, const int* outPitch, void* stream) {
-  return transformFrameCamera("Could not transform the frame with a rectilinear view", t, rig, pose, &kPinhole, numPlanes, dIn, dOut, inW, inH,
-                              inPitch, outW, outH, outPitch, stream);
+  return transformFrameView("Could not transform the frame with a rectilinear view", t, plainView(rig, pose, &kPinhole), numPlanes,
+                            dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, stream);
 }
 T360_API int T360B200_cameraMipMaps(const FrameTransformContext* ctx, const T360LensRig* rig, const T360Pose* pose, const T360Camera* camera,
                                     const T360Minify* minify, int inW, int inH, int outW, int outH, float* map0, float* map1, uint8_t* level,
                                     uint16_t* weight) {
-  const char* what = "Could not compute the camera mip maps";
-  std::string why;
-  if (!ctx) why = "a NULL context";
-  else if (cameraMipRefused(*ctx, rig, pose, camera, minify, &why)) {}
-  else if (!map0 || !map1 || !level || !weight || inW <= 0 || inH <= 0 || outW <= 0 || outH <= 0)
-    why = "a NULL map, level or weight array or a plane size that is not positive";
-  if (!why.empty()) {
-    std::printf("%s. Error: %s\n", what, why.c_str());
-    return 0;
-  }
-  const t360::SphereGeometry g = rectilinearGeometry(*ctx, rig != nullptr, inW, inH, outW, outH);
-  const t360::RectilinearCamera c = cameraConstants(*pose, *camera);
-  const t360::LensRigModel model = rig ? lensRigModel(*rig) : t360::LensRigModel{};
-  const t360::MipGeometry m = t360::mipGeometry(g, minify->maxLevel);
-  const int bias = mipBias(*minify);
-  for (int i = 0; i < outH; ++i)
-    for (int j = 0; j < outW; ++j) {
-      const size_t at = static_cast<size_t>(i) * outW + j;
+  const CameraView v = plainView(rig, pose, camera, minify);
+  auto refused = [&](const FrameTransformContext& c, std::string* why) {
+    return viewRefused(c, v, why) || (!minify && minifyRefused(minify, why)) ||
+           outputsRefused({map0, map1, level, weight}, inW, inH, outW, outH, "a NULL map, level or weight array or a plane size that is not positive",
+                          why);
+  };
+  return twinCall("Could not compute the camera mip maps", ctx, refused, [&](const FrameTransformContext& c) {
+    forCameraPixels(c, v, inW, inH, outW, outH, [&](const t360::SphereGeometry& g, const t360::RectilinearCamera& cam, const t360::LensRigModel& model,
+                                                    const t360::MipGeometry& m, int bias, int i, int j, size_t at) {
       int w;
-      level[at] = static_cast<uint8_t>(rig ? t360::mipCameraPoint<true>(g, c, model, m, bias, i, j, map0 + 2 * at, map1 + 2 * at, &w)
-                                           : t360::mipCameraPoint<false>(g, c, model, m, bias, i, j, map0 + 2 * at, map1 + 2 * at, &w));
+      level[at] = static_cast<uint8_t>(rig ? t360::mipCameraPoint<true>(g, cam, model, m, bias, i, j, map0 + 2 * at, map1 + 2 * at, &w)
+                                           : t360::mipCameraPoint<false>(g, cam, model, m, bias, i, j, map0 + 2 * at, map1 + 2 * at, &w));
       weight[at] = static_cast<uint16_t>(w);
-    }
-  return 1;
+    });
+  });
 }
 T360_API int T360B200_transformFrameCameraMipAsync(VideoFrameTransform* t, const T360LensRig* rig, const T360Pose* pose, const T360Camera* camera,
                                                    const T360Minify* minify, int numPlanes, const uint8_t* const* dIn, uint8_t* const* dOut,
                                                    const int* inW, const int* inH, const int* inPitch, const int* outW, const int* outH,
                                                    const int* outPitch, void* stream) {
   const char* what = "Could not transform the frame with an anti-aliased camera view";
-  if (!t) {
-    std::printf("%s. Error: a NULL argument\n", what);
-    return 0;
-  }
-  FramePlanes f;
-  if (!describeFrame(what, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, f)) return 0;
-  return t->transformFrameCameraMip(what, rig, pose, camera, minify, f, static_cast<cudaStream_t>(stream));
+  return frameCall(what, t, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, stream,
+                   [&](VideoFrameTransform& vft, const FramePlanes& f, cudaStream_t s) {
+                     std::string why;
+                     if (minifyRefused(minify, &why)) {  // (this call checks its minify before the pose and camera)
+                       std::printf("%s. Error: %s\n", what, why.c_str());
+                       return false;
+                     }
+                     return vft.transformFrameView(what, plainView(rig, pose, camera, minify), f, s);
+                   });
 }
 T360_API int T360B200_cameraPhotoMaps(const FrameTransformContext* ctx, const T360LensRig* rig, const T360RigPhotometry* photometry, float seamWidth,
                                       const T360Pose* pose, const T360Camera* camera, const T360Minify* minify, int lens, int plane, int inW,
                                       int inH, int outW, int outH, float* map0, float* map1, uint8_t* level, uint16_t* weight, uint16_t* gain,
                                       uint16_t* seamWeight) {
-  const char* what = "Could not compute the camera photometry maps";
-  std::string why;
-  if (!ctx) why = "a NULL context";
-  else if (cameraPhotoRefused(*ctx, rig, photometry, seamWidth, pose, camera, minify, &why)) {}
-  else if (lens < 0 || lens > 1) why = formatted("lens %d is outside 0..1", lens);
-  else if (plane < 0 || plane > 2) why = formatted("plane %d is outside 0..2", plane);
-  else if (!map0 || !map1 || !level || !weight || !gain || !seamWeight || inW <= 0 || inH <= 0 || outW <= 0 || outH <= 0)
-    why = "a NULL map, level, weight or gain array or a plane size that is not positive";
-  if (!why.empty()) {
-    std::printf("%s. Error: %s\n", what, why.c_str());
-    return 0;
-  }
-  cameraPhotoTwin<false>(*ctx, *rig, *photometry, seamWidth, *pose, *camera, minify, lens, plane, inW, inH, outW, outH, map0, map1, level, weight,
-                         gain, seamWeight);
-  return 1;
+  return cameraPhotoMaps("Could not compute the camera photometry maps", ctx,
+                         photoView(rig, photometry, seamWidth, pose, camera, minify, nullptr, false),
+                         lens, plane, inW, inH, outW, outH, map0, map1, level, weight, gain, seamWeight);
 }
 T360_API int T360B200_transformFrameCameraPhotoAsync(VideoFrameTransform* t, const T360LensRig* rig, const T360RigPhotometry* photometry,
                                                      float seamWidth, const T360Pose* pose, const T360Camera* camera, const T360Minify* minify,
                                                      unsigned long long* deviceStats, int numPlanes, const uint8_t* const* dIn,
                                                      uint8_t* const* dOut, const int* inW, const int* inH, const int* inPitch, const int* outW,
                                                      const int* outH, const int* outPitch, void* stream) {
-  const char* what = "Could not transform the frame with a camera view of a lens rig with photometry";
-  if (!t) {
-    std::printf("%s. Error: a NULL argument\n", what);
-    return 0;
-  }
-  FramePlanes f;
-  if (!describeFrame(what, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, f)) return 0;
-  return t->transformFrameCameraPhoto(what, false, rig, photometry, seamWidth, pose, camera, minify, deviceStats, f, static_cast<cudaStream_t>(stream));
+  return transformFrameView("Could not transform the frame with a camera view of a lens rig with photometry", t,
+                            photoView(rig, photometry, seamWidth, pose, camera, minify, deviceStats, false),
+                            numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, stream);
 }
 T360_API int T360B200_stereoCameraMaps(const FrameTransformContext* ctx, const T360LensRig* rig, const T360RigPhotometry* photometry, const T360Pose* pose,
                                        const T360Camera* camera, const T360Minify* minify, int lens, int plane, int inW, int inH, int outW, int outH,
                                        float* map0, float* map1, uint8_t* level, uint16_t* weight, uint16_t* gain, uint16_t* eyeWeight) {
-  const char* what = "Could not compute the stereo camera maps";
-  std::string why;
-  if (!ctx) why = "a NULL context";
-  else if (stereoCameraRefused(*ctx, rig, photometry, pose, camera, minify, &why)) {}
-  else if (lens < 0 || lens > 1) why = formatted("lens %d is outside 0..1", lens);
-  else if (plane < 0 || plane > 2) why = formatted("plane %d is outside 0..2", plane);
-  else if (!map0 || !map1 || !level || !weight || !gain || !eyeWeight || inW <= 0 || inH <= 0 || outW <= 0 || outH <= 0)
-    why = "a NULL map, level, weight or gain array or a plane size that is not positive";
-  if (!why.empty()) {
-    std::printf("%s. Error: %s\n", what, why.c_str());
-    return 0;
-  }
-  cameraPhotoTwin<true>(*ctx, *rig, *photometry, 0.0f, *pose, *camera, minify, lens, plane, inW, inH, outW, outH, map0, map1, level, weight, gain,
-                        eyeWeight);
-  return 1;
+  return cameraPhotoMaps("Could not compute the stereo camera maps", ctx,
+                         photoView(rig, photometry, 0.0f, pose, camera, minify, nullptr, true),
+                         lens, plane, inW, inH, outW, outH, map0, map1, level, weight, gain, eyeWeight);
 }
 T360_API int T360B200_transformFrameStereoCameraAsync(VideoFrameTransform* t, const T360LensRig* rig, const T360RigPhotometry* photometry,
                                                       const T360Pose* pose, const T360Camera* camera, const T360Minify* minify,
                                                       unsigned long long* deviceStats, int numPlanes, const uint8_t* const* dIn,
                                                       uint8_t* const* dOut, const int* inW, const int* inH, const int* inPitch, const int* outW,
                                                       const int* outH, const int* outPitch, void* stream) {
-  const char* what = "Could not transform the frame with a camera view of a stereo rig";
-  if (!t) {
-    std::printf("%s. Error: a NULL argument\n", what);
-    return 0;
-  }
-  FramePlanes f;
-  if (!describeFrame(what, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, f)) return 0;
-  return t->transformFrameCameraPhoto(what, true, rig, photometry, 0.0f, pose, camera, minify, deviceStats, f, static_cast<cudaStream_t>(stream));
+  return transformFrameView("Could not transform the frame with a camera view of a stereo rig", t,
+                            photoView(rig, photometry, 0.0f, pose, camera, minify, deviceStats, true),
+                            numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, stream);
 }
 T360_API void T360B200_setPinHostPlanes(VideoFrameTransform* t, int enable) { if (t) t->setPinHostPlanes(enable != 0); }
 T360_API void T360B200_debugTrace(VideoFrameTransform* t, int enable) { if (t) t->enableTrace(enable != 0); }
