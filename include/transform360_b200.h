@@ -55,6 +55,19 @@ int T360B200_hostPlanGather(T360HostPlan* plan, int info[10], const int32_t** jo
  * Returns 1 on success; the pointers stay valid until T360B200_hostPlanDestroy. */
 int T360B200_hostPlanPoleCaps(T360HostPlan* plan, int info[4], const int32_t** capJobs, const uint32_t** capRecords,
                               const int32_t** launchJobs);
+/* Per job of the launch list of T360B200_hostPlanPoleCaps, what the planner records for streaming a host plane through the
+ * device: *needRows = the source rows [0, n) the job reads (the whole plane if a window wraps vertically), *rects = the
+ * bounding rectangle {x0, y0, x1, y1} (exclusive ends) of the output pixels it writes.  *numJobs = launch jobs.  Returns 1
+ * on success; the pointers stay valid until T360B200_hostPlanDestroy. */
+int T360B200_hostPlanLaunchExtents(T360HostPlan* plan, int* numJobs, const int32_t** needRows, const int32_t** rects);
+/* The schedule the synchronous host-pointer call streams a large plane with (csrc/gather_plan.h: scheduleWaves), for
+ * `chunks` input row bands (0: as many as the call takes for the plan's input size).  needRows: per launch job, in place of
+ * the planner's (NULL: the planner's).  info = {chunks, launch jobs, rectangles}; *chunkRowEnd: per chunk the end of the
+ * rows delivered with it; *waveStart: chunks + 1 entries, wave c = (*order)[waveStart[c] .. waveStart[c + 1]); *order: the
+ * launch-job indices wave by wave; *rects: per output rectangle {wave it is copied back after, x0, y0, x1, y1}.  Returns 1
+ * on success; the pointers stay valid until the next call with this plan or its T360B200_hostPlanDestroy. */
+int T360B200_hostPlanWaves(T360HostPlan* plan, int chunks, const int32_t* needRows, int info[3], const int32_t** chunkRowEnd,
+                           const int32_t** waveStart, const int32_t** order, const int32_t** rects);
 /* The job list and record buffer the frame kernel reads (csrc/gather_plan.h: deviceJobs, deviceRecords): the launch list
  * of T360B200_hostPlanPoleCaps with the width of each class-0 source box (csrc/kernels.cuh: class0BoxW) in bits 28-31
  * of recordOffset, and the compact records followed by the pole-cap records, the window offsets of a job with a narrow

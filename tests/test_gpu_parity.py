@@ -583,29 +583,6 @@ def test_random_contexts_product_vs_oracle(torch_cuda):
     assert checked >= 200, (checked, refused)
 
 
-@pytest.mark.parametrize("name", ["cube_cubic", "cube_linear", "cube_lanczos", "rotated", "eac_mono_cubic", "cube_to_equirect", "cube_cubic_odd"])
-def test_streamed_host_path_on_small_planes(name, torch_cuda, monkeypatch):
-    """Large host planes are streamed through the device in row bands (chunked H2D || gather waves || D2H of finished
-    rectangles).  T360B200_PIPELINE_MIN_BYTES=0 sends small planes down that path too: same bytes as the oracle."""
-    monkeypatch.setenv("T360B200_PIPELINE_MIN_BYTES", "0")
-    case = SMALL[name]
-    ctx, octx = _ctxs(case)
-    with t360.VideoFrameTransform(ctx) as vft:
-        for idx in (0, 1):
-            iw, ih, ow, oh, _ = plane_dims(case, idx)
-            assert vft.generateMapForPlane(iw, ih, ow, oh, idx)
-        for plane in (0, 1, 2):
-            iw, ih, ow, oh, idx = plane_dims(case, plane)
-            plan = co.OraclePlan(octx, iw, ih, ow, oh)
-            for frame in (0, 1):
-                src = co.noise_plane(iw, ih, plane=plane, frame=frame, pitch=iw + 5)
-                out = np.full((oh, ow + 3), 0x5A, np.uint8)
-                assert vft.transformFramePlane(src.ctypes.data, out.ctypes.data, iw, ih, src.strides[0], ow, oh, out.strides[0], idx, plane)
-                want = co.transform_plane(octx, plan, np.ascontiguousarray(src[:, :iw]), ow, oh, map_index=idx)
-                assert np.array_equal(out[:, :ow], want), f"{name} plane {plane} frame {frame}: {(out[:, :ow] != want).sum()} px differ"
-                assert (out[:, ow:] == 0x5A).all()
-
-
 def test_concurrent_calls_on_different_planes(torch_cuda):
     """The reference object is safe for concurrent transformFramePlane calls on different planes after init
     (VideoFrameTransform.h:150-159: read-only maps); three host threads, one plane each, several frames."""

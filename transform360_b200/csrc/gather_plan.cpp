@@ -708,6 +708,47 @@ void buildGatherPlan(const HostPlan& h, bool stageTiles, GatherPlan& g) {
   if (offset / 16 > static_cast<size_t>(kJobRecordMask)) throw std::invalid_argument("gather plan: too many sampling records");
 }
 
+int pipelineChunks(int inW, int inH) {
+  const long long bytes = static_cast<long long>(inW) * inH;
+  return static_cast<int>(std::min<long long>(8, std::max<long long>(2, bytes / (3ll << 20))));
+}
+
+WaveSchedule scheduleWaves(const std::vector<int>& needRows, const std::vector<JobRect>& rects, int inH, int mapW, int mapH, int chunks) {
+  WaveSchedule w;
+  const int rowsPer = ((inH + chunks - 1) / chunks + 7) & ~7;
+  w.chunkRowEnd.assign(chunks, inH);
+  for (int c = 0; c < chunks; ++c) w.chunkRowEnd[c] = std::min(inH, (c + 1) * rowsPer);
+  auto waveOf = [&](int rows) {
+    int c = 0;
+    while (c + 1 < chunks && w.chunkRowEnd[c] < rows) ++c;
+    return c;
+  };
+  std::vector<std::vector<int>> byWave(chunks);
+  const int bands = (mapH + 31) / 32;
+  std::vector<int> complete(bands, 0);  // per band: the wave after which it is complete
+  for (size_t i = 0; i < needRows.size(); ++i) {
+    const int c = waveOf(needRows[i]);
+    byWave[c].push_back(static_cast<int>(i));
+    const JobRect& r = rects[i];
+    for (int band = r.y0 / 32; band <= (r.y1 - 1) / 32; ++band) complete[band] = std::max(complete[band], c);
+  }
+  w.waveStart.assign(chunks + 1, 0);
+  for (int c = 0; c < chunks; ++c) {
+    w.waveStart[c] = static_cast<int>(w.order.size());
+    w.order.insert(w.order.end(), byWave[c].begin(), byWave[c].end());
+  }
+  w.waveStart[chunks] = static_cast<int>(w.order.size());
+  w.rects.assign(chunks, {});
+  for (int band = 0; band < bands;) {  // adjacent bands that complete together: one copy
+    const int c = complete[band];
+    int end = band + 1;
+    while (end < bands && complete[end] == c) ++end;
+    w.rects[c].push_back(JobRect{0, band * 32, mapW, std::min(mapH, end * 32)});
+    band = end;
+  }
+  return w;
+}
+
 std::vector<GatherJob> deviceJobs(const GatherPlan& g) {
   std::vector<GatherJob> out(g.launchJobs);
   for (size_t i = 0; i < out.size(); ++i) out[i].recordOffset |= static_cast<int>(g.launchBoxWidths[i]) << kJobWidthShift;

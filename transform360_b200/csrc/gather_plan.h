@@ -68,6 +68,23 @@ inline int jobLaunchRank(const GatherJob& job) {
 }
 
 
+// Streaming a large host plane through the device (the synchronous host-pointer call): the input arrives in `chunks` row
+// bands of one size, rounded up to 8 rows; wave c is one frame-kernel launch of the launch jobs whose source rows
+// [0, needRows) have all arrived with chunk c (launch order kept inside a wave); the output goes back in 32-row bands of
+// the full width, each after the last wave that writes into it (adjacent bands that complete together: one rectangle).
+// Contiguous bands, not per-job rectangles: a band split into the faces of a cube-map row would finish earlier per face,
+// but strided rectangle copies are much slower than whole contiguous bands.
+struct WaveSchedule {
+  std::vector<int> chunkRowEnd;             // per chunk: rows [0, end) have arrived after it (trailing chunks may be empty)
+  std::vector<int> order;                   // the launch jobs, wave by wave
+  std::vector<int> waveStart;               // chunks + 1 entries: wave c is order[waveStart[c] .. waveStart[c + 1])
+  std::vector<std::vector<JobRect>> rects;  // per wave: the output rectangles copied back after it
+};
+// How many row bands a plane of inW x inH bytes is streamed in: one per 3 MiB, 2 to 8.
+int pipelineChunks(int inW, int inH);
+// needRows, rects: per launch job (GatherPlan::launchNeedRows, launchRects).
+WaveSchedule scheduleWaves(const std::vector<int>& needRows, const std::vector<JobRect>& rects, int inH, int mapW, int mapH, int chunks);
+
 // Deals n <= 32 pixels of one warp step to lanes (and table copies) so that the lanes one shared-memory pass serves
 // together ask for different bank groups of the weight table.  slot[i] = weightSlotOf(k, phase of pixel i).
 // laneOf[i] = lane of pixel i, copyOf[i] = table copy it reads.  Returns the modelled wavefronts of one weight load.

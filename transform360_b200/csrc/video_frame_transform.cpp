@@ -282,17 +282,16 @@ struct FrameListRefs {
   t360::BlurLayout blurLayout;
 };
 
-// How the synchronous host-pointer call streams a large plane through the GPU: the input arrives in `chunks` row bands;
-// wave c = the gather jobs that only read rows delivered by chunks 0..c; rects[c] = the output rectangles that are
-// complete after wave c (copied back while later chunks are still on their way: PCIe carries both directions at once).
+// How the synchronous host-pointer call streams a large plane through the GPU (t360::scheduleWaves): the input arrives in
+// `chunks` row bands; wave c = the gather jobs that only read rows delivered by chunks 0..c; rects[c] = the output
+// rectangles that are complete after wave c (copied back while later chunks are still on their way: PCIe carries both
+// directions at once).
 struct WavePlan {
-  struct Rect { int x, y, w, h; };
   int chunks = 0;
   const void* plan = nullptr;  // the DevicePlan it was made for
   unsigned long long generation = ~0ull;
-  std::vector<int> chunkRowEnd, waveStart;
+  t360::WaveSchedule schedule;
   DeviceBuffer<GatherJob> jobs;  // wave-major
-  std::vector<std::vector<Rect>> rects;
 };
 
 // The streamed host-plane call is ~100 runtime calls (chunk copies, events, wave launches, rectangle copies); issued one by
@@ -915,6 +914,8 @@ class VideoFrameTransform {
     const char* e = std::getenv("T360B200_PIN_HOST_PLANES");
     pinHostPlanes_ = e && *e && *e != '0';
     if (const char* m = std::getenv("T360B200_PIPELINE_MIN_BYTES")) pipelineMinBytes_ = std::atoll(m);  // tests: 0 = always
+    const char* strict = std::getenv("T360B200_PIPELINE_STRICT");
+    pipelineStrict_ = strict && *strict && *strict != '0';
   }
   void setPinHostPlanes(bool on) { pinHostPlanes_ = on; }
 
@@ -958,6 +959,7 @@ class VideoFrameTransform {
       trace_.release();
       for (cudaEvent_t e : chunkIn_) cudaEventDestroy(e);
       for (cudaEvent_t e : waveDone_) cudaEventDestroy(e);
+      for (cudaEvent_t e : copiedOut_) cudaEventDestroy(e);
       for (WavePlan& w : wavePlans_) w.jobs.release();
       for (PlaneGraph& g : planeGraphs_) cudaGraphExecDestroy(g.exec);
       for (cudaEvent_t e : {graphFork_, graphJoinIn_, graphJoinOut_}) if (e) cudaEventDestroy(e);
@@ -1151,43 +1153,12 @@ class VideoFrameTransform {
     w.chunks = chunks;
     w.plan = &plan;
     w.generation = planGeneration_;
-    const int rowsPer = ((plan.inH + chunks - 1) / chunks + 7) & ~7;
-    w.chunkRowEnd.assign(chunks, plan.inH);
-    for (int c = 0; c < chunks; ++c) w.chunkRowEnd[c] = std::min(plan.inH, (c + 1) * rowsPer);
-    auto waveOf = [&](int needRows) {
-      int c = 0;
-      while (c + 1 < chunks && w.chunkRowEnd[c] < needRows) ++c;
-      return c;
-    };
-    std::vector<std::vector<GatherJob>> byWave(chunks);
-    // Which output rectangles are complete after which wave: 32-row bands of the full width (contiguous copies: a band
-    // split into the three faces of a cube-map row finishes earlier per face, but strided rectangle copies are much
-    // slower than whole contiguous bands).
-    const int bands = (plan.mapH + 31) / 32;
-    std::vector<int> complete(bands, 0);  // per band: the wave after which it is complete
-    for (size_t i = 0; i < plan.hostJobs.size(); ++i) {
-      const int c = waveOf(plan.jobNeedRows[i]);
-      byWave[c].push_back(plan.hostJobs[i]);
-      const t360::JobRect& r = plan.jobRects[i];
-      for (int band = r.y0 / 32; band <= (r.y1 - 1) / 32; ++band) complete[band] = std::max(complete[band], c);
-    }
+    w.schedule = t360::scheduleWaves(plan.jobNeedRows, plan.jobRects, plan.inH, plan.mapW, plan.mapH, chunks);
     std::vector<GatherJob> all;
-    w.waveStart.assign(chunks + 1, 0);
-    for (int c = 0; c < chunks; ++c) {
-      w.waveStart[c] = static_cast<int>(all.size());
-      all.insert(all.end(), byWave[c].begin(), byWave[c].end());
-    }
-    w.waveStart[chunks] = static_cast<int>(all.size());
+    all.reserve(w.schedule.order.size());
+    for (int i : w.schedule.order) all.push_back(plan.hostJobs[i]);
     w.jobs.reserve(all.size());
     CU(cudaMemcpy(w.jobs.ptr, all.data(), all.size() * sizeof(GatherJob), cudaMemcpyHostToDevice));
-    w.rects.assign(chunks, {});
-    for (int band = 0; band < bands;) {  // adjacent bands that complete together: one copy
-      const int c = complete[band];
-      int end = band + 1;
-      while (end < bands && complete[end] == c) ++end;
-      w.rects[c].push_back(WavePlan::Rect{0, band * 32, plan.mapW, std::min(plan.mapH, end * 32) - band * 32});
-      band = end;
-    }
     return w;
   }
 
@@ -1222,20 +1193,20 @@ class VideoFrameTransform {
   // reference transformFramePlane for large host planes (same result as the plain path): chunked H2D || gather || D2H
   bool transformHostPlanePipelined(const DevicePlan& plan, uint8_t* in, uint8_t* out, int inW, int inH, int inPitch, int outW, int outH,
                                    int outPitch, int planIndex, int imagePlaneIndex) {
-    const long long bytes = static_cast<long long>(inW) * inH;
-    const int chunks = static_cast<int>(std::min<long long>(8, std::max<long long>(2, bytes / (3ll << 20))));
+    const int chunks = t360::pipelineChunks(inW, inH);
     WavePlan& w = wavePlanFor(plan, planIndex, chunks);
+    const t360::WaveSchedule& ws = w.schedule;
     if (!copyIn_) {
       CU(cudaStreamCreateWithFlags(&copyIn_, cudaStreamNonBlocking));
       CU(cudaStreamCreateWithFlags(&copyOut_, cudaStreamNonBlocking));
       for (cudaEvent_t* e : {&graphFork_, &graphJoinIn_, &graphJoinOut_}) CU(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
     }
     while (static_cast<int>(chunkIn_.size()) < chunks) {
-      cudaEvent_t a = nullptr, b = nullptr;
-      CU(cudaEventCreateWithFlags(&a, cudaEventDisableTiming));
-      chunkIn_.push_back(a);
-      CU(cudaEventCreateWithFlags(&b, cudaEventDisableTiming));
-      waveDone_.push_back(b);
+      for (std::vector<cudaEvent_t>* v : {&chunkIn_, &waveDone_, &copiedOut_}) {
+        cudaEvent_t e = nullptr;
+        CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+        v->push_back(e);
+      }
     }
     pinIfRecurring(in, static_cast<size_t>(inPitch) * (inH - 1) + inW);
     pinIfRecurring(out, static_cast<size_t>(outPitch) * (outH - 1) + outW);
@@ -1254,8 +1225,16 @@ class VideoFrameTransform {
     }
     armScheduler(hostLane.claimCounter, stream_);
     CU(t360::prepareGatherFrame(plan.kernelSize));
+    // pipelineStrict_ (T360B200_PIPELINE_STRICT): the staging planes start out poisoned, chunk c + 1 is uploaded only after
+    // wave c, and wave c + 1 runs only after wave c's rectangles are back on the host.  A legal order of the same work in
+    // which a job that reads rows not yet delivered, or a band copied back before its last writer, gives wrong bytes on
+    // every call instead of only when a copy loses its race against a kernel.
     auto issue = [&](bool forkJoin) {
-      if (forkJoin) {  // (capture: the side streams become branches of the graph)
+      if (pipelineStrict_) {
+        CU(cudaMemsetAsync(stagingIn_.ptr, kStrictPoison, static_cast<size_t>(dInPitch) * inH, stream_));
+        CU(cudaMemsetAsync(stagingOut_.ptr, kStrictPoison, static_cast<size_t>(dOutPitch) * outH, stream_));
+      }
+      if (forkJoin || pipelineStrict_) {  // (capture: the side streams become branches of the graph)
         CU(cudaEventRecord(graphFork_, stream_));
         CU(cudaStreamWaitEvent(copyIn_, graphFork_, 0));
         CU(cudaStreamWaitEvent(copyOut_, graphFork_, 0));
@@ -1266,23 +1245,29 @@ class VideoFrameTransform {
       fp.kernelSize = plan.kernelSize;
       fp.numPlanes = 1;
       for (int c = 0; c < chunks; ++c) {
-        const int r0 = c ? w.chunkRowEnd[c - 1] : 0, r1 = w.chunkRowEnd[c];
+        const int r0 = c ? ws.chunkRowEnd[c - 1] : 0, r1 = ws.chunkRowEnd[c];
         if (r1 > r0)
           CU(cudaMemcpy2DAsync(stagingIn_.ptr + static_cast<size_t>(r0) * dInPitch, dInPitch, in + static_cast<size_t>(r0) * inPitch, inPitch, inW,
                                r1 - r0, cudaMemcpyHostToDevice, copyIn_));
         CU(cudaEventRecord(chunkIn_[c], copyIn_));
         CU(cudaStreamWaitEvent(stream_, chunkIn_[c], 0));
-        const int n = w.waveStart[c + 1] - w.waveStart[c];
+        if (pipelineStrict_ && c) CU(cudaStreamWaitEvent(stream_, copiedOut_[c - 1], 0));
+        const int n = ws.waveStart[c + 1] - ws.waveStart[c];
         if (n > 0) {
-          t360::StagedParams jobs{w.jobs.ptr + w.waveStart[c], n, hostLane.claimCounter.ptr, nullptr};
+          t360::StagedParams jobs{w.jobs.ptr + ws.waveStart[c], n, hostLane.claimCounter.ptr, nullptr};
           CU(t360::launchGatherFrame(fp, jobs, work.maps, numSMs_, stream_, /*programmatic=*/false));
         }
-        if (!w.rects[c].empty()) {
-          CU(cudaEventRecord(waveDone_[c], stream_));
+        if (!ws.rects[c].empty() || (pipelineStrict_ && c + 1 < chunks)) CU(cudaEventRecord(waveDone_[c], stream_));
+        if (!ws.rects[c].empty()) {
           CU(cudaStreamWaitEvent(copyOut_, waveDone_[c], 0));
-          for (const WavePlan::Rect& r : w.rects[c])
-            CU(cudaMemcpy2DAsync(out + static_cast<size_t>(r.y) * outPitch + r.x, outPitch,
-                                 stagingOut_.ptr + static_cast<size_t>(r.y) * dOutPitch + r.x, dOutPitch, r.w, r.h, cudaMemcpyDeviceToHost, copyOut_));
+          for (const t360::JobRect& r : ws.rects[c])
+            CU(cudaMemcpy2DAsync(out + static_cast<size_t>(r.y0) * outPitch + r.x0, outPitch,
+                                 stagingOut_.ptr + static_cast<size_t>(r.y0) * dOutPitch + r.x0, dOutPitch, r.x1 - r.x0, r.y1 - r.y0,
+                                 cudaMemcpyDeviceToHost, copyOut_));
+        }
+        if (pipelineStrict_ && c + 1 < chunks) {
+          CU(cudaStreamWaitEvent(copyIn_, waveDone_[c], 0));
+          CU(cudaEventRecord(copiedOut_[c], copyOut_));
         }
       }
       if (forkJoin) {
@@ -1316,7 +1301,7 @@ class VideoFrameTransform {
         cudaGraphDestroy(graph);
         if (e != cudaSuccess) throw CudaFail{e, "cudaGraphInstantiate"};
         int kernels = 0;
-        for (int c = 0; c < chunks; ++c) kernels += w.waveStart[c + 1] > w.waveStart[c];
+        for (int c = 0; c < chunks; ++c) kernels += ws.waveStart[c + 1] > ws.waveStart[c];
         planeGraphs_.push_back(PlaneGraph{&plan, planGeneration_, in, out, inPitch, outPitch, stagingIn_.ptr, stagingOut_.ptr, inW, inH, outW, outH,
                                           kernels, exec, 0});
         g = &planeGraphs_.back();
@@ -2688,9 +2673,11 @@ class VideoFrameTransform {
   DeviceBuffer<uint8_t> stagingIn_, stagingOut_;
   std::mutex hostCallMu_;  // the synchronous host-pointer path shares the staging planes and the streams: one call at a time
   cudaStream_t copyIn_ = nullptr, copyOut_ = nullptr;
-  std::vector<cudaEvent_t> chunkIn_, waveDone_;
+  std::vector<cudaEvent_t> chunkIn_, waveDone_, copiedOut_;  // per chunk
   WavePlan wavePlans_[2];  // plan index 0 / 1
   long long pipelineMinBytes_ = 6ll << 20;
+  bool pipelineStrict_ = false;  // T360B200_PIPELINE_STRICT (tests): see transformHostPlanPipelined
+  static constexpr uint8_t kStrictPoison = 0xA5;
   std::vector<PlaneGraph> planeGraphs_;  // (see PlaneGraph)
   unsigned long long graphClock_ = 0;
   cudaEvent_t graphFork_ = nullptr, graphJoinIn_ = nullptr, graphJoinOut_ = nullptr;
@@ -2762,6 +2749,8 @@ struct T360HostPlan {
   std::vector<GatherJob> deviceJobs;      // built on first use by T360B200_hostPlanDeviceLists
   std::vector<uint32_t> deviceRecords;
   std::vector<uint8_t> blurImage;  // the last T360B200_hostPlanBlurLists image made with this plan first
+  t360::WaveSchedule waves;        // the last T360B200_hostPlanWaves schedule
+  std::vector<int32_t> waveRects;  // its rectangles, {wave, x0, y0, x1, y1} each
 };
 
 T360_API T360HostPlan* T360B200_hostPlanCreate(const FrameTransformContext* ctx, int inW, int inH, int outW, int outH) {
@@ -2834,6 +2823,36 @@ T360_API int T360B200_hostPlanPoleCaps(T360HostPlan* plan, int info[4], const in
   if (capJobs) *capJobs = g.capJobs.empty() ? nullptr : reinterpret_cast<const int32_t*>(g.capJobs.data());
   if (capRecords) *capRecords = g.capRecords.empty() ? nullptr : g.capRecords.data();
   if (launchJobs) *launchJobs = g.launchJobs.empty() ? nullptr : reinterpret_cast<const int32_t*>(g.launchJobs.data());
+  return 1;
+}
+T360_API int T360B200_hostPlanLaunchExtents(T360HostPlan* plan, int* numJobs, const int32_t** needRows, const int32_t** rects) {
+  int gatherInfo[10];
+  if (!plan || !numJobs || !T360B200_hostPlanGather(plan, gatherInfo, nullptr, nullptr, nullptr)) return 0;
+  const t360::GatherPlan& g = plan->gather;
+  *numJobs = static_cast<int>(g.launchJobs.size());
+  if (needRows) *needRows = g.launchNeedRows.empty() ? nullptr : g.launchNeedRows.data();
+  if (rects) *rects = g.launchRects.empty() ? nullptr : reinterpret_cast<const int32_t*>(g.launchRects.data());
+  return 1;
+}
+T360_API int T360B200_hostPlanWaves(T360HostPlan* plan, int chunks, const int32_t* needRows, int info[3], const int32_t** chunkRowEnd,
+                                    const int32_t** waveStart, const int32_t** order, const int32_t** rects) {
+  int gatherInfo[10];
+  if (!plan || !info || chunks < 0 || chunks > 64 || !T360B200_hostPlanGather(plan, gatherInfo, nullptr, nullptr, nullptr)) return 0;
+  const t360::GatherPlan& g = plan->gather;
+  const HostPlan& h = plan->plan;
+  if (!chunks) chunks = t360::pipelineChunks(h.inW, h.inH);
+  const std::vector<int> rows = needRows ? std::vector<int>(needRows, needRows + g.launchNeedRows.size()) : g.launchNeedRows;
+  plan->waves = t360::scheduleWaves(rows, g.launchRects, h.inH, h.mapW, h.mapH, chunks);
+  plan->waveRects.clear();
+  for (int c = 0; c < chunks; ++c)
+    for (const t360::JobRect& r : plan->waves.rects[c]) plan->waveRects.insert(plan->waveRects.end(), {c, r.x0, r.y0, r.x1, r.y1});
+  info[0] = chunks;
+  info[1] = static_cast<int>(plan->waves.order.size());
+  info[2] = static_cast<int>(plan->waveRects.size() / 5);
+  if (chunkRowEnd) *chunkRowEnd = plan->waves.chunkRowEnd.data();
+  if (waveStart) *waveStart = plan->waves.waveStart.data();
+  if (order) *order = plan->waves.order.empty() ? nullptr : plan->waves.order.data();
+  if (rects) *rects = plan->waveRects.empty() ? nullptr : plan->waveRects.data();
   return 1;
 }
 T360_API int T360B200_hostPlanDeviceLists(T360HostPlan* plan, int info[2], const int32_t** jobs, const uint32_t** records) {

@@ -243,6 +243,10 @@ def load(path: os.PathLike | None = None):
     L.T360B200_hostPlanBlurLists.restype = ci
     L.T360B200_hostPlanBlurLists.argtypes = [vp, ci, ci, ci, C.POINTER(ci), C.POINTER(vp)]
     L.T360B200_hostPlanPoleCaps.argtypes = [vp, C.POINTER(ci), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]
+    L.T360B200_hostPlanLaunchExtents.restype = ci
+    L.T360B200_hostPlanLaunchExtents.argtypes = [vp, C.POINTER(ci), C.POINTER(vp), C.POINTER(vp)]
+    L.T360B200_hostPlanWaves.restype = ci
+    L.T360B200_hostPlanWaves.argtypes = [vp, ci, vp, C.POINTER(ci)] + [C.POINTER(vp)] * 4
     L.T360B200_hostPlanDeviceLists.restype = ci
     L.T360B200_hostPlanDeviceLists.argtypes = [vp, C.POINTER(ci), C.POINTER(vp), C.POINTER(vp)]
     L.T360B200_weightImage.restype = ci
@@ -341,7 +345,7 @@ EXPORTED_SYMBOLS = [
     "VideoFrameTransform_transformFramePlane", "T360B200_hostPlanCreate", "T360B200_hostPlanCreateFromWarp", "T360B200_hostPlanDestroy",
     "T360B200_generateMapFromWarp", "T360B200_remapFrameAsync",
     "T360B200_hostPlanInfo", "T360B200_hostPlanMap", "T360B200_hostPlanSamples", "T360B200_hostPlanSegment",
-    "T360B200_hostPlanGather", "T360B200_hostPlanPoleCaps", "T360B200_hostPlanDeviceLists", "T360B200_hostPlanBlurLists", "T360B200_weightImage", "T360B200_dealLanes",
+    "T360B200_hostPlanGather", "T360B200_hostPlanPoleCaps", "T360B200_hostPlanLaunchExtents", "T360B200_hostPlanWaves", "T360B200_hostPlanDeviceLists", "T360B200_hostPlanBlurLists", "T360B200_weightImage", "T360B200_dealLanes",
     "T360B200_remapTable", "T360B200_transformFramePlaneAsync", "T360B200_transformFrameAsync",
     "T360B200_lowPassPlaneAsync", "T360B200_reconfigure", "T360B200_reconfigureAsync", "T360B200_reconfigureWait",
     "T360B200_transformFrameViewAsync", "T360B200_viewSamples",
@@ -676,6 +680,37 @@ class HostPlan:
         as_jobs = lambda p, k: np.frombuffer((C.c_int32 * (k * 4)).from_address(p.value), np.int32).reshape(k, 4).copy() if k and p.value else np.zeros((0, 4), np.int32)
         records = np.frombuffer((C.c_uint32 * info[2]).from_address(recs.value), np.uint32).copy() if info[2] and recs.value else np.zeros(0, np.uint32)
         return dict(counts=dict(cap=info[0], border=info[1]), jobs=as_jobs(jobs, n), records=records, launch=as_jobs(launch, m))
+
+    def launch_extents(self):
+        """What the planner records per job of pole_caps()["launch"] for streaming a host plane through the device
+        (T360B200_hostPlanLaunchExtents): a dict of need_rows int32[m] (the source rows [0, n) the job reads) and rects
+        int32[m][4] (x0, y0, x1, y1 of the output pixels it writes, exclusive ends)."""
+        n, rows, rects = C.c_int(), C.c_void_p(), C.c_void_p()
+        if not self._lib.T360B200_hostPlanLaunchExtents(self._h, C.byref(n), C.byref(rows), C.byref(rects)):
+            raise ValueError("T360B200_hostPlanLaunchExtents failed")
+        m = n.value
+        return dict(need_rows=np.frombuffer((C.c_int32 * m).from_address(rows.value), np.int32).copy() if m else np.zeros(0, np.int32),
+                    rects=np.frombuffer((C.c_int32 * (4 * m)).from_address(rects.value), np.int32).reshape(m, 4).copy() if m else np.zeros((0, 4), np.int32))
+
+    def waves(self, chunks=None, need_rows=None):
+        """The schedule the synchronous host-pointer call streams a large plane of this plan with (T360B200_hostPlanWaves):
+        `chunks` input row bands (None: as many as the call takes for the plan's input size), the planner's need-rows or
+        `need_rows` (int per launch job) in their place.  Returns a dict: chunks, chunk_row_end int32[chunks], wave_start
+        int32[chunks + 1], order int32[m] (launch-job indices wave by wave), rects int32[r][5] (wave, x0, y0, x1, y1 of each
+        output rectangle copied back after that wave)."""
+        rows = None
+        if need_rows is not None:
+            rows = np.ascontiguousarray(need_rows, np.int32)
+            if rows.shape != (len(self.pole_caps()["launch"]),):
+                raise ValueError("need_rows: one value per launch job")
+        info = (C.c_int * 3)()
+        ends, starts, order, rects = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_void_p()
+        if not self._lib.T360B200_hostPlanWaves(self._h, chunks or 0, None if rows is None else rows.ctypes.data, info, C.byref(ends),
+                                                C.byref(starts), C.byref(order), C.byref(rects)):
+            raise ValueError("T360B200_hostPlanWaves failed")
+        c, m, r = info[0], info[1], info[2]
+        arr = lambda p, n: np.frombuffer((C.c_int32 * n).from_address(p.value), np.int32).copy() if n and p.value else np.zeros(0, np.int32)
+        return dict(chunks=c, chunk_row_end=arr(ends, c), wave_start=arr(starts, c + 1), order=arr(order, m), rects=arr(rects, 5 * r).reshape(r, 5))
 
     def device_lists(self):
         """The job list and record buffer the frame kernel reads (T360B200_hostPlanDeviceLists): a dict of jobs int32[m][4]
