@@ -692,6 +692,86 @@ int T360B200_transformFrameStereoCameraAsync(VideoFrameTransform* transform, con
                                              uint8_t* const* deviceOutputs, const int* inputWidths, const int* inputHeights,
                                              const int* inputPitches, const int* outputWidths, const int* outputHeights,
                                              const int* outputPitches, void* cudaStream);
+/* ---- rolling-shutter lens rigs ------------------------------------------------------------------------------------
+ * A CMOS sensor reads its rows over milliseconds, not at one instant, so a camera that turns during the readout records
+ * each row from another orientation: the per-frame orientation removes the shake between frames and leaves the shear and
+ * wobble within the frame.  These calls give the photometric lens and camera calls a rig motion over the readout.
+ *
+ * Readout time: lens i's point at normalised calibration coordinates u = (fx x' + cx + 0.5) / calibWidth, v = (fy y' + cy
+ * + 0.5) / calibHeight (the lens projection above, before the plane's size is applied; the same for every plane) is read
+ * at t = (a u + b v) + c, each step in float rounded to nearest, clamped to [0, 1] (a NaN gives 0), with (a, b, c) =
+ * readout[i].  (0, 1, 0): top to bottom over the whole frame; (0, -1, 1): bottom to top; (2, 0, -1): left to right over
+ * the right half of a side-by-side frame (a sensor mounted at 90 degrees).
+ * Sample matrices: the rig at t_k = k / (N - 1), k = 0..N-1 (N = numSamples), is turned by delta[k] from where the frame's
+ * orientation (sphere outputs) or pose (camera views) puts it: lens i's extrinsic rotation becomes R_ik = Rot(delta[k]) R_i,
+ * Rot(yaw, pitch, roll) = Ry(yaw) Rx(-pitch) Rz(roll) as for the lens extrinsics, computed in double; M_ik is R_ik^T with
+ * its y row negated (the lens projection's M), stored as float.  A zero delta gives the lens's own M bit for bit.
+ * Per pixel and lens, for the direction d the camera or sphere chain hands to the lens:
+ *   1. t = 0.5;
+ *   2. three projections, each: s = t (N - 1), k = min(floor(s), N - 2), f = s - k; M = M_ik + f (M_i,k+1 - M_ik) per
+ *      entry, each step rounded (an entry equal in both neighbours is taken as it is, so a -0 entry stays -0); the lens
+ *      projection with M; where it covers d, t becomes the readout time of its (u, v), where it does not t stays;
+ *   3. the third projection is the lens's entry, theta, coverage and theta_d (for Gq).
+ * So the fixed point t = readout(project(M(t) d)) is refined twice, a fixed count, and host and device agree bit for bit.
+ * The hard seam picks the lens with the larger Z under each lens's M at t = 0.5; the feathered seam's weight takes each
+ * lens's third-projection theta; the statistics' overlap is where both third projections cover d.  With a pyramid, a lens's
+ * footprint is its Jacobian (the anti-aliased views' step 2) with its third-projection M: the motion's own stretch of the
+ * footprint is left out.  Matrix interpolation is part of the contract, not an approximation of a slerp (it differs from
+ * one at third order in the angle between neighbouring samples).
+ * All-zero deltas give the records, frames and statistics of the photometric calls bit for bit, for any readout and N.
+ *
+ * Refused, with 0 and a message on stdout before any CUDA call, after every refusal of the call extended (and, for the
+ * host twins, before their index, array and size checks): a NULL motion, numSamples outside [2, 16], a delta angle that is
+ * not finite or lies outside [-30, 30] degrees, and a readout field of a lens that is read (readout[1] with two lenses)
+ * that is not finite.  The stereo camera call takes no motion. */
+typedef struct T360LensReadout {
+  float a, b, c; /* readout time of a lens point: t = a u + b v + c, clamped to [0, 1] */
+} T360LensReadout;
+typedef struct T360RigMotion {
+  int numSamples;             /* 2..16 */
+  T360Orientation delta[16];  /* the rig at readout time t_k = k / (numSamples - 1), turned from where it was for the
+                                 frame's orientation / pose; degrees, each in [-30, 30] */
+  T360LensReadout readout[2]; /* readout[1] is read only with two lenses */
+} T360RigMotion;
+/* Host only, no CUDA: the host twin of T360B200_transformFrameLensMotionAsync: T360B200_lensPhotoMaps' arguments and arrays
+ * with `motion`.  The oracle composite of T360B200_lensPhotoMaps' arrays (cv::remap of each map, s', the seam) gives the
+ * frame's plane and statistics bit for bit.  Returns 1; 0 (message) for the refusals above, a plane outside 0..2, a NULL
+ * array or non-positive sizes. */
+int T360B200_lensMotionMaps(const FrameTransformContext* ctx, const T360LensRig* rig, const T360RigPhotometry* photometry, float seamWidth,
+                            const T360Orientation* orientation, const T360RigMotion* motion, int plane, int inputWidth, int inputHeight,
+                            int outputWidth, int outputHeight, float* map0, float* map1, uint16_t* weight, uint16_t* gain0, uint16_t* gain1);
+/* One frame of a lens rig with photometry and a rig motion over the readout, every plane in one gather launch:
+ * T360B200_transformFrameLensPhotoAsync's arguments and asynchronous contract plus `motion`, which may change every frame.
+ * With the identity photometry it is the motion version of the lens (seamWidth 0) and blend calls.  The sample table
+ * (numLenses x numSamples x 9 floats) is uploaded in stream order from page-locked memory.  Returns 1 if everything was
+ * enqueued; 0 with a message on stdout, before any CUDA call, for the refusals above, 0 or more than 3 planes, or an
+ * invalid plane description. */
+int T360B200_transformFrameLensMotionAsync(VideoFrameTransform* transform, const T360LensRig* rig, const T360RigPhotometry* photometry,
+                                           float seamWidth, const T360Orientation* orientation, const T360RigMotion* motion,
+                                           unsigned long long* deviceStats, int numPlanes, const uint8_t* const* deviceInputs,
+                                           uint8_t* const* deviceOutputs, const int* inputWidths, const int* inputHeights,
+                                           const int* inputPitches, const int* outputWidths, const int* outputHeights,
+                                           const int* outputPitches, void* cudaStream);
+/* Host only, no CUDA: the host twin of T360B200_transformFrameCameraMotionAsync: T360B200_cameraPhotoMaps' arguments and
+ * arrays with `motion` after minify.  Returns 1; 0 (message) for the refusals above, a lens outside 0..1, a plane outside
+ * 0..2, a NULL array or non-positive sizes. */
+int T360B200_cameraMotionMaps(const FrameTransformContext* ctx, const T360LensRig* rig, const T360RigPhotometry* photometry, float seamWidth,
+                              const T360Pose* pose, const T360Camera* camera, const T360Minify* minify /* NULL: no pyramid */,
+                              const T360RigMotion* motion, int lens, int plane, int inputWidth, int inputHeight, int outputWidth,
+                              int outputHeight, float* map0, float* map1, uint8_t* level, uint16_t* weight, uint16_t* gain,
+                              uint16_t* seamWeight);
+/* One frame of a camera view of a lens rig with photometry and a rig motion over the readout (rectilinear views, every
+ * camera model, the pyramid, the seam and the statistics): T360B200_transformFrameCameraPhotoAsync's arguments and
+ * asynchronous contract plus `motion` after minify.  With one lens, this undistorts, stabilises and corrects the readout
+ * of an action camera in one pass.  Returns 1 if everything was enqueued; 0 with a message on stdout, before any CUDA
+ * call, for the refusals above, 0 or more than 3 planes, or an invalid plane description. */
+int T360B200_transformFrameCameraMotionAsync(VideoFrameTransform* transform, const T360LensRig* rig, const T360RigPhotometry* photometry,
+                                             float seamWidth, const T360Pose* pose, const T360Camera* camera,
+                                             const T360Minify* minify /* NULL: no pyramid */, const T360RigMotion* motion,
+                                             unsigned long long* deviceStats /* NULL: none */, int numPlanes,
+                                             const uint8_t* const* deviceInputs, uint8_t* const* deviceOutputs, const int* inputWidths,
+                                             const int* inputHeights, const int* inputPitches, const int* outputWidths,
+                                             const int* outputHeights, const int* outputPitches, void* cudaStream);
 /* Opt-in (also: environment T360B200_PIN_HOST_PLANES=1): page-lock pageable caller planes in place the second time
  * the same buffer is seen (cudaHostRegister), so that recycled frame-pool buffers are DMA'd at full PCIe speed.  The
  * caller must keep such buffers alive until VideoFrameTransform_delete. */

@@ -3,6 +3,7 @@
 
 #include <cuda_runtime.h>
 
+#include <cstddef>
 #include <cstdint>
 
 #include "flat_view.h"
@@ -403,7 +404,13 @@ void countKernelLaunches(long long n);  // kernels launched through a replayed C
 //                 blend; level 0 alone without a pyramid), then corrected, combined and counted as kLensPhoto's.
 //   kStereoCamera a camera view of a stereo rig (kCameraPhoto's constants, no seam; cameraPhotoSample<MIP, true>): the
 //                 output eye split of the context's output_stereo_format, and eye e's pixels take lens e alone.
-enum class PerFrameSource { kView, kSphere, kMap, kLens, kLensBlend, kRectilinear, kCameraMip, kLensPhoto, kCameraPhoto, kStereoCamera };
+//   kLensMotion   kLensPhoto with a rig motion over the readout (rotation, rig, seamScale, lensMotion: the photometric
+//                 constants and the motion's sample table; lensMotionSample): each lens's M follows the readout time of
+//                 the point it projects.
+//   kCameraMotion kCameraPhoto with a rig motion (cameraMotion: kCameraPhoto's constants and the motion;
+//                 cameraMotionSample).
+enum class PerFrameSource { kView, kSphere, kMap, kLens, kLensBlend, kRectilinear, kCameraMip, kLensPhoto, kCameraPhoto, kStereoCamera,
+                            kLensMotion, kCameraMotion };
 struct PerFramePlane {
   const uint8_t* src;  // (blurred) input plane, geometry.inW x geometry.inH
   uint8_t* dst;        // render target, geometry.mapW x geometry.mapH
@@ -459,17 +466,33 @@ struct PerFrameGatherParams {
     CameraPhotoPlane mip[kMaxFramePlanes];
     LensPhoto photo;
   };
-  // (the three sources' constants share their storage, so the block keeps the size and layout every other source's
-  // kernel was compiled against: a larger block would move the kernels' next parameter)
+  // kLensMotion / kCameraMotion: kLensPhoto's / kCameraPhoto's constants and the rig motion (its sample table staged in
+  // device memory, numSamples and the lenses' readouts)
+  struct LensMotion {
+    LensPhoto photo;
+    RigMotion motion;
+  };
+  struct CameraMotion {
+    CameraPhoto cameraPhoto;
+    RigMotion motion;
+  };
+  // (the sources' constants share their storage, so the block keeps the size and layout every other source's kernel was
+  // compiled against: a larger block would move the kernels' next parameter)
   union {
     MipPlane mip[kMaxFramePlanes];
     LensPhoto photo;
     CameraPhoto cameraPhoto;
+    LensMotion lensMotion;
+    CameraMotion cameraMotion;
   };
   int mipBias;
 };
 static_assert(sizeof(PerFrameGatherParams::LensPhoto) <= sizeof(PerFrameGatherParams::MipPlane) * kMaxFramePlanes);
 static_assert(sizeof(PerFrameGatherParams::CameraPhoto) <= sizeof(PerFrameGatherParams::MipPlane) * kMaxFramePlanes);
+static_assert(sizeof(PerFrameGatherParams::LensMotion) <= sizeof(PerFrameGatherParams::MipPlane) * kMaxFramePlanes);
+static_assert(sizeof(PerFrameGatherParams::CameraMotion) <= sizeof(PerFrameGatherParams::MipPlane) * kMaxFramePlanes);
+// (the block the kernels were compiled against before the motion sources: its size and where its last member lies)
+static_assert(sizeof(PerFrameGatherParams) == 1496 && offsetof(PerFrameGatherParams, mipBias) == 1488);
 constexpr int kPhotoStats = 6;  // sums per plane of kLensPhoto's statistics
 // a CTA takes tiles of 32 output columns x viewTileRows(k) rows; a thread owns one column of a tile and walks down
 // kViewRowsPerThread of its rows

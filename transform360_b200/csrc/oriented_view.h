@@ -1152,6 +1152,213 @@ T360_HD int cameraPhotoSample(const SphereGeometry& g, const RectilinearCamera& 
   return w;
 }
 
+// ---- rolling-shutter lens rigs (T360B200_lensMotionMaps, T360B200_cameraMotionMaps and their frame calls) ---------------
+// Each lens's M depends on the readout time t of the point it projects: M(t) = M_k + f (M_k+1 - M_k) between the sample
+// matrices of the rig motion (the table: [numLenses][numSamples][9], computed on the host in double and stored as float,
+// rigMotionTable in video_frame_transform.cpp), and t = clamp((a u + b v) + c, 0, 1) of the lens point's normalised
+// calibration coordinates.  lensMotionHit solves t = readout(project(M(t) d)) by a fixed count of refinements from t =
+// 0.5; everything else (the projection, the gain, the seam weight, the footprint) is the photometric calls' code with
+// the lens's M replaced.  With all-zero deltas every table entry is the lens's own M and the interpolation returns it as
+// it is, so the records are the photometric calls' bit for bit.
+constexpr int kMotionMaxSamples = 16;
+constexpr int kMotionProjections = 3;  // the fixed point refined twice
+struct RigMotion {
+  const float* table;      // [numLenses][numSamples][9]: M_ik (device memory in a launch, host memory in the twins)
+  int numSamples;          // N, 2..16
+  float readout[2][3];     // (a, b, c) of each lens
+};
+
+// A table entry: read-only global loads on the device (the table is at most 1152 bytes and stays in L1)
+T360_HD float motionEntry(const float* p) {
+#ifdef __CUDA_ARCH__
+  return __ldg(p);
+#else
+  return *p;
+#endif
+}
+
+// Lens L with the M of readout time t (0..1) of lens `lens`: s = t (N - 1), k = min(floor(s), N - 2), f = s - k, each
+// entry M_k + f (M_k+1 - M_k), or M_k itself where both neighbours hold the same value
+T360_HD LensModel motionLens(const LensModel& L, const RigMotion& mo, int lens, float t) {
+  const float s = fMul(t, static_cast<float>(mo.numSamples - 1));
+  int k = truncToInt(s);
+  k = k > mo.numSamples - 2 ? mo.numSamples - 2 : k;
+  const float f = fSub(s, static_cast<float>(k));
+  const float* a = mo.table + (lens * mo.numSamples + k) * 9;
+  LensModel M = L;
+#pragma unroll
+  for (int e = 0; e < 9; ++e) {
+    const float lo = motionEntry(a + e), hi = motionEntry(a + 9 + e);
+    M.m[e] = lo == hi ? lo : fAdd(lo, fMul(f, fSub(hi, lo)));
+  }
+  return M;
+}
+
+// Z of rig direction d under lens `lens`'s M at t = 0.5: the hard seam's lens choice
+T360_HD float motionZ(const LensModel& L, const RigMotion& mo, int lens, const SphereVec& d) {
+  return lensRow(motionLens(L, mo, lens, 0.5f).m + 6, d);
+}
+
+// The readout time of where lens M projects d (h covers d): t = clamp((a u + b v) + c, 0, 1), with u, v the normalised
+// calibration coordinates lensHit forms before toPixel (its s = theta_d / rho, recomputed from the hit's r = theta_d)
+T360_HD float readoutTime(const LensModel& M, const LensHitR& h, const SphereVec& d, const float* r) {
+  const float X = lensRow(M.m, d), Y = lensRow(M.m + 3, d);
+  const float rho = fSqrt(fAdd(fMul(X, X), fMul(Y, Y)));
+  const float s = rho > 0.0f ? fDiv(h.r, rho) : 0.0f;
+  const float u = fAdd(fMul(M.ax, fMul(s, X)), M.bx), v = fAdd(fMul(M.ay, fMul(s, Y)), M.by);
+  const float t = fAdd(fAdd(fMul(r[0], u), fMul(r[1], v)), r[2]);
+  return t > 0.0f ? (t < 1.0f ? t : 1.0f) : 0.0f;
+}
+
+// Lens `lens` of the rig with the motion, for rig direction d: kMotionProjections projections, each with the M of the
+// current readout time, which a covered hit moves to its own readout time.  Returns the last hit; *at: the lens with that
+// hit's M (the footprint's lens).  *times (optional): the readout times the projections used.
+T360_HD LensHitR lensMotionHit(const LensModel& L, const RigMotion& mo, int lens, const SphereVec& d, int inW, int inH, LensModel* at,
+                               float* times = nullptr) {
+  float t = 0.5f;
+  LensHitR h;
+#pragma unroll 1
+  for (int n = 0; n < kMotionProjections; ++n) {
+    if (times) times[n] = t;
+    *at = motionLens(L, mo, lens, t);
+    h = lensHit<true>(*at, d, lensRow(at->m + 6, d), inW, inH);
+    if (h.covered) t = readoutTime(*at, h, d, mo.readout[lens]);
+  }
+  return h;
+}
+
+// lensPhotoPosition (not STEREO) with the motion: the hard seam picks the lens by Z under each lens's M at t = 0.5, and
+// each projected lens is lensMotionHit's.  at[l]: lens l with its last M where it was projected (the footprint's lens).
+T360_HD int lensMotionPosition(const LensRigModel& rig, const RigMotion& mo, float s, bool both, const LensPhotoPlane& c, const SphereVec& d,
+                               int inW, int inH, float* p0, float* p1, int* g0, int* g1, bool* overlap, LensModel* at) {
+  const float nan = bitsFloat(0x7fc00000u);
+  const float z0 = motionZ(rig.lens[0], mo, 0, d);
+  const float z1 = rig.numLenses > 1 ? motionZ(rig.lens[1], mo, 1, d) : z0;
+  const bool second = z1 > z0;
+  if (s == 0.0f && !both) {  // the closer lens alone
+    const int l = second ? 1 : 0;
+    const LensHitR h = lensMotionHit(rig.lens[l], mo, l, d, inW, inH, &at[l]);
+    float* p = second ? p1 : p0;
+    float* q = second ? p0 : p1;
+    p[0] = h.px; p[1] = h.py;
+    q[0] = q[1] = nan;
+    *(second ? g1 : g0) = lensGain(h, c.v[l], c.gain[l]);
+    *(second ? g0 : g1) = 0;
+    *overlap = false;
+    return second ? 256 : 0;
+  }
+  LensHitR h0 = lensMotionHit(rig.lens[0], mo, 0, d, inW, inH, &at[0]), h1;
+  h1.covered = false;
+  h1.px = h1.py = h1.r = nan;
+  if (rig.numLenses > 1) h1 = lensMotionHit(rig.lens[1], mo, 1, d, inW, inH, &at[1]);
+  int w = second ? 256 : 0;
+  if (s > 0.0f) {
+    w = h1.covered ? 256 : 0;
+    if (h0.covered && h1.covered) w = seamWeight(h0.theta, h1.theta, s);
+  }
+  p0[0] = h0.px; p0[1] = h0.py;
+  p1[0] = h1.px; p1[1] = h1.py;
+  *g0 = lensGain(h0, c.v[0], c.gain[0]);
+  *g1 = lensGain(h1, c.v[1], c.gain[1]);
+  *overlap = h0.covered && h1.covered;
+  return w;
+}
+
+// lensPhotoPoint with the motion (T360B200_lensMotionMaps)
+template <bool BARREL = true>
+T360_HD int lensMotionPoint(const SphereGeometry& g, const Rotation& r, const LensRigModel& rig, const RigMotion& mo, float s, bool both,
+                            const LensPhotoPlane& c, const float* colTab, const float* rowTab, int i, int j, float* p0, float* p1, int* g0,
+                            int* g1, bool* overlap) {
+  bool eye;
+  SphereVec d;
+  if (!spherePoint<BARREL>(g, r, colTab, rowTab, i, j, &eye, &d)) {
+    p0[0] = p0[1] = p1[0] = p1[1] = bitsFloat(0x7fc00000u);
+    *g0 = *g1 = 0;
+    *overlap = false;
+    return 0;
+  }
+  LensModel at[2];
+  return lensMotionPosition(rig, mo, s, both, c, d, g.inW, g.inH, p0, p1, g0, g1, overlap, at);
+}
+
+// lensPhotoSample with the motion (the kLensMotion kernels)
+template <bool BARREL = true>
+T360_HD int lensMotionSample(const SphereGeometry& g, const Rotation& r, const LensRigModel& rig, const RigMotion& mo, float s, bool both,
+                             const LensPhotoPlane& c, const float* colTab, const float* rowTab, int i, int j, int32_t* rec0, int32_t* rec1,
+                             int* g0, int* g1, bool* overlap) {
+  float p[2][2];
+  const int w = lensMotionPoint<BARREL>(g, r, rig, mo, s, both, c, colTab, rowTab, i, j, p[0], p[1], g0, g1, overlap);
+  int32_t* rec[2] = {rec0, rec1};
+  for (int l = 0; l < 2; ++l) {
+    int r0, fracX, fracY;
+    quantizeAxis(p[l][0], g.kernelSize, &rec[l][0], &fracX);
+    quantizeAxis(p[l][1], g.kernelSize, &r0, &fracY);
+    rec[l][1] = r0 * 1024 + fracY * 32 + fracX;
+  }
+  return w;
+}
+
+// cameraPhotoPoint (not STEREO) with the motion: the lenses from lensMotionPosition, and each used lens's footprint from
+// lensJacobian of that lens with its last M (the motion's own stretch of the footprint is left out)
+template <bool MIP>
+T360_HD int cameraMotionPoint(const SphereGeometry& g, const RectilinearCamera& c, const LensRigModel& rig, const RigMotion& mo,
+                              const MipGeometry& m, int bias256, float s, bool both, const LensPhotoPlane& ph, int i, int j, CameraPhotoLens* lens,
+                              bool* overlap) {
+  float X, Y;
+  bool eye;
+  cameraXY(g, i, j, &X, &Y, &eye);
+  const SphereVec t = rotateHD(c.r, modelRay(c, X, Y));
+  float p[2][2];
+  LensModel at[2];
+  const int w = lensMotionPosition(rig, mo, s, both, ph, t, g.inW, g.inH, p[0], p[1], &lens[0].gain, &lens[1].gain, overlap, at);
+  const bool used[2] = {p[0][0] == p[0][0], p[1][0] == p[1][0]};
+  const bool footprint = MIP && m.top > 0 && (used[0] || used[1]);
+  SphereVec rx{}, ry{};
+  if (footprint) {
+    rx = rayDifferential(c, fSub(X, m.halfX), Y, fAdd(X, m.halfX), Y);
+    ry = rayDifferential(c, X, fSub(Y, m.halfY), X, fAdd(Y, m.halfY));
+  }
+  const float nan = bitsFloat(0x7fc00000u);
+  for (int l = 0; l < 2; ++l) {
+    CameraPhotoLens& e = lens[l];
+    e.level = e.w = 0;
+    if (footprint && used[l]) {
+      float a[2], b[2];
+      lensJacobian(at[l], lensRow(at[l].m + 6, t), t, rx, ry, g.inW, g.inH, a, b);
+      e.level = mipLevelOf(fAdd(fMul(a[0], a[0]), fMul(a[1], a[1])), fAdd(fMul(b[0], b[0]), fMul(b[1], b[1])), m.top, bias256, &e.w);
+    }
+    e.p0[0] = e.level ? mipScale(p[l][0], m.sx[e.level]) : p[l][0];
+    e.p0[1] = e.level ? mipScale(p[l][1], m.sy[e.level]) : p[l][1];
+    e.p1[0] = e.w ? mipScale(p[l][0], m.sx[e.level + 1]) : nan;
+    e.p1[1] = e.w ? mipScale(p[l][1], m.sy[e.level + 1]) : nan;
+  }
+  return w;
+}
+
+// cameraPhotoSample with the motion (the kCameraMotion kernels)
+template <bool MIP>
+T360_HD int cameraMotionSample(const SphereGeometry& g, const RectilinearCamera& c, const LensRigModel& rig, const RigMotion& mo,
+                               const MipGeometry& m, int bias256, float s, bool both, const LensPhotoPlane& ph, int i, int j,
+                               CameraPhotoRecords* lens, bool* overlap) {
+  CameraPhotoLens e[2];
+  const int w = cameraMotionPoint<MIP>(g, c, rig, mo, m, bias256, s, both, ph, i, j, e, overlap);
+  for (int l = 0; l < 2; ++l) {
+    int r0, fracX, fracY;
+    quantizeAxis(e[l].p0[0], g.kernelSize, &lens[l].rec0[0], &fracX);
+    quantizeAxis(e[l].p0[1], g.kernelSize, &r0, &fracY);
+    lens[l].rec0[1] = r0 * 1024 + fracY * 32 + fracX;
+    if (e[l].w) {
+      quantizeAxis(e[l].p1[0], g.kernelSize, &lens[l].rec1[0], &fracX);
+      quantizeAxis(e[l].p1[1], g.kernelSize, &r0, &fracY);
+      lens[l].rec1[1] = r0 * 1024 + fracY * 32 + fracX;
+    }
+    lens[l].level = e[l].level;
+    lens[l].w = e[l].w;
+    lens[l].gain = e[l].gain;
+  }
+  return w;
+}
+
 // Whether the per-frame orientation chain covers the layouts of `ctx`
 inline bool orientedLayouts(const FrameTransformContext& ctx) {
   const int o = ctx.output_layout, in = ctx.input_layout;

@@ -360,6 +360,9 @@ struct StreamSlot {
     size_t xTaps = SIZE_MAX, xFirst, yTaps, yFirst;  // byte offsets in mipTapBytes (SIZE_MAX: exact 2 x 2 cells)
   } mipTapAt[kPlaneLanes][t360::kMipMaxLevels];      // per plane and level l (at l - 1)
   std::vector<int> mipSizes;                         // inW, inH, top per plane
+  // the rig motion's sample table of the motion calls (they change every frame)
+  UploadRing motionTables;
+  std::vector<uint8_t> motionBytes;
 };
 
 // A w x h scratch plane in buf (a lane's or the staging planes), grown on demand: its pitch, 256-byte aligned
@@ -575,30 +578,110 @@ bool lensBlendRefused(const FrameTransformContext& ctx, const T360LensRig* rig, 
 // lensBlendPosition)
 float lensSeamScale(float seamWidth) { return static_cast<float>(1.0 / (2.0 * static_cast<double>(seamWidth) * M_PI / 180.0)); }
 
+// Ry(yaw) Rx(-pitch) Rz(roll) of angles in degrees, in double: the lens extrinsics' rotation (and the rig motion's)
+void extrinsicRotation(float yaw, float pitch, float roll, double r[3][3]) {
+  const double a = yaw * M_PI / 180.0, b = -pitch * M_PI / 180.0, g = roll * M_PI / 180.0;
+  const double ry[3][3] = {{std::cos(a), 0, std::sin(a)}, {0, 1, 0}, {-std::sin(a), 0, std::cos(a)}};
+  const double rx[3][3] = {{1, 0, 0}, {0, std::cos(b), -std::sin(b)}, {0, std::sin(b), std::cos(b)}};
+  const double rz[3][3] = {{std::cos(g), -std::sin(g), 0}, {std::sin(g), std::cos(g), 0}, {0, 0, 1}};
+  double ryx[3][3];
+  for (int u = 0; u < 3; ++u)
+    for (int v = 0; v < 3; ++v) ryx[u][v] = ry[u][0] * rx[0][v] + ry[u][1] * rx[1][v] + ry[u][2] * rx[2][v];
+  for (int u = 0; u < 3; ++u)
+    for (int v = 0; v < 3; ++v) r[u][v] = ryx[u][0] * rz[0][v] + ryx[u][1] * rz[1][v] + ryx[u][2] * rz[2][v];
+}
+
+// A lens's M from its rotation r: R^T, the y row negated (OpenCV's camera coordinates), stored as float
+void lensMatrix(const double r[3][3], float* m) {
+  for (int u = 0; u < 3; ++u)
+    for (int v = 0; v < 3; ++v) m[3 * u + v] = static_cast<float>(u == 1 ? -r[v][u] : r[v][u]);
+}
+
 // The per-frame constants of a rig (oriented_view.h: LensModel), in double and stored as float
 t360::LensRigModel lensRigModel(const T360LensRig& rig) {
   t360::LensRigModel m{};
   m.numLenses = rig.numLenses;
   for (int i = 0; i < rig.numLenses; ++i) {
     const T360Lens& L = rig.lens[i];
-    const double a = L.yaw * M_PI / 180.0, b = -L.pitch * M_PI / 180.0, g = L.roll * M_PI / 180.0;
-    const double ry[3][3] = {{std::cos(a), 0, std::sin(a)}, {0, 1, 0}, {-std::sin(a), 0, std::cos(a)}};
-    const double rx[3][3] = {{1, 0, 0}, {0, std::cos(b), -std::sin(b)}, {0, std::sin(b), std::cos(b)}};
-    const double rz[3][3] = {{std::cos(g), -std::sin(g), 0}, {std::sin(g), std::cos(g), 0}, {0, 0, 1}};
-    double ryx[3][3], r[3][3];
-    for (int u = 0; u < 3; ++u)
-      for (int v = 0; v < 3; ++v) ryx[u][v] = ry[u][0] * rx[0][v] + ry[u][1] * rx[1][v] + ry[u][2] * rx[2][v];
-    for (int u = 0; u < 3; ++u)
-      for (int v = 0; v < 3; ++v) r[u][v] = ryx[u][0] * rz[0][v] + ryx[u][1] * rz[1][v] + ryx[u][2] * rz[2][v];
+    double r[3][3];
+    extrinsicRotation(L.yaw, L.pitch, L.roll, r);
     t360::LensModel& l = m.lens[i];
-    for (int u = 0; u < 3; ++u)  // R^T, the y row negated: OpenCV's camera coordinates
-      for (int v = 0; v < 3; ++v) l.m[3 * u + v] = static_cast<float>(u == 1 ? -r[v][u] : r[v][u]);
+    lensMatrix(r, l.m);
     l.ax = static_cast<float>(static_cast<double>(L.fx) / rig.calibWidth);
     l.bx = static_cast<float>((static_cast<double>(L.cx) + 0.5) / rig.calibWidth);
     l.ay = static_cast<float>(static_cast<double>(L.fy) / rig.calibHeight);
     l.by = static_cast<float>((static_cast<double>(L.cy) + 0.5) / rig.calibHeight);
     for (int j = 0; j < 4; ++j) l.k[j] = L.k[j];
     l.thetaMax = static_cast<float>(L.maxAngle * M_PI / 180.0);
+  }
+  return m;
+}
+
+// ---- rolling-shutter lens rigs (T360B200_lensMotionMaps, T360B200_cameraMotionMaps and their frame calls) ---------------
+// true, with the reason in *why, when a rig motion cannot be used with a usable rig: NULL, a sample count outside [2, 16],
+// a delta angle that is not finite or lies outside [-30, 30] degrees, a readout field of a lens that is read that is not
+// finite
+bool motionRefused(const T360LensRig& rig, const T360RigMotion* mo, std::string* why) {
+  if (!mo) {
+    *why = "a NULL motion";
+    return true;
+  }
+  if (mo->numSamples < 2 || mo->numSamples > t360::kMotionMaxSamples) {
+    *why = formatted("numSamples %d is outside [2, %d]", mo->numSamples, t360::kMotionMaxSamples);
+    return true;
+  }
+  for (int k = 0; k < mo->numSamples; ++k) {
+    const T360Orientation& d = mo->delta[k];
+    for (float a : {d.yaw, d.pitch, d.roll})
+      if (!std::isfinite(a) || !(a >= -30.0f && a <= 30.0f)) {
+        *why = formatted("delta[%d] (yaw %g, pitch %g, roll %g) must be finite and lie in [-30, 30] degrees", k, d.yaw, d.pitch, d.roll);
+        return true;
+      }
+  }
+  for (int i = 0; i < rig.numLenses; ++i) {
+    const T360LensReadout& r = mo->readout[i];
+    if (!std::isfinite(r.a) || !std::isfinite(r.b) || !std::isfinite(r.c)) {
+      *why = formatted("the readout of lens %d has a field that is not finite", i);
+      return true;
+    }
+  }
+  return false;
+}
+
+// The motion's sample matrices M_ik, [numLenses][numSamples][9] floats: lens i's rotation R_i turned by delta[k], R_ik =
+// Rot(delta[k]) R_i in double, then lensMatrix; a zero delta gives lensRigModel's M itself
+std::vector<float> rigMotionTable(const T360LensRig& rig, const T360RigMotion& mo, const t360::LensRigModel& model) {
+  std::vector<float> t(static_cast<size_t>(rig.numLenses) * mo.numSamples * 9);
+  for (int i = 0; i < rig.numLenses; ++i) {
+    const T360Lens& L = rig.lens[i];
+    double ri[3][3];
+    extrinsicRotation(L.yaw, L.pitch, L.roll, ri);
+    for (int k = 0; k < mo.numSamples; ++k) {
+      float* m = t.data() + (static_cast<size_t>(i) * mo.numSamples + k) * 9;
+      const T360Orientation& d = mo.delta[k];
+      if (d.yaw == 0.0f && d.pitch == 0.0f && d.roll == 0.0f) {
+        std::memcpy(m, model.lens[i].m, sizeof(model.lens[i].m));
+        continue;
+      }
+      double q[3][3], r[3][3];
+      extrinsicRotation(d.yaw, d.pitch, d.roll, q);
+      for (int u = 0; u < 3; ++u)
+        for (int v = 0; v < 3; ++v) r[u][v] = q[u][0] * ri[0][v] + q[u][1] * ri[1][v] + q[u][2] * ri[2][v];
+      lensMatrix(r, m);
+    }
+  }
+  return t;
+}
+
+// The per-frame constants of a motion (oriented_view.h: RigMotion) with its table at `table`
+t360::RigMotion rigMotion(const T360RigMotion& mo, const float* table) {
+  t360::RigMotion m{};
+  m.table = table;
+  m.numSamples = mo.numSamples;
+  for (int i = 0; i < 2; ++i) {
+    m.readout[i][0] = mo.readout[i].a;
+    m.readout[i][1] = mo.readout[i].b;
+    m.readout[i][2] = mo.readout[i].c;
   }
   return m;
 }
@@ -719,7 +802,8 @@ constexpr T360Camera kPinhole{T360_CAMERA_PINHOLE, 0.0f};
 
 // What a camera call was given; the arguments a call does not take stay NULL / 0.  rig == nullptr: a view of the
 // context's input.  photometric: the call corrects the rig's lenses, so it needs a rig and a photometry (the photometric
-// and stereo calls); stereo: each eye takes its own lens (no seam).  minify == nullptr: no pyramid.
+// and stereo calls); stereo: each eye takes its own lens (no seam).  minify == nullptr: no pyramid.  motion: a rig motion
+// over the readout (the camera-motion calls: a photometric view).
 struct CameraView {
   const T360LensRig* rig = nullptr;
   const T360RigPhotometry* photometry = nullptr;
@@ -730,6 +814,8 @@ struct CameraView {
   unsigned long long* stats = nullptr;
   bool photometric = false;
   bool stereo = false;
+  const T360RigMotion* motion = nullptr;
+  bool moving = false;  // (the camera-motion calls: motion is checked, NULL included)
 };
 // A view of ctx's input (rig == nullptr) or of a rig's lenses as they are: the rectilinear, camera and camera-mip calls
 CameraView plainView(const T360LensRig* rig, const T360Pose* pose, const T360Camera* camera, const T360Minify* minify = nullptr) {
@@ -739,6 +825,14 @@ CameraView plainView(const T360LensRig* rig, const T360Pose* pose, const T360Cam
 CameraView photoView(const T360LensRig* rig, const T360RigPhotometry* photometry, float seamWidth, const T360Pose* pose, const T360Camera* camera,
                      const T360Minify* minify, unsigned long long* stats, bool stereo) {
   return {rig, photometry, seamWidth, pose, camera, minify, stats, true, stereo};
+}
+// A view of a rig's lenses with photometry and a rig motion: the camera-motion calls
+CameraView motionView(const T360LensRig* rig, const T360RigPhotometry* photometry, float seamWidth, const T360Pose* pose, const T360Camera* camera,
+                      const T360Minify* minify, const T360RigMotion* motion, unsigned long long* stats) {
+  CameraView v = photoView(rig, photometry, seamWidth, pose, camera, minify, stats, false);
+  v.motion = motion;
+  v.moving = true;
+  return v;
 }
 
 // true, with the reason in *why, when `minify` is NULL or out of range
@@ -761,8 +855,8 @@ bool minifyRefused(const T360Minify* minify, std::string* why) {
 // true, with the reason in *why, when view v of ctx's input or of its rig cannot be rendered, in this order: a photometric
 // view's NULL rig; a stereo rig without two lenses or an output_stereo_format other than TB, LR or MONO; the pose, the
 // camera and its fields of view, the rig (rigRefused), the low-pass filter and the interpolation; a photometric view's
-// seam (seamWidthRefused, featherRefused) and photometry (photometryRefused); the minify where there is one.  The output
-// layout plays no part: the pose replaces it.
+// seam (seamWidthRefused, featherRefused) and photometry (photometryRefused); the minify where there is one; a moving
+// view's motion (motionRefused).  The output layout plays no part: the pose replaces it.
 bool viewRefused(const FrameTransformContext& ctx, const CameraView& v, std::string* why) {
   if (v.photometric && !v.rig) {
     *why = v.stereo ? "a NULL rig (a stereo rig's lenses are its eyes)" : "a NULL rig (the photometry corrects a rig's lenses)";
@@ -837,7 +931,8 @@ bool viewRefused(const FrameTransformContext& ctx, const CameraView& v, std::str
     if (seamWidthRefused(v.seamWidth, why) || (v.seamWidth > 0.0f && featherRefused(*v.rig, v.seamWidth, why))) return true;
     if (photometryRefused(*v.rig, v.photometry, why)) return true;
   }
-  return v.minify && minifyRefused(v.minify, why);
+  if (v.minify && minifyRefused(v.minify, why)) return true;
+  return v.moving && motionRefused(*v.rig, v.motion, why);
 }
 
 // The per-frame constants of v's pose and camera (oriented_view.h: cameraConstants)
@@ -944,7 +1039,7 @@ class VideoFrameTransform {
         }
         kv.second->frameClaim.release();
         if (kv.second->fork) cudaEventDestroy(kv.second->fork);
-        for (UploadRing* ring : {&kv.second->viewJobs, &kv.second->viewTaps, &kv.second->sphereTables})
+        for (UploadRing* ring : {&kv.second->viewJobs, &kv.second->viewTaps, &kv.second->sphereTables, &kv.second->motionTables})
           for (UploadRing::Entry& e : ring->entries) {
             if (e.released) cudaEventSynchronize(e.released);
             if (e.device) cudaFree(e.device);
@@ -1470,10 +1565,13 @@ class VideoFrameTransform {
   // photo: a photometry (T360B200_transformFrameLensPhotoAsync: lensPhotoSample), with *seamWidth 0 for the hard seam; each
   // lens's sample is corrected before the seam, and with stats set (device, [numPlanes][6]) the overlap's sums are zeroed
   // with a memset and accumulated by the same gather.
+  // moving: a photometric frame with a rig motion (T360B200_transformFrameLensMotionAsync: lensMotionSample), motion checked
+  // after the photometric refusals; its sample table comes through the slot's upload ring.
   bool transformFrameLens(const char* what, const T360LensRig* rig, const float* seamWidth, const T360Orientation* o, const FramePlanes& f,
-                          cudaStream_t stream, const T360RigPhotometry* photo = nullptr, unsigned long long* stats = nullptr) {
+                          cudaStream_t stream, const T360RigPhotometry* photo = nullptr, unsigned long long* stats = nullptr,
+                          bool moving = false, const T360RigMotion* motion = nullptr) {
     auto refused = [&](const FrameTransformContext& ctx, std::string* why) {
-      if (photo) return lensPhotoRefused(ctx, rig, photo, *seamWidth, o, why);
+      if (photo) return lensPhotoRefused(ctx, rig, photo, *seamWidth, o, why) || (moving && motionRefused(*rig, motion, why));
       return seamWidth ? lensBlendRefused(ctx, rig, *seamWidth, o, why) : lensRefused(ctx, rig, o, why);
     };
     return unplannedFrame(what, stream, refused, [&](const FrameTransformContext& ctx, int k, cudaStream_t s) {
@@ -1488,13 +1586,17 @@ class VideoFrameTransform {
       const bool feathered = seamWidth && *seamWidth > 0.0f;
       if (feathered) gp.seamScale = lensSeamScale(*seamWidth);
       t360::PerFrameSource source = feathered ? t360::PerFrameSource::kLensBlend : t360::PerFrameSource::kLens;
+      UploadRing::Entry* motionStaged = nullptr;
       if (photo) {
-        source = t360::PerFrameSource::kLensPhoto;
-        for (int p = 0; p < f.numPlanes; ++p) gp.photo.plane[p] = lensPhotoPlane(*photo, rig->numLenses, p);
-        gp.photo.stats = stats;
+        source = moving ? t360::PerFrameSource::kLensMotion : t360::PerFrameSource::kLensPhoto;
+        t360::PerFrameGatherParams::LensPhoto& ph = moving ? gp.lensMotion.photo : gp.photo;
+        for (int p = 0; p < f.numPlanes; ++p) ph.plane[p] = lensPhotoPlane(*photo, rig->numLenses, p);
+        ph.stats = stats;
+        if (moving) gp.lensMotion.motion = stageMotion(*rig, *motion, gp.rig, slotFor(s), s, &motionStaged);
         if (stats) CU(cudaMemsetAsync(stats, 0, sizeof(unsigned long long) * t360::kPhotoStats * f.numPlanes, s));
       }
       perFrameGather(source, gp, ctx, f, f.in, f.inPitch, nullptr, /*transparent=*/true, tables, staged, nullptr, s);
+      releaseAfter(motionStaged, s);
       return true;
     });
   }
@@ -1507,7 +1609,9 @@ class VideoFrameTransform {
   //   - kCameraMip (mipCameraSample) without a photometry, after the planes' pyramids (buildPyramids);
   //   - kCameraPhoto / kStereoCamera (cameraPhotoSample<MIP, stereo>) with one, after the pyramids when a plane has a
   //     level, and with v.stats (device, [numPlanes][6]) the overlap's sums zeroed with a memset first and accumulated by
-  //     the same gather.
+  //     the same gather;
+  //   - kCameraMotion (cameraMotionSample<MIP>) for a moving view: kCameraPhoto's steps, and the motion's sample table
+  //     through the slot's upload ring.
   // rig == nullptr: the context's input under BORDER_WRAP; else the rig's lenses under BORDER_TRANSPARENT, with the lens
   // call's pre-fill.  Needs no plan and leaves the plans alone; no tables.
   bool transformFrameView(const char* what, const CameraView& v, const FramePlanes& f, cudaStream_t stream) {
@@ -1535,9 +1639,12 @@ class VideoFrameTransform {
       if (v.seamWidth > 0.0f) gp.seamScale = lensSeamScale(v.seamWidth);
       if (v.minify) gp.mipBias = mipBias(*v.minify);
       t360::PerFrameSource source = topMax > 0 ? t360::PerFrameSource::kCameraMip : t360::PerFrameSource::kRectilinear;
-      t360::PerFrameGatherParams::CameraPhoto& cp = gp.cameraPhoto;
+      t360::PerFrameGatherParams::CameraPhoto& cp = v.moving ? gp.cameraMotion.cameraPhoto : gp.cameraPhoto;
+      UploadRing::Entry* motionStaged = nullptr;
+      if (v.moving) gp.cameraMotion.motion = stageMotion(*v.rig, *v.motion, gp.rig, slotFor(s), s, &motionStaged);
       if (v.photometric) {
-        source = v.stereo ? t360::PerFrameSource::kStereoCamera : t360::PerFrameSource::kCameraPhoto;
+        source = v.stereo ? t360::PerFrameSource::kStereoCamera
+                          : (v.moving ? t360::PerFrameSource::kCameraMotion : t360::PerFrameSource::kCameraPhoto);
         for (int p = 0; p < f.numPlanes; ++p) {
           cp.mip[p].geometry = pyramids.mip[p].geometry;
           cp.photo.plane[p] = lensPhotoPlane(*v.photometry, v.rig->numLenses, p);
@@ -1558,6 +1665,7 @@ class VideoFrameTransform {
       }
       perFrameGather(source, gp, ctx, f, f.in, f.inPitch, nullptr, gp.lens, nullptr, nullptr, nullptr, s);
       releaseAfter(staged, s);
+      releaseAfter(motionStaged, s);
       return true;
     });
   }
@@ -2658,6 +2766,16 @@ class VideoFrameTransform {
     }
   }
 
+  // The motion's sample table (rigMotionTable) on the device for work enqueued next on s, through the slot's upload ring
+  // (*used: the entry to release after the launch), and the motion's per-frame constants pointing at it
+  t360::RigMotion stageMotion(const T360LensRig& rig, const T360RigMotion& motion, const t360::LensRigModel& model, StreamSlot& slot,
+                              cudaStream_t s, UploadRing::Entry** used) {
+    const std::vector<float> table = rigMotionTable(rig, motion, model);
+    const uint8_t* bytes = reinterpret_cast<const uint8_t*>(table.data());
+    slot.motionBytes.assign(bytes, bytes + table.size() * sizeof(float));
+    return rigMotion(motion, reinterpret_cast<const float*>(stageUpload(slot.motionTables, slot.motionBytes, s, used)));
+  }
+
   FrameTransformContext ctx_;
   // Every entry point that enqueues work holds configMu_ shared for as long as it uses a plan or ctx_; install() swaps the
   // plans and reconfigureAsync replaces ctx_ under it exclusively.  planMu_ serialises planning (generateMapForPlane,
@@ -3144,6 +3262,47 @@ T360_API int T360B200_transformFrameLensPhotoAsync(VideoFrameTransform* t, const
                      return vft.transformFrameLens(what, rig, &seamWidth, orientation, f, s, photometry, deviceStats);
                    });
 }
+T360_API int T360B200_lensMotionMaps(const FrameTransformContext* ctx, const T360LensRig* rig, const T360RigPhotometry* photometry, float seamWidth,
+                                     const T360Orientation* orientation, const T360RigMotion* motion, int plane, int inW, int inH, int outW,
+                                     int outH, float* map0, float* map1, uint16_t* weight, uint16_t* gain0, uint16_t* gain1) {
+  auto refused = [&](const FrameTransformContext& c, std::string* why) {
+    return lensPhotoRefused(c, rig, photometry, seamWidth, orientation, why) || motionRefused(*rig, motion, why) ||
+           indexRefused("plane", plane, 2, why) ||
+           outputsRefused({map0, map1, weight, gain0, gain1}, inW, inH, outW, outH,
+                          "a NULL map, weight or gain array or a plane size that is not positive", why);
+  };
+  return twinCall("Could not compute the lens motion maps", ctx, refused, [&](const FrameTransformContext& c) {
+    const t360::LensRigModel model = lensRigModel(*rig);
+    const std::vector<float> table = rigMotionTable(*rig, *motion, model);
+    const t360::RigMotion mo = rigMotion(*motion, table.data());
+    const t360::LensPhotoPlane ph = lensPhotoPlane(*photometry, rig->numLenses, plane);
+    const float s = seamWidth > 0.0f ? lensSeamScale(seamWidth) : 0.0f;
+    forLensPixels(c, *orientation, inW, inH, outW, outH, [&](const t360::SphereGeometry& g, const t360::Rotation& r, const float* colTab,
+                                                             const float* rowTab, int i, int j, size_t at) {
+      int g0, g1;
+      bool overlap;
+      weight[at] = static_cast<uint16_t>(t360::lensMotionPoint(g, r, model, mo, s, /*both=*/true, ph, colTab, rowTab, i, j, map0 + 2 * at,
+                                                               map1 + 2 * at, &g0, &g1, &overlap));
+      gain0[at] = static_cast<uint16_t>(g0);
+      gain1[at] = static_cast<uint16_t>(g1);
+    });
+  });
+}
+T360_API int T360B200_transformFrameLensMotionAsync(VideoFrameTransform* t, const T360LensRig* rig, const T360RigPhotometry* photometry,
+                                                    float seamWidth, const T360Orientation* orientation, const T360RigMotion* motion,
+                                                    unsigned long long* deviceStats, int numPlanes, const uint8_t* const* dIn, uint8_t* const* dOut,
+                                                    const int* inW, const int* inH, const int* inPitch, const int* outW, const int* outH,
+                                                    const int* outPitch, void* stream) {
+  const char* what = "Could not transform the frame of a lens rig with a rig motion";
+  if (t && !photometry) {  // (as the photometric call: without a photometry transformFrameLens is the plain lens call)
+    std::printf("%s. Error: a NULL photometry\n", what);
+    return 0;
+  }
+  return frameCall(what, t, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, stream,
+                   [&](VideoFrameTransform& vft, const FramePlanes& f, cudaStream_t s) {
+                     return vft.transformFrameLens(what, rig, &seamWidth, orientation, f, s, photometry, deviceStats, true, motion);
+                   });
+}
 namespace {
 int cameraMap(const char* what, const FrameTransformContext* ctx, const CameraView& v, int inW, int inH, int outW, int outH, float* map) {
   auto refused = [&](const FrameTransformContext& c, std::string* why) {
@@ -3157,9 +3316,9 @@ int cameraMap(const char* what, const FrameTransformContext* ctx, const CameraVi
     });
   });
 }
-// The twin of one lens and plane of a photometric (cameraPhotoMaps) or stereo (stereoCameraMaps) view:
-// cameraPhotoPoint<true, stereo> of every pixel with both lenses projected; lensWeight the seam weight or the eye weight
-// 256 e
+// The twin of one lens and plane of a photometric (cameraPhotoMaps), stereo (stereoCameraMaps) or moving
+// (cameraMotionMaps) view: cameraPhotoPoint<true, stereo> or cameraMotionPoint<true> of every pixel with both lenses
+// projected; lensWeight the seam weight or the eye weight 256 e
 int cameraPhotoMaps(const char* what, const FrameTransformContext* ctx, const CameraView& v, int lens, int plane, int inW, int inH, int outW,
                     int outH, float* map0, float* map1, uint8_t* level, uint16_t* weight, uint16_t* gain, uint16_t* lensWeight) {
   auto refused = [&](const FrameTransformContext& c, std::string* why) {
@@ -3170,12 +3329,15 @@ int cameraPhotoMaps(const char* what, const FrameTransformContext* ctx, const Ca
   return twinCall(what, ctx, refused, [&](const FrameTransformContext& c) {
     const t360::LensPhotoPlane ph = lensPhotoPlane(*v.photometry, v.rig->numLenses, plane);
     const float s = v.seamWidth > 0.0f ? lensSeamScale(v.seamWidth) : 0.0f;
+    const std::vector<float> table = v.moving ? rigMotionTable(*v.rig, *v.motion, lensRigModel(*v.rig)) : std::vector<float>{};
+    const t360::RigMotion mo = v.moving ? rigMotion(*v.motion, table.data()) : t360::RigMotion{};
     forCameraPixels(c, v, inW, inH, outW, outH, [&](const t360::SphereGeometry& g, const t360::RectilinearCamera& cam, const t360::LensRigModel& model,
                                                     const t360::MipGeometry& m, int bias, int i, int j, size_t at) {
       t360::CameraPhotoLens e[2];
       bool overlap;
-      lensWeight[at] = static_cast<uint16_t>(v.stereo ? t360::cameraPhotoPoint<true, true>(g, cam, model, m, bias, s, /*both=*/true, ph, i, j, e, &overlap)
-                                                      : t360::cameraPhotoPoint<true>(g, cam, model, m, bias, s, /*both=*/true, ph, i, j, e, &overlap));
+      lensWeight[at] = static_cast<uint16_t>(v.moving ? t360::cameraMotionPoint<true>(g, cam, model, mo, m, bias, s, /*both=*/true, ph, i, j, e, &overlap)
+                                             : v.stereo ? t360::cameraPhotoPoint<true, true>(g, cam, model, m, bias, s, /*both=*/true, ph, i, j, e, &overlap)
+                                                        : t360::cameraPhotoPoint<true>(g, cam, model, m, bias, s, /*both=*/true, ph, i, j, e, &overlap));
       map0[2 * at] = e[lens].p0[0];
       map0[2 * at + 1] = e[lens].p0[1];
       map1[2 * at] = e[lens].p1[0];
@@ -3261,6 +3423,22 @@ T360_API int T360B200_transformFrameCameraPhotoAsync(VideoFrameTransform* t, con
                                                      const int* outH, const int* outPitch, void* stream) {
   return transformFrameView("Could not transform the frame with a camera view of a lens rig with photometry", t,
                             photoView(rig, photometry, seamWidth, pose, camera, minify, deviceStats, false),
+                            numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, stream);
+}
+T360_API int T360B200_cameraMotionMaps(const FrameTransformContext* ctx, const T360LensRig* rig, const T360RigPhotometry* photometry, float seamWidth,
+                                       const T360Pose* pose, const T360Camera* camera, const T360Minify* minify, const T360RigMotion* motion, int lens,
+                                       int plane, int inW, int inH, int outW, int outH, float* map0, float* map1, uint8_t* level, uint16_t* weight,
+                                       uint16_t* gain, uint16_t* seamWeight) {
+  return cameraPhotoMaps("Could not compute the camera motion maps", ctx, motionView(rig, photometry, seamWidth, pose, camera, minify, motion, nullptr),
+                         lens, plane, inW, inH, outW, outH, map0, map1, level, weight, gain, seamWeight);
+}
+T360_API int T360B200_transformFrameCameraMotionAsync(VideoFrameTransform* t, const T360LensRig* rig, const T360RigPhotometry* photometry,
+                                                      float seamWidth, const T360Pose* pose, const T360Camera* camera, const T360Minify* minify,
+                                                      const T360RigMotion* motion, unsigned long long* deviceStats, int numPlanes,
+                                                      const uint8_t* const* dIn, uint8_t* const* dOut, const int* inW, const int* inH,
+                                                      const int* inPitch, const int* outW, const int* outH, const int* outPitch, void* stream) {
+  return transformFrameView("Could not transform the frame with a camera view of a lens rig with a rig motion", t,
+                            motionView(rig, photometry, seamWidth, pose, camera, minify, motion, deviceStats),
                             numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, stream);
 }
 T360_API int T360B200_stereoCameraMaps(const FrameTransformContext* ctx, const T360LensRig* rig, const T360RigPhotometry* photometry, const T360Pose* pose,

@@ -26,8 +26,11 @@
 //   - a camera view of a lens rig with photometry (CameraPhotoPositions): the camera view's ray, then both lenses' records,
 //     levels and gains (cameraPhotoSample); each lens's sample is the blend of its two levels, then the tile loop goes on
 //     as for LensPhotoPositions;
-//   - a camera view of a stereo rig (StereoCameraPositions): the same, with the output eye picking the lens.
-// In all ten, the records come from the same host/device functions the planner (or its host twin) uses: bit-identical.
+//   - a camera view of a stereo rig (StereoCameraPositions): the same, with the output eye picking the lens;
+//   - a lens rig or a camera view of one with photometry and a rig motion over the readout (LensMotionPositions,
+//     CameraMotionPositions): the photometric records with each lens's M following the readout time of its point
+//     (lensMotionSample, cameraMotionSample).
+// In all twelve, the records come from the same host/device functions the planner (or its host twin) uses: bit-identical.
 #include "gather_common.cuh"
 
 #include <algorithm>
@@ -404,6 +407,47 @@ struct StereoCameraPositions : CameraPhotoPositions<K, MIP> {
   }
 };
 
+// A lens rig with photometry and a rig motion (kLensMotion): LensPhotoPositions with each lens's M following the readout
+// time of the point it projects (lensMotionSample).  The motion's sample table is read with read-only global loads: at
+// most 1152 bytes and the same for every pixel of the launch, it stays in L1 (DESIGN.md section 5).
+template <int K, bool BARREL>
+struct LensMotionPositions : LensPhotoPositions<K, BARREL> {
+  using LensPhotoPositions<K, BARREL>::LensPhotoPositions;
+  __device__ int record(const PerFrameGatherParams& p, const PerFramePlane& v, int pl, int i, int j, int32_t* rec0, int32_t* rec1, int* g0,
+                        int* g1, bool* overlap) const {
+    const PerFrameGatherParams::LensMotion& m = p.lensMotion;
+    return lensMotionSample<BARREL>(v.geometry, p.rotation, p.rig, m.motion, p.seamScale, m.photo.stats != nullptr, m.photo.plane[pl],
+                                    v.colTable, v.rowTable, i, j, rec0, rec1, g0, g1, overlap);
+  }
+  __device__ static const PerFrameGatherParams::LensPhoto& photo(const PerFrameGatherParams& p) { return p.lensMotion.photo; }
+};
+
+// A camera view of a lens rig with photometry and a rig motion (kCameraMotion): CameraPhotoPositions' records, levels and
+// pixel blend, the records from cameraMotionSample.  The table as for LensMotionPositions.
+template <int, bool MIP>
+struct CameraMotionPositions : NoTables {
+  static constexpr bool kPhoto = true, kTransparent = true;
+  CameraPhotoRecords lens[2];
+  using NoTables::NoTables;
+  __device__ int record(const PerFrameGatherParams& p, const PerFramePlane& v, int pl, int i, int j, int32_t*, int32_t*, int* g0, int* g1,
+                        bool* overlap) {
+    const PerFrameGatherParams::CameraMotion& m = p.cameraMotion;
+    const PerFrameGatherParams::LensPhoto& photo = m.cameraPhoto.photo;
+    const int w = cameraMotionSample<MIP>(v.geometry, p.camera, p.rig, m.motion, m.cameraPhoto.mip[pl].geometry, p.mipBias, p.seamScale,
+                                          photo.stats != nullptr, photo.plane[pl], i, j, lens, overlap);
+    *g0 = lens[0].gain;
+    *g1 = lens[1].gain;
+    return w;
+  }
+  __device__ static const PerFrameGatherParams::LensPhoto& photo(const PerFrameGatherParams& p) { return p.cameraMotion.cameraPhoto.photo; }
+  template <int K, bool TRANSPARENT>
+  __device__ int pixel(const PerFrameGatherParams& p, int pl, const SrcView& s, const unsigned char* smem, int l, const int32_t*) const {
+    const CameraPhotoRecords& r = lens[l];
+    if constexpr (MIP) return levelPixel<K, TRANSPARENT>(p.cameraMotion.cameraPhoto.mip[pl].level, s, smem, r.level, r.rec0, r.rec1, r.w);
+    else return viewPixel<K, TRANSPARENT>(s, smem, r.rec0[0], r.rec0[1]);
+  }
+};
+
 template <class Pos, class = void>
 struct HasPinholeLoop : std::false_type {};
 template <class Pos>
@@ -493,6 +537,12 @@ cudaError_t launchPerFrameGather(PerFrameGatherParams p, PerFrameSource source, 
       for (int i = 0; i < p.numPlanes; ++i) mip = mip || p.cameraPhoto.mip[i].geometry.top > 0;
       if (source == PerFrameSource::kStereoCamera) return launchPositions<StereoCameraPositions>(p, mip, numTiles, numSMs, stream);
       return launchPositions<CameraPhotoPositions>(p, mip, numTiles, numSMs, stream);
+    }
+    case PerFrameSource::kLensMotion: return launchPositions<LensMotionPositions>(p, barrel, numTiles, numSMs, stream);
+    case PerFrameSource::kCameraMotion: {
+      bool mip = false;
+      for (int i = 0; i < p.numPlanes; ++i) mip = mip || p.cameraMotion.cameraPhoto.mip[i].geometry.top > 0;
+      return launchPositions<CameraMotionPositions>(p, mip, numTiles, numSMs, stream);
     }
   }
   return cudaErrorInvalidValue;

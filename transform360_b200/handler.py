@@ -186,6 +186,30 @@ class T360RigPhotometry(C.Structure):
     _fields_ = [("lumaPivot", C.c_int), ("lens", T360LensPhotometry * 2)]
 
 
+class T360LensReadout(C.Structure):
+    """When a lens reads a point (include/transform360_b200.h): t = a u + b v + c, clamped to [0, 1], of the point's
+    normalised calibration coordinates u = (fx x' + cx + 0.5) / calibWidth, v = (fy y' + cy + 0.5) / calibHeight."""
+    _fields_ = [("a", C.c_float), ("b", C.c_float), ("c", C.c_float)]
+
+
+class T360RigMotion(C.Structure):
+    """A rig's motion over the readout (include/transform360_b200.h): numSamples (2..16) orientations delta[k] of the rig
+    at readout time k / (numSamples - 1), turned from the frame's orientation or pose (degrees, each in [-30, 30]), and
+    each lens's readout (readout[1] is read only with two lenses)."""
+    _fields_ = [("numSamples", C.c_int), ("delta", T360Orientation * 16), ("readout", T360LensReadout * 2)]
+
+
+def rig_motion(deltas, readouts=((0.0, 1.0, 0.0), (0.0, 1.0, 0.0))) -> T360RigMotion:
+    """A T360RigMotion from a sequence of (yaw, pitch, roll) deltas (numSamples = len(deltas)) and one or two (a, b, c)
+    readouts."""
+    m = T360RigMotion(len(deltas))
+    for k, d in enumerate(deltas):
+        m.delta[k] = as_orientation(d)
+    for i, r in enumerate(readouts):
+        m.readout[i] = T360LensReadout(*[float(x) for x in r])
+    return m
+
+
 def make_context(**overrides) -> FrameTransformContext:
     vals = dict(FILTER_DEFAULTS)
     for k in overrides:
@@ -291,6 +315,12 @@ def load(path: os.PathLike | None = None):
     L.T360B200_transformFrameLensPhotoAsync.restype = ci
     L.T360B200_transformFrameLensPhotoAsync.argtypes = [vp, C.POINTER(T360LensRig), C.POINTER(T360RigPhotometry), C.c_float,
                                                         C.POINTER(T360Orientation), vp, ci] + planes
+    L.T360B200_lensMotionMaps.restype = ci
+    L.T360B200_lensMotionMaps.argtypes = [C.POINTER(FrameTransformContext), C.POINTER(T360LensRig), C.POINTER(T360RigPhotometry), C.c_float,
+                                          C.POINTER(T360Orientation), C.POINTER(T360RigMotion)] + [ci] * 5 + [vp] * 5
+    L.T360B200_transformFrameLensMotionAsync.restype = ci
+    L.T360B200_transformFrameLensMotionAsync.argtypes = [vp, C.POINTER(T360LensRig), C.POINTER(T360RigPhotometry), C.c_float,
+                                                         C.POINTER(T360Orientation), C.POINTER(T360RigMotion), vp, ci] + planes
     L.T360B200_rectilinearMap.restype = ci
     L.T360B200_rectilinearMap.argtypes = [C.POINTER(FrameTransformContext), C.POINTER(T360LensRig), C.POINTER(T360Pose)] + [ci] * 4 + [vp]
     L.T360B200_transformFrameRectilinearAsync.restype = ci
@@ -312,6 +342,13 @@ def load(path: os.PathLike | None = None):
     L.T360B200_transformFrameCameraPhotoAsync.restype = ci
     L.T360B200_transformFrameCameraPhotoAsync.argtypes = [vp, C.POINTER(T360LensRig), C.POINTER(T360RigPhotometry), C.c_float,
                                                           C.POINTER(T360Pose), C.POINTER(T360Camera), C.POINTER(T360Minify), vp, ci] + planes
+    L.T360B200_cameraMotionMaps.restype = ci
+    L.T360B200_cameraMotionMaps.argtypes = [C.POINTER(FrameTransformContext), C.POINTER(T360LensRig), C.POINTER(T360RigPhotometry), C.c_float,
+                                            C.POINTER(T360Pose), C.POINTER(T360Camera), C.POINTER(T360Minify), C.POINTER(T360RigMotion)] + [ci] * 6 + [vp] * 6
+    L.T360B200_transformFrameCameraMotionAsync.restype = ci
+    L.T360B200_transformFrameCameraMotionAsync.argtypes = [vp, C.POINTER(T360LensRig), C.POINTER(T360RigPhotometry), C.c_float,
+                                                           C.POINTER(T360Pose), C.POINTER(T360Camera), C.POINTER(T360Minify),
+                                                           C.POINTER(T360RigMotion), vp, ci] + planes
     L.T360B200_stereoCameraMaps.restype = ci
     L.T360B200_stereoCameraMaps.argtypes = [C.POINTER(FrameTransformContext), C.POINTER(T360LensRig), C.POINTER(T360RigPhotometry),
                                             C.POINTER(T360Pose), C.POINTER(T360Camera), C.POINTER(T360Minify)] + [ci] * 6 + [vp] * 6
@@ -355,6 +392,7 @@ EXPORTED_SYMBOLS = [
     "T360B200_rectilinearMap", "T360B200_transformFrameRectilinearAsync", "T360B200_cameraMap", "T360B200_transformFrameCameraAsync",
     "T360B200_cameraMipMaps", "T360B200_transformFrameCameraMipAsync", "T360B200_cameraPhotoMaps", "T360B200_transformFrameCameraPhotoAsync",
     "T360B200_stereoCameraMaps", "T360B200_transformFrameStereoCameraAsync",
+    "T360B200_lensMotionMaps", "T360B200_transformFrameLensMotionAsync", "T360B200_cameraMotionMaps", "T360B200_transformFrameCameraMotionAsync",
     "T360B200_setPinHostPlanes", "T360B200_debugTrace", "T360B200_debugTraceRead", "T360B200_synchronize", "T360B200_stream", "T360B200_kernelLaunchCount", "T360B200_planDeviceBytes",
     "T360B200_planTileCounts", "T360B200_deviceCount", "T360B200_version",
 ]
@@ -476,6 +514,14 @@ class VideoFrameTransform:
         return lambda rig, photometry, seam_width, orientation, stream=0, stats=0: enqueue(
             (C.byref(rig), C.byref(photometry), seam_width, C.byref(as_orientation(orientation)), stats or None, n), stream)
 
+    def make_lens_motion_frame_call(self, in_planes, out_planes, dims):
+        """Like make_lens_photo_frame_call, for T360B200_transformFrameLensMotionAsync (a rig with photometry and a rig
+        motion over the readout): returns a callable f(rig, photometry, seam_width, orientation, motion, stream=0, stats=0)
+        -> bool, `motion` a T360RigMotion."""
+        n, enqueue = self._frame_call("T360B200_transformFrameLensMotionAsync", in_planes, out_planes, dims)
+        return lambda rig, photometry, seam_width, orientation, motion, stream=0, stats=0: enqueue(
+            (C.byref(rig), C.byref(photometry), seam_width, C.byref(as_orientation(orientation)), C.byref(motion), stats or None, n), stream)
+
     def make_rectilinear_frame_call(self, in_planes, out_planes, dims):
         """Like make_frame_call, for T360B200_transformFrameRectilinearAsync (a perspective view, no plan needed): returns a
         callable f(pose, stream, rig=None) -> bool that enqueues the whole frame with `pose` (a T360Pose or (yaw, pitch,
@@ -509,6 +555,15 @@ class VideoFrameTransform:
         return lambda rig, photometry, seam_width, pose, camera, minify=None, stream=0, stats=0: enqueue(
             (C.byref(rig), C.byref(photometry), seam_width, C.byref(as_pose(pose)), C.byref(as_camera(camera)),
              C.byref(as_minify(minify)) if minify is not None else None, stats or None, n), stream)
+
+    def make_camera_motion_frame_call(self, in_planes, out_planes, dims):
+        """Like make_camera_photo_frame_call, for T360B200_transformFrameCameraMotionAsync (a camera view of a rig with
+        photometry and a rig motion over the readout): returns a callable f(rig, photometry, seam_width, pose, camera,
+        minify, motion, stream=0, stats=0) -> bool, `minify` None for no pyramid and `motion` a T360RigMotion."""
+        n, enqueue = self._frame_call("T360B200_transformFrameCameraMotionAsync", in_planes, out_planes, dims)
+        return lambda rig, photometry, seam_width, pose, camera, minify, motion, stream=0, stats=0: enqueue(
+            (C.byref(rig), C.byref(photometry), seam_width, C.byref(as_pose(pose)), C.byref(as_camera(camera)),
+             C.byref(as_minify(minify)) if minify is not None else None, C.byref(motion), stats or None, n), stream)
 
     def make_stereo_camera_frame_call(self, in_planes, out_planes, dims):
         """Like make_camera_photo_frame_call, for T360B200_transformFrameStereoCameraAsync (a camera view of a stereo rig:
@@ -810,6 +865,19 @@ def lens_photo_maps(ctx: FrameTransformContext, rig: T360LensRig, photometry: T3
     return map0, map1, weight, gain0, gain1
 
 
+def lens_motion_maps(ctx: FrameTransformContext, rig: T360LensRig, photometry: T360RigPhotometry, seam_width, orientation,
+                     motion: T360RigMotion, plane, in_w, in_h, out_w, out_h) -> tuple[np.ndarray, np.ndarray, np.ndarray, np.ndarray, np.ndarray]:
+    """The host twin of one plane of a rig with photometry and a rig motion over the readout (T360B200_lensMotionMaps, no
+    CUDA): lens_photo_maps' (map0, map1, weight, gain0, gain1) with each lens's M following the readout time of its point."""
+    map0, map1 = np.empty((out_h, out_w, 2), np.float32), np.empty((out_h, out_w, 2), np.float32)
+    weight, gain0, gain1 = (np.empty((out_h, out_w), np.uint16) for _ in range(3))
+    if not load().T360B200_lensMotionMaps(C.byref(ctx), C.byref(rig), C.byref(photometry), seam_width, C.byref(as_orientation(orientation)),
+                                          C.byref(motion), plane, in_w, in_h, out_w, out_h, map0.ctypes.data, map1.ctypes.data,
+                                          weight.ctypes.data, gain0.ctypes.data, gain1.ctypes.data):
+        raise ValueError("T360B200_lensMotionMaps refused the arguments (message on stdout)")
+    return map0, map1, weight, gain0, gain1
+
+
 def rectilinear_map(ctx: FrameTransformContext, pose, in_w, in_h, out_w, out_h, rig: T360LensRig | None = None) -> np.ndarray:
     """The CV_32FC2 map of one plane of a rectilinear view (T360B200_rectilinearMap, no CUDA): float32 [out_h][out_w][2],
     the source x, y of every output pixel in a plane of in_w x in_h, from the context's input, or from `rig` (NaN where no
@@ -865,6 +933,22 @@ def camera_photo_maps(ctx: FrameTransformContext, rig: T360LensRig, photometry: 
                                            plane, in_w, in_h, out_w, out_h, map0.ctypes.data, map1.ctypes.data, level.ctypes.data,
                                            weight.ctypes.data, gain.ctypes.data, seam_weight.ctypes.data):
         raise ValueError("T360B200_cameraPhotoMaps refused the arguments (message on stdout)")
+    return map0, map1, level, weight, gain, seam_weight
+
+
+def camera_motion_maps(ctx: FrameTransformContext, rig: T360LensRig, photometry: T360RigPhotometry, seam_width, pose, camera, minify,
+                       motion: T360RigMotion, lens, plane, in_w, in_h, out_w, out_h) -> tuple[np.ndarray, ...]:
+    """The host twin of one lens of one plane of a camera view of a rig with photometry and a rig motion
+    (T360B200_cameraMotionMaps, no CUDA): camera_photo_maps' (map0, map1, level, weight, gain, seam_weight)."""
+    shape = (max(out_h, 0), max(out_w, 0))
+    map0, map1 = np.zeros(shape + (2,), np.float32), np.zeros(shape + (2,), np.float32)
+    level = np.zeros(shape, np.uint8)
+    weight, gain, seam_weight = (np.zeros(shape, np.uint16) for _ in range(3))
+    if not load().T360B200_cameraMotionMaps(C.byref(ctx), C.byref(rig), C.byref(photometry), seam_width, C.byref(as_pose(pose)),
+                                            C.byref(as_camera(camera)), C.byref(as_minify(minify)) if minify is not None else None,
+                                            C.byref(motion), lens, plane, in_w, in_h, out_w, out_h, map0.ctypes.data, map1.ctypes.data,
+                                            level.ctypes.data, weight.ctypes.data, gain.ctypes.data, seam_weight.ctypes.data):
+        raise ValueError("T360B200_cameraMotionMaps refused the arguments (message on stdout)")
     return map0, map1, level, weight, gain, seam_weight
 
 
