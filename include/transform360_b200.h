@@ -582,6 +582,56 @@ int T360B200_transformFrameCameraMipAsync(VideoFrameTransform* transform, const 
                                           const uint8_t* const* deviceInputs, uint8_t* const* deviceOutputs, const int* inputWidths,
                                           const int* inputHeights, const int* inputPitches, const int* outputWidths,
                                           const int* outputHeights, const int* outputPitches, void* cudaStream);
+/* ---- anisotropic camera views ------------------------------------------------------------------------------------
+ * The anti-aliased views above pick one level per pixel from the longer footprint axis, so where the footprint is a long
+ * thin ellipse (a little planet's outer ring, the rim of a wide dome, an equirect camera near its poles, any oblique
+ * view) the short axis is blurred as much as the long one.  These calls read the pyramid with N probes per pixel spread
+ * along its longer axis, each at the level of max(long / N, short): the probes along the major axis of hardware
+ * anisotropic filtering (McCormack et al., Feline, 1999), with the longer screen-axis derivative in place of the
+ * ellipse's true major axis.  Steps 1-2 of the anti-aliased views (the pyramid; the footprint a, b of the centre ray)
+ * are unchanged; aa = a.a and bb = b.b as there.  Each step below is computed bit for bit alike on host and device:
+ *   1. probe count and level: where aa or bb is not below +inf (an exact pole, NaN), step 3 of the anti-aliased views
+ *      with N = 1.  Otherwise, with L(x) = ((int32) bits(x) - 0x3f800000) >> 16: lmaj = L(max(aa, bb)), lmin =
+ *      L(min(aa, bb)), e = min((lmaj - lmin + 255) >> 8, log2 maxProbes), N = 1 << e, lambda = max(lmaj - 256 e, lmin) +
+ *      round(256 lodBias); level and next-level weight follow from lambda as in step 3 (clamped to [0, T], w = lambda &
+ *      255 inside).  A zero aa or bb gives the largest N.  The footprint is taken wherever T > 0 or maxProbes > 1, so
+ *      maxLevel = 0 with maxProbes > 1 supersamples level 0 along the long axis;
+ *   2. probe rays: the axis is the column axis where aa >= bb, the row axis otherwise.  Probe k (0..N-1) sits at o_k =
+ *      (2k + 1 - N) / N (exact in float): Xk = X + o_k dX / 2 on the column axis, Yk = Y + o_k dY / 2 on the row axis,
+ *      each operation rounded to float (with N = 1 the centre ray itself, no offset added).  Each probe takes the camera
+ *      view's whole chain (the model's ray, the pose, then the context's input lookup with the pixel's eye or the rig's
+ *      closer lens), so on cube-map input each probe picks its own face and on a rig its own lens.  Its entries at level
+ *      and level + 1 are step 4's; all probes share the pixel's level and weight;
+ *   3. pixel: v_k is step 5 of the anti-aliased views on probe k's entries.  BORDER_WRAP (the context's input): (sum v_k +
+ *      N / 2) >> e.  BORDER_TRANSPARENT (a rig): a probe whose two samples are both skipped drops out, and with n probes
+ *      left the pixel is (sum v_k + n / 2) / n (integer division); n = 0 keeps the output's bytes (the pre-fill).
+ * maxProbes = 1 gives T360B200_transformFrameCameraMipAsync byte for byte (records, levels, weights, frames), and with
+ * maxLevel = 0 T360B200_transformFrameCameraAsync.  A frame takes the camera-mip call's launches: T_max + 1 (one per
+ * pyramid level, then the gather), or one without a pyramid.  The probe loop multiplies a pixel's chain and gathers by
+ * its N.  There is no planned path: a plan carries one record per pixel.
+ *
+ * Refused, with 0 and a message on stdout before any CUDA call: every refusal of T360B200_transformFrameCameraMipAsync,
+ * then a maxProbes other than 1, 2, 4, 8 or 16. */
+/* Host only, no CUDA: the twin of one plane of inputWidth x inputHeight.  map0 / map1: float32 [maxProbes][outputHeight]
+ * [outputWidth][2], probe k's entry in its level's pixels / in level + 1's pixels (map1 NaN where the weight is 0; both
+ * NaN for k >= N); level: uint8 [outputHeight][outputWidth]; weight: uint16, the next level's weight; probes: uint8, N.
+ * cv::remap of each probe's entries over the pyramid, each probe's levels blended as in step 5 of the anti-aliased views,
+ * then the probes averaged as in step 3, gives the plane of T360B200_transformFrameCameraAnisoAsync bit for bit.  With
+ * maxProbes = 1, probe 0 is T360B200_cameraMipMaps' arrays.  Returns 1; 0 (message) for the refusals above, a NULL context
+ * or array, or non-positive sizes. */
+int T360B200_cameraAnisoMaps(const FrameTransformContext* ctx, const T360LensRig* rig, const T360Pose* pose, const T360Camera* camera,
+                             const T360Minify* minify, int maxProbes, int inputWidth, int inputHeight, int outputWidth, int outputHeight,
+                             float* map0, float* map1, uint8_t* level, uint16_t* weight, uint8_t* probes);
+/* One frame of an anisotropic camera view: T360B200_transformFrameCameraMipAsync's arguments and asynchronous contract,
+ * plus maxProbes, which may change every frame like the rig, pose, camera and minify.  Needs no plan and does not touch
+ * the plans; takes the reader lock; never synchronises the device; the pyramids use the camera-mip call's scratch.
+ * Returns 1 if everything was enqueued; 0 with a message on stdout, before any CUDA call, for the refusals above, 0 or
+ * more than 3 planes, or an invalid plane description. */
+int T360B200_transformFrameCameraAnisoAsync(VideoFrameTransform* transform, const T360LensRig* rig, const T360Pose* pose,
+                                            const T360Camera* camera, const T360Minify* minify, int maxProbes, int numPlanes,
+                                            const uint8_t* const* deviceInputs, uint8_t* const* deviceOutputs, const int* inputWidths,
+                                            const int* inputHeights, const int* inputPitches, const int* outputWidths,
+                                            const int* outputHeights, const int* outputPitches, void* cudaStream);
 /* ---- camera views of a lens rig with photometry ----------------------------------------------------------
  * The camera views above take a rig's hard, uncorrected seam, so a view panned across the seam of a dual-fisheye clip
  * shows the step the lens photometry removes from sphere outputs.  This call gives the rectilinear view (the pinhole

@@ -409,8 +409,11 @@ void countKernelLaunches(long long n);  // kernels launched through a replayed C
 //                 the point it projects.
 //   kCameraMotion kCameraPhoto with a rig motion (cameraMotion: kCameraPhoto's constants and the motion;
 //                 cameraMotionSample).
+//   kCameraAniso  anisotropic camera views (kCameraMip's constants and cameraAniso; anisoFootprint, anisoCameraSample):
+//                 the pixel's footprint once, then up to 2^cameraAniso probes along its longer axis, each gathered as
+//                 kCameraMip gathers a pixel, averaged over the probes BORDER_TRANSPARENT does not skip.
 enum class PerFrameSource { kView, kSphere, kMap, kLens, kLensBlend, kRectilinear, kCameraMip, kLensPhoto, kCameraPhoto, kStereoCamera,
-                            kLensMotion, kCameraMotion };
+                            kLensMotion, kCameraMotion, kCameraAniso };
 struct PerFramePlane {
   const uint8_t* src;  // (blurred) input plane, geometry.inW x geometry.inH
   uint8_t* dst;        // render target, geometry.mapW x geometry.mapH
@@ -433,6 +436,7 @@ struct PerFrameGatherParams {
   float seamScale;   // s = 1 / (2 seamWidth), seamWidth in radians
   bool transparent;  // kMap: BORDER_TRANSPARENT instead of BORDER_WRAP
   bool lens;         // kRectilinear: the rig's lenses instead of the context's input
+  uint8_t cameraAniso;  // kCameraAniso: log2 maxProbes (in the padding before weights, so no member moves)
   const int16_t* weights;  // device copy of the [1024][k][k] table (nullptr for nearest)
   int kernelSize;
   // kCameraMip: per plane its footprint constants and pyramid levels 1..geometry.top (level 0 is the plane's src), and
@@ -493,6 +497,9 @@ static_assert(sizeof(PerFrameGatherParams::LensMotion) <= sizeof(PerFrameGatherP
 static_assert(sizeof(PerFrameGatherParams::CameraMotion) <= sizeof(PerFrameGatherParams::MipPlane) * kMaxFramePlanes);
 // (the block the kernels were compiled against before the motion sources: its size and where its last member lies)
 static_assert(sizeof(PerFrameGatherParams) == 1496 && offsetof(PerFrameGatherParams, mipBias) == 1488);
+// (cameraAniso takes two bytes of padding: weights and every member after it stay where the kernels read them)
+static_assert(offsetof(PerFrameGatherParams, cameraAniso) < offsetof(PerFrameGatherParams, weights) &&
+              offsetof(PerFrameGatherParams, weights) == 632);
 constexpr int kPhotoStats = 6;  // sums per plane of kLensPhoto's statistics
 // a CTA takes tiles of 32 output columns x viewTileRows(k) rows; a thread owns one column of a tile and walks down
 // kViewRowsPerThread of its rows

@@ -1071,6 +1071,123 @@ T360_HD int mipCameraSample(const SphereGeometry& g, const RectilinearCamera& c,
   return level;
 }
 
+// ---- anisotropic camera views (T360B200_cameraAnisoMaps, T360B200_transformFrameCameraAnisoAsync) --------------------
+// The anti-aliased view's footprint a, b, read by N = 2^e probes spread along its longer screen axis (the column axis
+// where a.a >= b.b, else the row axis), each probe at the level of max(long / N, short): the probes along the major axis
+// of hardware anisotropic filtering (McCormack et al. 1999), with the longer screen-axis derivative in place of the
+// ellipse's true major axis.  With N = 1 the probe is the centre ray, and the records are mipCameraSample's.
+// (These are written beside mipCameraPoint rather than through it: built on a shared footprint step, the anti-aliased
+// views' kernels compile to different SASS.)
+
+// lambda256 of the longer and the shorter axis, L(x) = ((int32) bits(x) - 0x3f800000) >> 16 as mipLevelOf takes it;
+// e = min(ceil((L(max) - L(min)) / 256), maxLog2), lambda256 = max(L(max) - 256 e, L(min)) + bias256, and the level and
+// next-level weight from lambda256 as mipLevelOf takes them.  Where aa or bb is not below +inf (an exact pole, NaN),
+// mipLevelOf itself with e = 0.  A zero or denormal axis gives e = maxLog2.  Returns the level.
+T360_HD int anisoLevelOf(float aa, float bb, int top, int bias256, int maxLog2, int* w, int* e) {
+  const float inf = bitsFloat(0x7f800000u);
+  *e = 0;
+  if (!(aa < inf && bb < inf)) return mipLevelOf(aa, bb, top, bias256, w);
+  const int hi = (static_cast<int32_t>(floatBits(aa > bb ? aa : bb)) - 0x3f800000) >> 16;
+  const int lo = (static_cast<int32_t>(floatBits(aa > bb ? bb : aa)) - 0x3f800000) >> 16;
+  const int steps = (hi - lo + 255) >> 8;
+  *e = steps < maxLog2 ? steps : maxLog2;
+  const int shortened = hi - 256 * *e;
+  const int lam = (shortened > lo ? shortened : lo) + bias256;
+  *w = lam >= 0 && lam < 256 * top ? (lam & 255) : 0;
+  const int level = lam >> 8;
+  return level < 0 ? 0 : (level > top ? top : level);
+}
+
+// The centre of output pixel (i, j) of an anisotropic camera view and what its probes share: the footprint is taken
+// wherever there is a pyramid or more than one probe (maxLog2 > 0), as mipCameraPoint takes it, else level 0, weight 0, e 0.
+struct AnisoFootprint {
+  float X, Y;       // the pixel's centre (cameraXY)
+  SphereVec t;      // its rotated ray
+  bool eye;         // its output eye
+  bool rows;        // the probes lie along the row axis (Y), not the column axis (X)
+  int level, w, e;  // the probes' level, the next level's weight (0..255), log2 of the probe count
+};
+template <bool LENS>
+T360_HD AnisoFootprint anisoFootprint(const SphereGeometry& g, const RectilinearCamera& c, const LensRigModel& rig, const MipGeometry& m,
+                                      int bias256, int maxLog2, int i, int j) {
+  AnisoFootprint f{};
+  cameraXY(g, i, j, &f.X, &f.Y, &f.eye);
+  f.t = rotateHD(c.r, modelRay(c, f.X, f.Y));
+  if (m.top > 0 || maxLog2 > 0) {
+    const SphereVec& t = f.t;
+    const SphereVec rx = rayDifferential(c, fSub(f.X, m.halfX), f.Y, fAdd(f.X, m.halfX), f.Y);
+    const SphereVec ry = rayDifferential(c, f.X, fSub(f.Y, m.halfY), f.X, fAdd(f.Y, m.halfY));
+    float a[2], b[2];
+    if constexpr (LENS) {
+      lensJacobian(rig, t, rx, ry, g.inW, g.inH, a, b);
+    } else if (g.cubeInput) {
+      const float n = fSqrt(fAdd(fAdd(fMul(t.x, t.x), fMul(t.y, t.y)), fMul(t.z, t.z)));
+      const int face = cubeInputFace(fDiv(t.x, n), fDiv(t.y, n), fDiv(t.z, n));
+      const float nan = bitsFloat(0x7fc00000u);
+      a[0] = a[1] = b[0] = b[1] = nan;
+      if (face >= 0) {
+        cubeJacobian(g, face, t, rx, &a[0], &a[1]);
+        cubeJacobian(g, face, t, ry, &b[0], &b[1]);
+      }
+    } else {
+      equirectJacobian(g, t, rx, &a[0], &a[1]);
+      equirectJacobian(g, t, ry, &b[0], &b[1]);
+    }
+    const float aa = fAdd(fMul(a[0], a[0]), fMul(a[1], a[1])), bb = fAdd(fMul(b[0], b[0]), fMul(b[1], b[1]));
+    f.level = anisoLevelOf(aa, bb, m.top, bias256, maxLog2, &f.w, &f.e);
+    f.rows = !(aa >= bb);
+  }
+  return f;
+}
+
+// The map entries of probe k (0..2^f.e - 1) of footprint f: p0 in level f.level's pixels, p1 in level + 1's (NaN where
+// f.w = 0).  The probe's centre is X + o_k dX / 2 (or Y + o_k dY / 2 on the row axis), o_k = (2k + 1 - N) / N (exact for
+// N a power of two), each step rounded to float; with N = 1 it is the pixel's centre ray as it is.  Each probe takes the
+// camera view's whole lookup, so on cube-map input it picks its own face and on a rig its own closer lens.
+template <bool LENS>
+T360_HD void anisoCameraPoint(const SphereGeometry& g, const RectilinearCamera& c, const LensRigModel& rig, const MipGeometry& m,
+                              const AnisoFootprint& f, int k, float* p0, float* p1) {
+  SphereVec t = f.t;
+  if (f.e > 0) {
+    const int n = 1 << f.e;
+    const float o = fDiv(static_cast<float>(2 * k + 1 - n), static_cast<float>(n));
+    t = f.rows ? rotateHD(c.r, modelRay(c, f.X, fAdd(f.Y, fMul(o, m.halfY))))
+               : rotateHD(c.r, modelRay(c, fAdd(f.X, fMul(o, m.halfX)), f.Y));
+  }
+  float px, py;
+  if constexpr (LENS) {
+    lensPosition(rig, t, g.inW, g.inH, &px, &py);
+  } else {
+    float u, v;
+    sphereInputHD(g, false, f.eye, t, &u, &v);
+    px = toPixel(u, g.inW);
+    py = toPixel(v, g.inH);
+  }
+  p0[0] = f.level ? mipScale(px, m.sx[f.level]) : px;
+  p0[1] = f.level ? mipScale(py, m.sy[f.level]) : py;
+  const float nan = bitsFloat(0x7fc00000u);
+  p1[0] = f.w ? mipScale(px, m.sx[f.level + 1]) : nan;
+  p1[1] = f.w ? mipScale(py, m.sy[f.level + 1]) : nan;
+}
+
+// The sampling records of probe k: anisoCameraPoint's entries quantised as mipCameraSample quantises its entries (rec1
+// only where f.w > 0)
+template <bool LENS>
+T360_HD void anisoCameraSample(const SphereGeometry& g, const RectilinearCamera& c, const LensRigModel& rig, const MipGeometry& m,
+                               const AnisoFootprint& f, int k, int32_t* rec0, int32_t* rec1) {
+  float p0[2], p1[2];
+  anisoCameraPoint<LENS>(g, c, rig, m, f, k, p0, p1);
+  int r0, fracX, fracY;
+  quantizeAxis(p0[0], g.kernelSize, &rec0[0], &fracX);
+  quantizeAxis(p0[1], g.kernelSize, &r0, &fracY);
+  rec0[1] = r0 * 1024 + fracY * 32 + fracX;
+  if (f.w) {
+    quantizeAxis(p1[0], g.kernelSize, &rec1[0], &fracX);
+    quantizeAxis(p1[1], g.kernelSize, &r0, &fracY);
+    rec1[1] = r0 * 1024 + fracY * 32 + fracX;
+  }
+}
+
 // ---- camera views of a lens rig with photometry (T360B200_cameraPhotoMaps, T360B200_transformFrameCameraPhotoAsync) ---
 // The camera view's ray (cameraXY, modelRay, rotateHD: the rig is mono), then lensPhotoPosition as the photometric lens
 // call applies it; with a pyramid each lens that covers the ray takes its own footprint from its own Kannala-Brandt

@@ -803,7 +803,8 @@ constexpr T360Camera kPinhole{T360_CAMERA_PINHOLE, 0.0f};
 // What a camera call was given; the arguments a call does not take stay NULL / 0.  rig == nullptr: a view of the
 // context's input.  photometric: the call corrects the rig's lenses, so it needs a rig and a photometry (the photometric
 // and stereo calls); stereo: each eye takes its own lens (no seam).  minify == nullptr: no pyramid.  motion: a rig motion
-// over the readout (the camera-motion calls: a photometric view).
+// over the readout (the camera-motion calls: a photometric view).  aniso: the anisotropic calls, maxProbes probes per
+// pixel along its footprint's longer axis (a plain view with a minify).
 struct CameraView {
   const T360LensRig* rig = nullptr;
   const T360RigPhotometry* photometry = nullptr;
@@ -816,6 +817,8 @@ struct CameraView {
   bool stereo = false;
   const T360RigMotion* motion = nullptr;
   bool moving = false;  // (the camera-motion calls: motion is checked, NULL included)
+  int maxProbes = 1;
+  bool aniso = false;   // (the anisotropic calls: maxProbes is checked, and so is a NULL minify)
 };
 // A view of ctx's input (rig == nullptr) or of a rig's lenses as they are: the rectilinear, camera and camera-mip calls
 CameraView plainView(const T360LensRig* rig, const T360Pose* pose, const T360Camera* camera, const T360Minify* minify = nullptr) {
@@ -833,6 +836,28 @@ CameraView motionView(const T360LensRig* rig, const T360RigPhotometry* photometr
   v.motion = motion;
   v.moving = true;
   return v;
+}
+
+// A view of ctx's input or of a rig's lenses with up to maxProbes probes per pixel: the anisotropic calls
+CameraView anisoView(const T360LensRig* rig, const T360Pose* pose, const T360Camera* camera, const T360Minify* minify, int maxProbes) {
+  CameraView v = plainView(rig, pose, camera, minify);
+  v.maxProbes = maxProbes;
+  v.aniso = true;
+  return v;
+}
+
+// true, with the reason in *why, when maxProbes is not a power of two in 1..16
+bool maxProbesRefused(int maxProbes, std::string* why) {
+  if (maxProbes == 1 || maxProbes == 2 || maxProbes == 4 || maxProbes == 8 || maxProbes == 16) return false;
+  *why = formatted("maxProbes %d is not 1, 2, 4, 8 or 16", maxProbes);
+  return true;
+}
+
+// log2 maxProbes, the form the footprint and the kernels take it in
+int probesLog2(int maxProbes) {
+  int e = 0;
+  while ((2 << e) <= maxProbes) ++e;
+  return e;
 }
 
 // true, with the reason in *why, when `minify` is NULL or out of range
@@ -855,8 +880,9 @@ bool minifyRefused(const T360Minify* minify, std::string* why) {
 // true, with the reason in *why, when view v of ctx's input or of its rig cannot be rendered, in this order: a photometric
 // view's NULL rig; a stereo rig without two lenses or an output_stereo_format other than TB, LR or MONO; the pose, the
 // camera and its fields of view, the rig (rigRefused), the low-pass filter and the interpolation; a photometric view's
-// seam (seamWidthRefused, featherRefused) and photometry (photometryRefused); the minify where there is one; a moving
-// view's motion (motionRefused).  The output layout plays no part: the pose replaces it.
+// seam (seamWidthRefused, featherRefused) and photometry (photometryRefused); the minify where there is one (an
+// anisotropic view's NULL minify included); a moving view's motion (motionRefused); an anisotropic view's maxProbes
+// (maxProbesRefused).  The output layout plays no part: the pose replaces it.
 bool viewRefused(const FrameTransformContext& ctx, const CameraView& v, std::string* why) {
   if (v.photometric && !v.rig) {
     *why = v.stereo ? "a NULL rig (a stereo rig's lenses are its eyes)" : "a NULL rig (the photometry corrects a rig's lenses)";
@@ -931,8 +957,9 @@ bool viewRefused(const FrameTransformContext& ctx, const CameraView& v, std::str
     if (seamWidthRefused(v.seamWidth, why) || (v.seamWidth > 0.0f && featherRefused(*v.rig, v.seamWidth, why))) return true;
     if (photometryRefused(*v.rig, v.photometry, why)) return true;
   }
-  if (v.minify && minifyRefused(v.minify, why)) return true;
-  return v.moving && motionRefused(*v.rig, v.motion, why);
+  if ((v.minify || v.aniso) && minifyRefused(v.minify, why)) return true;
+  if (v.moving && motionRefused(*v.rig, v.motion, why)) return true;
+  return v.aniso && maxProbesRefused(v.maxProbes, why);
 }
 
 // The per-frame constants of v's pose and camera (oriented_view.h: cameraConstants)
@@ -1611,7 +1638,10 @@ class VideoFrameTransform {
   //     level, and with v.stats (device, [numPlanes][6]) the overlap's sums zeroed with a memset first and accumulated by
   //     the same gather;
   //   - kCameraMotion (cameraMotionSample<MIP>) for a moving view: kCameraPhoto's steps, and the motion's sample table
-  //     through the slot's upload ring.
+  //     through the slot's upload ring;
+  //   - kCameraAniso (anisoFootprint, anisoCameraSample) for an anisotropic view with maxProbes > 1, after the pyramids
+  //     when a plane has a level (without one, the probes supersample level 0).  With maxProbes = 1 its records are
+  //     kCameraMip's (kRectilinear's without a level), so it takes that source.
   // rig == nullptr: the context's input under BORDER_WRAP; else the rig's lenses under BORDER_TRANSPARENT, with the lens
   // call's pre-fill.  Needs no plan and leaves the plans alone; no tables.
   bool transformFrameView(const char* what, const CameraView& v, const FramePlanes& f, cudaStream_t stream) {
@@ -1639,6 +1669,11 @@ class VideoFrameTransform {
       if (v.seamWidth > 0.0f) gp.seamScale = lensSeamScale(v.seamWidth);
       if (v.minify) gp.mipBias = mipBias(*v.minify);
       t360::PerFrameSource source = topMax > 0 ? t360::PerFrameSource::kCameraMip : t360::PerFrameSource::kRectilinear;
+      if (v.aniso && v.maxProbes > 1) {
+        source = t360::PerFrameSource::kCameraAniso;
+        gp.cameraAniso = static_cast<uint8_t>(probesLog2(v.maxProbes));
+        for (int p = 0; p < f.numPlanes; ++p) gp.mip[p].geometry = pyramids.mip[p].geometry;  // (the levels follow below)
+      }
       t360::PerFrameGatherParams::CameraPhoto& cp = v.moving ? gp.cameraMotion.cameraPhoto : gp.cameraPhoto;
       UploadRing::Entry* motionStaged = nullptr;
       if (v.moving) gp.cameraMotion.motion = stageMotion(*v.rig, *v.motion, gp.rig, slotFor(s), s, &motionStaged);
@@ -3406,6 +3441,53 @@ T360_API int T360B200_transformFrameCameraMipAsync(VideoFrameTransform* t, const
                        return false;
                      }
                      return vft.transformFrameView(what, plainView(rig, pose, camera, minify), f, s);
+                   });
+}
+T360_API int T360B200_cameraAnisoMaps(const FrameTransformContext* ctx, const T360LensRig* rig, const T360Pose* pose, const T360Camera* camera,
+                                      const T360Minify* minify, int maxProbes, int inW, int inH, int outW, int outH, float* map0, float* map1,
+                                      uint8_t* level, uint16_t* weight, uint8_t* probes) {
+  const CameraView v = anisoView(rig, pose, camera, minify, maxProbes);
+  auto refused = [&](const FrameTransformContext& c, std::string* why) {
+    return viewRefused(c, v, why) || outputsRefused({map0, map1, level, weight, probes}, inW, inH, outW, outH,
+                                                    "a NULL map, level, weight or probes array or a plane size that is not positive", why);
+  };
+  return twinCall("Could not compute the camera aniso maps", ctx, refused, [&](const FrameTransformContext& c) {
+    const int maxLog2 = probesLog2(maxProbes);
+    const size_t plane = static_cast<size_t>(outW) * outH;
+    forCameraPixels(c, v, inW, inH, outW, outH, [&](const t360::SphereGeometry& g, const t360::RectilinearCamera& cam, const t360::LensRigModel& model,
+                                                    const t360::MipGeometry& m, int bias, int i, int j, size_t at) {
+      const t360::AnisoFootprint f = rig ? t360::anisoFootprint<true>(g, cam, model, m, bias, maxLog2, i, j)
+                                         : t360::anisoFootprint<false>(g, cam, model, m, bias, maxLog2, i, j);
+      for (int k = 0; k < maxProbes; ++k) {
+        float* p0 = map0 + 2 * (k * plane + at);
+        float* p1 = map1 + 2 * (k * plane + at);
+        if (k >= (1 << f.e)) {
+          p0[0] = p0[1] = p1[0] = p1[1] = t360::bitsFloat(0x7fc00000u);
+        } else if (rig) {
+          t360::anisoCameraPoint<true>(g, cam, model, m, f, k, p0, p1);
+        } else {
+          t360::anisoCameraPoint<false>(g, cam, model, m, f, k, p0, p1);
+        }
+      }
+      level[at] = static_cast<uint8_t>(f.level);
+      weight[at] = static_cast<uint16_t>(f.w);
+      probes[at] = static_cast<uint8_t>(1 << f.e);
+    });
+  });
+}
+T360_API int T360B200_transformFrameCameraAnisoAsync(VideoFrameTransform* t, const T360LensRig* rig, const T360Pose* pose, const T360Camera* camera,
+                                                     const T360Minify* minify, int maxProbes, int numPlanes, const uint8_t* const* dIn,
+                                                     uint8_t* const* dOut, const int* inW, const int* inH, const int* inPitch, const int* outW,
+                                                     const int* outH, const int* outPitch, void* stream) {
+  const char* what = "Could not transform the frame with an anisotropic camera view";
+  return frameCall(what, t, numPlanes, dIn, dOut, inW, inH, inPitch, outW, outH, outPitch, stream,
+                   [&](VideoFrameTransform& vft, const FramePlanes& f, cudaStream_t s) {
+                     std::string why;
+                     if (minifyRefused(minify, &why)) {  // (as the camera-mip call: the minify before the pose and camera)
+                       std::printf("%s. Error: %s\n", what, why.c_str());
+                       return false;
+                     }
+                     return vft.transformFrameView(what, anisoView(rig, pose, camera, minify, maxProbes), f, s);
                    });
 }
 T360_API int T360B200_cameraPhotoMaps(const FrameTransformContext* ctx, const T360LensRig* rig, const T360RigPhotometry* photometry, float seamWidth,

@@ -29,8 +29,10 @@
 //   - a camera view of a stereo rig (StereoCameraPositions): the same, with the output eye picking the lens;
 //   - a lens rig or a camera view of one with photometry and a rig motion over the readout (LensMotionPositions,
 //     CameraMotionPositions): the photometric records with each lens's M following the readout time of its point
-//     (lensMotionSample, cameraMotionSample).
-// In all twelve, the records come from the same host/device functions the planner (or its host twin) uses: bit-identical.
+//     (lensMotionSample, cameraMotionSample);
+//   - an anisotropic camera view (AnisoCameraPositions): the anti-aliased view's footprint once per pixel, then up to 16
+//     probes along its longer axis, each probe's records at the pixel's two levels (anisoFootprint, anisoCameraSample).
+// In all thirteen, the records come from the same host/device functions the planner (or its host twin) uses: bit-identical.
 #include "gather_common.cuh"
 
 #include <algorithm>
@@ -91,6 +93,10 @@ struct IsMip : std::false_type {};
 template <class Pos>
 struct IsMip<Pos, std::enable_if_t<Pos::kMip>> : std::true_type {};
 template <class Pos, class = void>
+struct IsAniso : std::false_type {};
+template <class Pos>
+struct IsAniso<Pos, std::enable_if_t<Pos::kAniso>> : std::true_type {};
+template <class Pos, class = void>
 struct IsPhoto : std::false_type {};
 template <class Pos>
 struct IsPhoto<Pos, std::enable_if_t<Pos::kPhoto>> : std::true_type {};
@@ -99,6 +105,10 @@ struct IsPhoto<Pos, std::enable_if_t<Pos::kPhoto>> : std::true_type {};
 // Positions::kMip (IsMip): record() returns the pixel's pyramid level and hands over its record there, the record at the
 // next level and that level's weight w (0..255); the next level is gathered only where w > 0, and blended as kBlend
 // blends.  (A branch of its own, so the other policies' loops are what they were.)
+// Positions::kAniso (IsAniso): footprint() gives the pixel's level, next-level weight w and probe count N = 2^e, and
+// probe() probe k's records at those levels, computed in registers as the loop reaches them.  Each probe is gathered and
+// blended as kMip gathers a pixel; the pixel is the rounded mean (sum + n / 2) / n of the n probes BORDER_TRANSPARENT
+// does not skip (all N under BORDER_WRAP), and keeps its byte where it skips them all.
 // Positions::kBlend: its record() hands over two records and the weight w (0..256) of the second; the first is gathered
 // for every pixel, the second only where 0 < w < 256, and the two values are blended (PerFrameSource::kLensBlend).  Where
 // BORDER_TRANSPARENT skips one of the two, the other stands alone.
@@ -167,6 +177,26 @@ __device__ __forceinline__ void gatherViewTiles(const PerFrameGatherParams& p, i
           value = value < 0 ? b : (b < 0 ? value : (value * (256 - w) + b * w + 128) >> 8);
         }
         if (TRANSPARENT && value < 0) continue;
+      } else if constexpr (IsAniso<Positions>::value) {
+        const AnisoFootprint f = pos.footprint(p, v, pl, i, j);
+        const SrcView lo = f.level ? mipView(p.mip[pl].level[f.level - 1]) : s;
+        int sum = 0, n = 0;
+#pragma unroll 1
+        for (int k = 0; k < (1 << f.e); ++k) {
+          int32_t rec0[2], rec1[2];
+          pos.probe(p, v, pl, f, k, rec0, rec1);
+          int a = viewPixel<K, TRANSPARENT>(lo, smem, rec0[0], rec0[1]);
+          if (f.w > 0) {
+            const int b = viewPixel<K, TRANSPARENT>(mipView(p.mip[pl].level[f.level]), smem, rec1[0], rec1[1]);
+            a = a < 0 ? b : (b < 0 ? a : (a * (256 - f.w) + b * f.w + 128) >> 8);
+          }
+          if (a >= 0) {
+            sum += a;
+            ++n;
+          }
+        }
+        if (TRANSPARENT && n == 0) continue;
+        value = (sum + n / 2) / n;
       } else if constexpr (Positions::kBlend) {
         int col1, rowPhase1, w;
         pos.record(p, v, lane, r, i, j, &col0, &rowPhase, &col1, &rowPhase1, &w);
@@ -340,6 +370,22 @@ struct MipCameraPositions : NoTables {
   __device__ int record(const PerFrameGatherParams& p, const PerFramePlane& v, int pl, int i, int j, int32_t* rec0, int32_t* rec1,
                         int* w) const {
     return mipCameraSample<LENS>(v.geometry, p.camera, p.rig, p.mip[pl].geometry, p.mipBias, i, j, rec0, rec1, w);
+  }
+};
+
+// An anisotropic camera view (kCameraAniso): MipCameraPositions' chain, footprint and levels, with the footprint's probe
+// count from cameraAniso (log2 maxProbes).  footprint() takes the centre ray's footprint (anisoFootprint), probe() one
+// probe's records (anisoCameraSample).  LENS as for CameraPositions.
+template <int, bool LENS>
+struct AnisoCameraPositions : NoTables {
+  static constexpr bool kAniso = true, kTransparent = LENS;
+  using NoTables::NoTables;
+  __device__ AnisoFootprint footprint(const PerFrameGatherParams& p, const PerFramePlane& v, int pl, int i, int j) const {
+    return anisoFootprint<LENS>(v.geometry, p.camera, p.rig, p.mip[pl].geometry, p.mipBias, p.cameraAniso, i, j);
+  }
+  __device__ void probe(const PerFrameGatherParams& p, const PerFramePlane& v, int pl, const AnisoFootprint& f, int k, int32_t* rec0,
+                        int32_t* rec1) const {
+    anisoCameraSample<LENS>(v.geometry, p.camera, p.rig, p.mip[pl].geometry, f, k, rec0, rec1);
   }
 };
 
@@ -530,6 +576,7 @@ cudaError_t launchPerFrameGather(PerFrameGatherParams p, PerFrameSource source, 
     case PerFrameSource::kLensBlend: return launchPositions<LensBlendPositions>(p, barrel, numTiles, numSMs, stream);
     case PerFrameSource::kRectilinear: return launchPositions<RectilinearPositions>(p, p.lens, numTiles, numSMs, stream);
     case PerFrameSource::kCameraMip: return launchPositions<MipCameraPositions>(p, p.lens, numTiles, numSMs, stream);
+    case PerFrameSource::kCameraAniso: return launchPositions<AnisoCameraPositions>(p, p.lens, numTiles, numSMs, stream);
     case PerFrameSource::kLensPhoto: return launchPositions<LensPhotoPositions>(p, barrel, numTiles, numSMs, stream);
     case PerFrameSource::kCameraPhoto:
     case PerFrameSource::kStereoCamera: {

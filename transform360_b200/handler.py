@@ -336,6 +336,12 @@ def load(path: os.PathLike | None = None):
     L.T360B200_transformFrameCameraMipAsync.restype = ci
     L.T360B200_transformFrameCameraMipAsync.argtypes = [vp, C.POINTER(T360LensRig), C.POINTER(T360Pose), C.POINTER(T360Camera),
                                                         C.POINTER(T360Minify), ci] + planes
+    L.T360B200_cameraAnisoMaps.restype = ci
+    L.T360B200_cameraAnisoMaps.argtypes = [C.POINTER(FrameTransformContext), C.POINTER(T360LensRig), C.POINTER(T360Pose),
+                                           C.POINTER(T360Camera), C.POINTER(T360Minify)] + [ci] * 5 + [vp] * 5
+    L.T360B200_transformFrameCameraAnisoAsync.restype = ci
+    L.T360B200_transformFrameCameraAnisoAsync.argtypes = [vp, C.POINTER(T360LensRig), C.POINTER(T360Pose), C.POINTER(T360Camera),
+                                                          C.POINTER(T360Minify), ci, ci] + planes
     L.T360B200_cameraPhotoMaps.restype = ci
     L.T360B200_cameraPhotoMaps.argtypes = [C.POINTER(FrameTransformContext), C.POINTER(T360LensRig), C.POINTER(T360RigPhotometry), C.c_float,
                                            C.POINTER(T360Pose), C.POINTER(T360Camera), C.POINTER(T360Minify)] + [ci] * 6 + [vp] * 6
@@ -390,7 +396,8 @@ EXPORTED_SYMBOLS = [
     "T360B200_lensMap", "T360B200_transformFrameLensAsync", "T360B200_lensBlendMaps", "T360B200_transformFrameLensBlendAsync",
     "T360B200_lensPhotoMaps", "T360B200_transformFrameLensPhotoAsync",
     "T360B200_rectilinearMap", "T360B200_transformFrameRectilinearAsync", "T360B200_cameraMap", "T360B200_transformFrameCameraAsync",
-    "T360B200_cameraMipMaps", "T360B200_transformFrameCameraMipAsync", "T360B200_cameraPhotoMaps", "T360B200_transformFrameCameraPhotoAsync",
+    "T360B200_cameraMipMaps", "T360B200_transformFrameCameraMipAsync", "T360B200_cameraAnisoMaps", "T360B200_transformFrameCameraAnisoAsync",
+    "T360B200_cameraPhotoMaps", "T360B200_transformFrameCameraPhotoAsync",
     "T360B200_stereoCameraMaps", "T360B200_transformFrameStereoCameraAsync",
     "T360B200_lensMotionMaps", "T360B200_transformFrameLensMotionAsync", "T360B200_cameraMotionMaps", "T360B200_transformFrameCameraMotionAsync",
     "T360B200_setPinHostPlanes", "T360B200_debugTrace", "T360B200_debugTraceRead", "T360B200_synchronize", "T360B200_stream", "T360B200_kernelLaunchCount", "T360B200_planDeviceBytes",
@@ -545,6 +552,15 @@ class VideoFrameTransform:
         return lambda pose, camera, minify, stream=0, rig=None: enqueue(
             (C.byref(rig) if rig is not None else None, C.byref(as_pose(pose)), C.byref(as_camera(camera)),
              C.byref(as_minify(minify)), n), stream)
+
+    def make_camera_aniso_frame_call(self, in_planes, out_planes, dims):
+        """Like make_camera_mip_frame_call, for T360B200_transformFrameCameraAnisoAsync (an anisotropic camera view: up to
+        max_probes pyramid probes per pixel along its footprint's longer axis): returns a callable f(pose, camera, minify,
+        max_probes, stream, rig=None) -> bool, max_probes 1, 2, 4, 8 or 16."""
+        n, enqueue = self._frame_call("T360B200_transformFrameCameraAnisoAsync", in_planes, out_planes, dims)
+        return lambda pose, camera, minify, max_probes, stream=0, rig=None: enqueue(
+            (C.byref(rig) if rig is not None else None, C.byref(as_pose(pose)), C.byref(as_camera(camera)),
+             C.byref(as_minify(minify)), max_probes, n), stream)
 
     def make_camera_photo_frame_call(self, in_planes, out_planes, dims):
         """Like make_camera_mip_frame_call, for T360B200_transformFrameCameraPhotoAsync (a camera view of a rig with
@@ -915,6 +931,25 @@ def camera_mip_maps(ctx: FrameTransformContext, pose, camera, minify, in_w, in_h
                                          map0.ctypes.data, map1.ctypes.data, level.ctypes.data, weight.ctypes.data):
         raise ValueError("T360B200_cameraMipMaps refused the arguments (message on stdout)")
     return map0, map1, level, weight
+
+
+def camera_aniso_maps(ctx: FrameTransformContext, pose, camera, minify, max_probes, in_w, in_h, out_w, out_h,
+                      rig: T360LensRig | None = None) -> tuple[np.ndarray, np.ndarray, np.ndarray, np.ndarray, np.ndarray]:
+    """The host twin of one plane of an anisotropic camera view (T360B200_cameraAnisoMaps, no CUDA): (map0, map1, level,
+    weight, probes).  map0 / map1: float32 [max_probes][out_h][out_w][2], probe k's entry in the pixel's level's pixels /
+    in the next level's (map1 NaN where the weight is 0, both NaN for k >= probes); level: uint8 [out_h][out_w]; weight:
+    uint16, the next level's weight w (0..255), shared by the probes; probes: uint8, the pixel's probe count N.  Each
+    probe is camera_mip_maps' composite of its entries; the pixel is their mean (sum + N / 2) // N, with a rig over the
+    probes not skipped.  max_probes 1 gives camera_mip_maps' arrays as probe 0."""
+    shape = (max(out_h, 0), max(out_w, 0))
+    k = max_probes if max_probes in (1, 2, 4, 8, 16) else 1  # (the call refuses other values before it writes)
+    map0, map1 = np.zeros((k,) + shape + (2,), np.float32), np.zeros((k,) + shape + (2,), np.float32)
+    level, weight, probes = np.zeros(shape, np.uint8), np.zeros(shape, np.uint16), np.zeros(shape, np.uint8)
+    if not load().T360B200_cameraAnisoMaps(C.byref(ctx), C.byref(rig) if rig is not None else None, C.byref(as_pose(pose)),
+                                           C.byref(as_camera(camera)), C.byref(as_minify(minify)), max_probes, in_w, in_h, out_w, out_h,
+                                           map0.ctypes.data, map1.ctypes.data, level.ctypes.data, weight.ctypes.data, probes.ctypes.data):
+        raise ValueError("T360B200_cameraAnisoMaps refused the arguments (message on stdout)")
+    return map0, map1, level, weight, probes
 
 
 def camera_photo_maps(ctx: FrameTransformContext, rig: T360LensRig, photometry: T360RigPhotometry, seam_width, pose, camera, minify, lens,
