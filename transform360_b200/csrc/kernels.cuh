@@ -399,16 +399,14 @@ void countKernelLaunches(long long n);  // kernels launched through a replayed C
 //   kLensPhoto    a lens rig with photometry (rotation, rig, seamScale, photo; lensPhotoSample): the hard seam
 //                 (seamScale = 0) or the feathered one; each lens's sample is corrected with its gain (photoCorrect)
 //                 before the seam combines them, and with photo.stats set the overlap's sums are accumulated.
-//   kCameraPhoto  a camera view of a lens rig with photometry (camera, rig, seamScale, cameraPhoto: the planes' pyramids
-//                 and the photometric constants, mipBias; cameraPhotoSample): each lens's sample is the blend of its own two levels (kCameraMip's
-//                 blend; level 0 alone without a pyramid), then corrected, combined and counted as kLensPhoto's.
+//   kCameraPhoto  a camera view of a lens rig with photometry (camera, rig, seamScale, mip, mipBias, photo;
+//                 cameraPhotoSample): each lens's sample is the blend of its own two levels (kCameraMip's blend; level 0
+//                 alone without a pyramid), then corrected, combined and counted as kLensPhoto's.
 //   kStereoCamera a camera view of a stereo rig (kCameraPhoto's constants, no seam; cameraPhotoSample<MIP, true>): the
 //                 output eye split of the context's output_stereo_format, and eye e's pixels take lens e alone.
-//   kLensMotion   kLensPhoto with a rig motion over the readout (rotation, rig, seamScale, lensMotion: the photometric
-//                 constants and the motion's sample table; lensMotionSample): each lens's M follows the readout time of
-//                 the point it projects.
-//   kCameraMotion kCameraPhoto with a rig motion (cameraMotion: kCameraPhoto's constants and the motion;
-//                 cameraMotionSample).
+//   kLensMotion   kLensPhoto with a rig motion over the readout (rotation, rig, seamScale, photo, motion;
+//                 lensMotionSample): each lens's M follows the readout time of the point it projects.
+//   kCameraMotion kCameraPhoto with a rig motion (kCameraPhoto's constants and motion; cameraMotionSample).
 //   kCameraAniso  anisotropic camera views (kCameraMip's constants and cameraAniso; anisoFootprint, anisoCameraSample):
 //                 the pixel's footprint once, then up to 2^cameraAniso probes along its longer axis, each gathered as
 //                 kCameraMip gathers a pixel, averaged over the probes BORDER_TRANSPARENT does not skip.
@@ -436,11 +434,11 @@ struct PerFrameGatherParams {
   float seamScale;   // s = 1 / (2 seamWidth), seamWidth in radians
   bool transparent;  // kMap: BORDER_TRANSPARENT instead of BORDER_WRAP
   bool lens;         // kRectilinear: the rig's lenses instead of the context's input
-  uint8_t cameraAniso;  // kCameraAniso: log2 maxProbes (in the padding before weights, so no member moves)
+  uint8_t cameraAniso;  // kCameraAniso: log2 maxProbes
   const int16_t* weights;  // device copy of the [1024][k][k] table (nullptr for nearest)
   int kernelSize;
-  // kCameraMip: per plane its footprint constants and pyramid levels 1..geometry.top (level 0 is the plane's src), and
-  // round(256 lodBias)
+  // the pyramid sources (kCameraMip, kCameraAniso, kCameraPhoto, kStereoCamera, kCameraMotion): per plane its footprint
+  // constants and pyramid levels 1..geometry.top (level 0 is the plane's src), and round(256 lodBias)
   struct MipLevel {
     uint8_t* bytes;  // written by the level's pyramid launch, read by the gather
     int w, h, pitch;
@@ -449,57 +447,22 @@ struct PerFrameGatherParams {
     MipGeometry geometry;
     MipLevel level[kMipMaxLevels];  // [l - 1]: level l
   };
-  // kLensPhoto: per plane its photometric constants, and the statistics buffer ([numPlanes][6] sums: n, sum a', sum b',
-  // sum a'^2, sum b'^2, sum a'b', zeroed by the caller in stream order; nullptr: none)
+  MipPlane mip[kMaxFramePlanes];
+  int mipBias;
+  // the photometric sources (kLensPhoto, kCameraPhoto, kStereoCamera, kLensMotion, kCameraMotion): per plane its
+  // photometric constants, and the statistics buffer ([numPlanes][6] sums: n, sum a', sum b', sum a'^2, sum b'^2, sum a'b',
+  // zeroed by the caller in stream order; nullptr: none)
   struct LensPhoto {
     LensPhotoPlane plane[kMaxFramePlanes];
     unsigned long long* stats;
   };
-  // kCameraPhoto: both of the above, per plane its footprint constants and pyramid levels (a level's sides in 16 bits, so
-  // the two fit in mip's storage), and the photometric constants
-  struct CameraPhotoLevel {
-    uint8_t* bytes;
-    int pitch;
-    uint16_t w, h;
-  };
-  struct CameraPhotoPlane {
-    MipGeometry geometry;
-    CameraPhotoLevel level[kMipMaxLevels];  // [l - 1]: level l
-  };
-  struct CameraPhoto {
-    CameraPhotoPlane mip[kMaxFramePlanes];
-    LensPhoto photo;
-  };
-  // kLensMotion / kCameraMotion: kLensPhoto's / kCameraPhoto's constants and the rig motion (its sample table staged in
-  // device memory, numSamples and the lenses' readouts)
-  struct LensMotion {
-    LensPhoto photo;
-    RigMotion motion;
-  };
-  struct CameraMotion {
-    CameraPhoto cameraPhoto;
-    RigMotion motion;
-  };
-  // (the sources' constants share their storage, so the block keeps the size and layout every other source's kernel was
-  // compiled against: a larger block would move the kernels' next parameter)
-  union {
-    MipPlane mip[kMaxFramePlanes];
-    LensPhoto photo;
-    CameraPhoto cameraPhoto;
-    LensMotion lensMotion;
-    CameraMotion cameraMotion;
-  };
-  int mipBias;
+  LensPhoto photo;
+  // the motion sources (kLensMotion, kCameraMotion): the rig motion (its sample table staged in device memory, numSamples
+  // and the lenses' readouts)
+  RigMotion motion;
 };
-static_assert(sizeof(PerFrameGatherParams::LensPhoto) <= sizeof(PerFrameGatherParams::MipPlane) * kMaxFramePlanes);
-static_assert(sizeof(PerFrameGatherParams::CameraPhoto) <= sizeof(PerFrameGatherParams::MipPlane) * kMaxFramePlanes);
-static_assert(sizeof(PerFrameGatherParams::LensMotion) <= sizeof(PerFrameGatherParams::MipPlane) * kMaxFramePlanes);
-static_assert(sizeof(PerFrameGatherParams::CameraMotion) <= sizeof(PerFrameGatherParams::MipPlane) * kMaxFramePlanes);
-// (the block the kernels were compiled against before the motion sources: its size and where its last member lies)
-static_assert(sizeof(PerFrameGatherParams) == 1496 && offsetof(PerFrameGatherParams, mipBias) == 1488);
-// (cameraAniso takes two bytes of padding: weights and every member after it stay where the kernels read them)
-static_assert(offsetof(PerFrameGatherParams, cameraAniso) < offsetof(PerFrameGatherParams, weights) &&
-              offsetof(PerFrameGatherParams, weights) == 632);
+// (the block and the launch's numTiles within the 4 KB of kernel parameters every driver accepts)
+static_assert(sizeof(PerFrameGatherParams) + sizeof(int) <= 4096);
 constexpr int kPhotoStats = 6;  // sums per plane of kLensPhoto's statistics
 // a CTA takes tiles of 32 output columns x viewTileRows(k) rows; a thread owns one column of a tile and walks down
 // kViewRowsPerThread of its rows

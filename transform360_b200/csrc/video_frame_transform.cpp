@@ -1616,10 +1616,9 @@ class VideoFrameTransform {
       UploadRing::Entry* motionStaged = nullptr;
       if (photo) {
         source = moving ? t360::PerFrameSource::kLensMotion : t360::PerFrameSource::kLensPhoto;
-        t360::PerFrameGatherParams::LensPhoto& ph = moving ? gp.lensMotion.photo : gp.photo;
-        for (int p = 0; p < f.numPlanes; ++p) ph.plane[p] = lensPhotoPlane(*photo, rig->numLenses, p);
-        ph.stats = stats;
-        if (moving) gp.lensMotion.motion = stageMotion(*rig, *motion, gp.rig, slotFor(s), s, &motionStaged);
+        for (int p = 0; p < f.numPlanes; ++p) gp.photo.plane[p] = lensPhotoPlane(*photo, rig->numLenses, p);
+        gp.photo.stats = stats;
+        if (moving) gp.motion = stageMotion(*rig, *motion, gp.rig, slotFor(s), s, &motionStaged);
         if (stats) CU(cudaMemsetAsync(stats, 0, sizeof(unsigned long long) * t360::kPhotoStats * f.numPlanes, s));
       }
       perFrameGather(source, gp, ctx, f, f.in, f.inPitch, nullptr, /*transparent=*/true, tables, staged, nullptr, s);
@@ -1648,20 +1647,19 @@ class VideoFrameTransform {
     auto refused = [&](const FrameTransformContext& ctx, std::string* why) {
       if (viewRefused(ctx, v, why)) return true;
       for (int p = 0; v.photometric && v.minify && v.minify->maxLevel > 0 && p < f.numPlanes; ++p)
-        if (f.inW[p] > 2 * 65535 || f.inH[p] > 2 * 65535) {  // (CameraPhotoLevel keeps a level's sides in 16 bits)
+        if (f.inW[p] > 2 * 65535 || f.inH[p] > 2 * 65535) {  // (documented by the photometric and stereo calls)
           *why = formatted("input plane %d is %dx%d: a pyramid needs sides of at most 131070", p, f.inW[p], f.inH[p]);
           return true;
         }
       return false;
     };
     return unplannedFrame(what, stream, refused, [&](const FrameTransformContext& ctx, int, cudaStream_t s) {
-      // (pyramids: the planes' footprint constants and buildPyramids' levels, copied into the source's member of gp's union)
-      t360::PerFrameGatherParams gp{}, pyramids{};
+      t360::PerFrameGatherParams gp{};
       int topMax = 0;
       for (int p = 0; p < f.numPlanes; ++p) {
         gp.plane[p].geometry = viewGeometry(ctx, v, f.inW[p], f.inH[p], f.outW[p], f.outH[p]);
-        pyramids.mip[p].geometry = t360::mipGeometry(gp.plane[p].geometry, v.minify ? v.minify->maxLevel : 0);
-        topMax = std::max(topMax, pyramids.mip[p].geometry.top);
+        gp.mip[p].geometry = t360::mipGeometry(gp.plane[p].geometry, v.minify ? v.minify->maxLevel : 0);
+        topMax = std::max(topMax, gp.mip[p].geometry.top);
       }
       gp.lens = v.rig != nullptr;
       gp.camera = cameraConstants(v);
@@ -1672,32 +1670,18 @@ class VideoFrameTransform {
       if (v.aniso && v.maxProbes > 1) {
         source = t360::PerFrameSource::kCameraAniso;
         gp.cameraAniso = static_cast<uint8_t>(probesLog2(v.maxProbes));
-        for (int p = 0; p < f.numPlanes; ++p) gp.mip[p].geometry = pyramids.mip[p].geometry;  // (the levels follow below)
       }
-      t360::PerFrameGatherParams::CameraPhoto& cp = v.moving ? gp.cameraMotion.cameraPhoto : gp.cameraPhoto;
       UploadRing::Entry* motionStaged = nullptr;
-      if (v.moving) gp.cameraMotion.motion = stageMotion(*v.rig, *v.motion, gp.rig, slotFor(s), s, &motionStaged);
+      if (v.moving) gp.motion = stageMotion(*v.rig, *v.motion, gp.rig, slotFor(s), s, &motionStaged);
       if (v.photometric) {
         source = v.stereo ? t360::PerFrameSource::kStereoCamera
                           : (v.moving ? t360::PerFrameSource::kCameraMotion : t360::PerFrameSource::kCameraPhoto);
-        for (int p = 0; p < f.numPlanes; ++p) {
-          cp.mip[p].geometry = pyramids.mip[p].geometry;
-          cp.photo.plane[p] = lensPhotoPlane(*v.photometry, v.rig->numLenses, p);
-        }
-        cp.photo.stats = v.stats;
+        for (int p = 0; p < f.numPlanes; ++p) gp.photo.plane[p] = lensPhotoPlane(*v.photometry, v.rig->numLenses, p);
+        gp.photo.stats = v.stats;
         if (v.stats) CU(cudaMemsetAsync(v.stats, 0, sizeof(unsigned long long) * t360::kPhotoStats * f.numPlanes, s));
       }
       UploadRing::Entry* staged = nullptr;
-      if (topMax > 0) {
-        buildPyramids(f, pyramids, slotFor(s), s, &staged);
-        for (int p = 0; p < f.numPlanes; ++p) {
-          if (!v.photometric) gp.mip[p] = pyramids.mip[p];
-          for (int l = 1; v.photometric && l <= cp.mip[p].geometry.top; ++l) {
-            const t360::PerFrameGatherParams::MipLevel& L = pyramids.mip[p].level[l - 1];
-            cp.mip[p].level[l - 1] = {L.bytes, L.pitch, static_cast<uint16_t>(L.w), static_cast<uint16_t>(L.h)};
-          }
-        }
-      }
+      if (topMax > 0) buildPyramids(f, gp, slotFor(s), s, &staged);
       perFrameGather(source, gp, ctx, f, f.in, f.inPitch, nullptr, gp.lens, nullptr, nullptr, nullptr, s);
       releaseAfter(staged, s);
       releaseAfter(motionStaged, s);

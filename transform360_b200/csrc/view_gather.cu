@@ -57,7 +57,7 @@ __device__ __forceinline__ int viewPixel(const SrcView& s, const unsigned char* 
   }
 }
 
-// Level l >= 1 of a plane's pyramid (kCameraMip) as a source
+// Level l >= 1 of a plane's pyramid as a source
 __device__ __forceinline__ SrcView mipView(const PerFrameGatherParams::MipLevel& l) {
   SrcView s;
   s.bytes = l.bytes;
@@ -66,56 +66,37 @@ __device__ __forceinline__ SrcView mipView(const PerFrameGatherParams::MipLevel&
   s.w = l.w; s.h = l.h; s.pitch = l.pitch;
   return s;
 }
-__device__ __forceinline__ SrcView mipView(const PerFrameGatherParams::CameraPhotoLevel& l) {  // (kCameraPhoto)
-  SrcView s;
-  s.bytes = l.bytes;
-  s.misalign = (int)(reinterpret_cast<uintptr_t>(l.bytes) & 3);
-  s.words = reinterpret_cast<const uint32_t*>(l.bytes - s.misalign);
-  s.w = l.w; s.h = l.h; s.pitch = l.pitch;
-  return s;
+// a and b blended by b's weight w (0..256), rounded; where BORDER_TRANSPARENT skipped one of the two (-1) the other stands
+// alone, -1 where it skipped both
+__device__ __forceinline__ int blendPixels(int a, int b, int w) {
+  return a < 0 ? b : (b < 0 ? a : (a * (256 - w) + b * w + 128) >> 8);
 }
-// A pixel at pyramid level `level` of a plane (0: the plane's src s; levels[l - 1]: level l) and, where w > 0, at level +
-// 1, blended by w (0..255); where BORDER_TRANSPARENT skips one of the two the other stands alone, -1 where it skips both.
-// (kCameraPhoto's per-lens blend.  kCameraMip's branch writes the same blend inline: through this helper its kernels
-// compile to other register assignments, and they are kept as they were.)
-template <int K, bool TRANSPARENT, class Level>
-__device__ __forceinline__ int levelPixel(const Level* levels, const SrcView& s, const unsigned char* smem, int level, const int32_t* rec0,
-                                          const int32_t* rec1, int w) {
-  int value = viewPixel<K, TRANSPARENT>(level ? mipView(levels[level - 1]) : s, smem, rec0[0], rec0[1]);
-  if (w > 0) {
-    const int b = viewPixel<K, TRANSPARENT>(mipView(levels[level]), smem, rec1[0], rec1[1]);
-    value = value < 0 ? b : (b < 0 ? value : (value * (256 - w) + b * w + 128) >> 8);
-  }
+// Pyramid level `level` of a plane as a source (0: the plane's src s; levels[l - 1]: level l)
+__device__ __forceinline__ SrcView levelView(const PerFrameGatherParams::MipLevel* levels, const SrcView& s, int level) {
+  return level ? mipView(levels[level - 1]) : s;
+}
+// A pixel at a level (its view lo) and, where w > 0, at the next one (levels[level]), blended by w (0..255)
+template <int K, bool TRANSPARENT>
+__device__ __forceinline__ int levelPixel(const SrcView& lo, const PerFrameGatherParams::MipLevel* levels, const unsigned char* smem,
+                                          int level, const int32_t* rec0, const int32_t* rec1, int w) {
+  int value = viewPixel<K, TRANSPARENT>(lo, smem, rec0[0], rec0[1]);
+  if (w > 0) value = blendPixels(value, viewPixel<K, TRANSPARENT>(mipView(levels[level]), smem, rec1[0], rec1[1]), w);
   return value;
 }
-template <class Pos, class = void>
-struct IsMip : std::false_type {};
-template <class Pos>
-struct IsMip<Pos, std::enable_if_t<Pos::kMip>> : std::true_type {};
-template <class Pos, class = void>
-struct IsAniso : std::false_type {};
-template <class Pos>
-struct IsAniso<Pos, std::enable_if_t<Pos::kAniso>> : std::true_type {};
-template <class Pos, class = void>
-struct IsPhoto : std::false_type {};
-template <class Pos>
-struct IsPhoto<Pos, std::enable_if_t<Pos::kPhoto>> : std::true_type {};
 
 // TRANSPARENT (barrel layouts): BORDER_TRANSPARENT, a pixel whose anchor tap lies outside the source keeps its byte.
-// Positions::kMip (IsMip): record() returns the pixel's pyramid level and hands over its record there, the record at the
-// next level and that level's weight w (0..255); the next level is gathered only where w > 0, and blended as kBlend
-// blends.  (A branch of its own, so the other policies' loops are what they were.)
-// Positions::kAniso (IsAniso): footprint() gives the pixel's level, next-level weight w and probe count N = 2^e, and
-// probe() probe k's records at those levels, computed in registers as the loop reaches them.  Each probe is gathered and
-// blended as kMip gathers a pixel; the pixel is the rounded mean (sum + n / 2) / n of the n probes BORDER_TRANSPARENT
-// does not skip (all N under BORDER_WRAP), and keeps its byte where it skips them all.
+// Positions::kMip: record() returns the pixel's pyramid level and hands over its record there, the record at the next
+// level and that level's weight w (0..255); the next level is gathered only where w > 0 (levelPixel).
+// Positions::kAniso: footprint() gives the pixel's level, next-level weight w and probe count N = 2^e, and probe() probe
+// k's records at those levels, computed in registers as the loop reaches them.  Each probe is gathered as kMip gathers a
+// pixel; the pixel is the rounded mean (sum + n / 2) / n of the n probes BORDER_TRANSPARENT does not skip (all N under
+// BORDER_WRAP), and keeps its byte where it skips them all.
 // Positions::kBlend: its record() hands over two records and the weight w (0..256) of the second; the first is gathered
-// for every pixel, the second only where 0 < w < 256, and the two values are blended (PerFrameSource::kLensBlend).  Where
-// BORDER_TRANSPARENT skips one of the two, the other stands alone.
-// Positions::kPhoto (IsPhoto, kLensPhoto and kCameraPhoto): record() hands over both lenses' records, their gains and w,
-// and the policy's pixel() gathers a lens's sample from them (photo() names the launch's photometric constants).  Lens 0
-// is gathered where w < 256, lens 1 where w > 0, and, with statistics, both wherever both cover the pixel; each sample is
-// corrected (photoCorrect) before w combines them.  A thread sums its overlap pixels' six values over its rows of the tile,
+// for every pixel, the second only where 0 < w < 256, and the two values are blended (PerFrameSource::kLensBlend).
+// Positions::kPhoto (the photometric sources): record() hands over both lenses' records, their gains and w, and the
+// policy's pixel() gathers a lens's sample from them.  Lens 0 is gathered where w < 256, lens 1 where w > 0, and, with
+// statistics, both wherever both cover the pixel; each sample is corrected (photoCorrect) before w combines them (as
+// kBlend combines its two values).  A thread sums its overlap pixels' six values over its rows of the tile,
 // its warp reduces them (__reduce_add_sync over the warp's live columns), and one lane adds them to the plane's sums with
 // one 64-bit atomic each.  Whether statistics are taken and which seam is used are launch-uniform branches.
 template <int K, bool TRANSPARENT, class Positions>
@@ -145,13 +126,13 @@ __device__ __forceinline__ void gatherViewTiles(const PerFrameGatherParams& p, i
       if (i >= v.geometry.mapH) break;
       int col0, rowPhase;
       int value;
-      if constexpr (IsPhoto<Positions>::value) {
+      if constexpr (Positions::kPhoto) {
         int32_t rec0[2], rec1[2];
         int g0, g1;
         bool overlap;
         const int w = pos.record(p, v, pl, i, j, rec0, rec1, &g0, &g1, &overlap);
-        const LensPhotoPlane& c = Positions::photo(p).plane[pl];
-        const bool stats = Positions::photo(p).stats && overlap;
+        const LensPhotoPlane& c = p.photo.plane[pl];
+        const bool stats = p.photo.stats && overlap;
         int a = -1, b = -1;
         if (w < 256 || stats) {
           a = pos.template pixel<K, TRANSPARENT>(p, pl, s, smem, 0, rec0);
@@ -165,31 +146,23 @@ __device__ __forceinline__ void gatherViewTiles(const PerFrameGatherParams& p, i
           sums[0] += 1; sums[1] += a; sums[2] += b;
           sums[3] += a * a; sums[4] += b * b; sums[5] += a * b;
         }
-        value = w == 0 ? a : (w == 256 ? b : (a < 0 ? b : (b < 0 ? a : (a * (256 - w) + b * w + 128) >> 8)));
+        value = w == 0 ? a : (w == 256 ? b : blendPixels(a, b, w));
         if (value < 0) continue;
-      } else if constexpr (IsMip<Positions>::value) {
+      } else if constexpr (Positions::kMip) {
         int32_t rec0[2], rec1[2];
         int w;
         const int level = pos.record(p, v, pl, i, j, rec0, rec1, &w);
-        value = viewPixel<K, TRANSPARENT>(level ? mipView(p.mip[pl].level[level - 1]) : s, smem, rec0[0], rec0[1]);
-        if (w > 0) {
-          const int b = viewPixel<K, TRANSPARENT>(mipView(p.mip[pl].level[level]), smem, rec1[0], rec1[1]);
-          value = value < 0 ? b : (b < 0 ? value : (value * (256 - w) + b * w + 128) >> 8);
-        }
+        value = levelPixel<K, TRANSPARENT>(levelView(p.mip[pl].level, s, level), p.mip[pl].level, smem, level, rec0, rec1, w);
         if (TRANSPARENT && value < 0) continue;
-      } else if constexpr (IsAniso<Positions>::value) {
+      } else if constexpr (Positions::kAniso) {
         const AnisoFootprint f = pos.footprint(p, v, pl, i, j);
-        const SrcView lo = f.level ? mipView(p.mip[pl].level[f.level - 1]) : s;
+        const SrcView lo = levelView(p.mip[pl].level, s, f.level);
         int sum = 0, n = 0;
 #pragma unroll 1
         for (int k = 0; k < (1 << f.e); ++k) {
           int32_t rec0[2], rec1[2];
           pos.probe(p, v, pl, f, k, rec0, rec1);
-          int a = viewPixel<K, TRANSPARENT>(lo, smem, rec0[0], rec0[1]);
-          if (f.w > 0) {
-            const int b = viewPixel<K, TRANSPARENT>(mipView(p.mip[pl].level[f.level]), smem, rec1[0], rec1[1]);
-            a = a < 0 ? b : (b < 0 ? a : (a * (256 - f.w) + b * f.w + 128) >> 8);
-          }
+          const int a = levelPixel<K, TRANSPARENT>(lo, p.mip[pl].level, smem, f.level, rec0, rec1, f.w);
           if (a >= 0) {
             sum += a;
             ++n;
@@ -201,10 +174,7 @@ __device__ __forceinline__ void gatherViewTiles(const PerFrameGatherParams& p, i
         int col1, rowPhase1, w;
         pos.record(p, v, lane, r, i, j, &col0, &rowPhase, &col1, &rowPhase1, &w);
         value = viewPixel<K, TRANSPARENT>(s, smem, col0, rowPhase);
-        if (w > 0 && w < 256) {
-          const int b = viewPixel<K, TRANSPARENT>(s, smem, col1, rowPhase1);
-          value = value < 0 ? b : (b < 0 ? value : (value * (256 - w) + b * w + 128) >> 8);
-        }
+        if (w > 0 && w < 256) value = blendPixels(value, viewPixel<K, TRANSPARENT>(s, smem, col1, rowPhase1), w);
         if (value < 0) continue;
       } else {
         pos.record(p, v, lane, r, i, j, &col0, &rowPhase);
@@ -219,12 +189,12 @@ __device__ __forceinline__ void gatherViewTiles(const PerFrameGatherParams& p, i
       }
       v.dst[(size_t)i * v.dstPitch + j] = (uint8_t)value;
     }
-    if constexpr (IsPhoto<Positions>::value) {
-      if (Positions::photo(p).stats) {  // (every lane of the warp's live columns gets here: a row bound breaks the whole warp)
+    if constexpr (Positions::kPhoto) {
+      if (p.photo.stats) {  // (every lane of the warp's live columns gets here: a row bound breaks the whole warp)
         const int live = v.geometry.mapW - x0;
         const unsigned mask = live >= 32 ? 0xffffffffu : (1u << live) - 1u;
         if (__reduce_add_sync(mask, sums[0])) {
-          unsigned long long* out = Positions::photo(p).stats + pl * kPhotoStats;
+          unsigned long long* out = p.photo.stats + pl * kPhotoStats;
 #pragma unroll
           for (int k = 0; k < kPhotoStats; ++k) {
             const unsigned total = __reduce_add_sync(mask, sums[k]);
@@ -242,7 +212,7 @@ __device__ __forceinline__ void gatherViewTiles(const PerFrameGatherParams& p, i
 // Positions without per-tile tables
 struct NoTables {
   static constexpr int kTableBytes = 0;
-  static constexpr bool kBlend = false;
+  static constexpr bool kBlend = false, kMip = false, kAniso = false, kPhoto = false;
   __device__ explicit NoTables(unsigned char*) {}
   __device__ void beginTile(const PerFrameGatherParams&, const PerFramePlane&, int, int) {}
   __device__ void beginColumn(int) {}
@@ -253,7 +223,7 @@ template <int K, bool>
 struct FlatPositions {
   static constexpr int kRows = viewTileRows(K);
   static constexpr int kTableBytes = 4 * 32 * (int)sizeof(FlatColumn) + 2 * kRows * (int)sizeof(FlatRow) + 32;
-  static constexpr bool kBlend = false, kTransparent = false;
+  static constexpr bool kBlend = false, kMip = false, kAniso = false, kPhoto = false, kTransparent = false;
   FlatColumn* colTab;  // [eye][fold][32]
   FlatRow* rowTab;     // [column eye][kRows]
   bool* colEye;        // [32]
@@ -400,7 +370,6 @@ struct LensPhotoPositions : NoTables {
     return lensPhotoSample<BARREL>(v.geometry, p.rotation, p.rig, p.seamScale, p.photo.stats != nullptr, p.photo.plane[pl], v.colTable,
                                    v.rowTable, i, j, rec0, rec1, g0, g1, overlap);
   }
-  __device__ static const PerFrameGatherParams::LensPhoto& photo(const PerFrameGatherParams& p) { return p.photo; }
   template <int K, bool TRANSPARENT>
   __device__ int pixel(const PerFrameGatherParams&, int, const SrcView& s, const unsigned char* smem, int, const int32_t* rec) const {
     return viewPixel<K, TRANSPARENT>(s, smem, rec[0], rec[1]);
@@ -419,19 +388,20 @@ struct CameraPhotoPositions : NoTables {
   using NoTables::NoTables;
   __device__ int record(const PerFrameGatherParams& p, const PerFramePlane& v, int pl, int i, int j, int32_t*, int32_t*, int* g0, int* g1,
                         bool* overlap) {
-    const PerFrameGatherParams::LensPhoto& photo = p.cameraPhoto.photo;
-    const int w = cameraPhotoSample<MIP>(v.geometry, p.camera, p.rig, p.cameraPhoto.mip[pl].geometry, p.mipBias, p.seamScale,
-                                         photo.stats != nullptr, photo.plane[pl], i, j, lens, overlap);
+    const int w = cameraPhotoSample<MIP>(v.geometry, p.camera, p.rig, p.mip[pl].geometry, p.mipBias, p.seamScale, p.photo.stats != nullptr,
+                                         p.photo.plane[pl], i, j, lens, overlap);
     *g0 = lens[0].gain;
     *g1 = lens[1].gain;
     return w;
   }
-  __device__ static const PerFrameGatherParams::LensPhoto& photo(const PerFrameGatherParams& p) { return p.cameraPhoto.photo; }
   template <int K, bool TRANSPARENT>
   __device__ int pixel(const PerFrameGatherParams& p, int pl, const SrcView& s, const unsigned char* smem, int l, const int32_t*) const {
     const CameraPhotoRecords& r = lens[l];
-    if constexpr (MIP) return levelPixel<K, TRANSPARENT>(p.cameraPhoto.mip[pl].level, s, smem, r.level, r.rec0, r.rec1, r.w);
-    else return viewPixel<K, TRANSPARENT>(s, smem, r.rec0[0], r.rec0[1]);
+    if constexpr (MIP) {
+      return levelPixel<K, TRANSPARENT>(levelView(p.mip[pl].level, s, r.level), p.mip[pl].level, smem, r.level, r.rec0, r.rec1, r.w);
+    } else {
+      return viewPixel<K, TRANSPARENT>(s, smem, r.rec0[0], r.rec0[1]);
+    }
   }
 };
 
@@ -443,10 +413,9 @@ struct StereoCameraPositions : CameraPhotoPositions<K, MIP> {
   using CameraPhotoPositions<K, MIP>::CameraPhotoPositions;
   __device__ int record(const PerFrameGatherParams& p, const PerFramePlane& v, int pl, int i, int j, int32_t*, int32_t*, int* g0, int* g1,
                         bool* overlap) {
-    const PerFrameGatherParams::LensPhoto& photo = p.cameraPhoto.photo;
     CameraPhotoRecords* lens = this->lens;
-    const int w = cameraPhotoSample<MIP, true>(v.geometry, p.camera, p.rig, p.cameraPhoto.mip[pl].geometry, p.mipBias, 0.0f,
-                                               photo.stats != nullptr, photo.plane[pl], i, j, lens, overlap);
+    const int w = cameraPhotoSample<MIP, true>(v.geometry, p.camera, p.rig, p.mip[pl].geometry, p.mipBias, 0.0f, p.photo.stats != nullptr,
+                                               p.photo.plane[pl], i, j, lens, overlap);
     *g0 = lens[0].gain;
     *g1 = lens[1].gain;
     return w;
@@ -461,36 +430,24 @@ struct LensMotionPositions : LensPhotoPositions<K, BARREL> {
   using LensPhotoPositions<K, BARREL>::LensPhotoPositions;
   __device__ int record(const PerFrameGatherParams& p, const PerFramePlane& v, int pl, int i, int j, int32_t* rec0, int32_t* rec1, int* g0,
                         int* g1, bool* overlap) const {
-    const PerFrameGatherParams::LensMotion& m = p.lensMotion;
-    return lensMotionSample<BARREL>(v.geometry, p.rotation, p.rig, m.motion, p.seamScale, m.photo.stats != nullptr, m.photo.plane[pl],
+    return lensMotionSample<BARREL>(v.geometry, p.rotation, p.rig, p.motion, p.seamScale, p.photo.stats != nullptr, p.photo.plane[pl],
                                     v.colTable, v.rowTable, i, j, rec0, rec1, g0, g1, overlap);
   }
-  __device__ static const PerFrameGatherParams::LensPhoto& photo(const PerFrameGatherParams& p) { return p.lensMotion.photo; }
 };
 
-// A camera view of a lens rig with photometry and a rig motion (kCameraMotion): CameraPhotoPositions' records, levels and
-// pixel blend, the records from cameraMotionSample.  The table as for LensMotionPositions.
-template <int, bool MIP>
-struct CameraMotionPositions : NoTables {
-  static constexpr bool kPhoto = true, kTransparent = true;
-  CameraPhotoRecords lens[2];
-  using NoTables::NoTables;
+// A camera view of a lens rig with photometry and a rig motion (kCameraMotion): CameraPhotoPositions' levels and pixel
+// blend, the records from cameraMotionSample.  The table as for LensMotionPositions.
+template <int K, bool MIP>
+struct CameraMotionPositions : CameraPhotoPositions<K, MIP> {
+  using CameraPhotoPositions<K, MIP>::CameraPhotoPositions;
   __device__ int record(const PerFrameGatherParams& p, const PerFramePlane& v, int pl, int i, int j, int32_t*, int32_t*, int* g0, int* g1,
                         bool* overlap) {
-    const PerFrameGatherParams::CameraMotion& m = p.cameraMotion;
-    const PerFrameGatherParams::LensPhoto& photo = m.cameraPhoto.photo;
-    const int w = cameraMotionSample<MIP>(v.geometry, p.camera, p.rig, m.motion, m.cameraPhoto.mip[pl].geometry, p.mipBias, p.seamScale,
-                                          photo.stats != nullptr, photo.plane[pl], i, j, lens, overlap);
+    CameraPhotoRecords* lens = this->lens;
+    const int w = cameraMotionSample<MIP>(v.geometry, p.camera, p.rig, p.motion, p.mip[pl].geometry, p.mipBias, p.seamScale,
+                                          p.photo.stats != nullptr, p.photo.plane[pl], i, j, lens, overlap);
     *g0 = lens[0].gain;
     *g1 = lens[1].gain;
     return w;
-  }
-  __device__ static const PerFrameGatherParams::LensPhoto& photo(const PerFrameGatherParams& p) { return p.cameraMotion.cameraPhoto.photo; }
-  template <int K, bool TRANSPARENT>
-  __device__ int pixel(const PerFrameGatherParams& p, int pl, const SrcView& s, const unsigned char* smem, int l, const int32_t*) const {
-    const CameraPhotoRecords& r = lens[l];
-    if constexpr (MIP) return levelPixel<K, TRANSPARENT>(p.cameraMotion.cameraPhoto.mip[pl].level, s, smem, r.level, r.rec0, r.rec1, r.w);
-    else return viewPixel<K, TRANSPARENT>(s, smem, r.rec0[0], r.rec0[1]);
   }
 };
 
@@ -578,18 +535,15 @@ cudaError_t launchPerFrameGather(PerFrameGatherParams p, PerFrameSource source, 
     case PerFrameSource::kCameraMip: return launchPositions<MipCameraPositions>(p, p.lens, numTiles, numSMs, stream);
     case PerFrameSource::kCameraAniso: return launchPositions<AnisoCameraPositions>(p, p.lens, numTiles, numSMs, stream);
     case PerFrameSource::kLensPhoto: return launchPositions<LensPhotoPositions>(p, barrel, numTiles, numSMs, stream);
-    case PerFrameSource::kCameraPhoto:
-    case PerFrameSource::kStereoCamera: {
-      bool mip = false;  // (a level table only where some plane has a pyramid)
-      for (int i = 0; i < p.numPlanes; ++i) mip = mip || p.cameraPhoto.mip[i].geometry.top > 0;
-      if (source == PerFrameSource::kStereoCamera) return launchPositions<StereoCameraPositions>(p, mip, numTiles, numSMs, stream);
-      return launchPositions<CameraPhotoPositions>(p, mip, numTiles, numSMs, stream);
-    }
     case PerFrameSource::kLensMotion: return launchPositions<LensMotionPositions>(p, barrel, numTiles, numSMs, stream);
+    case PerFrameSource::kCameraPhoto:
+    case PerFrameSource::kStereoCamera:
     case PerFrameSource::kCameraMotion: {
-      bool mip = false;
-      for (int i = 0; i < p.numPlanes; ++i) mip = mip || p.cameraMotion.cameraPhoto.mip[i].geometry.top > 0;
-      return launchPositions<CameraMotionPositions>(p, mip, numTiles, numSMs, stream);
+      bool mip = false;  // (a level table only where some plane has a pyramid)
+      for (int i = 0; i < p.numPlanes; ++i) mip = mip || p.mip[i].geometry.top > 0;
+      if (source == PerFrameSource::kStereoCamera) return launchPositions<StereoCameraPositions>(p, mip, numTiles, numSMs, stream);
+      if (source == PerFrameSource::kCameraMotion) return launchPositions<CameraMotionPositions>(p, mip, numTiles, numSMs, stream);
+      return launchPositions<CameraPhotoPositions>(p, mip, numTiles, numSMs, stream);
     }
   }
   return cudaErrorInvalidValue;
