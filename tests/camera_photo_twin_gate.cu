@@ -36,7 +36,6 @@ struct GateData {
   int nGeo;
 };
 
-T360_HD SphereVec drawVec(Draw& d, float scale) { return SphereVec{d.component(scale), d.component(scale), d.component(scale)}; }
 T360_HD uint32_t packLens(int level, int w, int gain) { return iw(level) | iw(w) << 8 | iw(gain) << 16; }
 
 struct CameraPhotoGate {

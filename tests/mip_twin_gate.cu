@@ -34,8 +34,6 @@ struct GateData {
   int nLensGeo;
 };
 
-T360_HD SphereVec drawVec(Draw& d, float scale) { return SphereVec{d.component(scale), d.component(scale), d.component(scale)}; }
-
 struct MipGate {
   static constexpr uint64_t kSeed = 20261018ull;
   static constexpr int kOut = 6;

@@ -54,7 +54,6 @@ struct GateData {
   int nCam;
 };
 
-T360_HD SphereVec drawVec(Draw& d, float scale) { return SphereVec{d.component(scale), d.component(scale), d.component(scale)}; }
 T360_HD RigMotion motionOf(const GateData& D, int k) {
   const MotionRec& m = D.motion[k];
   RigMotion mo;

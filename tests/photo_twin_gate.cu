@@ -34,8 +34,6 @@ struct GateData {
   const float* tables;  // every geometry's sphere tables, back to back
 };
 
-T360_HD SphereVec drawVec(Draw& d, float scale) { return SphereVec{d.component(scale), d.component(scale), d.component(scale)}; }
-
 struct PhotoGate {
   static constexpr uint64_t kSeed = 20261019ull;
   static constexpr int kOut = 6;

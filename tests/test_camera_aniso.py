@@ -8,14 +8,13 @@ What pins what:
   - that it anti-aliases better than the isotropic pyramid: the zone plate of test_camera_mip.py through a little planet
     and a dome;
   - the refusals and their order;
-  - the twin gate (tests/aniso_twin_gate.cu): the device build of anisoLevelOf, anisoFootprint, anisoCameraPoint and
-    anisoCameraSample against the host build the twin runs;
+  - the device build of the anisotropic steps against the host build the twin runs: tests/aniso_twin_gate.cu, run from
+    tests/test_twin_gates.py;
   - on the GPU, frames against the oracle's composite of the twin (cv::resize INTER_AREA pyramids, cv::remap per probe
     and level, the level blend, the probe mean), and against the camera-mip and camera calls where they must agree.
 Poses, rigs and planes are made from seeds."""
 import ctypes as C
 import math
-import re
 import subprocess
 
 import numpy as np
@@ -31,7 +30,6 @@ from tests.test_camera_mip import zone  # noqa: F401 (fixture)
 from tests.test_camera_models import EQUIDISTANT, PANNINI, PINHOLE, STEREOGRAPHIC, _bad_calls
 from tests.test_rectilinear import INTERPS, RECT_CTX, _ctx, _rig
 from tests.test_rectilinear import torch_cuda  # noqa: F401 (fixture)
-from tests.test_twin_gates import THREADS, gate_command, run
 from tests.test_warp_map import _check, _refused, _stdout
 
 WRAP, TRANSPARENT = t360.BORDER_WRAP, t360.BORDER_TRANSPARENT
@@ -367,74 +365,6 @@ def test_refusals_happen_without_a_gpu(capfd):
         t360.camera_aniso_maps(ctx, ok_pose, ok_cam, (0, -4.0), probes, 64, 32, 8, 8)
     with pytest.raises(ValueError):
         t360.camera_aniso_maps(ctx, ok_pose, ok_cam, (4, 0.0), 5, 64, 32, 8, 8)
-
-
-# ---- the twin gate (tests/aniso_twin_gate.cu on tests/twin_gate.cuh) ---------------------------------------------------
-GATE_PROBES = ("anisoLevelOf", "anisoFootprint<ctx>", "anisoFootprint<lens>", "anisoCameraPoint<ctx>", "anisoCameraPoint<lens>",
-               "anisoCameraSample<ctx>", "anisoCameraSample<lens>")
-GATE_CLASSES = {("anisoLevelOf", c) for c in ("equal", "multipleOf256", "zero", "denormal", "infNaN", "clamped")} | \
-    {(p, c) for p in ("anisoFootprint<ctx>", "anisoFootprint<lens>") for c in ("columnAxis", "rowAxis")} | \
-    {(f"anisoCamera{k}<ctx>", "faceChange") for k in ("Point", "Sample")} | {(f"anisoCamera{k}<lens>", "lensChange") for k in ("Point", "Sample")}
-
-
-@pytest.fixture(scope="module")
-def aniso_gate(tmp_path_factory):
-    exe = tmp_path_factory.mktemp("aniso_twin_gate") / "aniso_twin_gate"
-    r = subprocess.run(gate_command("aniso_twin_gate", exe), capture_output=True, text=True)
-    assert r.returncode == 0, r.stdout + r.stderr
-    return "aniso_twin_gate", exe
-
-
-def test_gate_builds_for_sm_90a_with_the_library_flags(aniso_gate):
-    import os
-    from transform360_b200 import build as b
-    cmd = gate_command(*aniso_gate)
-    assert cmd[cmd.index("-Xcompiler") + 1] == b.HOST_FLAGS and "arch=compute_90a,code=sm_90a" in cmd and "-O3" in cmd
-    elf = subprocess.run([os.path.join(os.path.dirname(b.nvcc_path()), "cuobjdump"), "--list-elf", str(aniso_gate[1])], capture_output=True,
-                         text=True, check=True).stdout
-    assert "sm_90a" in elf
-
-
-def test_gate_host_half_does_not_depend_on_the_thread_count(aniso_gate):
-    fp = lambda out: [line for line in out.splitlines() if line.startswith("fingerprint ")]
-    one = fp(run(aniso_gate, "--host-only", "--threads", "1").stdout)
-    many = fp(run(aniso_gate, "--host-only", "--threads", str(THREADS)).stdout)
-    assert [line.split()[1] for line in one] == list(GATE_PROBES) and one == many
-
-
-def test_gate_self_test_reports_exactly_the_flipped_element(aniso_gate):
-    r = run(aniso_gate, "--self-test", "--threads", str(THREADS), check=False)
-    assert r.returncode == 1, r.stdout + r.stderr
-    flipped = re.search(r"self-test: flipped (\S+) (\d+) word (\d) bit (\d)", r.stdout)
-    assert flipped, r.stdout
-    reports = [line.split() for line in r.stdout.splitlines() if len(line.split()) == 5 and not line.startswith("self-test")]
-    assert len(reports) == 1 and (reports[0][0], int(reports[0][1])) == (flipped.group(1), int(flipped.group(2))), r.stdout
-    h, o = [int(x, 16) for x in reports[0][3].split(":")], [int(x, 16) for x in reports[0][4].split(":")]
-    word, bit = int(flipped.group(3)), int(flipped.group(4))
-    assert [x ^ y for x, y in zip(h, o)] == [(1 << bit) if k == word else 0 for k in range(len(h))]
-    assert r.stdout.strip().splitlines()[-1].endswith(" 1 mismatches"), r.stdout
-
-
-def test_gate_ledger_reaches_every_class(aniso_gate):
-    """anisoLevelOf reaches aa == bb, an exact multiple of 256 between the axes, a zero and a denormal axis, a pole (inf
-    or NaN) and N clamped by maxProbes; the footprints take both axes; a probe row crosses a cube face edge and a
-    two-lens rig's seam."""
-    counts = {}
-    for line in run(aniso_gate, "--ledger", "--threads", str(THREADS)).stdout.splitlines():
-        _, probe, cls, n = line.split()
-        counts[(probe, cls)] = int(n)
-    missed = sorted(k for k, n in counts.items() if n == 0)
-    assert not missed, missed
-    assert GATE_CLASSES <= set(counts), counts
-
-
-# ---- on the GPU --------------------------------------------------------------------------------------------------------
-@pytest.mark.gpu
-def test_gate_device_twins_equal_the_host_twins(aniso_gate):
-    r = run(aniso_gate, "--threads", str(THREADS), check=False)
-    print(r.stdout)
-    m = re.fullmatch(r"(\d+) probes, (\d+) inputs, (\d+) mismatches", r.stdout.strip().splitlines()[-1])
-    assert m and r.returncode == 0 and m.group(3) == "0", r.stdout + r.stderr
 
 
 class AnisoFrame(MipFrame):

@@ -10,7 +10,9 @@ What pins what:
   - the seam: a synthetic rig of a smooth scene with a falloff and an exposure mismatch, seen through a pinhole view across
     the seam, has a luma step at most a quarter of the uncorrected hard seam's;
   - the frames and statistics against the oracle's composite of the twin (the camera-mip composite per lens, then s',
-    then the seam), and the identity frames against the camera and camera-mip calls byte for byte.
+    then the seam), and the identity frames against the camera and camera-mip calls byte for byte;
+  - the device build of the chain against its host build: tests/camera_photo_twin_gate.cu, run from
+    tests/test_twin_gates.py.
 Poses, rigs and planes are made from seeds."""
 import ctypes as C
 import subprocess
@@ -523,71 +525,3 @@ def test_refused_calls_launch_nothing_and_leave_the_outputs(torch_cuda, capfd):
     assert all(np.array_equal(a, b) for a, b in zip(before, f.host()))
     assert (stats.cpu().numpy() == 5).all()
     vft.close()
-
-
-# ---- the twin gate (tests/camera_photo_twin_gate.cu on tests/twin_gate.cuh) --------------------------------------------
-GATE_PROBES = ("lensJacobian<lens>", "cameraPhotoPoint", "cameraPhotoSample<MIP>", "cameraPhotoSample<plain>")
-
-
-@pytest.fixture(scope="module")
-def photo_gate(tmp_path_factory):
-    """(name, executable) of the camera photometry gate, built once with the library's nvcc flags."""
-    from tests.test_twin_gates import gate_command
-    exe = tmp_path_factory.mktemp("camera_photo_twin_gate") / "camera_photo_twin_gate"
-    r = subprocess.run(gate_command("camera_photo_twin_gate", exe), capture_output=True, text=True)
-    assert r.returncode == 0, r.stdout + r.stderr
-    return "camera_photo_twin_gate", exe
-
-
-def test_gate_builds_for_sm_90a_with_the_library_flags(photo_gate):
-    from tests.test_twin_gates import test_gate_builds_for_sm_90a_with_the_library_flags as check
-    check(photo_gate)
-
-
-def test_gate_host_half_does_not_depend_on_the_thread_count(photo_gate):
-    from tests.test_twin_gates import THREADS, _fingerprints, run
-    one = _fingerprints(run(photo_gate, "--host-only", "--threads", "1").stdout)
-    many = _fingerprints(run(photo_gate, "--host-only", "--threads", str(THREADS)).stdout)
-    assert [line.split()[1] for line in one] == list(GATE_PROBES), one
-    assert one == many
-
-
-def test_gate_self_test_reports_exactly_the_flipped_element(photo_gate):
-    import re
-    from tests.test_twin_gates import THREADS, run
-    r = run(photo_gate, "--self-test", "--threads", str(THREADS), check=False)
-    assert r.returncode == 1, r.stdout + r.stderr
-    flipped = re.search(r"self-test: flipped (\S+) (\d+) word (\d+) bit (\d+)", r.stdout)
-    assert flipped, r.stdout
-    probe, index, word, bit = flipped.group(1), int(flipped.group(2)), int(flipped.group(3)), int(flipped.group(4))
-    reports = [line.split() for line in r.stdout.splitlines() if len(line.split()) == 5 and not line.startswith("self-test")]
-    assert len(reports) == 1, r.stdout
-    name, at, _, host, other = reports[0]
-    assert (name, int(at)) == (probe, index)
-    h, o = [int(x, 16) for x in host.split(":")], [int(x, 16) for x in other.split(":")]
-    assert [x ^ y for x, y in zip(h, o)] == [(1 << bit) if k == word else 0 for k in range(11)]
-    assert r.stdout.strip().splitlines()[-1].endswith(" 1 mismatches"), r.stdout
-
-
-def test_gate_ledger_reaches_every_class(photo_gate):
-    """Rays on a used lens's axis, a lens's thetaMax, belt pixels and the infinite footprint of a used lens's back axis are
-    all reached by the first 2^20 inputs of cameraPhotoPoint."""
-    from tests.test_twin_gates import THREADS, run
-    counts = {}
-    for line in run(photo_gate, "--ledger", "--threads", str(THREADS)).stdout.splitlines():
-        _, probe, cls, n = line.split()
-        counts[(probe, cls)] = int(n)
-    print(counts)
-    assert sorted(counts) == [("cameraPhotoPoint", c) for c in sorted(("belt", "infiniteFootprint", "lensAxis", "thetaMax"))], counts
-    assert all(n >= 100 for n in counts.values()), counts
-
-
-@pytest.mark.gpu
-def test_gate_device_twins_equal_the_host_twins(photo_gate):
-    import re
-    from tests.test_twin_gates import THREADS, run
-    r = run(photo_gate, "--threads", str(THREADS), check=False)
-    print(r.stdout)
-    last = r.stdout.strip().splitlines()[-1]
-    m = re.fullmatch(r"(\d+) probes, (\d+) inputs, (\d+) mismatches", last)
-    assert m and r.returncode == 0 and m.group(3) == "0", r.stdout + r.stderr

@@ -7,11 +7,11 @@ What pins what:
   - a constant delta against the photometric twin of the rig whose lenses are turned by it (the convention);
   - the twin against a float64 model whose fixed point t = readout(project(M(t) d)) is solved to convergence;
   - a synthetic rolling-shutter frame, rendered through a float64 forward model, corrected against the still frame;
-  - the frames against the oracle composites of test_lens_photo / test_camera_photo, bit for bit, and the device half of
-    the twin gate (tests/motion_twin_gate.cu) against its host half.
+  - the frames against the oracle composites of test_lens_photo / test_camera_photo, bit for bit;
+  - the device build of the motion chains against their host build: tests/motion_twin_gate.cu, run from
+    tests/test_twin_gates.py.
 Rigs, motions, readouts and poses are made from seeds."""
 import ctypes as C
-import re
 import subprocess
 
 import numpy as np
@@ -27,7 +27,6 @@ from tests.test_lens import IN_DIMS, LAYOUTS, LENS_CTX, OUT_DIMS, Frame, _orient
 from tests.test_lens_blend import INTERPS
 from tests.test_lens_photo import IDENTITY, STATS, equidistant_pair, photo_composite, rig_photos
 from tests.test_rectilinear import RECT_CTX, _ctx
-from tests.test_twin_gates import THREADS, gate_command, run
 from tests.test_warp_map import _check, _refused, _stdout
 
 READOUTS = {"rows": (0.0, 1.0, 0.0), "reversed": (0.0, -1.0, 1.0), "columns": (1.0, 0.0, 0.0), "half": (2.0, 0.0, -1.0)}
@@ -390,65 +389,6 @@ def test_refusals_happen_without_a_gpu(capfd):
     t360.camera_motion_maps(cam_ctx, single, IDENTITY, 0.0, (0, 0, 0, 90.0, 60.0), PINHOLE, None, mo, 0, 0, 64, 32, 8, 8)
 
 
-# ---- the twin gate (tests/motion_twin_gate.cu on tests/twin_gate.cuh) --------------------------------------------------
-GATE_PROBES = ("motionLens", "lensMotionPosition", "lensMotionSample<BARREL>", "lensMotionSample<plain>", "cameraMotionSample<plain>",
-               "cameraMotionSample<MIP>")
-GATE_CLASSES = {("lensMotionPosition", c) for c in ("clampedAt0", "clampedAt1", "coveredThenUncovered", "segmentBoundary", "hard", "feathered",
-                                                    "bothLenses")}
-
-
-@pytest.fixture(scope="module")
-def motion_gate(tmp_path_factory):
-    exe = tmp_path_factory.mktemp("motion_twin_gate") / "motion_twin_gate"
-    r = subprocess.run(gate_command("motion_twin_gate", exe), capture_output=True, text=True)
-    assert r.returncode == 0, r.stdout + r.stderr
-    return "motion_twin_gate", exe
-
-
-def test_gate_builds_for_sm_90a_with_the_library_flags(motion_gate):
-    from transform360_b200 import build as b
-    cmd = gate_command(*motion_gate)
-    assert cmd[cmd.index("-Xcompiler") + 1] == b.HOST_FLAGS and "arch=compute_90a,code=sm_90a" in cmd and "-O3" in cmd
-    import os
-    elf = subprocess.run([os.path.join(os.path.dirname(b.nvcc_path()), "cuobjdump"), "--list-elf", str(motion_gate[1])], capture_output=True,
-                         text=True, check=True).stdout
-    assert "sm_90a" in elf
-
-
-def test_gate_host_half_does_not_depend_on_the_thread_count(motion_gate):
-    fp = lambda out: [line for line in out.splitlines() if line.startswith("fingerprint ")]
-    one = fp(run(motion_gate, "--host-only", "--threads", "1").stdout)
-    many = fp(run(motion_gate, "--host-only", "--threads", str(THREADS)).stdout)
-    assert [line.split()[1] for line in one] == list(GATE_PROBES) and one == many
-
-
-def test_gate_self_test_reports_exactly_the_flipped_element(motion_gate):
-    r = run(motion_gate, "--self-test", "--threads", str(THREADS), check=False)
-    assert r.returncode == 1, r.stdout + r.stderr
-    flipped = re.search(r"self-test: flipped (\S+) (\d+) word (\d) bit (\d)", r.stdout)
-    assert flipped, r.stdout
-    reports = [line.split() for line in r.stdout.splitlines() if len(line.split()) == 5 and not line.startswith("self-test")]
-    assert len(reports) == 1 and (reports[0][0], int(reports[0][1])) == (flipped.group(1), int(flipped.group(2))), r.stdout
-    h, o = [int(x, 16) for x in reports[0][3].split(":")], [int(x, 16) for x in reports[0][4].split(":")]
-    word, bit = int(flipped.group(3)), int(flipped.group(4))
-    assert [x ^ y for x, y in zip(h, o)] == [(1 << bit) if k == word else 0 for k in range(len(h))]
-    assert r.stdout.strip().splitlines()[-1].endswith(" 1 mismatches"), r.stdout
-
-
-def test_gate_ledger_reaches_every_class(motion_gate):
-    """The interpolation reaches t = 0, t = 1 and inner segment boundaries; lensMotionPosition reaches t clamped at 0 and
-    at 1, the first projection covered with the last one not (the converse cannot happen: an uncovered projection keeps
-    t), a projection on a segment boundary, the hard seam, both lenses and the feathered seam."""
-    counts = {}
-    for line in run(motion_gate, "--ledger", "--threads", str(THREADS)).stdout.splitlines():
-        _, probe, cls, n = line.split()
-        counts[(probe, cls)] = int(n)
-    missed = sorted(k for k, n in counts.items() if n == 0)
-    assert not missed, missed
-    assert GATE_CLASSES <= set(counts), counts
-    assert {("motionLens", c) for c in ("t0", "t1", "boundary")} <= set(counts), counts
-
-
 # ---- on the GPU --------------------------------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
 def torch_cuda():
@@ -456,14 +396,6 @@ def torch_cuda():
     if not torch.cuda.is_available():
         pytest.fail("no CUDA device: the GPU tests must run on an H100 (there is no CPU fallback to test)")
     return torch
-
-
-@pytest.mark.gpu
-def test_gate_device_twins_equal_the_host_twins(motion_gate):
-    r = run(motion_gate, "--threads", str(THREADS), check=False)
-    print(r.stdout)
-    m = re.fullmatch(r"(\d+) probes, (\d+) inputs, (\d+) mismatches", r.stdout.strip().splitlines()[-1])
-    assert m and r.returncode == 0 and m.group(3) == "0", r.stdout + r.stderr
 
 
 def want_motion(f, ctx, rig, ph, seam, o, mo):

@@ -13,9 +13,8 @@ What pins what:
     brighter, has a mean luma difference between the eyes at most a quarter of the naive one's;
   - the frames and statistics against test_camera_photo's oracle composite of the stereo twin, the MONO frame against the
     camera-photo call, and the eye-combined twin map planned through generateMapFromWarp against the frame.
-  - the device build of the equirect ray and of the stereo chain against the host build, bit for bit
-    (tests/stereo_camera_twin_gate.cu on tests/twin_gate.cuh), with a ledger of the eye boundaries, each lens's thetaMax,
-    lon = +-pi, lat near +-90, TB with vflip and the back-axis infinite footprint.
+  - the device build of the equirect ray and of the stereo chain against the host build: tests/stereo_camera_twin_gate.cu,
+    run from tests/test_twin_gates.py.
 Poses, rigs and planes are made from seeds."""
 import ctypes as C
 import math
@@ -669,74 +668,3 @@ def test_refused_calls_launch_nothing_and_leave_the_outputs(torch_cuda, capfd):
     assert t360.kernel_launch_count() == n0
     assert all(np.array_equal(a, b) for a, b in zip(before, f.host()))
     assert (stats.cpu().numpy() == 5).all()
-
-
-# ---- the twin gate (tests/stereo_camera_twin_gate.cu on tests/twin_gate.cuh) --------------------------------------------
-GATE_PROBES = ("cameraRay<equirect>", "cameraPhotoPoint<stereo>", "cameraPhotoSample<MIP,stereo>", "cameraPhotoSample<plain,stereo>")
-GATE_CLASSES = {"cameraRay<equirect>": ("lonPi", "latPole"),
-                "cameraPhotoPoint<stereo>": ("eyeBoundaryCol", "eyeBoundaryRow", "thetaMax0", "thetaMax1", "tbVflip", "infiniteFootprint")}
-
-
-@pytest.fixture(scope="module")
-def stereo_gate(tmp_path_factory):
-    """(name, executable) of the stereo camera gate, built once with the library's nvcc flags."""
-    from tests.test_twin_gates import gate_command
-    exe = tmp_path_factory.mktemp("stereo_camera_twin_gate") / "stereo_camera_twin_gate"
-    r = subprocess.run(gate_command("stereo_camera_twin_gate", exe), capture_output=True, text=True)
-    assert r.returncode == 0, r.stdout + r.stderr
-    return "stereo_camera_twin_gate", exe
-
-
-def test_gate_builds_for_sm_90a_with_the_library_flags(stereo_gate):
-    from tests.test_twin_gates import test_gate_builds_for_sm_90a_with_the_library_flags as check
-    check(stereo_gate)
-
-
-def test_gate_host_half_does_not_depend_on_the_thread_count(stereo_gate):
-    from tests.test_twin_gates import THREADS, _fingerprints, run
-    one = _fingerprints(run(stereo_gate, "--host-only", "--threads", "1").stdout)
-    many = _fingerprints(run(stereo_gate, "--host-only", "--threads", str(THREADS)).stdout)
-    assert [line.split()[1] for line in one] == list(GATE_PROBES), one
-    assert one == many
-
-
-def test_gate_self_test_reports_exactly_the_flipped_element(stereo_gate):
-    import re
-    from tests.test_twin_gates import THREADS, run
-    r = run(stereo_gate, "--self-test", "--threads", str(THREADS), check=False)
-    assert r.returncode == 1, r.stdout + r.stderr
-    flipped = re.search(r"self-test: flipped (\S+) (\d+) word (\d+) bit (\d+)", r.stdout)
-    assert flipped, r.stdout
-    probe, index, word, bit = flipped.group(1), int(flipped.group(2)), int(flipped.group(3)), int(flipped.group(4))
-    reports = [line.split() for line in r.stdout.splitlines() if len(line.split()) == 5 and not line.startswith("self-test")]
-    assert len(reports) == 1, r.stdout
-    name, at, _, host, other = reports[0]
-    assert (name, int(at)) == (probe, index)
-    h, o = [int(x, 16) for x in host.split(":")], [int(x, 16) for x in other.split(":")]
-    assert [x ^ y for x, y in zip(h, o)] == [(1 << bit) if k == word else 0 for k in range(11)]
-    assert r.stdout.strip().splitlines()[-1].endswith(" 1 mismatches"), r.stdout
-
-
-def test_gate_ledger_reaches_every_class(stereo_gate):
-    """The eye boundary columns and rows, each lens's thetaMax, the flipped eye of a TB vflip view and the infinite
-    footprint of a used lens's back axis (cameraPhotoPoint<stereo>), lon = +-pi at hfov 360 and lat within 0.1 degree of
-    +-90 (cameraRay<equirect>): each reached at least 10000 times by the first 2^20 inputs."""
-    from tests.test_twin_gates import THREADS, run
-    counts = {}
-    for line in run(stereo_gate, "--ledger", "--threads", str(THREADS)).stdout.splitlines():
-        _, probe, cls, n = line.split()
-        counts[(probe, cls)] = int(n)
-    print(counts)
-    assert sorted(counts) == sorted((p, c) for p, cs in GATE_CLASSES.items() for c in cs), counts
-    assert all(n >= 10000 for n in counts.values()), counts
-
-
-@pytest.mark.gpu
-def test_gate_device_twins_equal_the_host_twins(stereo_gate):
-    import re
-    from tests.test_twin_gates import THREADS, run
-    r = run(stereo_gate, "--threads", str(THREADS), check=False)
-    print(r.stdout)
-    last = r.stdout.strip().splitlines()[-1]
-    m = re.fullmatch(r"(\d+) probes, (\d+) inputs, (\d+) mismatches", last)
-    assert m and r.returncode == 0 and m.group(3) == "0", r.stdout + r.stderr

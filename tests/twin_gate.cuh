@@ -1,7 +1,7 @@
 // Host / device twin gates: the device build of float functions of the per-frame position chains (csrc/flat_view.h,
 // libm_ports.h, oriented_view.h) against their host build, the one the planner and the host twins run.  This header is
-// the harness every gate shares (tests/twin_gate.cu, mip_twin_gate.cu, photo_twin_gate.cu); tests/test_twin_gates.py
-// builds each gate with the library's own nvcc flags (transform360_b200/build.py: ARCH, -O3, HOST_FLAGS) and runs it.
+// the harness every gate shares (tests/*twin_gate.cu); tests/test_twin_gates.py builds each gate with the library's own
+// nvcc flags (transform360_b200/build.py: ARCH, -O3, HOST_FLAGS) and runs it.
 //
 // A probe is a T360_HD function of an index i: it draws its inputs from (probe, i) alone -- a Draw, a splitmix64 stream
 // seeded with a hash of (the gate's seed, probe, i) -- calls one twin function or chain, and packs the result into the
@@ -92,6 +92,8 @@ struct Draw {
     return t360::fMul(range(-1.0f, 1.0f), scale);
   }
 };
+// a ray or differential of three components (x, y, z drawn in that order)
+T360_HD t360::SphereVec drawVec(Draw& d, float scale) { return t360::SphereVec{d.component(scale), d.component(scale), d.component(scale)}; }
 
 struct HostRng {  // host-only draws for building a gate's shared data (double, libm: not part of any probe's inputs)
   uint64_t s;
